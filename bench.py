@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — pose-graph windows/sec (10 keyframes x 2000 correspondences, 640x480 synthetic RGB-D) on N B200s.
+"""bench.py — pose-graph windows/sec (10 keyframes x 2000 correspondences, 640x480 synthetic RGB-D) on N H100s.
 
 Contract (see the task statement): `python bench.py --gpus N --steps K --warmup W` (torchrun for N>1) prints ONE JSON
 line on rank 0.  One "step" = one pass of the hot path over one batch of `--windows` independent tracking windows per GPU
-(BASELINE.json configs[1] replicated; configs[3] is 32 windows/GPU x 8 GPUs), i.e. weak scaling.  Every timed region runs its
-K-step block back to back until --min-seconds have passed (CUDA events around every block, median block reported, max over
-ranks), so the clocks sampled during the region mean something.
+(BASELINE.json configs[1] replicated; configs[3] is 32 windows/GPU x 8 GPUs), i.e. weak scaling.  Every timed region runs
+exactly K steps back to back after W warm-up steps (CUDA events around the block, max over ranks).  --dump-outputs DIR writes
+the poses the timed paths returned in their last step as DIR/<name>.npy (float32); the inputs are seeded, so two builds run
+with the same arguments can be compared output for output.
 
   value     windows/s, whole job, inputs (keyframe maps, correspondences, poses, tables) already resident in HBM: per step
             ONE new frame per window is stored into the keyframe cache (k_frame_cache_store: its quarter-resolution maps are
@@ -17,7 +18,7 @@ ranks), so the clocks sampled during the region mean something.
             reference API (Frame::_depth_gpu/_normal_gpu) and are passed as device pointers.
   keyframe_cache.rebuild_every_call   the same batch with the reference's pattern (all N maps of every window rebuilt in every call).
   roofline  dominant kernel = k_solve; achieved = algorithmic bytes (SURVEY.md 8d: iters*(N*npix*32 + C*32) + 2*N*64 per window) /
-            CUDA-event duration of that kernel; peak = MEASURED_PEAKS.json hbm_gbs (fallback 6650); plus the FP32 and the
+            CUDA-event duration of that kernel; peak = MEASURED_PEAKS.json hbm_gbs (fallback: the H100 SXM data sheet's 3350); plus the FP32 and the
             issue-slot view, because the kernel's working set stays in L2 (SURVEY.md 8d asks for the FP32 bound in that case).
   cpu_baseline  oracle/ (CPU restatement, "port": the reference has no CPU optimizer) on the host cores, bounded sample; and the
             reference's own kernels on ONE window in this same process (single_window_vs_reference).
@@ -52,13 +53,13 @@ def parse():
     ap.add_argument("--scenes", type=int, default=4, help="distinct rendered scenes per GPU; windows cycle through them with their own pose noise and their own copy of the frame maps")
     ap.add_argument("--cpu-windows", type=int, default=0, help="cpu_baseline sample size (0 = 2 per core)")
     ap.add_argument("--ref-windows", type=int, default=8, help="windows per step for --impl reference")
-    ap.add_argument("--min-seconds", type=float, default=1.0, help="each timed region repeats its K-step block until it has run this long")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the poses the timed paths computed in their last step as DIR/<name>.npy")
     ap.add_argument("--skip-cfg3", action="store_true", help="leave out the BASELINE configs[2] block (30-keyframe pool)")
     return ap.parse_args()
 
 
 class ClockSampler(threading.Thread):
-    """Samples nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks/throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index: int):
         super().__init__(daemon=True)
@@ -100,12 +101,12 @@ def hbm_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "fallback (H100 SXM data sheet)"
 
 
 def make_batch(args, rank, dev):
     """`windows` windows per GPU: `scenes` rendered scenes, every window gets its OWN device copy of the frame maps (so
-    the batch footprint, windows*frames*6.1 MB, is far larger than the 126 MB L2) and its own initial-pose noise."""
+    the batch footprint, windows*frames*6.1 MB, is far larger than the 50 MB L2) and its own initial-pose noise."""
     import torch
     from bundletrack_b200 import synth
     from bundletrack_b200.optimizer import SolveWindow
@@ -140,12 +141,12 @@ def tensor_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["bf16_tflops"]), "measured"
     except Exception:
-        return 1590.0, "fallback"
+        return 989.0, "fallback (H100 SXM data sheet, dense fp16/bf16)"
 
 
 def tensor_peak_sustained():
     """cuBLAS 16-bit throughput run back to back for seconds (MEASURED_PEAKS.json bf16_tflops_sustained): the chip's power-limited rate.  The
-    matcher's tensor pass is one 84 us kernel between non-tensor kernels, so the BURST figure is the denominator of tc_frac_of_tensor_peak;
+    matcher's tensor pass is one short kernel between non-tensor kernels, so the BURST figure is the denominator of tc_frac_of_tensor_peak;
     the sustained one is reported next to it."""
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
@@ -405,23 +406,20 @@ def cpu_baseline(host, n_windows, check_against=None, single_window=None):
     return out
 
 
-def timed_blocks(step, steps, min_seconds, sync, est_ms):
-    """K steps per block, as many back-to-back blocks as it takes to fill `min_seconds` (a 12 ms timed region tells little about clocks);
-    CUDA events bracket every block on the launching stream.  Returns per-block ms and wall ms lists."""
+def timed_blocks(step, steps, sync):
+    """One block of exactly `steps` back-to-back steps, CUDA events around it on the launching stream.  Returns [block ms] and
+    [block wall ms]."""
     import torch
-    n_blocks = int(max(1, min(400, np.ceil(min_seconds * 1e3 / max(steps * est_ms, 1e-3)))))
-    evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(n_blocks)]
-    walls = []
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     sync()
-    for b in range(n_blocks):
-        t0 = time.perf_counter()
-        evs[b][0].record()
-        for _ in range(steps):
-            step()
-        evs[b][1].record()
-        walls.append((time.perf_counter() - t0) * 1e3)
+    t0 = time.perf_counter()
+    e0.record()
+    for _ in range(steps):
+        step()
+    e1.record()
+    wall = (time.perf_counter() - t0) * 1e3
     sync()
-    return [a.elapsed_time(b) for a, b in evs], walls
+    return [e0.elapsed_time(e1)], [wall]
 
 
 def main():
@@ -534,7 +532,7 @@ def main():
         store_new(); opt.run()
     for _ in range(args.warmup):
         step_value()
-    blk_ms, _ = timed_blocks(step_value, args.steps, args.min_seconds, sync_all, 0.5)
+    blk_ms, _ = timed_blocks(step_value, args.steps, sync_all)
     tm = opt.timing_ms()                      # per-kernel device time of the last step
     stats = opt.stats()
     poses = opt.fetch()
@@ -554,7 +552,7 @@ def main():
     step_e2e.inflight = False
     for _ in range(max(args.warmup, 2)):
         step_e2e()
-    _, wall_ms = timed_blocks(step_e2e, args.steps, args.min_seconds, sync_all, 0.6)
+    _, wall_ms = timed_blocks(step_e2e, args.steps, sync_all)
     opt.end_prepared(batch, pose_buf); step_e2e.inflight = False
     out_poses = [pose_buf[batch.off[i]:batch.off[i + 1]].copy() for i in range(len(cwins))]
     t_e2e = torch.tensor([float(np.median(wall_ms)) / args.steps], device=dev)
@@ -564,18 +562,18 @@ def main():
         opt.solve_prepared(batch, pose_buf)
     for _ in range(args.warmup):
         step_sync()
-    _, sync_wall = timed_blocks(step_sync, args.steps, min(args.min_seconds, 0.3), sync_all, 0.7)
+    _, sync_wall = timed_blocks(step_sync, args.steps, sync_all)
     host_us = opt.host_timing_us()
     t_sync = torch.tensor([float(np.median(sync_wall)) / args.steps], device=dev)
     # ---- the reference's own calling pattern, for comparison: every map rebuilt inside every call
     opt.stage(wins)
     for _ in range(args.warmup):
         opt.run()
-    rb_ms, _ = timed_blocks(opt.run, args.steps, min(args.min_seconds, 0.3), sync_all, 0.7)
+    rb_ms, _ = timed_blocks(opt.run, args.steps, sync_all)
     tm_rb = opt.timing_ms()
     for _ in range(args.warmup):
         opt.optimizeWindows(wins)
-    _, rb_wall = timed_blocks(lambda: opt.optimizeWindows(wins), args.steps, min(args.min_seconds, 0.3), sync_all, 0.8)
+    _, rb_wall = timed_blocks(lambda: opt.optimizeWindows(wins), args.steps, sync_all)
     t_rb = torch.tensor([float(np.median(rb_ms)) / args.steps, float(np.median(rb_wall)) / args.steps], device=dev)
     clocks = sampler.stop()      # sampled across all timed regions
     if world > 1:
@@ -590,27 +588,35 @@ def main():
     h2d = sum(len(w.corr) * 32 + w.n_frames * 64 + w.n_frames * 20 + 120 + 45 * 8 + 46 * 12 for w in wins) + new_frame_bytes
     d2h = sum(w.n_frames * 64 for w in wins)
 
+    if rank == 0 and args.dump_outputs:
+        # what the two timed paths handed back in their last step: the poses of every window (value: bt_solve_fetch after the
+        # resident-input steps; e2e: the streaming call's last batch)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "poses_value.npy"), np.concatenate(poses, 0).astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "poses_e2e.npy"), np.concatenate(out_poses, 0).astype(np.float32))
+
     if rank == 0:
+        n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
         peak, peak_src = hbm_peak()
         alg_bytes = args.windows * (7 * (N * npix * 32 + C * 32) + 2 * N * 64)
         ach = alg_bytes / (tm["solve"] * 1e-3) / 1e9
         prof = ncu_profile("k_solve")
-        sm_clock = (clocks.get("sm_mhz") or 1965.0) * 1e6
+        sm_clock = (clocks.get("sm_mhz") or 1980.0) * 1e6
         # SURVEY.md 8d: when dram__bytes falls below B_alg (the batch's maps stay in L2) report the FP32 bound as well.  F_alg counts every
         # quarter-resolution pixel of every pair (400 flop each); the kernel only walks the compacted valid source lists (n_src_pixels).
         f_alg = args.windows * 7.0 * (N * (N - 1) / 2) * npix * 400
         f_valid = 7.0 * stats["n_src_pixels"] * 400
-        fp32_peak = 148 * 128 * 2 * sm_clock / 1e12
+        fp32_peak = n_sm * 128 * 2 * sm_clock / 1e12
         roof = {"bound": "hbm", "kernel": "k_solve", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": prof.get("dram_bytes_per_launch"),
                 "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": tm,
                 "note": "effective-bandwidth figure: the batch's working set stays in L2 (traffic << algorithmic bytes); the kernel is latency/issue-bound, see fp32 / issue",
-                "fp32": {"peak_tflops": fp32_peak, "peak_source": "148 SMs x 128 FMA lanes x 2 x sampled SM clock",
+                "fp32": {"peak_tflops": fp32_peak, "peak_source": f"{n_sm} SMs x 128 FMA lanes x 2 x sampled SM clock",
                          "alg_tflops_all_pixels": f_alg / (tm["solve"] * 1e-3) / 1e12, "alg_tflops_valid_pixels": f_valid / (tm["solve"] * 1e-3) / 1e12,
                          "frac_valid_pixels": f_valid / (tm["solve"] * 1e-3) / 1e12 / fp32_peak,
                          "executed_fp32_thread_inst_per_launch": prof.get("fp32_thread_inst_per_launch")},
                 "issue": {"warp_inst_per_launch": prof.get("warp_inst_per_launch"),
-                          "frac_of_issue_peak": (prof["warp_inst_per_launch"] / (tm["solve"] * 1e-3 * sm_clock * 148 * 4)) if prof.get("warp_inst_per_launch") else None,
-                          "note": "warp instructions of the committed ncu capture / (live kernel time x 4 schedulers x 148 SMs x SM clock)"}}
+                          "frac_of_issue_peak": (prof["warp_inst_per_launch"] / (tm["solve"] * 1e-3 * sm_clock * n_sm * 4)) if prof.get("warp_inst_per_launch") else None,
+                          "note": "warp instructions of an ncu capture / (live kernel time x 4 schedulers x SMs x SM clock)"}}
         one = [wins[0]]
         for _ in range(5):
             opt.optimizeWindows(one)

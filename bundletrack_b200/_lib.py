@@ -1,5 +1,5 @@
 """ctypes binding of the C-ABI (include/bundletrack_b200.h).  The shared library is built in-tree by
-__graft_entry__.build() / `make -C bundletrack_b200/csrc`; if it is missing, or the machine has no sm_100 GPU,
+__graft_entry__.build() / `make -C bundletrack_b200/csrc`; if it is missing, or the machine has no sm_90 GPU,
 every entry point fails loudly — there is no CPU or PyTorch fallback anywhere in this package."""
 from __future__ import annotations
 
@@ -148,7 +148,7 @@ def load() -> ctypes.CDLL:
     if not os.path.exists(LIB_PATH):
         raise BtError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). bundletrack_b200 has no CPU fallback."
+            "(nvcc, sm_90a). bundletrack_b200 has no CPU fallback."
         )
     lib = ctypes.CDLL(LIB_PATH)
     lib.bt_last_error.restype = ctypes.c_char_p

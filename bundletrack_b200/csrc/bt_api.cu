@@ -28,8 +28,8 @@ extern "C" int bt_ctx_create(bt_ctx** out, int device) {
 	BT_CUDA(cudaSetDevice(device));
 	cudaDeviceProp prop;
 	BT_CUDA(cudaGetDeviceProperties(&prop, device));
-	if (prop.major != 10) {
-		bt::set_error("bt_ctx_create: device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+	if (prop.major != 9 || prop.minor != 0) {
+		bt::set_error("bt_ctx_create: device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
 		return BT_ERR_NO_DEVICE;
 	}
 	bt_ctx* c = new bt_ctx();

@@ -1,4 +1,4 @@
-// bt_common.cuh — shared declarations for the sm_100a hot-path library (no torch, no third-party headers).
+// bt_common.cuh — shared declarations for the sm_90a hot-path library (no torch, no third-party headers).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// knn.cu — all-pairs L2 k-nearest-neighbour matching of 256-d LF-Net descriptors on the 5th-gen tensor cores.
+// knn.cu — all-pairs L2 k-nearest-neighbour matching of 256-d LF-Net descriptors on the Hopper tensor cores (wgmma).
 //
 // Replaces the two cv::cuda::DescriptorMatcher::knnMatch(…, k=5) calls of SiftManager::findCorresbyNN
 // (/root/reference/src/FeatureManager.cpp:271-273) for a BATCH of frame pairs.  OpenCV's CUDA matcher materialises the nQ x nT
@@ -9,18 +9,17 @@
 //                  copy for the exact stage, |x~|^2 of the ROUNDED rows (padding rows: zero data, norm +inf) and the measured
 //                  rounding error |x~ - x| of every row.  Done once per descriptor set - once per FRAME with the persistent
 //                  pool (bt_desc_pool_store at detectFeature time, FeatureManager.cpp:907), once per call otherwise.
-//   k_knn_tc       persistent, warp-specialised tcgen05 kernel over the flattened list of (pair, 256-row B tile, 128-row A tile)
-//                  units, cut into equal contiguous ranges (one per SM: no wave quantisation).  Warp 0 keeps the B tile resident
-//                  in shared memory (128 KB, reloaded K-chunk by K-chunk while the last unit of the previous tile still runs)
-//                  and streams A tiles through a 5-stage ring with TMA (SWIZZLE_128B, K-major); warp 1 issues
-//                  tcgen05.mma.cta_group::1.kind::f16 (fp16 x fp16 -> fp32, M=128, N=256, K=16) into a double-buffered TMEM
-//                  accumulator; eight epilogue warps read it with tcgen05.ld (thread = A row, registers = 32 B columns), form
-//                  d2 = |a~|^2 + |b~|^2 - 2 a~.b~ (scaled into [0,1] by a per-pair power of two) and reduce it BOTH ways:
-//                    A->B  min over each group of 4 consecutive B columns, in registers            -> G_rowT[B group][A row]
-//                    B->A  min over each group of 4 consecutive A rows: two butterfly steps of
-//                          packed-fp16 shuffles across the lanes that hold those rows             -> G_col [A row group][B row]
+//   k_knn_tc       persistent, warp-specialised wgmma kernel over the flattened list of (pair, 256-row B tile, 128-row A tile)
+//                  units, cut into equal contiguous ranges (one per SM: no wave quantisation).  One producer thread keeps the B tile
+//                  resident in shared memory (128 KB, reloaded K-chunk by K-chunk while the last unit of the previous tile still
+//                  runs) and streams A tiles through a 5-stage ring with TMA (SWIZZLE_128B, K-major); two consumer warpgroups each
+//                  own one 128-row half of the B tile and issue wgmma.m64n128k16 (fp16 x fp16 -> fp32) for the A tile's two 64-row
+//                  halves into registers, then form d2 = |a~|^2 + |b~|^2 - 2 a~.b~ (scaled into [0,1] by a per-pair power of two)
+//                  and reduce it BOTH ways inside the thread (a group is four rows / columns one thread holds, see knn_unpos):
+//                    A->B  min over each group of 4 B columns                                      -> G_rowT[B group][A position]
+//                    B->A  min over each group of 4 A rows                                         -> G_col [A group][B position]
 //                  both stored as fp16 (round to nearest; the bound below carries the half ulp).  No data-dependent branch, no
-//                  candidate lists, ~5 issue slots per matrix element: the kernel is paced by the tensor pipe.
+//                  candidate lists, no shuffles.
 //   k_knn_select   per query (lane) over its column of group minima: exact k-th smallest key -> a rigorous threshold (measured
 //                  fp16 rounding error of both rows + accumulation slack + storage rounding) -> the groups that can still hold
 //                  one of the k nearest; each member of such a group is then checked against the OTHER direction's matrix (the
@@ -41,30 +40,23 @@
 namespace bt {
 
 static constexpr int KD = 256;              // descriptor dimension handled by the tensor path
-static constexpr int BM = 128;              // A rows per unit (UMMA M = TMEM lanes)
-static constexpr int BN = 256;              // B rows per unit (UMMA N = TMEM columns)
+static constexpr int BM = 128;              // A rows per unit (two wgmma M = 64 row blocks)
+static constexpr int BN = 256;              // B rows per unit (two consumer warpgroups)
+static constexpr int WN = 128;              // B rows per consumer warpgroup (wgmma N)
 static constexpr int BK = 64;               // K elements per smem chunk: 64 fp16 = 128 B = one SWIZZLE_128B atom row
 static constexpr int KCH = KD / BK;         // 4 chunks
 static constexpr int STAGES = 5;            // A-operand pipeline depth (16 KB each)
 static constexpr int GRP = 4;               // rows / columns per group minimum
-static constexpr int EPI_WARPS = 16;        // 4 per TMEM lane quarter, 64 accumulator columns each: 4 epilogue warps per scheduler hide the shuffle / TMEM-load latencies
-static constexpr int KNN_THREADS = 32 * (2 + EPI_WARPS); // warp 0 TMA, warp 1 MMA, warps 2..17 epilogue
+static constexpr int KNN_THREADS = 128 * 3; // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue
+static constexpr uint32_t CONSUMER_WARPS = 8;         // arrivals that free an A stage / a B chunk (lane 0 of every consumer warp)
 static constexpr uint32_t SA_BYTES = BM * BK * 2;     // 16 KB per stage: one K-chunk of an A tile
 static constexpr uint32_t SB_BYTES = BN * BK * 2;     // 32 KB per K-chunk of the resident B tile
 static constexpr uint32_t SMEM_B = KCH * SB_BYTES;    // 128 KB
 static constexpr uint32_t SMEM_A = STAGES * SA_BYTES; // 80 KB
 static constexpr uint32_t SMEM_NORM = BN * 4;         // 1 KB
 static constexpr uint32_t SMEM_BAR = 256;
-static constexpr uint32_t SMEM_TOTAL = SMEM_B + SMEM_A + SMEM_NORM + SMEM_BAR + 1024;   // + alignment slack
-// CTA-pair form (cta_group::2, M = 256): a CTA keeps HALF of the B tile (128 rows, 64 KB) and streams its own 128 A rows through a deeper ring
-static constexpr int STAGES_P = 5;
-static constexpr uint32_t SBH_BYTES = (BN / 2) * BK * 2;                 // 16 KB per K-chunk of the B half tile
-static constexpr uint32_t SMEM_BH = KCH * SBH_BYTES;                     // 64 KB: one B half tile
-static constexpr uint32_t SMEM_B_P = 2 * SMEM_BH;                        // 128 KB: DOUBLE-BUFFERED - the next B tile loads while the current one is used (its own producer warp)
-static constexpr uint32_t SMEM_A_P = STAGES_P * SA_BYTES;                // 80 KB
-static constexpr uint32_t SMEM_TOTAL_P = SMEM_B_P + SMEM_A_P + SMEM_NORM + SMEM_BAR + 1024;
-static constexpr int KNN_THREADS_P = KNN_THREADS + 32;                   // + the B-tile producer warp
-static constexpr int SEL_MAXG = 16;         // groups / candidates kept per query; more => exact fallback
+static constexpr uint32_t SMEM_TOTAL = SMEM_B + SMEM_A + SMEM_NORM + SMEM_BAR + 1024;   // + alignment slack: 210 KB of the 227 KB a block may have
+static constexpr int SEL_MAXG = 16;        // groups / candidates kept per query; more => exact fallback
 static constexpr int SEL_MAXC = 16;
 
 struct KnnPair {          // one non-empty frame pair: units (B tile tt, A tile qt), qt fastest
@@ -109,76 +101,45 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
 	             "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
 	             : "memory");
 }
-// ---- CTA-pair (cta_group::2) variants: both CTAs of a pair issue their TMA loads against the LEADER's (rank 0) full barrier, the leader's
-//      MMA thread commits to the same barrier offset in BOTH CTAs (multicast), the peer's epilogue arrives on the leader's barrier remotely
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1) {
-	asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
-	             "l"(tmap), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)      // peer bit cleared: the transaction bytes land on CTA 0's barrier
-	             : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair(uint64_t* bar) {
-	asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"((unsigned short)3) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-	asm volatile(
-	    "{\n"
-	    ".reg .pred p;\n"
-	    "setp.ne.b32 p, %4, 0;\n"
-	    "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-	    "}\n" ::"r"(d_tmem),
-	    "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-	    : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_rank0(uint64_t* bar) {      // arrive on the barrier at this offset in the cluster's CTA 0
-	uint32_t remote;
-	asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(0u));
-	asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");      // (default .release.cta: with .release.cluster the arrive queued behind the previous unit's global stores - 26 % of the kernel's stall samples)
-}
-__device__ __forceinline__ void cluster_sync_all() {
-	asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-	asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-	asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, fp16 inputs, fp32 accumulate
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-	asm volatile(
-	    "{\n"
-	    ".reg .pred p;\n"
-	    "setp.ne.b32 p, %4, 0;\n"
-	    "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-	    "}\n" ::"r"(d_tmem),
-	    "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-	    : "memory");
-}
-// UMMA shared-memory descriptor, K-major operand, SWIZZLE_128B, rows at 128-byte pitch, 8-row groups 1024 B apart.
-//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major) | [32,46) stride byte
-//   offset >> 4 (= 1024 >> 4) | [46,48) descriptor version = 1 (sm_100) | [61,64) layout type (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t smem_addr) {
+// wgmma shared-memory matrix descriptor, K-major operand, SWIZZLE_128B, rows at 128-byte pitch, 8-row groups 1024 B apart.
+//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major) | [32,46) stride byte offset >> 4
+//   (= 1024 >> 4) | [62,64) layout type (1 = SWIZZLE_128B).  A K step of 16 halves inside the 128-byte swizzle row adds 32 B to the start.
+__device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t smem_addr) {
 	uint64_t d = 0;
 	d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+	d |= (uint64_t)1 << 16;
 	d |= (uint64_t)(1024 >> 4) << 32;
-	d |= (uint64_t)1 << 46;
-	d |= (uint64_t)2 << 61;
+	d |= (uint64_t)1 << 62;
 	return d;
 }
-// UMMA instruction descriptor (kind::f16): c_format F32 (1) @4, a_format / b_format F16 (0) @7 / @10, a/b K-major (0) @15/@16,
-// N>>3 @17, M>>4 @24.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-	return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulator registers are written asynchronously: nothing may read or move them across a wait
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[64]) {
+#pragma unroll
+	for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-#define TMEM_LD32(taddr, v)                                                                                                   \
-	asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                                     \
-	             "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                      \
-	             "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"                      \
-	             : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),     \
-	               "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),          \
-	               "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),         \
-	               "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])                       \
-	             : "r"(taddr))
+// D[64 x 128] (+)= A[smem, 64 x 16] * B[smem, 128 x 16]^T, fp16 inputs, fp32 accumulate, both operands K-major
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+	asm volatile(
+	    "{\n"
+	    ".reg .pred p;\n"
+	    "setp.ne.b32 p, %66, 0;\n"
+	    "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+	    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, "
+	    "%28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, "
+	    "%54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n"
+	    "}\n"
+	    : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+	      "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+	      "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+	      "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+	      "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+	      "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+	      "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+	    : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
 
 // ------------------------------------------------------------------------------------------------ k_desc_prep
 struct PrepSet { const float* src; size_t pitch_bytes; int n; int row0; int rows_padded; int slot; };
@@ -271,283 +232,168 @@ __device__ __forceinline__ uint32_t hmin2_u32(uint32_t a, uint32_t b) {
 	return h2_as_u32(r);
 }
 
-// ---- the epilogue's view of the accumulator -----------------------------------------------------------------------------------
-// tcgen05.ld.16x256b hands a thread the m16n8 accumulator fragment (probed on a B200, scripts/probe/tmem_layout.cu): register 4j + e of
-// thread T = TMEM lane base + T/4 + 8 (e >> 1), column 8j + 2 (T % 4) + (e & 1).  Two such loads (lanes +0..15, +16..31) give a thread
-// FOUR rows (T/4 + 8k, k = 0..3) x the column pairs (8j + 2m, 8j + 2m + 1), m = T % 4.  Both group minima the matcher needs then stay
-// inside the thread when a "group" is four indices 8 apart in a block of 32 - rows {r, r+8, r+16, r+24}, columns {c, c+8, c+16, c+24}:
+// ---- the consumer's view of the accumulator -----------------------------------------------------------------------------------
+// wgmma.m64nNk16 hands thread T of a warpgroup (warp w = T / 32, lane l) register 4j + 2i + e = row 16 w + l / 4 + 8 i, column
+// 8 j + 2 (l % 4) + e.  With two such accumulators (A rows 0..63 and 64..127 of the tile) a thread holds FOUR rows r + {0, 8, 64, 72},
+// r = 16 w + l / 4, and of each of them the columns c + {0, 8, 64, 72}, c = 16 w' + 2 (l % 4) + e, w' = 0..3.  A "group" of four rows
+// (columns) is such a set, so both group minima the matcher needs stay inside the thread:
 //   B->A  min over the thread's four rows, per column                      (3 packed-fp16 min per column pair)
-//   A->B  min over four column pairs 8 apart, per row                      (3 packed-fp16 min per two groups)
-// no shuffle, no select, no cross-half step (the first version grouped 4 CONSECUTIVE rows / columns of the 32x32b layout: 24 selects +
-// 12 shuffles + 24 fp32 min per 32 columns, and the ALU pipe, not the tensor pipe, paced the kernel).
-// In POSITION space pos(i) = (i & ~31) + 4 (i % 8) + (i % 32) / 8 such a group is four CONSECUTIVE positions; both group-minimum matrices
-// are stored by position, and a thread's results land on 8 / 16 contiguous bytes.  k_knn_select works in position space and converts
-// back with unpos() where it touches real rows.
-__host__ __device__ __forceinline__ int knn_unpos(int p) { return (p & ~31) + 8 * (p & 3) + ((p & 31) >> 2); }
+//   A->B  min over the four columns of a group, per row                    (3 packed-fp16 min per two groups)
+// no shuffle, no select.  In POSITION space a group is four CONSECUTIVE positions: in a block of 128, position p belongs to group
+// g = (p / 4) % 32 = 8 w + q and is row 16 w + q + 8 (p & 1) + 64 ((p >> 1) & 1).  Both group-minimum matrices are stored by position,
+// and a thread's results land on 8 / 16 contiguous bytes.  k_knn_select works in position space and converts back with knn_unpos()
+// where it touches real rows.
+__host__ __device__ __forceinline__ int knn_unpos(int p) { return (p & ~127) + 16 * ((p >> 5) & 3) + ((p >> 2) & 7) + 8 * (p & 1) + 64 * ((p >> 1) & 1); }
 
-#define TMEM_LD_16x256b_x8(taddr, v)                                                                                          \
-	asm volatile("tcgen05.ld.sync.aligned.16x256b.x8.b32 "                                                                    \
-	             "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                      \
-	             "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"                      \
-	             : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),     \
-	               "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),          \
-	               "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),         \
-	               "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])                       \
-	             : "r"(taddr))
-
-// one 16-lane load (two of the thread's rows x 8 column pairs): d2 (scaled) = |a~|^2 + |b~|^2 - 2 a~.b~ with packed f32x2 arithmetic,
-// clamped at zero and rounded to fp16 pairs (cvt.rn.relu: a rounding-level negative d2 becomes +0, so the halves order like unsigned integers)
-__device__ __forceinline__ void epi_rows(const uint32_t (&v)[32], const unsigned long long (&nb)[8], float nAs0, float nAs1, unsigned long long m2s2,
-                                         uint32_t (&h0)[8], uint32_t (&h1)[8]) {
-	unsigned long long na0, na1;
-	asm("mov.b64 %0, {%1, %1};" : "=l"(na0) : "f"(nAs0));
-	asm("mov.b64 %0, {%1, %1};" : "=l"(na1) : "f"(nAs1));
-#pragma unroll
-	for (int j = 0; j < 8; j++) {
-		unsigned long long x0, x1;
-		float lo, hi;
-		asm("mov.b64 %0, {%1, %2};" : "=l"(x0) : "r"(v[4 * j]), "r"(v[4 * j + 1]));
-		asm("mov.b64 %0, {%1, %2};" : "=l"(x1) : "r"(v[4 * j + 2]), "r"(v[4 * j + 3]));
-		asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(x0) : "l"(m2s2), "l"(x0), "l"(nb[j]));
-		asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(x1) : "l"(m2s2), "l"(x1), "l"(nb[j]));
-		asm("add.rn.f32x2 %0, %1, %2;" : "=l"(x0) : "l"(x0), "l"(na0));
-		asm("add.rn.f32x2 %0, %1, %2;" : "=l"(x1) : "l"(x1), "l"(na1));
-		asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(x0));
-		asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(h0[j]) : "f"(hi), "f"(lo));
-		asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(x1));
-		asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(h1[j]) : "f"(hi), "f"(lo));
-	}
+// d2 (scaled) = |a~|^2 + |b~|^2 - 2 a~.b~ of a column pair, clamped at zero and rounded to an fp16 pair (cvt.rn.relu: a rounding-level
+// negative d2 becomes +0, so the halves order like unsigned integers)
+__device__ __forceinline__ uint32_t d2_f16x2(float acc_lo, float acc_hi, float2 nb, float na, float m2s) {
+	const float lo = __fadd_rn(__fmaf_rn(m2s, acc_lo, nb.x), na), hi = __fadd_rn(__fmaf_rn(m2s, acc_hi, nb.y), na);
+	uint32_t h;
+	asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(hi), "f"(lo));
+	return h;
 }
 
-// developer aid: cycles the MMA-issuing thread of every CTA spent waiting, by cause (read with bt_knn_debug_prof)
-__device__ long long g_knn_prof[160][6];
-
-// PAIR = false: one CTA per (128 A rows x 256 B rows) unit.  PAIR = true: a CLUSTER OF TWO CTAs (one TPC) per (256 x 256) unit -
-// tcgen05.mma.cta_group::2, M = 256: CTA r holds A rows [128 r, 128 r + 128) of the unit and HALF of the B tile; the leader (rank 0)
-// issues every MMA, each SM's tensor core accumulates its own 128 rows x 256 columns in its own TMEM, the B operand is read from shared
-// memory once per pair instead of once per SM, and the freed 64 KB hold a SECOND B buffer filled by its own producer warp (no bubble at
-// a tile switch).  Measured on B200 (45 pairs x 2000^2): correct on the first run, but NOT faster - 0.083-0.088 ms vs 0.081 ms.  The MMA
-// thread's own clock (bt_knn_debug_prof) shows why: per unit it waits ~100 cycles for the epilogue, ~110-250 for B and ~320 for A tiles in
-// BOTH forms, and issues for ~2500 - the pass is paced by the tensor pipe at the clock the chip sustains under this load (~1.5 GHz: the
-// kernel's 125 k cycles take 81 us), not by shared-memory bandwidth.  Kept behind BT_KNN_CTA_PAIRS=1 (tested), not the default.
-template <bool PAIR> __global__ void __launch_bounds__(PAIR ? KNN_THREADS_P : KNN_THREADS, 1)
+// One CTA per SM, persistent over its slice of the unit list.  Warpgroup 0: one thread issues every TMA load (the resident B tile per
+// K-chunk, the A tiles through the STAGES ring).  Warpgroups 1 and 2 (consumer c = 0, 1): B rows [128 c, 128 c + 128) of the tile against
+// all 128 A rows as two 64 x 128 accumulators in registers, then the epilogue straight from the registers into the two matrices.
+__global__ void __launch_bounds__(KNN_THREADS, 1)
 k_knn_tc(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const KnnPair* __restrict__ pairs, int n_pairs, int total_units,
          const float* __restrict__ norms, const PairConst* __restrict__ pconst, __half* __restrict__ G) {
-	constexpr int NST = PAIR ? STAGES_P : STAGES;
-	constexpr uint32_t B_CHUNK = PAIR ? SBH_BYTES : SB_BYTES;
-	constexpr uint32_t B_BYTES = PAIR ? SMEM_B_P : SMEM_B, A_BYTES = PAIR ? SMEM_A_P : SMEM_A;
-	constexpr int UM = PAIR ? 2 * BM : BM;      // A rows per unit
 	extern __shared__ uint8_t smem_raw[];
 	uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B needs 1024-B alignment
 	uint8_t* sB = smem;
-	uint8_t* sA = smem + B_BYTES;
-	float* sNorm = reinterpret_cast<float*>(smem + B_BYTES + A_BYTES);
-	uint64_t* bars = reinterpret_cast<uint64_t*>(smem + B_BYTES + A_BYTES + SMEM_NORM);
+	uint8_t* sA = smem + SMEM_B;
+	float* sNorm = reinterpret_cast<float*>(smem + SMEM_B + SMEM_A);
+	uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SMEM_B + SMEM_A + SMEM_NORM);
 	uint64_t* b_full = bars + 0;               // [KCH]  resident B tile, per K-chunk
 	uint64_t* b_empty = bars + KCH;            // [KCH]
-	uint64_t* full = bars + 2 * KCH;           // [NST]
-	uint64_t* empty = full + NST;              // [NST]
-	uint64_t* tm_full = empty + NST;           // [2]
-	uint64_t* tm_empty = tm_full + 2;          // [2]
-	uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tm_empty + 2);
+	uint64_t* full = bars + 2 * KCH;           // [STAGES]
+	uint64_t* empty = full + STAGES;           // [STAGES]
 
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	uint32_t cr = 0;      // rank of this CTA in its pair
-	if constexpr (PAIR) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cr));
-	if (warp == 0 && lane == 0) {
+	if (threadIdx.x == 0) {
 		asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
 		asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
-		for (int s = 0; s < KCH; s++) { mbar_init(b_full + s, 1); mbar_init(b_empty + s, 1); }
-		for (int s = 0; s < NST; s++) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
-		for (int b = 0; b < 2; b++) { mbar_init(tm_full + b, 1); mbar_init(tm_empty + b, PAIR ? 2 * EPI_WARPS : EPI_WARPS); }
+		for (int s = 0; s < KCH; s++) { mbar_init(b_full + s, 1); mbar_init(b_empty + s, CONSUMER_WARPS); }
+		for (int s = 0; s < STAGES; s++) { mbar_init(full + s, 1); mbar_init(empty + s, CONSUMER_WARPS); }
 		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 	}
-	if constexpr (PAIR) cluster_sync_all();      // the peer's barriers exist before anything can arrive on them
-	if (warp == 1) {   // TMEM: all 512 columns (two 256-column accumulators); this kernel runs 1 CTA / SM
-		if constexpr (PAIR) {
-			asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(512u) : "memory");
-			asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-		} else {
-			asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(512u) : "memory");
-			asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-		}
-	}
-	tc_fence_before();
 	__syncthreads();
-	tc_fence_after();
-	const uint32_t tmem_base = *tmem_ptr_smem;
-	// this CTA's (pair's) contiguous slice of the unit list (balanced to +-1 unit)
-	const int wid_ = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, nw_ = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-	const int u0 = (int)(((long long)wid_ * total_units) / nw_), u1 = (int)(((long long)(wid_ + 1) * total_units) / nw_);
+	// this CTA's contiguous slice of the unit list (balanced to +-1 unit)
+	const int u0 = (int)(((long long)blockIdx.x * total_units) / gridDim.x), u1 = (int)(((long long)(blockIdx.x + 1) * total_units) / gridDim.x);
+	if (u0 >= u1) return;
 
-	if (warp == 0) {
+	if (warp < 4) {
 		// ================================================= TMA producer
-		if (lane == 0 && u0 < u1) {
+		asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");      // registers go to the consumers: 128 x 40 + 256 x 232 <= 64 K
+		if (threadIdx.x == 0) {
 			uint32_t stage = 0, sphase = 0, bphase = 0;
 			UnitWalk w; w.init(pairs, n_pairs, u0);
 			for (int u = u0; u < u1; u++) {
 				const bool newb = (u == u0) || (w.qt == 0);
 				for (int kc = 0; kc < KCH; kc++) {
-					if constexpr (!PAIR) {
-						if (newb) {      // the previous B tile's last MMAs of this K-chunk have retired: reload the chunk while the others still run
-							mbar_wait(b_empty + kc, bphase ^ 1);
-							mbar_expect_tx(b_full + kc, SB_BYTES);
-							tma_load_2d(sB + kc * SB_BYTES, &tmap_b, b_full + kc, kc * BK, w.pr.b_row0 + w.tt * BN);
-						}
-					}      // (pair: the B tiles have their own producer warp and two buffers - this thread never blocks behind a tile switch)
+					if (newb) {      // the previous B tile's last MMAs of this K-chunk have retired: reload the chunk while the others still run
+						mbar_wait(b_empty + kc, bphase ^ 1);
+						mbar_expect_tx(b_full + kc, SB_BYTES);
+						tma_load_2d(sB + kc * SB_BYTES, &tmap_b, b_full + kc, kc * BK, w.pr.b_row0 + w.tt * BN);
+					}
 					mbar_wait(empty + stage, sphase ^ 1);
-					if constexpr (PAIR) {
-						if (cr == 0) mbar_expect_tx(full + stage, 2 * SA_BYTES);
-						tma_load_2d_pair(sA + stage * SA_BYTES, &tmap_a, full + stage, kc * BK, w.pr.a_row0 + w.qt * UM + (int)cr * BM);
-					} else {
-						mbar_expect_tx(full + stage, SA_BYTES);
-						tma_load_2d(sA + stage * SA_BYTES, &tmap_a, full + stage, kc * BK, w.pr.a_row0 + w.qt * BM);
-					}
-					if (++stage == NST) { stage = 0; sphase ^= 1; }
+					mbar_expect_tx(full + stage, SA_BYTES);
+					tma_load_2d(sA + stage * SA_BYTES, &tmap_a, full + stage, kc * BK, w.pr.a_row0 + w.qt * BM);
+					if (++stage == STAGES) { stage = 0; sphase ^= 1; }
 				}
 				if (newb) bphase ^= 1;
 				if (u + 1 < u1) w.next();
 			}
 		}
-	} else if (warp == 1) {
-		// ================================================= MMA issuer (one thread)
-		if (lane == 0 && u0 < u1 && cr == 0) {      // (pair: the leader issues for both SMs)
-			constexpr uint32_t idesc = umma_idesc_f16(UM, BN);
-			uint32_t stage = 0, sphase = 0, bphase = 0, tcount = 0, btile = 0;
-			UnitWalk w; w.init(pairs, n_pairs, u0);
-			long long t_tm = 0, t_b = 0, t_a = 0; const long long t_begin = clock64();
-			for (int u = u0; u < u1; u++, tcount++) {
-				const bool newb = (u == u0) || (w.qt == 0);
-				const bool lastb = (u + 1 == u1) || (w.qt == w.pr.n_qt - 1);
-				const uint32_t buf = tcount & 1, tphase = (tcount >> 1) & 1;
-				long long t0 = clock64();
-				mbar_wait(tm_empty + buf, tphase ^ 1);      // epilogue drained this accumulator
-				t_tm += clock64() - t0;
-				tc_fence_after();
-				const uint32_t d_tmem = tmem_base + buf * BN;
-				if constexpr (PAIR) { if (newb) { t0 = clock64(); mbar_wait(b_full + (btile & 1), (btile >> 1) & 1); t_b += clock64() - t0; } }      // the whole half tile (both CTAs') has landed
-				for (int kc = 0; kc < KCH; kc++) {
-					t0 = clock64();
-					if constexpr (!PAIR) { if (newb) mbar_wait(b_full + kc, bphase); }
-					long long t1 = clock64();
-					mbar_wait(full + stage, sphase);
-					t_b += t1 - t0; t_a += clock64() - t1;
-					tc_fence_after();
-					const uint32_t a_base = smem_u32(sA + stage * SA_BYTES), b_base = smem_u32(sB + (PAIR ? (btile & 1) * SMEM_BH : 0u) + kc * B_CHUNK);
-#pragma unroll
-					for (int k = 0; k < BK / 16; k++) {      // UMMA K = 16 halves = 32 bytes inside the 128-byte swizzle row
-						if constexpr (PAIR) tc_mma_f16_pair(d_tmem, umma_desc_k128(a_base + k * 32), umma_desc_k128(b_base + k * 32), idesc, (uint32_t)((kc | k) != 0));
-						else tc_mma_f16(d_tmem, umma_desc_k128(a_base + k * 32), umma_desc_k128(b_base + k * 32), idesc, (uint32_t)((kc | k) != 0));
-					}
-					if constexpr (PAIR) { tc_commit_pair(empty + stage); if (lastb && kc == KCH - 1) tc_commit_pair(b_empty + (btile & 1)); }      // (the same barrier in both CTAs; the B buffer is free after the tile's last MMA)
-					else { tc_commit(empty + stage);                // frees the A stage when these MMAs retire
-					       if (lastb) tc_commit(b_empty + kc); }    // ... and this K-chunk of the B tile after its last use
-					if (++stage == NST) { stage = 0; sphase ^= 1; }
-				}
-				if constexpr (PAIR) tc_commit_pair(tm_full + buf); else tc_commit(tm_full + buf);      // accumulator complete -> epilogue
-				if (newb) bphase ^= 1;
-				if (lastb) btile++;
-				if (u + 1 < u1) w.next();
-			}
-			if (blockIdx.x < 160) { long long* o = g_knn_prof[blockIdx.x]; o[0] = t_tm; o[1] = t_b; o[2] = t_a; o[3] = clock64() - t_begin; o[4] = u1 - u0; o[5] = 0; }
-		}
-	} else if (warp == 2 + EPI_WARPS) {
-		// ================================================= (pair only) B-tile producer: the next tile's half loads into the other buffer while the current one is in use
-		if constexpr (PAIR) {
-			if (lane == 0 && u0 < u1) {
-				uint32_t btile = 0;
-				UnitWalk w; w.init(pairs, n_pairs, u0);
-				for (int u = u0; u < u1; u++) {
-					const bool newb = (u == u0) || (w.qt == 0);
-					if (newb) {
-						const uint32_t bb = btile & 1, ph = (btile >> 1) & 1;
-						mbar_wait(b_empty + bb, ph ^ 1);      // the tile that used this buffer two tiles ago has retired
-						if (cr == 0) mbar_expect_tx(b_full + bb, 2 * SMEM_BH);      // both CTAs' halves land on the leader's barrier
-						for (int kc = 0; kc < KCH; kc++)
-							tma_load_2d_pair(sB + bb * SMEM_BH + kc * SBH_BYTES, &tmap_a, b_full + bb, kc * BK, w.pr.b_row0 + w.tt * BN + (int)cr * (BN / 2));
-						btile++;
-					}
-					if (u + 1 < u1) w.next();
-				}
-			}
-		}
-	} else if (u0 < u1) {
-		// ================================================= epilogue: 16 warps, lane quarter = warp % 4, column quarter = (warp-2) / 4
-		const int ew = warp - 2;
-		const int quarter = warp & 3;            // TMEM lanes [32*quarter, 32*quarter+32) are the only ones this warp may read
-		const int cq = ew >> 2;                  // columns [64*cq, 64*cq+64) of the 256-column tile
-		const int rq = lane >> 2, m = lane & 3;  // this thread: tile rows 32*quarter + rq + 8k (k = 0..3), column pairs 64*cq + 8j + 2m (+1), j = 0..7
-		const int etid = threadIdx.x - 64;       // 0..511
-		uint32_t tcount = 0;
-		UnitWalk w; w.init(pairs, n_pairs, u0);
-		int cur_p = -1;
-		float s = 1.f;
-		for (int u = u0; u < u1; u++, tcount++) {
-			const bool newb = (u == u0) || (w.qt == 0);
-			if (w.p != cur_p) { cur_p = w.p; s = pconst[cur_p].s; }
-			const int qrow0 = w.qt * UM + (int)cr * BM;      // first A row (within the pair's set) of this CTA's 128-row tile
-			const float* nAp = norms + w.pr.a_row0 + qrow0 + quarter * 32 + rq;      // (used after the accumulator wait: the loads have long landed)
-			const float nA0 = __ldg(nAp) * s, nA1 = __ldg(nAp + 8) * s, nA2 = __ldg(nAp + 16) * s, nA3 = __ldg(nAp + 24) * s;
-			if (newb) {      // |b~|^2 of the resident B tile (scaled) -> smem, one float per thread of the first 8 epilogue warps
-				asm volatile("bar.sync 1, 512;" ::: "memory");       // every epilogue thread is done with the previous tile's norms
-				if (etid < BN) sNorm[etid] = __ldg(norms + w.pr.b_row0 + w.tt * BN + etid) * s;
-				asm volatile("bar.sync 1, 512;" ::: "memory");
-			}
-			unsigned long long m2s2;
-			{ const float m2s = -2.0f * s; asm("mov.b64 %0, {%1, %1};" : "=l"(m2s2) : "f"(m2s)); }
-			const uint32_t buf = tcount & 1, tphase = (tcount >> 1) & 1;
-			unsigned long long nb[8];      // (|b~|^2 of columns 8j + 2m, 8j + 2m + 1), j = 0..7
-			{
-				const uint32_t nrm_s = smem_u32(sNorm + cq * 64 + 2 * m);
-#pragma unroll
-				for (int j = 0; j < 8; j++) asm volatile("ld.shared.b64 %0, [%1];" : "=l"(nb[j]) : "r"(nrm_s + 32u * j));
-			}
-			const uint32_t taddr0 = tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * BN + cq * 64;
-			// A->B matrix [B group][A position]: this thread's four rows are positions 4 rq .. 4 rq + 3 of their block of 32; its groups are 2m, 2m + 1 of each block of 32 columns
-			__half* rowp = G + w.pr.g_row + (size_t)(w.tt * (BN / GRP) + cq * 16 + 2 * m) * (size_t)w.pr.nA_pad + (size_t)(qrow0 + quarter * 32 + 4 * rq);
-			// B->A matrix [A group][B position]: row group rq of this quarter; its eight columns of a block of 32 are positions 8m .. 8m + 7
-			__half* colp = G + w.pr.g_col + (size_t)(qrow0 / GRP + quarter * 8 + rq) * (size_t)w.pr.nB_pad + (size_t)(w.tt * BN + cq * 64 + 8 * m);
-			const size_t rstride = (size_t)w.pr.nA_pad;
-			mbar_wait(tm_full + buf, tphase);
-			tc_fence_after();
-			// TMEM -> registers: the second half (rows +16, +24) is in flight while the first is converted
-			uint32_t va[32], vb[32];
-			uint32_t h0[8], h1[8], h2[8], h3[8];
-			TMEM_LD_16x256b_x8(taddr0, va);
-			asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-			TMEM_LD_16x256b_x8(taddr0 + (16u << 16), vb);
-			epi_rows(va, nb, nA0, nA1, m2s2, h0, h1);
-			asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-			tc_fence_before();
-			__syncwarp();
-			if (lane == 0) { if constexpr (PAIR) mbar_arrive_rank0(tm_empty + buf); else mbar_arrive(tm_empty + buf); }      // the accumulator is in registers: the next unit's MMAs may overwrite it
-			epi_rows(vb, nb, nA2, nA3, m2s2, h2, h3);
-#pragma unroll
-			for (int jb = 0; jb < 2; jb++) {
-				// ---- B->A: minimum over the thread's four rows, per column pair; transposed into position order and stored as 16 bytes
-				uint32_t c[4];
-#pragma unroll
-				for (int jj = 0; jj < 4; jj++) { const int j = 4 * jb + jj; c[jj] = hmin2_u32(hmin2_u32(h0[j], h1[j]), hmin2_u32(h2[j], h3[j])); }
-				*reinterpret_cast<uint4*>(colp + 32 * jb) = make_uint4(__byte_perm(c[0], c[1], 0x5410), __byte_perm(c[2], c[3], 0x5410), __byte_perm(c[0], c[1], 0x7632), __byte_perm(c[2], c[3], 0x7632));
-				// ---- A->B: minimum over the four column pairs of this block of 32 columns, per row: (group 2m, group 2m + 1) x four rows
-				const uint32_t r0 = hmin2_u32(hmin2_u32(h0[4 * jb], h0[4 * jb + 1]), hmin2_u32(h0[4 * jb + 2], h0[4 * jb + 3]));
-				const uint32_t r1 = hmin2_u32(hmin2_u32(h1[4 * jb], h1[4 * jb + 1]), hmin2_u32(h1[4 * jb + 2], h1[4 * jb + 3]));
-				const uint32_t r2 = hmin2_u32(hmin2_u32(h2[4 * jb], h2[4 * jb + 1]), hmin2_u32(h2[4 * jb + 2], h2[4 * jb + 3]));
-				const uint32_t r3 = hmin2_u32(hmin2_u32(h3[4 * jb], h3[4 * jb + 1]), hmin2_u32(h3[4 * jb + 2], h3[4 * jb + 3]));
-				__half* rp = rowp + (size_t)(8 * jb) * rstride;
-				*reinterpret_cast<uint2*>(rp) = make_uint2(__byte_perm(r0, r1, 0x5410), __byte_perm(r2, r3, 0x5410));
-				*reinterpret_cast<uint2*>(rp + rstride) = make_uint2(__byte_perm(r0, r1, 0x7632), __byte_perm(r2, r3, 0x7632));
-			}
-			if (u + 1 < u1) w.next();
-		}
+		return;
 	}
-	tc_fence_before();
-	__syncthreads();
-	if constexpr (PAIR) cluster_sync_all();      // neither CTA's shared memory / tensor memory goes away while the other still uses it
-	if (warp == 1) {
-		tc_fence_after();
-		if constexpr (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-		else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+	// ================================================= consumers
+	asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");      // two 64 x 128 fp32 accumulators = 128 registers per thread
+	const int c = warp / 4 - 1;                 // B rows [128 c, 128 c + 128) of the tile
+	const int wq = warp & 3;                    // warp of the warpgroup: accumulator rows 16 wq .. 16 wq + 15 of each 64-row half
+	const int q = lane >> 2, m = lane & 3;      // this thread: tile rows 16 wq + q + {0, 8, 64, 72}, columns 128 c + 8 j + 2 m (+1), j = 0..15
+	const int ctid = threadIdx.x - 128;         // 0..255
+	uint32_t stage = 0, sphase = 0, bphase = 0;
+	UnitWalk w; w.init(pairs, n_pairs, u0);
+	int cur_p = -1;
+	float s = 1.f;
+	float acc0[64], acc1[64];
+	for (int u = u0; u < u1; u++) {
+		const bool newb = (u == u0) || (w.qt == 0);
+		const bool lastb = (u + 1 == u1) || (w.qt == w.pr.n_qt - 1);
+		if (w.p != cur_p) { cur_p = w.p; s = pconst[cur_p].s; }
+		if (newb) {      // |b~|^2 of the resident B tile (scaled) -> smem, one float per consumer thread
+			asm volatile("bar.sync 1, 256;" ::: "memory");       // every consumer is done with the previous tile's norms
+			sNorm[ctid] = __ldg(norms + w.pr.b_row0 + w.tt * BN + ctid) * s;
+			asm volatile("bar.sync 1, 256;" ::: "memory");
+		}
+		const int qrow0 = w.qt * BM;                // first A row (within the pair's set) of this tile
+		const float* nAp = norms + w.pr.a_row0 + qrow0 + 16 * wq + q;
+		const float nA[4] = { __ldg(nAp) * s, __ldg(nAp + 8) * s, __ldg(nAp + 64) * s, __ldg(nAp + 72) * s };
+		// ---- four K-chunks; the A stage (and, after a tile's last unit, the B chunk) of chunk kc - 1 is released once chunk kc's MMAs
+		//      are issued and kc - 1's have retired
+		uint32_t prev = 0;
+		for (int kc = 0; kc < KCH; kc++) {
+			if (newb) mbar_wait(b_full + kc, bphase);
+			mbar_wait(full + stage, sphase);
+			wgmma_fence();
+			const uint32_t a_base = smem_u32(sA + stage * SA_BYTES), b_base = smem_u32(sB + kc * SB_BYTES + c * WN * 128);
+#pragma unroll
+			for (int k = 0; k < BK / 16; k++) {      // wgmma K = 16 halves = 32 bytes inside the 128-byte swizzle row
+				const uint32_t accumulate = (uint32_t)((kc | k) != 0);
+				const uint64_t bd = wgmma_desc_k128(b_base + k * 32);
+				wgmma_m64n128k16(acc0, wgmma_desc_k128(a_base + k * 32), bd, accumulate);
+				wgmma_m64n128k16(acc1, wgmma_desc_k128(a_base + 64 * 128 + k * 32), bd, accumulate);
+			}
+			wgmma_commit();
+			if (kc > 0) {
+				wgmma_wait<1>();
+				if (lane == 0) { mbar_arrive(empty + prev); if (lastb) mbar_arrive(b_empty + kc - 1); }
+			}
+			prev = stage;
+			if (++stage == STAGES) { stage = 0; sphase ^= 1; }
+		}
+		wgmma_wait<0>();
+		wgmma_fence_acc(acc0);
+		wgmma_fence_acc(acc1);
+		if (lane == 0) { mbar_arrive(empty + prev); if (lastb) mbar_arrive(b_empty + KCH - 1); }
+		if (newb) bphase ^= 1;
+		// ---- epilogue
+		const float m2s = -2.0f * s;
+		// A->B matrix [B group][A position]: this thread's four rows are positions 4 g .. 4 g + 3, g = 8 wq + q; its B groups are 8 w' + 2 m + e
+		__half* rowp = G + w.pr.g_row + (size_t)(w.tt * (BN / GRP) + c * (WN / GRP) + 2 * m) * (size_t)w.pr.nA_pad + (size_t)(qrow0 + 32 * wq + 4 * q);
+		// B->A matrix [A group][B position]: A group 8 wq + q of the tile; the members of its B groups 8 w' + 2 m + e are positions 32 w' + 8 m .. + 7
+		__half* colp = G + w.pr.g_col + (size_t)(qrow0 / GRP + 8 * wq + q) * (size_t)w.pr.nB_pad + (size_t)(w.tt * BN + c * WN + 8 * m);
+		const size_t rstride = (size_t)w.pr.nA_pad;
+		const float* nbs = sNorm + c * WN + 2 * m;
+#pragma unroll
+		for (int gw = 0; gw < 4; gw++) {      // w' = gw: member columns 16 w' + 2 m + e + {0, 8, 64, 72} = accumulator column blocks j = 2 w' + {0, 1, 8, 9}
+			uint32_t h[4][4];                 // [row][member column] as (e = 0, e = 1) fp16 pairs
+#pragma unroll
+			for (int jj = 0; jj < 4; jj++) {
+				const int j = 2 * gw + (jj & 1) + 8 * (jj >> 1);
+				const float2 nb = *reinterpret_cast<const float2*>(nbs + 8 * j);
+				h[0][jj] = d2_f16x2(acc0[4 * j], acc0[4 * j + 1], nb, nA[0], m2s);
+				h[1][jj] = d2_f16x2(acc0[4 * j + 2], acc0[4 * j + 3], nb, nA[1], m2s);
+				h[2][jj] = d2_f16x2(acc1[4 * j], acc1[4 * j + 1], nb, nA[2], m2s);
+				h[3][jj] = d2_f16x2(acc1[4 * j + 2], acc1[4 * j + 3], nb, nA[3], m2s);
+			}
+			// ---- B->A: minimum over the thread's four rows, per column pair; transposed into position order and stored as 16 bytes
+			uint32_t cm[4];
+#pragma unroll
+			for (int jj = 0; jj < 4; jj++) cm[jj] = hmin2_u32(hmin2_u32(h[0][jj], h[1][jj]), hmin2_u32(h[2][jj], h[3][jj]));
+			*reinterpret_cast<uint4*>(colp + 32 * gw) = make_uint4(__byte_perm(cm[0], cm[1], 0x5410), __byte_perm(cm[2], cm[3], 0x5410), __byte_perm(cm[0], cm[1], 0x7632), __byte_perm(cm[2], cm[3], 0x7632));
+			// ---- A->B: minimum over the four member columns, per row: (group 8 w' + 2 m, group 8 w' + 2 m + 1) x four rows
+			uint32_t r[4];
+#pragma unroll
+			for (int i = 0; i < 4; i++) r[i] = hmin2_u32(hmin2_u32(h[i][0], h[i][1]), hmin2_u32(h[i][2], h[i][3]));
+			__half* rp = rowp + (size_t)(8 * gw) * rstride;
+			*reinterpret_cast<uint2*>(rp) = make_uint2(__byte_perm(r[0], r[1], 0x5410), __byte_perm(r[2], r[3], 0x5410));
+			*reinterpret_cast<uint2*>(rp + rstride) = make_uint2(__byte_perm(r[0], r[1], 0x7632), __byte_perm(r[2], r[3], 0x7632));
+		}
+		if (u + 1 < u1) w.next();
 	}
 }
 
@@ -722,7 +568,7 @@ __device__ __forceinline__ bool dist_less(double da, int ia, double db, int ib) 
 
 // one warp per query row: exact float64 distance of every candidate on the fp32 copies of the rows (two rows in flight), top k by
 // (distance, index).  The kernel is paced by the float -> double conversions (XU pipe) and the FP64 pipe; a variant with eight lanes per
-// candidate and four candidates in flight (three shuffle steps instead of five) was measured SLOWER (0.30 vs 0.23 ms for 180 k rows): it
+// candidate and four candidates in flight (three shuffle steps instead of five) is slower: it
 // converts the query's slice four times as often and idles on the last round's unused candidate slots.
 __global__ void __launch_bounds__(256) k_knn_rerank(const SelJob* __restrict__ jobs, const int* __restrict__ qjob, int total_q,
                                                     const int32_t* __restrict__ cand, const int32_t* __restrict__ cand_cnt, const float* __restrict__ pool_f,
@@ -731,7 +577,7 @@ __global__ void __launch_bounds__(256) k_knn_rerank(const SelJob* __restrict__ j
 	const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
 	if (gw >= total_q) return;
 	const SelJob jb = jobs[__ldg(qjob + gw)];      // (k_knn_select wrote the job of every query next to its candidate count: a binary search over the
-	                                               //  job table per warp cost 66 instructions and 10 % of this kernel's stall samples)
+	                                               //  job table per warp would cost dozens of instructions per query)
 	const int r = gw - jb.q_base;
 	const int kk = min(k, jb.nt);
 	const float INF = __int_as_float(0x7f800000);
@@ -915,7 +761,6 @@ struct MatcherState {
 	int last_units = 0, last_rows = 0;
 	cudaEvent_t ev[5] = { nullptr, nullptr, nullptr, nullptr, nullptr };
 	bool timing = false;
-	bool cta_pairs = false;     // BT_KNN_CTA_PAIRS=1: tensor pass on clusters of two CTAs (cta_group::2, M = 256).  Measured on B200: no faster than one CTA per tile (0.083-0.088 vs 0.081 ms for 45 pairs x 2000^2) - see the kernel's header - so it is not the default
 	int force_fallback = 0;     // test knob: every n-th query row is sent to the exact fallback regardless of its candidates
 };
 
@@ -978,7 +823,6 @@ static int launch_prep(bt_ctx* ctx, const std::vector<PrepSet>& sets, char* hb, 
 static int knn_run(bt_ctx* ctx, int n_pairs, const PoolSetRef* A, const PoolSetRef* B, int k, int32_t* idxAB, float* distAB, int32_t* idxBA, float* distBA,
                    char* hb, size_t hoff, cudaStream_t stream) {
 	MatcherState* m = ctx->matcher;
-	const int UM = m->cta_pairs ? 2 * BM : BM;
 	std::vector<KnnPair> pairs;
 	std::vector<SelJob> jobs;
 	std::vector<int> blk_start, q_start;
@@ -991,8 +835,8 @@ static int knn_run(bt_ctx* ctx, int n_pairs, const PoolSetRef* A, const PoolSetR
 		KnnPair pr; memset(&pr, 0, sizeof pr);
 		if (live) {
 			pr.a_row0 = A[p].slot * m->slot_rows; pr.b_row0 = B[p].slot * m->slot_rows; pr.nA = nA; pr.nB = nB;
-			pr.n_qt = (nA + UM - 1) / UM; pr.n_tt = (nB + BN - 1) / BN; pr.unit0 = (int)units;      // a unit = UM A rows x 256 B rows (UM = 256 with CTA pairs)
-			pr.nA_pad = pr.n_qt * UM; pr.nB_pad = pr.n_tt * BN; pr.setA = A[p].slot; pr.setB = B[p].slot;
+			pr.n_qt = (nA + BM - 1) / BM; pr.n_tt = (nB + BN - 1) / BN; pr.unit0 = (int)units;      // a unit = 128 A rows x 256 B rows
+			pr.nA_pad = pr.n_qt * BM; pr.nB_pad = pr.n_tt * BN; pr.setA = A[p].slot; pr.setB = B[p].slot;
 			pr.g_row = g_off; g_off += (long long)(pr.nB_pad / GRP) * pr.nA_pad;
 			pr.g_col = g_off; g_off += (long long)(pr.nA_pad / GRP) * pr.nB_pad;
 			units += (long long)pr.n_qt * pr.n_tt;
@@ -1000,7 +844,7 @@ static int knn_run(bt_ctx* ctx, int n_pairs, const PoolSetRef* A, const PoolSetR
 		}
 		for (int dir = 0; dir < 2; dir++) {
 			SelJob jb; memset(&jb, 0, sizeof jb);
-			jb.nq = dir == 0 ? nA : nB; jb.nt = dir == 0 ? nB : nA; jb.n_groups = (jb.nt + 31) / 32 * (32 / GRP);      // whole blocks of 32 positions: a block's valid rows are spread over all of its groups
+			jb.nq = dir == 0 ? nA : nB; jb.nt = dir == 0 ? nB : nA; jb.n_groups = (jb.nt + 127) / 128 * (128 / GRP);      // whole blocks of 128 positions: a block's valid rows are spread over all of its groups
 			jb.q_pool_row0 = (dir == 0 ? A[p].slot : B[p].slot) * m->slot_rows; jb.t_pool_row0 = (dir == 0 ? B[p].slot : A[p].slot) * m->slot_rows;
 			jb.pconst = live ? (int)pairs.size() - 1 : -1;
 			if (live) {
@@ -1010,7 +854,7 @@ static int knn_run(bt_ctx* ctx, int n_pairs, const PoolSetRef* A, const PoolSetR
 			jb.dir = dir; jb.out_off = (int)off_dir[dir]; jb.q_base = q_total; jb.blk0 = blocks;
 			jobs.push_back(jb);
 			blk_start.push_back(blocks); q_start.push_back(q_total);
-			blocks += (jb.nq + 63) / 64; q_total += jb.nq; off_dir[dir] += (size_t)jb.nq;
+			blocks += (jb.nq + 127) / 128 * 2; q_total += jb.nq; off_dir[dir] += (size_t)jb.nq;
 		}
 	}
 	BT_REQUIRE((size_t)g_off <= m->g_halves_cap && q_total <= m->max_q_total && blocks <= m->max_blocks && units < (1ll << 31), BT_ERR_CAPACITY, "bt_knn_match_pairs: work list overflow");
@@ -1033,19 +877,8 @@ static int knn_run(bt_ctx* ctx, int n_pairs, const PoolSetRef* A, const PoolSetR
 	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[1], stream));      // [ev0, ev1) = descriptor conversion + table upload + per-pair constants; [ev1, ev2) = k_knn_tc alone
 	// ---- kernels
 	if (n_live > 0) {
-		if (m->cta_pairs) {      // clusters of two CTAs (one TPC each): cta_group::2 MMAs, M = 256
-			cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof cfg);
-			const int n_cl = (int)std::min<long long>(units, ctx->sm_count / 2);
-			cfg.gridDim = dim3(2 * n_cl); cfg.blockDim = dim3(KNN_THREADS_P); cfg.dynamicSmemBytes = SMEM_TOTAL_P; cfg.stream = stream;
-			cudaLaunchAttribute at[1];
-			at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-			cfg.attrs = at; cfg.numAttrs = 1;
-			BT_CUDA(cudaLaunchKernelEx(&cfg, k_knn_tc<true>, m->tmap_a, m->tmap_b, (const KnnPair*)m->pairs.as<KnnPair>(), n_live, (int)units, (const float*)m->norms.as<float>(),
-			                           (const PairConst*)m->pconst.as<PairConst>(), m->G.as<__half>()));
-		} else {
-			const int grid = (int)std::min<long long>(units, ctx->sm_count);
-			k_knn_tc<false><<<grid, KNN_THREADS, SMEM_TOTAL, stream>>>(m->tmap_a, m->tmap_b, m->pairs.as<KnnPair>(), n_live, (int)units, m->norms.as<float>(), m->pconst.as<PairConst>(), m->G.as<__half>());
-		}
+		const int grid = (int)std::min<long long>(units, ctx->sm_count);
+		k_knn_tc<<<grid, KNN_THREADS, SMEM_TOTAL, stream>>>(m->tmap_a, m->tmap_b, m->pairs.as<KnnPair>(), n_live, (int)units, m->norms.as<float>(), m->pconst.as<PairConst>(), m->G.as<__half>());
 	}
 	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[2], stream));
 	KnnOut out; out.idx[0] = idxAB; out.idx[1] = idxBA; out.dist[0] = distAB; out.dist[1] = distBA;
@@ -1088,12 +921,11 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 	m->n_transient = std::min(2 * max_pairs, 128);       // distinct descriptor sets one bt_knn_match_pairs call may name (all pairs of K frames: K sets)
 	int rc;
 	if ((rc = pool_alloc(m)) != BT_OK) return rc;
-	{ const char* e = getenv("BT_KNN_CTA_PAIRS"); m->cta_pairs = (e && atoi(e) != 0); }
-	const int pad_a = (max_feats + 2 * BM - 1) / (2 * BM) * (2 * BM);      // A sets are padded to whole 256-row units of the CTA-pair kernel
+	const int pad_a = (max_feats + BM - 1) / BM * BM;      // A sets are padded to whole 128-row tiles
 	m->g_halves_cap = (size_t)max_pairs * ((size_t)(slot_rows / GRP) * pad_a + (size_t)(pad_a / GRP) * slot_rows);
 	m->max_jobs = 2 * max_pairs;
 	m->max_q_total = 2 * max_pairs * max_feats;
-	m->max_blocks = 2 * max_pairs * ((max_feats + 63) / 64);
+	m->max_blocks = 2 * max_pairs * ((max_feats + 127) / 128 * 2);      // k_knn_select covers whole 128-position blocks, 64 queries per CTA
 #define RES(buf, bytes) if ((rc = m->buf.alloc(bytes)) != BT_OK) return rc
 	RES(sets, sizeof(PrepSet) * (size_t)std::max(m->n_transient, 1));
 	RES(pairs, sizeof(KnnPair) * ((size_t)max_pairs + 1));
@@ -1112,8 +944,7 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 #undef RES
 	if ((rc = m->h_stage.alloc(sizeof(PrepSet) * 2 * max_pairs + sizeof(KnnPair) * ((size_t)max_pairs + 1) + (sizeof(SelJob) + 2 * sizeof(int)) * m->max_jobs + 4096)) != BT_OK) return rc;
 	if (!m->ev_up) BT_CUDA(cudaEventCreateWithFlags(&m->ev_up, cudaEventDisableTiming));
-	BT_CUDA(cudaFuncSetAttribute(k_knn_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_TOTAL));
-	BT_CUDA(cudaFuncSetAttribute(k_knn_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_TOTAL_P));
+	BT_CUDA(cudaFuncSetAttribute(k_knn_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_TOTAL));
 	return BT_OK;
 }
 
@@ -1175,9 +1006,6 @@ extern "C" int bt_knn_match_slots(bt_ctx* ctx, int n_pairs, const int32_t* slotA
 	return knn_run(ctx, n_pairs, A.data(), B.data(), k, idxAB, distAB, idxBA, distBA, m->h_stage.as<char>(), 0, stream);
 }
 
-extern "C" BT_API int bt_knn_debug_prof(long long* out960) {      // developer aid, not part of the public header
-	return cudaMemcpyFromSymbol(out960, g_knn_prof, sizeof(long long) * 160 * 6) == cudaSuccess ? BT_OK : BT_ERR_CUDA;
-}
 extern "C" int bt_knn_debug_force_fallback(bt_ctx* ctx, int every_nth) {
 	BT_REQUIRE(ctx && ctx->matcher, BT_ERR_INVALID_ARG, "bt_knn_debug_force_fallback: call bt_matcher_reserve first");
 	ctx->matcher->force_fallback = every_nth > 0 ? every_nth : 0;

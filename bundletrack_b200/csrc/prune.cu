@@ -211,7 +211,7 @@ __global__ void __launch_bounds__(1024) k_emit_entryj(const PrunePair* __restric
 	if (tid == 0) *total_out = min(s_carry, capacity);
 }
 
-// one CTA per pair: its EntryJ block (a lone CTA filling all pairs took 0.1 ms for 20 k entries)
+// one CTA per pair: its EntryJ block (a lone CTA filling all pairs would serialise the whole list)
 __global__ void __launch_bounds__(256) k_emit_fill(const PrunePair* __restrict__ pairs, const bt_correspondence* __restrict__ corr, const int32_t* __restrict__ inlier_ids,
                                                     const int32_t* __restrict__ n_entry, const int32_t* __restrict__ entry_off, bt_entryj* __restrict__ entry_out, int capacity,
                                                     float4* __restrict__ uv_out) {

@@ -120,15 +120,16 @@ static constexpr int kEvalCheck = 128;   // points between two looks at the best
 //    is <= thresh (computed on the host): same truth value for every float, no square root;
 //  * a trial stops as soon as it can no longer reach the best count any trial of this pair has finished with so far
 //    (count + points left < best): it cannot win and it cannot tie, so the winner (max count, then lowest trial) is unchanged.
-// packed f32x2 arithmetic (sm_100): two points per instruction, each lane an ordinary IEEE operation
-__device__ __forceinline__ unsigned long long pk2(float lo, float hi) { unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ unsigned long long mul2(unsigned long long a, unsigned long long b) { unsigned long long r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) { unsigned long long r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ unsigned long long add2(unsigned long long a, unsigned long long b) { unsigned long long r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ unsigned long long sub2(unsigned long long a, unsigned long long b) { unsigned long long r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
+// two points side by side: sm_90 has no packed f32x2 arithmetic, so each helper is two scalar IEEE operations (the _rn intrinsics keep
+// nvcc from contracting them into other forms)
+__device__ __forceinline__ float2 pk2(float lo, float hi) { return make_float2(lo, hi); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 sub2(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
 
-// One thread per trial, the pair's points broadcast from shared memory; TWO points per instruction (the kernel is issue-bound: 2000
-// trials x ~2-3 k candidate points x 45 pairs).  Every lane performs exactly the operations, in exactly the order, of the scalar
+// One thread per trial, the pair's points broadcast from shared memory, two points per loop step (the kernel is issue-bound: 2000
+// trials x ~2-3 k candidate points x 45 pairs).  Every point gets exactly the operations, in exactly the order, of the scalar
 // expression `pb - (P[0]*pa.x + P[1]*pa.y + P[2]*pa.z + P[3])` as nvcc contracts it (mul y, fma x, fma z, add t; squares: mul dy, fma dx, fma
 // dz), so the inlier counts are bit-identical to the scalar version that was pinned against the reference's ransacMultiPairGPU.
 __global__ void __launch_bounds__(256) k_ransac_eval(const RansacPair* __restrict__ pairs, int n_trials, const float* __restrict__ poses, const int* __restrict__ good,
@@ -137,7 +138,7 @@ __global__ void __launch_bounds__(256) k_ransac_eval(const RansacPair* __restric
 	const int pair = blockIdx.y, t = blockIdx.x * blockDim.x + threadIdx.x;
 	const RansacPair pr = pairs[pair];
 	const bool live = t < n_trials && good[(size_t)pair * n_trials + t] != 0;
-	unsigned long long P2[12];
+	float2 P2[12];
 	{
 		const float* Pg = poses + ((size_t)pair * n_trials + t) * 12;
 		for (int k = 0; k < 12; k++) { const float v = live ? Pg[k] : 0.f; P2[k] = pk2(v, v); }
@@ -160,15 +161,13 @@ __global__ void __launch_bounds__(256) k_ransac_eval(const RansacPair* __restric
 #pragma unroll 4
 			for (int j = k0 >> 1; j < (k1 + 1) >> 1; j++) {
 				const float4 u = sP[0][j], v = sP[1][j], w = sP[2][j];
-				const unsigned long long ax = pk2(u.x, u.y), ay = pk2(u.z, u.w), az = pk2(v.x, v.y), bx = pk2(v.z, v.w), by = pk2(w.x, w.y), bz = pk2(w.z, w.w);
-				const unsigned long long dx = sub2(bx, add2(fma2(P2[2], az, fma2(P2[0], ax, mul2(P2[1], ay))), P2[3]));
-				const unsigned long long dy = sub2(by, add2(fma2(P2[6], az, fma2(P2[4], ax, mul2(P2[5], ay))), P2[7]));
-				const unsigned long long dz = sub2(bz, add2(fma2(P2[10], az, fma2(P2[8], ax, mul2(P2[9], ay))), P2[11]));
-				const unsigned long long d2 = fma2(dz, dz, fma2(dx, dx, mul2(dy, dy)));
-				float d2a, d2b;
-				asm("mov.b64 {%0, %1}, %2;" : "=f"(d2a), "=f"(d2b) : "l"(d2));
-				count += (d2a <= d2_max) ? 1 : 0;
-				count += (d2b <= d2_max) ? 1 : 0;
+				const float2 ax = pk2(u.x, u.y), ay = pk2(u.z, u.w), az = pk2(v.x, v.y), bx = pk2(v.z, v.w), by = pk2(w.x, w.y), bz = pk2(w.z, w.w);
+				const float2 dx = sub2(bx, add2(fma2(P2[2], az, fma2(P2[0], ax, mul2(P2[1], ay))), P2[3]));
+				const float2 dy = sub2(by, add2(fma2(P2[6], az, fma2(P2[4], ax, mul2(P2[5], ay))), P2[7]));
+				const float2 dz = sub2(bz, add2(fma2(P2[10], az, fma2(P2[8], ax, mul2(P2[9], ay))), P2[11]));
+				const float2 d2 = fma2(dz, dz, fma2(dx, dx, mul2(dy, dy)));
+				count += (d2.x <= d2_max) ? 1 : 0;
+				count += (d2.y <= d2_max) ? 1 : 0;
 			}
 			// best[pair] only ever holds counts of trials that have seen ALL points
 			const int best_cnt = (int)(__ldcg(best + pair) >> 32);

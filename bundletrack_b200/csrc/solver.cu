@@ -1,4 +1,4 @@
-// solver.cu — B200-native Gauss-Newton x PCG pose-graph solve for a BATCH of independent tracking windows.
+// solver.cu — H100-native Gauss-Newton x PCG pose-graph solve for a BATCH of independent tracking windows.
 //
 // Replaces (behind the C-ABI in include/bundletrack_b200.h) the reference's OptimizerGpu::optimizeFrames
 // (/root/reference/src/cuda/LossGPU.cu:53-139) -> CUDACache::storeFrame (CUDACache.cpp:76-88) -> SBA::align
@@ -52,9 +52,8 @@ static constexpr int kTileVals = 28;          // 21 (sym 6x6) + 6 (rhs) + 1 (#co
 static constexpr int kGrpVals = 44;           // sparse moment sums per pair group
 static constexpr int kMaxFrames = 32;
 static constexpr int kSparseTiles = 2;        // sparse tiles per window and GN iteration: each takes a contiguous share of the window's (i,j) groups (45 groups = 23 + 22: one round of
-                                              // 32 eight-lane teams each instead of two; measured as the longest tile of a lone window when it was one tile)
+                                              // 32 eight-lane teams each instead of two; as one tile it was the longest tile of a lone window)
 static constexpr size_t kTailSmemMax = 224 * 1024;   // dynamic shared memory a tail may use (227 KB per CTA minus k_solve's static arrays)
-// (a 128-thread CTA variant of k_solve was measured on B200: SLOWER, 0.55 vs 0.46 ms for 32 windows - dropped)
 static constexpr float kEps = 0.000001f;      // FLOAT_EPSILON, /root/reference/src/cuda/SolverUtil.h:10
 
 struct WinDesc {
@@ -220,9 +219,8 @@ __device__ __forceinline__ float huber_w(float e, float delta) {  // rho.y of hu
 }
 // The dense pixel loop's quotients.  Default: correctly rounded (__frcp_rn, IEEE Huber weight).  -DBT_DENSE_FAST_RCP builds the variant
 // with one MUFU reciprocal (1 ulp) per quotient: the reference itself is compiled with -use_fast_math (/root/reference/CMakeLists.txt:7),
-// and against its live kernels over 200 windows the two variants have the same parity statistics (DESIGN.md); the variant is 6 % faster
-// on the batch, but individual gate-sensitive windows move by ~1e-4 either way, so the shipped default keeps the arithmetic the
-// committed parity windows were pinned with.
+// but individual gate-sensitive windows move by ~1e-4 either way between the two variants, so the shipped default keeps the
+// arithmetic the committed parity windows were pinned with.
 #ifndef BT_DENSE_FAST_RCP      // default: correctly rounded reciprocals / IEEE Huber weight; -DBT_DENSE_FAST_RCP builds the MUFU variant (A/B in DESIGN.md)
 __device__ __forceinline__ float rcp_fast(float x) { return __frcp_rn(x); }
 __device__ __forceinline__ float huber_w_fast(float e, float delta) { return huber_w(e, delta); }
@@ -233,12 +231,12 @@ __device__ __forceinline__ float huber_w_fast(float e, float delta) {
 	return (e <= delta * delta) ? 1.0f : delta * r;
 }
 #endif
-// 256-bit global load through the read-only path (sm_100: LDG.E.ENL2.256.CONSTANT): one instruction per 32-byte texel / source record
+// one 32-byte texel / source record through the read-only path: two 128-bit loads (the widest global load sm_90 has)
 struct __align__(32) F8 { float4 lo, hi; };
 __device__ __forceinline__ F8 ldg256(const float4* p) {
 	F8 r;
-	asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-	             : "=f"(r.lo.x), "=f"(r.lo.y), "=f"(r.lo.z), "=f"(r.lo.w), "=f"(r.hi.x), "=f"(r.hi.y), "=f"(r.hi.z), "=f"(r.hi.w) : "l"(p));
+	r.lo = __ldg(p);
+	r.hi = __ldg(p + 1);
 	return r;
 }
 __device__ __forceinline__ float warp_sum(float v) {
@@ -261,7 +259,7 @@ __device__ __forceinline__ int ld_relaxed(const int* p) {
 }
 // ticket with release (orders this thread's - and, through the preceding __syncwarp / barrier, its warp's / CTA's - earlier writes
 // before it) and acquire (the CTA that draws the last ticket sees every other tile's writes) semantics in ONE instruction; a full
-// __threadfence() by every writer lane in front of a relaxed atomic cost ~1 k cycles per tile
+// __threadfence() by every writer lane in front of a relaxed atomic costs far more per tile
 __device__ __forceinline__ int ticket_acq_rel(int* p) {
 	int old;
 	asm volatile("atom.add.acq_rel.gpu.global.s32 %0, [%1], 1;" : "=r"(old) : "l"(p) : "memory");
@@ -396,7 +394,7 @@ __device__ int build_frame_maps(const FrameGeom& g, const float* __restrict__ de
 
 // Frame preparation, one CTA per 1024 quarter-res pixels of a frame (two launches): k_prep_count counts the valid pixels of
 // every block, k_prep_frames turns the counts of the blocks before it into its offset in the frame's ordered source list and
-// writes its slice of the texel map and of the list.  (One CTA per frame walked 19 rounds serially: 50 us for a lone window.)
+// writes its slice of the texel map and of the list.  (One CTA per frame would walk 19 rounds serially.)
 __device__ __forceinline__ bool prep_sample(const WinDesc& wd, int idx, unsigned& xi, unsigned& yi) {
 	// nearest-neighbour sample position of quarter-res pixel idx in the full-res maps (resampleFloat4, CUDAImageUtil.cu:82-99)
 	const int x = idx % wd.w, y = idx / wd.w;
@@ -515,7 +513,7 @@ __global__ void __launch_bounds__(1024, 2) k_frame_cache_store(CacheStoreArgs c)
 }
 
 // The same store spread over one CTA per 1024 quarter-res pixels (count + build, like k_prep_count / k_prep_frames): a handful of new
-// frames per step - one per tracked window - otherwise runs on a handful of CTAs walking 19 rounds each (50 us for 32 frames).
+// frames per step - one per tracked window - otherwise runs on a handful of CTAs walking 19 rounds each.
 __device__ __forceinline__ bool geom_sample(const FrameGeom& g, int idx, unsigned& xi, unsigned& yi) {
 	const int x = idx % g.w, y = idx / g.w;
 	xi = (unsigned)((float)x * g.scaleW + 0.5f); yi = (unsigned)((float)y * g.scaleH + 0.5f);
@@ -651,7 +649,7 @@ __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw) {
 			atomicAdd(&s_cnt[lo - base], nch);
 			px += (unsigned long long)n;
 		}
-		// one 64-bit shared atomic per warp: 1024 threads hammering one 64-bit shared word (a CAS loop in hardware) cost 30 us here
+		// one 64-bit shared atomic per warp, not per thread: 1024 threads hammering one 64-bit shared word serialise (a CAS loop in hardware)
 #pragma unroll
 		for (int o = 16; o > 0; o >>= 1) px += __shfl_xor_sync(0xffffffffu, px, o);
 		if ((tid & 31) == 0 && px) atomicAdd(&s_px, px);
@@ -743,7 +741,7 @@ __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw) {
 struct TileAcc { float v[kTileVals]; };
 
 // Software-pipelined over a thread's pixels (stride kThreads): iteration i issues the source load of pixel i+2 while it
-// evaluates pixel i (an explicit L1 prefetch of the taps of pixel i+1 was measured SLOWER on B200 and was removed).
+// evaluates pixel i.
 template <int NT> __device__ __forceinline__ void tile_pixels(const SolveArgs& a, const WinDesc& wd, const float4* __restrict__ src,
                                             const float4* __restrict__ tex, const float* __restrict__ sM, int start, int count, TileAcc& acc) {
 	const float m00 = sM[0], m01 = sM[1], m02 = sM[2], m03 = sM[3];
@@ -1203,13 +1201,13 @@ template <int NT> __device__ void window_tail(const SolveArgs& a, const WinDesc&
 	//      with 16-byte loads (conflict-free, see tail_ld) against p in shared memory (broadcast) - no cross-lane reduction inside the
 	//      matrix-vector product; only the two scalar products of a step are reduced (warp shuffle + one word per warp through shared
 	//      memory, named barrier among the ceil(dimp / 32) warps that take part).  The first version spread every ROW over the lanes of
-	//      a warp: 20 dependent shuffles per four rows, 2.2 k cycles per step for 54 unknowns; this one takes ~0.8 k.
+	//      a warp: 20 dependent shuffles per four rows.
 	{
 		__shared__ float s_dot[3][8];
 		const int nwp = (dimp + 31) >> 5;      // warps that take part (<= 6)
 		if (dimp <= 64) {
 			// up to 11 frames (the shipped max_BA_frames is 10): ONE warp, two rows per lane - the scalar products are plain warp shuffles,
-			// nothing crosses a barrier (8.1 k -> ~4 k cycles for the five steps of a 10-frame window)
+			// nothing crosses a barrier
 			if (wid == 0) {
 				const int r0 = lane, r1 = lane + 32;
 				const bool act0 = r0 < dimp, act1 = r1 < dimp;
@@ -1347,8 +1345,7 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 	const int all = total * a.prm.num_iter_outer;      // (the tile plan reports an overflow when this does not fit 31 bits)
 	// One iteration's tiles fit the grid (a single window, a handful of windows): STATIC assignment - CTA c runs tile c of every GN
 	// iteration.  With the queue the CTAs claim one tile ahead, i.e. into the NEXT iteration, and then sit on the iteration flag while
-	// the current iteration's last tiles wait for a CTA that finishes its first one: measured on the device-wide timer for one 10-frame
-	// window, 213 of 296 CTAs had a tile of an iteration, 35 of them two in a row, and an iteration's tile phase took 12-13 us instead of 7.
+	// the current iteration's last tiles wait for a CTA that finishes its first one, and an iteration's tile phase takes up to two tiles' time.
 	const bool fixed = total <= (int)gridDim.x;
 	if (fixed && (int)blockIdx.x >= total) return;
 	if (tid == 0) {
@@ -1781,7 +1778,7 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 	}
 	// Two device staging blocks, used alternately: every upload of this batch runs on the private copy stream and only waits for the
 	// k_solve that last read THIS block (two batches ago) - so with the streaming form the 2 MB of batch k+1 cross PCIe while batch k is
-	// still being solved.  (With one block the uploads queued behind the previous k_solve: ~50 us of every streaming step.)
+	// still being solved.  (With one block the uploads would queue behind the previous k_solve.)
 	s->stage_cur ^= 1;
 	DevBuf& stage_dev = s->stage_buf[s->stage_cur];
 	if (!s->ev_stage_free[s->stage_cur]) BT_CUDA(cudaEventCreateWithFlags(&s->ev_stage_free[s->stage_cur], cudaEventDisableTiming));

@@ -1,5 +1,5 @@
 /*
- * bundletrack_b200.h — C-ABI of the B200-native pose-graph optimizer + feature matcher that drops in behind
+ * bundletrack_b200.h — C-ABI of the H100-native (sm_90a) pose-graph optimizer + feature matcher that drops in behind
  * BundleTrack's C++ surface.  Plain pointers and sizes only; no C++/torch types.  Every entry point returns
  * BT_OK (0) or a negative bt_status — it never exits, throws or hangs (the reference does all three, SURVEY.md §5).
  *
@@ -30,7 +30,7 @@ typedef enum {
 	BT_ERR_INVALID_ARG = -1,
 	BT_ERR_CAPACITY = -2,     /* more windows / frames / correspondences / features than the context was created for */
 	BT_ERR_CUDA = -3,         /* a CUDA runtime call failed; bt_last_error() has the string */
-	BT_ERR_NO_DEVICE = -4,    /* no CUDA device, or not an sm_100 part: there is NO CPU fallback */
+	BT_ERR_NO_DEVICE = -4,    /* no CUDA device, or not an sm_90 part: there is NO CPU fallback */
 	BT_ERR_UNSUPPORTED = -5
 } bt_status;
 

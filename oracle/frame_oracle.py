@@ -9,7 +9,7 @@ Follows, statement by statement (same neighbour order in the float accumulations
   computeNormals_Kernel                        /root/reference/src/cuda/CUDAImageUtil.cu:342-413
 in the order Frame::processDepth / Frame::depthToCloudAndNormals call them (/root/reference/src/Frame.cpp:152-233).
 Pinned against the reference's own kernels (oracle/_ref, compiled with the reference's -use_fast_math) through
-tests/golden/ref_frame_*.npz (made on a B200 by scripts/make_golden_frame.py): the only differences are the fast-math exp and
+tests/golden/ref_frame_*.npz (made by scripts/make_golden_frame.py): the only differences are the fast-math exp and
 division of the reference build, i.e. ~1e-7 relative on the filtered depth and a handful of threshold flips per image.
 """
 import numpy as np

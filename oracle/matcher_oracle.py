@@ -61,7 +61,7 @@ def knn_cv2(query, train, k=5):
 def ransac_pair(A, B, u3, dist_thresh):
     """Restatement of ransacMultiPairGPU for ONE pair (/root/reference/src/cuda/cuda_ransac.cu:1145-1217,1293-1302).
     A, B: [n,3] model-frame points; u3: [n_trials,3] the uniforms curand_uniform() yields after curand_init(0, trial, 0)
-    (XORWOW; taken from tests/golden/curand_xorwow_seed0.npy, generated on a B200 with the same curand call).
+    (XORWOW; taken from tests/golden/curand_xorwow_seed0.npy, generated with the same curand call).
     Rigid fit = least-squares rotation (Kabsch, float64 SVD) — the reference uses an approximate fp32 SVD of the same
     3x3 matrix.  Winner = max inlier count, ties -> lowest trial id (the reference's arg-max is racy, SURVEY.md Q8).
     Returns (inlier ids ascending, best trial id, per-trial counts)."""

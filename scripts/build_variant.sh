@@ -4,6 +4,6 @@ set -e
 cd "$(dirname "$0")/../bundletrack_b200/csrc"
 name=$1; src=$2; shift 2
 mkdir -p ../lib/variants
-nvcc -std=c++17 -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibility=hidden -I. "$@" -c "$src" -o ../lib/variants/solver_$name.o
-nvcc -shared -gencode arch=compute_100a,code=sm_100a -o ../lib/variants/libbt_$name.so ../lib/variants/solver_$name.o $(ls ../lib/obj/*.o | grep -v /solver.o) -lcuda
+nvcc -std=c++17 -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibility=hidden -I. "$@" -c "$src" -o ../lib/variants/solver_$name.o
+nvcc -shared -gencode arch=compute_90a,code=sm_90a -o ../lib/variants/libbt_$name.so ../lib/variants/solver_$name.o $(ls ../lib/obj/*.o | grep -v /solver.o) -lcuda
 echo built ../lib/variants/libbt_$name.so

@@ -2,7 +2,7 @@
 REFERENCE'S OWN ransacMultiPairGPU (oracle/_ref/libbt_ref.so = /root/reference/src/cuda/cuda_ransac.cu compiled verbatim:
 XORWOW sampling, McAdams-SVD 3-point fit :998-1102, inlier rule :1183-1200, racy arg-max :1202-1217) - the inputs and the
 inlier ids it returned.  The CPU suite pins oracle/matcher_oracle.ransac_pair against these vectors without a GPU; the GPU
-suite compares bt_ransac_pairs with them and with the reference run live.
+suite compares bt_ransac_pairs with them (and with the inlier sets scripts/make_golden_live.py records).
 
     gpurun -- 'python scripts/make_golden_ransac.py gpurun_out/golden'   &&  cp gpurun_out/golden/ref_ransac.npz tests/golden/
 """

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90); run with -m gpu on a machine that has one")
     # The built library is git-ignored: a fresh checkout has none.  Build it (nvcc cross-compiles without a GPU) rather than fail every
     # test at import; where nvcc is missing too the tests fail loudly in _lib.load(), as the product does.
     lib = os.path.join(ROOT, "bundletrack_b200", "lib", "libbundletrack_b200.so")

@@ -1,10 +1,12 @@
 """GPU parity tests of the fused frame front end (bt_frames_preprocess through the C-ABI) against the CPU restatement
-(oracle/frame_oracle.py), the committed golden vectors of the reference's kernels and - when oracle/_ref is present - the
-reference's kernels run live.  Tolerances: filtered depth 2e-6 m (a few float ulps at ~1 m; the reference build uses
+(oracle/frame_oracle.py) and the committed golden vectors of the reference's kernels (ref_frame_*.npz, and ref_live_frame.npz:
+the reference's outputs for a whole 640x480 frame, recorded on an H100 by scripts/make_golden_live.py and stored to within a
+small fraction of the tolerances below).  Tolerances: filtered depth 2e-6 m (a few float ulps at ~1 m; the reference build uses
 fast-math exp/division), normals 1e-3 (unit vectors from ~1e-3 m differences amplify depth ulps), both allowing a small
 fraction of pixels where a hard threshold (1 cm filter gate, 2 cm normal gate, 0.1 m validity) flips."""
 import glob
 import os
+import zlib
 
 import numpy as np
 import pytest
@@ -117,14 +119,41 @@ def test_golden_reference_kernels(fe, cuda_device, path):
     _check(d[0], n[0], x[0], g["depth"], rn, rx)
 
 
+# (name, quantisation step): at most half a step from the reference, i.e. <= 6 % of the depth / point tolerance and < 1 % of the normal one
+_FRAME_OUT = (("depth", 2.0 ** -22), ("xyz", 2.0 ** -22), ("normal", 2.0 ** -16))
+
+
+def frame_encode(raw, K, *ref):
+    """The reference's front-end outputs (depth, xyz, normal) of a whole frame, stored as their difference from what
+    oracle/frame_oracle.py computes for the same raw frame, in int8 multiples of a step far below the test tolerances (zero almost
+    everywhere: a few tens of KB), plus a CRC of the decoded arrays that catches a restatement which no longer decodes them."""
+    out = {}
+    for (name, step), r, o in zip(_FRAME_OUT, ref, frame_oracle.preprocess(raw, K)):
+        assert np.isfinite(r).all() and np.isfinite(o).all(), name
+        q = np.rint((np.asarray(r, np.float64) - np.asarray(o, np.float64)) / step)
+        assert np.abs(q).max() <= 127, f"{name}: the reference differs from the restatement by more than int8 steps hold"
+        out[name] = q.astype(np.int8)
+        out[name + "_crc"] = np.uint32(zlib.crc32(_decode(o, out[name], step).tobytes()))
+    return out
+
+
+def _decode(o, q, step):
+    return (np.asarray(o, np.float64) + q.astype(np.float64) * step).astype(np.float32)
+
+
+def frame_decode(raw, K, g):
+    ref = []
+    for (name, step), o in zip(_FRAME_OUT, frame_oracle.preprocess(raw, K)):
+        r = _decode(o, g[name], step)
+        assert zlib.crc32(r.tobytes()) == int(g[name + "_crc"]), f"{name}: oracle/frame_oracle.py changed; re-record tests/golden/ref_live_frame.npz"
+        ref.append(r)
+    return ref
+
+
 def test_matches_reference_kernels_live(fe, cuda_device):
-    import oracle
-    try:
-        oracle.ref_lib()
-    except Exception:
-        pytest.skip("oracle/_ref not built")
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "ref_live_frame.npz"))
     raw, K = synth.make_raw_depth(7, 480, 640)
-    rd, rx, rn, _ = oracle.ref_frame_preprocess(raw, K)
+    rd, rx, rn = frame_decode(raw, K, g)
     d, n, x = _run(fe, [raw], K, cuda_device)
     _check(d[0], n[0], x[0], rd, rn, rx)
 

@@ -1,5 +1,5 @@
 """CPU tests of the frame front-end oracle (oracle/frame_oracle.py): pinned against the golden vectors of the reference's own
-kernels (tests/golden/ref_frame_*.npz, made on a B200 by scripts/make_golden_frame.py) and checked for the properties the
+kernels (tests/golden/ref_frame_*.npz, made by scripts/make_golden_frame.py) and checked for the properties the
 reference's front end has by construction."""
 import glob
 import os

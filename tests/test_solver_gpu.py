@@ -1,5 +1,6 @@
-"""GPU parity tests of the CUDA solver (through the C-ABI) against Oracle A (CPU restatement), the committed golden
-vectors of the reference's kernels, and — when oracle/_ref is present — the reference's own kernels run live.
+"""GPU parity tests of the CUDA solver (through the C-ABI) against Oracle A (CPU restatement) and the committed golden
+vectors of the reference's own kernels (tests/golden/ref_window_*.npz, and ref_live_solver.npz: what the reference returned on
+an H100 for the windows these tests generate, recorded by scripts/make_golden_live.py).
 Tolerance everywhere: north_star's 1e-4 rad / 1e-4 m after the same 7x5 iterations."""
 import glob
 import os
@@ -191,7 +192,7 @@ def test_edge_cases(opt, cuda_device):
     assert r <= TOL and t <= TOL
     # no correspondences: dense term alone.  Without the sparse anchors the 3-frame problem is only held by the gated ICP term, and on
     # seed 6 that makes it gate-sensitive: the float and double builds of oracle A differ by 3e-5 there (3.4e-4 with the reference's
-    # pair directions) and the reference's own kernels by 4e-5 ... 8e-5 from run to run (scripts/dev_edge_dense_only.py on a B200) - no
+    # pair directions) and the reference's own kernels by 4e-5 ... 8e-5 from run to run (scripts/dev_edge_dense_only.py) - no
     # two implementations agree to 1e-4 on it.  Seed 7 is a well-conditioned window of the same shape (oracle float vs double 3e-6): the
     # 1e-4 gate is enforced there, and seed 6 is held to a multiple of the oracle's own float/double spread.
     w7 = synth.make_window(7, n_frames=3, n_corr=60)
@@ -261,14 +262,16 @@ def test_matches_reference_kernels_golden(cuda_device, path):
     o.close()
 
 
+def _recorded():
+    return np.load(os.path.join(GOLD, "ref_live_solver.npz"))
+
+
 def test_matches_reference_kernels_live(opt, cuda_device):
-    """Oracle B live: the reference's own kernels on this GPU, same inputs, its pair directions fed to both."""
-    if not os.path.exists(os.path.join(os.path.dirname(oracle.__file__), "_ref", "libbt_ref.so")):
-        pytest.skip("oracle/_ref not built")
-    for seed, N, C in ((0, 10, 2000), (40, 6, 1200)):
+    """Oracle B: the reference's own kernels on the same inputs (recorded, ref_live_solver.npz), its pair directions fed to both."""
+    g = _recorded()
+    for name, seed, N, C in (("w0", 0, 10, 2000), ("w40", 40, 6, 1200)):
         w = synth.make_window(seed, n_frames=N, n_corr=C)
-        depth, normal = _upload(w, cuda_device)
-        ref, pairs, _, _ = oracle.ref_optimize_frames([d.data_ptr() for d in depth], [n.data_ptr() for n in normal], w.H, w.W, w.K, w.corr, w.poses_init)
+        ref, pairs = g[f"{name}_poses"], g[f"{name}_pairs"]
         out = _solve(opt, w, cuda_device, dense_pairs=pairs)
         r, t = synth.pose_errors(out, ref)
         assert r <= TOL and t <= TOL, (seed, r, t)
@@ -415,7 +418,7 @@ def test_prepared_argument_blocks_equal_the_convenience_calls(cuda_device):
 def test_cfg3_whole_pool_window_n30(cuda_device):
     """BASELINE configs[2] with max_BA_frames overridden to the whole 30-keyframe pool: 435 dense pairs, 3000 correspondences,
     YCBInEOAT-style occlusion; a 174 x 174 system (the groups' moment sums stay in global memory: the tail's shared memory would not
-    hold them).  Against Oracle A and, when oracle/_ref is present, the reference's own kernels run live."""
+    hold them).  Against Oracle A and the reference's own kernels (recorded, ref_live_solver.npz)."""
     from bundletrack_b200.optimizer import OptimizerGpu, SolveWindow
     w = synth.make_window(63, n_frames=30, n_corr=3000, occlusion=True)
     depth, normal = _upload(w, cuda_device)
@@ -427,25 +430,26 @@ def test_cfg3_whole_pool_window_n30(cuda_device):
     assert synth.pose_errors(out, w.poses_gt)[0] < synth.pose_errors(w.poses_init, w.poses_gt)[0]
     again = o.optimizeWindows([SolveWindow(w.corr, w.H, w.W, depth, normal, w.poses_init, w.K)] * 2)
     assert np.array_equal(again[0], again[1])
-    if os.path.exists(os.path.join(os.path.dirname(oracle.__file__), "_ref", "libbt_ref.so")):
-        ref_b, pairs, _, _ = oracle.ref_optimize_frames([d.data_ptr() for d in depth], [n.data_ptr() for n in normal], w.H, w.W, w.K, w.corr, w.poses_init)
-        out_b = o.optimizeWindows([SolveWindow(w.corr, w.H, w.W, depth, normal, w.poses_init, w.K, dense_pairs=pairs)])[0]
-        r, t = synth.pose_errors(out_b, ref_b)
-        print(f"N=30 vs live reference kernels: rot {r:.2e} rad trans {t:.2e} m ({len(pairs)} dense pairs)")
-        assert r <= 3e-4 and t <= 2e-4, (r, t)
+    g = _recorded()
+    ref_b, pairs = g["cfg3_poses"], g["cfg3_pairs"]
+    out_b = o.optimizeWindows([SolveWindow(w.corr, w.H, w.W, depth, normal, w.poses_init, w.K, dense_pairs=pairs)])[0]
+    r, t = synth.pose_errors(out_b, ref_b)
+    print(f"N=30 vs the reference kernels: rot {r:.2e} rad trans {t:.2e} m ({len(pairs)} dense pairs)")
+    assert r <= 3e-4 and t <= 2e-4, (r, t)
     o.close()
 
 
 def test_parity_sweep_against_live_reference(cuda_device):
     """How often does a window fall outside north_star's 1e-4 rad / 1e-4 m against the reference's OWN kernels?  200 seeded windows
-    (3-8 frames, 640x480), each solved by the reference (oracle/_ref, live) and by the library with the reference's pair directions.
-    The hard dense gates amplify rounding-level differences on some windows (test_gate_sensitive_window); for every window beyond
-    the tolerance the reference is run a second time: its own float atomics make it differ from ITSELF, and that run-to-run
-    difference is the yardstick the excess is held against."""
+    (3-8 frames, 640x480), each solved by the reference (recorded, ref_live_solver.npz) and by the library with the reference's pair
+    directions.  The hard dense gates amplify rounding-level differences on some windows (test_gate_sensitive_window); the reference
+    was run twice on every window: its own float atomics make it differ from ITSELF, and that run-to-run difference is the yardstick
+    the excess is held against."""
     from bundletrack_b200.optimizer import OptimizerGpu, SolveWindow
-    if not os.path.exists(os.path.join(os.path.dirname(oracle.__file__), "_ref", "libbt_ref.so")):
-        pytest.skip("oracle/_ref not built")
     import torch
+    g = _recorded()
+    f_off = np.concatenate([[0], np.cumsum([3 + seed % 6 for seed in range(200)])])
+    p_off = np.concatenate([[0], np.cumsum(g["sweep_n_pairs"])])
     o = OptimizerGpu(None, max_windows=1, max_frames=8, max_corr=2000)
     errs, beyond, self_jitter = [], [], []
     n_seeds = 200
@@ -454,17 +458,17 @@ def test_parity_sweep_against_live_reference(cuda_device):
         w = synth.make_window(5000 + seed, n_frames=N, n_corr=200 * N)
         depth = [torch.from_numpy(w.depth[k]).to(cuda_device) for k in range(N)]
         normal = [torch.from_numpy(w.normal[k]).to(cuda_device) for k in range(N)]
-        dp, nq = [d.data_ptr() for d in depth], [n.data_ptr() for n in normal]
-        ref, pairs, _, _ = oracle.ref_optimize_frames(dp, nq, w.H, w.W, w.K, w.corr, w.poses_init)
+        rv, tv = g["sweep_rotvec"][f_off[seed]:f_off[seed + 1]], g["sweep_t"][f_off[seed]:f_off[seed + 1]]
+        ref = np.stack([np.concatenate([synth.so3_exp(r), t[:, None]], 1) for r, t in zip(rv, tv)])
+        pairs = g["sweep_pairs"][p_off[seed]:p_off[seed + 1]]
         out = o.optimizeWindows([SolveWindow(w.corr, w.H, w.W, depth, normal, w.poses_init, w.K, dense_pairs=pairs)])[0]
         e = max(synth.pose_errors(out, ref))
         errs.append(e)
         if e > TOL:
-            ref2 = oracle.ref_optimize_frames(dp, nq, w.H, w.W, w.K, w.corr, w.poses_init)[0]
             a = oracle.solve_window(w.depth, w.normal, w.K, w.corr, w.poses_init, pairs=pairs)
-            beyond.append((seed, N, e)); self_jitter.append((max(synth.pose_errors(ref2, ref)), max(synth.pose_errors(a, ref))))
+            beyond.append((seed, N, e)); self_jitter.append((float(g["sweep_jitter"][seed]), max(synth.pose_errors(a, ref))))
     errs = np.asarray(errs)
-    print(f"parity sweep vs live reference kernels: {n_seeds} windows; median {np.median(errs):.2e}, p90 {np.percentile(errs, 90):.2e}, p99 {np.percentile(errs, 99):.2e}, max {errs.max():.2e}; "
+    print(f"parity sweep vs the reference kernels: {n_seeds} windows; median {np.median(errs):.2e}, p90 {np.percentile(errs, 90):.2e}, p99 {np.percentile(errs, 99):.2e}, max {errs.max():.2e}; "
           f"{len(beyond)} beyond 1e-4: {[(s_, n_, float(f'{e_:.1e}')) for s_, n_, e_ in beyond]}; on those, reference run-to-run / oracle A vs reference: {[(float(f'{x:.1e}'), float(f'{y:.1e}')) for x, y in self_jitter]}")
     assert np.median(errs) <= 2e-5 and np.percentile(errs, 90) <= TOL, (np.median(errs), np.percentile(errs, 90))
     o.close()
