@@ -7,8 +7,8 @@
 // window there; THREE launches per BATCH here, none of them allocating:
 //
 //   k_prep_count   one CTA per 1024 quarter-res pixels of a (window, frame): number of valid pixels of the block.
-//   k_prep_frames  same grid: quarter-res cache (camera-space point + normal interleaved in one
-//                  32-byte texel so a bilinear tap is a single sector) + an order-preserving COMPACTED list of the
+//   k_prep_frames  same grid: quarter-res cache (one 16-byte texel {depth, normal} per pixel: a bilinear tap is one
+//                  128-bit load and rebuilds the camera point) + an order-preserving COMPACTED list of the
 //                  valid source pixels (the object mask leaves ~10 % of the image valid), + se(3) of the input pose.
 //                  Each block's offset in the ordered list = the counts of the blocks before it.
 //   (plan)         the LAST CTA of k_prep_frames to finish: per-window tile counts -> exclusive scan -> flat tile list.
@@ -56,14 +56,19 @@ static constexpr int kSparseTiles = 2;        // sparse tiles per window and GN 
 static constexpr size_t kTailSmemMax = 224 * 1024;   // dynamic shared memory a tail may use (227 KB per CTA minus k_solve's static arrays)
 static constexpr float kEps = 0.000001f;      // FLOAT_EPSILON, /root/reference/src/cuda/SolverUtil.h:10
 
+// What turns a quarter-res pixel into its full-res sample and camera-space point (texel_sample / texel_coord)
+struct TexelGeom {
+	float ifx, ify, icx, icy;         // inverse full-res intrinsics (m_inputIntrinsicsInv)
+	float scaleW, scaleH;             // (W-1)/(w-1), (H-1)/(h-1)  (CUDAImageUtil.cu:57-58)
+};
+
 struct WinDesc {
 	int n_frames, n_corr, n_groups, n_pairs;
 	int corr_off, grp_off, pair_off, frame_off;
 	int tile_off, n_tiles;            // per GN iteration; written by the tile plan (last CTA of k_prep_frames)
 	int H, W, w, h;                   // full / quarter resolution
 	float fx, fy, cx, cy;             // quarter-res intrinsics (CUDACache.cpp:20-24)
-	float ifx, ify, icx, icy;         // inverse full-res intrinsics (m_inputIntrinsicsInv)
-	float scaleW, scaleH;             // (W-1)/(w-1), (H-1)/(h-1)  (CUDAImageUtil.cu:57-58)
+	TexelGeom tg;
 	int compat_flip;
 	int mem_off;                      // per-frame membership CSR of this window (see SolveArgs::mem)
 	int unique_blocks;                // 1: no two groups / no two dense pairs share an unordered frame pair => cross blocks need no atomics
@@ -92,7 +97,7 @@ struct SolveArgs {
 	const float* const* depth_ptr;
 	const float4* const* normal_ptr;
 	const int* frame_win;
-	float4* texel;        // [F][2*npix_max]  the context's own maps (frames prepared by this call)
+	float4* texel;        // [F][npix_max]    the context's own maps (frames prepared by this call)
 	float4* src;          // [F][2*npix_max]
 	int* nsrc;            // [F]
 	float* grp_sums;      // [groups of the batch][kGrpVals] sparse moment sums of the current GN iteration (written by the window's sparse tile)
@@ -231,7 +236,43 @@ __device__ __forceinline__ float huber_w_fast(float e, float delta) {
 	return (e <= delta * delta) ? 1.0f : delta * r;
 }
 #endif
-// one 32-byte texel / source record through the read-only path: two 128-bit loads (the widest global load sm_90 has)
+// ---- the quarter-resolution texel map, one 16-byte record per pixel: {d', nx, ny, nz}.  d' is the nearest-neighbour depth sample
+// when it lies inside the full-resolution image and is >= 0.1, else 0; the normal is the sample's as stored (0 outside the image).
+// The camera-space point is not stored: it is rebuilt from the pixel's integer sample position with the operation order
+// ifx * (xi * d) + icx * d, pinned (no contraction choice left to the compiler), so the builders' source records and the dense
+// tap's rebuilt points are the same floats.  Every writer and reader of the record goes through the helpers below.
+// full-resolution sample position of quarter-res coordinate x (resampleFloat4 nearest, CUDAImageUtil.cu:82-99)
+__device__ __forceinline__ unsigned texel_sample(int x, float scale) { return __float2uint_rz(__fmaf_rn((float)x, scale, 0.5f)); }
+// one camera-space coordinate of the point behind sample position xi at depth d (convertDepthFloatToCameraSpaceFloat4)
+__device__ __forceinline__ float texel_coord(unsigned xi, float d, float inv_f, float inv_c) { return __fmaf_rn(inv_c, d, __fmul_rn(inv_f, __fmul_rn((float)xi, d))); }
+__device__ __forceinline__ bool texel_sample_xy(const TexelGeom& g, int W, int H, int w, int idx, unsigned& xi, unsigned& yi) {
+	xi = texel_sample(idx % w, g.scaleW); yi = texel_sample(idx / w, g.scaleH);
+	return xi < (unsigned)W && yi < (unsigned)H;
+}
+// Loads the sample of quarter-res pixel idx: returns the texel record and sets cp to the camera point ({0,0,0} and w = 0 when d' = 0).
+__device__ __forceinline__ float4 texel_build(const TexelGeom& g, int W, int H, int w, const float* __restrict__ depth, const float4* __restrict__ normal,
+                                              int idx, float4& cp, float4& nr) {
+	unsigned xi, yi;
+	float d = 0.f;
+	cp = make_float4(0.f, 0.f, 0.f, 0.f); nr = make_float4(0.f, 0.f, 0.f, 0.f);
+	if (texel_sample_xy(g, W, H, w, idx, xi, yi)) {
+		const size_t sidx = (size_t)yi * W + xi;
+		const float ds = __ldg(depth + sidx);
+		nr = __ldg(normal + sidx);
+		if (ds >= 0.1f) { d = ds; cp = make_float4(texel_coord(xi, d, g.ifx, g.icx), texel_coord(yi, d, g.ify, g.icy), d, 1.0f); }
+	}
+	return make_float4(d, nr.x, nr.y, nr.z);
+}
+// Depth of the sample of quarter-res pixel idx as texel_build sees it (0 outside the image or below 0.1): the counting sweeps use
+// it so that they agree bit for bit with the build.
+__device__ __forceinline__ float texel_depth(const TexelGeom& g, int W, int H, int w, const float* __restrict__ depth, int idx) {
+	unsigned xi, yi;
+	if (!texel_sample_xy(g, W, H, w, idx, xi, yi)) return 0.f;
+	const float d = __ldg(depth + (size_t)yi * W + xi);
+	return (d >= 0.1f) ? d : 0.f;
+}
+
+// one 32-byte source record through the read-only path: two 128-bit loads (the widest global load sm_90 has)
 struct __align__(32) F8 { float4 lo, hi; };
 __device__ __forceinline__ F8 ldg256(const float4* p) {
 	F8 r;
@@ -277,6 +318,13 @@ __device__ __forceinline__ void cp_async4(void* smem_dst, const void* gsrc) {   
 __device__ __forceinline__ void cp_async16_cg(void* smem_dst, const void* gsrc) {  // 16-byte asynchronous copy from L2 (data other CTAs wrote during this launch)
 	asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
 }
+// 16-byte shared-memory load the compiler keeps where it is written: the pixel loop re-reads its per-tile constants (transform,
+// geometry) at every use instead of holding 24 registers across the loop
+__device__ __forceinline__ float4 lds128(const float* p) {
+	float4 v;
+	asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"((unsigned)__cvta_generic_to_shared(p)));
+	return v;
+}
 __device__ __forceinline__ void tile_fetch_wait() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ void st_release(int* p, int v) {
 	asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
@@ -311,19 +359,13 @@ __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw);
 // source records at their final position.  No barrier inside either sweep, so the loads of consecutive rounds overlap.
 static constexpr int kPrepRounds = 64;      // rounds of 1024 pixels per scan (one scan covers 65536 quarter-res pixels)
 
-struct FrameGeom { int W, H, w, h; float ifx, ify, icx, icy, scaleW, scaleH; };
+struct FrameGeom { int W, H, w, h; TexelGeom tg; };
 
 // Builds one frame's quarter-resolution texel map and compacted source list (1024 threads); returns the source count.
 __device__ int build_frame_maps(const FrameGeom& g, const float* __restrict__ depth, const float4* __restrict__ normal, float4* texel, float4* src,
                                 float dmin, float dmax, int* s_cnt, int* s_wt) {
 	const int npix = g.w * g.h;
 	const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-	// nearest-neighbour sample position of quarter-res pixel idx in the full-res maps, or -1 (resampleFloat4, CUDAImageUtil.cu:82-99)
-	auto sample = [&](int idx, unsigned& xi, unsigned& yi) -> bool {
-		const int x = idx % g.w, y = idx / g.w;
-		xi = (unsigned)((float)x * g.scaleW + 0.5f); yi = (unsigned)((float)y * g.scaleH + 0.5f);
-		return xi < (unsigned)g.W && yi < (unsigned)g.H;
-	};
 	int base = 0;
 	for (int sb = 0; sb < npix; sb += kPrepRounds * 1024) {
 		const int rounds = min(kPrepRounds, (npix - sb + 1023) >> 10);
@@ -332,10 +374,8 @@ __device__ int build_frame_maps(const FrameGeom& g, const float* __restrict__ de
 		for (int r = 0; r < rounds; r++) {
 			const int idx = sb + (r << 10) + tid;
 			bool valid = false;
-			if (idx < npix) {       // must agree bit for bit with sweep 2: z = 0 for a missing / too-near sample
-				unsigned xi, yi;
-				float z = 0.f;
-				if (sample(idx, xi, yi)) { const float d = __ldg(depth + (size_t)yi * g.W + xi); if (d >= 0.1f) z = d; }
+			if (idx < npix) {
+				const float z = texel_depth(g.tg, g.W, g.H, g.w, depth, idx);
 				valid = (z > dmin && z < dmax);
 			}
 			const unsigned bal = __ballot_sync(0xffffffffu, valid);
@@ -366,18 +406,10 @@ __device__ int build_frame_maps(const FrameGeom& g, const float* __restrict__ de
 #pragma unroll 2
 		for (int r = 0; r < rounds; r++) {
 			const int idx = sb + (r << 10) + tid;
-			float4 cp = make_float4(0.f, 0.f, 0.f, 0.f), nr = make_float4(0.f, 0.f, 0.f, 0.f);
+			float4 cp, nr;
 			bool valid = false;
 			if (idx < npix) {
-				unsigned xi, yi;
-				if (sample(idx, xi, yi)) {
-					const size_t sidx = (size_t)yi * g.W + xi;
-					const float d = __ldg(depth + sidx);
-					nr = __ldg(normal + sidx);
-					if (d >= 0.1f) cp = make_float4(g.ifx * ((float)xi * d) + g.icx * d, g.ify * ((float)yi * d) + g.icy * d, d, 1.0f);
-				}
-				texel[2 * idx] = make_float4(cp.x, cp.y, cp.z, nr.x);      // 32-byte texel: point xyz + normal xyz (+ pad)
-				texel[2 * idx + 1] = make_float4(nr.y, nr.z, 0.f, 0.f);
+				texel[idx] = texel_build(g.tg, g.W, g.H, g.w, depth, normal, idx, cp, nr);
 				valid = (cp.z > dmin && cp.z < dmax);
 			}
 			const unsigned bal = __ballot_sync(0xffffffffu, valid);
@@ -395,13 +427,6 @@ __device__ int build_frame_maps(const FrameGeom& g, const float* __restrict__ de
 // Frame preparation, one CTA per 1024 quarter-res pixels of a frame (two launches): k_prep_count counts the valid pixels of
 // every block, k_prep_frames turns the counts of the blocks before it into its offset in the frame's ordered source list and
 // writes its slice of the texel map and of the list.  (One CTA per frame would walk 19 rounds serially.)
-__device__ __forceinline__ bool prep_sample(const WinDesc& wd, int idx, unsigned& xi, unsigned& yi) {
-	// nearest-neighbour sample position of quarter-res pixel idx in the full-res maps (resampleFloat4, CUDAImageUtil.cu:82-99)
-	const int x = idx % wd.w, y = idx / wd.w;
-	xi = (unsigned)((float)x * wd.scaleW + 0.5f); yi = (unsigned)((float)y * wd.scaleH + 0.5f);
-	return xi < (unsigned)wd.W && yi < (unsigned)wd.H;
-}
-
 __global__ void __launch_bounds__(1024, 2) k_prep_count(SolveArgs a, int* __restrict__ blk_cnt) {
 	const int fs = blockIdx.y, b = blockIdx.x;
 	if (a.nsrc_cached[fs] || !(a.prm.w_dense > 0.0f)) return;
@@ -409,10 +434,8 @@ __global__ void __launch_bounds__(1024, 2) k_prep_count(SolveArgs a, int* __rest
 	const int npix = wd.w * wd.h, idx = b * 1024 + threadIdx.x;
 	__shared__ int s_w[32];
 	bool valid = false;
-	if (idx < npix) {       // must agree bit for bit with k_prep_frames: z = 0 for a missing / too-near sample
-		unsigned xi, yi;
-		float z = 0.f;
-		if (prep_sample(wd, idx, xi, yi)) { const float d = __ldg(a.depth_ptr[fs] + (size_t)yi * wd.W + xi); if (d >= 0.1f) z = d; }
+	if (idx < npix) {
+		const float z = texel_depth(wd.tg, wd.W, wd.H, wd.w, a.depth_ptr[fs], idx);
 		valid = (z > a.prm.depth_min && z < a.prm.depth_max);
 	}
 	const unsigned bal = __ballot_sync(0xffffffffu, valid);
@@ -445,21 +468,13 @@ __global__ void __launch_bounds__(1024, 2) k_prep_frames(SolveArgs a, WinDesc* w
 			if (lane == 0) s_base = t;
 		}
 		const float dmin = a.prm.depth_min, dmax = a.prm.depth_max;
-		float4* texel = a.texel + (size_t)fs * 2 * a.npix_max;
+		float4* texel = a.texel + (size_t)fs * a.npix_max;
 		float4* src = a.src + (size_t)fs * 2 * a.npix_max;
 		const int idx = b * 1024 + tid;
-		float4 cp = make_float4(0.f, 0.f, 0.f, 0.f), nr = make_float4(0.f, 0.f, 0.f, 0.f);
+		float4 cp, nr;
 		bool valid = false;
 		if (idx < npix) {
-			unsigned xi, yi;
-			if (prep_sample(wd, idx, xi, yi)) {
-				const size_t sidx = (size_t)yi * wd.W + xi;
-				const float d = __ldg(a.depth_ptr[fs] + sidx);
-				nr = __ldg(a.normal_ptr[fs] + sidx);
-				if (d >= 0.1f) cp = make_float4(wd.ifx * ((float)xi * d) + wd.icx * d, wd.ify * ((float)yi * d) + wd.icy * d, d, 1.0f);
-			}
-			texel[2 * idx] = make_float4(cp.x, cp.y, cp.z, nr.x);      // 32-byte texel: point xyz + normal xyz (+ pad)
-			texel[2 * idx + 1] = make_float4(nr.y, nr.z, 0.f, 0.f);
+			texel[idx] = texel_build(wd.tg, wd.W, wd.H, wd.w, a.depth_ptr[fs], a.normal_ptr[fs], idx, cp, nr);
 			valid = (cp.z > dmin && cp.z < dmax);
 		}
 		const unsigned bal = __ballot_sync(0xffffffffu, valid);
@@ -500,34 +515,27 @@ __global__ void __launch_bounds__(1024, 2) k_prep_frames(SolveArgs a, WinDesc* w
 struct CacheStoreArgs {
 	FrameGeom g;
 	const float* const* depth; const float4* const* normal; const int* slots;
-	float4* texel; float4* src; int* nsrc; size_t slot_stride;   // float4 per slot (2 * npix_max)
+	float4* texel; float4* src; int* nsrc; size_t slot_npix;   // quarter-res pixels per slot: texel map slot_npix float4, source list 2 * slot_npix
 	float dmin, dmax;
 };
 __global__ void __launch_bounds__(1024, 2) k_frame_cache_store(CacheStoreArgs c) {
 	__shared__ int s_cnt[kPrepRounds * 32];
 	__shared__ int s_wt[32];
 	const int slot = c.slots[blockIdx.x];
-	const int n = build_frame_maps(c.g, c.depth[blockIdx.x], c.normal[blockIdx.x], c.texel + (size_t)slot * c.slot_stride, c.src + (size_t)slot * c.slot_stride,
+	const int n = build_frame_maps(c.g, c.depth[blockIdx.x], c.normal[blockIdx.x], c.texel + (size_t)slot * c.slot_npix, c.src + (size_t)slot * 2 * c.slot_npix,
 	                               c.dmin, c.dmax, s_cnt, s_wt);
 	if (threadIdx.x == 0) c.nsrc[slot] = n;
 }
 
 // The same store spread over one CTA per 1024 quarter-res pixels (count + build, like k_prep_count / k_prep_frames): a handful of new
 // frames per step - one per tracked window - otherwise runs on a handful of CTAs walking 19 rounds each.
-__device__ __forceinline__ bool geom_sample(const FrameGeom& g, int idx, unsigned& xi, unsigned& yi) {
-	const int x = idx % g.w, y = idx / g.w;
-	xi = (unsigned)((float)x * g.scaleW + 0.5f); yi = (unsigned)((float)y * g.scaleH + 0.5f);
-	return xi < (unsigned)g.W && yi < (unsigned)g.H;
-}
 __global__ void __launch_bounds__(1024, 2) k_cache_count(CacheStoreArgs c, int* __restrict__ blk_cnt) {
 	const int f = blockIdx.y, b = blockIdx.x;
 	const int npix = c.g.w * c.g.h, idx = b * 1024 + threadIdx.x;
 	__shared__ int s_w[32];
 	bool valid = false;
-	if (idx < npix) {       // must agree bit for bit with k_cache_build: z = 0 for a missing / too-near sample
-		unsigned xi, yi;
-		float z = 0.f;
-		if (geom_sample(c.g, idx, xi, yi)) { const float d = __ldg(c.depth[f] + (size_t)yi * c.g.W + xi); if (d >= 0.1f) z = d; }
+	if (idx < npix) {
+		const float z = texel_depth(c.g.tg, c.g.W, c.g.H, c.g.w, c.depth[f], idx);
 		valid = (z > c.dmin && z < c.dmax);
 	}
 	const unsigned bal = __ballot_sync(0xffffffffu, valid);
@@ -555,21 +563,13 @@ __global__ void __launch_bounds__(1024, 2) k_cache_build(CacheStoreArgs c, const
 		for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
 		if (lane == 0) s_base = t;
 	}
-	float4* texel = c.texel + (size_t)slot * c.slot_stride;
-	float4* src = c.src + (size_t)slot * c.slot_stride;
+	float4* texel = c.texel + (size_t)slot * c.slot_npix;
+	float4* src = c.src + (size_t)slot * 2 * c.slot_npix;
 	const int idx = b * 1024 + tid;
-	float4 cp = make_float4(0.f, 0.f, 0.f, 0.f), nr = make_float4(0.f, 0.f, 0.f, 0.f);
+	float4 cp, nr;
 	bool valid = false;
 	if (idx < npix) {
-		unsigned xi, yi;
-		if (geom_sample(c.g, idx, xi, yi)) {
-			const size_t sidx = (size_t)yi * c.g.W + xi;
-			const float d = __ldg(c.depth[f] + sidx);
-			nr = __ldg(c.normal[f] + sidx);
-			if (d >= 0.1f) cp = make_float4(c.g.ifx * ((float)xi * d) + c.g.icx * d, c.g.ify * ((float)yi * d) + c.g.icy * d, d, 1.0f);
-		}
-		texel[2 * idx] = make_float4(cp.x, cp.y, cp.z, nr.x);
-		texel[2 * idx + 1] = make_float4(nr.y, nr.z, 0.f, 0.f);
+		texel[idx] = texel_build(c.g.tg, c.g.W, c.g.H, c.g.w, c.depth[f], c.normal[f], idx, cp, nr);
 		valid = (cp.z > c.dmin && cp.z < c.dmax);
 	}
 	const unsigned bal = __ballot_sync(0xffffffffu, valid);
@@ -740,78 +740,91 @@ __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw) {
 // the model frame with the 6x6 adjoint of T_i.
 struct TileAcc { float v[kTileVals]; };
 
-// Software-pipelined over a thread's pixels (stride kThreads): iteration i issues the source load of pixel i+2 while it
-// evaluates pixel i.
-template <int NT> __device__ __forceinline__ void tile_pixels(const SolveArgs& a, const WinDesc& wd, const float4* __restrict__ src,
-                                            const float4* __restrict__ tex, const float* __restrict__ sM, int start, int count, TileAcc& acc) {
-	const float m00 = sM[0], m01 = sM[1], m02 = sM[2], m03 = sM[3];
-	const float m10 = sM[4], m11 = sM[5], m12 = sM[6], m13 = sM[7];
-	const float m20 = sM[8], m21 = sM[9], m22 = sM[10], m23 = sM[11];
-	const float fx = wd.fx, fy = wd.fy, cx = wd.cx, cy = wd.cy;
-	const unsigned W = (unsigned)wd.w, Hh = (unsigned)wd.h;
+// One pixel between the issue of its loads and its evaluation: the source point mapped into the target camera, the source normal,
+// the projection and the four bilinear taps of the texel map (zeros for a tap outside the map).  in = the pixel projects into the map.
+struct PixTaps { float tx, ty, tz, nx, ny, nz, sx, sy; float4 t00, t01, t10, t11; bool in; };
+
+// Software-pipelined over a thread's pixels (stride NT): iteration k issues the projection and taps of pixel k and the source load
+// of pixel k + 2 NT, then evaluates pixel k.
+// sM: the transform (3 rows of 4); sG: {fx, fy, cx, cy}, {ifx, ify, icx, icy}, {scaleW, scaleH, w, h (int bits)} of the window.
+template <int NT> __device__ __forceinline__ void tile_pixels(const SolveArgs& a, const float4* __restrict__ src, const float4* __restrict__ tex,
+                                            const float* sM, const float* sG, int start, int count, TileAcc& acc) {
 	const float dmin = a.prm.depth_min, dmax = a.prm.depth_max, cos_t = a.prm.dense_cos_normal_thresh;
 	const float delta = a.prm.robust_delta, wdense = a.prm.w_dense;
 	// `sqrtf(d2) <= dist_t` evaluated as `d2 <= d2max`, d2max = the largest float whose correctly rounded square root is <= dist_t
 	// (same truth value for every float, no square root in the loop; found once on the host, make_args)
 	const float d2max = a.d2max;
-	const float4* sp = src + 2 * (size_t)start;
-	int k = threadIdx.x;
-	F8 cc, nn, ff;      // current, next, next-next source records
-	cc.lo = cc.hi = nn.lo = nn.hi = ff.lo = ff.hi = make_float4(0.f, 0.f, 0.f, 0.f);
-	if (k < count) cc = ldg256(sp + 2 * k);
-	if (k + NT < count) nn = ldg256(sp + 2 * (k + NT));
-	for (; k < count; k += NT) {
-		const int k2 = k + 2 * NT;
-		if (k2 < count) ff = ldg256(sp + 2 * k2);
-		const float4 s0 = cc.lo, s1 = cc.hi;
-		cc = nn; nn = ff;
-		const float px = s0.x, py = s0.y, pz = s0.z, nx = s0.w, ny = s1.x, nz = s1.y;
-		// camPosSrcToTgt = transform * camPosSrc ; nrmj = transform(3x3) * n  (w of the normal is 0)
-		const float tx = m00 * px + m01 * py + m02 * pz + m03;
-		const float ty = m10 * px + m11 * py + m12 * pz + m13;
-		const float tz = m20 * px + m21 * py + m22 * pz + m23;
+	auto issue = [&](const F8& s, PixTaps& q) {
+		const float4 M0 = lds128(sM), M1 = lds128(sM + 4), M2 = lds128(sM + 8), K = lds128(sG), Z = lds128(sG + 8);
+		const float m00 = M0.x, m01 = M0.y, m02 = M0.z, m03 = M0.w, m10 = M1.x, m11 = M1.y, m12 = M1.z, m13 = M1.w, m20 = M2.x, m21 = M2.y, m22 = M2.z, m23 = M2.w;
+		const float fx = K.x, fy = K.y, cx = K.z, cy = K.w;
+		const unsigned W = __float_as_uint(Z.z), Hh = __float_as_uint(Z.w);
+		const float px = s.lo.x, py = s.lo.y, pz = s.lo.z;
+		q.nx = s.lo.w; q.ny = s.hi.x; q.nz = s.hi.y;
+		// camPosSrcToTgt = transform * camPosSrc
+		q.tx = m00 * px + m01 * py + m02 * pz + m03;
+		q.ty = m10 * px + m11 * py + m12 * pz + m13;
+		q.tz = m20 * px + m21 * py + m22 * pz + m23;
 		// cameraToDepth, CUDACameraUtil.h:9-14.  One reciprocal serves both quotients (the reference itself is built with
 		// -use_fast_math: its divisions are rcp.approx too; either way the result differs from the exact quotient by an ulp or two)
-		const float itz = rcp_fast(tz);
-		const float sx = (tx * fx) * itz + cx, sy = (ty * fy) * itz + cy;
-		const int ix = (int)roundf(sx), iy = (int)roundf(sy);
-		if (!(ix >= 0 && iy >= 0 && ix < (int)W && iy < (int)Hh)) continue;
-		// bilinearInterpolationFloat4 on camera-space points AND normals (same taps, same weights)
-		const float fx0 = floorf(sx), fy0 = floorf(sy);
+		const float itz = rcp_fast(q.tz);
+		q.sx = (q.tx * fx) * itz + cx; q.sy = (q.ty * fy) * itz + cy;
+		const int ix = (int)roundf(q.sx), iy = (int)roundf(q.sy);
+		q.in = ix >= 0 && iy >= 0 && ix < (int)W && iy < (int)Hh;
+		q.t00 = q.t01 = q.t10 = q.t11 = make_float4(0.f, 0.f, 0.f, 0.f);
+		if (q.in) {
+			const int x0 = (int)floorf(q.sx), y0 = (int)floorf(q.sy);
+			const bool inx0 = (unsigned)x0 < W, inx1 = (unsigned)(x0 + 1) < W;
+			if ((unsigned)y0 < Hh) { const float4* row = tex + (size_t)y0 * W; if (inx0) q.t00 = __ldg(row + x0); if (inx1) q.t01 = __ldg(row + x0 + 1); }
+			if ((unsigned)(y0 + 1) < Hh) { const float4* row = tex + (size_t)(y0 + 1) * W; if (inx0) q.t10 = __ldg(row + x0); if (inx1) q.t11 = __ldg(row + x0 + 1); }
+		}
+	};
+	auto evaluate = [&](const PixTaps& q) {
+		if (!q.in) return;
+		const float4 I = lds128(sG + 4), Z = lds128(sG + 8);
+		TexelGeom tg; tg.ifx = I.x; tg.ify = I.y; tg.icx = I.z; tg.icy = I.w; tg.scaleW = Z.x; tg.scaleH = Z.y;
+		const unsigned W = __float_as_uint(Z.z), Hh = __float_as_uint(Z.w);
+		const float tx = q.tx, ty = q.ty, tz = q.tz;
+		// bilinearInterpolationFloat4 on camera-space points AND normals (same taps, same weights); the tap's point is rebuilt from its
+		// depth at the tap's full-res sample position
+		const float fx0 = floorf(q.sx), fy0 = floorf(q.sy);
 		const int x0 = (int)fx0, y0 = (int)fy0;
-		const float al = sx - fx0, be = sy - fy0;
+		const float al = q.sx - fx0, be = q.sy - fy0;
+		const unsigned xs0 = texel_sample(x0, tg.scaleW), xs1 = texel_sample(x0 + 1, tg.scaleW);
+		const unsigned ys0 = texel_sample(y0, tg.scaleH), ys1 = texel_sample(y0 + 1, tg.scaleH);
 		float a0[3] = { 0.f, 0.f, 0.f }, b0[3] = { 0.f, 0.f, 0.f }, a1[3] = { 0.f, 0.f, 0.f }, b1[3] = { 0.f, 0.f, 0.f };
 		float w0 = 0.f, w1 = 0.f;
+		auto tap = [&](const float4& t, unsigned xs, unsigned ys, float wt, float* ac, float* bc, float& wsum) {
+			ac[0] += wt * texel_coord(xs, t.x, tg.ifx, tg.icx); ac[1] += wt * texel_coord(ys, t.x, tg.ify, tg.icy); ac[2] += wt * t.x;
+			bc[0] += wt * t.y; bc[1] += wt * t.z; bc[2] += wt * t.w; wsum += wt;
+		};
 		const bool inx0 = (unsigned)x0 < W, inx1 = (unsigned)(x0 + 1) < W, iny0 = (unsigned)y0 < Hh, iny1 = (unsigned)(y0 + 1) < Hh;
 		if (iny0) {
-			const float4* row = tex + 2 * ((size_t)y0 * W);
-			if (inx0) { const F8 t8 = ldg256(row + 2 * x0); const float4 cp = t8.lo; const float2 nr = make_float2(t8.hi.x, t8.hi.y); const float wt = 1.0f - al;
-				a0[0] += wt * cp.x; a0[1] += wt * cp.y; a0[2] += wt * cp.z; b0[0] += wt * cp.w; b0[1] += wt * nr.x; b0[2] += wt * nr.y; w0 += wt; }
-			if (inx1) { const F8 t8 = ldg256(row + 2 * (x0 + 1)); const float4 cp = t8.lo; const float2 nr = make_float2(t8.hi.x, t8.hi.y); const float wt = al;
-				a0[0] += wt * cp.x; a0[1] += wt * cp.y; a0[2] += wt * cp.z; b0[0] += wt * cp.w; b0[1] += wt * nr.x; b0[2] += wt * nr.y; w0 += wt; }
+			if (inx0) tap(q.t00, xs0, ys0, 1.0f - al, a0, b0, w0);
+			if (inx1) tap(q.t01, xs1, ys0, al, a0, b0, w0);
 		}
 		if (iny1) {
-			const float4* row = tex + 2 * ((size_t)(y0 + 1) * W);
-			if (inx0) { const F8 t8 = ldg256(row + 2 * x0); const float4 cp = t8.lo; const float2 nr = make_float2(t8.hi.x, t8.hi.y); const float wt = 1.0f - al;
-				a1[0] += wt * cp.x; a1[1] += wt * cp.y; a1[2] += wt * cp.z; b1[0] += wt * cp.w; b1[1] += wt * nr.x; b1[2] += wt * nr.y; w1 += wt; }
-			if (inx1) { const F8 t8 = ldg256(row + 2 * (x0 + 1)); const float4 cp = t8.lo; const float2 nr = make_float2(t8.hi.x, t8.hi.y); const float wt = al;
-				a1[0] += wt * cp.x; a1[1] += wt * cp.y; a1[2] += wt * cp.z; b1[0] += wt * cp.w; b1[1] += wt * nr.x; b1[2] += wt * nr.y; w1 += wt; }
+			if (inx0) tap(q.t10, xs0, ys1, 1.0f - al, a1, b1, w1);
+			if (inx1) tap(q.t11, xs1, ys1, al, a1, b1, w1);
 		}
 		float ww = 0.f, cxs = 0.f, cys = 0.f, czs = 0.f, nxs = 0.f, nys = 0.f, nzs = 0.f;
 		if (w0 > 0.f) { const float r = (1.0f - be) * rcp_fast(w0); cxs += r * a0[0]; cys += r * a0[1]; czs += r * a0[2]; nxs += r * b0[0]; nys += r * b0[1]; nzs += r * b0[2]; ww += (1.0f - be); }
 		if (w1 > 0.f) { const float r = be * rcp_fast(w1); cxs += r * a1[0]; cys += r * a1[1]; czs += r * a1[2]; nxs += r * b1[0]; nys += r * b1[1]; nzs += r * b1[2]; ww += be; }
-		if (!(ww > 0.f)) continue;
+		if (!(ww > 0.f)) return;
 		const float rw = rcp_fast(ww);
 		const float qx = cxs * rw, qy = cys * rw, qz = czs * rw;        // camPosTgt
-		if (!(qz > dmin && qz < dmax)) continue;
+		if (!(qz > dmin && qz < dmax)) return;
 		const float tnx = nxs * rw, tny = nys * rw, tnz = nzs * rw;     // normalTgt
-		const float rnx = m00 * nx + m01 * ny + m02 * nz;
-		const float rny = m10 * nx + m11 * ny + m12 * nz;
-		const float rnz = m20 * nx + m21 * ny + m22 * nz;
+		// nrmj = transform(3x3) * n  (w of the normal is 0)
+		const float4 M0 = lds128(sM), M1 = lds128(sM + 4), M2 = lds128(sM + 8);
+		const float m00 = M0.x, m01 = M0.y, m02 = M0.z, m10 = M1.x, m11 = M1.y, m12 = M1.z, m20 = M2.x, m21 = M2.y, m22 = M2.z;
+		const float rnx = m00 * q.nx + m01 * q.ny + m02 * q.nz;
+		const float rny = m10 * q.nx + m11 * q.ny + m12 * q.nz;
+		const float rnz = m20 * q.nx + m21 * q.ny + m22 * q.nz;
 		const float dx = tx - qx, dy = ty - qy, dz = tz - qz;
 		const float dist2 = dx * dx + dy * dy + dz * dz;
 		const float dn = rnx * tnx + rny * tny + rnz * tnz;
-		if (!(dn >= cos_t && dist2 <= d2max)) continue;
+		if (!(dn >= cos_t && dist2 <= d2max)) return;
 		const float res = -(dx * tnx + dy * tny + dz * tnz);            // dot(camPosTgt - camPosSrcToTgt, normalTgt)
 		const float wgt = wdense * huber_w_fast(res * res, delta);
 		float g[6];
@@ -827,6 +840,19 @@ template <int NT> __device__ __forceinline__ void tile_pixels(const SolveArgs& a
 #pragma unroll
 		for (int r = 0; r < 6; r++) acc.v[21 + r] += wgt * g[r] * res;
 		acc.v[27] += 1.0f;
+	};
+	const float4* sp = src + 2 * (size_t)start;
+	int k = threadIdx.x;
+	F8 c0, c1;      // source records of pixels k and k + NT
+	c0.lo = c0.hi = c1.lo = c1.hi = make_float4(0.f, 0.f, 0.f, 0.f);
+	if (k < count) c0 = ldg256(sp + 2 * k);
+	if (k + NT < count) c1 = ldg256(sp + 2 * (k + NT));
+	for (; k < count; k += NT) {
+		PixTaps q;
+		issue(c0, q);
+		c0 = c1;
+		if (k + 2 * NT < count) c1 = ldg256(sp + 2 * (k + 2 * NT));
+		evaluate(q);
 	}
 }
 
@@ -1330,11 +1356,25 @@ template <int NT> __device__ void window_tail(const SolveArgs& a, const WinDesc&
 }
 
 // ------------------------------------------------------------------------------------------------ k_solve
+// One step of the tile's transposing butterfly, then the next (HALF = 16, 8, ..., 1): the lanes with bit HALF set keep the upper half
+// of v and send the lower one, the others the reverse.  A template parameter, so every index into v is a compile-time constant and
+// v stays in registers.
+template <int HALF> __device__ __forceinline__ void butterfly_step(float (&v)[32], int lane) {
+	const bool up = (lane & HALF) != 0;
+#pragma unroll
+	for (int k = 0; k < HALF; k++) {
+		const float send = up ? v[k] : v[k + HALF];
+		const float keep = up ? v[k + HALF] : v[k];
+		v[k] = keep + __shfl_xor_sync(0xffffffffu, send, HALF);
+	}
+	if constexpr (HALF > 1) butterfly_step<HALF / 2>(v, lane);
+}
 template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(SolveArgs a) {
 	extern __shared__ __align__(16) float dyn_smem[];
 	__shared__ int s_tile, s_it, s_idx;
 	__shared__ Tile s_tl[2];      // the tile being processed and the one claimed for the next round (thread 0 fetches its record a tile ahead)
-	__shared__ float s_M[12];
+	__shared__ __align__(16) float s_M[12];
+	__shared__ __align__(16) float s_G[12];
 	__shared__ float s_X[36];
 	__shared__ float s_red[kTileVals];
 	__shared__ float s_part[(NT / 32)][kTileVals];
@@ -1409,10 +1449,14 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 				else if (c >= 3) v = __ldcg(Ti + (r - 3) * 4 + (c - 3));
 				else { const float t3[3] = { __ldcg(Ti + 3), __ldcg(Ti + 7), __ldcg(Ti + 11) }; v = 0.f; for (int kk = 0; kk < 3; kk++) v += skew(t3, r - 3, kk) * __ldcg(Ti + kk * 4 + c); }
 				s_X[e] = v;
+			} else if (tid == 96) {   // the window's projection / texel geometry, read by the pixel loop where it is used
+				s_G[0] = wd.fx; s_G[1] = wd.fy; s_G[2] = wd.cx; s_G[3] = wd.cy;
+				s_G[4] = wd.tg.ifx; s_G[5] = wd.tg.ify; s_G[6] = wd.tg.icx; s_G[7] = wd.tg.icy;
+				s_G[8] = wd.tg.scaleW; s_G[9] = wd.tg.scaleH; s_G[10] = __int_as_float(wd.w); s_G[11] = __int_as_float(wd.h);
 			}
 			__syncthreads();
 			PROF_T(2);
-			tile_pixels<NT>(a, wd, tl.src, tl.tex, s_M, tl.start, tl.count, acc);
+			tile_pixels<NT>(a, tl.src, tl.tex, s_M, s_G, tl.start, tl.count, acc);
 		}
 		PROF_T(3);
 		int itn = 0, idxn = 0;
@@ -1423,16 +1467,7 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 			float v[32];
 #pragma unroll
 			for (int k = 0; k < 32; k++) v[k] = (k < kTileVals) ? acc.v[k] : 0.f;
-#pragma unroll
-			for (int half = 16; half >= 1; half >>= 1) {
-				const bool up = (lane & half) != 0;
-#pragma unroll
-				for (int k = 0; k < half; k++) {
-					const float send = up ? v[k] : v[k + half];
-					const float keep = up ? v[k + half] : v[k];
-					v[k] = keep + __shfl_xor_sync(0xffffffffu, send, half);
-				}
-			}
+			butterfly_step<16>(v, lane);
 			if (lane < kTileVals) s_part[wid][lane] = v[0];
 		}
 		__syncthreads();
@@ -1593,7 +1628,7 @@ static int reserve_impl(bt_ctx* ctx, const bt_solver_limits* lim) {
 		const StageLayout L = stage_layout(lim->max_windows, (size_t)F, (size_t)lim->max_corr * lim->max_windows, lim->max_frames, (size_t)s->max_groups, (size_t)s->max_pairs);
 		RES(stage_buf[0], L.total); RES(stage_buf[1], L.total);
 	}
-	RES(texel, sizeof(float4) * 2 * (size_t)s->npix_max * F);
+	RES(texel, sizeof(float4) * (size_t)s->npix_max * F);
 	RES(src, sizeof(float4) * 2 * (size_t)s->npix_max * F);
 	RES(nsrc, sizeof(int) * F);
 	RES(grp_sums, sizeof(float) * kGrpVals * (size_t)s->max_groups * lim->max_windows);
@@ -1717,8 +1752,8 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 		d.w = (int)(bw.W / params->image_downscale); d.h = (int)(bw.H / params->image_downscale);   // LossGPU.cu:56-57
 		d.fx = bw.fx * ((float)d.w / (float)bw.W); d.fy = bw.fy * ((float)d.h / (float)bw.H);         // CUDACache.cpp:20-24
 		d.cx = bw.cx * ((float)(d.w - 1) / (float)(bw.W - 1)); d.cy = bw.cy * ((float)(d.h - 1) / (float)(bw.H - 1));
-		d.ifx = 1.0f / bw.fx; d.ify = 1.0f / bw.fy; d.icx = -bw.cx / bw.fx; d.icy = -bw.cy / bw.fy;
-		d.scaleW = (float)(bw.W - 1) / (float)(d.w - 1); d.scaleH = (float)(bw.H - 1) / (float)(d.h - 1);
+		d.tg.ifx = 1.0f / bw.fx; d.tg.ify = 1.0f / bw.fy; d.tg.icx = -bw.cx / bw.fx; d.tg.icy = -bw.cy / bw.fy;
+		d.tg.scaleW = (float)(bw.W - 1) / (float)(d.w - 1); d.tg.scaleH = (float)(bw.H - 1) / (float)(d.h - 1);
 		d.compat_flip = bw.compat_flip;
 		d.frame_off = (int)f_off; d.pair_off = (int)p_off;
 		s->frame_off[w] = (int)f_off; s->n_frames[w] = N;
@@ -1732,12 +1767,12 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 				               && s->c_downscale == params->image_downscale,
 				           BT_ERR_INVALID_ARG, "window %d frame %d: cache slot %d was stored with another image size, K, depth range or downscale", w, f, cs);
 				hdp[fs] = nullptr; hnp[fs] = nullptr;
-				htex[fs] = s->c_texel.as<float4>() + (size_t)cs * 2 * s->c_npix; hsrc[fs] = s->c_src.as<float4>() + (size_t)cs * 2 * s->c_npix;
+				htex[fs] = s->c_texel.as<float4>() + (size_t)cs * s->c_npix; hsrc[fs] = s->c_src.as<float4>() + (size_t)cs * 2 * s->c_npix;
 				hnsrc[fs] = s->c_nsrc.as<int>() + cs;
 			} else {
 				hdp[fs] = (params->w_dense > 0.f) ? bw.depth_dev[f] : nullptr;
 				hnp[fs] = (params->w_dense > 0.f) ? bw.normal_dev[f] : nullptr;
-				htex[fs] = s->texel.as<float4>() + fs * 2 * (size_t)s->npix_max; hsrc[fs] = s->src.as<float4>() + fs * 2 * (size_t)s->npix_max;
+				htex[fs] = s->texel.as<float4>() + fs * (size_t)s->npix_max; hsrc[fs] = s->src.as<float4>() + fs * 2 * (size_t)s->npix_max;
 				hnsrc[fs] = nullptr;
 				if (params->w_dense > 0.f) s->any_uncached = true;
 			}
@@ -2149,7 +2184,7 @@ extern "C" int bt_frame_cache_reserve(bt_ctx* ctx, int capacity, int H, int W, f
 	const int w = (int)(W / image_downscale), h = (int)(H / image_downscale);
 	BT_REQUIRE(w >= 2 && h >= 2, BT_ERR_INVALID_ARG, "bt_frame_cache_reserve: image too small");
 	int rc;
-	if ((rc = s->c_texel.alloc(sizeof(float4) * 2 * (size_t)w * h * capacity)) != BT_OK) return rc;
+	if ((rc = s->c_texel.alloc(sizeof(float4) * (size_t)w * h * capacity)) != BT_OK) return rc;
 	if ((rc = s->c_src.alloc(sizeof(float4) * 2 * (size_t)w * h * capacity)) != BT_OK) return rc;
 	if ((rc = s->c_nsrc.alloc(sizeof(int) * (size_t)capacity)) != BT_OK) return rc;
 	if ((rc = s->c_blk.alloc(sizeof(int) * (size_t)capacity * ((w * h + 1023) / 1024))) != BT_OK) return rc;
@@ -2187,11 +2222,11 @@ extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* sl
 	BT_CUDA(cudaEventRecord(s->c_ev[fl], stream));
 	CacheStoreArgs c;
 	c.g.W = W; c.g.H = H; c.g.w = w; c.g.h = h;                                                   // same expressions as bt_solve_stage (CUDACache.cpp:20-24)
-	c.g.ifx = 1.0f / fx; c.g.ify = 1.0f / fy; c.g.icx = -cx / fx; c.g.icy = -cy / fy;
-	c.g.scaleW = (float)(W - 1) / (float)(w - 1); c.g.scaleH = (float)(H - 1) / (float)(h - 1);
+	c.g.tg.ifx = 1.0f / fx; c.g.tg.ify = 1.0f / fy; c.g.tg.icx = -cx / fx; c.g.tg.icy = -cy / fy;
+	c.g.tg.scaleW = (float)(W - 1) / (float)(w - 1); c.g.tg.scaleH = (float)(H - 1) / (float)(h - 1);
 	char* db = s->c_tables.as<char>();
 	c.depth = (const float* const*)db; c.normal = (const float4* const*)(db + b_ptr); c.slots = (const int*)(db + 2 * b_ptr);
-	c.texel = s->c_texel.as<float4>(); c.src = s->c_src.as<float4>(); c.nsrc = s->c_nsrc.as<int>(); c.slot_stride = 2 * (size_t)s->c_npix;
+	c.texel = s->c_texel.as<float4>(); c.src = s->c_src.as<float4>(); c.nsrc = s->c_nsrc.as<int>(); c.slot_npix = (size_t)s->c_npix;
 	c.dmin = depth_min; c.dmax = depth_max;
 	if (n_frames >= 2 * ctx->sm_count) k_frame_cache_store<<<n_frames, 1024, 0, stream>>>(c);      // many frames: one CTA per frame fills the machine
 	else {
