@@ -63,3 +63,13 @@ def depth_params(yml: Union[None, str, Mapping[str, Any]] = None):
     dp = y.get("depth_processing", NOCS_DEFAULTS["depth_processing"])
     e, b = dp["erode"], dp["bilateral_filter"]
     return DepthParams(int(e["radius"]), float(e["diff"]), float(e["ratio"]), int(b["radius"]), float(b["sigma_D"]), float(b["sigma_R"]))
+
+
+def mask_mode(yml: Union[None, str, Mapping[str, Any]] = None) -> int:
+    """config "data_dir" -> bt_frames_preprocess_masked's mask_mode.  The reference keeps only the convex hull of the mask's largest
+    component when data_dir contains "NOCS" and uses the mask as it is otherwise (Frame.cpp:251,267).  Without a yml: the NOCS
+    defaults, i.e. largest-hull mode."""
+    from ._lib import BT_MASK_AS_IS, BT_MASK_LARGEST_HULL
+    if yml is None:
+        return BT_MASK_LARGEST_HULL
+    return BT_MASK_LARGEST_HULL if "NOCS" in str(load_yml(yml).get("data_dir", "")) else BT_MASK_AS_IS

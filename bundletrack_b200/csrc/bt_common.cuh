@@ -84,4 +84,9 @@ void ransac_destroy(bt_ctx* ctx);
 void prune_destroy(bt_ctx* ctx);
 void mcache_destroy(bt_ctx* ctx);
 void front_destroy(bt_ctx* ctx);
+// segment.cu: largest-hull mode for the masked front end, and the LF-Net request
+size_t hull_fill_smem(int H);
+int segment_largest_hull(const uint8_t* const* mask_tbl_dev, int n, int H, int W, int32_t* label, int32_t* count, unsigned long long* best,
+                         uint8_t* fill, cudaStream_t stream);
+int launch_lfnet_request(const void* const* tbl_dev, const int32_t* roi_dev, int n, int H, int W, cudaStream_t stream);
 }

@@ -222,6 +222,33 @@ inline void processDepthAndNormals(bt_ctx* ctx, const float* depth_raw_gpu, floa
 		throw std::runtime_error(std::string("bt_frames_preprocess: ") + bt_last_error());
 }
 
+// ---- Frame::segmentationByMaskFile + invalidatePixelsByMask (Frame.cpp:236-374) on top of the front end -----------------------------
+// mask_gpu: the mask PNG's bytes (device uint8 H*W); mode: BT_MASK_LARGEST_HULL when data_dir contains "NOCS", else BT_MASK_AS_IS.
+// Writes the masked maps, fg_gpu (= Frame::_fg_mask, device uint8 H*W, not mask_gpu) and roi_gpu (device int32[4], kept for
+// lfnetRequest), then reads the ROI back into roi (Vector4-like: roi(0..3) = umin, umax, vmin, vmax; waits for the stream).
+template <class Float4T, class Mat3, class Vec4>
+inline void processDepthNormalsAndMask(bt_ctx* ctx, const float* depth_raw_gpu, const uint8_t* mask_gpu, int mode, float* depth_gpu, Float4T* normal_gpu,
+                                       Float4T* xyz_gpu, uint8_t* fg_gpu, int32_t* roi_gpu, int H, int W, const Mat3& K, const BtDepthConfig& cfg, Vec4& roi,
+                                       void* stream = nullptr) {
+	const bt_depth_params prm = cfg.to_params();
+	const float* in[1] = { depth_raw_gpu }; float* out[1] = { depth_gpu };
+	float* nrm[1] = { reinterpret_cast<float*>(normal_gpu) }; float* xyz[1] = { reinterpret_cast<float*>(xyz_gpu) };
+	const uint8_t* msk[1] = { mask_gpu }; uint8_t* fg[1] = { fg_gpu };
+	if (bt_frames_preprocess_masked(ctx, 1, in, msk, mode, H, W, K(0, 0), K(1, 1), K(0, 2), K(1, 2), &prm, out, xyz_gpu ? xyz : nullptr, nrm, fg, roi_gpu, stream) != BT_OK)
+		throw std::runtime_error(std::string("bt_frames_preprocess_masked: ") + bt_last_error());
+	int32_t r[4];
+	if (bt_memcpy_d2h(r, roi_gpu, sizeof r, stream) != BT_OK) throw std::runtime_error(std::string("bt_memcpy_d2h: ") + bt_last_error());
+	for (int i = 0; i < 4; i++) roi(i) = r[i];
+}
+// Lfnet::detectFeature's request image (FeatureManager.cpp:813-858, rot_deg = 0) from processDepthNormalsAndMask's fg / roi:
+// request_gpu (device uint8 400*400*3) receives the BGR bytes of the second message part; untouched when the ROI fails the gate.
+inline void lfnetRequest(bt_ctx* ctx, const uint8_t* color_gpu, const uint8_t* fg_gpu, const int32_t* roi_gpu, int H, int W, uint8_t* request_gpu,
+                         void* stream = nullptr) {
+	const uint8_t* col[1] = { color_gpu }; const uint8_t* fg[1] = { fg_gpu }; uint8_t* out[1] = { request_gpu };
+	if (bt_lfnet_request(ctx, 1, col, fg, roi_gpu, H, W, out, stream) != BT_OK)
+		throw std::runtime_error(std::string("bt_lfnet_request: ") + bt_last_error());
+}
+
 // ---- the two knnMatch calls of SiftManager::findCorresbyNN (/root/reference/src/FeatureManager.cpp:271-273) in one call --------
 // desA/desB: device CV_32F descriptor matrices (GpuMat::data, rows, step).  DMatchT needs queryIdx, trainIdx, distance (cv::DMatch).
 // The device result buffers belong to the object (sized once for max_feats x k), nothing is allocated per call.

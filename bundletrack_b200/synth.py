@@ -308,6 +308,29 @@ def make_raw_depth(seed: int, H: int = 480, W: int = 640, K=None, noise: float =
     return raw.astype(np.float32), K
 
 
+def make_object_mask(seed: int, H: int = 480, W: int = 640, n_distractors: int = 3, speckle_frac: float = 0.002, n_holes: int = 4,
+                     value: int = 255) -> np.ndarray:
+    """An object mask as the reference reads it from a mask PNG (uint8 H x W, non-zero = object): a rotated elliptic main blob, smaller
+    disc-shaped distractor blobs, isolated speckle pixels and a few holes punched into the main blob.  Pure numpy (no OpenCV), so the
+    segmentation tests and benchmarks can make their inputs anywhere.  value: the foreground byte (any non-zero value)."""
+    rng = np.random.default_rng(np.uint64(0x5E6) + np.uint64(seed))
+    y, x = np.mgrid[0:H, 0:W].astype(np.float64)
+    m = np.zeros((H, W), bool)
+    cx, cy = rng.uniform(0.3, 0.7) * W, rng.uniform(0.3, 0.7) * H
+    a, b = rng.uniform(0.12, 0.3) * W, rng.uniform(0.12, 0.3) * H
+    th = rng.uniform(0, np.pi)
+    u, v = (x - cx) * np.cos(th) + (y - cy) * np.sin(th), -(x - cx) * np.sin(th) + (y - cy) * np.cos(th)
+    m |= (u / max(a, 0.5)) ** 2 + (v / max(b, 0.5)) ** 2 <= 1.0
+    for _ in range(n_holes):
+        hx, hy = cx + rng.uniform(-0.5, 0.5) * a, cy + rng.uniform(-0.5, 0.5) * b
+        m &= (x - hx) ** 2 + (y - hy) ** 2 > rng.uniform(1.0, 0.15 * min(a, b) + 1.5) ** 2
+    for _ in range(n_distractors):
+        r = rng.uniform(0.02, 0.06) * min(H, W) + 0.5
+        m |= (x - rng.uniform(0, W)) ** 2 + (y - rng.uniform(0, H)) ** 2 <= r * r
+    m |= rng.random((H, W)) < speckle_frac
+    return (m * np.uint8(value)).astype(np.uint8)
+
+
 def make_ransac_case(seed: int, n: int, inlier_frac: float = 0.7, noise: float = 0.0005):
     """Model-frame point pairs as SiftManager::runRansacMultiPairGPU uploads them (/root/reference/src/FeatureManager.cpp:676-706):
     B = T A + noise for the inliers, the rest displaced by centimetres.  Returns (A [n,4], B [n,4] float32 with w = 1, inlier mask)."""

@@ -326,6 +326,29 @@ BT_API int bt_frames_preprocess(bt_ctx* ctx, int n_frames, const float* const* d
                          float fx, float fy, float cx, float cy, const bt_depth_params* prm,
                          float* const* depth_out_dev, float* const* xyz_out_dev, float* const* normal_out_dev, void* stream);
 
+/* ---- object mask: Frame::segmentationByMaskFile + Frame::invalidatePixelsByMask (reference src/Frame.cpp:267-374) -----------
+ * mask_dev: DEVICE uint8 H*W per frame as cv::imread(IMREAD_UNCHANGED) returns the mask PNG, non-zero = object.
+ * BT_MASK_LARGEST_HULL (the reference's NOCS datasets): the largest 8-connected component of mask != 0 (ties: the component whose
+ * first pixel in row-major order comes first), replaced by cv::fillConvexPoly of its convex hull (0/1); an empty mask stays empty.
+ * BT_MASK_AS_IS (every other dataset): the mask as given.  Then fg = cv::dilate(mask, 5 x 5 rectangle) = Frame::_fg_mask, written to
+ * fg_out_dev (DEVICE uint8 H*W per frame; must not alias mask_dev), and roi_out_dev (DEVICE int32 [n_frames][4]) = Frame::_roi =
+ * (umin, umax, vmin, vmax) of fg != 0, (9999, 0, 9999, 0) when fg is empty.  The maps are exactly bt_frames_preprocess's with depth,
+ * xyz and normal zeroed where fg == 0 (computed from the unmasked depth first, as in the reference).  Asynchronous like
+ * bt_frames_preprocess: the ROI stays on the device for bt_lfnet_request; read it back when the tracker's gate needs it
+ * (umax - umin < 10 || vmax - vmin < 10 -> Frame::FAIL, Bundler.cpp:88-93).  Largest-hull mode keeps label scratch in the context,
+ * grown on the first call at a size. */
+enum { BT_MASK_AS_IS = 0, BT_MASK_LARGEST_HULL = 1 };
+BT_API int bt_frames_preprocess_masked(bt_ctx* ctx, int n_frames, const float* const* depth_raw_dev, const uint8_t* const* mask_dev, int mask_mode,
+                         int H, int W, float fx, float fy, float cx, float cy, const bt_depth_params* prm, float* const* depth_out_dev,
+                         float* const* xyz_out_dev, float* const* normal_out_dev, uint8_t* const* fg_out_dev, int32_t* roi_out_dev, void* stream);
+/* Lfnet::detectFeature's request image (src/FeatureManager.cpp:813-873, rot_deg = 0): the colour zeroed where fg == 0, cropped to
+ * [vmin, vmax) x [umin, umax) of roi_dev (the reference's crop drops the last row and column), padded with zeros to a square and
+ * resized to 400 x 400 as cv::resize(INTER_LINEAR) does on 8-bit images.  colour_dev: DEVICE uint8 H*W*3 BGR (cv::Mat CV_8UC3 data);
+ * fg_dev / roi_dev: bt_frames_preprocess_masked's outputs; request_out_dev: DEVICE uint8 400*400*3 per frame, the bytes of the second
+ * message part of the request.  Frames whose roi fails the tracker's 10-pixel gate are left untouched.  Asynchronous. */
+BT_API int bt_lfnet_request(bt_ctx* ctx, int n_frames, const uint8_t* const* colour_dev, const uint8_t* const* fg_dev, const int32_t* roi_dev,
+                         int H, int W, uint8_t* const* request_out_dev, void* stream);
+
 /* Frame cache (SURVEY.md 8f rank 1, second half).  The reference re-creates a CUDACache and re-downsamples every keyframe of
  * the window in EVERY optimizeFrames call (/root/reference/src/cuda/LossGPU.cu:74-101, CUDACache.cpp:76-88); a keyframe
  * takes part in many windows, so its quarter-resolution point/normal texel map and compacted source list are built here
