@@ -49,6 +49,7 @@ extern "C" void bt_ctx_destroy(bt_ctx* ctx) {
 	bt::ransac_destroy(ctx);
 	bt::prune_destroy(ctx);
 	bt::mcache_destroy(ctx);
+	bt::tracks_dev_destroy(ctx);
 	bt::front_destroy(ctx);
 	delete ctx;
 }

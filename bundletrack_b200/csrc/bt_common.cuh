@@ -62,6 +62,7 @@ struct RansacState;   // ransac.cu
 struct FrontState;    // frontend.cu
 struct PruneState;    // prune.cu
 struct MatchCache;    // prune.cu
+struct TracksDev;     // tracks_dev.cu
 
 }  // namespace bt
 
@@ -75,6 +76,7 @@ struct bt_ctx {
 	bt::FrontState* front = nullptr;
 	bt::PruneState* prune = nullptr;
 	bt::MatchCache* mcache = nullptr;
+	bt::TracksDev* tracks = nullptr;
 };
 
 namespace bt {
@@ -89,4 +91,15 @@ size_t hull_fill_smem(int H);
 int segment_largest_hull(const uint8_t* const* mask_tbl_dev, int n, int H, int W, int32_t* label, int32_t* count, unsigned long long* best,
                          uint8_t* fill, cudaStream_t stream);
 int launch_lfnet_request(const void* const* tbl_dev, const int32_t* roi_dev, int n, int H, int W, cudaStream_t stream);
+// tracks_dev.cu: the device map-point table, driven pair by pair from bt_find_corres_pairs (prune.cu).  Frames are named by slot;
+// tracks_slot maps a frame id to its slot (-1: the frame has no map yet, unless create is set).
+void tracks_dev_destroy(bt_ctx* ctx);
+int tracks_slot(bt_ctx* ctx, int frame_id, bool create, int* slot);
+int tracks_free_slots(bt_ctx* ctx);
+// where an update takes its (uA, vA, uB, vB) list from: entry i = base + stride * (ids ? ids[i] : i) floats.  The count is *n_dev, or, when
+// n_inl is set, pair `pair`'s emitted count (n_inl[pair] < 5 -> 0, clamped to `capacity` behind the earlier pairs) as k_emit_entryj writes it.
+struct TrkSrc { const float* base; int stride; const int32_t* ids; const int32_t* n_dev; int max_n; const int32_t* n_inl; int pair; int capacity; };
+int tracks_launch_update(bt_ctx* ctx, int slot_a, int slot_b, const TrkSrc& src, cudaStream_t stream);
+int tracks_launch_propagate(bt_ctx* ctx, int slot_a, int slot_b, const float4* existing, int n_existing, float4* out, int capacity, int32_t* n_out,
+                            cudaStream_t stream);
 }

@@ -15,6 +15,7 @@
 //                    (Bundler::optimizeGPU, /root/reference/src/Bundler.cpp:308-317), < 5 inliers => pair dropped
 //                    (FeatureManager.cpp:233-241,727-730); pairs written back to back, which is the grouping the
 //                    solver's tail wants.
+#include <algorithm>
 #include <map>
 #include <vector>
 #include "bt_common.cuh"
@@ -115,7 +116,7 @@ __global__ void __launch_bounds__(512) k_prune_mutual(const PrunePair* __restric
 // are appended in order with the organised-cloud points at round(u), round(v) (zeros where the depth is < 0.1, as the cloud holds them).
 __global__ void __launch_bounds__(256) k_append_propagated(const PrunePair* __restrict__ pairs, PruneCam cam, const float4* __restrict__ extra_uv,
                                                             bt_correspondence* __restrict__ corr, float4* __restrict__ PA, float4* __restrict__ PB,
-                                                            int32_t* __restrict__ n_corr, int32_t* __restrict__ n_nn) {
+                                                            int32_t* __restrict__ n_corr, int32_t* __restrict__ n_nn, const int32_t* __restrict__ n_extra_dev) {
 	__shared__ int s_warp[8];
 	__shared__ int s_base;
 	const PrunePair pp = pairs[blockIdx.x];
@@ -123,13 +124,14 @@ __global__ void __launch_bounds__(256) k_append_propagated(const PrunePair* __re
 	const int n0 = n_corr[blockIdx.x];
 	if (tid == 0) { n_nn[blockIdx.x] = n0; s_base = n0; }
 	__syncthreads();
-	if (pp.n_extra <= 0 || abs(pp.A.frame_id - pp.B.frame_id) == 1) return;
+	const int n_extra = n_extra_dev ? n_extra_dev[blockIdx.x] : pp.n_extra;      // (bt_find_corres_pairs: the count the device table wrote)
+	if (n_extra <= 0 || abs(pp.A.frame_id - pp.B.frame_id) == 1) return;
 	const bt_correspondence* ex = corr + pp.out_off;
-	for (int base = 0; base < pp.n_extra; base += blockDim.x) {
+	for (int base = 0; base < n_extra; base += blockDim.x) {
 		const int e = base + tid;
 		bool keep = false;
 		float4 uv = make_float4(0.f, 0.f, 0.f, 0.f);
-		if (e < pp.n_extra) {
+		if (e < n_extra) {
 			uv = __ldg(extra_uv + pp.extra_off + e);
 			keep = true;
 			for (int i = 0; i < n0; i++) {      // only the matches of the two knnMatch directions are compared: map-point keys are unique per frame
@@ -231,7 +233,7 @@ __global__ void __launch_bounds__(256) k_emit_fill(const PrunePair* __restrict__
 
 struct PruneState {
 	int max_pairs = 0, max_feats = 0;
-	DevBuf pairs, corr, PA, PB, n_corr, n_nn, rpairs, inl, n_inl, idxAB, distAB, idxBA, distBA, entry_off, total, extra;
+	DevBuf pairs, corr, PA, PB, n_corr, n_nn, rpairs, inl, n_inl, idxAB, distAB, idxBA, distBA, entry_off, total, extra, n_prop;
 	PinnedBuf h_pairs, h_extra;
 	size_t extra_cap = 0;               // propagated matches (float4 each) one call may carry
 	cudaEvent_t ev_up = nullptr;      // recorded behind the upload of h_pairs (the calls are asynchronous: see fill_pairs)
@@ -248,7 +250,7 @@ static PruneState* g_prune_of(bt_ctx* ctx) { return ctx->prune; }
 void prune_destroy(bt_ctx* ctx) {
 	PruneState* s = ctx->prune;
 	if (!s) return;
-	DevBuf* bufs[] = { &s->pairs, &s->corr, &s->PA, &s->PB, &s->n_corr, &s->n_nn, &s->extra, &s->rpairs, &s->inl, &s->n_inl, &s->idxAB, &s->distAB, &s->idxBA, &s->distBA, &s->entry_off, &s->total };
+	DevBuf* bufs[] = { &s->pairs, &s->corr, &s->PA, &s->PB, &s->n_corr, &s->n_nn, &s->extra, &s->rpairs, &s->inl, &s->n_inl, &s->idxAB, &s->distAB, &s->idxBA, &s->distBA, &s->entry_off, &s->total, &s->n_prop };
 	for (DevBuf* b : bufs) b->release();
 	s->h_pairs.release(); s->h_extra.release();
 	if (s->ev_up) cudaEventDestroy(s->ev_up);
@@ -278,13 +280,16 @@ extern "C" int bt_pipeline_reserve(bt_ctx* ctx, int max_pairs, int max_feats, in
 	RES(inl, sizeof(int32_t) * cap); RES(n_inl, sizeof(int32_t) * max_pairs);
 	RES(idxAB, sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs); RES(distAB, sizeof(float) * 8 * (size_t)max_feats * max_pairs);
 	RES(idxBA, sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs); RES(distBA, sizeof(float) * 8 * (size_t)max_feats * max_pairs);
-	RES(entry_off, sizeof(int32_t) * max_pairs); RES(total, 16);
+	RES(entry_off, sizeof(int32_t) * max_pairs); RES(total, 16); RES(n_prop, sizeof(int32_t) * max_pairs);
 #undef RES
 	if ((rc = s->h_extra.alloc(sizeof(float4) * s->extra_cap)) != BT_OK) return rc;
 	return s->h_pairs.alloc(sizeof(PrunePair) * max_pairs);
 }
 
-static int fill_pairs(PruneState* s, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, cudaStream_t stream, const bt_match_extra* extra = nullptr) {
+// prop_room > 0 (bt_find_corres_pairs): no host extras; pair p keeps room for prop_room propagated matches behind its mutual ones, and its
+// candidates go to extra[p * prop_room, ...) when the device table writes them
+static int fill_pairs(PruneState* s, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, cudaStream_t stream, const bt_match_extra* extra = nullptr,
+                      int prop_room = 0) {
 	// an earlier asynchronous call's upload may still be reading the pinned table: wait for it before rewriting the block
 	if (!s->ev_up) BT_CUDA(cudaEventCreateWithFlags(&s->ev_up, cudaEventDisableTiming));
 	else BT_CUDA(cudaEventSynchronize(s->ev_up));
@@ -306,10 +311,10 @@ static int fill_pairs(PruneState* s, int n_pairs, const bt_match_frame* A, const
 		const int nx = (extra && extra[p].n > 0 && abs(A[p].frame_id - B[p].frame_id) != 1) ? extra[p].n : 0;
 		BT_REQUIRE(nx == 0 || extra[p].uv, BT_ERR_INVALID_ARG, "pair %d: NULL propagated-match array", p);
 		BT_REQUIRE(nx <= s->max_feats && (size_t)(xoff + nx) <= s->extra_cap, BT_ERR_CAPACITY, "pair %d: %d propagated matches exceed the reserved room", p, nx);
-		hp[p].n_extra = nx; hp[p].extra_off = xoff;
+		hp[p].n_extra = nx; hp[p].extra_off = prop_room ? p * prop_room : xoff;
 		if (nx) memcpy(hx + xoff, extra[p].uv, sizeof(float4) * (size_t)nx);
 		xoff += nx;
-		offA += A[p].n; offB += B[p].n; out += A[p].n + B[p].n + nx;
+		offA += A[p].n; offB += B[p].n; out += A[p].n + B[p].n + nx + prop_room;
 	}
 	if (xoff) BT_CUDA(cudaMemcpyAsync(s->extra.p, hx, sizeof(float4) * (size_t)xoff, cudaMemcpyHostToDevice, stream));
 	BT_CUDA(cudaMemcpyAsync(s->pairs.p, hp, sizeof(PrunePair) * n_pairs, cudaMemcpyHostToDevice, stream));
@@ -330,7 +335,7 @@ static int prune_mutual_impl(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, 
 	PruneCam cam; cam.H = H; cam.W = W; cam.ifx = 1.0f / fx; cam.ify = 1.0f / fy; cam.icx = -cx / fx; cam.icy = -cy / fy;
 	k_prune_mutual<<<n_pairs, 512, 0, stream>>>(s->pairs.as<PrunePair>(), cam, idxAB, idxBA, k, *prm, corr_out, s->PA.as<float4>(), s->PB.as<float4>(), n_corr_out);
 	// findCorresByMapPoints for the non-neighbour pairs; also records the matches the two knnMatch directions gave (n_nn)
-	k_append_propagated<<<n_pairs, 256, 0, stream>>>(s->pairs.as<PrunePair>(), cam, s->extra.as<float4>(), corr_out, s->PA.as<float4>(), s->PB.as<float4>(), n_corr_out, s->n_nn.as<int32_t>());
+	k_append_propagated<<<n_pairs, 256, 0, stream>>>(s->pairs.as<PrunePair>(), cam, s->extra.as<float4>(), corr_out, s->PA.as<float4>(), s->PB.as<float4>(), n_corr_out, s->n_nn.as<int32_t>(), nullptr);
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;
 }
@@ -392,6 +397,75 @@ extern "C" int bt_match_pairs_ex(bt_ctx* ctx, int n_pairs, const bt_match_frame*
 	BT_REQUIRE(((dA && dB) ? 1 : 0) + ((slotA && slotB) ? 1 : 0) == 1, BT_ERR_INVALID_ARG, "bt_match_pairs_ex: give either descriptor views or pool slots");
 	return match_pairs_impl(ctx, n_pairs, A, B, dA, dB, slotA, slotB, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, entry_out, entry_capacity, n_entry_out, entry_off_out, total_out,
 	                        stream_, extra, status_out, uv_out);
+}
+
+// Bundler::optimizeGPU's findCorres loop (/root/reference/src/Bundler.cpp:298-305) in one asynchronous call: the pairs are matched in the
+// given order against the context's device map-point table (bt_tracks_dev_*), so a pair's propagated matches see the map points every
+// earlier pair of the call created or extended.  kNN, prune and the mutual union do not read the table and run batched; then per pair:
+// propagate (non-neighbour pairs) -> RANSAC -> update the table from the emitted entries.  The EntryJ list is written once at the end.
+extern "C" int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, const bt_desc_view* dA, const bt_desc_view* dB,
+                                    const int32_t* slotA, const int32_t* slotB, int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune,
+                                    int ransac_trials, float ransac_inlier_dist, uint64_t ransac_seed, bt_entryj* entry_out, int entry_capacity,
+                                    int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, int32_t* status_out, float* uv_out, void* stream_) {
+	PruneState* s = ctx ? g_prune_of(ctx) : nullptr;
+	BT_REQUIRE(s && ctx->tracks, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: call bt_pipeline_reserve and bt_tracks_dev_reserve first");
+	BT_REQUIRE(((dA && dB) ? 1 : 0) + ((slotA && slotB) ? 1 : 0) == 1, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: give either descriptor views or pool slots");
+	BT_REQUIRE(A && B && prune && entry_out && entry_capacity >= 0 && n_entry_out && entry_off_out && total_out && n_pairs > 0 && n_pairs <= s->max_pairs,
+	           BT_ERR_INVALID_ARG, "bt_find_corres_pairs: bad argument");
+	{   // frame A is the newer frame of every pair; the frames that are new to the table must fit before anything is queued
+		std::vector<int> fresh;
+		for (int p = 0; p < n_pairs; p++) {
+			BT_REQUIRE(A[p].frame_id > B[p].frame_id, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: pair %d: frame A must be the newer frame (id %d <= %d)", p, A[p].frame_id, B[p].frame_id);
+			for (int id : { A[p].frame_id, B[p].frame_id }) {
+				int sl;
+				tracks_slot(ctx, id, false, &sl);
+				if (sl < 0 && std::find(fresh.begin(), fresh.end(), id) == fresh.end()) fresh.push_back(id);
+			}
+		}
+		BT_REQUIRE((int)fresh.size() <= tracks_free_slots(ctx), BT_ERR_CAPACITY, "bt_find_corres_pairs: %d new frames do not fit the map-point table", (int)fresh.size());
+	}
+	cudaStream_t stream = (cudaStream_t)stream_;
+	BT_CUDA(cudaSetDevice(ctx->device));
+	const int k = 5;   // k_near, FeatureManager.cpp:264
+	int rc = dA ? bt_knn_match_pairs(ctx, n_pairs, dA, dB, k, s->idxAB.as<int32_t>(), s->distAB.as<float>(), s->idxBA.as<int32_t>(), s->distBA.as<float>(), stream_)
+	            : bt_knn_match_slots(ctx, n_pairs, slotA, slotB, k, s->idxAB.as<int32_t>(), s->distAB.as<float>(), s->idxBA.as<int32_t>(), s->distBA.as<float>(), stream_);
+	if (rc != BT_OK) return rc;
+	if ((rc = fill_pairs(s, n_pairs, A, B, stream, nullptr, s->max_feats)) != BT_OK) return rc;
+	PruneCam cam; cam.H = H; cam.W = W; cam.ifx = 1.0f / fx; cam.ify = 1.0f / fy; cam.icx = -cx / fx; cam.icy = -cy / fy;
+	PrunePair* dp = s->pairs.as<PrunePair>();
+	bt_correspondence* corr = s->corr.as<bt_correspondence>();
+	int32_t* n_corr = s->n_corr.as<int32_t>();
+	k_prune_mutual<<<n_pairs, 512, 0, stream>>>(dp, cam, s->idxAB.as<int32_t>(), s->idxBA.as<int32_t>(), k, *prune, corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr);
+	BT_CUDA(cudaGetLastError());
+	const PrunePair* hp = s->h_pairs.as<PrunePair>();       // (fill_pairs' host copy: out_off per pair)
+	for (int p = 0; p < n_pairs; p++) {
+		int sa, sb;
+		if (abs(A[p].frame_id - B[p].frame_id) != 1) {       // findCorresByMapPoints
+			tracks_slot(ctx, A[p].frame_id, false, &sa);
+			tracks_slot(ctx, B[p].frame_id, false, &sb);
+			if (sa >= 0 && sb >= 0) {
+				float4* cand = s->extra.as<float4>() + (size_t)p * s->max_feats;
+				if ((rc = tracks_launch_propagate(ctx, sa, sb, nullptr, 0, cand, s->max_feats, s->n_prop.as<int32_t>() + p, stream)) != BT_OK) return rc;
+				k_append_propagated<<<1, 256, 0, stream>>>(dp + p, cam, s->extra.as<float4>(), corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr + p,
+				                                           s->n_nn.as<int32_t>() + p, s->n_prop.as<int32_t>() + p);
+			}
+		}
+		k_ransac_table_from_counts<<<1, 128, 0, stream>>>(dp + p, 1, n_corr + p, s->PA.as<float4>(), s->PB.as<float4>(), s->rpairs.as<RansacPair>() + p);
+		BT_CUDA(cudaGetLastError());
+		rc = ransac_run_device(ctx, s->rpairs.as<RansacPair>() + p, 1, ransac_trials, ransac_inlier_dist, ransac_seed, s->inl.as<int32_t>(), s->n_inl.as<int32_t>() + p, stream);
+		if (rc != BT_OK) return rc;
+		// updateFramePairMapPoints on the entries the pair emits (none unless its status is OK)
+		if ((rc = tracks_slot(ctx, A[p].frame_id, true, &sa)) != BT_OK) return rc;
+		if ((rc = tracks_slot(ctx, B[p].frame_id, true, &sb)) != BT_OK) return rc;
+		const int off = hp[p].out_off;
+		TrkSrc src{ reinterpret_cast<const float*>(corr + off), (int)(sizeof(bt_correspondence) / sizeof(float)), s->inl.as<int32_t>() + off, nullptr, 0,
+		            s->n_inl.as<int32_t>(), p, entry_capacity };
+		if ((rc = tracks_launch_update(ctx, sa, sb, src, stream)) != BT_OK) return rc;
+	}
+	k_emit_entryj<<<1, 1024, 0, stream>>>(dp, n_pairs, corr, s->inl.as<int32_t>(), s->n_inl.as<int32_t>(), entry_out, n_entry_out, entry_off_out, total_out, entry_capacity, status_out);
+	k_emit_fill<<<n_pairs, 256, 0, stream>>>(dp, corr, s->inl.as<int32_t>(), n_entry_out, entry_off_out, entry_out, entry_capacity, reinterpret_cast<float4*>(uv_out));
+	BT_CUDA(cudaGetLastError());
+	return BT_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ per-pair result cache

@@ -274,17 +274,93 @@ class MatchPipeline:
         return np.asarray(entry_off, np.int32), np.asarray(n_entry, np.int32), bi, bj
 
 
+class DeviceTracks:
+    """The map-point table on the device (bt_tracks_dev_*), owned by a context: the methods of policy.Tracks with the same results,
+    host arrays in and out.  FindCorres keeps one; bt_find_corres_pairs reads and updates it without leaving the device.
+    Capacities: frames alive (<= 64), keys per frame (<= 8192), map points alive (default 16 x max_keys_per_frame).  The table takes
+    about max_points x max_frames x 8 B for the observations plus max_frames x max_keys_per_frame x 48 B for the frame maps: 34 MB and
+    13 MB at the defaults.  All work, including the uploads and read-backs of the methods below, runs on `stream`."""
+
+    def __init__(self, ctx=None, device: int = 0, max_frames: int = 64, max_keys_per_frame: int = 4096, max_points: int = 0, stream: int = 0):
+        self.lib = _lib.load()
+        self.stream = ctypes.c_void_p(stream)
+        self._own = ctx is None
+        self.ctx = ctypes.c_void_p() if ctx is None else ctx
+        if self._own:
+            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
+        self.device = device
+        _lib.check(self.lib.bt_tracks_dev_reserve(self.ctx, ctypes.c_int(max_frames), ctypes.c_int(max_keys_per_frame),
+                                                  ctypes.c_int(max_points or 16 * max_keys_per_frame)), "bt_tracks_dev_reserve")
+
+    def close(self):
+        if self._own and self.ctx:
+            self.lib.bt_ctx_destroy(self.ctx)
+            self.ctx = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _on_stream(self):
+        """torch work (allocation, upload, read-back) on the table's stream: the kernels then see the uploads complete, the read-backs
+        see the kernels complete, and the caching allocator hands a freed buffer only to later work on the same stream."""
+        import contextlib
+        import torch
+        if not self.stream.value:
+            return contextlib.nullcontext()       # the legacy default stream orders against every other stream already
+        return torch.cuda.stream(torch.cuda.ExternalStream(self.stream.value, device=torch.device("cuda", self.device)))
+
+    def update_pair(self, frame_a: int, frame_b: int, uv, is_inlier=None):
+        import numpy as np
+        import torch
+        uv = np.ascontiguousarray(uv, np.float32).reshape(-1, 4)
+        if is_inlier is not None:
+            uv = np.ascontiguousarray(uv[np.asarray(is_inlier).astype(bool)])
+        dev = torch.device("cuda", self.device)
+        with self._on_stream():
+            d_uv = torch.from_numpy(uv).to(dev) if len(uv) else torch.zeros((1, 4), dtype=torch.float32, device=dev)
+            d_n = torch.tensor([len(uv)], dtype=torch.int32, device=dev)
+            _lib.check(self.lib.bt_tracks_dev_update_pair(self.ctx, ctypes.c_int(frame_a), ctypes.c_int(frame_b), ctypes.c_void_p(d_uv.data_ptr()),
+                                                          ctypes.c_void_p(d_n.data_ptr()), ctypes.c_int(len(uv)), self.stream), "bt_tracks_dev_update_pair")
+
+    def propagate(self, frame_a: int, frame_b: int, existing_uv, capacity: int = 65536):
+        import numpy as np
+        import torch
+        ex = np.ascontiguousarray(existing_uv, np.float32).reshape(-1, 4)
+        dev = torch.device("cuda", self.device)
+        with self._on_stream():
+            d_ex = torch.from_numpy(ex).to(dev) if len(ex) else None
+            out = torch.empty((max(capacity, 1), 4), dtype=torch.float32, device=dev)
+            n = torch.zeros(1, dtype=torch.int32, device=dev)
+            _lib.check(self.lib.bt_tracks_dev_propagate(self.ctx, ctypes.c_int(frame_a), ctypes.c_int(frame_b), None if d_ex is None else ctypes.c_void_p(d_ex.data_ptr()),
+                                                        ctypes.c_int(len(ex)), ctypes.c_void_p(out.data_ptr()), ctypes.c_int(capacity), ctypes.c_void_p(n.data_ptr()),
+                                                        self.stream), "bt_tracks_dev_propagate")
+            self.stats()                # synchronises the stream; a propagation longer than `capacity` is an error, as on the host
+            k = int(n.item())
+            return out[:k].cpu().numpy()
+
+    def forget_frame(self, frame: int):
+        _lib.check(self.lib.bt_tracks_dev_forget_frame(self.ctx, ctypes.c_int(frame), self.stream), "bt_tracks_dev_forget_frame")
+
+    def stats(self):
+        a, b = ctypes.c_int(0), ctypes.c_int(0)
+        _lib.check(self.lib.bt_tracks_dev_stats(self.ctx, ctypes.byref(a), ctypes.byref(b), self.stream), "bt_tracks_dev_stats")
+        return a.value, b.value
+
+
 class FindCorres:
     """`SiftManager::findCorres` (/root/reference/src/FeatureManager.cpp:173-242) on the device-resident chain: per pair (A newer)
     kNN both ways -> prune -> mutual union -> [non-neighbour: map-point propagation] -> RANSAC -> EntryJ, with the `_matches` cache
-    (a pair is matched once), the map-point bookkeeping (bt_tracks_*) and the Frame::FAIL outcome.  Descriptors live in the pool."""
+    (a pair is matched once), the map-point table on the device (`tracks`, a DeviceTracks: max_frames alive, max_points map points,
+    default 16 x the pipeline's max_feats; see DeviceTracks for its memory) and the Frame::FAIL outcome.  Descriptors live in the pool."""
 
-    def __init__(self, pipeline: "MatchPipeline", max_pairs_cached: int = 512, max_entries_per_pair: int = 0):
-        from .policy import Tracks
+    def __init__(self, pipeline: "MatchPipeline", max_pairs_cached: int = 512, max_entries_per_pair: int = 0, max_frames: int = 64, max_points: int = 0):
         self.mp = pipeline
         self.lib = pipeline.lib
         self.ctx = pipeline.ctx
-        self.tracks = Tracks()
+        self.tracks = DeviceTracks(ctx=pipeline.ctx, max_frames=max_frames, max_keys_per_frame=pipeline.max_feats, max_points=max_points, stream=pipeline.stream.value or 0)
         self.slot_entries = max_entries_per_pair or 3 * pipeline.max_feats
         _lib.check(self.lib.bt_match_cache_reserve(self.ctx, ctypes.c_int(max_pairs_cached), ctypes.c_int(self.slot_entries)), "bt_match_cache_reserve")
         self.failed = set()          # ids of frames the reference would mark Frame::FAIL
@@ -294,8 +370,10 @@ class FindCorres:
 
     def find_corres(self, pairs, slots, H, W, K, seed: int = 0):
         """pairs: list of (frameA newer, frameB older) dicts as for MatchPipeline.match_pairs; slots: their descriptor-pool slots.
-        Pairs already in the cache are skipped (FeatureManager.cpp:176).  The pairs of ONE call must not depend on each other's map
-        points (the reference matches them one after the other): hand a new frame's neighbour pair first, then its other pairs.
+        Pairs already in the cache are skipped (FeatureManager.cpp:176).  The others are matched IN THE GIVEN ORDER in one asynchronous
+        call (bt_find_corres_pairs): a pair's propagated map-point matches see what the earlier pairs of the same call added to the table,
+        exactly as the reference's pair-by-pair loop does (Bundler.cpp:298-305) - hand a new frame's neighbour pair first, then its older
+        frames oldest first.  One small read-back (counts, offsets, status) at the end feeds the cache.
         Returns {(idA, idB): (n_entries, status)} of the pairs processed in this call."""
         import numpy as np
         import torch
@@ -306,40 +384,30 @@ class FindCorres:
         sl = [slots[k] for k, _ in todo]
         n = len(prs)
         A, B, _, _ = self.mp._views(prs)      # (descriptor views unused: the pool is named by slot)
-        extra = (_lib.MatchExtra * n)()
-        keep = []
-        for i, (a, b) in enumerate(prs):
-            if abs(a["id"] - b["id"]) != 1:
-                uv = np.ascontiguousarray(self.tracks.propagate(a["id"], b["id"], np.zeros((0, 4), np.float32)), np.float32)
-                keep.append(uv)
-                extra[i].uv, extra[i].n = (uv.ctypes.data if len(uv) else None), len(uv)
-        cap = sum(a["kpts"].shape[0] + b["kpts"].shape[0] + extra[i].n for i, (a, b) in enumerate(prs))
+        cap = sum(a["kpts"].shape[0] + b["kpts"].shape[0] for a, b in prs) + n * self.mp.max_feats      # never truncates: room for every propagated match
         dev = prs[0][0]["kpts"].device
         ent = torch.empty((max(cap, 1), 8), dtype=torch.int32, device=dev)
-        uvo = torch.empty((max(cap, 1), 4), dtype=torch.float32, device=dev)
         meta = torch.zeros((3, n), dtype=torch.int32, device=dev)              # n_entry, entry_off, status
         tot = torch.zeros(4, dtype=torch.int32, device=dev)
         sa = (ctypes.c_int32 * n)(*[int(a) for a, _ in sl]); sb = (ctypes.c_int32 * n)(*[int(b) for _, b in sl])
         mp = self.mp
-        _lib.check(self.lib.bt_match_pairs_ex(self.ctx, ctypes.c_int(n), A, B, None, None, sa, sb, ctypes.c_int(H), ctypes.c_int(W),
-                                              ctypes.c_float(K[0]), ctypes.c_float(K[1]), ctypes.c_float(K[2]), ctypes.c_float(K[3]), ctypes.byref(mp.prune),
-                                              ctypes.c_int(mp.ransac_trials), ctypes.c_float(mp.ransac_inlier_dist), ctypes.c_uint64(seed), extra,
-                                              ctypes.c_void_p(ent.data_ptr()), ctypes.c_int(cap), ctypes.c_void_p(meta[0].data_ptr()), ctypes.c_void_p(meta[1].data_ptr()),
-                                              ctypes.c_void_p(tot.data_ptr()), ctypes.c_void_p(meta[2].data_ptr()), ctypes.c_void_p(uvo.data_ptr()), mp.stream), "bt_match_pairs_ex")
-        m = meta.cpu().numpy()                                                  # 3 x n ints: the only per-call read-back besides the inliers' pixel coordinates
-        uv_h = uvo[: int((m[0] + m[1]).max())].cpu().numpy() if m[0].sum() else np.zeros((0, 4), np.float32)
+        _lib.check(self.lib.bt_find_corres_pairs(self.ctx, ctypes.c_int(n), A, B, None, None, sa, sb, ctypes.c_int(H), ctypes.c_int(W),
+                                                 ctypes.c_float(K[0]), ctypes.c_float(K[1]), ctypes.c_float(K[2]), ctypes.c_float(K[3]), ctypes.byref(mp.prune),
+                                                 ctypes.c_int(mp.ransac_trials), ctypes.c_float(mp.ransac_inlier_dist), ctypes.c_uint64(seed),
+                                                 ctypes.c_void_p(ent.data_ptr()), ctypes.c_int(cap), ctypes.c_void_p(meta[0].data_ptr()), ctypes.c_void_p(meta[1].data_ptr()),
+                                                 ctypes.c_void_p(tot.data_ptr()), ctypes.c_void_p(meta[2].data_ptr()), None, mp.stream), "bt_find_corres_pairs")
+        m = meta.cpu().numpy()                                                  # 3 x n ints: the call's only read-back
+        self.tracks.stats()                                                     # (the stream is idle: raises if the table ran out of room)
         ida = (ctypes.c_int32 * n)(*[int(a["id"]) for a, _ in prs]); idb = (ctypes.c_int32 * n)(*[int(b["id"]) for _, b in prs])
         n_h = np.ascontiguousarray(m[0]); off_h = np.ascontiguousarray(m[1]); st_h = np.ascontiguousarray(m[2])
         _lib.check(self.lib.bt_match_cache_put(self.ctx, ctypes.c_int(n), ida, idb, ctypes.c_void_p(ent.data_ptr()), n_h.ctypes.data_as(ctypes.c_void_p),
                                                off_h.ctypes.data_as(ctypes.c_void_p), st_h.ctypes.data_as(ctypes.c_void_p), mp.stream), "bt_match_cache_put")
         out = {}
         for i, (a, b) in enumerate(prs):
-            if n_h[i] > 0:        # updateFramePairMapPoints on the surviving matches (all inliers)
-                self.tracks.update_pair(a["id"], b["id"], uv_h[off_h[i]:off_h[i] + n_h[i]])
             if st_h[i] == 2:
                 self.failed.add(a["id"])
             out[(a["id"], b["id"])] = (int(n_h[i]), int(st_h[i]))
-        self._keep = (ent, uvo, keep)
+        self._keep = ent
         return out
 
     def window_entries(self, frames, device):

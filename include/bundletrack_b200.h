@@ -413,6 +413,35 @@ BT_API int bt_tracks_propagate(bt_tracks* t, int frame_a, int frame_b, const flo
 BT_API int bt_tracks_forget_frame(bt_tracks* t, int frame);
 BT_API int bt_tracks_stats(const bt_tracks* t, int* n_points, int* n_observations);
 
+/* The same table on the device, owned by the context, with the same results as bt_tracks (output bits and order included).  Everything is
+ * asynchronous on `stream` except stats; use one stream for a context's table.
+ *   reserve       capacities: frames alive (<= 64), keys per frame (<= 8192), map points alive.  Empties the table.  Nothing is allocated
+ *                 later.  A call that would exceed a capacity changes nothing and latches a flag: the next bt_tracks_dev_stats returns
+ *                 BT_ERR_CAPACITY (and clears it).  Frames are mapped to slots on the host; a frame past the limit fails at once.
+ *   update_pair   uv_dev: DEVICE (uA, vA, uB, vB) per match, *n_dev (DEVICE) of them, at most uv_capacity; so it can follow an emit without
+ *                 a synchronisation.  Keys must not be NaN.
+ *   propagate     bt_tracks_propagate with existing_uv_dev / out_uv_dev DEVICE and the count written to *n_out_dev.
+ *   stats         synchronises the stream; n_points counts every map point ever created, as bt_tracks_stats does. */
+BT_API int bt_tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_per_frame, int max_points);
+BT_API int bt_tracks_dev_update_pair(bt_ctx* ctx, int frame_a, int frame_b, const float* uv_dev, const int32_t* n_dev, int uv_capacity, void* stream);
+BT_API int bt_tracks_dev_propagate(bt_ctx* ctx, int frame_a, int frame_b, const float* existing_uv_dev, int n_existing,
+                            float* out_uv_dev, int capacity, int32_t* n_out_dev, void* stream);
+BT_API int bt_tracks_dev_forget_frame(bt_ctx* ctx, int frame, void* stream);
+BT_API int bt_tracks_dev_stats(bt_ctx* ctx, int* n_points, int* n_observations, void* stream);
+
+/* SiftManager::findCorres for an ORDERED list of pairs on the context's device table (Bundler::optimizeGPU's loop, Bundler.cpp:298-305):
+ * bt_match_pairs_ex's arguments without `extra` - a non-neighbour pair's propagated matches come from the table as the earlier pairs of
+ * the same call left it, and every pair with status BT_PAIR_OK updates the table with its emitted entries.  The outputs equal those of
+ * calling bt_match_pairs_ex one pair at a time in the same order (propagated matches from bt_tracks_propagate, bt_tracks_update_pair fed
+ * from uv_out), with the pairs back to back in entry_out.  Needs bt_pipeline_reserve and bt_tracks_dev_reserve; A[p].frame_id >
+ * B[p].frame_id.  No device-to-host copy and no synchronisation inside the call. */
+BT_API int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B,
+                         const bt_desc_view* dA, const bt_desc_view* dB, const int32_t* slotA, const int32_t* slotB,
+                         int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune,
+                         int ransac_trials, float ransac_inlier_dist, uint64_t ransac_seed,
+                         bt_entryj* entry_out, int entry_capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out,
+                         int32_t* status_out, float* uv_out, void* stream);
+
 /* Small device-memory helpers so non-CUDA hosts (ctypes, cgo, JNI) can drive the library without another runtime. */
 BT_API int bt_dev_alloc(void** out, size_t bytes);
 BT_API int bt_dev_free(void* p);
