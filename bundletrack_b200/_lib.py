@@ -12,7 +12,11 @@ LIB_PATH = os.environ.get("BT_B200_LIB") or os.path.join(_HERE, "lib", "libbundl
 
 BT_OK = 0
 BT_ERR_INVALID_ARG = -1
+BT_ERR_CAPACITY = -2
+BT_ERR_NO_DEVICE = -4
 BT_MASK_AS_IS, BT_MASK_LARGEST_HULL = 0, 1      # bt_frames_preprocess_masked's mask_mode
+BT_PAIR_OK, BT_PAIR_EMPTY, BT_PAIR_FAIL = 0, 1, 2
+BT_FRAME_OTHER, BT_FRAME_FAIL, BT_FRAME_NO_BA = 0, 1, 2      # Frame::_status as the tracker reports it
 
 
 class BtError(RuntimeError):
@@ -112,6 +116,20 @@ class PruneParams(ctypes.Structure):
     ]
 
 
+class TrackerParams(ctypes.Structure):
+    _fields_ = [
+        ("H", ctypes.c_int), ("W", ctypes.c_int),
+        ("fx", ctypes.c_float), ("fy", ctypes.c_float), ("cx", ctypes.c_float), ("cy", ctypes.c_float),
+        ("max_feats", ctypes.c_int),
+        ("max_frames_alive", ctypes.c_int),
+        ("mask_mode", ctypes.c_int),
+        ("depth", DepthParams), ("solver", SolverParams), ("prune", PruneParams),
+        ("ransac_trials", ctypes.c_int), ("ransac_inlier_dist", ctypes.c_float),
+        ("window_size", ctypes.c_int), ("max_BA_frames", ctypes.c_int), ("min_fm_edges_newframe", ctypes.c_int), ("min_feat_num", ctypes.c_int),
+        ("min_rot_deg", ctypes.c_float),
+    ]
+
+
 class MatchExtra(ctypes.Structure):
     _fields_ = [("uv", ctypes.c_void_p), ("n", ctypes.c_int)]
 
@@ -136,6 +154,7 @@ EXPORTS = [
     "bt_rotation_geodesic", "bt_keyframe_check", "bt_select_keyframes", "bt_rigid_transform", "bt_lfnet_parse_reply", "bt_ba_gate", "bt_pose_format", "bt_pose_write_txt",
     "bt_tracks_create", "bt_tracks_destroy", "bt_tracks_update_pair", "bt_tracks_propagate", "bt_tracks_forget_frame", "bt_tracks_stats",
     "bt_tracks_dev_reserve", "bt_tracks_dev_update_pair", "bt_tracks_dev_propagate", "bt_tracks_dev_forget_frame", "bt_tracks_dev_stats", "bt_find_corres_pairs",
+    "bt_pose_init", "bt_tracker_create", "bt_tracker_destroy", "bt_tracker_begin_frame", "bt_tracker_end_frame", "bt_tracker_drop_frame", "bt_tracker_state",
     "bt_dev_alloc", "bt_dev_free", "bt_memcpy_h2d", "bt_memcpy_d2h", "bt_host_alloc_pinned", "bt_host_free_pinned",
     "bt_stream_sync",
 ]
@@ -157,11 +176,12 @@ def load() -> ctypes.CDLL:
     lib.bt_last_error.restype = ctypes.c_char_p
     for name in EXPORTS:
         fn = getattr(lib, name)
-        if name not in ("bt_last_error", "bt_ctx_destroy", "bt_rotation_geodesic", "bt_tracks_destroy"):
+        if name not in ("bt_last_error", "bt_ctx_destroy", "bt_rotation_geodesic", "bt_tracks_destroy", "bt_tracker_destroy"):
             fn.restype = ctypes.c_int
     lib.bt_ctx_destroy.restype = None
     lib.bt_rotation_geodesic.restype = ctypes.c_float
     lib.bt_tracks_destroy.restype = None
+    lib.bt_tracker_destroy.restype = None
     _lib = lib
     return lib
 

@@ -8,6 +8,8 @@ structs.  Keys and their readers in the reference:
   feature_corres.max_dist_*/max_normal_*                    FeatureManager.cpp:292-295
   ransac.max_iter / ransac.inlier_dist                      FeatureManager.cpp:663-670,713
   bundle.max_BA_frames / min_fm_edges_newframe              Bundler.cpp:222-274,343
+  bundle.window_size                                        Bundler.cpp:149
+  keyframe.min_feat_num / keyframe.min_rot                  Bundler.cpp:195-196
 """
 from __future__ import annotations
 
@@ -63,6 +65,14 @@ def depth_params(yml: Union[None, str, Mapping[str, Any]] = None):
     dp = y.get("depth_processing", NOCS_DEFAULTS["depth_processing"])
     e, b = dp["erode"], dp["bilateral_filter"]
     return DepthParams(int(e["radius"]), float(e["diff"]), float(e["ratio"]), int(b["radius"]), float(b["sigma_D"]), float(b["sigma_R"]))
+
+
+def prune_params(yml: Union[None, str, Mapping[str, Any]] = None):
+    """config "feature_corres" -> bt_prune_params, the angles as cosines (FeatureManager.cpp:292-295)."""
+    from ._lib import PruneParams
+    fc = load_yml(yml)["feature_corres"]
+    return PruneParams(float(fc["max_dist_no_neighbor"]), math.cos(float(fc["max_normal_no_neighbor"]) / 180.0 * math.pi),
+                       float(fc["max_dist_neighbor"]), math.cos(float(fc["max_normal_neighbor"]) / 180.0 * math.pi))
 
 
 def mask_mode(yml: Union[None, str, Mapping[str, Any]] = None) -> int:

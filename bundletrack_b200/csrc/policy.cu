@@ -14,6 +14,7 @@
 #include <stdio.h>
 #include <string.h>
 #include "bt_common.cuh"
+#include "rigid.cuh"
 
 namespace {
 
@@ -25,60 +26,6 @@ float geodesic(const float* A, const float* B) {
 	float t = (tr - 1.f) / 2.0f;
 	t = std::max(std::min(1.0f, t), -1.0f);
 	return acosf(t);
-}
-
-// one-sided Jacobi SVD of a 3x3 (double): M = U diag(s) V^T, singular values sorted descending
-void svd3(const double M[9], double U[9], double S[3], double V[9]) {
-	double A[9];
-	for (int i = 0; i < 9; i++) { A[i] = M[i]; V[i] = (i % 4 == 0) ? 1.0 : 0.0; }
-	for (int sweep = 0; sweep < 60; sweep++) {
-		double off = 0.0;
-		for (int p = 0; p < 2; p++)
-			for (int q = p + 1; q < 3; q++) {
-				double a = 0, b = 0, g = 0;      // columns p, q of A
-				for (int r = 0; r < 3; r++) { a += A[r * 3 + p] * A[r * 3 + p]; b += A[r * 3 + q] * A[r * 3 + q]; g += A[r * 3 + p] * A[r * 3 + q]; }
-				off = std::max(off, fabs(g) / (sqrt(a * b) + 1e-300));
-				if (fabs(g) < 1e-300) continue;
-				const double zeta = (b - a) / (2.0 * g);
-				const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
-				const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
-				for (int r = 0; r < 3; r++) {
-					const double ap = A[r * 3 + p], aq = A[r * 3 + q];
-					A[r * 3 + p] = c * ap - s * aq; A[r * 3 + q] = s * ap + c * aq;
-					const double vp = V[r * 3 + p], vq = V[r * 3 + q];
-					V[r * 3 + p] = c * vp - s * vq; V[r * 3 + q] = s * vp + c * vq;
-				}
-			}
-		if (off < 1e-15) break;
-	}
-	int order[3] = { 0, 1, 2 };
-	double n[3];
-	for (int j = 0; j < 3; j++) n[j] = sqrt(A[j] * A[j] + A[3 + j] * A[3 + j] + A[6 + j] * A[6 + j]);
-	std::sort(order, order + 3, [&](int x, int y) { return n[x] > n[y]; });
-	double Vs[9];
-	for (int j = 0; j < 3; j++) {
-		const int o = order[j];
-		S[j] = n[o];
-		for (int r = 0; r < 3; r++) { U[r * 3 + j] = n[o] > 1e-300 ? A[r * 3 + o] / n[o] : 0.0; Vs[r * 3 + j] = V[r * 3 + o]; }
-	}
-	// A singular value that is rounding noise next to the largest one (coplanar points: one column of M V is ~1e-18) carries no
-	// direction: normalising that column would give a U that is not orthogonal.  Treat it as zero and complete U below.
-	for (int j = 1; j < 3; j++) if (S[j] <= 1e-12 * S[0]) S[j] = 0.0;
-	for (int i = 0; i < 9; i++) V[i] = Vs[i];
-	// complete U to an orthonormal basis when M is rank deficient (Eigen's thin U is full for a 3x3 as well)
-	if (!(S[0] > 1e-300)) { for (int i = 0; i < 9; i++) U[i] = (i % 4 == 0) ? 1.0 : 0.0; return; }      // M = 0
-	if (!(S[1] > 1e-300)) {      // rank 1: any unit vector orthogonal to column 0
-		const int m = fabs(U[0]) < fabs(U[3]) ? (fabs(U[0]) < fabs(U[6]) ? 0 : 2) : (fabs(U[3]) < fabs(U[6]) ? 1 : 2);
-		double e[3] = { 0, 0, 0 }; e[m] = 1.0;
-		const double c[3] = { U[3] * e[2] - U[6] * e[1], U[6] * e[0] - U[0] * e[2], U[0] * e[1] - U[3] * e[0] };
-		const double cn = sqrt(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]);
-		for (int r = 0; r < 3; r++) U[r * 3 + 1] = c[r] / cn;
-	}
-	if (!(S[2] > 1e-300)) {      // rank <= 2: column 2 = column 0 x column 1
-		U[2] = U[3] * U[7] - U[6] * U[4];
-		U[5] = U[6] * U[1] - U[0] * U[7];
-		U[8] = U[0] * U[4] - U[3] * U[1];
-	}
 }
 
 }  // namespace
@@ -133,37 +80,12 @@ extern "C" int bt_select_keyframes(const float* pose_new, const float* keyframe_
 
 extern "C" int bt_rigid_transform(const float* pts1, const float* pts2, int n, float* pose_out) {
 	BT_REQUIRE(pts1 && pts2 && pose_out && n >= 3, BT_ERR_INVALID_ARG, "bt_rigid_transform: needs two arrays of >= 3 points");
-	float* T = pose_out;
-	for (int i = 0; i < 16; i++) T[i] = (i % 5 == 0) ? 1.f : 0.f;
-	double m1[3] = { 0, 0, 0 }, m2[3] = { 0, 0, 0 };
-	for (int i = 0; i < n; i++) for (int k = 0; k < 3; k++) { m1[k] += pts1[3 * i + k]; m2[k] += pts2[3 * i + k]; }
-	for (int k = 0; k < 3; k++) { m1[k] /= n; m2[k] /= n; }
-	double S[9] = { 0 };                                 // S = P^T Q with P, Q the centred point sets
-	for (int i = 0; i < n; i++)
-		for (int r = 0; r < 3; r++)
-			for (int c = 0; c < 3; c++) S[r * 3 + c] += ((double)pts1[3 * i + r] - m1[r]) * ((double)pts2[3 * i + c] - m2[c]);
-	double U[9], sv[3], V[9];
-	svd3(S, U, sv, V);
-	auto vut = [&](double R[9]) { for (int r = 0; r < 3; r++) for (int c = 0; c < 3; c++) { R[r * 3 + c] = 0; for (int k = 0; k < 3; k++) R[r * 3 + c] += V[r * 3 + k] * U[c * 3 + k]; } };
-	double R[9];
-	vut(R);                                              // R = V U^T
-	for (int r = 0; r < 3; r++)                          // R^T R must be the identity (isApprox, Utils.cpp:196), else the pose stays identity
-		for (int c = 0; c < 3; c++) {
-			double d = 0;
-			for (int k = 0; k < 3; k++) d += R[k * 3 + r] * R[k * 3 + c];
-			if (!(fabs(d - (r == c ? 1.0 : 0.0)) <= 1e-5)) return BT_OK;
-		}
-	const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) + R[2] * (R[3] * R[7] - R[4] * R[6]);
-	if (det < 0) { for (int r = 0; r < 3; r++) V[r * 3 + 2] = -V[r * 3 + 2]; vut(R); }      // reflection: flip the last right singular vector
-	float out[16] = { 0 };
-	out[15] = 1.f;
-	for (int r = 0; r < 3; r++) {
-		double t = m2[r];
-		for (int c = 0; c < 3; c++) { out[r * 4 + c] = (float)R[r * 3 + c]; t -= R[r * 3 + c] * m1[c]; }
-		out[r * 4 + 3] = (float)t;
-	}
-	for (int i = 0; i < 16; i++) if (!isfinite(out[i])) return BT_OK;      // isMatrixFinite, Utils.cpp:209
-	for (int i = 0; i < 16; i++) T[i] = out[i];
+	bt::RigidSums r;                                     // the same fit k_pose_init runs on the device (rigid.cuh)
+	bt::rigid_init(r);
+	for (int i = 0; i < n; i++) bt::rigid_add_means(r, pts1 + 3 * (size_t)i, pts2 + 3 * (size_t)i);
+	bt::rigid_means(r, n);
+	for (int i = 0; i < n; i++) bt::rigid_add_cov(r, pts1 + 3 * (size_t)i, pts2 + 3 * (size_t)i);
+	bt::rigid_solve(r, pose_out);
 	return BT_OK;
 }
 

@@ -1,0 +1,437 @@
+// tracker.cu — the whole tracking step, Bundler::processNewFrame (the reference's src/Bundler.cpp:56-183), as one library object over the
+// existing entry points, plus k_pose_init: SiftManager::procrustesByCorrespondence (FeatureManager.cpp:523-557) on the device.
+//
+// The tracker is host code: it calls bt_frames_preprocess_masked, bt_lfnet_request, bt_desc_pool_store, bt_find_corres_pairs, bt_pose_init,
+// bt_match_cache_*, bt_tracks_dev_forget_frame, bt_select_keyframes, bt_ba_gate, bt_frame_cache_store, bt_solve_windows and bt_keyframe_check
+// in the reference's order.  Its own state is the frame deque, the keyframe list and which slot of its reserved buffers each frame holds.
+// Synchronisations per frame: the ROI read-back in begin_frame; in end_frame the initial pose (with the neighbour pair's count and status),
+// the window pairs' counts when any pair of the window was not matched before, and the poses of the solve when bundle adjustment runs.
+// Compiled with -fmad=false: rigid_solve (rigid.cuh) must give the bits bt_rigid_transform gives on the host.
+#include <algorithm>
+#include <deque>
+#include <map>
+#include <vector>
+#include "bt_common.cuh"
+#include "rigid.cuh"
+
+namespace bt {
+
+constexpr int kPoseInitThreads = 256;
+constexpr int kDescDim = 256;          // LF-Net descriptors
+struct PoseInitArgs { float A[16], B[16]; };
+
+// pcl::transformPointWithNormal's point part, ((m0 x + m1 y) + m2 z) + m3 per coordinate, each operation rounded on its own
+__device__ __forceinline__ void xform_point(const float* P, const float* p, float* o) {
+#pragma unroll
+	for (int r = 0; r < 3; r++)
+		o[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(P[r * 4], p[0]), __fmul_rn(P[r * 4 + 1], p[1])), __fmul_rn(P[r * 4 + 2], p[2])), P[r * 4 + 3]);
+}
+
+// One CTA.  The threads transform a chunk of entries into shared memory; thread 0 adds them to the sums in entry order (the host's serial order:
+// a parallel reduction would round differently), once for the means and once more for S, then solves and composes offset * pose_A.
+__global__ void __launch_bounds__(kPoseInitThreads) k_pose_init(const bt_entryj* __restrict__ entries, const int32_t* __restrict__ n_dev,
+                                                               const int32_t* __restrict__ status_dev, PoseInitArgs a, float* __restrict__ pose_out) {
+	__shared__ float s1[kPoseInitThreads][3], s2[kPoseInitThreads][3];
+	const int n = *n_dev;
+	const bool ok = *status_dev == BT_PAIR_OK && n >= 3;       // block-uniform
+	RigidSums r;
+	rigid_init(r);
+	if (ok) {
+		for (int pass = 0; pass < 2; pass++) {
+			for (int base = 0; base < n; base += kPoseInitThreads) {
+				const int i = base + threadIdx.x;
+				if (i < n) {
+					const bt_entryj e = entries[i];
+					xform_point(a.A, e.pos_j, s1[threadIdx.x]);      // src: the newer frame's point in the model frame
+					xform_point(a.B, e.pos_i, s2[threadIdx.x]);      // dst: the older frame's
+				}
+				__syncthreads();
+				if (threadIdx.x == 0) {
+					const int m = min(kPoseInitThreads, n - base);
+					if (pass == 0) for (int k = 0; k < m; k++) rigid_add_means(r, s1[k], s2[k]);
+					else for (int k = 0; k < m; k++) rigid_add_cov(r, s1[k], s2[k]);
+				}
+				__syncthreads();
+			}
+			if (pass == 0 && threadIdx.x == 0) rigid_means(r, n);
+		}
+	}
+	if (threadIdx.x != 0) return;
+	float O[16];
+	if (ok) rigid_solve(r, O);
+	else for (int i = 0; i < 16; i++) O[i] = (i % 5 == 0) ? 1.f : 0.f;
+	for (int i = 0; i < 4; i++)
+		for (int j = 0; j < 4; j++)
+			pose_out[i * 4 + j] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(O[i * 4], a.A[j]), __fmul_rn(O[i * 4 + 1], a.A[4 + j])), __fmul_rn(O[i * 4 + 2], a.A[8 + j])),
+			                                __fmul_rn(O[i * 4 + 3], a.A[12 + j]));
+}
+
+}  // namespace bt
+
+using namespace bt;
+
+extern "C" int bt_pose_init(bt_ctx* ctx, const bt_entryj* entry_dev, const int32_t* n_entry_dev, const int32_t* status_dev, const float* pose_a,
+                            const float* pose_b, float* pose_out_dev, void* stream) {
+	BT_REQUIRE(ctx && entry_dev && n_entry_dev && status_dev && pose_a && pose_b && pose_out_dev, BT_ERR_INVALID_ARG, "bt_pose_init: NULL argument");
+	BT_CUDA(cudaSetDevice(ctx->device));
+	PoseInitArgs a;
+	memcpy(a.A, pose_a, sizeof a.A);
+	memcpy(a.B, pose_b, sizeof a.B);
+	k_pose_init<<<1, kPoseInitThreads, 0, (cudaStream_t)stream>>>(entry_dev, n_entry_dev, status_dev, a, pose_out_dev);
+	BT_CUDA(cudaGetLastError());
+	return BT_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ the tracker
+namespace {
+struct TFrame {
+	int id = 0, slot = -1, cslot = -1;     // map / descriptor-pool slot, frame-cache slot (-1: none)
+	int n_kpts = 0;
+	bool keyframe = false;
+	float pose[16];
+};
+// device scratch in int32 units: the neighbour pair's initial pose and (count, offset, status), then the window call's counts
+enum { M_POSE = 0, M_N = 16, M_OFF = 17, M_STATUS = 18, M_TOTAL = 20, M_WIN = 24 };
+}  // namespace
+
+struct bt_tracker {
+	bt_ctx* ctx = nullptr;
+	bt_tracker_params p;
+	int n_slots = 0, max_pairs = 0, slot_entries = 0, win_entries = 0;
+	size_t hw = 0;
+	DevBuf depth, normal, fg, kpts, roi, entries, gather, meta;
+	PinnedBuf h_meta;
+	std::vector<int> free_slots, free_cslots;
+	std::map<int, TFrame> alive;           // the deque's frames and the keyframes, by id
+	std::deque<int> frames;                // Bundler::_frames (ids)
+	std::vector<int> keyframes;            // Bundler::_keyframes (ids, admission order = id order)
+	bool pending = false;
+	TFrame pend;
+};
+
+static int tr_forget(bt_tracker* t, int id, cudaStream_t stream) {
+	int rc = bt_match_cache_forget_frame(t->ctx, id);
+	if (rc != BT_OK) return rc;
+	return bt_tracks_dev_forget_frame(t->ctx, id, stream);
+}
+static void tr_release(bt_tracker* t, const TFrame& f) {
+	t->free_slots.push_back(f.slot);
+	if (f.cslot >= 0) t->free_cslots.push_back(f.cslot);
+}
+static float* tr_depth(bt_tracker* t, int slot) { return t->depth.as<float>() + t->hw * slot; }
+static float* tr_normal(bt_tracker* t, int slot) { return t->normal.as<float>() + 4 * t->hw * slot; }
+static uint8_t* tr_fg(bt_tracker* t, int slot) { return t->fg.as<uint8_t>() + t->hw * slot; }
+static float* tr_kpts(bt_tracker* t, int slot) { return t->kpts.as<float>() + 2 * (size_t)t->p.max_feats * slot; }
+
+static bt_match_frame tr_match_frame(bt_tracker* t, const TFrame& f, int window_index) {
+	bt_match_frame m{};
+	m.kpts_dev = tr_kpts(t, f.slot); m.n = f.n_kpts;
+	m.depth_dev = tr_depth(t, f.slot); m.normal_dev = tr_normal(t, f.slot);
+	memcpy(m.pose, f.pose, sizeof m.pose);
+	m.frame_id = f.id; m.window_index = window_index;
+	return m;
+}
+// the frame's quarter-resolution maps in the frame cache (CUDACache::storeFrame), once
+static int tr_cache(bt_tracker* t, TFrame& f, cudaStream_t stream) {
+	if (f.cslot >= 0) return BT_OK;
+	BT_REQUIRE(!t->free_cslots.empty(), BT_ERR_CAPACITY, "bt_tracker: no frame-cache slot left");
+	const int cs = t->free_cslots.back();
+	const float* d[1] = { tr_depth(t, f.slot) };
+	const float* n[1] = { tr_normal(t, f.slot) };
+	const bt_tracker_params& p = t->p;
+	int rc = bt_frame_cache_store(t->ctx, 1, &cs, d, n, p.H, p.W, p.fx, p.fy, p.cx, p.cy, p.solver.depth_min, p.solver.depth_max, stream);
+	if (rc != BT_OK) return rc;
+	t->free_cslots.pop_back();
+	f.cslot = cs;
+	return BT_OK;
+}
+static int tr_read(void* dst, const void* src, size_t bytes, cudaStream_t stream) {
+	BT_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, stream));
+	BT_CUDA(cudaStreamSynchronize(stream));
+	return BT_OK;
+}
+// findCorres on an ordered pair list (A newer) in one asynchronous call: (count, offset, status) of the n pairs go to meta_dev[0, 3n)
+static int tr_find_corres(bt_tracker* t, const std::vector<std::pair<const TFrame*, const TFrame*>>& prs, const std::vector<std::pair<int, int>>& widx,
+                          int32_t* meta_dev, cudaStream_t stream) {
+	const int n = (int)prs.size();
+	std::vector<bt_match_frame> A(n), B(n);
+	std::vector<int32_t> sa(n), sb(n);
+	int cap = n * t->p.max_feats;                         // room for every propagated match: never truncates
+	for (int k = 0; k < n; k++) {
+		A[k] = tr_match_frame(t, *prs[k].first, widx[k].first); B[k] = tr_match_frame(t, *prs[k].second, widx[k].second);
+		sa[k] = prs[k].first->slot; sb[k] = prs[k].second->slot;
+		cap += A[k].n + B[k].n;
+	}
+	const bt_tracker_params& p = t->p;
+	return bt_find_corres_pairs(t->ctx, n, A.data(), B.data(), nullptr, nullptr, sa.data(), sb.data(), p.H, p.W, p.fx, p.fy, p.cx, p.cy, &p.prune, p.ransac_trials,
+	                            p.ransac_inlier_dist, 0, t->entries.as<bt_entryj>(), cap, meta_dev, meta_dev + n, t->meta.as<int32_t>() + M_TOTAL, meta_dev + 2 * n,
+	                            nullptr, stream);
+}
+// after the counts are read back: the table's overflow flag, then the _matches cache (SiftManager::_matches) for the same pairs
+static int tr_put(bt_tracker* t, const std::vector<std::pair<const TFrame*, const TFrame*>>& prs, const int32_t* h, cudaStream_t stream) {
+	const int n = (int)prs.size();
+	int pts, obs;
+	int rc = bt_tracks_dev_stats(t->ctx, &pts, &obs, stream);     // (the stream is idle: reports a map-point table overflow)
+	if (rc != BT_OK) return rc;
+	std::vector<int32_t> ia(n), ib(n);
+	for (int k = 0; k < n; k++) { ia[k] = prs[k].first->id; ib[k] = prs[k].second->id; }
+	return bt_match_cache_put(t->ctx, n, ia.data(), ib.data(), t->entries.as<bt_entryj>(), h, h + n, h + 2 * n, stream);
+}
+
+extern "C" int bt_tracker_create(bt_tracker** out, int device, const bt_tracker_params* p) {
+	BT_REQUIRE(out && p, BT_ERR_INVALID_ARG, "bt_tracker_create: NULL argument");
+	*out = nullptr;
+	BT_REQUIRE(p->H > 0 && p->W > 0 && p->max_feats > 0 && p->max_feats <= 8192 && p->max_frames_alive >= 2 && p->max_frames_alive <= 64, BT_ERR_INVALID_ARG,
+	           "bt_tracker_create: bad sizes (max_feats 1..8192, max_frames_alive 2..64)");
+	BT_REQUIRE(p->max_BA_frames >= 2 && p->max_BA_frames <= 32 && p->window_size >= 0 && p->ransac_trials >= 1 &&
+	           (p->mask_mode == BT_MASK_AS_IS || p->mask_mode == BT_MASK_LARGEST_HULL), BT_ERR_INVALID_ARG,
+	           "bt_tracker_create: bad parameters (max_BA_frames 2..32, window_size >= 0, ransac_trials >= 1, mask_mode)");
+	bt_ctx* ctx = nullptr;
+	int rc = bt_ctx_create(&ctx, device);
+	if (rc != BT_OK) return rc;
+	bt_tracker* t = new bt_tracker();
+	t->ctx = ctx;
+	t->p = *p;
+	t->n_slots = p->max_frames_alive + 1;                  // + the frame between begin_frame and end_frame
+	t->max_pairs = p->max_BA_frames * (p->max_BA_frames - 1) / 2;
+	t->slot_entries = 3 * p->max_feats;
+	t->win_entries = t->max_pairs * t->slot_entries;
+	t->hw = (size_t)p->H * p->W;
+	const int F = p->max_frames_alive;
+	const bt_solver_limits lim = { 1, p->max_BA_frames, t->win_entries, p->H, p->W, p->solver.image_downscale };
+#define TRY(x) if ((rc = (x)) != BT_OK) { bt_tracker_destroy(t); return rc; }
+	TRY(bt_solver_reserve(ctx, &lim));
+	TRY(bt_frame_cache_reserve(ctx, F, p->H, p->W, p->solver.image_downscale));
+	TRY(bt_pipeline_reserve(ctx, t->max_pairs, p->max_feats, kDescDim, p->ransac_trials));
+	TRY(bt_desc_pool_reserve(ctx, t->n_slots));
+	TRY(bt_tracks_dev_reserve(ctx, F, p->max_feats, 16 * p->max_feats));
+	TRY(bt_match_cache_reserve(ctx, F * (F - 1) / 2, t->slot_entries));
+	TRY(t->depth.alloc(sizeof(float) * t->hw * t->n_slots));
+	TRY(t->normal.alloc(4 * sizeof(float) * t->hw * t->n_slots));
+	TRY(t->fg.alloc(t->hw * t->n_slots));
+	TRY(t->kpts.alloc(2 * sizeof(float) * (size_t)p->max_feats * t->n_slots));
+	TRY(t->roi.alloc(4 * sizeof(int32_t)));
+	TRY(t->entries.alloc(sizeof(bt_entryj) * (size_t)t->win_entries));
+	TRY(t->gather.alloc(sizeof(bt_entryj) * (size_t)t->win_entries));
+	TRY(t->meta.alloc(sizeof(int32_t) * (M_WIN + 3 * (size_t)t->max_pairs)));
+	TRY(t->h_meta.alloc(sizeof(int32_t) * (M_WIN + 3 * (size_t)t->max_pairs)));
+#undef TRY
+	for (int s = t->n_slots - 1; s >= 0; s--) t->free_slots.push_back(s);
+	for (int s = F - 1; s >= 0; s--) t->free_cslots.push_back(s);
+	*out = t;
+	return BT_OK;
+}
+
+extern "C" void bt_tracker_destroy(bt_tracker* t) {
+	if (!t) return;
+	if (t->ctx) {
+		cudaSetDevice(t->ctx->device);
+		DevBuf* bufs[] = { &t->depth, &t->normal, &t->fg, &t->kpts, &t->roi, &t->entries, &t->gather, &t->meta };
+		for (DevBuf* b : bufs) b->release();
+		t->h_meta.release();
+		bt_ctx_destroy(t->ctx);
+	}
+	delete t;
+}
+
+extern "C" int bt_tracker_begin_frame(bt_tracker* t, int loader_id, const float* first_pose, const float* depth_raw_dev, const uint8_t* mask_dev,
+                                      const uint8_t* colour_dev, uint8_t* request_out_dev, int32_t* roi_out, int* status_out, void* stream_) {
+	BT_REQUIRE(t && depth_raw_dev && mask_dev && colour_dev && request_out_dev && status_out, BT_ERR_INVALID_ARG, "bt_tracker_begin_frame: NULL argument");
+	BT_REQUIRE(!t->pending, BT_ERR_INVALID_ARG, "bt_tracker_begin_frame: frame %d is pending: finish it with end_frame or drop_frame first", t->pend.id);
+	cudaStream_t stream = (cudaStream_t)stream_;
+	BT_CUDA(cudaSetDevice(t->ctx->device));
+	const bt_tracker_params& p = t->p;
+	TFrame f;
+	if (!t->frames.empty()) {                              // Bundler.cpp:74-81
+		const TFrame& last = t->alive.at(t->frames.back());
+		f.id = last.id + 1;
+		memcpy(f.pose, last.pose, sizeof f.pose);
+	} else {
+		f.id = loader_id;
+		for (int i = 0; i < 16; i++) f.pose[i] = first_pose ? first_pose[i] : ((i % 5 == 0) ? 1.f : 0.f);
+	}
+	f.slot = t->free_slots.back();                         // (one slot more than frames alive: never empty here)
+	const float* din[1] = { depth_raw_dev };
+	const uint8_t* msk[1] = { mask_dev };
+	float* dout[1] = { tr_depth(t, f.slot) };
+	float* nout[1] = { tr_normal(t, f.slot) };
+	uint8_t* fg[1] = { tr_fg(t, f.slot) };
+	int rc = bt_frames_preprocess_masked(t->ctx, 1, din, msk, p.mask_mode, p.H, p.W, p.fx, p.fy, p.cx, p.cy, &p.depth, dout, nullptr, nout, fg,
+	                                     t->roi.as<int32_t>(), stream);
+	if (rc != BT_OK) return rc;
+	int32_t* roi = t->h_meta.as<int32_t>();
+	if ((rc = tr_read(roi, t->roi.p, 4 * sizeof(int32_t), stream)) != BT_OK) return rc;
+	if (roi_out) memcpy(roi_out, roi, 4 * sizeof(int32_t));
+	if (roi[1] - roi[0] < 10 || roi[3] - roi[2] < 10) {   // Bundler.cpp:88-93: FAIL, nothing is kept or forgotten
+		*status_out = BT_FRAME_FAIL;
+		return BT_OK;
+	}
+	const uint8_t* col[1] = { colour_dev };
+	const uint8_t* fgc[1] = { fg[0] };
+	uint8_t* req[1] = { request_out_dev };
+	if ((rc = bt_lfnet_request(t->ctx, 1, col, fgc, t->roi.as<int32_t>(), p.H, p.W, req, stream)) != BT_OK) return rc;
+	t->free_slots.pop_back();
+	t->pend = f;
+	t->pending = true;
+	*status_out = BT_FRAME_OTHER;
+	return BT_OK;
+}
+
+extern "C" int bt_tracker_drop_frame(bt_tracker* t, float* pose_out) {
+	BT_REQUIRE(t, BT_ERR_INVALID_ARG, "bt_tracker_drop_frame: NULL tracker");
+	BT_REQUIRE(t->pending, BT_ERR_INVALID_ARG, "bt_tracker_drop_frame: no frame is pending");
+	BT_CUDA(cudaSetDevice(t->ctx->device));
+	int rc = tr_forget(t, t->pend.id, nullptr);
+	if (rc != BT_OK) return rc;
+	tr_release(t, t->pend);
+	t->pending = false;
+	if (pose_out) memcpy(pose_out, t->pend.pose, sizeof t->pend.pose);
+	return BT_OK;
+}
+
+extern "C" int bt_tracker_end_frame(bt_tracker* t, const float* kpts_host, int n_kpts, const bt_desc_view* desc, float* pose_out, int* status_out, void* stream_) {
+	BT_REQUIRE(t && desc && pose_out && status_out, BT_ERR_INVALID_ARG, "bt_tracker_end_frame: NULL argument");
+	BT_REQUIRE(t->pending, BT_ERR_INVALID_ARG, "bt_tracker_end_frame: no frame is pending (begin_frame first; a frame that failed the ROI gate is done)");
+	const bt_tracker_params& p = t->p;
+	BT_REQUIRE(n_kpts >= 0 && n_kpts <= p.max_feats, BT_ERR_INVALID_ARG, "bt_tracker_end_frame: %d keypoints, the tracker was created for %d", n_kpts, p.max_feats);
+	BT_REQUIRE((n_kpts == 0 || (kpts_host && desc->dev)) && desc->n == n_kpts && desc->dim == kDescDim, BT_ERR_INVALID_ARG,
+	           "bt_tracker_end_frame: the descriptor view must hold n_kpts rows of %d floats", kDescDim);
+	BT_REQUIRE((int)t->alive.size() + 1 <= p.max_frames_alive, BT_ERR_CAPACITY, "bt_tracker_end_frame: %d frames alive + the new one > max_frames_alive %d",
+	           (int)t->alive.size(), p.max_frames_alive);
+	cudaStream_t stream = (cudaStream_t)stream_;
+	BT_CUDA(cudaSetDevice(t->ctx->device));
+	TFrame f = t->pend;
+	f.n_kpts = n_kpts;
+	int rc;
+	if (n_kpts) BT_CUDA(cudaMemcpyAsync(tr_kpts(t, f.slot), kpts_host, 2 * sizeof(float) * (size_t)n_kpts, cudaMemcpyHostToDevice, stream));
+	if ((rc = bt_desc_pool_store(t->ctx, f.slot, desc, stream)) != BT_OK) return rc;
+	t->pending = false;                                    // from here on the frame is the tracker's
+	int status = BT_FRAME_OTHER;
+	int32_t* md = t->meta.as<int32_t>();
+	int32_t* mh = t->h_meta.as<int32_t>();
+	auto finish_fail = [&](bool in_deque) -> int {         // forgetFrame (+ pop_back); the reported pose is the one the frame has
+		if ((rc = tr_forget(t, f.id, stream)) != BT_OK) return rc;
+		if (in_deque) { t->frames.pop_back(); t->alive.erase(f.id); }
+		tr_release(t, f);
+		memcpy(pose_out, f.pose, sizeof f.pose);
+		*status_out = BT_FRAME_FAIL;
+		return BT_OK;
+	};
+	if (!t->frames.empty()) {                              // Bundler.cpp:119-138
+		const TFrame& last = t->alive.at(t->frames.back());
+		std::vector<std::pair<const TFrame*, const TFrame*>> prs = { { &f, &last } };
+		if ((rc = tr_find_corres(t, prs, { { 1, 0 } }, md + M_N, stream)) != BT_OK) return rc;
+		if ((rc = bt_pose_init(t->ctx, t->entries.as<bt_entryj>(), md + M_N, md + M_STATUS, f.pose, last.pose, reinterpret_cast<float*>(md + M_POSE), stream)) != BT_OK) return rc;
+		if ((rc = tr_read(mh, md, sizeof(int32_t) * (M_STATUS + 1), stream)) != BT_OK) return rc;     // the pose, count, offset and status
+		if ((rc = tr_put(t, prs, mh + M_N, stream)) != BT_OK) return rc;
+		if (mh[M_STATUS] == BT_PAIR_FAIL) return finish_fail(false);
+		memcpy(f.pose, mh + M_POSE, sizeof f.pose);
+	}
+	if ((int)t->frames.size() >= p.window_size + 3) {      // Bundler.cpp:149-157
+		const int old = t->frames.front();
+		TFrame& o = t->alive.at(old);
+		if (!o.keyframe) {
+			if ((rc = tr_forget(t, old, stream)) != BT_OK) return rc;
+			tr_release(t, o);
+			t->alive.erase(old);
+		}
+		t->frames.pop_front();
+	}
+	t->frames.push_back(f.id);
+	t->alive[f.id] = f;
+	TFrame& nf = t->alive.at(f.id);
+	if (f.id != 0) {                                       // selectKeyFramesForBA + optimizeGPU (Bundler.cpp:222-358)
+		const int K = (int)t->keyframes.size();
+		std::vector<float> kp(16 * (size_t)std::max(K, 1));
+		for (int k = 0; k < K; k++) memcpy(&kp[16 * (size_t)k], t->alive.at(t->keyframes[k]).pose, 64);
+		std::vector<int32_t> chosen(std::max(K, 1));
+		int n_chosen = 0;
+		if ((rc = bt_select_keyframes(nf.pose, kp.data(), K, p.max_BA_frames, chosen.data(), &n_chosen)) != BT_OK) return rc;
+		std::vector<TFrame*> win;
+		for (int k = 0; k < n_chosen; k++) win.push_back(&t->alive.at(t->keyframes[chosen[k]]));
+		win.push_back(&nf);                                // the newest frame sorts last
+		const int N = (int)win.size();
+		std::vector<std::pair<const TFrame*, const TFrame*>> todo;
+		std::vector<std::pair<int, int>> widx;
+		std::vector<int32_t> ga, gb;
+		std::vector<uint32_t> wi, wj;
+		for (int i = 0; i < N; i++)
+			for (int j = i + 1; j < N; j++) {
+				ga.push_back(win[j]->id); gb.push_back(win[i]->id); wi.push_back(i); wj.push_back(j);
+				if (!bt_match_cache_has(t->ctx, win[j]->id, win[i]->id)) { todo.push_back({ win[j], win[i] }); widx.push_back({ j, i }); }
+			}
+		if (!todo.empty()) {
+			const int n = (int)todo.size();
+			if ((rc = tr_find_corres(t, todo, widx, md + M_WIN, stream)) != BT_OK) return rc;
+			if ((rc = tr_read(mh + M_WIN, md + M_WIN, sizeof(int32_t) * 3 * n, stream)) != BT_OK) return rc;
+			if ((rc = tr_put(t, todo, mh + M_WIN, stream)) != BT_OK) return rc;
+			for (int k = 0; k < n; k++)
+				if (mh[M_WIN + 2 * n + k] == BT_PAIR_FAIL && todo[k].first == &nf) status = BT_FRAME_FAIL;
+		}
+		int n_edges = 0;
+		const int np = (int)ga.size();
+		std::vector<int32_t> boff(std::max(np, 1)), bn(std::max(np, 1));
+		if (np > 0) {
+			if ((rc = bt_match_cache_gather(t->ctx, np, ga.data(), gb.data(), wi.data(), wj.data(), t->gather.as<bt_entryj>(), t->win_entries, boff.data(), bn.data(), stream)) != BT_OK)
+				return rc;
+			for (int k = 0; k < np; k++) if ((int)wj[k] == N - 1) n_edges += bn[k];
+		}
+		if (status != BT_FRAME_FAIL) {
+			if (!bt_ba_gate(n_edges, p.min_fm_edges_newframe)) status = BT_FRAME_NO_BA;
+			else if (N >= 2) {
+				if ((rc = tr_cache(t, nf, stream)) != BT_OK) return rc;
+				std::vector<const float*> dptr(N), nptr(N);
+				std::vector<int32_t> cs(N);
+				std::vector<float> poses(16 * (size_t)N);
+				for (int k = 0; k < N; k++) {
+					dptr[k] = tr_depth(t, win[k]->slot); nptr[k] = tr_normal(t, win[k]->slot); cs[k] = win[k]->cslot;
+					memcpy(&poses[16 * (size_t)k], win[k]->pose, 64);
+				}
+				bt_window w{};
+				w.n_frames = N; w.H = p.H; w.W = p.W;
+				w.depth_dev = dptr.data(); w.normal_dev = nptr.data();
+				w.fx = p.fx; w.fy = p.fy; w.cx = p.cx; w.cy = p.cy;
+				w.compat_flip = 1;
+				w.cache_slots = cs.data();
+				w.corr_dev = t->gather.as<bt_entryj>();
+				w.n_blocks = np; w.block_off = boff.data(); w.block_n = bn.data(); w.block_i = wi.data(); w.block_j = wj.data();
+				if ((rc = bt_solve_windows(t->ctx, 1, &w, &p.solver, poses.data(), stream)) != BT_OK) return rc;
+				for (int k = 0; k < N; k++) memcpy(win[k]->pose, &poses[16 * (size_t)k], 64);     // every frame of the window, keyframes included
+			}
+		}
+	}
+	f = nf;
+	if (status == BT_FRAME_FAIL) return finish_fail(true);   // Bundler.cpp:173-179
+	bool admit = false;                                    // checkAndAddKeyframe (Bundler.cpp:185-221)
+	if (status == BT_FRAME_OTHER) {
+		const int K = (int)t->keyframes.size();
+		std::vector<float> kp(16 * (size_t)std::max(K, 1));
+		for (int k = 0; k < K; k++) memcpy(&kp[16 * (size_t)k], t->alive.at(t->keyframes[k]).pose, 64);
+		admit = bt_keyframe_check(nf.pose, nf.id, nf.n_kpts, kp.data(), K, p.min_feat_num, p.min_rot_deg) == 1;
+	}
+	if (admit) {
+		if ((rc = tr_cache(t, nf, stream)) != BT_OK) return rc;
+		nf.keyframe = true;
+		t->keyframes.push_back(nf.id);
+	} else if (nf.cslot >= 0) {                            // only keyframes take part in later windows
+		t->free_cslots.push_back(nf.cslot);
+		nf.cslot = -1;
+	}
+	memcpy(pose_out, nf.pose, sizeof nf.pose);
+	*status_out = status;
+	return BT_OK;
+}
+
+extern "C" int bt_tracker_state(bt_tracker* t, int32_t* ids, float* poses, int32_t* is_keyframe, int cap, int* n) {
+	BT_REQUIRE(t && n && cap >= 0, BT_ERR_INVALID_ARG, "bt_tracker_state: NULL argument");
+	*n = (int)t->alive.size();
+	BT_REQUIRE(*n <= cap, BT_ERR_CAPACITY, "bt_tracker_state: %d frames alive > cap %d", *n, cap);
+	int k = 0;
+	for (const auto& kv : t->alive) {
+		if (ids) ids[k] = kv.first;
+		if (poses) memcpy(poses + 16 * (size_t)k, kv.second.pose, 64);
+		if (is_keyframe) is_keyframe[k] = kv.second.keyframe ? 1 : 0;
+		k++;
+	}
+	return BT_OK;
+}

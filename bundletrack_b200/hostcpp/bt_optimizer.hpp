@@ -298,3 +298,64 @@ inline void knnMatchBothDirections(bt_ctx* ctx, const float* desA, int nA, size_
 	KnnMatcherGpu m(ctx, (nA > nB ? nA : nB) > 0 ? (nA > nB ? nA : nB) : 1, dim, k);
 	m.knnMatchBothDirections(desA, nA, stepA, desB, nB, stepB, matchesAB, matchesBA, stream);
 }
+
+// ---- Bundler::processNewFrame (the reference's src/Bundler.cpp:56-183) as one object over bt_tracker_* -------------------------------------
+// The reference's call is split where it asks the LF-Net server for features (Lfnet::detectFeature, Bundler.cpp:108): beginFrame segments the
+// frame and returns the request image, the caller does the ZMQ round trip (bt_lfnet_parse_reply maps the keypoints back) and calls endFrame,
+// or dropFrame when detection threw.  Statuses are Frame::_status values (BT_FRAME_OTHER / FAIL / NO_BA); poses are cam->model through
+// operator()(row, col) (Eigen::Matrix4f works); endFrame's pose is what Bundler::saveNewframeResult records for the frame.
+class BundlerGpu {
+public:
+	explicit BundlerGpu(const bt_tracker_params& p, int device = 0) { check(bt_tracker_create(&t_, device, &p), "bt_tracker_create"); }
+	~BundlerGpu() { bt_tracker_destroy(t_); }
+	BundlerGpu(const BundlerGpu&) = delete;
+	BundlerGpu& operator=(const BundlerGpu&) = delete;
+
+	// loader_id / first_pose (nullptr: identity) name the frame when the tracker holds none.  roi (optional): Frame::_roi.
+	template <class Mat4>
+	int beginFrame(int loader_id, const Mat4* first_pose, const float* depth_raw_gpu, const uint8_t* mask_gpu, const uint8_t* color_gpu, uint8_t* request_gpu,
+	               int32_t* roi = nullptr, void* stream = nullptr) {
+		float fp[16];
+		if (first_pose) to_flat(*first_pose, fp);
+		int st = -1;
+		check(bt_tracker_begin_frame(t_, loader_id, first_pose ? fp : nullptr, depth_raw_gpu, mask_gpu, color_gpu, request_gpu, roi, &st, stream), "bt_tracker_begin_frame");
+		return st;
+	}
+	// kpts: n x (x, y) image pixels; desc_gpu: n x 256 device floats, desc_step bytes per row (GpuMat::step; 0 = packed)
+	template <class Mat4>
+	int endFrame(const float* kpts, int n, const float* desc_gpu, size_t desc_step, Mat4& pose, void* stream = nullptr) {
+		bt_desc_view d{}; d.dev = desc_gpu; d.n = n; d.dim = 256; d.pitch_bytes = desc_step;
+		float fp[16];
+		int st = -1;
+		check(bt_tracker_end_frame(t_, kpts, n, &d, fp, &st, stream), "bt_tracker_end_frame");
+		from_flat(fp, pose);
+		return st;
+	}
+	template <class Mat4>
+	void dropFrame(Mat4& pose) {
+		float fp[16];
+		check(bt_tracker_drop_frame(t_, fp), "bt_tracker_drop_frame");
+		from_flat(fp, pose);
+	}
+	// every frame alive, oldest first
+	template <class Mat4, class Alloc>
+	void state(std::vector<int>& ids, std::vector<Mat4, Alloc>& poses, std::vector<bool>& is_keyframe) {
+		int n = 0;
+		const int rc = bt_tracker_state(t_, nullptr, nullptr, nullptr, 0, &n);      // the count (BT_ERR_CAPACITY unless no frame is alive)
+		if (rc != BT_ERR_CAPACITY) check(rc, "bt_tracker_state");
+		std::vector<int32_t> id(n), kf(n);
+		std::vector<float> p(16 * (size_t)n);
+		check(bt_tracker_state(t_, id.data(), p.data(), kf.data(), n, &n), "bt_tracker_state");
+		ids.assign(id.begin(), id.end());
+		poses.resize(n);
+		is_keyframe.resize(n);
+		for (int k = 0; k < n; k++) { from_flat(&p[16 * (size_t)k], poses[k]); is_keyframe[k] = kf[k] != 0; }
+	}
+	bt_tracker* handle() { return t_; }
+
+private:
+	static void check(int rc, const char* what) { if (rc != BT_OK) throw std::runtime_error(std::string(what) + ": " + bt_last_error()); }
+	template <class Mat4> static void to_flat(const Mat4& m, float* f) { for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) f[4 * r + c] = m(r, c); }
+	template <class Mat4> static void from_flat(const float* f, Mat4& m) { for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) m(r, c) = f[4 * r + c]; }
+	bt_tracker* t_ = nullptr;
+};

@@ -156,16 +156,14 @@ class MatchPipeline:
     Bundler::optimizeGPU would build (/root/reference/src/FeatureManager.cpp:173-368,561-741; src/Bundler.cpp:298-324)."""
 
     def __init__(self, yml=None, device: int = 0, max_pairs: int = 64, max_feats: int = 4096, dim: int = 256, stream: int = 0):
-        import math
-        from .config import load_yml
+        from .config import load_yml, prune_params
         self.lib = _lib.load()
         self.stream = ctypes.c_void_p(stream)
         self.ctx = ctypes.c_void_p()
         _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
         y = load_yml(yml)
-        fc, rs = y["feature_corres"], y["ransac"]
-        self.prune = _lib.PruneParams(float(fc["max_dist_no_neighbor"]), math.cos(float(fc["max_normal_no_neighbor"]) / 180.0 * math.pi),
-                                      float(fc["max_dist_neighbor"]), math.cos(float(fc["max_normal_neighbor"]) / 180.0 * math.pi))
+        rs = y["ransac"]
+        self.prune = prune_params(y)
         self.ransac_trials = int(rs["max_iter"])
         self.ransac_inlier_dist = float(rs["inlier_dist"])
         _lib.check(self.lib.bt_pipeline_reserve(self.ctx, ctypes.c_int(max_pairs), ctypes.c_int(max_feats), ctypes.c_int(dim), ctypes.c_int(max(self.ransac_trials, 1))), "bt_pipeline_reserve")

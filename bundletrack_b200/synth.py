@@ -343,3 +343,93 @@ def make_ransac_case(seed: int, n: int, inlier_frac: float = 0.7, noise: float =
     A4 = np.concatenate([A, np.ones((n, 1))], 1).astype(np.float32)
     B4 = np.concatenate([B, np.ones((n, 1))], 1).astype(np.float32)
     return A4, B4, ~out
+
+
+@dataclasses.dataclass
+class Sequence:
+    """A tracked object over time, as the tracker's caller sees it: per frame the raw depth, the mask PNG's bytes, the colour image and
+    what the LF-Net server would reply (keypoints, descriptors; None where feature detection fails)."""
+    depth_raw: np.ndarray    # [N,H,W] f32, metres, 0 = hole
+    mask: np.ndarray         # [N,H,W] u8, 255 = object (the silhouette plus a distractor blob)
+    colour: np.ndarray       # [N,H,W,3] u8 BGR
+    feats: list              # per frame {kpts [n,2] f32, desc [n,dim] f32, ids [n]} or None
+    poses_gt: np.ndarray     # [N,4,4] f64 cam->model, model = camera frame 0
+    K: tuple
+    roi_fail: tuple          # frames whose mask is empty (the tracker's ROI gate fails)
+    neighbour_fail: tuple    # frames whose features cannot match the previous frame
+    detect_fail: tuple       # frames without features (detection failed)
+
+    @property
+    def n_frames(self) -> int:
+        return self.depth_raw.shape[0]
+
+
+def _dilate(m: np.ndarray, r: int) -> np.ndarray:
+    p = np.pad(m, r)
+    out = np.zeros_like(m)
+    for dy in range(2 * r + 1):
+        for dx in range(2 * r + 1):
+            out |= p[dy:dy + m.shape[0], dx:dx + m.shape[1]]
+    return out
+
+
+def make_sequence(seed: int, n_frames: int, H: int = 480, W: int = 640, K=None, n_feats: int = 500, rot_deg=(2.0, 6.0), hole_frac: float = 0.02,
+                  roi_fail=(), neighbour_fail=(), detect_fail=()) -> Sequence:
+    """A smooth trajectory of one rendered ellipsoid (render_ellipsoid) with features from make_feature_frames: per frame a rotation of
+    rot_deg degrees about an axis that drifts slowly, and a few millimetres of translation.  Raw depth has 1 mm noise and `hole_frac` holes;
+    the mask is the silhouette plus a disc-shaped distractor blob away from it (largest-hull mode drops it, as-is mode keeps it); the colour
+    image is a gradient with the object shaded by its normals.  Events at the listed frames: an empty mask (roi_fail), random descriptors at
+    background pixels that have no depth (neighbour_fail: the neighbour pair finds no match), no features at all (detect_fail: feats is None)."""
+    K = tuple(v * W / 640.0 for v in NOCS_K) if K is None else tuple(K)
+    rng = np.random.default_rng(np.uint64(0x5EC) + np.uint64(seed))
+    radii = rng.uniform(0.05, 0.1, size=3)
+    R, _ = _sample_pose(rng)
+    c = np.array([rng.uniform(-0.02, 0.02), rng.uniform(-0.02, 0.02), rng.uniform(0.6, 0.75)])
+    axis = rng.normal(size=3)
+    axis /= np.linalg.norm(axis)
+    ob_in_cam = np.zeros((n_frames, 4, 4))
+    ob_in_cam[0] = se3(R, c)
+    for k in range(1, n_frames):
+        axis = axis + rng.normal(0, 0.3, 3)
+        axis /= np.linalg.norm(axis)
+        R = so3_exp(axis * np.deg2rad(rng.uniform(*rot_deg))) @ R
+        c = c + rng.normal(0, 0.003, 3)
+        c[2] = np.clip(c[2], 0.55, 0.8)
+        c[:2] = np.clip(c[:2], -0.04, 0.04)
+        ob_in_cam[k] = se3(R, c)
+    poses_gt = np.stack([ob_in_cam[0] @ np.linalg.inv(ob_in_cam[k]) for k in range(n_frames)])
+    depth = np.zeros((n_frames, H, W), np.float32)
+    normal = np.zeros((n_frames, H, W, 4), np.float32)
+    for k in range(n_frames):
+        depth[k], normal[k] = render_ellipsoid(radii, ob_in_cam[k], K, H, W, rng)
+    win = Window(depth, normal, poses_gt.astype(np.float32), poses_gt, np.zeros(0, ENTRYJ_DTYPE), K, radii, ob_in_cam)
+    feats = make_feature_frames(win, n_feats=n_feats, seed=seed, n_surface=max(4000, 4 * n_feats))
+    yy, xx = np.mgrid[0:H, 0:W]
+    raw = depth.copy()
+    mask = np.zeros((n_frames, H, W), np.uint8)
+    colour = np.zeros((n_frames, H, W, 3), np.uint8)
+    r_blob = 0.05 * min(H, W)
+    for k in range(n_frames):
+        sil = depth[k] > 0
+        raw[k][rng.random((H, W)) < hole_frac] = 0.0
+        ys, xs = np.nonzero(sil)
+        # the distractor sits in the image corner farthest from the silhouette's centre
+        bx = r_blob + 1 if xs.mean() > W / 2 else W - r_blob - 2
+        by = r_blob + 1 if ys.mean() > H / 2 else H - r_blob - 2
+        blob = (xx - bx) ** 2 + (yy - by) ** 2 <= r_blob ** 2
+        mask[k] = (sil | blob).astype(np.uint8) * 255
+        shade = (60 + 150 * np.abs(normal[k][..., :3])).astype(np.uint8)
+        bg = np.stack([xx * 255 // W, yy * 255 // H, np.full((H, W), 128)], -1).astype(np.uint8)
+        colour[k] = np.where(sil[..., None], shade, bg)
+        if k in neighbour_fail:
+            n = len(feats[k]["kpts"])
+            far = np.nonzero(~_dilate(sil, 4))
+            sel = rng.integers(0, len(far[0]), n)
+            d = rng.normal(size=(n, feats[k]["desc"].shape[1]))
+            feats[k] = {"kpts": np.stack([far[1][sel], far[0][sel]], 1).astype(np.float32),
+                        "desc": (d / np.linalg.norm(d, axis=1, keepdims=True)).astype(np.float32), "ids": -np.ones(n, int)}
+        if k in roi_fail:
+            mask[k] = 0
+        if k in detect_fail:
+            feats[k] = None
+    return Sequence(raw, mask, colour, feats, poses_gt, K, tuple(roi_fail), tuple(neighbour_fail), tuple(detect_fail))

@@ -1,0 +1,99 @@
+"""`Bundler::processNewFrame` (the reference's src/Bundler.cpp:56-183) as one object: give it frames, get poses.  A thin ctypes mirror of
+bt_tracker_* (include/bundletrack_b200.h); the step itself - ids, the frame deque, keyframes, matching, the initial pose, the BA gate and the
+solve - runs in the library.  The step is split where the reference asks the LF-Net server for features: `begin_frame` returns the request
+image, the caller does the round trip (its reply goes through policy.lfnet_parse_reply) and hands keypoints and descriptors to `end_frame`,
+or calls `drop_frame` when detection failed."""
+from __future__ import annotations
+
+import ctypes
+
+import numpy as np
+
+from . import _lib
+from .config import depth_params, load_yml, mask_mode, prune_params, solver_params
+
+
+def tracker_params(yml, H: int, W: int, K, max_feats: int, max_frames_alive: int, mode: int = None) -> "_lib.TrackerParams":
+    """bt_tracker_params from the config keys the reference reads (bundle.window_size / max_BA_frames / min_fm_edges_newframe,
+    keyframe.min_feat_num / min_rot, ransac.max_iter / inlier_dist and those config.py maps).  mode: _lib.BT_MASK_* (default: config.mask_mode)."""
+    y = load_yml(yml)
+    Kn = np.asarray(K, np.float64)
+    fx, fy, cx, cy = (Kn[0, 0], Kn[1, 1], Kn[0, 2], Kn[1, 2]) if Kn.ndim == 2 else Kn
+    b, kf, rs = y["bundle"], y["keyframe"], y["ransac"]
+    p = _lib.TrackerParams()
+    p.H, p.W, p.fx, p.fy, p.cx, p.cy = int(H), int(W), float(fx), float(fy), float(cx), float(cy)
+    p.max_feats, p.max_frames_alive = int(max_feats), int(max_frames_alive)
+    p.mask_mode = mask_mode(yml) if mode is None else int(mode)
+    p.depth, p.solver, p.prune = depth_params(y), solver_params(y), prune_params(y)
+    p.ransac_trials, p.ransac_inlier_dist = int(rs["max_iter"]), float(rs["inlier_dist"])
+    p.window_size, p.max_BA_frames, p.min_fm_edges_newframe = int(b["window_size"]), int(b["max_BA_frames"]), int(b["min_fm_edges_newframe"])
+    p.min_feat_num, p.min_rot_deg = int(kf["min_feat_num"]), float(kf["min_rot"])
+    return p
+
+
+def _ptr(x) -> int:
+    return int(x.data_ptr()) if hasattr(x, "data_ptr") else int(x)
+
+
+class Tracker:
+    """Tracker(yml, H, W, K, max_feats, max_frames_alive): everything is reserved here (bt_tracker_create states the memory).  Device
+    arguments are torch CUDA tensors (or raw device addresses); the library works on `stream` (default: the legacy default stream)."""
+
+    def __init__(self, yml, H: int, W: int, K, max_feats: int, max_frames_alive: int, device: int = 0, stream: int = 0, mode: int = None):
+        self.lib = _lib.load()
+        self.params = tracker_params(yml, H, W, K, max_feats, max_frames_alive, mode)
+        self.stream = ctypes.c_void_p(stream)
+        self.t = ctypes.c_void_p()
+        _lib.check(self.lib.bt_tracker_create(ctypes.byref(self.t), ctypes.c_int(device), ctypes.byref(self.params)), "bt_tracker_create")
+
+    def close(self):
+        if self.t:
+            self.lib.bt_tracker_destroy(self.t)
+            self.t = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def begin_frame(self, depth_raw, mask, colour, request_out, loader_id: int = 0, first_pose=None):
+        """depth_raw float32 [H,W], mask uint8 [H,W], colour uint8 [H,W,3] BGR, request_out uint8 [400,400,3]: device.  loader_id / first_pose
+        (4x4 cam->model) are used only when the tracker holds no frame.  Returns (status, roi (umin, umax, vmin, vmax))."""
+        roi = np.zeros(4, np.int32)
+        st = ctypes.c_int(-1)
+        fp = None if first_pose is None else np.ascontiguousarray(first_pose, np.float32).reshape(16)
+        _lib.check(self.lib.bt_tracker_begin_frame(self.t, ctypes.c_int(loader_id), None if fp is None else fp.ctypes.data_as(ctypes.c_void_p),
+                                                   ctypes.c_void_p(_ptr(depth_raw)), ctypes.c_void_p(_ptr(mask)), ctypes.c_void_p(_ptr(colour)),
+                                                   ctypes.c_void_p(_ptr(request_out)), roi.ctypes.data_as(ctypes.c_void_p), ctypes.byref(st), self.stream),
+                   "bt_tracker_begin_frame")
+        return st.value, roi
+
+    def end_frame(self, kpts, desc):
+        """kpts: numpy [n,2] float32 image pixels; desc: device float32 [n,256].  Returns (pose [4,4] float32 cam->model, status)."""
+        k = np.ascontiguousarray(kpts, np.float32).reshape(-1, 2)
+        v = _lib.DescView()
+        v.dev, v.n, v.dim = _ptr(desc), int(desc.shape[0]), int(desc.shape[1])
+        v.pitch_bytes = desc.stride(0) * 4 if desc.shape[0] > 1 else desc.shape[1] * 4
+        pose = np.zeros((4, 4), np.float32)
+        st = ctypes.c_int(-1)
+        _lib.check(self.lib.bt_tracker_end_frame(self.t, k.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(len(k)), ctypes.byref(v),
+                                                 pose.ctypes.data_as(ctypes.c_void_p), ctypes.byref(st), self.stream), "bt_tracker_end_frame")
+        return pose, st.value
+
+    def drop_frame(self):
+        """Feature detection failed: the pending frame is FAIL and forgotten.  Returns its pose."""
+        pose = np.zeros((4, 4), np.float32)
+        _lib.check(self.lib.bt_tracker_drop_frame(self.t, pose.ctypes.data_as(ctypes.c_void_p)), "bt_tracker_drop_frame")
+        return pose
+
+    def state(self):
+        """Every frame alive, oldest first: (ids int32 [n], poses float32 [n,4,4], is_keyframe bool [n])."""
+        n = ctypes.c_int(0)
+        cap = self.params.max_frames_alive
+        ids = np.zeros(cap, np.int32)
+        poses = np.zeros((cap, 4, 4), np.float32)
+        kf = np.zeros(cap, np.int32)
+        _lib.check(self.lib.bt_tracker_state(self.t, ids.ctypes.data_as(ctypes.c_void_p), poses.ctypes.data_as(ctypes.c_void_p), kf.ctypes.data_as(ctypes.c_void_p),
+                                             ctypes.c_int(cap), ctypes.byref(n)), "bt_tracker_state")
+        return ids[:n.value].copy(), poses[:n.value].copy(), kf[:n.value].astype(bool)

@@ -442,6 +442,59 @@ BT_API int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_frame* 
                          bt_entryj* entry_out, int entry_capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out,
                          int32_t* status_out, float* uv_out, void* stream);
 
+/* SiftManager::procrustesByCorrespondence (the reference's src/FeatureManager.cpp:523-557) plus the pose update after it (Bundler.cpp:134-135)
+ * on the device, for one pair as bt_find_corres_pairs leaves it: entry_dev / n_entry_dev / status_dev are the pair's EntryJ block (pos_j =
+ * the newer frame A's camera point, pos_i = the older frame B's), its count and its BT_PAIR_* status, all DEVICE memory.  pose_a / pose_b:
+ * HOST row-major cam->model poses of A and B.  src = pose_a * pos_j and dst = pose_b * pos_i per entry, each coordinate
+ * ((m0 x + m1 y) + m2 z) + m3 in float; offset = bt_rigid_transform(src, dst) bit for bit, or the identity when the status is not BT_PAIR_OK;
+ * pose_out_dev (DEVICE, 16 floats) = offset * pose_a, each element ((o0 p0 + o1 p1) + o2 p2) + o3 p3 in float.  Asynchronous; one CTA. */
+BT_API int bt_pose_init(bt_ctx* ctx, const bt_entryj* entry_dev, const int32_t* n_entry_dev, const int32_t* status_dev, const float* pose_a,
+                        const float* pose_b, float* pose_out_dev, void* stream);
+
+/* ---- the whole tracking step: Bundler::processNewFrame (the reference's src/Bundler.cpp:56-183) as one object -------------------------
+ * A tracker owns its own bt_ctx and reserves everything in bt_tracker_create, for frames of H x W with at most max_feats keypoints and
+ * 256-dimensional descriptors: max_frames_alive + 1 sets of full-resolution maps (depth, normals, foreground mask: 25 B per pixel) with their
+ * keypoints and descriptor-pool slots, max_frames_alive frame-cache slots, the device map-point table (max_frames_alive frames, 16 x max_feats
+ * points), the match cache (every pair of max_frames_alive frames, 3 x max_feats entries of 32 B each) and the matcher and solver for
+ * windows of max_BA_frames frames.  At 640 x 480, 2000 features, max_frames_alive = 32 and max_BA_frames = 15 that is roughly 0.6 GB: 0.25 GB
+ * of frame maps, 0.1 GB each of descriptor pool and match cache, the rest matcher and solver scratch.
+ * A frame's step is split where the reference calls the LF-Net server: begin_frame (id, pose, segmentation, the 10-pixel ROI gate and the
+ * request image) and end_frame (descriptors, findCorres on the neighbour pair, the initial pose on the device, the frame deque, keyframe
+ * selection, findCorres on the window, the BA gate, the solve, keyframe admission).  Poses are row-major 4 x 4 cam->model. */
+typedef struct bt_tracker bt_tracker;
+typedef struct {
+	int H, W; float fx, fy, cx, cy;
+	int max_feats;                 /* keypoints per frame */
+	int max_frames_alive;          /* frames held at once during a step: keyframes + the recent-frame deque + the new frame; <= 64 (the device
+	                                * map-point table's limit).  The oldest recent frame is released only after the new frame's neighbour pair is
+	                                * matched, as in the reference, so it counts too. */
+	int mask_mode;                 /* BT_MASK_AS_IS / BT_MASK_LARGEST_HULL */
+	bt_depth_params depth; bt_solver_params solver; bt_prune_params prune;
+	int ransac_trials; float ransac_inlier_dist;
+	int window_size, max_BA_frames, min_fm_edges_newframe, min_feat_num; float min_rot_deg;
+} bt_tracker_params;
+enum { BT_FRAME_OTHER = 0, BT_FRAME_FAIL = 1, BT_FRAME_NO_BA = 2 };   /* Frame::_status */
+/* BT_ERR_NO_DEVICE without an sm_90 GPU; BT_ERR_INVALID_ARG for parameters out of range (max_BA_frames 2..32, max_frames_alive 2..64). */
+BT_API int bt_tracker_create(bt_tracker** out, int device, const bt_tracker_params* p);
+BT_API void bt_tracker_destroy(bt_tracker* t);
+/* The new frame's id and pose: the last frame's id + 1 and its pose when the tracker holds frames, else loader_id and first_pose (identity when
+ * NULL).  depth_raw_dev (float H*W, metres), mask_dev (uint8 H*W, the mask PNG's bytes), colour_dev (uint8 H*W*3 BGR): DEVICE.  Writes the ROI
+ * (umin, umax, vmin, vmax) to roi_out (host, optional) after one synchronisation.  A frame that fails the 10-pixel gate gets BT_FRAME_FAIL: the
+ * tracker keeps nothing of it, so the next frame gets the same id.  Otherwise request_out_dev (DEVICE uint8 400*400*3) receives the LF-Net
+ * request image and *status_out = BT_FRAME_OTHER; finish the frame with end_frame or drop_frame. */
+BT_API int bt_tracker_begin_frame(bt_tracker* t, int loader_id, const float* first_pose, const float* depth_raw_dev, const uint8_t* mask_dev,
+                                  const uint8_t* colour_dev, uint8_t* request_out_dev, int32_t* roi_out, int* status_out, void* stream);
+/* kpts_host: n_kpts x (x, y) image pixels (bt_lfnet_parse_reply's output); desc: the n_kpts x 256 descriptors on the device.  Writes the frame's
+ * pose as Bundler::saveNewframeResult would record it and its status.  BT_ERR_INVALID_ARG without a pending begin_frame, for n_kpts > max_feats
+ * or a NULL argument; BT_ERR_CAPACITY when the frames alive plus the new one exceed max_frames_alive.  Both change nothing: the frame stays
+ * pending. */
+BT_API int bt_tracker_end_frame(bt_tracker* t, const float* kpts_host, int n_kpts, const bt_desc_view* desc, float* pose_out, int* status_out, void* stream);
+/* Lfnet::detectFeature threw: the pending frame becomes FAIL and is forgotten (Bundler.cpp:108-116).  pose_out (optional): its pose. */
+BT_API int bt_tracker_drop_frame(bt_tracker* t, float* pose_out);
+/* Every frame alive (the deque and the keyframes), oldest first: ids, poses (16 floats each) and whether it is a keyframe.  *n = the count;
+ * BT_ERR_CAPACITY when it exceeds cap (the arrays may be NULL when cap is 0). */
+BT_API int bt_tracker_state(bt_tracker* t, int32_t* ids, float* poses, int32_t* is_keyframe, int cap, int* n);
+
 /* Small device-memory helpers so non-CUDA hosts (ctypes, cgo, JNI) can drive the library without another runtime. */
 BT_API int bt_dev_alloc(void** out, size_t bytes);
 BT_API int bt_dev_free(void* p);
