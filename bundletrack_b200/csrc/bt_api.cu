@@ -13,7 +13,7 @@ void set_error(const char* fmt, ...) {
 }  // namespace bt
 
 extern "C" const char* bt_last_error(void) { return bt::g_err; }
-extern "C" int bt_version(void) { return 100; }
+extern "C" int bt_version(void) { return 101; }
 
 extern "C" int bt_ctx_create(bt_ctx** out, int device) {
 	BT_REQUIRE(out != nullptr, BT_ERR_INVALID_ARG, "bt_ctx_create: out is NULL");

@@ -96,6 +96,8 @@ int launch_lfnet_request(const void* const* tbl_dev, const int32_t* roi_dev, int
 void tracks_dev_destroy(bt_ctx* ctx);
 int tracks_slot(bt_ctx* ctx, int frame_id, bool create, int* slot);
 int tracks_free_slots(bt_ctx* ctx);
+// map points alive now (created and not freed by forgets); synchronises `stream`
+int tracks_points_alive(bt_ctx* ctx, cudaStream_t stream, int* n);
 // where an update takes its (uA, vA, uB, vB) list from: entry i = base + stride * (ids ? ids[i] : i) floats.  The count is *n_dev, or, when
 // n_inl is set, pair `pair`'s emitted count (n_inl[pair] < 5 -> 0, clamped to `capacity` behind the earlier pairs) as k_emit_entryj writes it.
 struct TrkSrc { const float* base; int stride; const int32_t* ids; const int32_t* n_dev; int max_n; const int32_t* n_inl; int pair; int capacity; };

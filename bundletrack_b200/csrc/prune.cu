@@ -16,6 +16,7 @@
 //                    (FeatureManager.cpp:233-241,727-730); pairs written back to back, which is the grouping the
 //                    solver's tail wants.
 #include <algorithm>
+#include <climits>
 #include <map>
 #include <vector>
 #include "bt_common.cuh"
@@ -470,7 +471,10 @@ extern "C" int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_fra
 
 // ------------------------------------------------------------------------------------------------ per-pair result cache
 // SiftManager::_matches (/root/reference/src/FeatureManager.cpp:176): a pair is matched once; later windows reuse its matches.  The
-// EntryJ blocks stay on the device in fixed-size slots; the host keeps {slot, count, status} per (idA, idB).
+// EntryJ blocks stay on the device in one arena, each block exactly as long as its pair's entry count; the host keeps {offset, count,
+// status} per (idA, idB).  Blocks are placed at the arena's top; a forgotten block's entries leave the live count at once and its room is
+// reclaimed when a put finds no room at the top: the live blocks then slide down, in offset order, to the arena's start (k_cache_compact),
+// on the put's stream and before the put's own copy.
 namespace bt {
 struct CacheMove { int src, dst, n; uint32_t wi, wj; };      // entries [src, src+n) -> [dst, dst+n); gather rewrites the frame indices
 __global__ void __launch_bounds__(128) k_cache_move(const CacheMove* __restrict__ tab, const bt_entryj* __restrict__ from, bt_entryj* __restrict__ to, int rewrite) {
@@ -481,15 +485,39 @@ __global__ void __launch_bounds__(128) k_cache_move(const CacheMove* __restrict_
 		to[m.dst + i] = e;
 	}
 }
+// In-place compaction: the moves are in ascending source order and every dst <= src, so a block's destination never reaches a source that is
+// still to be read - provided each chunk is read completely before it is written.  One CTA; compaction is rare (only when the top is full).
+constexpr int kCompactThreads = 1024, kCompactUnroll = 4;
+__global__ void __launch_bounds__(kCompactThreads) k_cache_compact(const CacheMove* __restrict__ tab, int n_moves, bt_entryj* arena) {
+	for (int k = 0; k < n_moves; k++) {
+		const CacheMove m = tab[k];
+		if (m.src == m.dst) continue;
+		for (int base = 0; base < m.n; base += kCompactThreads * kCompactUnroll) {
+			bt_entryj e[kCompactUnroll];
+#pragma unroll
+			for (int u = 0; u < kCompactUnroll; u++) {
+				const int i = base + u * kCompactThreads + threadIdx.x;
+				if (i < m.n) e[u] = arena[m.src + i];
+			}
+			__syncthreads();
+#pragma unroll
+			for (int u = 0; u < kCompactUnroll; u++) {
+				const int i = base + u * kCompactThreads + threadIdx.x;
+				if (i < m.n) arena[m.dst + i] = e[u];
+			}
+			__syncthreads();
+		}
+	}
+}
 struct MatchCache {
-	int max_pairs = 0, slot_entries = 0;
+	int max_pairs = 0, max_block = 0;  // pairs cached at once; entries per block (the arena size for bt_match_cache_reserve_entries)
+	long long cap = 0, top = 0, live = 0;   // arena entries: size, end of the last block placed, entries in live blocks
 	DevBuf arena, tab;
 	PinnedBuf h_tab[2];
 	cudaEvent_t ev[2] = { nullptr, nullptr };
 	int flip = 0;
-	struct Rec { int slot, n, status; };
+	struct Rec { long long off; int n, status; };
 	std::map<std::pair<int, int>, Rec> recs;
-	std::vector<int> free_slots;
 };
 void mcache_destroy(bt_ctx* ctx) {
 	MatchCache* c = ctx->mcache;
@@ -508,21 +536,31 @@ static int cache_upload(MatchCache* c, const std::vector<CacheMove>& mv, cudaStr
 	BT_CUDA(cudaEventRecord(c->ev[fl], stream));
 	return BT_OK;
 }
-}  // namespace bt
-
-extern "C" int bt_match_cache_reserve(bt_ctx* ctx, int max_pairs_cached, int max_entries_per_pair) {
-	BT_REQUIRE(ctx && max_pairs_cached > 0 && max_entries_per_pair > 0, BT_ERR_INVALID_ARG, "bt_match_cache_reserve: bad arguments");
+static int cache_reserve(bt_ctx* ctx, int max_pairs_cached, int max_block, long long total) {
 	BT_CUDA(cudaSetDevice(ctx->device));
 	if (!ctx->mcache) ctx->mcache = new MatchCache();
 	MatchCache* c = ctx->mcache;
 	int rc;
-	if ((rc = c->arena.alloc(sizeof(bt_entryj) * (size_t)max_pairs_cached * max_entries_per_pair)) != BT_OK) return rc;
-	if ((rc = c->tab.alloc(sizeof(CacheMove) * (size_t)max_pairs_cached)) != BT_OK) return rc;
-	for (auto& h : c->h_tab) if ((rc = h.alloc(sizeof(CacheMove) * (size_t)max_pairs_cached)) != BT_OK) return rc;
-	c->max_pairs = max_pairs_cached; c->slot_entries = max_entries_per_pair;
-	c->recs.clear(); c->free_slots.clear();
-	for (int k = max_pairs_cached - 1; k >= 0; k--) c->free_slots.push_back(k);
+	if ((rc = c->arena.alloc(sizeof(bt_entryj) * (size_t)total)) != BT_OK) return rc;
+	// a put uploads the compaction (every live block) and its own blocks in one table
+	if ((rc = c->tab.alloc(sizeof(CacheMove) * 2 * (size_t)max_pairs_cached)) != BT_OK) return rc;
+	for (auto& h : c->h_tab) if ((rc = h.alloc(sizeof(CacheMove) * 2 * (size_t)max_pairs_cached)) != BT_OK) return rc;
+	c->max_pairs = max_pairs_cached; c->max_block = max_block;
+	c->cap = total; c->top = 0; c->live = 0;
+	c->recs.clear();
 	return BT_OK;
+}
+}  // namespace bt
+
+extern "C" int bt_match_cache_reserve(bt_ctx* ctx, int max_pairs_cached, int max_entries_per_pair) {
+	BT_REQUIRE(ctx && max_pairs_cached > 0 && max_entries_per_pair > 0, BT_ERR_INVALID_ARG, "bt_match_cache_reserve: bad arguments");
+	return cache_reserve(ctx, max_pairs_cached, max_entries_per_pair, (long long)max_pairs_cached * max_entries_per_pair);
+}
+
+extern "C" int bt_match_cache_reserve_entries(bt_ctx* ctx, int max_pairs_cached, long long max_entries_total) {
+	BT_REQUIRE(ctx && max_pairs_cached > 0 && max_entries_total > 0 && max_entries_total <= INT_MAX, BT_ERR_INVALID_ARG,
+	           "bt_match_cache_reserve_entries: need max_pairs_cached > 0 and 0 < max_entries_total <= %d", INT_MAX);
+	return cache_reserve(ctx, max_pairs_cached, (int)max_entries_total, max_entries_total);
 }
 
 extern "C" int bt_match_cache_put(bt_ctx* ctx, int n_pairs, const int32_t* idA, const int32_t* idB, const bt_entryj* entry_dev,
@@ -531,23 +569,60 @@ extern "C" int bt_match_cache_put(bt_ctx* ctx, int n_pairs, const int32_t* idA, 
 	MatchCache* c = ctx->mcache;
 	BT_REQUIRE(n_pairs <= c->max_pairs, BT_ERR_CAPACITY, "bt_match_cache_put: %d pairs > table of %d", n_pairs, c->max_pairs);
 	BT_CUDA(cudaSetDevice(ctx->device));
-	std::vector<CacheMove> mv;
+	// check everything before changing anything: a refused put leaves the cache as it was.  A pair listed twice keeps its last block.
+	std::map<std::pair<int, int>, int> last;            // pair -> index of its last occurrence in the list
 	for (int p = 0; p < n_pairs; p++) {
 		BT_REQUIRE(idA[p] > idB[p], BT_ERR_INVALID_ARG, "bt_match_cache_put: pair %d: frame A must be the newer frame", p);
-		BT_REQUIRE(n_entry_host[p] >= 0 && n_entry_host[p] <= c->slot_entries, BT_ERR_CAPACITY, "bt_match_cache_put: pair %d has %d entries > slot size %d", p, n_entry_host[p], c->slot_entries);
+		BT_REQUIRE(n_entry_host[p] >= 0 && n_entry_host[p] <= c->max_block, BT_ERR_CAPACITY, "bt_match_cache_put: pair %d has %d entries > block limit %d", p, n_entry_host[p], c->max_block);
+		BT_REQUIRE(n_entry_host[p] == 0 || entry_dev, BT_ERR_INVALID_ARG, "bt_match_cache_put: NULL entry list");
+		last[std::make_pair((int)idA[p], (int)idB[p])] = p;
+	}
+	int new_pairs = 0;
+	long long live = c->live, need = 0;
+	for (const auto& kv : last) {
+		const auto it = c->recs.find(kv.first);
+		if (it == c->recs.end()) new_pairs++;
+		else live -= it->second.n;
+		live += n_entry_host[kv.second];
+		need += n_entry_host[kv.second];
+	}
+	BT_REQUIRE((long long)c->recs.size() + new_pairs <= c->max_pairs, BT_ERR_CAPACITY, "bt_match_cache_put: more than %d pairs cached", c->max_pairs);
+	BT_REQUIRE(live <= c->cap, BT_ERR_CAPACITY, "bt_match_cache_put: %lld live entries > the cache's %lld", live, c->cap);
+	for (const auto& kv : last) {                       // a re-put pair gives its old block back
+		const auto it = c->recs.find(kv.first);
+		if (it != c->recs.end()) { c->live -= it->second.n; c->recs.erase(it); }
+	}
+	std::vector<CacheMove> mv;
+	if (c->top + need > c->cap) {                       // no room at the top: slide the live blocks down in offset order
+		std::vector<MatchCache::Rec*> by_off;
+		by_off.reserve(c->recs.size());
+		for (auto& kv : c->recs) if (kv.second.n > 0) by_off.push_back(&kv.second);
+		std::sort(by_off.begin(), by_off.end(), [](const MatchCache::Rec* a, const MatchCache::Rec* b) { return a->off < b->off; });
+		long long off = 0;
+		for (MatchCache::Rec* r : by_off) {
+			mv.push_back(CacheMove{ (int)r->off, (int)off, r->n, 0u, 0u });
+			r->off = off;
+			off += r->n;
+		}
+		c->top = off;
+	}
+	const int n_compact = (int)mv.size();
+	for (int p = 0; p < n_pairs; p++) {
 		const auto key = std::make_pair((int)idA[p], (int)idB[p]);
-		auto it = c->recs.find(key);
-		int slot;
-		if (it != c->recs.end()) slot = it->second.slot;
-		else { BT_REQUIRE(!c->free_slots.empty(), BT_ERR_CAPACITY, "bt_match_cache_put: all %d slots are in use", c->max_pairs); slot = c->free_slots.back(); c->free_slots.pop_back(); }
-		c->recs[key] = MatchCache::Rec{ slot, n_entry_host[p], status_host ? status_host[p] : (n_entry_host[p] > 0 ? BT_PAIR_OK : BT_PAIR_EMPTY) };
-		if (n_entry_host[p] > 0) { BT_REQUIRE(entry_dev, BT_ERR_INVALID_ARG, "bt_match_cache_put: NULL entry list"); mv.push_back(CacheMove{ entry_off_host[p], slot * c->slot_entries, n_entry_host[p], 0u, 0u }); }
+		if (last[key] != p) continue;
+		const int n = n_entry_host[p];
+		c->recs[key] = MatchCache::Rec{ c->top, n, status_host ? status_host[p] : (n > 0 ? BT_PAIR_OK : BT_PAIR_EMPTY) };
+		if (n > 0) mv.push_back(CacheMove{ entry_off_host[p], (int)c->top, n, 0u, 0u });
+		c->top += n;
+		c->live += n;
 	}
 	if (mv.empty()) return BT_OK;
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc = cache_upload(c, mv, stream);
 	if (rc != BT_OK) return rc;
-	k_cache_move<<<(unsigned)mv.size(), 128, 0, stream>>>(c->tab.as<CacheMove>(), entry_dev, c->arena.as<bt_entryj>(), 0);
+	if (n_compact > 0) k_cache_compact<<<1, kCompactThreads, 0, stream>>>(c->tab.as<CacheMove>(), n_compact, c->arena.as<bt_entryj>());
+	if ((int)mv.size() > n_compact)
+		k_cache_move<<<(unsigned)mv.size() - n_compact, 128, 0, stream>>>(c->tab.as<CacheMove>() + n_compact, entry_dev, c->arena.as<bt_entryj>(), 0);
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;
 }
@@ -566,6 +641,13 @@ extern "C" int bt_match_cache_status(bt_ctx* ctx, int idA, int idB, int* n_entry
 	return BT_OK;
 }
 
+extern "C" int bt_match_cache_usage(bt_ctx* ctx, int* n_pairs, long long* n_entries) {
+	BT_REQUIRE(ctx && ctx->mcache && n_pairs && n_entries, BT_ERR_INVALID_ARG, "bt_match_cache_usage: call bt_match_cache_reserve first / NULL argument");
+	*n_pairs = (int)ctx->mcache->recs.size();
+	*n_entries = ctx->mcache->live;
+	return BT_OK;
+}
+
 extern "C" int bt_match_cache_gather(bt_ctx* ctx, int n_pairs, const int32_t* idA, const int32_t* idB, const uint32_t* win_i, const uint32_t* win_j,
                                      bt_entryj* dst_dev, int capacity, int32_t* block_off_host, int32_t* block_n_host, void* stream_) {
 	BT_REQUIRE(ctx && ctx->mcache && idA && idB && win_i && win_j && dst_dev && block_off_host && block_n_host && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_match_cache_gather: NULL argument");
@@ -580,7 +662,7 @@ extern "C" int bt_match_cache_gather(bt_ctx* ctx, int n_pairs, const int32_t* id
 		const int n = it->second.n;
 		BT_REQUIRE(off + n <= capacity, BT_ERR_CAPACITY, "bt_match_cache_gather: %d entries > capacity %d", off + n, capacity);
 		block_off_host[p] = off; block_n_host[p] = n;
-		if (n > 0) mv.push_back(CacheMove{ it->second.slot * c->slot_entries, off, n, win_i[p], win_j[p] });
+		if (n > 0) mv.push_back(CacheMove{ (int)it->second.off, off, n, win_i[p], win_j[p] });
 		off += n;
 	}
 	if (mv.empty()) return BT_OK;
@@ -596,7 +678,7 @@ extern "C" int bt_match_cache_forget_frame(bt_ctx* ctx, int frame_id) {
 	BT_REQUIRE(ctx && ctx->mcache, BT_ERR_INVALID_ARG, "bt_match_cache_forget_frame: call bt_match_cache_reserve first");
 	MatchCache* c = ctx->mcache;
 	for (auto it = c->recs.begin(); it != c->recs.end();) {
-		if (it->first.first == frame_id || it->first.second == frame_id) { c->free_slots.push_back(it->second.slot); it = c->recs.erase(it); }
+		if (it->first.first == frame_id || it->first.second == frame_id) { c->live -= it->second.n; it = c->recs.erase(it); }
 		else ++it;
 	}
 	return BT_OK;

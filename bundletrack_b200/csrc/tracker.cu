@@ -18,6 +18,7 @@ namespace bt {
 
 constexpr int kPoseInitThreads = 256;
 constexpr int kDescDim = 256;          // LF-Net descriptors
+constexpr int kMaxKeyframes = 1024;    // bt_tracker_params::max_keyframes; with max_frames_alive <= 64 the map-point table's bt_tracks_dev_reserve_ex limit
 struct PoseInitArgs { float A[16], B[16]; };
 
 // pcl::transformPointWithNormal's point part, ((m0 x + m1 y) + m2 z) + m3 per coordinate, each operation rounded on its own
@@ -178,11 +179,18 @@ static int tr_put(bt_tracker* t, const std::vector<std::pair<const TFrame*, cons
 	return bt_match_cache_put(t->ctx, n, ia.data(), ib.data(), t->entries.as<bt_entryj>(), h, h + n, h + 2 * n, stream);
 }
 
+// the keyframe pool's match-cache budget (the header states it): max_BA_frames / 2 worst-case blocks of 3 x max_feats entries per frame slot.
+// A frame's cached pairs are those of the windows it was new in, with at most max_BA_frames - 1 older frames each.
+static long long tr_cache_budget(const bt_tracker_params* p) {
+	return (long long)(p->max_frames_alive + p->max_keyframes) * p->max_BA_frames * 3 * p->max_feats / 2;
+}
+
 extern "C" int bt_tracker_create(bt_tracker** out, int device, const bt_tracker_params* p) {
 	BT_REQUIRE(out && p, BT_ERR_INVALID_ARG, "bt_tracker_create: NULL argument");
 	*out = nullptr;
 	BT_REQUIRE(p->H > 0 && p->W > 0 && p->max_feats > 0 && p->max_feats <= 8192 && p->max_frames_alive >= 2 && p->max_frames_alive <= 64, BT_ERR_INVALID_ARG,
 	           "bt_tracker_create: bad sizes (max_feats 1..8192, max_frames_alive 2..64)");
+	BT_REQUIRE(p->max_keyframes >= 0 && p->max_keyframes <= kMaxKeyframes, BT_ERR_INVALID_ARG, "bt_tracker_create: max_keyframes 0..%d", kMaxKeyframes);
 	BT_REQUIRE(p->max_BA_frames >= 2 && p->max_BA_frames <= 32 && p->window_size >= 0 && p->ransac_trials >= 1 &&
 	           (p->mask_mode == BT_MASK_AS_IS || p->mask_mode == BT_MASK_LARGEST_HULL), BT_ERR_INVALID_ARG,
 	           "bt_tracker_create: bad parameters (max_BA_frames 2..32, window_size >= 0, ransac_trials >= 1, mask_mode)");
@@ -192,20 +200,21 @@ extern "C" int bt_tracker_create(bt_tracker** out, int device, const bt_tracker_
 	bt_tracker* t = new bt_tracker();
 	t->ctx = ctx;
 	t->p = *p;
-	t->n_slots = p->max_frames_alive + 1;                  // + the frame between begin_frame and end_frame
+	const int F = p->max_frames_alive + p->max_keyframes;    // frames with maps at once (max_keyframes = 0: max_frames_alive counts keyframes too)
+	t->n_slots = F + 1;                                    // + the frame between begin_frame and end_frame
 	t->max_pairs = p->max_BA_frames * (p->max_BA_frames - 1) / 2;
 	t->slot_entries = 3 * p->max_feats;
 	t->win_entries = t->max_pairs * t->slot_entries;
 	t->hw = (size_t)p->H * p->W;
-	const int F = p->max_frames_alive;
 	const bt_solver_limits lim = { 1, p->max_BA_frames, t->win_entries, p->H, p->W, p->solver.image_downscale };
 #define TRY(x) if ((rc = (x)) != BT_OK) { bt_tracker_destroy(t); return rc; }
 	TRY(bt_solver_reserve(ctx, &lim));
 	TRY(bt_frame_cache_reserve(ctx, F, p->H, p->W, p->solver.image_downscale));
 	TRY(bt_pipeline_reserve(ctx, t->max_pairs, p->max_feats, kDescDim, p->ransac_trials));
 	TRY(bt_desc_pool_reserve(ctx, t->n_slots));
-	TRY(bt_tracks_dev_reserve(ctx, F, p->max_feats, 16 * p->max_feats));
-	TRY(bt_match_cache_reserve(ctx, F * (F - 1) / 2, t->slot_entries));
+	TRY(bt_tracks_dev_reserve_ex(ctx, F, p->max_feats, 16 * p->max_feats * ((F + 63) / 64)));
+	TRY(p->max_keyframes == 0 ? bt_match_cache_reserve(ctx, F * (F - 1) / 2, t->slot_entries)
+	                          : bt_match_cache_reserve_entries(ctx, F * (F - 1) / 2, tr_cache_budget(p)));
 	TRY(t->depth.alloc(sizeof(float) * t->hw * t->n_slots));
 	TRY(t->normal.alloc(4 * sizeof(float) * t->hw * t->n_slots));
 	TRY(t->fg.alloc(t->hw * t->n_slots));
@@ -296,8 +305,15 @@ extern "C" int bt_tracker_end_frame(bt_tracker* t, const float* kpts_host, int n
 	BT_REQUIRE(n_kpts >= 0 && n_kpts <= p.max_feats, BT_ERR_INVALID_ARG, "bt_tracker_end_frame: %d keypoints, the tracker was created for %d", n_kpts, p.max_feats);
 	BT_REQUIRE((n_kpts == 0 || (kpts_host && desc->dev)) && desc->n == n_kpts && desc->dim == kDescDim, BT_ERR_INVALID_ARG,
 	           "bt_tracker_end_frame: the descriptor view must hold n_kpts rows of %d floats", kDescDim);
-	BT_REQUIRE((int)t->alive.size() + 1 <= p.max_frames_alive, BT_ERR_CAPACITY, "bt_tracker_end_frame: %d frames alive + the new one > max_frames_alive %d",
-	           (int)t->alive.size(), p.max_frames_alive);
+	if (p.max_keyframes == 0) {
+		BT_REQUIRE((int)t->alive.size() + 1 <= p.max_frames_alive, BT_ERR_CAPACITY, "bt_tracker_end_frame: %d frames alive + the new one > max_frames_alive %d",
+		           (int)t->alive.size(), p.max_frames_alive);
+	} else {                                               // the new frame may become a keyframe: the pool must have room for it
+		const int n_kf = (int)t->keyframes.size(), n_other = (int)t->alive.size() - n_kf;
+		BT_REQUIRE(n_other + 1 <= p.max_frames_alive, BT_ERR_CAPACITY, "bt_tracker_end_frame: %d frames alive that are not keyframes + the new one > max_frames_alive %d",
+		           n_other, p.max_frames_alive);
+		BT_REQUIRE(n_kf < p.max_keyframes, BT_ERR_CAPACITY, "bt_tracker_end_frame: the keyframe pool is full (%d keyframes)", n_kf);
+	}
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(t->ctx->device));
 	TFrame f = t->pend;
@@ -434,4 +450,12 @@ extern "C" int bt_tracker_state(bt_tracker* t, int32_t* ids, float* poses, int32
 		k++;
 	}
 	return BT_OK;
+}
+
+extern "C" int bt_tracker_usage(bt_tracker* t, int* n_points, int* n_pairs_cached, long long* n_entries_cached, void* stream) {
+	BT_REQUIRE(t && n_points && n_pairs_cached && n_entries_cached, BT_ERR_INVALID_ARG, "bt_tracker_usage: NULL argument");
+	BT_CUDA(cudaSetDevice(t->ctx->device));
+	int rc = tracks_points_alive(t->ctx, (cudaStream_t)stream, n_points);
+	if (rc != BT_OK) return rc;
+	return bt_match_cache_usage(t->ctx, n_pairs_cached, n_entries_cached);
 }

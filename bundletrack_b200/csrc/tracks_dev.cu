@@ -4,13 +4,15 @@
 //   SiftManager::findCorresByMapPoints      /root/reference/src/FeatureManager.cpp:489-520
 //   SiftManager::forgetFrame (map points)   /root/reference/src/FeatureManager.cpp:163-169
 //
-// Layout (every capacity fixed by bt_tracks_dev_reserve; nothing is allocated on the call path):
+// Layout (every capacity fixed by bt_tracks_dev_reserve / _ex; nothing is allocated on the call path):
 //   frame slot f (the host maps frame ids to slots):  keys[f][0, n_keys[f])  {u bits, v bits, point id, 0} in insertion order, the bits
 //                          the key was FIRST inserted with; an open-addressing hash (normalised key -> index into keys[f]).  A key is
 //                          normalised by turning -0 into +0, so keys compare as floats compare, as std::map<std::pair<float,float>> does.
-//   point p:               obs[p][f] = (u, v) of its observation in slot f (the bits last assigned), valid where bit f of mask[p] is set.
-//                          A point whose mask drops to 0 (forget) is unreferenced - no frame map can point at it - and its id is reused;
-//                          `created` still counts every point ever made, as the host's vector does.
+//   point p:               obs[f][p] = (u, v) of its observation in slot f (the bits last assigned), or the all-ones pattern (a NaN key,
+//                          which never occurs) where the point is not seen in slot f; n_obs[p] = how many slots see it.  Slot-major, so
+//                          forget reads one slot's column contiguously.  A point whose count drops to 0 (forget) is unreferenced - no
+//                          frame map can point at it - and its id is reused; `created` still counts every point ever made, as the host's
+//                          vector does.  The observations take max_points x max_frames x 8 B.
 // A capacity overflow never writes: the kernel leaves the table as it was and latches a flag that bt_tracks_dev_stats reports.
 //
 // k_trk_update applies one pair's list with the order dependence resolved in closed form.  Walking the list in order, entry i is skipped
@@ -26,7 +28,8 @@ namespace bt {
 
 static constexpr unsigned long long kTrkEmpty = ~0ull;   // normalised (NaN, NaN): never a key
 static constexpr int kTrkThreads = 1024;
-static constexpr int kTrkMaxFrames = 64;                  // one bit per frame slot in a point's mask
+static constexpr int kTrkMaxFrames = 64;                  // bt_tracks_dev_reserve's documented range
+static constexpr int kTrkMaxFramesEx = 64 + 1024;         // bt_tracks_dev_reserve_ex: a tracker's frames alive plus its largest keyframe pool
 static constexpr int kTrkMaxKeys = 8192;                  // propagate sorts a frame's keys in shared memory
 
 struct TrkTable {
@@ -34,8 +37,8 @@ struct TrkTable {
 	unsigned long long* hkey;      // [max_frames][hcap] normalised key or kTrkEmpty
 	int* hidx;                     // [max_frames][hcap] index into keys
 	int* n_keys;                   // [max_frames]
-	float2* obs;                   // [max_points][max_frames]
-	unsigned long long* mask;      // [max_points]
+	float2* obs;                   // [max_frames][max_points], kTrkEmpty bits where the point is not seen in the slot
+	int* n_obs;                    // [max_points] slots that see the point
 	unsigned long long* last;      // [max_points] (epoch << 32 | entry) of the last writer of the point's observation in A
 	int* free_pts;                 // [max_points] ids of dead points
 	int* ctr;                      // created, next unused id, n free, n observations, overflow flag
@@ -51,6 +54,9 @@ __device__ __forceinline__ unsigned norm_bits(float x) { const unsigned b = __fl
 __device__ __forceinline__ unsigned long long norm_key(float u, float v) { return ((unsigned long long)norm_bits(u) << 32) | norm_bits(v); }
 __device__ __forceinline__ unsigned ord_bits(unsigned b) { return (b & 0x80000000u) ? ~b : (b | 0x80000000u); }   // float order as unsigned order
 __device__ __forceinline__ unsigned long long ord_key(unsigned long long k) { return ((unsigned long long)ord_bits((unsigned)(k >> 32)) << 32) | ord_bits((unsigned)k); }
+__device__ __forceinline__ float2* obs_at(const TrkTable& t, int p, int f) { return t.obs + (size_t)f * t.max_points + p; }
+__device__ __forceinline__ bool obs_seen(float2 o) { return !(__float_as_uint(o.x) == 0xffffffffu && __float_as_uint(o.y) == 0xffffffffu); }
+__device__ __forceinline__ float2 obs_empty() { return make_float2(__uint_as_float(0xffffffffu), __uint_as_float(0xffffffffu)); }
 __device__ __forceinline__ unsigned hmix(unsigned long long k) {
 	k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
 	return (unsigned)k;
@@ -180,16 +186,15 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_update(TrkTable t, int sa, 
 	}
 	__syncthreads();
 	if (!s_ok) return;
-	const unsigned long long bitA = 1ull << sa, bitB = 1ull << sb;
-	// 3: new points, anchored at B
+	// 3: new points, anchored at B (a reused id was forgotten in every slot: its column entries are all empty)
 	for (int i = tid; i < n; i += blockDim.x) {
 		const TrkEnt e = ent[i];
 		if (!(e.flags & E_CREATE)) continue;
 		const int id = e.rc < s_nfree ? t.free_pts[s_nfree - 1 - e.rc] : s_next + (e.rc - s_nfree);
 		ent[i].id = id;
 		const float4 uv = src_uv(src, i);
-		t.obs[(size_t)id * t.max_frames + sb] = make_float2(uv.z, uv.w);
-		t.mask[id] = bitB;
+		*obs_at(t, id, sb) = make_float2(uv.z, uv.w);
+		t.n_obs[id] = 1;
 		t.keys[(size_t)sb * t.max_keys + s_nkB + e.rc] = make_int4(__float_as_int(uv.z), __float_as_int(uv.w), id, 0);
 		frame_insert(t, sb, norm_key(uv.z, uv.w), s_nkB + e.rc);
 	}
@@ -222,9 +227,9 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_update(TrkTable t, int sa, 
 			}
 		}
 		if (t.last[e.id] == (((unsigned long long)epoch << 32) | (unsigned)i)) {
-			t.obs[(size_t)e.id * t.max_frames + sa] = make_float2(uv.x, uv.y);
-			const unsigned long long m = t.mask[e.id];
-			if (!(m & bitA)) { t.mask[e.id] = m | bitA; add_obs++; }
+			float2* o = obs_at(t, e.id, sa);         // (one last writer per point: no other thread touches the point here)
+			if (!obs_seen(*o)) { t.n_obs[e.id]++; add_obs++; }
+			*o = make_float2(uv.x, uv.y);
 		}
 	}
 	int tot;
@@ -255,13 +260,12 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_propagate(TrkTable t, int s
 	unsigned char* s_drop = reinterpret_cast<unsigned char*>(s_ord + t.sort_cap);
 	if (tid == 0) s_m = 0;
 	__syncthreads();
-	const unsigned long long bitB = 1ull << sb;
 	for (int k = tid; k < P; k += blockDim.x) {
 		unsigned long long key = kTrkEmpty;
 		if (k < nk) {
 			const int4 e = t.keys[(size_t)sa * t.max_keys + k];
-			if (t.mask[e.z] & bitB) {
-				const float2 ob = t.obs[(size_t)e.z * t.max_frames + sb];
+			const float2 ob = *obs_at(t, e.z, sb);
+			if (obs_seen(ob)) {
 				const float uA = __int_as_float(e.x), vA = __int_as_float(e.y);
 				bool keep = true;
 				for (int j = 0; j < n_existing && keep; j++) {
@@ -294,7 +298,7 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_propagate(TrkTable t, int s
 	for (int k = tid; k < P; k += blockDim.x) {
 		unsigned long long key = kTrkEmpty;
 		if (k < m) {
-			const float2 ob = t.obs[(size_t)t.keys[(size_t)sa * t.max_keys + s_ord[k]].z * t.max_frames + sb];
+			const float2 ob = *obs_at(t, t.keys[(size_t)sa * t.max_keys + s_ord[k]].z, sb);
 			key = ord_key(norm_key(ob.x, ob.y));
 		}
 		s_key[k] = key; s_pay[k] = k; s_drop[k] = 0;
@@ -324,7 +328,7 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_propagate(TrkTable t, int s
 		if (keep) {
 			if (r < capacity) {
 				const int4 e = t.keys[(size_t)sa * t.max_keys + s_ord[k]];
-				const float2 ob = t.obs[(size_t)e.z * t.max_frames + sb];
+				const float2 ob = *obs_at(t, e.z, sb);
 				out[r] = make_float4(__int_as_float(e.x), __int_as_float(e.y), ob.x, ob.y);
 			} else {
 				t.ctr[C_OVERFLOW] = 1;
@@ -337,15 +341,16 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_propagate(TrkTable t, int s
 
 // forgetFrame: the slot's observations leave every point; points left with none are free for reuse; the slot's map is emptied
 __global__ void __launch_bounds__(256) k_trk_forget(TrkTable t, int slot) {
-	const unsigned long long bit = 1ull << slot;
 	const int next = t.ctr[C_NEXT];
 	const int stride = gridDim.x * blockDim.x;
 	for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < next; p += stride) {
-		const unsigned long long m = t.mask[p];
-		if (!(m & bit)) continue;
-		t.mask[p] = m & ~bit;
+		float2* o = obs_at(t, p, slot);
+		if (!obs_seen(*o)) continue;
+		*o = obs_empty();
 		atomicSub(t.ctr + C_NOBS, 1);
-		if ((m & ~bit) == 0ull) t.free_pts[atomicAdd(t.ctr + C_NFREE, 1)] = p;
+		const int left = t.n_obs[p] - 1;         // (one thread per point)
+		t.n_obs[p] = left;
+		if (left == 0) t.free_pts[atomicAdd(t.ctr + C_NFREE, 1)] = p;
 	}
 	for (int h = blockIdx.x * blockDim.x + threadIdx.x; h < t.hcap; h += stride) t.hkey[(size_t)slot * t.hcap + h] = kTrkEmpty;
 	if (blockIdx.x == 0 && threadIdx.x == 0) t.n_keys[slot] = 0;
@@ -354,7 +359,7 @@ __global__ void __launch_bounds__(256) k_trk_forget(TrkTable t, int slot) {
 struct TracksDev {
 	TrkTable t{};
 	int list_cap = 0, scap = 0;
-	DevBuf keys, hkey, hidx, n_keys, obs, mask, last, free_pts, ctr, shk, smn, smx, ent;
+	DevBuf keys, hkey, hidx, n_keys, obs, n_obs, last, free_pts, ctr, shk, smn, smx, ent;
 	std::map<int, int> slot_of;          // frame id -> slot
 	std::vector<int> free_slots;
 	unsigned epoch = 0;
@@ -364,7 +369,7 @@ struct TracksDev {
 void tracks_dev_destroy(bt_ctx* ctx) {
 	TracksDev* d = ctx->tracks;
 	if (!d) return;
-	DevBuf* bufs[] = { &d->keys, &d->hkey, &d->hidx, &d->n_keys, &d->obs, &d->mask, &d->last, &d->free_pts, &d->ctr, &d->shk, &d->smn, &d->smx, &d->ent };
+	DevBuf* bufs[] = { &d->keys, &d->hkey, &d->hidx, &d->n_keys, &d->obs, &d->n_obs, &d->last, &d->free_pts, &d->ctr, &d->shk, &d->smn, &d->smx, &d->ent };
 	for (DevBuf* b : bufs) b->release();
 	delete d;
 	ctx->tracks = nullptr;
@@ -384,6 +389,14 @@ int tracks_slot(bt_ctx* ctx, int frame_id, bool create, int* slot) {
 }
 
 int tracks_free_slots(bt_ctx* ctx) { return (int)ctx->tracks->free_slots.size(); }
+
+int tracks_points_alive(bt_ctx* ctx, cudaStream_t stream, int* n) {
+	int c[C_N];
+	BT_CUDA(cudaMemcpyAsync(c, ctx->tracks->ctr.p, sizeof(c), cudaMemcpyDeviceToHost, stream));
+	BT_CUDA(cudaStreamSynchronize(stream));
+	*n = c[C_NEXT] - c[C_NFREE];
+	return BT_OK;
+}
 
 int tracks_launch_update(bt_ctx* ctx, int slot_a, int slot_b, const TrkSrc& src, cudaStream_t stream) {
 	TracksDev* d = ctx->tracks;
@@ -406,9 +419,7 @@ int tracks_launch_propagate(bt_ctx* ctx, int slot_a, int slot_b, const float4* e
 
 using namespace bt;
 
-extern "C" int bt_tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_per_frame, int max_points) {
-	BT_REQUIRE(ctx && max_frames > 0 && max_frames <= kTrkMaxFrames && max_keys_per_frame > 0 && max_keys_per_frame <= kTrkMaxKeys && max_points > 0,
-	           BT_ERR_INVALID_ARG, "bt_tracks_dev_reserve: need 0 < max_frames <= %d, 0 < max_keys_per_frame <= %d, max_points > 0", kTrkMaxFrames, kTrkMaxKeys);
+static int tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_per_frame, int max_points) {
 	BT_CUDA(cudaSetDevice(ctx->device));
 	if (!ctx->tracks) ctx->tracks = new TracksDev();
 	TracksDev* d = ctx->tracks;
@@ -421,20 +432,21 @@ extern "C" int bt_tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_p
 	int rc;
 #define RES(buf, bytes) if ((rc = d->buf.alloc(bytes)) != BT_OK) return rc
 	RES(keys, sizeof(int4) * F * K); RES(hkey, sizeof(unsigned long long) * F * hcap); RES(hidx, sizeof(int) * F * hcap); RES(n_keys, sizeof(int) * F);
-	RES(obs, sizeof(float2) * Pn * F); RES(mask, sizeof(unsigned long long) * Pn); RES(last, sizeof(unsigned long long) * Pn); RES(free_pts, sizeof(int) * Pn);
+	RES(obs, sizeof(float2) * Pn * F); RES(n_obs, sizeof(int) * Pn); RES(last, sizeof(unsigned long long) * Pn); RES(free_pts, sizeof(int) * Pn);
 	RES(ctr, sizeof(int) * C_N);
 	RES(shk, sizeof(unsigned long long) * 2 * d->scap); RES(smn, sizeof(int) * 2 * d->scap); RES(smx, sizeof(int) * d->scap);
 	RES(ent, sizeof(TrkEnt) * d->list_cap);
 #undef RES
 	BT_CUDA(cudaMemset(d->hkey.p, 0xff, sizeof(unsigned long long) * F * hcap));
 	BT_CUDA(cudaMemset(d->n_keys.p, 0, sizeof(int) * F));
-	BT_CUDA(cudaMemset(d->mask.p, 0, sizeof(unsigned long long) * Pn));
+	BT_CUDA(cudaMemset(d->obs.p, 0xff, sizeof(float2) * Pn * F));        // every observation empty
+	BT_CUDA(cudaMemset(d->n_obs.p, 0, sizeof(int) * Pn));
 	BT_CUDA(cudaMemset(d->last.p, 0, sizeof(unsigned long long) * Pn));
 	BT_CUDA(cudaMemset(d->ctr.p, 0, sizeof(int) * C_N));
 	BT_CUDA(cudaDeviceSynchronize());
 	TrkTable& t = d->t;
 	t.keys = d->keys.as<int4>(); t.hkey = d->hkey.as<unsigned long long>(); t.hidx = d->hidx.as<int>(); t.n_keys = d->n_keys.as<int>();
-	t.obs = d->obs.as<float2>(); t.mask = d->mask.as<unsigned long long>(); t.last = d->last.as<unsigned long long>(); t.free_pts = d->free_pts.as<int>();
+	t.obs = d->obs.as<float2>(); t.n_obs = d->n_obs.as<int>(); t.last = d->last.as<unsigned long long>(); t.free_pts = d->free_pts.as<int>();
 	t.ctr = d->ctr.as<int>();
 	t.max_frames = max_frames; t.max_keys = max_keys_per_frame; t.hcap = hcap; t.max_points = max_points;
 	t.sort_cap = 1;
@@ -445,6 +457,19 @@ extern "C" int bt_tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_p
 	d->prop_smem = (size_t)t.sort_cap * (sizeof(unsigned long long) + 2 * sizeof(int) + 1);
 	BT_CUDA(cudaFuncSetAttribute(k_trk_propagate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d->prop_smem));
 	return BT_OK;
+}
+
+extern "C" int bt_tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_per_frame, int max_points) {
+	BT_REQUIRE(ctx && max_frames > 0 && max_frames <= kTrkMaxFrames && max_keys_per_frame > 0 && max_keys_per_frame <= kTrkMaxKeys && max_points > 0,
+	           BT_ERR_INVALID_ARG, "bt_tracks_dev_reserve: need 0 < max_frames <= %d, 0 < max_keys_per_frame <= %d, max_points > 0", kTrkMaxFrames, kTrkMaxKeys);
+	return tracks_dev_reserve(ctx, max_frames, max_keys_per_frame, max_points);
+}
+
+extern "C" int bt_tracks_dev_reserve_ex(bt_ctx* ctx, int max_frames, int max_keys_per_frame, int max_points) {
+	BT_REQUIRE(ctx && max_frames > 0 && max_frames <= kTrkMaxFramesEx && max_keys_per_frame > 0 && max_keys_per_frame <= kTrkMaxKeys && max_points > 0,
+	           BT_ERR_INVALID_ARG, "bt_tracks_dev_reserve_ex: need 0 < max_frames <= %d, 0 < max_keys_per_frame <= %d, max_points > 0", kTrkMaxFramesEx,
+	           kTrkMaxKeys);
+	return tracks_dev_reserve(ctx, max_frames, max_keys_per_frame, max_points);
 }
 
 extern "C" int bt_tracks_dev_update_pair(bt_ctx* ctx, int frame_a, int frame_b, const float* uv_dev, const int32_t* n_dev, int uv_capacity, void* stream_) {

@@ -275,9 +275,10 @@ class MatchPipeline:
 class DeviceTracks:
     """The map-point table on the device (bt_tracks_dev_*), owned by a context: the methods of policy.Tracks with the same results,
     host arrays in and out.  FindCorres keeps one; bt_find_corres_pairs reads and updates it without leaving the device.
-    Capacities: frames alive (<= 64), keys per frame (<= 8192), map points alive (default 16 x max_keys_per_frame).  The table takes
-    about max_points x max_frames x 8 B for the observations plus max_frames x max_keys_per_frame x 48 B for the frame maps: 34 MB and
-    13 MB at the defaults.  All work, including the uploads and read-backs of the methods below, runs on `stream`."""
+    Capacities: frames alive (<= 64 + 1024, bt_tracks_dev_reserve_ex), keys per frame (<= 8192), map points alive (default
+    16 x max_keys_per_frame x ceil(max_frames / 64)).  The table takes max_points x max_frames x 8 B for the observations plus
+    max_frames x max_keys_per_frame x 48 B for the frame maps: 34 MB and 13 MB at the defaults, 0.34 GB and 25 MB at 264 frames of 2000 keys.
+    All work, including the uploads and read-backs of the methods below, runs on `stream`."""
 
     def __init__(self, ctx=None, device: int = 0, max_frames: int = 64, max_keys_per_frame: int = 4096, max_points: int = 0, stream: int = 0):
         self.lib = _lib.load()
@@ -287,8 +288,9 @@ class DeviceTracks:
         if self._own:
             _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
         self.device = device
-        _lib.check(self.lib.bt_tracks_dev_reserve(self.ctx, ctypes.c_int(max_frames), ctypes.c_int(max_keys_per_frame),
-                                                  ctypes.c_int(max_points or 16 * max_keys_per_frame)), "bt_tracks_dev_reserve")
+        max_points = max_points or 16 * max_keys_per_frame * -(-max_frames // 64)
+        _lib.check(self.lib.bt_tracks_dev_reserve_ex(self.ctx, ctypes.c_int(max_frames), ctypes.c_int(max_keys_per_frame), ctypes.c_int(max_points)),
+                   "bt_tracks_dev_reserve_ex")
 
     def close(self):
         if self._own and self.ctx:
@@ -352,15 +354,22 @@ class FindCorres:
     """`SiftManager::findCorres` (/root/reference/src/FeatureManager.cpp:173-242) on the device-resident chain: per pair (A newer)
     kNN both ways -> prune -> mutual union -> [non-neighbour: map-point propagation] -> RANSAC -> EntryJ, with the `_matches` cache
     (a pair is matched once), the map-point table on the device (`tracks`, a DeviceTracks: max_frames alive, max_points map points,
-    default 16 x the pipeline's max_feats; see DeviceTracks for its memory) and the Frame::FAIL outcome.  Descriptors live in the pool."""
+    default 16 x the pipeline's max_feats x ceil(max_frames / 64); see DeviceTracks for its memory) and the Frame::FAIL outcome.  Descriptors
+    live in the pool.  The cache's arena holds max_entries_total entries of 32 B (None: max_pairs_cached x max_entries_per_pair, each pair
+    at most max_entries_per_pair; bt_match_cache_reserve / _reserve_entries)."""
 
-    def __init__(self, pipeline: "MatchPipeline", max_pairs_cached: int = 512, max_entries_per_pair: int = 0, max_frames: int = 64, max_points: int = 0):
+    def __init__(self, pipeline: "MatchPipeline", max_pairs_cached: int = 512, max_entries_per_pair: int = 0, max_frames: int = 64, max_points: int = 0,
+                 max_entries_total: int = None):
         self.mp = pipeline
         self.lib = pipeline.lib
         self.ctx = pipeline.ctx
         self.tracks = DeviceTracks(ctx=pipeline.ctx, max_frames=max_frames, max_keys_per_frame=pipeline.max_feats, max_points=max_points, stream=pipeline.stream.value or 0)
         self.slot_entries = max_entries_per_pair or 3 * pipeline.max_feats
-        _lib.check(self.lib.bt_match_cache_reserve(self.ctx, ctypes.c_int(max_pairs_cached), ctypes.c_int(self.slot_entries)), "bt_match_cache_reserve")
+        if max_entries_total is None:
+            _lib.check(self.lib.bt_match_cache_reserve(self.ctx, ctypes.c_int(max_pairs_cached), ctypes.c_int(self.slot_entries)), "bt_match_cache_reserve")
+        else:
+            _lib.check(self.lib.bt_match_cache_reserve_entries(self.ctx, ctypes.c_int(max_pairs_cached), ctypes.c_longlong(max_entries_total)),
+                       "bt_match_cache_reserve_entries")
         self.failed = set()          # ids of frames the reference would mark Frame::FAIL
 
     def has(self, id_a: int, id_b: int) -> bool:

@@ -13,16 +13,17 @@ from . import _lib
 from .config import depth_params, load_yml, mask_mode, prune_params, solver_params
 
 
-def tracker_params(yml, H: int, W: int, K, max_feats: int, max_frames_alive: int, mode: int = None) -> "_lib.TrackerParams":
+def tracker_params(yml, H: int, W: int, K, max_feats: int, max_frames_alive: int, mode: int = None, max_keyframes: int = 0) -> "_lib.TrackerParams":
     """bt_tracker_params from the config keys the reference reads (bundle.window_size / max_BA_frames / min_fm_edges_newframe,
-    keyframe.min_feat_num / min_rot, ransac.max_iter / inlier_dist and those config.py maps).  mode: _lib.BT_MASK_* (default: config.mask_mode)."""
+    keyframe.min_feat_num / min_rot, ransac.max_iter / inlier_dist and those config.py maps).  mode: _lib.BT_MASK_* (default: config.mask_mode).
+    max_keyframes > 0 holds that many keyframes apart from max_frames_alive (the header's bt_tracker_params)."""
     y = load_yml(yml)
     Kn = np.asarray(K, np.float64)
     fx, fy, cx, cy = (Kn[0, 0], Kn[1, 1], Kn[0, 2], Kn[1, 2]) if Kn.ndim == 2 else Kn
     b, kf, rs = y["bundle"], y["keyframe"], y["ransac"]
     p = _lib.TrackerParams()
     p.H, p.W, p.fx, p.fy, p.cx, p.cy = int(H), int(W), float(fx), float(fy), float(cx), float(cy)
-    p.max_feats, p.max_frames_alive = int(max_feats), int(max_frames_alive)
+    p.max_feats, p.max_frames_alive, p.max_keyframes = int(max_feats), int(max_frames_alive), int(max_keyframes)
     p.mask_mode = mask_mode(yml) if mode is None else int(mode)
     p.depth, p.solver, p.prune = depth_params(y), solver_params(y), prune_params(y)
     p.ransac_trials, p.ransac_inlier_dist = int(rs["max_iter"]), float(rs["inlier_dist"])
@@ -36,12 +37,15 @@ def _ptr(x) -> int:
 
 
 class Tracker:
-    """Tracker(yml, H, W, K, max_feats, max_frames_alive): everything is reserved here (bt_tracker_create states the memory).  Device
-    arguments are torch CUDA tensors (or raw device addresses); the library works on `stream` (default: the legacy default stream)."""
+    """Tracker(yml, H, W, K, max_feats, max_frames_alive, max_keyframes=0): everything is reserved here (bt_tracker_create states the
+    memory).  For a whole sequence give it a keyframe pool: max_frames_alive = window_size + 4 or so and max_keyframes = the most keyframes the
+    sequence can admit.  Device arguments are torch CUDA tensors (or raw device addresses); the library works on `stream` (default: the legacy
+    default stream)."""
 
-    def __init__(self, yml, H: int, W: int, K, max_feats: int, max_frames_alive: int, device: int = 0, stream: int = 0, mode: int = None):
+    def __init__(self, yml, H: int, W: int, K, max_feats: int, max_frames_alive: int, device: int = 0, stream: int = 0, mode: int = None,
+                 max_keyframes: int = 0):
         self.lib = _lib.load()
-        self.params = tracker_params(yml, H, W, K, max_feats, max_frames_alive, mode)
+        self.params = tracker_params(yml, H, W, K, max_feats, max_frames_alive, mode, max_keyframes)
         self.stream = ctypes.c_void_p(stream)
         self.t = ctypes.c_void_p()
         _lib.check(self.lib.bt_tracker_create(ctypes.byref(self.t), ctypes.c_int(device), ctypes.byref(self.params)), "bt_tracker_create")
@@ -90,10 +94,16 @@ class Tracker:
     def state(self):
         """Every frame alive, oldest first: (ids int32 [n], poses float32 [n,4,4], is_keyframe bool [n])."""
         n = ctypes.c_int(0)
-        cap = self.params.max_frames_alive
+        cap = self.params.max_frames_alive + self.params.max_keyframes
         ids = np.zeros(cap, np.int32)
         poses = np.zeros((cap, 4, 4), np.float32)
         kf = np.zeros(cap, np.int32)
         _lib.check(self.lib.bt_tracker_state(self.t, ids.ctypes.data_as(ctypes.c_void_p), poses.ctypes.data_as(ctypes.c_void_p), kf.ctypes.data_as(ctypes.c_void_p),
                                              ctypes.c_int(cap), ctypes.byref(n)), "bt_tracker_state")
         return ids[:n.value].copy(), poses[:n.value].copy(), kf[:n.value].astype(bool)
+
+    def usage(self):
+        """(map points alive, pairs in the match cache, entries of their blocks); synchronises the tracker's stream."""
+        pts, pairs, ents = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_longlong(0)
+        _lib.check(self.lib.bt_tracker_usage(self.t, ctypes.byref(pts), ctypes.byref(pairs), ctypes.byref(ents), self.stream), "bt_tracker_usage")
+        return pts.value, pairs.value, ents.value

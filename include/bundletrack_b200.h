@@ -299,8 +299,18 @@ BT_API int bt_match_pairs_ex(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, 
  *   has     1 / 0.
  *   gather  writes the cached blocks of the listed pairs back to back into dst_dev with imgIdx_i / imgIdx_j rewritten to the given
  *           window indices (a frame's index changes from window to window) and fills block_off / block_n for bt_window::corr_dev;
- *           pairs with no cached matches contribute empty blocks. */
+ *           pairs with no cached matches contribute empty blocks.
+ *   usage   the pairs cached now and the entries their blocks hold.
+ * The blocks live in one device arena of 32-B entries; each takes exactly its pair's entry count.  forget_frame gives a pair's block back.  A put
+ * that finds no room behind the last block first moves the live blocks to the arena's start (a device-to-device copy on the put's stream, no
+ * host synchronisation; gather's output does not change).  put returns BT_ERR_CAPACITY, and changes nothing, only when the pairs cached would
+ * exceed max_pairs_cached, the live entries would exceed the arena, or a block is longer than the per-pair limit.
+ *   bt_match_cache_reserve          arena of max_pairs_cached x max_entries_per_pair entries, per-pair limit max_entries_per_pair.
+ *   bt_match_cache_reserve_entries  arena of max_entries_total entries (<= INT_MAX), no per-pair limit beyond that.
+ * Both empty the cache; the arena takes 32 B per entry. */
 BT_API int bt_match_cache_reserve(bt_ctx* ctx, int max_pairs_cached, int max_entries_per_pair);
+BT_API int bt_match_cache_reserve_entries(bt_ctx* ctx, int max_pairs_cached, long long max_entries_total);
+BT_API int bt_match_cache_usage(bt_ctx* ctx, int* n_pairs, long long* n_entries);
 BT_API int bt_match_cache_put(bt_ctx* ctx, int n_pairs, const int32_t* idA, const int32_t* idB, const bt_entryj* entry_dev,
                        const int32_t* n_entry_host, const int32_t* entry_off_host, const int32_t* status_host, void* stream);
 BT_API int bt_match_cache_has(bt_ctx* ctx, int idA, int idB);
@@ -416,13 +426,16 @@ BT_API int bt_tracks_stats(const bt_tracks* t, int* n_points, int* n_observation
 /* The same table on the device, owned by the context, with the same results as bt_tracks (output bits and order included).  Everything is
  * asynchronous on `stream` except stats; use one stream for a context's table.
  *   reserve       capacities: frames alive (<= 64), keys per frame (<= 8192), map points alive.  Empties the table.  Nothing is allocated
- *                 later.  A call that would exceed a capacity changes nothing and latches a flag: the next bt_tracks_dev_stats returns
+ *                 later.  The table takes max_points x max_frames x 8 B of observations plus max_frames x max_keys_per_frame x 48 B of frame maps
+ *                 (and 20 B per point).
+ *   reserve_ex    the same with max_frames up to 64 + 1024 (BT_ERR_INVALID_ARG above that).  A call that would exceed a capacity changes nothing and latches a flag: the next bt_tracks_dev_stats returns
  *                 BT_ERR_CAPACITY (and clears it).  Frames are mapped to slots on the host; a frame past the limit fails at once.
  *   update_pair   uv_dev: DEVICE (uA, vA, uB, vB) per match, *n_dev (DEVICE) of them, at most uv_capacity; so it can follow an emit without
  *                 a synchronisation.  Keys must not be NaN.
  *   propagate     bt_tracks_propagate with existing_uv_dev / out_uv_dev DEVICE and the count written to *n_out_dev.
  *   stats         synchronises the stream; n_points counts every map point ever created, as bt_tracks_stats does. */
 BT_API int bt_tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_per_frame, int max_points);
+BT_API int bt_tracks_dev_reserve_ex(bt_ctx* ctx, int max_frames, int max_keys_per_frame, int max_points);
 BT_API int bt_tracks_dev_update_pair(bt_ctx* ctx, int frame_a, int frame_b, const float* uv_dev, const int32_t* n_dev, int uv_capacity, void* stream);
 BT_API int bt_tracks_dev_propagate(bt_ctx* ctx, int frame_a, int frame_b, const float* existing_uv_dev, int n_existing,
                             float* out_uv_dev, int capacity, int32_t* n_out_dev, void* stream);
@@ -453,11 +466,15 @@ BT_API int bt_pose_init(bt_ctx* ctx, const bt_entryj* entry_dev, const int32_t* 
 
 /* ---- the whole tracking step: Bundler::processNewFrame (the reference's src/Bundler.cpp:56-183) as one object -------------------------
  * A tracker owns its own bt_ctx and reserves everything in bt_tracker_create, for frames of H x W with at most max_feats keypoints and
- * 256-dimensional descriptors: max_frames_alive + 1 sets of full-resolution maps (depth, normals, foreground mask: 25 B per pixel) with their
- * keypoints and descriptor-pool slots, max_frames_alive frame-cache slots, the device map-point table (max_frames_alive frames, 16 x max_feats
- * points), the match cache (every pair of max_frames_alive frames, 3 x max_feats entries of 32 B each) and the matcher and solver for
- * windows of max_BA_frames frames.  At 640 x 480, 2000 features, max_frames_alive = 32 and max_BA_frames = 15 that is roughly 0.6 GB: 0.25 GB
- * of frame maps, 0.1 GB each of descriptor pool and match cache, the rest matcher and solver scratch.
+ * 256-dimensional descriptors.  With S = max_frames_alive + max_keyframes frame slots: S + 1 sets of full-resolution maps (depth, normals,
+ * foreground mask: 25 B per pixel) with their keypoints and descriptor-pool slots (1 KB per feature), S frame-cache slots, the device map-point
+ * table (S frames, 16 x max_feats x ceil(S / 64) points: S x points x 8 B of observations), the match cache and the matcher and solver for
+ * windows of max_BA_frames frames.  The match cache holds every pair of S frames at 3 x max_feats entries of 32 B each when max_keyframes = 0,
+ * and S x max_BA_frames x 3 x max_feats / 2 entries in all (max_BA_frames / 2 worst-case blocks per frame slot) otherwise.
+ * At 640 x 480, 2000 features, max_frames_alive = 32 and max_BA_frames = 15 that is roughly 0.6 GB: 0.25 GB of frame maps, 0.1 GB each of
+ * descriptor pool and match cache, the rest matcher and solver scratch.  One frame slot costs about 11.7 MB at 640 x 480 with 2000 features
+ * (7.7 MB of maps, 3.1 MB of descriptor pool, 0.9 MB of frame cache), plus 0.26 MB x ceil(S / 64) of map-point observations and 1.4 MB of
+ * match cache at max_BA_frames = 15: max_frames_alive = 8 with max_keyframes = 256 reserved 4.65 GB in all (DESIGN.md §9.5).
  * A frame's step is split where the reference calls the LF-Net server: begin_frame (id, pose, segmentation, the 10-pixel ROI gate and the
  * request image) and end_frame (descriptors, findCorres on the neighbour pair, the initial pose on the device, the frame deque, keyframe
  * selection, findCorres on the window, the BA gate, the solve, keyframe admission).  Poses are row-major 4 x 4 cam->model. */
@@ -465,16 +482,20 @@ typedef struct bt_tracker bt_tracker;
 typedef struct {
 	int H, W; float fx, fy, cx, cy;
 	int max_feats;                 /* keypoints per frame */
-	int max_frames_alive;          /* frames held at once during a step: keyframes + the recent-frame deque + the new frame; <= 64 (the device
-	                                * map-point table's limit).  The oldest recent frame is released only after the new frame's neighbour pair is
-	                                * matched, as in the reference, so it counts too. */
+	int max_frames_alive;          /* 2..64.  max_keyframes = 0: the frames held at once during a step, keyframes + the recent-frame deque + the
+	                                * new frame.  max_keyframes > 0: the same without the keyframes.  The oldest recent frame is released only after
+	                                * the new frame's neighbour pair is matched, as in the reference, so it counts too. */
 	int mask_mode;                 /* BT_MASK_AS_IS / BT_MASK_LARGEST_HULL */
 	bt_depth_params depth; bt_solver_params solver; bt_prune_params prune;
 	int ransac_trials; float ransac_inlier_dist;
 	int window_size, max_BA_frames, min_fm_edges_newframe, min_feat_num; float min_rot_deg;
+	int max_keyframes;             /* 0..1024.  0: keyframes count against max_frames_alive (at most 64 frames alive in all).  > 0: a keyframe pool of
+	                                * this many, held apart from max_frames_alive; the reference never releases a keyframe, so this bounds the
+	                                * sequence's keyframes.  Value-initialise the struct (= {0}) so older callers get 0. */
 } bt_tracker_params;
 enum { BT_FRAME_OTHER = 0, BT_FRAME_FAIL = 1, BT_FRAME_NO_BA = 2 };   /* Frame::_status */
-/* BT_ERR_NO_DEVICE without an sm_90 GPU; BT_ERR_INVALID_ARG for parameters out of range (max_BA_frames 2..32, max_frames_alive 2..64). */
+/* BT_ERR_NO_DEVICE without an sm_90 GPU; BT_ERR_INVALID_ARG for parameters out of range (max_BA_frames 2..32, max_frames_alive 2..64,
+ * max_keyframes 0..1024), checked before the device is looked at. */
 BT_API int bt_tracker_create(bt_tracker** out, int device, const bt_tracker_params* p);
 BT_API void bt_tracker_destroy(bt_tracker* t);
 /* The new frame's id and pose: the last frame's id + 1 and its pose when the tracker holds frames, else loader_id and first_pose (identity when
@@ -486,14 +507,17 @@ BT_API int bt_tracker_begin_frame(bt_tracker* t, int loader_id, const float* fir
                                   const uint8_t* colour_dev, uint8_t* request_out_dev, int32_t* roi_out, int* status_out, void* stream);
 /* kpts_host: n_kpts x (x, y) image pixels (bt_lfnet_parse_reply's output); desc: the n_kpts x 256 descriptors on the device.  Writes the frame's
  * pose as Bundler::saveNewframeResult would record it and its status.  BT_ERR_INVALID_ARG without a pending begin_frame, for n_kpts > max_feats
- * or a NULL argument; BT_ERR_CAPACITY when the frames alive plus the new one exceed max_frames_alive.  Both change nothing: the frame stays
- * pending. */
+ * or a NULL argument.  BT_ERR_CAPACITY when max_keyframes = 0 and the frames alive plus the new one exceed max_frames_alive, or when
+ * max_keyframes > 0 and either the frames alive that are not keyframes plus the new one exceed max_frames_alive or the keyframe pool is full
+ * (the new frame might be admitted).  Both change nothing: the frame stays pending. */
 BT_API int bt_tracker_end_frame(bt_tracker* t, const float* kpts_host, int n_kpts, const bt_desc_view* desc, float* pose_out, int* status_out, void* stream);
 /* Lfnet::detectFeature threw: the pending frame becomes FAIL and is forgotten (Bundler.cpp:108-116).  pose_out (optional): its pose. */
 BT_API int bt_tracker_drop_frame(bt_tracker* t, float* pose_out);
 /* Every frame alive (the deque and the keyframes), oldest first: ids, poses (16 floats each) and whether it is a keyframe.  *n = the count;
  * BT_ERR_CAPACITY when it exceeds cap (the arrays may be NULL when cap is 0). */
 BT_API int bt_tracker_state(bt_tracker* t, int32_t* ids, float* poses, int32_t* is_keyframe, int cap, int* n);
+/* What the tracker's tables hold now: map points alive, pairs in the match cache and the entries of their blocks.  Synchronises `stream`. */
+BT_API int bt_tracker_usage(bt_tracker* t, int* n_points, int* n_pairs_cached, long long* n_entries_cached, void* stream);
 
 /* Small device-memory helpers so non-CUDA hosts (ctypes, cgo, JNI) can drive the library without another runtime. */
 BT_API int bt_dev_alloc(void** out, size_t bytes);
