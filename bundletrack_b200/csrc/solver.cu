@@ -272,6 +272,67 @@ __device__ __forceinline__ float texel_depth(const TexelGeom& g, int W, int H, i
 	return (d >= 0.1f) ? d : 0.f;
 }
 
+struct FrameGeom { int W, H, w, h; TexelGeom tg; };
+
+// A frame's maps are built one CTA per 1024 quarter-res pixels (block b, 1024 threads) in two launches.  The compacted source list
+// keeps pixel order (fixed summation order downstream), so each block needs the number of valid pixels before it: the first launch
+// counts the valid pixels of every block (frame_block_count), the second turns the counts of the blocks before it into the block's
+// offset in the list and writes its slice of the texel map and its source records there (frame_block_build).  blk_cnt is the
+// frame's row of block counts.
+__device__ __forceinline__ void frame_block_count(const FrameGeom& g, const float* __restrict__ depth, float dmin, float dmax, int b, int* __restrict__ blk_cnt) {
+	const int npix = g.w * g.h, idx = b * 1024 + threadIdx.x;
+	__shared__ int s_w[32];
+	bool valid = false;
+	if (idx < npix) {
+		const float z = texel_depth(g.tg, g.W, g.H, g.w, depth, idx);
+		valid = (z > dmin && z < dmax);
+	}
+	const unsigned bal = __ballot_sync(0xffffffffu, valid);
+	if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = __popc(bal);
+	__syncthreads();
+	if (threadIdx.x < 32) {
+		int t = s_w[threadIdx.x];
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+		if (threadIdx.x == 0) blk_cnt[b] = t;
+	}
+}
+// The frame's last block also writes the source count to *nsrc.  Blocks past the end of the frame do nothing.
+__device__ __forceinline__ void frame_block_build(const FrameGeom& g, const float* __restrict__ depth, const float4* __restrict__ normal, float dmin, float dmax, int b,
+                                                  const int* __restrict__ blk_cnt, float4* texel, float4* src, int* nsrc) {
+	__shared__ int s_w[32];
+	__shared__ int s_base;
+	const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+	const int npix = g.w * g.h;
+	if (b * 1024 >= npix) return;
+	if (wid == 0) {      // offset of this block = valid pixels of the blocks before it (at most a few dozen)
+		int t = 0;
+		for (int q = lane; q < b; q += 32) t += blk_cnt[q];
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+		if (lane == 0) s_base = t;
+	}
+	const int idx = b * 1024 + tid;
+	float4 cp, nr;
+	bool valid = false;
+	if (idx < npix) {
+		texel[idx] = texel_build(g.tg, g.W, g.H, g.w, depth, normal, idx, cp, nr);
+		valid = (cp.z > dmin && cp.z < dmax);
+	}
+	const unsigned bal = __ballot_sync(0xffffffffu, valid);
+	if (lane == 0) s_w[wid] = __popc(bal);
+	__syncthreads();
+	int off = (lane < wid) ? s_w[lane] : 0;       // exclusive prefix over the warps of this block
+#pragma unroll
+	for (int o = 16; o > 0; o >>= 1) off += __shfl_xor_sync(0xffffffffu, off, o);
+	if (valid) {
+		const int o = s_base + off + __popc(bal & ((1u << lane) - 1u));
+		src[2 * o] = make_float4(cp.x, cp.y, cp.z, nr.x);
+		src[2 * o + 1] = make_float4(nr.y, nr.z, nr.w, 0.f);
+	}
+	if ((b + 1) * 1024 >= npix && tid == 1023) *nsrc = s_base + off + __popc(bal);     // last block of the frame, last warp: the total
+}
+
 // one 32-byte source record through the read-only path: two 128-bit loads (the widest global load sm_90 has)
 struct __align__(32) F8 { float4 lo, hi; };
 __device__ __forceinline__ F8 ldg256(const float4* p) {
@@ -359,8 +420,6 @@ __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw);
 // source records at their final position.  No barrier inside either sweep, so the loads of consecutive rounds overlap.
 static constexpr int kPrepRounds = 64;      // rounds of 1024 pixels per scan (one scan covers 65536 quarter-res pixels)
 
-struct FrameGeom { int W, H, w, h; TexelGeom tg; };
-
 // Builds one frame's quarter-resolution texel map and compacted source list (1024 threads); returns the source count.
 __device__ int build_frame_maps(const FrameGeom& g, const float* __restrict__ depth, const float4* __restrict__ normal, float4* texel, float4* src,
                                 float dmin, float dmax, int* s_cnt, int* s_wt) {
@@ -424,71 +483,27 @@ __device__ int build_frame_maps(const FrameGeom& g, const float* __restrict__ de
 	return base;
 }
 
-// Frame preparation, one CTA per 1024 quarter-res pixels of a frame (two launches): k_prep_count counts the valid pixels of
-// every block, k_prep_frames turns the counts of the blocks before it into its offset in the frame's ordered source list and
-// writes its slice of the texel map and of the list.  (One CTA per frame would walk 19 rounds serially.)
+// Frame preparation of the frames a call rebuilds itself, one CTA per 1024 quarter-res pixels of a (window, frame) slot:
+// frame_block_count, then frame_block_build.  (One CTA per frame would walk 19 rounds serially.)
 __global__ void __launch_bounds__(1024, 2) k_prep_count(SolveArgs a, int* __restrict__ blk_cnt) {
 	const int fs = blockIdx.y, b = blockIdx.x;
 	if (a.nsrc_cached[fs] || !(a.prm.w_dense > 0.0f)) return;
 	const WinDesc wd = a.wins[a.frame_win[fs]];
-	const int npix = wd.w * wd.h, idx = b * 1024 + threadIdx.x;
-	__shared__ int s_w[32];
-	bool valid = false;
-	if (idx < npix) {
-		const float z = texel_depth(wd.tg, wd.W, wd.H, wd.w, a.depth_ptr[fs], idx);
-		valid = (z > a.prm.depth_min && z < a.prm.depth_max);
-	}
-	const unsigned bal = __ballot_sync(0xffffffffu, valid);
-	if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = __popc(bal);
-	__syncthreads();
-	if (threadIdx.x < 32) {
-		int t = s_w[threadIdx.x];
-#pragma unroll
-		for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-		if (threadIdx.x == 0) blk_cnt[fs * gridDim.x + b] = t;
-	}
+	const FrameGeom g = {wd.W, wd.H, wd.w, wd.h, wd.tg};
+	frame_block_count(g, a.depth_ptr[fs], a.prm.depth_min, a.prm.depth_max, b, blk_cnt + fs * gridDim.x);
 }
 
 __global__ void __launch_bounds__(1024, 2) k_prep_frames(SolveArgs a, WinDesc* wins_rw, int* prep_ticket, const int* __restrict__ blk_cnt) {
 	const int fs = blockIdx.y, b = blockIdx.x;
 	const WinDesc wd = a.wins[a.frame_win[fs]];
-	__shared__ int s_w[32];
-	__shared__ int s_base;
-	const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+	const int tid = threadIdx.x;
 	const int* cached = a.nsrc_cached[fs];
-	const int npix = wd.w * wd.h;
 	if (cached) { if (b == 0 && tid == 0) a.nsrc[fs] = *cached; }      // maps and source list were built by bt_frame_cache_store
 	else if (!(a.prm.w_dense > 0.0f)) { if (b == 0 && tid == 0) a.nsrc[fs] = 0; }
-	else if (b * 1024 < npix) {
-		if (wid == 0) {      // offset of this block = valid pixels of the blocks before it (at most a few dozen)
-			int t = 0;
-			for (int q = lane; q < b; q += 32) t += blk_cnt[fs * gridDim.x + q];
-#pragma unroll
-			for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-			if (lane == 0) s_base = t;
-		}
-		const float dmin = a.prm.depth_min, dmax = a.prm.depth_max;
-		float4* texel = a.texel + (size_t)fs * a.npix_max;
-		float4* src = a.src + (size_t)fs * 2 * a.npix_max;
-		const int idx = b * 1024 + tid;
-		float4 cp, nr;
-		bool valid = false;
-		if (idx < npix) {
-			texel[idx] = texel_build(wd.tg, wd.W, wd.H, wd.w, a.depth_ptr[fs], a.normal_ptr[fs], idx, cp, nr);
-			valid = (cp.z > dmin && cp.z < dmax);
-		}
-		const unsigned bal = __ballot_sync(0xffffffffu, valid);
-		if (lane == 0) s_w[wid] = __popc(bal);
-		__syncthreads();
-		int off = (lane < wid) ? s_w[lane] : 0;       // exclusive prefix over the warps of this block
-#pragma unroll
-		for (int o = 16; o > 0; o >>= 1) off += __shfl_xor_sync(0xffffffffu, off, o);
-		if (valid) {
-			const int o = s_base + off + __popc(bal & ((1u << lane) - 1u));
-			src[2 * o] = make_float4(cp.x, cp.y, cp.z, nr.x);
-			src[2 * o + 1] = make_float4(nr.y, nr.z, nr.w, 0.f);
-		}
-		if ((b + 1) * 1024 >= npix && tid == 1023) a.nsrc[fs] = s_base + off + __popc(bal);     // last block of the frame, last warp: the total
+	else {
+		const FrameGeom g = {wd.W, wd.H, wd.w, wd.h, wd.tg};
+		frame_block_build(g, a.depth_ptr[fs], a.normal_ptr[fs], a.prm.depth_min, a.prm.depth_max, b, blk_cnt + fs * gridDim.x,
+		                  a.texel + (size_t)fs * a.npix_max, a.src + (size_t)fs * 2 * a.npix_max, a.nsrc + fs);
 	}
 	if (b == 0 && tid == 1023) {      // pose -> (rot, trans) -> T of iteration 0 (one lane of the frame's first block)
 		float Tm[12];
@@ -530,60 +545,13 @@ __global__ void __launch_bounds__(1024, 2) k_frame_cache_store(CacheStoreArgs c)
 // The same store spread over one CTA per 1024 quarter-res pixels (count + build, like k_prep_count / k_prep_frames): a handful of new
 // frames per step - one per tracked window - otherwise runs on a handful of CTAs walking 19 rounds each.
 __global__ void __launch_bounds__(1024, 2) k_cache_count(CacheStoreArgs c, int* __restrict__ blk_cnt) {
-	const int f = blockIdx.y, b = blockIdx.x;
-	const int npix = c.g.w * c.g.h, idx = b * 1024 + threadIdx.x;
-	__shared__ int s_w[32];
-	bool valid = false;
-	if (idx < npix) {
-		const float z = texel_depth(c.g.tg, c.g.W, c.g.H, c.g.w, c.depth[f], idx);
-		valid = (z > c.dmin && z < c.dmax);
-	}
-	const unsigned bal = __ballot_sync(0xffffffffu, valid);
-	if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = __popc(bal);
-	__syncthreads();
-	if (threadIdx.x < 32) {
-		int t = s_w[threadIdx.x];
-#pragma unroll
-		for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-		if (threadIdx.x == 0) blk_cnt[f * gridDim.x + b] = t;
-	}
+	const int f = blockIdx.y;
+	frame_block_count(c.g, c.depth[f], c.dmin, c.dmax, blockIdx.x, blk_cnt + f * gridDim.x);
 }
 __global__ void __launch_bounds__(1024, 2) k_cache_build(CacheStoreArgs c, const int* __restrict__ blk_cnt) {
-	const int f = blockIdx.y, b = blockIdx.x;
-	__shared__ int s_w[32];
-	__shared__ int s_base;
-	const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-	const int npix = c.g.w * c.g.h;
-	if (b * 1024 >= npix) return;
-	const int slot = c.slots[f];
-	if (wid == 0) {      // offset of this block = valid pixels of the blocks before it
-		int t = 0;
-		for (int q = lane; q < b; q += 32) t += blk_cnt[f * gridDim.x + q];
-#pragma unroll
-		for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-		if (lane == 0) s_base = t;
-	}
-	float4* texel = c.texel + (size_t)slot * c.slot_npix;
-	float4* src = c.src + (size_t)slot * 2 * c.slot_npix;
-	const int idx = b * 1024 + tid;
-	float4 cp, nr;
-	bool valid = false;
-	if (idx < npix) {
-		texel[idx] = texel_build(c.g.tg, c.g.W, c.g.H, c.g.w, c.depth[f], c.normal[f], idx, cp, nr);
-		valid = (cp.z > c.dmin && cp.z < c.dmax);
-	}
-	const unsigned bal = __ballot_sync(0xffffffffu, valid);
-	if (lane == 0) s_w[wid] = __popc(bal);
-	__syncthreads();
-	int off = (lane < wid) ? s_w[lane] : 0;
-#pragma unroll
-	for (int o = 16; o > 0; o >>= 1) off += __shfl_xor_sync(0xffffffffu, off, o);
-	if (valid) {
-		const int o = s_base + off + __popc(bal & ((1u << lane) - 1u));
-		src[2 * o] = make_float4(cp.x, cp.y, cp.z, nr.x);
-		src[2 * o + 1] = make_float4(nr.y, nr.z, nr.w, 0.f);
-	}
-	if ((b + 1) * 1024 >= npix && tid == 1023) c.nsrc[slot] = s_base + off + __popc(bal);
+	const int f = blockIdx.y, slot = c.slots[f];
+	frame_block_build(c.g, c.depth[f], c.normal[f], c.dmin, c.dmax, blockIdx.x, blk_cnt + f * gridDim.x,
+	                  c.texel + (size_t)slot * c.slot_npix, c.src + (size_t)slot * 2 * c.slot_npix, c.nsrc + slot);
 }
 
 // ------------------------------------------------------------------------------------------------ tile plan
@@ -1679,6 +1647,16 @@ extern "C" int bt_solve_get_timing(bt_ctx* ctx, float* ms3) {
 	return BT_OK;
 }
 
+// Full- and quarter-resolution size and texel geometry of a frame (LossGPU.cu:56-57, CUDACache.cpp:20-24).  The per-call build and the
+// frame cache both take it from here: the dense tap rebuilds camera points from these floats, so cached and per-call maps must share them.
+static FrameGeom frame_geom(int H, int W, float fx, float fy, float cx, float cy, float image_downscale) {
+	FrameGeom g;
+	g.W = W; g.H = H; g.w = (int)(W / image_downscale); g.h = (int)(H / image_downscale);
+	g.tg.ifx = 1.0f / fx; g.tg.ify = 1.0f / fy; g.tg.icx = -cx / fx; g.tg.icy = -cy / fy;
+	g.tg.scaleW = (float)(W - 1) / (float)(g.w - 1); g.tg.scaleH = (float)(H - 1) / (float)(g.h - 1);
+	return g;
+}
+
 static SolveArgs make_args(bt_ctx* ctx);
 static int launch_prep(bt_ctx* ctx, cudaStream_t stream);
 
@@ -1748,12 +1726,10 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 		const int N = bw.n_frames;
 		WinDesc& d = hw[w];
 		memset(&d, 0, sizeof d);
-		d.n_frames = N; d.H = bw.H; d.W = bw.W;
-		d.w = (int)(bw.W / params->image_downscale); d.h = (int)(bw.H / params->image_downscale);   // LossGPU.cu:56-57
+		const FrameGeom geom = frame_geom(bw.H, bw.W, bw.fx, bw.fy, bw.cx, bw.cy, params->image_downscale);
+		d.n_frames = N; d.H = geom.H; d.W = geom.W; d.w = geom.w; d.h = geom.h; d.tg = geom.tg;
 		d.fx = bw.fx * ((float)d.w / (float)bw.W); d.fy = bw.fy * ((float)d.h / (float)bw.H);         // CUDACache.cpp:20-24
 		d.cx = bw.cx * ((float)(d.w - 1) / (float)(bw.W - 1)); d.cy = bw.cy * ((float)(d.h - 1) / (float)(bw.H - 1));
-		d.tg.ifx = 1.0f / bw.fx; d.tg.ify = 1.0f / bw.fy; d.tg.icx = -bw.cx / bw.fx; d.tg.icy = -bw.cy / bw.fy;
-		d.tg.scaleW = (float)(bw.W - 1) / (float)(d.w - 1); d.tg.scaleH = (float)(bw.H - 1) / (float)(d.h - 1);
 		d.compat_flip = bw.compat_flip;
 		d.frame_off = (int)f_off; d.pair_off = (int)p_off;
 		s->frame_off[w] = (int)f_off; s->n_frames[w] = N;
@@ -2199,8 +2175,8 @@ extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* sl
 	SolverState* s = ctx->solver;
 	BT_REQUIRE(s->c_capacity > 0, BT_ERR_INVALID_ARG, "bt_frame_cache_store: call bt_frame_cache_reserve first");
 	BT_REQUIRE(n_frames > 0 && n_frames <= s->c_capacity, BT_ERR_CAPACITY, "bt_frame_cache_store: %d frames > capacity %d", n_frames, s->c_capacity);
-	const int w = (int)(W / s->c_downscale), h = (int)(H / s->c_downscale);
-	BT_REQUIRE(H > 0 && W > 0 && w >= 2 && h >= 2 && w * h <= s->c_npix, BT_ERR_CAPACITY, "bt_frame_cache_store: image %dx%d does not fit the reserved cache", W, H);
+	const FrameGeom geom = frame_geom(H, W, fx, fy, cx, cy, s->c_downscale);
+	BT_REQUIRE(H > 0 && W > 0 && geom.w >= 2 && geom.h >= 2 && geom.w * geom.h <= s->c_npix, BT_ERR_CAPACITY, "bt_frame_cache_store: image %dx%d does not fit the reserved cache", W, H);
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
 	const size_t b_ptr = sizeof(void*) * (size_t)n_frames, bytes = 2 * b_ptr + sizeof(int) * (size_t)n_frames;
@@ -2221,16 +2197,14 @@ extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* sl
 	BT_CUDA(cudaMemcpyAsync(s->c_tables.p, hb, bytes, cudaMemcpyHostToDevice, stream));
 	BT_CUDA(cudaEventRecord(s->c_ev[fl], stream));
 	CacheStoreArgs c;
-	c.g.W = W; c.g.H = H; c.g.w = w; c.g.h = h;                                                   // same expressions as bt_solve_stage (CUDACache.cpp:20-24)
-	c.g.tg.ifx = 1.0f / fx; c.g.tg.ify = 1.0f / fy; c.g.tg.icx = -cx / fx; c.g.tg.icy = -cy / fy;
-	c.g.tg.scaleW = (float)(W - 1) / (float)(w - 1); c.g.tg.scaleH = (float)(H - 1) / (float)(h - 1);
+	c.g = geom;
 	char* db = s->c_tables.as<char>();
 	c.depth = (const float* const*)db; c.normal = (const float4* const*)(db + b_ptr); c.slots = (const int*)(db + 2 * b_ptr);
 	c.texel = s->c_texel.as<float4>(); c.src = s->c_src.as<float4>(); c.nsrc = s->c_nsrc.as<int>(); c.slot_npix = (size_t)s->c_npix;
 	c.dmin = depth_min; c.dmax = depth_max;
-	if (n_frames >= 2 * ctx->sm_count) k_frame_cache_store<<<n_frames, 1024, 0, stream>>>(c);      // many frames: one CTA per frame fills the machine
+	if (n_frames >= 2 * ctx->sm_count) k_frame_cache_store<<<n_frames, 1024, 0, stream>>>(c);      // many frames: one CTA per frame fills the machine (faster than count + build there, DESIGN §9.6)
 	else {
-		const dim3 grid((unsigned)((w * h + 1023) / 1024), (unsigned)n_frames);
+		const dim3 grid((unsigned)((geom.w * geom.h + 1023) / 1024), (unsigned)n_frames);
 		k_cache_count<<<grid, 1024, 0, stream>>>(c, s->c_blk.as<int>());
 		k_cache_build<<<grid, 1024, 0, stream>>>(c, s->c_blk.as<int>());
 	}

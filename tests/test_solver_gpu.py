@@ -314,6 +314,27 @@ def test_frame_cache_is_bit_identical(cuda_device):
     o.close()
 
 
+def test_frame_cache_store_of_many_frames_is_bit_identical(cuda_device):
+    """One bt_frame_cache_store call of 2 x SM-count + 8 frames (a keyframe pool filled at once) builds the same maps as the per-call
+    rebuild: windows whose slots sit at the start, the middle and the end of that call give exactly the poses of the rebuild."""
+    from bundletrack_b200.optimizer import OptimizerGpu, SolveWindow
+    import torch
+    n = 2 * torch.cuda.get_device_properties(cuda_device).multi_processor_count + 8
+    w = synth.make_window(53, n_frames=6, n_corr=900)
+    F = w.n_frames
+    depth, normal = _upload(w, cuda_device)
+    o = OptimizerGpu(None, max_windows=3, max_frames=F, max_corr=2000)
+    o.reserve_frame_cache(n)
+    o.store_frames(list(range(n)), [depth[k % F] for k in range(n)], [normal[k % F] for k in range(n)], w.H, w.W, w.K)      # slot k holds frame k % F
+    plain = o.optimizeWindows([SolveWindow(w.corr, w.H, w.W, depth, normal, w.poses_init, w.K)] * 3)
+    # frame f of the window from the slot at or after p that holds it
+    slots = [[p + (f - p) % F for f in range(F)] for p in (0, n // 2, n - F)]
+    cached = o.optimizeWindows([SolveWindow(w.corr, w.H, w.W, None, None, w.poses_init, w.K, cache_slots=s) for s in slots])
+    for a, b in zip(plain, cached):
+        assert a.tobytes() == b.tobytes()
+    o.close()
+
+
 def test_pinned_correspondences_are_read_in_place(opt, cuda_device):
     """Correspondences in page-locked host memory (one block for consecutive windows, or one window alone) skip the library's
     staging copy; the poses equal the pageable-memory path bit for bit, also when pinned and pageable windows alternate."""
