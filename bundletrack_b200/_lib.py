@@ -156,6 +156,7 @@ EXPORTS = [
     "bt_tracks_create", "bt_tracks_destroy", "bt_tracks_update_pair", "bt_tracks_propagate", "bt_tracks_forget_frame", "bt_tracks_stats",
     "bt_tracks_dev_reserve", "bt_tracks_dev_reserve_ex", "bt_tracks_dev_update_pair", "bt_tracks_dev_propagate", "bt_tracks_dev_forget_frame", "bt_tracks_dev_stats", "bt_find_corres_pairs",
     "bt_pose_init", "bt_tracker_create", "bt_tracker_destroy", "bt_tracker_begin_frame", "bt_tracker_end_frame", "bt_tracker_drop_frame", "bt_tracker_state", "bt_tracker_usage",
+    "bt_metrics_reserve", "bt_pose_metrics", "bt_vocap",
     "bt_dev_alloc", "bt_dev_free", "bt_memcpy_h2d", "bt_memcpy_d2h", "bt_host_alloc_pinned", "bt_host_free_pinned",
     "bt_stream_sync",
 ]

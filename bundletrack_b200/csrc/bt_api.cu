@@ -51,6 +51,7 @@ extern "C" void bt_ctx_destroy(bt_ctx* ctx) {
 	bt::mcache_destroy(ctx);
 	bt::tracks_dev_destroy(ctx);
 	bt::front_destroy(ctx);
+	bt::metrics_destroy(ctx);
 	delete ctx;
 }
 

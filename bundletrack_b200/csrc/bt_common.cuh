@@ -63,6 +63,7 @@ struct FrontState;    // frontend.cu
 struct PruneState;    // prune.cu
 struct MatchCache;    // prune.cu
 struct TracksDev;     // tracks_dev.cu
+struct MetricsState;  // metrics.cu
 
 }  // namespace bt
 
@@ -77,6 +78,7 @@ struct bt_ctx {
 	bt::PruneState* prune = nullptr;
 	bt::MatchCache* mcache = nullptr;
 	bt::TracksDev* tracks = nullptr;
+	bt::MetricsState* metrics = nullptr;
 };
 
 namespace bt {
@@ -86,6 +88,7 @@ void ransac_destroy(bt_ctx* ctx);
 void prune_destroy(bt_ctx* ctx);
 void mcache_destroy(bt_ctx* ctx);
 void front_destroy(bt_ctx* ctx);
+void metrics_destroy(bt_ctx* ctx);
 // segment.cu: largest-hull mode for the masked front end, and the LF-Net request
 size_t hull_fill_smem(int H);
 int segment_largest_hull(const uint8_t* const* mask_tbl_dev, int n, int H, int W, int32_t* label, int32_t* count, unsigned long long* best,

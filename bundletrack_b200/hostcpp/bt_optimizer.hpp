@@ -152,6 +152,28 @@ inline void saveNewframePose(const std::string& path, const Mat4& cur_in_model) 
 	if (bt_pose_write_txt(path.c_str(), flat) != BT_OK) throw std::runtime_error(std::string("bt_pose_write_txt: ") + bt_last_error());
 }
 
+// scripts/Utils.py add / adi for a whole sequence in one device call: ADD and ADD-S per frame (metres) into add_gpu / adds_gpu (device double
+// [n_frames]), asynchronous on `stream`.  model_pts_gpu: device double n_pts x 3 (points.xyz); pred / gt: ob_in_cam per frame as the
+// reference's poses/<id>.txt hold them.  The context needs bt_metrics_reserve(ctx, >= n_pts, >= pred.size()).
+template <class Mat4>
+inline void poseMetrics(bt_ctx* ctx, const double* model_pts_gpu, int n_pts, const std::vector<Mat4>& pred, const std::vector<Mat4>& gt, double* add_gpu,
+                        double* adds_gpu, void* stream = nullptr) {
+	if (pred.size() != gt.size()) throw std::runtime_error("poseMetrics: pred and gt differ in length");
+	std::vector<double> p(16 * pred.size()), g(16 * gt.size());
+	for (size_t f = 0; f < pred.size(); f++)
+		for (int r = 0; r < 4; r++)
+			for (int c = 0; c < 4; c++) { p[16 * f + 4 * r + c] = pred[f](r, c); g[16 * f + 4 * r + c] = gt[f](r, c); }
+	if (bt_pose_metrics(ctx, model_pts_gpu, n_pts, p.data(), g.data(), (int)pred.size(), add_gpu, adds_gpu, stream) != BT_OK)
+		throw std::runtime_error(std::string("bt_pose_metrics: ") + bt_last_error());
+}
+
+// eval_ycbineoat.py's VOCap: the AUC of the errors up to max_err (0.1 m), divided by max_err; x 100 is the number the paper's table prints.
+inline double voCap(const std::vector<double>& err, double max_err = 0.1) {
+	double auc = 0.0;
+	if (bt_vocap(err.data(), (int)err.size(), max_err, &auc) != BT_OK) throw std::runtime_error(std::string("bt_vocap: ") + bt_last_error());
+	return auc;
+}
+
 // ransacMultiPairGPU with the reference's argument list (device float4 arrays per pair, host result vectors).  The device result
 // buffers and the library's scratch belong to the object: nothing is allocated per call (the reference allocates six arrays and a
 // stream per pair per call, cuda_ransac.cu:1240-1275).

@@ -358,6 +358,8 @@ class Sequence:
     roi_fail: tuple          # frames whose mask is empty (the tracker's ROI gate fails)
     neighbour_fail: tuple    # frames whose features cannot match the previous frame
     detect_fail: tuple       # frames without features (detection failed)
+    radii: Optional[np.ndarray] = None        # the ellipsoid's radii (object frame), metres
+    ob_in_cam0: Optional[np.ndarray] = None   # [4,4] f64 object -> camera 0: a point x of the object frame is ob_in_cam0 x in the model frame
 
     @property
     def n_frames(self) -> int:
@@ -432,4 +434,4 @@ def make_sequence(seed: int, n_frames: int, H: int = 480, W: int = 640, K=None, 
             mask[k] = 0
         if k in detect_fail:
             feats[k] = None
-    return Sequence(raw, mask, colour, feats, poses_gt, K, tuple(roi_fail), tuple(neighbour_fail), tuple(detect_fail))
+    return Sequence(raw, mask, colour, feats, poses_gt, K, tuple(roi_fail), tuple(neighbour_fail), tuple(detect_fail), radii, ob_in_cam[0].copy())

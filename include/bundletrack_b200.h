@@ -519,6 +519,27 @@ BT_API int bt_tracker_state(bt_tracker* t, int32_t* ids, float* poses, int32_t* 
 /* What the tracker's tables hold now: map points alive, pairs in the match cache and the entries of their blocks.  Synchronises `stream`. */
 BT_API int bt_tracker_usage(bt_tracker* t, int* n_points, int* n_pairs_cached, long long* n_entries_cached, void* stream);
 
+/* ---- pose accuracy: the reference's evaluation (scripts/Utils.py add / adi, scripts/eval_ycbineoat.py VOCap) -------------------------
+ * bt_pose_metrics: per frame f, ADD = mean_i |gt_f p_i - pred_f p_i| and ADD-S = mean_i min_j |gt_f p_i - pred_f p_j| over the model points p,
+ * in metres, float64.  ADD-S is the exact nearest neighbour (brute force on the device, an fp32 filter whose rounding is bounded, then the
+ * candidates it keeps in float64; DESIGN.md §3.7): equal to a float64 k-d tree query up to float64 rounding.
+ *   model_pts_dev  DEVICE float64 n_pts x 3 (the rows of points.xyz), finite.
+ *   pred / gt      HOST row-major 4 x 4 ob_in_cam per frame (model -> camera: what poses/<id>.txt and bt_pose_write_txt hold), n_frames
+ *                  of each back to back.  The last row is not read.
+ *   add_out / adds_out  DEVICE float64 [n_frames].
+ * Asynchronous on `stream`: the poses are copied before the call returns (the host arrays may be reused at once), the results are ready
+ * when the stream is.  BT_ERR_INVALID_ARG for n_pts < 1, n_frames < 1, a NULL pointer, a non-finite pose element, or a context without
+ * bt_metrics_reserve; BT_ERR_CAPACITY above the reserved sizes.
+ * bt_metrics_reserve: scratch for up to max_pts model points (<= 67,107,840) and max_frames frames per call: 16 B per point, 304 B per
+ * frame (device and pinned host) and 16 B per frame per 1024 points. */
+BT_API int bt_metrics_reserve(bt_ctx* ctx, int max_pts, int max_frames);
+BT_API int bt_pose_metrics(bt_ctx* ctx, const double* model_pts_dev, int n_pts, const double* pred_ob_in_cam, const double* gt_ob_in_cam, int n_frames,
+                           double* add_out, double* adds_out, void* stream);
+/* VOCap (eval_ycbineoat.py): the area under the accuracy-threshold curve of n errors up to max_err (the reference's 0.1 m), divided by
+ * max_err; the paper's tables print it x 100.  Host code, no GPU.  n = 0 or no error below max_err gives 0; NaN errors count in n but never
+ * as below max_err.  BT_ERR_INVALID_ARG for n < 0, err NULL with n > 0, auc_out NULL or max_err not positive and finite. */
+BT_API int bt_vocap(const double* err, int n, double max_err, double* auc_out);
+
 /* Small device-memory helpers so non-CUDA hosts (ctypes, cgo, JNI) can drive the library without another runtime. */
 BT_API int bt_dev_alloc(void** out, size_t bytes);
 BT_API int bt_dev_free(void* p);
