@@ -158,7 +158,7 @@ EXPORTS = [
     "bt_pose_init", "bt_tracker_create", "bt_tracker_destroy", "bt_tracker_begin_frame", "bt_tracker_end_frame", "bt_tracker_drop_frame", "bt_tracker_state", "bt_tracker_usage",
     "bt_metrics_reserve", "bt_pose_metrics", "bt_vocap",
     "bt_dev_alloc", "bt_dev_free", "bt_memcpy_h2d", "bt_memcpy_d2h", "bt_host_alloc_pinned", "bt_host_free_pinned",
-    "bt_stream_sync",
+    "bt_stream_sync", "bt_debug_live_resources",
 ]
 
 _lib = None

@@ -44,15 +44,15 @@ extern "C" int bt_ctx_create(bt_ctx** out, int device) {
 extern "C" void bt_ctx_destroy(bt_ctx* ctx) {
 	if (!ctx) return;
 	cudaSetDevice(ctx->device);
-	bt::solver_destroy(ctx);
-	bt::matcher_destroy(ctx);
-	bt::ransac_destroy(ctx);
-	bt::prune_destroy(ctx);
-	bt::mcache_destroy(ctx);
-	bt::tracks_dev_destroy(ctx);
-	bt::front_destroy(ctx);
-	bt::metrics_destroy(ctx);
 	delete ctx;
+}
+
+// Test aid: what the handle types of bt_common.cuh hold right now, across the process.  Memory from bt_dev_alloc / bt_host_alloc_pinned
+// is the caller's and is not counted.
+extern "C" int bt_debug_live_resources(long long* device_bytes, long long* pinned_bytes, int* handles) {
+	BT_REQUIRE(device_bytes && pinned_bytes && handles, BT_ERR_INVALID_ARG, "bt_debug_live_resources: NULL argument");
+	*device_bytes = bt::g_live.dev_bytes; *pinned_bytes = bt::g_live.pinned_bytes; *handles = bt::g_live.handles;
+	return BT_OK;
 }
 
 extern "C" int bt_dev_alloc(void** out, size_t bytes) {

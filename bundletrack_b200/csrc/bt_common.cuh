@@ -4,6 +4,9 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <atomic>
+#include <memory>
+#include <utility>
 #include <vector>
 #include "../../include/bundletrack_b200.h"
 
@@ -25,35 +28,105 @@ void set_error(const char* fmt, ...);
 		if (!(cond)) { bt::set_error(__VA_ARGS__); return (code); }                                  \
 	} while (0)
 
-// A growable device buffer owned by the context (allocation happens in *_reserve, never on the per-call path
-// unless a call exceeds what was reserved, in which case the call fails with BT_ERR_CAPACITY).
-struct DevBuf {
+#define BT_TRY(x)                                                                                    \
+	do {                                                                                             \
+		const int rc_ = (x);                                                                         \
+		if (rc_ != BT_OK) return rc_;                                                                \
+	} while (0)
+
+// What the handle types below hold right now, across the process (bt_debug_live_resources).
+struct LiveResources { std::atomic<long long> dev_bytes{0}, pinned_bytes{0}; std::atomic<int> handles{0}; };
+inline LiveResources g_live;
+
+// A growable block of device memory (DevBuf) or page-locked host memory (PinnedBuf), freed with its owner.  `alloc` only grows: a block
+// that is large enough is kept, a larger one replaces it (contents are not kept).  The contexts allocate in *_reserve, never on the
+// per-call path unless a call exceeds what was reserved, in which case the call fails with BT_ERR_CAPACITY.
+template <bool Pinned>
+struct Block {
 	void* p = nullptr;
 	size_t bytes = 0;
+	Block() = default;
+	Block(const Block&) = delete;
+	Block& operator=(const Block&) = delete;
+	Block(Block&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+	Block& operator=(Block&& o) noexcept { std::swap(p, o.p); std::swap(bytes, o.bytes); return *this; }
+	~Block() { free(); }
 	int alloc(size_t n) {
 		if (n <= bytes) return BT_OK;
-		if (p) cudaFree(p);
-		p = nullptr; bytes = 0;
-		BT_CUDA(cudaMalloc(&p, n));
+		free();
+		if (Pinned) BT_CUDA(cudaMallocHost(&p, n));
+		else BT_CUDA(cudaMalloc(&p, n));
 		bytes = n;
+		live() += (long long)n;
 		return BT_OK;
 	}
-	void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
 	template <class T> T* as() const { return reinterpret_cast<T*>(p); }
+private:
+	static std::atomic<long long>& live() { return Pinned ? g_live.pinned_bytes : g_live.dev_bytes; }
+	void free() {
+		if (!p) return;
+		if (Pinned) cudaFreeHost(p);
+		else cudaFree(p);
+		live() -= (long long)bytes;
+		p = nullptr; bytes = 0;
+	}
 };
-struct PinnedBuf {
-	void* p = nullptr;
-	size_t bytes = 0;
-	int alloc(size_t n) {
-		if (n <= bytes) return BT_OK;
-		if (p) cudaFreeHost(p);
-		p = nullptr; bytes = 0;
-		BT_CUDA(cudaMallocHost(&p, n));
-		bytes = n;
+using DevBuf = Block<false>;
+using PinnedBuf = Block<true>;
+
+// A CUDA event created on first use and destroyed with its owner.  Timing events are created with create(true) before they are
+// recorded; record() creates the others without timing.
+struct Event {
+	cudaEvent_t e = nullptr;
+	Event() = default;
+	Event(const Event&) = delete;
+	Event& operator=(const Event&) = delete;
+	~Event() { if (e) { cudaEventDestroy(e); g_live.handles--; } }
+	int create(bool timing = false) {
+		if (e) return BT_OK;
+		BT_CUDA(cudaEventCreateWithFlags(&e, timing ? cudaEventDefault : cudaEventDisableTiming));
+		g_live.handles++;
 		return BT_OK;
 	}
-	void release() { if (p) cudaFreeHost(p); p = nullptr; bytes = 0; }
-	template <class T> T* as() const { return reinterpret_cast<T*>(p); }
+	int record(cudaStream_t stream) { BT_TRY(create()); BT_CUDA(cudaEventRecord(e, stream)); return BT_OK; }
+	int sync() const { if (e) BT_CUDA(cudaEventSynchronize(e)); return BT_OK; }     // (an event never recorded has nothing to wait for)
+	operator cudaEvent_t() const { return e; }
+};
+
+// A non-blocking CUDA stream created on first use and destroyed with its owner.
+struct Stream {
+	cudaStream_t s = nullptr;
+	Stream() = default;
+	Stream(const Stream&) = delete;
+	Stream& operator=(const Stream&) = delete;
+	~Stream() { if (s) { cudaStreamDestroy(s); g_live.handles--; } }
+	int create() {
+		if (s) return BT_OK;
+		BT_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+		g_live.handles++;
+		return BT_OK;
+	}
+	operator cudaStream_t() const { return s; }
+};
+
+// A page-locked block the host fills for an asynchronous upload, and the event recorded behind the copies that read it.  The entry
+// points return before those copies run, so the block is rewritten (acquire) or regrown (reserve) only once the event has passed.
+struct UploadBuf {
+	PinnedBuf buf;
+	Event ev;
+	// the block, at least `bytes` large (0: as reserved), once the last upload from it is done
+	template <class T> int acquire(size_t bytes, T** host) {
+		BT_TRY(ev.sync());
+		BT_TRY(buf.alloc(bytes));
+		*host = buf.as<T>();
+		return BT_OK;
+	}
+	int reserve(size_t bytes) {
+		if (bytes > buf.bytes) BT_TRY(ev.sync());
+		return buf.alloc(bytes);
+	}
+	// the copies from the block are queued on `stream`
+	int in_flight(cudaStream_t stream) { return ev.record(stream); }
 };
 
 struct SolverState;   // solver.cu
@@ -65,30 +138,36 @@ struct MatchCache;    // prune.cu
 struct TracksDev;     // tracks_dev.cu
 struct MetricsState;  // metrics.cu
 
+// The context owns the module states; each module defines the deleter of its state next to it, so the states stay private to their files.
+struct StateDeleter {
+	void operator()(SolverState*) const;
+	void operator()(MatcherState*) const;
+	void operator()(RansacState*) const;
+	void operator()(FrontState*) const;
+	void operator()(PruneState*) const;
+	void operator()(MatchCache*) const;
+	void operator()(TracksDev*) const;
+	void operator()(MetricsState*) const;
+};
+template <class T> using StatePtr = std::unique_ptr<T, StateDeleter>;
+
 }  // namespace bt
 
 struct bt_ctx {
 	int device = 0;
 	int sm_count = 0;
 	int cc_major = 0, cc_minor = 0;
-	bt::SolverState* solver = nullptr;
-	bt::MatcherState* matcher = nullptr;
-	bt::RansacState* ransac = nullptr;
-	bt::FrontState* front = nullptr;
-	bt::PruneState* prune = nullptr;
-	bt::MatchCache* mcache = nullptr;
-	bt::TracksDev* tracks = nullptr;
-	bt::MetricsState* metrics = nullptr;
+	bt::StatePtr<bt::SolverState> solver;
+	bt::StatePtr<bt::MatcherState> matcher;
+	bt::StatePtr<bt::RansacState> ransac;
+	bt::StatePtr<bt::FrontState> front;
+	bt::StatePtr<bt::PruneState> prune;
+	bt::StatePtr<bt::MatchCache> mcache;
+	bt::StatePtr<bt::TracksDev> tracks;
+	bt::StatePtr<bt::MetricsState> metrics;
 };
 
 namespace bt {
-void solver_destroy(bt_ctx* ctx);
-void matcher_destroy(bt_ctx* ctx);
-void ransac_destroy(bt_ctx* ctx);
-void prune_destroy(bt_ctx* ctx);
-void mcache_destroy(bt_ctx* ctx);
-void front_destroy(bt_ctx* ctx);
-void metrics_destroy(bt_ctx* ctx);
 // segment.cu: largest-hull mode for the masked front end, and the LF-Net request
 size_t hull_fill_smem(int H);
 int segment_largest_hull(const uint8_t* const* mask_tbl_dev, int n, int H, int W, int32_t* label, int32_t* count, unsigned long long* best,
@@ -96,7 +175,6 @@ int segment_largest_hull(const uint8_t* const* mask_tbl_dev, int n, int H, int W
 int launch_lfnet_request(const void* const* tbl_dev, const int32_t* roi_dev, int n, int H, int W, cudaStream_t stream);
 // tracks_dev.cu: the device map-point table, driven pair by pair from bt_find_corres_pairs (prune.cu).  Frames are named by slot;
 // tracks_slot maps a frame id to its slot (-1: the frame has no map yet, unless create is set).
-void tracks_dev_destroy(bt_ctx* ctx);
 int tracks_slot(bt_ctx* ctx, int frame_id, bool create, int* slot);
 int tracks_free_slots(bt_ctx* ctx);
 // map points alive now (created and not freed by forgets); synchronises `stream`

@@ -251,30 +251,18 @@ __global__ void __launch_bounds__(FE_THREADS) k_frame_frontend_masked(FrontArgs 
 
 struct FrontState {
 	DevBuf tables;
-	PinnedBuf h_tables;
+	UploadBuf h_tables;
 	int cap = 0;
-	cudaEvent_t ev_up = nullptr;
 	// largest-hull mode scratch (segment.cu), grown on demand: label / pixel-count maps, per-frame winner, the filled hull maps
 	DevBuf seg_label, seg_count, seg_best, seg_fill;
 	// bt_lfnet_request's own pointer tables, so it never waits on or overwrites the front end's
 	DevBuf req_tables;
-	PinnedBuf h_req;
-	cudaEvent_t ev_req = nullptr;
+	UploadBuf h_req;
 };
+void StateDeleter::operator()(FrontState* s) const { delete s; }
 static FrontState* g_front(bt_ctx* ctx, bool create) {
-	if (!ctx->front && create) ctx->front = new FrontState();
-	return ctx->front;
-}
-void front_destroy(bt_ctx* ctx) {
-	FrontState* s = ctx->front;
-	if (!s) return;
-	s->tables.release(); s->h_tables.release();
-	s->seg_label.release(); s->seg_count.release(); s->seg_best.release(); s->seg_fill.release();
-	s->req_tables.release(); s->h_req.release();
-	if (s->ev_up) cudaEventDestroy(s->ev_up);
-	if (s->ev_req) cudaEventDestroy(s->ev_req);
-	delete s;
-	ctx->front = nullptr;
+	if (!ctx->front && create) ctx->front.reset(new FrontState());
+	return ctx->front.get();
 }
 
 // The optional mask part of a front-end call (bt_frames_preprocess_masked).
@@ -316,10 +304,8 @@ static int frames_preprocess(bt_ctx* ctx, const char* who, int n_frames, const f
 		if ((rc = s->seg_fill.alloc(hw)) != BT_OK) return rc;
 		if ((rc = s->seg_best.alloc(sizeof(unsigned long long) * n_frames)) != BT_OK) return rc;
 	}
-	if (s->ev_up) BT_CUDA(cudaEventSynchronize(s->ev_up));
-	if ((rc = s->h_tables.alloc(bytes + roi_bytes)) != BT_OK) return rc;
-	if (!s->ev_up) BT_CUDA(cudaEventCreateWithFlags(&s->ev_up, cudaEventDisableTiming));
-	const void** ht = s->h_tables.as<const void*>();
+	const void** ht;
+	BT_TRY(s->h_tables.acquire(bytes + roi_bytes, &ht));
 	bool any_xyz = false;
 	for (int f = 0; f < n_frames; f++) {
 		BT_REQUIRE(depth_raw_dev[f] && depth_out_dev[f] && normal_out_dev[f], BT_ERR_INVALID_ARG, "%s: frame %d has a NULL map", who, f);
@@ -337,11 +323,11 @@ static int frames_preprocess(bt_ctx* ctx, const char* who, int n_frames, const f
 	if (xyz_out_dev) for (int f = 0; f < n_frames; f++) BT_REQUIRE(!any_xyz || xyz_out_dev[f], BT_ERR_INVALID_ARG, "%s: xyz outputs must be given for all frames or none", who);
 	BT_CUDA(cudaMemcpyAsync(s->tables.p, ht, bytes, cudaMemcpyHostToDevice, stream));
 	if (mask) {
-		int32_t* hr = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(s->h_tables.p) + bytes);
+		int32_t* hr = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(ht) + bytes);
 		for (int f = 0; f < n_frames; f++) { hr[4 * f] = 9999; hr[4 * f + 1] = 0; hr[4 * f + 2] = 9999; hr[4 * f + 3] = 0; }
 		BT_CUDA(cudaMemcpyAsync(mask->roi_out, hr, roi_bytes, cudaMemcpyHostToDevice, stream));
 	}
-	BT_CUDA(cudaEventRecord(s->ev_up, stream));
+	BT_TRY(s->h_tables.in_flight(stream));
 	FrontArgs a;
 	const void** dt = s->tables.as<const void*>();
 	a.depth_in = (const float* const*)dt; a.depth_out = (float* const*)(dt + n_frames);
@@ -402,15 +388,13 @@ extern "C" int bt_lfnet_request(bt_ctx* ctx, int n_frames, const uint8_t* const*
 	const size_t bytes = sizeof(void*) * 3 * (size_t)n_frames;   // [colour | fg | out]
 	int rc;
 	if ((rc = s->req_tables.alloc(bytes)) != BT_OK) return rc;
-	if (s->ev_req) BT_CUDA(cudaEventSynchronize(s->ev_req));
-	if ((rc = s->h_req.alloc(bytes)) != BT_OK) return rc;
-	if (!s->ev_req) BT_CUDA(cudaEventCreateWithFlags(&s->ev_req, cudaEventDisableTiming));
-	const void** ht = s->h_req.as<const void*>();
+	const void** ht;
+	BT_TRY(s->h_req.acquire(bytes, &ht));
 	for (int f = 0; f < n_frames; f++) {
 		BT_REQUIRE(colour_dev[f] && fg_dev[f] && request_out_dev[f], BT_ERR_INVALID_ARG, "bt_lfnet_request: frame %d has a NULL image", f);
 		ht[f] = colour_dev[f]; ht[n_frames + f] = fg_dev[f]; ht[2 * n_frames + f] = request_out_dev[f];
 	}
 	BT_CUDA(cudaMemcpyAsync(s->req_tables.p, ht, bytes, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaEventRecord(s->ev_req, stream));
+	BT_TRY(s->h_req.in_flight(stream));
 	return launch_lfnet_request(s->req_tables.as<const void*>(), roi_dev, n_frames, H, W, stream);
 }

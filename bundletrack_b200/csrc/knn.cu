@@ -751,31 +751,18 @@ struct MatcherState {
 	int n_transient = 0, n_persist = 0;     // transient slots [0, n_transient) serve bt_knn_match_pairs; persistent ones follow
 	std::vector<int> slot_n;                // persistent slots: number of rows stored, -1 = empty
 	DevBuf pool_h, pool_f, norms, errn, slot_meta, sets, pairs, pconst, G, jobs, blk_start, q_start, cand, cand_cnt, qjob, fb_rows, fb_count, fb_part_d, fb_part_i, fb_tickets;
-	PinnedBuf h_stage;
-	cudaEvent_t ev_up = nullptr;            // behind the upload of h_stage: the next call waits on it before rewriting the pinned block
+	UploadBuf h_stage;                      // the set and pair tables of a call
 	PFN_encodeTiled encode = nullptr;
 	CUtensorMap tmap_a, tmap_b;
 	bool maps_ready = false;
 	size_t g_halves_cap = 0;
 	int max_jobs = 0, max_q_total = 0, max_blocks = 0;
 	int last_units = 0, last_rows = 0;
-	cudaEvent_t ev[5] = { nullptr, nullptr, nullptr, nullptr, nullptr };
+	Event ev[5];
 	bool timing = false;
 	int force_fallback = 0;     // test knob: every n-th query row is sent to the exact fallback regardless of its candidates
 };
-
-void matcher_destroy(bt_ctx* ctx) {
-	MatcherState* m = ctx->matcher;
-	if (!m) return;
-	DevBuf* bufs[] = { &m->pool_h, &m->pool_f, &m->norms, &m->errn, &m->slot_meta, &m->sets, &m->pairs, &m->pconst, &m->G, &m->jobs, &m->blk_start, &m->q_start, &m->cand, &m->cand_cnt, &m->qjob,
-	                   &m->fb_rows, &m->fb_count, &m->fb_part_d, &m->fb_part_i, &m->fb_tickets };
-	for (DevBuf* b : bufs) b->release();
-	m->h_stage.release();
-	if (m->ev_up) cudaEventDestroy(m->ev_up);
-	for (auto& e : m->ev) if (e) cudaEventDestroy(e);
-	delete m;
-	ctx->matcher = nullptr;
-}
+void StateDeleter::operator()(MatcherState* m) const { delete m; }
 
 static int make_tmap(MatcherState* m, CUtensorMap* out, void* base, uint64_t rows, uint32_t box_rows) {
 	const cuuint64_t gdim[2] = { (cuuint64_t)KD, rows };
@@ -806,7 +793,7 @@ static int pool_alloc(MatcherState* m) {
 struct PoolSetRef { int slot; int n; };      // a descriptor set in the pool: rows [slot * slot_rows, +n)
 
 static int launch_prep(bt_ctx* ctx, const std::vector<PrepSet>& sets, char* hb, size_t& hoff, cudaStream_t stream) {
-	MatcherState* m = ctx->matcher;
+	MatcherState* m = ctx->matcher.get();
 	if (sets.empty()) return BT_OK;
 	const size_t b_sets = sizeof(PrepSet) * sets.size();
 	memcpy(hb + hoff, sets.data(), b_sets);
@@ -822,7 +809,7 @@ static int launch_prep(bt_ctx* ctx, const std::vector<PrepSet>& sets, char* hb, 
 // the matcher proper on descriptor sets that are already in the pool
 static int knn_run(bt_ctx* ctx, int n_pairs, const PoolSetRef* A, const PoolSetRef* B, int k, int32_t* idxAB, float* distAB, int32_t* idxBA, float* distBA,
                    char* hb, size_t hoff, cudaStream_t stream) {
-	MatcherState* m = ctx->matcher;
+	MatcherState* m = ctx->matcher.get();
 	std::vector<KnnPair> pairs;
 	std::vector<SelJob> jobs;
 	std::vector<int> blk_start, q_start;
@@ -871,7 +858,7 @@ static int knn_run(bt_ctx* ctx, int n_pairs, const PoolSetRef* A, const PoolSetR
 	BT_CUDA(cudaMemcpyAsync(m->jobs.p, h0 + b_pairs, b_jobs, cudaMemcpyHostToDevice, stream));
 	BT_CUDA(cudaMemcpyAsync(m->blk_start.p, h0 + b_pairs + b_jobs, b_int, cudaMemcpyHostToDevice, stream));
 	BT_CUDA(cudaMemcpyAsync(m->q_start.p, h0 + b_pairs + b_jobs + b_int, b_int, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaEventRecord(m->ev_up, stream));
+	BT_TRY(m->h_stage.in_flight(stream));
 	BT_CUDA(cudaMemsetAsync(m->fb_count.p, 0, 16, stream));
 	if (n_live > 0) k_knn_pairconst<<<(n_live + 127) / 128, 128, 0, stream>>>(m->pairs.as<KnnPair>(), n_live, m->slot_meta.as<int>(), m->pconst.as<PairConst>());
 	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[1], stream));      // [ev0, ev1) = descriptor conversion + table upload + per-pair constants; [ev1, ev2) = k_knn_tc alone
@@ -906,8 +893,8 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 	BT_REQUIRE(dim == KD, BT_ERR_UNSUPPORTED, "bt_matcher_reserve: descriptor dim %d unsupported (the tensor path is built for %d)", dim, KD);
 	BT_REQUIRE(max_pairs > 0 && max_feats > 0, BT_ERR_INVALID_ARG, "bt_matcher_reserve: bad limits");
 	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->matcher) ctx->matcher = new MatcherState();
-	MatcherState* m = ctx->matcher;
+	if (!ctx->matcher) ctx->matcher.reset(new MatcherState());
+	MatcherState* m = ctx->matcher.get();
 	if (!m->encode) {
 		void* fn = nullptr;
 		cudaDriverEntryPointQueryResult qres;
@@ -919,31 +906,27 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 	if (slot_rows != m->slot_rows || std::min(2 * max_pairs, 128) != m->n_transient) std::fill(m->slot_n.begin(), m->slot_n.end(), -1);     // the persistent slots move: what they held is dropped
 	m->max_pairs = max_pairs; m->max_feats = max_feats; m->dim = dim; m->slot_rows = slot_rows;
 	m->n_transient = std::min(2 * max_pairs, 128);       // distinct descriptor sets one bt_knn_match_pairs call may name (all pairs of K frames: K sets)
-	int rc;
-	if ((rc = pool_alloc(m)) != BT_OK) return rc;
+	BT_TRY(pool_alloc(m));
 	const int pad_a = (max_feats + BM - 1) / BM * BM;      // A sets are padded to whole 128-row tiles
 	m->g_halves_cap = (size_t)max_pairs * ((size_t)(slot_rows / GRP) * pad_a + (size_t)(pad_a / GRP) * slot_rows);
 	m->max_jobs = 2 * max_pairs;
 	m->max_q_total = 2 * max_pairs * max_feats;
 	m->max_blocks = 2 * max_pairs * ((max_feats + 127) / 128 * 2);      // k_knn_select covers whole 128-position blocks, 64 queries per CTA
-#define RES(buf, bytes) if ((rc = m->buf.alloc(bytes)) != BT_OK) return rc
-	RES(sets, sizeof(PrepSet) * (size_t)std::max(m->n_transient, 1));
-	RES(pairs, sizeof(KnnPair) * ((size_t)max_pairs + 1));
-	RES(pconst, sizeof(PairConst) * (size_t)max_pairs);
-	RES(G, m->g_halves_cap * 2 + 64);
-	RES(jobs, sizeof(SelJob) * m->max_jobs);
-	RES(blk_start, sizeof(int) * m->max_jobs); RES(q_start, sizeof(int) * m->max_jobs);
-	RES(cand, sizeof(int32_t) * SEL_MAXC * (size_t)m->max_q_total);
-	RES(cand_cnt, sizeof(int32_t) * (size_t)m->max_q_total);
-	RES(qjob, sizeof(int) * (size_t)m->max_q_total);
-	RES(fb_rows, sizeof(int) * (size_t)m->max_q_total);
-	RES(fb_count, 16);
-	RES(fb_part_d, sizeof(double) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8); RES(fb_part_i, sizeof(int) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8);
-	RES(fb_tickets, sizeof(int) * (size_t)FB_SPLIT_ROWS);
+	BT_TRY(m->sets.alloc(sizeof(PrepSet) * (size_t)std::max(m->n_transient, 1)));
+	BT_TRY(m->pairs.alloc(sizeof(KnnPair) * ((size_t)max_pairs + 1)));
+	BT_TRY(m->pconst.alloc(sizeof(PairConst) * (size_t)max_pairs));
+	BT_TRY(m->G.alloc(m->g_halves_cap * 2 + 64));
+	BT_TRY(m->jobs.alloc(sizeof(SelJob) * m->max_jobs));
+	BT_TRY(m->blk_start.alloc(sizeof(int) * m->max_jobs)); BT_TRY(m->q_start.alloc(sizeof(int) * m->max_jobs));
+	BT_TRY(m->cand.alloc(sizeof(int32_t) * SEL_MAXC * (size_t)m->max_q_total));
+	BT_TRY(m->cand_cnt.alloc(sizeof(int32_t) * (size_t)m->max_q_total));
+	BT_TRY(m->qjob.alloc(sizeof(int) * (size_t)m->max_q_total));
+	BT_TRY(m->fb_rows.alloc(sizeof(int) * (size_t)m->max_q_total));
+	BT_TRY(m->fb_count.alloc(16));
+	BT_TRY(m->fb_part_d.alloc(sizeof(double) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8)); BT_TRY(m->fb_part_i.alloc(sizeof(int) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8));
+	BT_TRY(m->fb_tickets.alloc(sizeof(int) * (size_t)FB_SPLIT_ROWS));
 	BT_CUDA(cudaMemset(m->fb_tickets.p, 0, sizeof(int) * (size_t)FB_SPLIT_ROWS));
-#undef RES
-	if ((rc = m->h_stage.alloc(sizeof(PrepSet) * 2 * max_pairs + sizeof(KnnPair) * ((size_t)max_pairs + 1) + (sizeof(SelJob) + 2 * sizeof(int)) * m->max_jobs + 4096)) != BT_OK) return rc;
-	if (!m->ev_up) BT_CUDA(cudaEventCreateWithFlags(&m->ev_up, cudaEventDisableTiming));
+	BT_TRY(m->h_stage.reserve(sizeof(PrepSet) * 2 * max_pairs + sizeof(KnnPair) * ((size_t)max_pairs + 1) + (sizeof(SelJob) + 2 * sizeof(int)) * m->max_jobs + 4096));
 	BT_CUDA(cudaFuncSetAttribute(k_knn_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_TOTAL));
 	return BT_OK;
 }
@@ -953,7 +936,7 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 extern "C" int bt_desc_pool_reserve(bt_ctx* ctx, int n_slots) {
 	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready, BT_ERR_INVALID_ARG, "bt_desc_pool_reserve: call bt_matcher_reserve first");
 	BT_REQUIRE(n_slots > 0, BT_ERR_INVALID_ARG, "bt_desc_pool_reserve: bad slot count");
-	MatcherState* m = ctx->matcher;
+	MatcherState* m = ctx->matcher.get();
 	BT_CUDA(cudaSetDevice(ctx->device));
 	if (n_slots <= m->n_persist) return BT_OK;
 	BT_CUDA(cudaDeviceSynchronize());          // the pool moves: nothing may still be reading the old one
@@ -964,7 +947,7 @@ extern "C" int bt_desc_pool_reserve(bt_ctx* ctx, int n_slots) {
 
 extern "C" int bt_desc_pool_store(bt_ctx* ctx, int slot, const bt_desc_view* desc, void* stream_) {
 	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready && desc, BT_ERR_INVALID_ARG, "bt_desc_pool_store: call bt_matcher_reserve / bt_desc_pool_reserve first");
-	MatcherState* m = ctx->matcher;
+	MatcherState* m = ctx->matcher.get();
 	BT_REQUIRE(slot >= 0 && slot < m->n_persist, BT_ERR_INVALID_ARG, "bt_desc_pool_store: slot %d outside [0,%d)", slot, m->n_persist);
 	BT_REQUIRE(desc->dim == KD, BT_ERR_UNSUPPORTED, "bt_desc_pool_store: descriptor dim %d != %d", desc->dim, KD);
 	BT_REQUIRE(desc->n >= 0 && desc->n <= m->max_feats, BT_ERR_CAPACITY, "bt_desc_pool_store: %d features > reserved %d", desc->n, m->max_feats);
@@ -972,13 +955,13 @@ extern "C" int bt_desc_pool_store(bt_ctx* ctx, int slot, const bt_desc_view* des
 	BT_REQUIRE(((uintptr_t)desc->dev & 15) == 0 && ((desc->pitch_bytes ? desc->pitch_bytes : (size_t)KD * 4) & 15) == 0, BT_ERR_INVALID_ARG, "bt_desc_pool_store: descriptors must be 16-byte aligned");
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
-	BT_CUDA(cudaEventSynchronize(m->ev_up));
+	char* hb;
+	BT_TRY(m->h_stage.acquire(0, &hb));
 	PrepSet s; s.src = desc->dev; s.pitch_bytes = desc->pitch_bytes ? desc->pitch_bytes : (size_t)KD * 4; s.n = desc->n;
 	s.slot = m->n_transient + slot; s.row0 = s.slot * m->slot_rows; s.rows_padded = (std::max(desc->n, 1) + BN - 1) / BN * BN;
 	size_t hoff = 0;
-	int rc = launch_prep(ctx, std::vector<PrepSet>(1, s), m->h_stage.as<char>(), hoff, stream);
-	if (rc != BT_OK) return rc;
-	BT_CUDA(cudaEventRecord(m->ev_up, stream));
+	BT_TRY(launch_prep(ctx, std::vector<PrepSet>(1, s), hb, hoff, stream));
+	BT_TRY(m->h_stage.in_flight(stream));
 	BT_CUDA(cudaGetLastError());
 	m->slot_n[slot] = desc->n;
 	return BT_OK;
@@ -989,7 +972,7 @@ extern "C" int bt_knn_match_slots(bt_ctx* ctx, int n_pairs, const int32_t* slotA
 	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready, BT_ERR_INVALID_ARG, "bt_knn_match_slots: call bt_matcher_reserve first");
 	BT_REQUIRE(slotA && slotB && idxAB && distAB && idxBA && distBA, BT_ERR_INVALID_ARG, "bt_knn_match_slots: NULL argument");
 	BT_REQUIRE(k >= 1 && k <= 8, BT_ERR_UNSUPPORTED, "bt_knn_match_slots: k=%d outside [1,8]", k);
-	MatcherState* m = ctx->matcher;
+	MatcherState* m = ctx->matcher.get();
 	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_REQUIRE(n_pairs > 0 && n_pairs <= m->max_pairs, BT_ERR_CAPACITY, "bt_knn_match_slots: %d pairs > reserved %d", n_pairs, m->max_pairs);
 	std::vector<PoolSetRef> A(n_pairs), B(n_pairs);
@@ -1000,10 +983,11 @@ extern "C" int bt_knn_match_slots(bt_ctx* ctx, int n_pairs, const int32_t* slotA
 			(s2 == 0 ? A[p] : B[p]) = PoolSetRef{ m->n_transient + sl, m->slot_n[sl] };
 		}
 	}
-	BT_CUDA(cudaEventSynchronize(m->ev_up));
+	char* hb;
+	BT_TRY(m->h_stage.acquire(0, &hb));
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[0], stream));
-	return knn_run(ctx, n_pairs, A.data(), B.data(), k, idxAB, distAB, idxBA, distBA, m->h_stage.as<char>(), 0, stream);
+	return knn_run(ctx, n_pairs, A.data(), B.data(), k, idxAB, distAB, idxBA, distBA, hb, 0, stream);
 }
 
 extern "C" int bt_knn_debug_force_fallback(bt_ctx* ctx, int every_nth) {
@@ -1014,15 +998,15 @@ extern "C" int bt_knn_debug_force_fallback(bt_ctx* ctx, int every_nth) {
 
 extern "C" int bt_knn_enable_timing(bt_ctx* ctx, int on) {
 	BT_REQUIRE(ctx && ctx->matcher, BT_ERR_INVALID_ARG, "bt_knn_enable_timing: call bt_matcher_reserve first");
-	MatcherState* m = ctx->matcher;
-	if (on) for (auto& e : m->ev) if (!e) BT_CUDA(cudaEventCreate(&e));
+	MatcherState* m = ctx->matcher.get();
+	if (on) for (Event& e : m->ev) BT_TRY(e.create(true));
 	m->timing = on != 0;
 	return BT_OK;
 }
 // ms4 = {descriptor prep, tensor-core pass, select + exact re-rank, exact fallback}; info3 = {units, query rows, fallback rows}
 extern "C" int bt_knn_get_timing(bt_ctx* ctx, float* ms4, int* info3) {
 	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->timing && ms4 && info3, BT_ERR_INVALID_ARG, "bt_knn_get_timing: timing not enabled");
-	MatcherState* m = ctx->matcher;
+	MatcherState* m = ctx->matcher.get();
 	BT_CUDA(cudaEventSynchronize(m->ev[4]));
 	for (int k = 0; k < 4; k++) BT_CUDA(cudaEventElapsedTime(ms4 + k, m->ev[k], m->ev[k + 1]));
 	int fb = 0;
@@ -1036,7 +1020,7 @@ extern "C" int bt_knn_match_pairs(bt_ctx* ctx, int n_pairs, const bt_desc_view* 
 	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready, BT_ERR_INVALID_ARG, "bt_knn_match_pairs: call bt_matcher_reserve first");
 	BT_REQUIRE(A && B && idxAB && distAB && idxBA && distBA, BT_ERR_INVALID_ARG, "bt_knn_match_pairs: NULL argument");
 	BT_REQUIRE(k >= 1 && k <= 8, BT_ERR_UNSUPPORTED, "bt_knn_match_pairs: k=%d outside [1,8]", k);
-	MatcherState* m = ctx->matcher;
+	MatcherState* m = ctx->matcher.get();
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_REQUIRE(n_pairs > 0 && n_pairs <= m->max_pairs, BT_ERR_CAPACITY, "bt_knn_match_pairs: %d pairs > reserved %d", n_pairs, m->max_pairs);
@@ -1064,11 +1048,10 @@ extern "C" int bt_knn_match_pairs(bt_ctx* ctx, int n_pairs, const bt_desc_view* 
 	std::vector<PoolSetRef> sa(n_pairs), sb(n_pairs);
 	for (int p = 0; p < n_pairs; p++) { sa[p] = PoolSetRef{ slot(A[p]), A[p].n }; sb[p] = PoolSetRef{ slot(B[p]), B[p].n }; }
 	BT_REQUIRE((int)sets.size() <= m->n_transient, BT_ERR_CAPACITY, "bt_knn_match_pairs: %d distinct descriptor sets in one call > %d (store them with bt_desc_pool_store and use bt_knn_match_slots)", (int)sets.size(), m->n_transient);
-	// the entry points are asynchronous: an earlier call's table upload may still be reading the pinned block
-	BT_CUDA(cudaEventSynchronize(m->ev_up));
+	char* hb;
+	BT_TRY(m->h_stage.acquire(0, &hb));
 	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[0], stream));
 	size_t hoff = 0;
-	int rc = launch_prep(ctx, sets, m->h_stage.as<char>(), hoff, stream);
-	if (rc != BT_OK) return rc;
-	return knn_run(ctx, n_pairs, sa.data(), sb.data(), k, idxAB, distAB, idxBA, distBA, m->h_stage.as<char>(), hoff, stream);
+	BT_TRY(launch_prep(ctx, sets, hb, hoff, stream));
+	return knn_run(ctx, n_pairs, sa.data(), sb.data(), k, idxAB, distAB, idxBA, distBA, hb, hoff, stream);
 }

@@ -227,19 +227,9 @@ void frame_const(const double* pred, const double* gt, FrameConst& fc) {
 struct MetricsState {
 	int max_pts = 0, max_frames = 0;
 	DevBuf pts32, frames, part, pmax;
-	PinnedBuf h_frames;
-	cudaEvent_t ev_up = nullptr;      // recorded behind the upload of h_frames: the next call waits on it before rewriting the pinned block
+	UploadBuf h_frames;
 };
-
-void metrics_destroy(bt_ctx* ctx) {
-	MetricsState* s = ctx->metrics;
-	if (!s) return;
-	s->pts32.release(); s->frames.release(); s->part.release(); s->pmax.release();
-	s->h_frames.release();
-	if (s->ev_up) cudaEventDestroy(s->ev_up);
-	delete s;
-	ctx->metrics = nullptr;
-}
+void StateDeleter::operator()(MetricsState* s) const { delete s; }
 
 }  // namespace bt
 
@@ -250,15 +240,14 @@ extern "C" int bt_metrics_reserve(bt_ctx* ctx, int max_pts, int max_frames) {
 	BT_REQUIRE(max_pts >= 1 && max_frames >= 1, BT_ERR_INVALID_ARG, "bt_metrics_reserve: max_pts %d / max_frames %d must be >= 1", max_pts, max_frames);
 	BT_REQUIRE((max_pts + kChunk - 1) / kChunk <= 65535, BT_ERR_INVALID_ARG, "bt_metrics_reserve: max_pts %d > %d", max_pts, 65535 * kChunk);
 	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->metrics) ctx->metrics = new MetricsState();
-	MetricsState* s = ctx->metrics;
+	if (!ctx->metrics) ctx->metrics.reset(new MetricsState());
+	MetricsState* s = ctx->metrics.get();
 	const size_t n_chunks = (size_t)(max_pts + kChunk - 1) / kChunk;
-	int rc;
-	if ((rc = s->pts32.alloc(sizeof(float4) * (size_t)max_pts)) != BT_OK) return rc;
-	if ((rc = s->frames.alloc(sizeof(FrameConst) * (size_t)max_frames)) != BT_OK) return rc;
-	if ((rc = s->part.alloc(2 * sizeof(double) * n_chunks * max_frames)) != BT_OK) return rc;
-	if ((rc = s->pmax.alloc(sizeof(unsigned long long))) != BT_OK) return rc;
-	if ((rc = s->h_frames.alloc(sizeof(FrameConst) * (size_t)max_frames)) != BT_OK) return rc;
+	BT_TRY(s->pts32.alloc(sizeof(float4) * (size_t)max_pts));
+	BT_TRY(s->frames.alloc(sizeof(FrameConst) * (size_t)max_frames));
+	BT_TRY(s->part.alloc(2 * sizeof(double) * n_chunks * max_frames));
+	BT_TRY(s->pmax.alloc(sizeof(unsigned long long)));
+	BT_TRY(s->h_frames.reserve(sizeof(FrameConst) * (size_t)max_frames));
 	s->max_pts = max_pts; s->max_frames = max_frames;
 	return BT_OK;
 }
@@ -270,19 +259,17 @@ extern "C" int bt_pose_metrics(bt_ctx* ctx, const double* model_pts_dev, int n_p
 	for (size_t k = 0; k < 16 * (size_t)n_frames; k++)
 		BT_REQUIRE(isfinite(pred_ob_in_cam[k]) && isfinite(gt_ob_in_cam[k]), BT_ERR_INVALID_ARG, "bt_pose_metrics: frame %d has a non-finite pose element", (int)(k / 16));
 	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_pose_metrics: ctx is NULL");
-	MetricsState* s = ctx->metrics;
+	MetricsState* s = ctx->metrics.get();
 	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_pose_metrics: call bt_metrics_reserve first");
 	BT_REQUIRE(n_pts <= s->max_pts && n_frames <= s->max_frames, BT_ERR_CAPACITY, "bt_pose_metrics: %d points / %d frames exceed the reserved %d / %d",
 	           n_pts, n_frames, s->max_pts, s->max_frames);
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
-	// the call is asynchronous: an earlier call's upload may still be reading the pinned block
-	if (!s->ev_up) BT_CUDA(cudaEventCreateWithFlags(&s->ev_up, cudaEventDisableTiming));
-	else BT_CUDA(cudaEventSynchronize(s->ev_up));
-	FrameConst* hf = s->h_frames.as<FrameConst>();
+	FrameConst* hf;
+	BT_TRY(s->h_frames.acquire(0, &hf));
 	for (int f = 0; f < n_frames; f++) frame_const(pred_ob_in_cam + 16 * (size_t)f, gt_ob_in_cam + 16 * (size_t)f, hf[f]);
 	BT_CUDA(cudaMemcpyAsync(s->frames.p, hf, sizeof(FrameConst) * (size_t)n_frames, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaEventRecord(s->ev_up, stream));
+	BT_TRY(s->h_frames.in_flight(stream));
 	BT_CUDA(cudaMemsetAsync(s->pmax.p, 0, sizeof(unsigned long long), stream));
 	k_metrics_prep<<<(n_pts + kThreads - 1) / kThreads, kThreads, 0, stream>>>(model_pts_dev, n_pts, s->pts32.as<float4>(), s->pmax.as<unsigned long long>());
 	const int n_chunks = (n_pts + kChunk - 1) / kChunk;

@@ -235,68 +235,47 @@ __global__ void __launch_bounds__(256) k_emit_fill(const PrunePair* __restrict__
 struct PruneState {
 	int max_pairs = 0, max_feats = 0;
 	DevBuf pairs, corr, PA, PB, n_corr, n_nn, rpairs, inl, n_inl, idxAB, distAB, idxBA, distBA, entry_off, total, extra, n_prop;
-	PinnedBuf h_pairs, h_extra;
+	UploadBuf h_pairs, h_extra;
 	size_t extra_cap = 0;               // propagated matches (float4 each) one call may carry
-	cudaEvent_t ev_up = nullptr;      // recorded behind the upload of h_pairs (the calls are asynchronous: see fill_pairs)
 };
-static PruneState* g_prune_of(bt_ctx* ctx);
+void StateDeleter::operator()(PruneState* s) const { delete s; }
 
 }  // namespace bt
 
 using namespace bt;
 
-// The prune state is owned by the context like the solver / matcher / RANSAC / front-end states.
-namespace bt {
-static PruneState* g_prune_of(bt_ctx* ctx) { return ctx->prune; }
-void prune_destroy(bt_ctx* ctx) {
-	PruneState* s = ctx->prune;
-	if (!s) return;
-	DevBuf* bufs[] = { &s->pairs, &s->corr, &s->PA, &s->PB, &s->n_corr, &s->n_nn, &s->extra, &s->rpairs, &s->inl, &s->n_inl, &s->idxAB, &s->distAB, &s->idxBA, &s->distBA, &s->entry_off, &s->total, &s->n_prop };
-	for (DevBuf* b : bufs) b->release();
-	s->h_pairs.release(); s->h_extra.release();
-	if (s->ev_up) cudaEventDestroy(s->ev_up);
-	delete s;
-	ctx->prune = nullptr;
-}
-}
-
 extern "C" int bt_pipeline_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int dim, int max_trials) {
 	BT_REQUIRE(ctx && max_pairs > 0 && max_feats > 0, BT_ERR_INVALID_ARG, "bt_pipeline_reserve: bad arguments");
-	int rc = bt_matcher_reserve(ctx, max_pairs, max_feats, dim);
-	if (rc != BT_OK) return rc;
-	rc = bt_ransac_reserve(ctx, max_pairs, 3 * max_feats, max_trials);
-	if (rc != BT_OK) return rc;
-	PruneState* s = g_prune_of(ctx);
-	if (!s) { s = new PruneState(); ctx->prune = s; }
+	BT_TRY(bt_matcher_reserve(ctx, max_pairs, max_feats, dim));
+	BT_TRY(bt_ransac_reserve(ctx, max_pairs, 3 * max_feats, max_trials));
+	if (!ctx->prune) ctx->prune.reset(new PruneState());
+	PruneState* s = ctx->prune.get();
 	s->max_pairs = max_pairs; s->max_feats = max_feats;
 	const size_t cap = (size_t)3 * max_feats * max_pairs;      // nA + nB mutual candidates + up to max_feats propagated map-point matches per pair
 	s->extra_cap = (size_t)max_feats * max_pairs;
-#define RES(buf, bytes) if ((rc = s->buf.alloc(bytes)) != BT_OK) return rc
-	RES(pairs, sizeof(PrunePair) * max_pairs);
-	RES(corr, sizeof(bt_correspondence) * cap);
-	RES(PA, sizeof(float4) * cap); RES(PB, sizeof(float4) * cap);
-	RES(n_corr, sizeof(int32_t) * max_pairs); RES(n_nn, sizeof(int32_t) * max_pairs);
-	RES(extra, sizeof(float4) * s->extra_cap);
-	RES(rpairs, sizeof(RansacPair) * max_pairs);
-	RES(inl, sizeof(int32_t) * cap); RES(n_inl, sizeof(int32_t) * max_pairs);
-	RES(idxAB, sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs); RES(distAB, sizeof(float) * 8 * (size_t)max_feats * max_pairs);
-	RES(idxBA, sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs); RES(distBA, sizeof(float) * 8 * (size_t)max_feats * max_pairs);
-	RES(entry_off, sizeof(int32_t) * max_pairs); RES(total, 16); RES(n_prop, sizeof(int32_t) * max_pairs);
-#undef RES
-	if ((rc = s->h_extra.alloc(sizeof(float4) * s->extra_cap)) != BT_OK) return rc;
-	return s->h_pairs.alloc(sizeof(PrunePair) * max_pairs);
+	BT_TRY(s->pairs.alloc(sizeof(PrunePair) * max_pairs));
+	BT_TRY(s->corr.alloc(sizeof(bt_correspondence) * cap));
+	BT_TRY(s->PA.alloc(sizeof(float4) * cap)); BT_TRY(s->PB.alloc(sizeof(float4) * cap));
+	BT_TRY(s->n_corr.alloc(sizeof(int32_t) * max_pairs)); BT_TRY(s->n_nn.alloc(sizeof(int32_t) * max_pairs));
+	BT_TRY(s->extra.alloc(sizeof(float4) * s->extra_cap));
+	BT_TRY(s->rpairs.alloc(sizeof(RansacPair) * max_pairs));
+	BT_TRY(s->inl.alloc(sizeof(int32_t) * cap)); BT_TRY(s->n_inl.alloc(sizeof(int32_t) * max_pairs));
+	BT_TRY(s->idxAB.alloc(sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs)); BT_TRY(s->distAB.alloc(sizeof(float) * 8 * (size_t)max_feats * max_pairs));
+	BT_TRY(s->idxBA.alloc(sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs)); BT_TRY(s->distBA.alloc(sizeof(float) * 8 * (size_t)max_feats * max_pairs));
+	BT_TRY(s->entry_off.alloc(sizeof(int32_t) * max_pairs)); BT_TRY(s->total.alloc(16)); BT_TRY(s->n_prop.alloc(sizeof(int32_t) * max_pairs));
+	BT_TRY(s->h_extra.reserve(sizeof(float4) * s->extra_cap));
+	return s->h_pairs.reserve(sizeof(PrunePair) * max_pairs);
 }
 
 // prop_room > 0 (bt_find_corres_pairs): no host extras; pair p keeps room for prop_room propagated matches behind its mutual ones, and its
 // candidates go to extra[p * prop_room, ...) when the device table writes them
 static int fill_pairs(PruneState* s, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, cudaStream_t stream, const bt_match_extra* extra = nullptr,
                       int prop_room = 0) {
-	// an earlier asynchronous call's upload may still be reading the pinned table: wait for it before rewriting the block
-	if (!s->ev_up) BT_CUDA(cudaEventCreateWithFlags(&s->ev_up, cudaEventDisableTiming));
-	else BT_CUDA(cudaEventSynchronize(s->ev_up));
-	PrunePair* hp = s->h_pairs.as<PrunePair>();
+	PrunePair* hp;
+	float4* hx;
+	BT_TRY(s->h_pairs.acquire(0, &hp));
+	BT_TRY(s->h_extra.acquire(0, &hx));
 	int offA = 0, offB = 0, out = 0, xoff = 0;
-	float4* hx = s->h_extra.as<float4>();
 	for (int p = 0; p < n_pairs; p++) {
 		const bt_match_frame* fr[2] = { &A[p], &B[p] };
 		PruneFrame* dst[2] = { &hp[p].A, &hp[p].B };
@@ -317,16 +296,18 @@ static int fill_pairs(PruneState* s, int n_pairs, const bt_match_frame* A, const
 		xoff += nx;
 		offA += A[p].n; offB += B[p].n; out += A[p].n + B[p].n + nx + prop_room;
 	}
-	if (xoff) BT_CUDA(cudaMemcpyAsync(s->extra.p, hx, sizeof(float4) * (size_t)xoff, cudaMemcpyHostToDevice, stream));
+	if (xoff) {
+		BT_CUDA(cudaMemcpyAsync(s->extra.p, hx, sizeof(float4) * (size_t)xoff, cudaMemcpyHostToDevice, stream));
+		BT_TRY(s->h_extra.in_flight(stream));
+	}
 	BT_CUDA(cudaMemcpyAsync(s->pairs.p, hp, sizeof(PrunePair) * n_pairs, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaEventRecord(s->ev_up, stream));
-	return BT_OK;
+	return s->h_pairs.in_flight(stream);
 }
 
 static int prune_mutual_impl(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, int H, int W, float fx, float fy, float cx, float cy,
                              const int32_t* idxAB, const int32_t* idxBA, int k, const bt_prune_params* prm,
                              bt_correspondence* corr_out, int32_t* n_corr_out, void* stream_, const bt_match_extra* extra) {
-	PruneState* s = ctx ? g_prune_of(ctx) : nullptr;
+	PruneState* s = ctx ? ctx->prune.get() : nullptr;
 	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_prune_mutual_pairs: call bt_pipeline_reserve first");
 	BT_REQUIRE(A && B && idxAB && idxBA && prm && corr_out && n_corr_out && n_pairs > 0 && n_pairs <= s->max_pairs && k >= 1 && k <= 8, BT_ERR_INVALID_ARG, "bt_prune_mutual_pairs: bad argument");
 	cudaStream_t stream = (cudaStream_t)stream_;
@@ -353,7 +334,7 @@ static int match_pairs_impl(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, c
                             const int32_t* slotA, const int32_t* slotB, int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune, int ransac_trials,
                             float ransac_inlier_dist, uint64_t ransac_seed, bt_entryj* entry_out, int entry_capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, void* stream_,
                             const bt_match_extra* extra = nullptr, int32_t* status_out = nullptr, float* uv_out = nullptr) {
-	PruneState* s = ctx ? g_prune_of(ctx) : nullptr;
+	PruneState* s = ctx ? ctx->prune.get() : nullptr;
 	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_match_pairs: call bt_pipeline_reserve first");
 	BT_REQUIRE(A && B && ((dA && dB) || (slotA && slotB)) && prune && entry_out && n_entry_out && entry_off_out && total_out && n_pairs > 0 && n_pairs <= s->max_pairs, BT_ERR_INVALID_ARG, "bt_match_pairs: bad argument");
 	cudaStream_t stream = (cudaStream_t)stream_;
@@ -408,7 +389,7 @@ extern "C" int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_fra
                                     const int32_t* slotA, const int32_t* slotB, int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune,
                                     int ransac_trials, float ransac_inlier_dist, uint64_t ransac_seed, bt_entryj* entry_out, int entry_capacity,
                                     int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, int32_t* status_out, float* uv_out, void* stream_) {
-	PruneState* s = ctx ? g_prune_of(ctx) : nullptr;
+	PruneState* s = ctx ? ctx->prune.get() : nullptr;
 	BT_REQUIRE(s && ctx->tracks, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: call bt_pipeline_reserve and bt_tracks_dev_reserve first");
 	BT_REQUIRE(((dA && dB) ? 1 : 0) + ((slotA && slotB) ? 1 : 0) == 1, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: give either descriptor views or pool slots");
 	BT_REQUIRE(A && B && prune && entry_out && entry_capacity >= 0 && n_entry_out && entry_off_out && total_out && n_pairs > 0 && n_pairs <= s->max_pairs,
@@ -438,7 +419,7 @@ extern "C" int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_fra
 	int32_t* n_corr = s->n_corr.as<int32_t>();
 	k_prune_mutual<<<n_pairs, 512, 0, stream>>>(dp, cam, s->idxAB.as<int32_t>(), s->idxBA.as<int32_t>(), k, *prune, corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr);
 	BT_CUDA(cudaGetLastError());
-	const PrunePair* hp = s->h_pairs.as<PrunePair>();       // (fill_pairs' host copy: out_off per pair)
+	const PrunePair* hp = s->h_pairs.buf.as<PrunePair>();   // (fill_pairs' host copy: out_off per pair)
 	for (int p = 0; p < n_pairs; p++) {
 		int sa, sb;
 		if (abs(A[p].frame_id - B[p].frame_id) != 1) {       // findCorresByMapPoints
@@ -513,38 +494,29 @@ struct MatchCache {
 	int max_pairs = 0, max_block = 0;  // pairs cached at once; entries per block (the arena size for bt_match_cache_reserve_entries)
 	long long cap = 0, top = 0, live = 0;   // arena entries: size, end of the last block placed, entries in live blocks
 	DevBuf arena, tab;
-	PinnedBuf h_tab[2];
-	cudaEvent_t ev[2] = { nullptr, nullptr };
+	UploadBuf h_tab[2];                 // used in turn: a call waits only for the upload of the call before last
 	int flip = 0;
 	struct Rec { long long off; int n, status; };
 	std::map<std::pair<int, int>, Rec> recs;
 };
-void mcache_destroy(bt_ctx* ctx) {
-	MatchCache* c = ctx->mcache;
-	if (!c) return;
-	c->arena.release(); c->tab.release(); c->h_tab[0].release(); c->h_tab[1].release();
-	for (auto& e : c->ev) if (e) cudaEventDestroy(e);
-	delete c;
-	ctx->mcache = nullptr;
-}
+void StateDeleter::operator()(MatchCache* c) const { delete c; }
 static int cache_upload(MatchCache* c, const std::vector<CacheMove>& mv, cudaStream_t stream) {
-	const int fl = c->flip; c->flip ^= 1;
-	if (!c->ev[fl]) BT_CUDA(cudaEventCreateWithFlags(&c->ev[fl], cudaEventDisableTiming));
-	else BT_CUDA(cudaEventSynchronize(c->ev[fl]));
-	memcpy(c->h_tab[fl].p, mv.data(), sizeof(CacheMove) * mv.size());
-	BT_CUDA(cudaMemcpyAsync(c->tab.p, c->h_tab[fl].p, sizeof(CacheMove) * mv.size(), cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaEventRecord(c->ev[fl], stream));
-	return BT_OK;
+	UploadBuf& up = c->h_tab[c->flip];
+	c->flip ^= 1;
+	CacheMove* h;
+	BT_TRY(up.acquire(0, &h));
+	memcpy(h, mv.data(), sizeof(CacheMove) * mv.size());
+	BT_CUDA(cudaMemcpyAsync(c->tab.p, h, sizeof(CacheMove) * mv.size(), cudaMemcpyHostToDevice, stream));
+	return up.in_flight(stream);
 }
 static int cache_reserve(bt_ctx* ctx, int max_pairs_cached, int max_block, long long total) {
 	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->mcache) ctx->mcache = new MatchCache();
-	MatchCache* c = ctx->mcache;
-	int rc;
-	if ((rc = c->arena.alloc(sizeof(bt_entryj) * (size_t)total)) != BT_OK) return rc;
+	if (!ctx->mcache) ctx->mcache.reset(new MatchCache());
+	MatchCache* c = ctx->mcache.get();
+	BT_TRY(c->arena.alloc(sizeof(bt_entryj) * (size_t)total));
 	// a put uploads the compaction (every live block) and its own blocks in one table
-	if ((rc = c->tab.alloc(sizeof(CacheMove) * 2 * (size_t)max_pairs_cached)) != BT_OK) return rc;
-	for (auto& h : c->h_tab) if ((rc = h.alloc(sizeof(CacheMove) * 2 * (size_t)max_pairs_cached)) != BT_OK) return rc;
+	BT_TRY(c->tab.alloc(sizeof(CacheMove) * 2 * (size_t)max_pairs_cached));
+	for (UploadBuf& h : c->h_tab) BT_TRY(h.reserve(sizeof(CacheMove) * 2 * (size_t)max_pairs_cached));
 	c->max_pairs = max_pairs_cached; c->max_block = max_block;
 	c->cap = total; c->top = 0; c->live = 0;
 	c->recs.clear();
@@ -566,7 +538,7 @@ extern "C" int bt_match_cache_reserve_entries(bt_ctx* ctx, int max_pairs_cached,
 extern "C" int bt_match_cache_put(bt_ctx* ctx, int n_pairs, const int32_t* idA, const int32_t* idB, const bt_entryj* entry_dev,
                                   const int32_t* n_entry_host, const int32_t* entry_off_host, const int32_t* status_host, void* stream_) {
 	BT_REQUIRE(ctx && ctx->mcache && idA && idB && n_entry_host && entry_off_host && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_match_cache_put: call bt_match_cache_reserve first / NULL argument");
-	MatchCache* c = ctx->mcache;
+	MatchCache* c = ctx->mcache.get();
 	BT_REQUIRE(n_pairs <= c->max_pairs, BT_ERR_CAPACITY, "bt_match_cache_put: %d pairs > table of %d", n_pairs, c->max_pairs);
 	BT_CUDA(cudaSetDevice(ctx->device));
 	// check everything before changing anything: a refused put leaves the cache as it was.  A pair listed twice keeps its last block.
@@ -651,7 +623,7 @@ extern "C" int bt_match_cache_usage(bt_ctx* ctx, int* n_pairs, long long* n_entr
 extern "C" int bt_match_cache_gather(bt_ctx* ctx, int n_pairs, const int32_t* idA, const int32_t* idB, const uint32_t* win_i, const uint32_t* win_j,
                                      bt_entryj* dst_dev, int capacity, int32_t* block_off_host, int32_t* block_n_host, void* stream_) {
 	BT_REQUIRE(ctx && ctx->mcache && idA && idB && win_i && win_j && dst_dev && block_off_host && block_n_host && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_match_cache_gather: NULL argument");
-	MatchCache* c = ctx->mcache;
+	MatchCache* c = ctx->mcache.get();
 	BT_REQUIRE(n_pairs <= c->max_pairs, BT_ERR_CAPACITY, "bt_match_cache_gather: %d pairs > table of %d", n_pairs, c->max_pairs);
 	BT_CUDA(cudaSetDevice(ctx->device));
 	std::vector<CacheMove> mv;
@@ -676,7 +648,7 @@ extern "C" int bt_match_cache_gather(bt_ctx* ctx, int n_pairs, const int32_t* id
 
 extern "C" int bt_match_cache_forget_frame(bt_ctx* ctx, int frame_id) {
 	BT_REQUIRE(ctx && ctx->mcache, BT_ERR_INVALID_ARG, "bt_match_cache_forget_frame: call bt_match_cache_reserve first");
-	MatchCache* c = ctx->mcache;
+	MatchCache* c = ctx->mcache.get();
 	for (auto it = c->recs.begin(); it != c->recs.end();) {
 		if (it->first.first == frame_id || it->first.second == frame_id) { c->live -= it->second.n; it = c->recs.erase(it); }
 		else ++it;

@@ -221,27 +221,16 @@ __global__ void __launch_bounds__(256) k_ransac_inliers(const RansacPair* __rest
 struct RansacState {
 	int max_pairs = 0, max_pts = 0, max_trials = 0;
 	DevBuf pairs, table, poses, good, best, best_trial;
-	PinnedBuf h_pairs;
-	cudaEvent_t ev_up = nullptr;      // recorded behind the upload of h_pairs: the next call waits on it before rewriting the pinned block
+	UploadBuf h_pairs;
 	unsigned long long table_seed = ~0ull;
 	int table_trials = 0;
 };
-
-void ransac_destroy(bt_ctx* ctx) {
-	RansacState* r = ctx->ransac;
-	if (!r) return;
-	DevBuf* bufs[] = { &r->pairs, &r->table, &r->poses, &r->good, &r->best, &r->best_trial };
-	for (DevBuf* b : bufs) b->release();
-	r->h_pairs.release();
-	if (r->ev_up) cudaEventDestroy(r->ev_up);
-	delete r;
-	ctx->ransac = nullptr;
-}
+void StateDeleter::operator()(RansacState* r) const { delete r; }
 
 // shared by the host-pointer API below and the fused matcher pipeline (pairs table already on the device)
 int ransac_run_device(bt_ctx* ctx, const RansacPair* d_pairs, int n_pairs, int n_trials, float dist_thresh, uint64_t seed,
                       int32_t* inlier_ids_out, int32_t* n_inliers_out, cudaStream_t stream) {
-	RansacState* r = ctx->ransac;
+	RansacState* r = ctx->ransac.get();
 	BT_REQUIRE(r, BT_ERR_INVALID_ARG, "ransac: call bt_ransac_reserve first");
 	BT_REQUIRE(n_pairs <= r->max_pairs && n_trials <= r->max_trials && n_trials > 0, BT_ERR_CAPACITY, "ransac: %d pairs / %d trials exceed the reserved %d / %d", n_pairs, n_trials, r->max_pairs, r->max_trials);
 	if (r->table_seed != seed || r->table_trials < n_trials) {
@@ -271,19 +260,16 @@ using namespace bt;
 extern "C" int bt_ransac_reserve(bt_ctx* ctx, int max_pairs, int max_pts, int max_trials) {
 	BT_REQUIRE(ctx && max_pairs > 0 && max_pts > 0 && max_trials > 0, BT_ERR_INVALID_ARG, "bt_ransac_reserve: bad arguments");
 	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->ransac) ctx->ransac = new RansacState();
-	RansacState* r = ctx->ransac;
+	if (!ctx->ransac) ctx->ransac.reset(new RansacState());
+	RansacState* r = ctx->ransac.get();
 	r->max_pairs = max_pairs; r->max_pts = max_pts; r->max_trials = max_trials;
-	int rc;
-#define RES(buf, bytes) if ((rc = r->buf.alloc(bytes)) != BT_OK) return rc
-	RES(pairs, sizeof(RansacPair) * max_pairs);
-	RES(table, sizeof(float) * 3 * max_trials);
-	RES(poses, sizeof(float) * 12 * (size_t)max_pairs * max_trials);
-	RES(good, sizeof(int) * (size_t)max_pairs * max_trials);
-	RES(best, sizeof(unsigned long long) * max_pairs);
-	RES(best_trial, sizeof(int32_t) * max_pairs);
-#undef RES
-	if ((rc = r->h_pairs.alloc(sizeof(RansacPair) * max_pairs)) != BT_OK) return rc;
+	BT_TRY(r->pairs.alloc(sizeof(RansacPair) * max_pairs));
+	BT_TRY(r->table.alloc(sizeof(float) * 3 * max_trials));
+	BT_TRY(r->poses.alloc(sizeof(float) * 12 * (size_t)max_pairs * max_trials));
+	BT_TRY(r->good.alloc(sizeof(int) * (size_t)max_pairs * max_trials));
+	BT_TRY(r->best.alloc(sizeof(unsigned long long) * max_pairs));
+	BT_TRY(r->best_trial.alloc(sizeof(int32_t) * max_pairs));
+	BT_TRY(r->h_pairs.reserve(sizeof(RansacPair) * max_pairs));
 	r->table_seed = ~0ull; r->table_trials = 0;
 	return BT_OK;
 }
@@ -292,14 +278,12 @@ extern "C" int bt_ransac_pairs(bt_ctx* ctx, int n_pairs, const float* const* pts
                                uint64_t seed, int32_t* inlier_ids_out, int32_t* n_inliers_out, void* stream_) {
 	BT_REQUIRE(ctx && ctx->ransac, BT_ERR_INVALID_ARG, "bt_ransac_pairs: call bt_ransac_reserve first");
 	BT_REQUIRE(ptsA && ptsB && n_pts && inlier_ids_out && n_inliers_out && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_ransac_pairs: NULL argument");
-	RansacState* r = ctx->ransac;
+	RansacState* r = ctx->ransac.get();
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_REQUIRE(n_pairs <= r->max_pairs, BT_ERR_CAPACITY, "bt_ransac_pairs: %d pairs > reserved %d", n_pairs, r->max_pairs);
-	// the entry points are asynchronous: an earlier call's upload may still be reading the pinned table
-	if (!r->ev_up) BT_CUDA(cudaEventCreateWithFlags(&r->ev_up, cudaEventDisableTiming));
-	else BT_CUDA(cudaEventSynchronize(r->ev_up));
-	RansacPair* hp = r->h_pairs.as<RansacPair>();
+	RansacPair* hp;
+	BT_TRY(r->h_pairs.acquire(0, &hp));
 	int off = 0;
 	for (int p = 0; p < n_pairs; p++) {
 		BT_REQUIRE(n_pts[p] >= 0 && n_pts[p] <= r->max_pts, BT_ERR_CAPACITY, "bt_ransac_pairs: pair %d has %d points > reserved %d", p, n_pts[p], r->max_pts);
@@ -307,14 +291,14 @@ extern "C" int bt_ransac_pairs(bt_ctx* ctx, int n_pairs, const float* const* pts
 		off += n_pts[p];
 	}
 	BT_CUDA(cudaMemcpyAsync(r->pairs.p, hp, sizeof(RansacPair) * n_pairs, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaEventRecord(r->ev_up, stream));
+	BT_TRY(r->h_pairs.in_flight(stream));
 	return ransac_run_device(ctx, r->pairs.as<RansacPair>(), n_pairs, n_trials, dist_thresh, seed, inlier_ids_out, n_inliers_out, stream);
 }
 
 // Debug/parity aid: the 3 uniforms per trial the sampler uses (seed as in bt_ransac_pairs), and the winning trial ids of the last call.
 extern "C" int bt_ransac_debug(bt_ctx* ctx, float* u3_out, int n_trials, int32_t* best_trial_out, int n_pairs) {
 	BT_REQUIRE(ctx && ctx->ransac, BT_ERR_INVALID_ARG, "bt_ransac_debug: call bt_ransac_reserve first");
-	RansacState* r = ctx->ransac;
+	RansacState* r = ctx->ransac.get();
 	BT_CUDA(cudaDeviceSynchronize());
 	if (u3_out) BT_CUDA(cudaMemcpy(u3_out, r->table.p, sizeof(float) * 3 * std::min(n_trials, r->table_trials), cudaMemcpyDeviceToHost));
 	if (best_trial_out) BT_CUDA(cudaMemcpy(best_trial_out, r->best_trial.p, sizeof(int32_t) * std::min(n_pairs, r->max_pairs), cudaMemcpyDeviceToHost));

@@ -1526,17 +1526,18 @@ struct SolverState {
 	// frame cache (bt_frame_cache_*): quarter-res maps of keyframes, built once, referenced by bt_window::cache_slots
 	struct CacheMeta { bool valid = false; int H = 0, W = 0; float fx = 0, fy = 0, cx = 0, cy = 0, dmin = 0, dmax = 0; };
 	DevBuf c_texel, c_src, c_nsrc, c_tables, c_blk;
-	PinnedBuf c_htables[2];              // two pinned table blocks, used alternately: a store only waits for the upload of the store before last,
-	cudaEvent_t c_ev[2] = { nullptr, nullptr };   // so back-to-back stores (one new frame per window per step) never stall the host behind the GPU
+	UploadBuf c_htables[2];              // two pinned table blocks, used alternately: a store only waits for the upload of the store before last,
+	                                     // so back-to-back stores (one new frame per window per step) never stall the host behind the GPU
 	int c_flip = 0;
 	int c_capacity = 0, c_npix = 0;
 	float c_downscale = 0.f;
 	std::vector<CacheMeta> c_meta;
 	int prof_cap = 0;
-	PinnedBuf h_stage, h_poses;
+	UploadBuf h_stage;                   // read by the uploads on copy_stream
+	PinnedBuf h_poses;
 	// streaming form (bt_solve_windows_begin / _end): two batches may be in flight; each has its own pinned pose block and completion event
 	PinnedBuf h_pipe[2];
-	cudaEvent_t ev_pipe[2] = { nullptr, nullptr };
+	Event ev_pipe[2];
 	bool pipe_pending[2] = { false, false };
 	int pipe_frames[2] = { 0, 0 };
 	int pipe_head = 0, pipe_tail = 0;
@@ -1552,32 +1553,17 @@ struct SolverState {
 	int launches = 0;
 	int attr_bytes = 0, occ = BT_SOLVE_MIN_CTAS, occ_smem = -1;
 	bool prep_launched = false, any_uncached = true;
-	cudaStream_t copy_stream = nullptr;
-	cudaEvent_t ev_prev = nullptr, ev_corr = nullptr, ev_h2d = nullptr, ev_early = nullptr;
-	cudaEvent_t ev_stage_free[2] = { nullptr, nullptr };   // behind the k_solve that last read staging block 0 / 1
+	Stream copy_stream;
+	Event ev_prev, ev_early;
+	Event ev_stage_free[2];              // behind the k_solve that last read staging block 0 / 1
 	int stage_cur = 0;
-	cudaEvent_t ev[4] = { nullptr, nullptr, nullptr, nullptr };
+	Event ev[4];
 };
-
-void solver_destroy(bt_ctx* ctx) {
-	SolverState* s = ctx->solver;
-	if (!s) return;
-	DevBuf* bufs[] = { &s->blk_cnt, &s->grp_sums, &s->c_texel, &s->c_src, &s->c_nsrc, &s->c_tables, &s->c_blk, &s->stage_buf[0], &s->stage_buf[1], &s->texel, &s->src, &s->nsrc, &s->x, &s->T, &s->pose_out, &s->tiles, &s->scalars, &s->partial,
-	                   &s->tiles_done, &s->iter_done, &s->pair_tile0, &s->pair_ntile, &s->dbgJ, &s->dbgR, &s->dbgC, &s->prof };
-	for (DevBuf* b : bufs) b->release();
-	s->h_stage.release(); s->h_poses.release(); s->h_pipe[0].release(); s->h_pipe[1].release();
-	for (auto& e : s->ev_pipe) if (e) cudaEventDestroy(e); s->c_htables[0].release(); s->c_htables[1].release();
-	for (auto& e : s->c_ev) if (e) cudaEventDestroy(e);
-	for (auto& e : s->ev) if (e) cudaEventDestroy(e);
-	for (cudaEvent_t e : { s->ev_prev, s->ev_corr, s->ev_h2d, s->ev_early, s->ev_stage_free[0], s->ev_stage_free[1] }) if (e) cudaEventDestroy(e);
-	if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
-	delete s;
-	ctx->solver = nullptr;
-}
+void StateDeleter::operator()(SolverState* s) const { delete s; }
 
 static int reserve_impl(bt_ctx* ctx, const bt_solver_limits* lim) {
-	if (!ctx->solver) ctx->solver = new SolverState();
-	SolverState* s = ctx->solver;
+	if (!ctx->solver) ctx->solver.reset(new SolverState());
+	SolverState* s = ctx->solver.get();
 	BT_REQUIRE(lim->max_windows > 0 && lim->max_frames >= 2 && lim->max_frames <= kMaxFrames && lim->max_corr >= 0 && lim->H > 0 && lim->W > 0 && lim->image_downscale >= 1.0f,
 	           BT_ERR_INVALID_ARG, "bt_solver_reserve: bad limits (max_frames must be 2..%d)", kMaxFrames);
 	s->lim = *lim;
@@ -1590,26 +1576,23 @@ static int reserve_impl(bt_ctx* ctx, const bt_solver_limits* lim) {
 	s->max_groups = lim->max_frames * lim->max_frames;
 	const int min_chunk = 256;   // worst case: every pixel valid at the smallest chunk the scheduler ever picks
 	s->max_tiles = lim->max_windows * (lim->max_frames * (lim->max_frames - 1) / 2) * ((s->npix_max + min_chunk - 1) / min_chunk + 1) + kSparseTiles * lim->max_windows;
-	int rc;
-#define RES(buf, bytes) if ((rc = s->buf.alloc(bytes)) != BT_OK) return rc
 	{   // worst case over every window count <= max_windows (the table offsets grow with the count, so the maximum is at max_windows)
 		const StageLayout L = stage_layout(lim->max_windows, (size_t)F, (size_t)lim->max_corr * lim->max_windows, lim->max_frames, (size_t)s->max_groups, (size_t)s->max_pairs);
-		RES(stage_buf[0], L.total); RES(stage_buf[1], L.total);
+		BT_TRY(s->stage_buf[0].alloc(L.total)); BT_TRY(s->stage_buf[1].alloc(L.total));
 	}
-	RES(texel, sizeof(float4) * (size_t)s->npix_max * F);
-	RES(src, sizeof(float4) * 2 * (size_t)s->npix_max * F);
-	RES(nsrc, sizeof(int) * F);
-	RES(grp_sums, sizeof(float) * kGrpVals * (size_t)s->max_groups * lim->max_windows);
-	RES(blk_cnt, sizeof(int) * (size_t)F * ((s->npix_max + 1023) / 1024));
-	RES(x, sizeof(float) * 6 * F); RES(T, sizeof(float) * 12 * F); RES(pose_out, sizeof(float) * 16 * F);
-	RES(pair_tile0, sizeof(int) * (size_t)s->max_pairs * lim->max_windows);
-	RES(pair_ntile, sizeof(int) * (size_t)s->max_pairs * lim->max_windows);
-	RES(tiles, sizeof(Tile) * (size_t)s->max_tiles);
-	RES(partial, sizeof(float) * kTileVals * (size_t)s->max_tiles);
-	RES(scalars, 64);
+	BT_TRY(s->texel.alloc(sizeof(float4) * (size_t)s->npix_max * F));
+	BT_TRY(s->src.alloc(sizeof(float4) * 2 * (size_t)s->npix_max * F));
+	BT_TRY(s->nsrc.alloc(sizeof(int) * F));
+	BT_TRY(s->grp_sums.alloc(sizeof(float) * kGrpVals * (size_t)s->max_groups * lim->max_windows));
+	BT_TRY(s->blk_cnt.alloc(sizeof(int) * (size_t)F * ((s->npix_max + 1023) / 1024)));
+	BT_TRY(s->x.alloc(sizeof(float) * 6 * F)); BT_TRY(s->T.alloc(sizeof(float) * 12 * F)); BT_TRY(s->pose_out.alloc(sizeof(float) * 16 * F));
+	BT_TRY(s->pair_tile0.alloc(sizeof(int) * (size_t)s->max_pairs * lim->max_windows));
+	BT_TRY(s->pair_ntile.alloc(sizeof(int) * (size_t)s->max_pairs * lim->max_windows));
+	BT_TRY(s->tiles.alloc(sizeof(Tile) * (size_t)s->max_tiles));
+	BT_TRY(s->partial.alloc(sizeof(float) * kTileVals * (size_t)s->max_tiles));
+	BT_TRY(s->scalars.alloc(64));
 	BT_CUDA(cudaMemset(s->scalars.p, 0, 64));
-	RES(tiles_done, sizeof(int) * lim->max_windows); RES(iter_done, sizeof(int) * lim->max_windows);
-#undef RES
+	BT_TRY(s->tiles_done.alloc(sizeof(int) * lim->max_windows)); BT_TRY(s->iter_done.alloc(sizeof(int) * lim->max_windows));
 	return BT_OK;
 }
 
@@ -1631,8 +1614,8 @@ extern "C" int bt_solve_enable_debug(bt_ctx* ctx, int on) {
 
 extern "C" int bt_solve_enable_timing(bt_ctx* ctx, int on) {
 	BT_REQUIRE(ctx && ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_enable_timing: call bt_solver_reserve first");
-	SolverState* s = ctx->solver;
-	if (on) for (auto& e : s->ev) if (!e) BT_CUDA(cudaEventCreate(&e));
+	SolverState* s = ctx->solver.get();
+	if (on) for (Event& e : s->ev) BT_TRY(e.create(true));
 	s->timing = on != 0;
 	return BT_OK;
 }
@@ -1641,7 +1624,7 @@ extern "C" int bt_solve_enable_timing(bt_ctx* ctx, int on) {
 // launching stream.  Synchronises on the last event.
 extern "C" int bt_solve_get_timing(bt_ctx* ctx, float* ms3) {
 	BT_REQUIRE(ctx && ctx->solver && ctx->solver->timing && ms3, BT_ERR_INVALID_ARG, "bt_solve_get_timing: timing not enabled");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	BT_CUDA(cudaEventSynchronize(s->ev[3]));
 	for (int k = 0; k < 3; k++) BT_CUDA(cudaEventElapsedTime(ms3 + k, s->ev[k], s->ev[k + 1]));
 	return BT_OK;
@@ -1668,7 +1651,7 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
                       const float* poses_in, void* stream_, bool early_prep) {
 	BT_REQUIRE(ctx && windows && params && poses_in, BT_ERR_INVALID_ARG, "bt_solve_stage: NULL argument");
 	BT_REQUIRE(ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_stage: call bt_solver_reserve first");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_REQUIRE(n_windows > 0 && n_windows <= s->lim.max_windows, BT_ERR_CAPACITY, "bt_solve_stage: %d windows > reserved %d", n_windows, s->lim.max_windows);
@@ -1677,7 +1660,6 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 	s->staged = false; s->prep_launched = false;
 	const auto t_h0 = std::chrono::steady_clock::now();
 	auto us_since = [](std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count(); };
-	if (s->ev_h2d) BT_CUDA(cudaEventSynchronize(s->ev_h2d));     // the previous upload still reads the pinned block
 	// ---- sizes
 	size_t F = 0, C = 0;
 	for (int w = 0; w < n_windows; w++) {
@@ -1706,9 +1688,9 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 	const size_t maxP = (size_t)s->max_pairs, maxG = (size_t)s->max_groups;
 	const StageLayout L = stage_layout(n_windows, F, C, s->lim.max_frames, maxG, maxP);
 	BT_REQUIRE(L.total <= s->stage_buf[0].bytes, BT_ERR_CAPACITY, "bt_solve_stage: staging block %zu > reserved %zu bytes", L.total, s->stage_buf[0].bytes);
-	int rc = s->h_stage.alloc(L.total);
-	if (rc != BT_OK) return rc;
-	char* hb = s->h_stage.as<char>();
+	int rc;
+	char* hb;
+	BT_TRY(s->h_stage.acquire(L.total, &hb));
 	WinDesc* hw = (WinDesc*)(hb + L.wins);
 	const void** hdp = (const void**)(hb + L.dp); const void** hnp = (const void**)(hb + L.np);
 	const void** htex = (const void**)(hb + L.texp); const void** hsrc = (const void**)(hb + L.srcp); const void** hnsrc = (const void**)(hb + L.nsrcp);
@@ -1781,28 +1763,21 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 		s->chunk = s->force_chunk ? s->force_chunk : (int)((c + 255) / 256 * 256);
 	}
 	s->layout = L;
-	if (!s->copy_stream) {
-		BT_CUDA(cudaStreamCreateWithFlags(&s->copy_stream, cudaStreamNonBlocking));
-		BT_CUDA(cudaEventCreateWithFlags(&s->ev_prev, cudaEventDisableTiming));
-		BT_CUDA(cudaEventCreateWithFlags(&s->ev_corr, cudaEventDisableTiming));
-		BT_CUDA(cudaEventCreateWithFlags(&s->ev_h2d, cudaEventDisableTiming));
-	}
+	BT_TRY(s->copy_stream.create());
 	// Two device staging blocks, used alternately: every upload of this batch runs on the private copy stream and only waits for the
 	// k_solve that last read THIS block (two batches ago) - so with the streaming form the 2 MB of batch k+1 cross PCIe while batch k is
 	// still being solved.  (With one block the uploads would queue behind the previous k_solve.)
 	s->stage_cur ^= 1;
 	DevBuf& stage_dev = s->stage_buf[s->stage_cur];
-	if (!s->ev_stage_free[s->stage_cur]) BT_CUDA(cudaEventCreateWithFlags(&s->ev_stage_free[s->stage_cur], cudaEventDisableTiming));
-	else BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_stage_free[s->stage_cur], 0));
+	if (s->ev_stage_free[s->stage_cur]) BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_stage_free[s->stage_cur], 0));
 	{   // correspondence blocks produced on the device (bt_match_pairs on the caller's stream) are copied device -> device on the copy stream: order them
 		bool any_dev = false;
 		for (int w = 0; w < n_windows && !any_dev; w++) any_dev = windows[w].corr_dev != nullptr;
-		if (any_dev) { BT_CUDA(cudaEventRecord(s->ev_prev, stream)); BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_prev, 0)); }
+		if (any_dev) { BT_TRY(s->ev_prev.record(stream)); BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_prev, 0)); }
 	}
 	// early tables first; the caller's stream (frame prep in the fused call) waits for them only
 	BT_CUDA(cudaMemcpyAsync(stage_dev.p, hb, L.late, cudaMemcpyHostToDevice, s->copy_stream));
-	if (!s->ev_early) BT_CUDA(cudaEventCreateWithFlags(&s->ev_early, cudaEventDisableTiming));
-	BT_CUDA(cudaEventRecord(s->ev_early, s->copy_stream));
+	BT_TRY(s->ev_early.record(s->copy_stream));
 	BT_CUDA(cudaStreamWaitEvent(stream, s->ev_early, 0));
 	s->host_us[0] = us_since(t_h0);
 	if (early_prep) { if ((rc = launch_prep(ctx, stream)) != BT_OK) return rc; }
@@ -1969,9 +1944,8 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 	BT_REQUIRE(smem_need <= kTailSmemMax, BT_ERR_CAPACITY, "bt_solve_stage: window needs %zu bytes of shared memory (> %d KB)", smem_need, (int)(kTailSmemMax / 1024));
 	s->smem_bytes = (int)smem_need;
 	BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.late, hb + L.late, L.corr - L.late, cudaMemcpyHostToDevice, s->copy_stream));      // group tables, CSR, WinSparse
-	BT_CUDA(cudaEventRecord(s->ev_corr, s->copy_stream));
-	BT_CUDA(cudaEventRecord(s->ev_h2d, s->copy_stream));
-	BT_CUDA(cudaStreamWaitEvent(stream, s->ev_corr, 0));     // everything later on the caller's stream sees the correspondences
+	BT_TRY(s->h_stage.in_flight(s->copy_stream));
+	BT_CUDA(cudaStreamWaitEvent(stream, s->h_stage.ev, 0));     // everything later on the caller's stream sees the correspondences
 	if (s->debug) {
 		const int st = 6 * s->lim.max_frames;
 		if ((rc = s->dbgJ.alloc(sizeof(float) * (size_t)st * st * s->lim.max_windows)) != BT_OK) return rc;
@@ -1989,7 +1963,7 @@ extern "C" int bt_solve_stage(bt_ctx* ctx, int n_windows, const bt_window* windo
 }
 
 static int ensure_occupancy(bt_ctx* ctx) {
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	if (s->attr_bytes == 0) {      // the attribute belongs to (function, device), not to the context: set it to the ceiling stage_impl enforces, once,
 		s->attr_bytes = (int)kTailSmemMax;   // so that a second context on the same device can never lower what another context's next launch needs
 		BT_CUDA(cudaFuncSetAttribute(k_solve<256, BT_SOLVE_MIN_CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, s->attr_bytes));
@@ -2003,7 +1977,7 @@ static int ensure_occupancy(bt_ctx* ctx) {
 }
 
 static SolveArgs make_args(bt_ctx* ctx) {
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	SolveArgs a;
 	memset(&a, 0, sizeof a);
 	char* sd = s->stage_buf[s->stage_cur].as<char>();
@@ -2037,7 +2011,7 @@ static SolveArgs make_args(bt_ctx* ctx) {
 }
 
 static int launch_prep(bt_ctx* ctx, cudaStream_t stream) {
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	// (in the fused call the tail's shared-memory size is not known yet: the tile plan then aims at the occupancy of the last batch)
 	SolveArgs a = make_args(ctx);
 	if (s->timing) BT_CUDA(cudaEventRecord(s->ev[0], stream));
@@ -2053,7 +2027,7 @@ static int launch_prep(bt_ctx* ctx, cudaStream_t stream) {
 
 extern "C" int bt_solve_run(bt_ctx* ctx, void* stream_) {
 	BT_REQUIRE(ctx && ctx->solver && ctx->solver->staged, BT_ERR_INVALID_ARG, "bt_solve_run: nothing staged");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
 	{ int rco = ensure_occupancy(ctx); if (rco != BT_OK) return rco; }
@@ -2070,7 +2044,7 @@ extern "C" int bt_solve_run(bt_ctx* ctx, void* stream_) {
 	const int grid = ctx->sm_count * occ;
 	k_solve<256, BT_SOLVE_MIN_CTAS><<<grid, 256, s->smem_bytes, stream>>>(a);
 	BT_CUDA(cudaGetLastError());
-	if (s->ev_stage_free[s->stage_cur]) BT_CUDA(cudaEventRecord(s->ev_stage_free[s->stage_cur], stream));      // this batch's staging block may be overwritten after this point
+	BT_TRY(s->ev_stage_free[s->stage_cur].record(stream));      // this batch's staging block may be overwritten after this point
 	if (s->timing) BT_CUDA(cudaEventRecord(s->ev[3], stream));
 	s->launches = s->any_uncached ? 3 : 2;
 	return BT_OK;
@@ -2078,7 +2052,7 @@ extern "C" int bt_solve_run(bt_ctx* ctx, void* stream_) {
 
 extern "C" int bt_solve_fetch(bt_ctx* ctx, float* poses_out, void* stream_) {
 	BT_REQUIRE(ctx && ctx->solver && ctx->solver->staged && poses_out, BT_ERR_INVALID_ARG, "bt_solve_fetch: nothing staged / NULL output");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	cudaStream_t stream = (cudaStream_t)stream_;
 	const size_t bytes = sizeof(float) * 16 * (size_t)s->frames_total;
 	int rc = s->h_poses.alloc(bytes + 64);
@@ -2103,7 +2077,7 @@ extern "C" int bt_solve_windows(bt_ctx* ctx, int n_windows, const bt_window* win
 	if (rc != BT_OK) return rc;
 	const double t2 = us();
 	rc = bt_solve_fetch(ctx, poses_inout, stream);
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	s->host_us[3] = t2 - t1; s->host_us[4] = us() - t2; s->host_us[5] = us();
 	return rc;
 }
@@ -2113,7 +2087,7 @@ extern "C" int bt_solve_windows(bt_ctx* ctx, int n_windows, const bt_window* win
 // uploads, launches) overlaps the GPU side of batch k; everything is ordered on `stream`.
 extern "C" int bt_solve_windows_begin(bt_ctx* ctx, int n_windows, const bt_window* windows, const bt_solver_params* params, const float* poses_in, void* stream_) {
 	BT_REQUIRE(ctx && ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_windows_begin: call bt_solver_reserve first");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	const int slot = s->pipe_head;
 	BT_REQUIRE(!s->pipe_pending[slot], BT_ERR_INVALID_ARG, "bt_solve_windows_begin: two batches are already in flight - call bt_solve_windows_end first");
 	int rc = stage_impl(ctx, n_windows, windows, params, poses_in, stream_, true);
@@ -2122,17 +2096,16 @@ extern "C" int bt_solve_windows_begin(bt_ctx* ctx, int n_windows, const bt_windo
 	if (rc != BT_OK) return rc;
 	cudaStream_t stream = (cudaStream_t)stream_;
 	const size_t bytes = sizeof(float) * 16 * (size_t)s->frames_total;
-	if ((rc = s->h_pipe[slot].alloc(bytes + 64)) != BT_OK) return rc;
-	if (!s->ev_pipe[slot]) BT_CUDA(cudaEventCreateWithFlags(&s->ev_pipe[slot], cudaEventDisableTiming));
+	BT_TRY(s->h_pipe[slot].alloc(bytes + 64));
 	BT_CUDA(cudaMemcpyAsync(s->h_pipe[slot].p, s->pose_out.p, bytes, cudaMemcpyDeviceToHost, stream));
 	BT_CUDA(cudaMemcpyAsync(s->h_pipe[slot].as<char>() + bytes, s->scalars.p, 32, cudaMemcpyDeviceToHost, stream));
-	BT_CUDA(cudaEventRecord(s->ev_pipe[slot], stream));
+	BT_TRY(s->ev_pipe[slot].record(stream));
 	s->pipe_pending[slot] = true; s->pipe_frames[slot] = s->frames_total; s->pipe_head ^= 1;
 	return BT_OK;
 }
 extern "C" int bt_solve_windows_end(bt_ctx* ctx, float* poses_out) {
 	BT_REQUIRE(ctx && ctx->solver && poses_out, BT_ERR_INVALID_ARG, "bt_solve_windows_end: NULL argument");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	const int slot = s->pipe_tail;
 	BT_REQUIRE(s->pipe_pending[slot], BT_ERR_INVALID_ARG, "bt_solve_windows_end: no batch in flight");
 	BT_CUDA(cudaEventSynchronize(s->ev_pipe[slot]));
@@ -2155,7 +2128,7 @@ extern "C" int bt_solve_get_host_timing(bt_ctx* ctx, double* us6) {
 extern "C" int bt_frame_cache_reserve(bt_ctx* ctx, int capacity, int H, int W, float image_downscale) {
 	BT_REQUIRE(ctx && ctx->solver, BT_ERR_INVALID_ARG, "bt_frame_cache_reserve: call bt_solver_reserve first");
 	BT_REQUIRE(capacity > 0 && H > 0 && W > 0 && image_downscale >= 1.0f, BT_ERR_INVALID_ARG, "bt_frame_cache_reserve: bad arguments");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	BT_CUDA(cudaSetDevice(ctx->device));
 	const int w = (int)(W / image_downscale), h = (int)(H / image_downscale);
 	BT_REQUIRE(w >= 2 && h >= 2, BT_ERR_INVALID_ARG, "bt_frame_cache_reserve: image too small");
@@ -2172,7 +2145,7 @@ extern "C" int bt_frame_cache_reserve(bt_ctx* ctx, int capacity, int H, int W, f
 extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* slots, const float* const* depth_dev, const float* const* normal_dev,
                                     int H, int W, float fx, float fy, float cx, float cy, float depth_min, float depth_max, void* stream_) {
 	BT_REQUIRE(ctx && ctx->solver && slots && depth_dev && normal_dev, BT_ERR_INVALID_ARG, "bt_frame_cache_store: NULL argument");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	BT_REQUIRE(s->c_capacity > 0, BT_ERR_INVALID_ARG, "bt_frame_cache_store: call bt_frame_cache_reserve first");
 	BT_REQUIRE(n_frames > 0 && n_frames <= s->c_capacity, BT_ERR_CAPACITY, "bt_frame_cache_store: %d frames > capacity %d", n_frames, s->c_capacity);
 	const FrameGeom geom = frame_geom(H, W, fx, fy, cx, cy, s->c_downscale);
@@ -2180,13 +2153,11 @@ extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* sl
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
 	const size_t b_ptr = sizeof(void*) * (size_t)n_frames, bytes = 2 * b_ptr + sizeof(int) * (size_t)n_frames;
-	int rc;
-	if ((rc = s->c_tables.alloc(bytes)) != BT_OK) return rc;
-	const int fl = s->c_flip; s->c_flip ^= 1;
-	if (s->c_ev[fl]) BT_CUDA(cudaEventSynchronize(s->c_ev[fl]));
-	if ((rc = s->c_htables[fl].alloc(bytes)) != BT_OK) return rc;
-	if (!s->c_ev[fl]) BT_CUDA(cudaEventCreateWithFlags(&s->c_ev[fl], cudaEventDisableTiming));
-	char* hb = s->c_htables[fl].as<char>();
+	BT_TRY(s->c_tables.alloc(bytes));
+	UploadBuf& up = s->c_htables[s->c_flip];
+	s->c_flip ^= 1;
+	char* hb;
+	BT_TRY(up.acquire(bytes, &hb));
 	const void** hd = (const void**)hb; const void** hn = (const void**)(hb + b_ptr); int* hs = (int*)(hb + 2 * b_ptr);
 	for (int f = 0; f < n_frames; f++) {
 		BT_REQUIRE(slots[f] >= 0 && slots[f] < s->c_capacity, BT_ERR_INVALID_ARG, "bt_frame_cache_store: slot %d out of range [0,%d)", slots[f], s->c_capacity);
@@ -2195,7 +2166,7 @@ extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* sl
 		hd[f] = depth_dev[f]; hn[f] = normal_dev[f]; hs[f] = slots[f];
 	}
 	BT_CUDA(cudaMemcpyAsync(s->c_tables.p, hb, bytes, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaEventRecord(s->c_ev[fl], stream));
+	BT_TRY(up.in_flight(stream));
 	CacheStoreArgs c;
 	c.g = geom;
 	char* db = s->c_tables.as<char>();
@@ -2218,7 +2189,7 @@ extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* sl
 
 extern "C" int bt_solve_get_stats(bt_ctx* ctx, bt_solve_stats* out) {
 	BT_REQUIRE(ctx && ctx->solver && out, BT_ERR_INVALID_ARG, "bt_solve_get_stats: NULL argument");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	char h[32];
 	BT_CUDA(cudaMemcpy(h, s->scalars.p, 32, cudaMemcpyDeviceToHost));
 	out->n_windows = s->n_windows;
@@ -2230,14 +2201,14 @@ extern "C" int bt_solve_get_stats(bt_ctx* ctx, bt_solve_stats* out) {
 
 extern "C" int bt_solve_enable_profile(bt_ctx* ctx, int max_records) {
 	BT_REQUIRE(ctx && ctx->solver && max_records >= 0, BT_ERR_INVALID_ARG, "bt_solve_enable_profile: call bt_solver_reserve first");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	if (max_records > 0) { int rc = s->prof.alloc(8 + (size_t)max_records * 96); if (rc != BT_OK) return rc; }
 	s->prof_cap = max_records;
 	return BT_OK;
 }
 extern "C" int bt_solve_get_profile(bt_ctx* ctx, long long* out, int max_records) {
 	BT_REQUIRE(ctx && ctx->solver && ctx->solver->prof_cap > 0 && out, BT_ERR_INVALID_ARG, "bt_solve_get_profile: profiling not enabled");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	BT_CUDA(cudaDeviceSynchronize());
 	long long n = 0;
 	BT_CUDA(cudaMemcpy(&n, s->prof.p, 8, cudaMemcpyDeviceToHost));
@@ -2249,7 +2220,7 @@ extern "C" int bt_solve_get_profile(bt_ctx* ctx, long long* out, int max_records
 
 extern "C" int bt_solve_debug_counts(bt_ctx* ctx, int w, int n_pairs, float* counts_out) {
 	BT_REQUIRE(ctx && ctx->solver && ctx->solver->debug && ctx->solver->staged && counts_out, BT_ERR_INVALID_ARG, "bt_solve_debug_counts: debug not enabled / nothing run");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	BT_REQUIRE(w >= 0 && w < s->n_windows && n_pairs >= 0 && n_pairs <= s->max_pairs, BT_ERR_INVALID_ARG, "bt_solve_debug_counts: bad index");
 	BT_CUDA(cudaDeviceSynchronize());
 	BT_CUDA(cudaMemcpy(counts_out, s->dbgC.as<float>() + (size_t)w * s->max_pairs, sizeof(float) * n_pairs, cudaMemcpyDeviceToHost));
@@ -2258,7 +2229,7 @@ extern "C" int bt_solve_debug_counts(bt_ctx* ctx, int w, int n_pairs, float* cou
 
 extern "C" int bt_solve_debug_dense(bt_ctx* ctx, int w, float* JtJ_out, float* Jtr_out) {
 	BT_REQUIRE(ctx && ctx->solver && ctx->solver->debug && ctx->solver->staged, BT_ERR_INVALID_ARG, "bt_solve_debug_dense: debug not enabled / nothing run");
-	SolverState* s = ctx->solver;
+	SolverState* s = ctx->solver.get();
 	BT_REQUIRE(w >= 0 && w < s->n_windows, BT_ERR_INVALID_ARG, "bt_solve_debug_dense: window %d out of range", w);
 	const int st = 6 * s->lim.max_frames, dim = 6 * s->n_frames[w];
 	BT_CUDA(cudaDeviceSynchronize());

@@ -233,14 +233,10 @@ extern "C" int bt_tracker_create(bt_tracker** out, int device, const bt_tracker_
 
 extern "C" void bt_tracker_destroy(bt_tracker* t) {
 	if (!t) return;
-	if (t->ctx) {
-		cudaSetDevice(t->ctx->device);
-		DevBuf* bufs[] = { &t->depth, &t->normal, &t->fg, &t->kpts, &t->roi, &t->entries, &t->gather, &t->meta };
-		for (DevBuf* b : bufs) b->release();
-		t->h_meta.release();
-		bt_ctx_destroy(t->ctx);
-	}
+	bt_ctx* ctx = t->ctx;
+	if (ctx) cudaSetDevice(ctx->device);
 	delete t;
+	bt_ctx_destroy(ctx);
 }
 
 extern "C" int bt_tracker_begin_frame(bt_tracker* t, int loader_id, const float* first_pose, const float* depth_raw_dev, const uint8_t* mask_dev,

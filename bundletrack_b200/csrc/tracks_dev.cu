@@ -366,17 +366,10 @@ struct TracksDev {
 	size_t prop_smem = 0;
 };
 
-void tracks_dev_destroy(bt_ctx* ctx) {
-	TracksDev* d = ctx->tracks;
-	if (!d) return;
-	DevBuf* bufs[] = { &d->keys, &d->hkey, &d->hidx, &d->n_keys, &d->obs, &d->n_obs, &d->last, &d->free_pts, &d->ctr, &d->shk, &d->smn, &d->smx, &d->ent };
-	for (DevBuf* b : bufs) b->release();
-	delete d;
-	ctx->tracks = nullptr;
-}
+void StateDeleter::operator()(TracksDev* d) const { delete d; }
 
 int tracks_slot(bt_ctx* ctx, int frame_id, bool create, int* slot) {
-	TracksDev* d = ctx->tracks;
+	TracksDev* d = ctx->tracks.get();
 	const auto it = d->slot_of.find(frame_id);
 	if (it != d->slot_of.end()) { *slot = it->second; return BT_OK; }
 	*slot = -1;
@@ -399,7 +392,7 @@ int tracks_points_alive(bt_ctx* ctx, cudaStream_t stream, int* n) {
 }
 
 int tracks_launch_update(bt_ctx* ctx, int slot_a, int slot_b, const TrkSrc& src, cudaStream_t stream) {
-	TracksDev* d = ctx->tracks;
+	TracksDev* d = ctx->tracks.get();
 	d->epoch++;
 	k_trk_update<<<1, kTrkThreads, 0, stream>>>(d->t, slot_a, slot_b, src, d->shk.as<unsigned long long>(), d->smn.as<int>(), d->smx.as<int>(), d->scap,
 	                                            d->ent.as<TrkEnt>(), d->list_cap, d->epoch);
@@ -409,7 +402,7 @@ int tracks_launch_update(bt_ctx* ctx, int slot_a, int slot_b, const TrkSrc& src,
 
 int tracks_launch_propagate(bt_ctx* ctx, int slot_a, int slot_b, const float4* existing, int n_existing, float4* out, int capacity, int32_t* n_out,
                             cudaStream_t stream) {
-	TracksDev* d = ctx->tracks;
+	TracksDev* d = ctx->tracks.get();
 	k_trk_propagate<<<1, kTrkThreads, d->prop_smem, stream>>>(d->t, slot_a, slot_b, existing, n_existing, out, capacity, n_out);
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;
@@ -421,22 +414,21 @@ using namespace bt;
 
 static int tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_per_frame, int max_points) {
 	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->tracks) ctx->tracks = new TracksDev();
-	TracksDev* d = ctx->tracks;
+	if (!ctx->tracks) ctx->tracks.reset(new TracksDev());
+	TracksDev* d = ctx->tracks.get();
 	int hcap = 64;
 	while (hcap < 2 * max_keys_per_frame) hcap <<= 1;
 	d->list_cap = 4 * max_keys_per_frame;       // one pair's list: mutual matches of both directions plus propagated ones, duplicates kept
 	d->scap = 64;
 	while (d->scap < 2 * d->list_cap) d->scap <<= 1;
 	const size_t F = (size_t)max_frames, K = (size_t)max_keys_per_frame, Pn = (size_t)max_points;
-	int rc;
-#define RES(buf, bytes) if ((rc = d->buf.alloc(bytes)) != BT_OK) return rc
-	RES(keys, sizeof(int4) * F * K); RES(hkey, sizeof(unsigned long long) * F * hcap); RES(hidx, sizeof(int) * F * hcap); RES(n_keys, sizeof(int) * F);
-	RES(obs, sizeof(float2) * Pn * F); RES(n_obs, sizeof(int) * Pn); RES(last, sizeof(unsigned long long) * Pn); RES(free_pts, sizeof(int) * Pn);
-	RES(ctr, sizeof(int) * C_N);
-	RES(shk, sizeof(unsigned long long) * 2 * d->scap); RES(smn, sizeof(int) * 2 * d->scap); RES(smx, sizeof(int) * d->scap);
-	RES(ent, sizeof(TrkEnt) * d->list_cap);
-#undef RES
+	BT_TRY(d->keys.alloc(sizeof(int4) * F * K)); BT_TRY(d->hkey.alloc(sizeof(unsigned long long) * F * hcap)); BT_TRY(d->hidx.alloc(sizeof(int) * F * hcap));
+	BT_TRY(d->n_keys.alloc(sizeof(int) * F));
+	BT_TRY(d->obs.alloc(sizeof(float2) * Pn * F)); BT_TRY(d->n_obs.alloc(sizeof(int) * Pn)); BT_TRY(d->last.alloc(sizeof(unsigned long long) * Pn));
+	BT_TRY(d->free_pts.alloc(sizeof(int) * Pn));
+	BT_TRY(d->ctr.alloc(sizeof(int) * C_N));
+	BT_TRY(d->shk.alloc(sizeof(unsigned long long) * 2 * d->scap)); BT_TRY(d->smn.alloc(sizeof(int) * 2 * d->scap)); BT_TRY(d->smx.alloc(sizeof(int) * d->scap));
+	BT_TRY(d->ent.alloc(sizeof(TrkEnt) * d->list_cap));
 	BT_CUDA(cudaMemset(d->hkey.p, 0xff, sizeof(unsigned long long) * F * hcap));
 	BT_CUDA(cudaMemset(d->n_keys.p, 0, sizeof(int) * F));
 	BT_CUDA(cudaMemset(d->obs.p, 0xff, sizeof(float2) * Pn * F));        // every observation empty
@@ -507,7 +499,7 @@ extern "C" int bt_tracks_dev_propagate(bt_ctx* ctx, int frame_a, int frame_b, co
 
 extern "C" int bt_tracks_dev_forget_frame(bt_ctx* ctx, int frame, void* stream_) {
 	BT_REQUIRE(ctx && ctx->tracks, BT_ERR_INVALID_ARG, "bt_tracks_dev_forget_frame: call bt_tracks_dev_reserve first");
-	TracksDev* d = ctx->tracks;
+	TracksDev* d = ctx->tracks.get();
 	const auto it = d->slot_of.find(frame);
 	if (it == d->slot_of.end()) return BT_OK;
 	BT_CUDA(cudaSetDevice(ctx->device));
@@ -522,7 +514,7 @@ extern "C" int bt_tracks_dev_forget_frame(bt_ctx* ctx, int frame, void* stream_)
 // Synchronises `stream`.  BT_ERR_CAPACITY when an earlier call overflowed a capacity (that call changed nothing); the flag is cleared.
 extern "C" int bt_tracks_dev_stats(bt_ctx* ctx, int* n_points, int* n_observations, void* stream_) {
 	BT_REQUIRE(ctx && ctx->tracks && n_points && n_observations, BT_ERR_INVALID_ARG, "bt_tracks_dev_stats: call bt_tracks_dev_reserve first / NULL argument");
-	TracksDev* d = ctx->tracks;
+	TracksDev* d = ctx->tracks.get();
 	BT_CUDA(cudaSetDevice(ctx->device));
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int c[C_N];

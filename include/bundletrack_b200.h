@@ -549,6 +549,11 @@ BT_API int bt_host_alloc_pinned(void** out, size_t bytes);
 BT_API int bt_host_free_pinned(void* p);
 BT_API int bt_stream_sync(void* stream);
 
+/* Test aid: what the contexts and trackers of this process hold right now - device bytes, page-locked host bytes, and CUDA events plus
+ * streams.  Destroying a context or tracker returns all three to their values from before it was created.  Memory from bt_dev_alloc /
+ * bt_host_alloc_pinned is the caller's and is not counted. */
+BT_API int bt_debug_live_resources(long long* device_bytes, long long* pinned_bytes, int* handles);
+
 #ifdef __cplusplus
 }
 #endif

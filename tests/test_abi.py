@@ -61,6 +61,15 @@ def test_no_gpu_fails_loudly():
         OptimizerGpu(None)
 
 
+def test_live_resource_counts_need_no_device():
+    """bt_debug_live_resources reads counters the handle types keep: it answers without a GPU and refuses NULL outputs."""
+    lib = _lib.load()
+    d, p, h = ctypes.c_longlong(-1), ctypes.c_longlong(-1), ctypes.c_int(-1)
+    assert lib.bt_debug_live_resources(ctypes.byref(d), ctypes.byref(p), ctypes.byref(h)) == 0
+    assert d.value >= 0 and p.value >= 0 and h.value >= 0
+    assert lib.bt_debug_live_resources(None, ctypes.byref(p), ctypes.byref(h)) == -1
+
+
 def test_product_never_imports_oracle():
     pkg = os.path.join(ROOT, "bundletrack_b200")
     for dirpath, _, files in os.walk(pkg):
