@@ -148,7 +148,7 @@ class DescView(ctypes.Structure):
 EXPORTS = [
     "bt_last_error", "bt_version", "bt_ctx_create", "bt_ctx_destroy", "bt_solver_reserve",
     "bt_solve_windows", "bt_solve_windows_begin", "bt_solve_windows_end", "bt_solve_stage", "bt_solve_run", "bt_solve_fetch", "bt_solve_get_stats",
-    "bt_solve_enable_debug", "bt_solve_debug_dense", "bt_solve_debug_counts", "bt_solve_enable_timing", "bt_solve_get_timing", "bt_solve_get_host_timing", "bt_solve_enable_profile", "bt_solve_get_profile",
+    "bt_solve_enable_debug", "bt_solve_debug_dense", "bt_solve_debug_counts", "bt_solve_debug_system", "bt_solve_enable_timing", "bt_solve_get_timing", "bt_solve_get_host_timing", "bt_solve_enable_profile", "bt_solve_get_profile",
     "bt_matcher_reserve", "bt_desc_pool_reserve", "bt_desc_pool_store", "bt_knn_match_slots", "bt_match_pairs_pool", "bt_match_pairs_ex", "bt_match_cache_reserve", "bt_match_cache_reserve_entries", "bt_match_cache_usage", "bt_match_cache_put", "bt_match_cache_has", "bt_match_cache_status", "bt_match_cache_gather", "bt_match_cache_forget_frame", "bt_knn_match_pairs", "bt_knn_enable_timing", "bt_knn_get_timing", "bt_knn_debug_force_fallback", "bt_ransac_reserve", "bt_ransac_pairs", "bt_ransac_debug",
     "bt_pipeline_reserve", "bt_prune_mutual_pairs", "bt_match_pairs", "bt_frames_preprocess", "bt_frames_preprocess_masked", "bt_lfnet_request",
     "bt_frame_cache_reserve", "bt_frame_cache_store",

@@ -133,6 +133,7 @@ struct SolveArgs {
 	bt_solver_params prm;
 	float* dbg_JtJ; float* dbg_Jtr; int dbg_stride;   // optional dense-system dump (last GN iteration)
 	float* dbg_cnt; int dbg_cnt_stride;               // optional per-pair #correspondences found (last GN iteration)
+	float* dbg_sys; int dbg_sys_stride;               // optional PCG system dump (last GN iteration): per window A [st][st], rhs, Jacobi diagonal, delta [st] each
 	long long* prof; int prof_cap;                    // optional phase timestamps: [0] = record count, then 12 x int64 per record
 };
 
@@ -1288,6 +1289,12 @@ template <int NT> __device__ void window_tail(const SolveArgs& a, const WinDesc&
 	}
 	__syncthreads();
 	PROF_T(7);
+	if (dbg && a.dbg_sys) {      // what the PCG saw and returned: A, rhs, Jacobi diagonal, delta (bt_solve_debug_system)
+		const int st = a.dbg_sys_stride;
+		float* Sg = a.dbg_sys + (size_t)w * st * (st + 3);
+		for (int k = tid; k < dimp * dimp; k += NT) { const int r = k / dimp; Sg[k] = s.A[r * ld + (k - r * dimp)]; }
+		for (int k = tid; k < dimp; k += NT) { Sg[st * st + k] = s.rhs[k]; Sg[st * st + st + k] = s.Minv[k]; Sg[st * st + 2 * st + k] = s.delta[k]; }
+	}
 	// ---- pose update: x <- log(exp(delta) * exp(x))  (computeLieUpdate), new T for the next iteration
 	const bool last = (it == a.prm.num_iter_outer - 1);
 	for (int f = tid; f < N; f += NT) {
@@ -1521,7 +1528,7 @@ static StageLayout stage_layout(int n_windows, size_t F, size_t C, int max_frame
 struct SolverState {
 	bt_solver_limits lim{};
 	int npix_max = 0, max_pairs = 0, max_frames_total = 0, max_tiles = 0, max_groups = 0;
-	DevBuf blk_cnt, grp_sums, stage_buf[2], texel, src, nsrc, x, T, pose_out, tiles, scalars, partial, tiles_done, iter_done, pair_tile0, pair_ntile, dbgJ, dbgR, dbgC, prof;
+	DevBuf blk_cnt, grp_sums, stage_buf[2], texel, src, nsrc, x, T, pose_out, tiles, scalars, partial, tiles_done, iter_done, pair_tile0, pair_ntile, dbgJ, dbgR, dbgC, dbgS, prof;
 	StageLayout layout{};
 	// frame cache (bt_frame_cache_*): quarter-res maps of keyframes, built once, referenced by bt_window::cache_slots
 	struct CacheMeta { bool valid = false; int H = 0, W = 0; float fx = 0, fy = 0, cx = 0, cy = 0, dmin = 0, dmax = 0; };
@@ -1896,6 +1903,9 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 				hcorr[c_off + bin[(size_t)e.imgIdx_i * N + e.imgIdx_j]++] = e;
 			}
 		}
+		// a group that pairs a frame with itself has no counterpart in the moment form of the sparse term (DESIGN.md §4): refused
+		for (int g = 0; g < ng; g++)
+			BT_REQUIRE(hgi[g_off + g] != hgj[g_off + g], BT_ERR_INVALID_ARG, "window %d: correspondences pair frame %d with itself", w, hgi[g_off + g]);
 		WinSparse& ws = hws[w];
 		memset(&ws, 0, sizeof ws);
 		ws.n_corr = n_valid; ws.n_groups = ng; ws.corr_off = (int)c_off; ws.grp_off = (int)g_off; ws.mem_off = (int)m_off;
@@ -1951,6 +1961,8 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 		if ((rc = s->dbgJ.alloc(sizeof(float) * (size_t)st * st * s->lim.max_windows)) != BT_OK) return rc;
 		if ((rc = s->dbgR.alloc(sizeof(float) * (size_t)st * s->lim.max_windows)) != BT_OK) return rc;
 		if ((rc = s->dbgC.alloc(sizeof(float) * (size_t)s->max_pairs * s->lim.max_windows)) != BT_OK) return rc;
+		const int sp = 6 * (s->lim.max_frames - 1);
+		if ((rc = s->dbgS.alloc(sizeof(float) * (size_t)sp * (sp + 3) * s->lim.max_windows)) != BT_OK) return rc;
 	}
 	s->staged = true;
 	s->host_us[2] = us_since(t_h0) - s->host_us[0] - s->host_us[1];
@@ -2006,7 +2018,8 @@ static SolveArgs make_args(bt_ctx* ctx) {
 		a.d2max = d2max;
 	}
 	if (s->prof_cap > 0) { a.prof = s->prof.as<long long>(); a.prof_cap = s->prof_cap; }
-	if (s->debug) { a.dbg_JtJ = s->dbgJ.as<float>(); a.dbg_Jtr = s->dbgR.as<float>(); a.dbg_stride = 6 * s->lim.max_frames; a.dbg_cnt = s->dbgC.as<float>(); a.dbg_cnt_stride = s->max_pairs; }
+	if (s->debug) { a.dbg_JtJ = s->dbgJ.as<float>(); a.dbg_Jtr = s->dbgR.as<float>(); a.dbg_stride = 6 * s->lim.max_frames; a.dbg_cnt = s->dbgC.as<float>(); a.dbg_cnt_stride = s->max_pairs;
+	                a.dbg_sys = s->dbgS.as<float>(); a.dbg_sys_stride = 6 * (s->lim.max_frames - 1); }
 	return a;
 }
 
@@ -2035,6 +2048,7 @@ extern "C" int bt_solve_run(bt_ctx* ctx, void* stream_) {
 	if (s->debug) {
 		BT_CUDA(cudaMemsetAsync(s->dbgJ.p, 0, s->dbgJ.bytes, stream));
 		BT_CUDA(cudaMemsetAsync(s->dbgR.p, 0, s->dbgR.bytes, stream));
+		BT_CUDA(cudaMemsetAsync(s->dbgS.p, 0, s->dbgS.bytes, stream));
 	}
 	if (s->prof_cap > 0) BT_CUDA(cudaMemsetAsync(s->prof.p, 0, 8, stream));
 	if (!s->prep_launched) { int rcp = launch_prep(ctx, stream); if (rcp != BT_OK) return rcp; }
@@ -2235,5 +2249,20 @@ extern "C" int bt_solve_debug_dense(bt_ctx* ctx, int w, float* JtJ_out, float* J
 	BT_CUDA(cudaDeviceSynchronize());
 	if (JtJ_out) BT_CUDA(cudaMemcpy(JtJ_out, s->dbgJ.as<float>() + (size_t)w * st * st, sizeof(float) * dim * dim, cudaMemcpyDeviceToHost));
 	if (Jtr_out) BT_CUDA(cudaMemcpy(Jtr_out, s->dbgR.as<float>() + (size_t)w * st, sizeof(float) * dim, cudaMemcpyDeviceToHost));
+	return BT_OK;
+}
+
+extern "C" int bt_solve_debug_system(bt_ctx* ctx, int w, int n_frames, float* A_out, float* rhs_out, float* minv_out, float* delta_out) {
+	BT_REQUIRE(ctx && ctx->solver && ctx->solver->debug && ctx->solver->staged, BT_ERR_INVALID_ARG, "bt_solve_debug_system: debug not enabled / nothing run");
+	SolverState* s = ctx->solver.get();
+	BT_REQUIRE(w >= 0 && w < s->n_windows, BT_ERR_INVALID_ARG, "bt_solve_debug_system: window %d out of range", w);
+	BT_REQUIRE(n_frames == s->n_frames[w], BT_ERR_INVALID_ARG, "bt_solve_debug_system: window %d has %d frames, the outputs are sized for %d", w, s->n_frames[w], n_frames);
+	const int st = 6 * (s->lim.max_frames - 1), dim = 6 * (s->n_frames[w] - 1);
+	const float* S = s->dbgS.as<float>() + (size_t)w * st * (st + 3);
+	BT_CUDA(cudaDeviceSynchronize());
+	if (A_out) BT_CUDA(cudaMemcpy(A_out, S, sizeof(float) * dim * dim, cudaMemcpyDeviceToHost));
+	if (rhs_out) BT_CUDA(cudaMemcpy(rhs_out, S + (size_t)st * st, sizeof(float) * dim, cudaMemcpyDeviceToHost));
+	if (minv_out) BT_CUDA(cudaMemcpy(minv_out, S + (size_t)st * st + st, sizeof(float) * dim, cudaMemcpyDeviceToHost));
+	if (delta_out) BT_CUDA(cudaMemcpy(delta_out, S + (size_t)st * st + 2 * st, sizeof(float) * dim, cudaMemcpyDeviceToHost));
 	return BT_OK;
 }

@@ -311,3 +311,12 @@ class OptimizerGpu:
         r = np.zeros(dim, np.float32)
         _lib.check(self.lib.bt_solve_debug_dense(self.ctx, ctypes.c_int(w), J.ctypes.data_as(ctypes.c_void_p), r.ctypes.data_as(ctypes.c_void_p)), "bt_solve_debug_dense")
         return J, r
+
+    def debug_system(self, w: int, n_frames: int):
+        """(A, rhs, minv, delta) the PCG of the last GN iteration of window w solved: unknowns of frames 1..N-1, trans 0-2 / rot 3-5."""
+        dim = 6 * (n_frames - 1)
+        A = np.zeros((dim, dim), np.float32)
+        rhs, minv, delta = (np.zeros(dim, np.float32) for _ in range(3))
+        _lib.check(self.lib.bt_solve_debug_system(self.ctx, ctypes.c_int(w), ctypes.c_int(n_frames), *(v.ctypes.data_as(ctypes.c_void_p) for v in (A, rhs, minv, delta))),
+                   "bt_solve_debug_system")
+        return A, rhs, minv, delta

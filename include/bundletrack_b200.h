@@ -177,6 +177,11 @@ BT_API int bt_solve_enable_debug(bt_ctx* ctx, int on);
 BT_API int bt_solve_debug_dense(bt_ctx* ctx, int w, float* JtJ_out, float* Jtr_out);
 /* Number of dense correspondences each pair found in the last GN iteration of window `w` (gating parity aid). */
 BT_API int bt_solve_debug_counts(bt_ctx* ctx, int w, int n_pairs, float* counts_out);
+/* The system the PCG of the LAST Gauss-Newton iteration of window `w` solved, over the free frames 1..N-1 (dim = 6(N-1), per frame
+ * trans 0-2 / rot 3-5): A (dim x dim, row-major, sparse + dense), the right-hand side, the Jacobi preconditioner (inverse diagonal)
+ * and the PCG result delta before the Lie update.  `n_frames` is the frame count the outputs are sized for and must equal the
+ * window's (BT_ERR_INVALID_ARG otherwise).  Any output may be NULL. */
+BT_API int bt_solve_debug_system(bt_ctx* ctx, int w, int n_frames, float* A_out, float* rhs_out, float* minv_out, float* delta_out);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Matcher.  Replaces the two cv::cuda::DescriptorMatcher::knnMatch calls in SiftManager::findCorresbyNN

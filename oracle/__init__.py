@@ -122,6 +122,68 @@ def dense_system(depth, normal, K, poses, pairs=None, params=None, precision="f3
     return JtJ, Jtr, nfound
 
 
+# A gate decision counts as MARGINAL when the pixel's gate quantity lies within this relative distance of the boundary (see
+# `dense_extra` in solver_oracle.c for what each distance is divided by).  A float32 implementation evaluates the transform chain
+# (pose round trip, 3x4 transform, projection, bilinear blend, distance and cosine) in roughly 30 dependent operations, each rounded
+# to 2^-24 relative to the magnitude the distance is scaled by; 64 * 2^-24 = 3.8e-6 covers twice that chain, so a pixel with a larger
+# margin is decided the same way by any correctly rounded float32 evaluation and by this float64 one.
+MARGIN_EPS = 64.0 * 2.0 ** -24
+
+
+def dense_system_ex(depth, normal, K, poses, pairs=None, params=None, precision="f64", flip=True):
+    """oracle_dense_system with everything a per-entry comparison needs.  Returns a dict: JtJ, Jtr (FlipJtJ applied when flip, else
+    the raw addToLocalSystem sums), JtJ_abs / Jtr_abs (the same sums over |term|), n_found [P], and per (pair, quarter-res source
+    pixel) margin / accepted / contrib ([P, h*w]; see dense_extra in solver_oracle.c)."""
+    lib = _lib(precision)
+    depth = np.ascontiguousarray(depth, np.float32)
+    normal = np.ascontiguousarray(normal, np.float32)
+    N, H, W = depth.shape
+    poses = np.ascontiguousarray(poses, np.float32)
+    pairs = np.ascontiguousarray(default_pairs(N) if pairs is None else pairs, np.uint32).reshape(-1, 2)
+    params = params or default_params()
+    dim, P = 6 * N, len(pairs)
+    npix = int(W / params.image_downscale) * int(H / params.image_downscale)
+    out = dict(JtJ=np.zeros((dim, dim)), Jtr=np.zeros(dim), n_found=np.zeros(P, np.int32), JtJ_abs=np.zeros((dim, dim)), Jtr_abs=np.zeros(dim),
+               margin=np.zeros((P, npix), np.float32), accepted=np.zeros((P, npix), np.uint8), contrib=np.zeros((P, npix), np.float32))
+    rc = lib.oracle_dense_system_ex(
+        ctypes.c_int(N), ctypes.c_int(H), ctypes.c_int(W), _fp(depth), _fp(normal),
+        ctypes.c_float(K[0]), ctypes.c_float(K[1]), ctypes.c_float(K[2]), ctypes.c_float(K[3]),
+        _fp(pairs) if P else None, ctypes.c_int(P), ctypes.byref(params), _fp(poses), ctypes.c_int(1 if flip else 0),
+        *(_fp(out[k]) for k in ("JtJ", "Jtr", "n_found", "JtJ_abs", "Jtr_abs", "margin", "accepted", "contrib")))
+    if rc != 0:
+        raise RuntimeError(f"oracle_dense_system_ex rc={rc}")
+    return out
+
+
+def sparse_system(corr, poses, params=None, precision="f64"):
+    """Explicit matrix of the reference's matrix-free sparse operator at `poses`, its right-hand side -wS J^T F, the Jacobi
+    preconditioner and the gradient's |term| sums: (A [6(N-1)]^2, rhs, minv, rhs_abs), unknowns of frames 1..N-1, trans 0-2 / rot 3-5."""
+    lib = _lib(precision)
+    corr = np.ascontiguousarray(corr)
+    poses = np.ascontiguousarray(poses, np.float32)
+    N = poses.shape[0]
+    d = 6 * (N - 1)
+    A, rhs, minv, ra = np.zeros((d, d)), np.zeros(d), np.zeros(d), np.zeros(d)
+    rc = lib.oracle_sparse_system(ctypes.c_int(N), ctypes.c_int(len(corr)), _fp(corr), ctypes.byref(params or default_params()), _fp(poses),
+                                  _fp(A), _fp(rhs), _fp(minv), _fp(ra))
+    if rc != 0:
+        raise RuntimeError(f"oracle_sparse_system rc={rc}")
+    return A, rhs, minv, ra
+
+
+def sparse_apply(corr, poses, x, params=None, precision="f64"):
+    """The matrix-free operator applyJT(applyJ(x)) itself, x in the layout of sparse_system."""
+    lib = _lib(precision)
+    corr = np.ascontiguousarray(corr)
+    poses = np.ascontiguousarray(poses, np.float32)
+    x = np.ascontiguousarray(x, np.float64)
+    y = np.zeros_like(x)
+    rc = lib.oracle_sparse_apply(ctypes.c_int(poses.shape[0]), ctypes.c_int(len(corr)), _fp(corr), ctypes.byref(params or default_params()), _fp(poses), _fp(x), _fp(y))
+    if rc != 0:
+        raise RuntimeError(f"oracle_sparse_apply rc={rc}")
+    return y
+
+
 def build_cache(depth, normal, K, downscale=4.0, precision="f32"):
     lib = _lib(precision)
     depth = np.ascontiguousarray(depth, np.float32)

@@ -312,21 +312,47 @@ static void evalLie_derivJ(const mat4* A, const mat4* D, vec3 p, real jac[3][6])
 
 /* ---- dense term: Solver/SolverBundling.cu:129-229 (BuildDenseSystem_Kernel<true,false>), findDenseCorr
  * (SolverBundlingDenseUtil.h:78-110), addToLocalSystem (:217-285), FlipJtJ_Kernel (SolverBundling.cu:49-58) ---- */
+/* Optional outputs of build_dense_system beyond the system itself (all NULL for the solve).
+ * JtJ_abs / Jtr_abs: the same sums over |term| (what a per-entry float tolerance scales with).
+ * margin [n_pairs][w*h]: per (pair, source pixel) the smallest relative distance of any gate quantity to its decision boundary,
+ *   over the gates the pixel reached (all of them when accepted); +1 when the source pixel has no valid depth.  Each distance is
+ *   divided by the magnitude its float32 rounding error scales with: depths by the depth, the projected pixel position by the image
+ *   width / height, the point distance by the length of the transformed source point; the normal cosine is already O(1).
+ * accepted [n_pairs][w*h]: 1 when the pixel passed every gate.
+ * contrib [n_pairs][w*h]: weight * (|J_i|^2 + |J_j|^2) of an accepted pixel: what it adds to the traces of the pair's diagonal blocks. */
+typedef struct { real* JtJ_abs; real* Jtr_abs; float* margin; unsigned char* accepted; float* contrib; int flip; } dense_extra;
+
+static real rel_gap(real v, real edge, real scale) { return (real)fabs((double)(v - edge)) / scale; }
+static real rmin(real a, real b) { return a < b ? a : b; }
+
 static void build_dense_system(const frame_cache* fc, int N, const mat4* T, const mat4* Tinv,
                                const uint32_t* pairs, int n_pairs, const oracle_params* prm,
-                               real* JtJ /*[6N][6N]*/, real* Jtr /*[6N]*/, int* n_found_per_pair) {
+                               real* JtJ /*[6N][6N]*/, real* Jtr /*[6N]*/, int* n_found_per_pair, const dense_extra* ex) {
 	const int dim = 6 * N, w = fc->w, h = fc->h, npix = w * h;
 	memset(JtJ, 0, sizeof(real) * dim * dim);
 	memset(Jtr, 0, sizeof(real) * dim);
+	real* JtJa = ex ? ex->JtJ_abs : NULL;
+	real* Jtra = ex ? ex->Jtr_abs : NULL;
+	if (JtJa) memset(JtJa, 0, sizeof(real) * dim * dim);
+	if (Jtra) memset(Jtra, 0, sizeof(real) * dim);
+	const real dmin = (real)prm->depth_min, dmax = (real)prm->depth_max;
 	for (int pidx = 0; pidx < n_pairs; pidx++) {
 		const unsigned i = pairs[2 * pidx], j = pairs[2 * pidx + 1];    /* i = target, j = source */
 		const mat4 transform = mat_mul(&Tinv[i], &T[j]);
 		const real* tgtCam = fc->campos + (size_t)i * npix * 4, *tgtNrm = fc->normal + (size_t)i * npix * 4;
 		const real* srcCam = fc->campos + (size_t)j * npix * 4, *srcNrm = fc->normal + (size_t)j * npix * 4;
+		float* marg = (ex && ex->margin) ? ex->margin + (size_t)pidx * npix : NULL;
+		unsigned char* acc = (ex && ex->accepted) ? ex->accepted + (size_t)pidx * npix : NULL;
+		float* ctb = (ex && ex->contrib) ? ex->contrib + (size_t)pidx * npix : NULL;
 		int found = 0;
 		for (int idx = 0; idx < npix; idx++) {
 			const real* cposj = srcCam + (size_t)idx * 4;
-			if (!(cposj[2] > (real)prm->depth_min && cposj[2] < (real)prm->depth_max)) continue;
+			real m = 1;
+			if (acc) acc[idx] = 0;
+			if (ctb) ctb[idx] = 0;
+			if (marg) { marg[idx] = 1; if (cposj[2] > 0) m = rmin(rel_gap(cposj[2], dmin, cposj[2]), rel_gap(cposj[2], dmax, cposj[2])); }
+#define GATE_FAIL(cond) if (cond) { if (marg) marg[idx] = (float)m; continue; }
+			GATE_FAIL(!(cposj[2] > (real)prm->depth_min && cposj[2] < (real)prm->depth_max));
 			const vec3 camPosSrc = v3(cposj[0], cposj[1], cposj[2]);
 			const real* nj = srcNrm + (size_t)idx * 4;
 			real nrmj[4];
@@ -334,16 +360,27 @@ static void build_dense_system(const frame_cache* fc, int N, const mat4* T, cons
 			const vec3 camPosSrcToTgt = mat_mul_p(&transform, camPosSrc);
 			const real sx = camPosSrcToTgt.x * fc->fx / camPosSrcToTgt.z + fc->cx;   /* CUDACameraUtil.h:9-14 */
 			const real sy = camPosSrcToTgt.y * fc->fy / camPosSrcToTgt.z + fc->cy;
+			if (marg) {   /* roundf bounds at -0.5 / size - 0.5; bilinear tap validity switches at 0 / size - 1 */
+				m = rmin(m, rmin(rel_gap(sx, R_(-0.5), (real)w), rel_gap(sx, (real)w - R_(0.5), (real)w)));
+				m = rmin(m, rmin(rel_gap(sy, R_(-0.5), (real)h), rel_gap(sy, (real)h - R_(0.5), (real)h)));
+				m = rmin(m, rmin(rel_gap(sx, R_(0), (real)w), rel_gap(sx, (real)(w - 1), (real)w)));
+				m = rmin(m, rmin(rel_gap(sy, R_(0), (real)h), rel_gap(sy, (real)(h - 1), (real)h)));
+			}
 			const int ix = (int)roundf((float)sx), iy = (int)roundf((float)sy);
-			if (!(ix >= 0 && iy >= 0 && ix < w && iy < h)) continue;
+			GATE_FAIL(!(ix >= 0 && iy >= 0 && ix < w && iy < h));
 			real cposi[4], nrmi[4];
-			if (!bilinear4(sx, sy, tgtCam, w, h, cposi)) continue;
-			if (!(cposi[2] > (real)prm->depth_min && cposi[2] < (real)prm->depth_max)) continue;
-			if (!bilinear4(sx, sy, tgtNrm, w, h, nrmi)) continue;
+			GATE_FAIL(!bilinear4(sx, sy, tgtCam, w, h, cposi));
+			if (marg) { const real sc = cposi[2] > dmin ? cposi[2] : dmin; m = rmin(m, rmin(rel_gap(cposi[2], dmin, sc), rel_gap(cposi[2], dmax, sc))); }
+			GATE_FAIL(!(cposi[2] > (real)prm->depth_min && cposi[2] < (real)prm->depth_max));
+			GATE_FAIL(!bilinear4(sx, sy, tgtNrm, w, h, nrmi));
 			const vec3 camPosTgt = v3(cposi[0], cposi[1], cposi[2]), normalTgt = v3(nrmi[0], nrmi[1], nrmi[2]);
 			const real dist = vlen(vsub(camPosSrcToTgt, camPosTgt));
 			const real dNormal = nrmj[0]*nrmi[0] + nrmj[1]*nrmi[1] + nrmj[2]*nrmi[2] + nrmj[3]*nrmi[3];
-			if (!(dNormal >= (real)prm->dense_cos_normal_thresh && dist <= (real)prm->dense_dist_thresh)) continue;
+			if (marg) m = rmin(m, rmin(rel_gap(dist, (real)prm->dense_dist_thresh, vlen(camPosSrcToTgt)), rel_gap(dNormal, (real)prm->dense_cos_normal_thresh, R_(1))));
+			GATE_FAIL(!(dNormal >= (real)prm->dense_cos_normal_thresh && dist <= (real)prm->dense_dist_thresh));
+#undef GATE_FAIL
+			if (marg) marg[idx] = (float)m;
+			if (acc) acc[idx] = 1;
 			found++;
 			const real depthRes = vdot(vsub(camPosTgt, camPosSrcToTgt), normalTgt);
 			const real weight = (real)prm->w_dense * huber_weight(depthRes * depthRes, (real)prm->robust_delta);
@@ -364,15 +401,28 @@ static void build_dense_system(const frame_cache* fc, int N, const mat4* T, cons
 						JtJ[(j * 6 + b) * dim + (i * 6 + a)] += Ji[a] * Jj[b] * weight;
 						if (a != b) JtJ[(j * 6 + a) * dim + (i * 6 + b)] += Ji[b] * Jj[a] * weight;
 					}
+					if (JtJa) {
+						if (i > 0) JtJa[(i * 6 + b) * dim + (i * 6 + a)] += (real)fabs((double)(Ji[a] * Ji[b] * weight));
+						if (j > 0) JtJa[(j * 6 + b) * dim + (j * 6 + a)] += (real)fabs((double)(Jj[a] * Jj[b] * weight));
+						if (i > 0 && j > 0) {
+							JtJa[(j * 6 + b) * dim + (i * 6 + a)] += (real)fabs((double)(Ji[a] * Jj[b] * weight));
+							if (a != b) JtJa[(j * 6 + a) * dim + (i * 6 + b)] += (real)fabs((double)(Ji[b] * Jj[a] * weight));
+						}
+					}
 				}
 				if (i > 0) Jtr[i * 6 + a] += Ji[a] * depthRes * weight;
 				if (j > 0) Jtr[j * 6 + a] += Jj[a] * depthRes * weight;
+				if (Jtra && i > 0) Jtra[i * 6 + a] += (real)fabs((double)(Ji[a] * depthRes * weight));
+				if (Jtra && j > 0) Jtra[j * 6 + a] += (real)fabs((double)(Jj[a] * depthRes * weight));
+				if (ctb) ctb[idx] += (float)((Ji[a] * Ji[a] + Jj[a] * Jj[a]) * weight);
 			}
 		}
 		if (n_found_per_pair) n_found_per_pair[pidx] = found;
 	}
+	if (ex && !ex->flip) return;     /* raw addToLocalSystem output: lower triangle of each diagonal block, each cross block where it was written */
 	/* FlipJtJ_Kernel: upper := lower (erases cross blocks that were written above the diagonal, SURVEY.md Q2) */
 	for (int y = 0; y < dim; y++) for (int x = y + 1; x < dim; x++) JtJ[y * dim + x] = JtJ[x * dim + y];
+	if (JtJa) for (int y = 0; y < dim; y++) for (int x = y + 1; x < dim; x++) JtJa[y * dim + x] = JtJa[x * dim + y];
 }
 
 /* ---- sparse term + PCG: SolverBundlingEquationsLie.h:60-211, SolverBundling.cu:575-887 ---- */
@@ -380,6 +430,78 @@ typedef struct { vec3 rot, trans; } pose6;
 
 static void lie_d(vec3 q, vec3* da, vec3* db, vec3* dc) { /* LieDerivUtil.h:215-226 */
 	*da = v3(0, -q.z, q.y); *db = v3(q.z, 0, -q.x); *dc = v3(-q.y, q.x, 0);
+}
+static vec3 vabs3(vec3 a) { return v3((real)fabs((double)a.x), (real)fabs((double)a.y), (real)fabs((double)a.z)); }
+
+/* evalMinusJTFDevice for frame v, sparse part: r = sum rho sign J^T res (rot, trans) and the Jacobi sums p (rot, trans).
+ * aRot / aTrans (optional): the same gradient sums over |term|. */
+static void sparse_jtf(int v, const mat4* T, int n_corr, const EntryJ* corr, real robust_delta,
+                       vec3* rRot_, vec3* rTrans_, vec3* pRot_, vec3* pTrans_, vec3* aRot, vec3* aTrans) {
+	vec3 rRot = v3(0,0,0), rTrans = v3(0,0,0), pRot = v3(0,0,0), pTrans = v3(0,0,0);
+	if (aRot) { *aRot = v3(0,0,0); *aTrans = v3(0,0,0); }
+	for (int c = 0; c < n_corr; c++) {
+		const EntryJ* e = &corr[c];
+		if (e->imgIdx_i == 0xFFFFFFFFu) continue;
+		if ((int)e->imgIdx_i != v && (int)e->imgIdx_j != v) continue;
+		const vec3 pi_ = v3((real)e->pos_i[0], (real)e->pos_i[1], (real)e->pos_i[2]);
+		const vec3 pj_ = v3((real)e->pos_j[0], (real)e->pos_j[1], (real)e->pos_j[2]);
+		const vec3 wi = mat_mul_p(&T[e->imgIdx_i], pi_), wj = mat_mul_p(&T[e->imgIdx_j], pj_);
+		real sign = 1; vec3 worldP = wi;
+		if ((unsigned)v != e->imgIdx_i) { sign = -1; worldP = wj; }
+		vec3 da, db, dc; lie_d(worldP, &da, &db, &dc);
+		const vec3 res = vsub(wi, wj);
+		const real rho = huber_weight(vdot(res, res), robust_delta);
+		const vec3 gr = vscale(v3(vdot(da, res), vdot(db, res), vdot(dc, res)), rho * sign), gt = vscale(res, rho * sign);
+		rRot = vadd(rRot, gr);
+		rTrans = vadd(rTrans, gt);
+		pRot = vadd(pRot, vscale(v3(vdot(da, da), vdot(db, db), vdot(dc, dc)), rho));
+		pTrans = vadd(pTrans, vscale(v3(1, 1, 1), rho));
+		if (aRot) { *aRot = vadd(*aRot, vabs3(gr)); *aTrans = vadd(*aTrans, vabs3(gt)); }
+	}
+	*rRot_ = rRot; *rTrans_ = rTrans; *pRot_ = pRot; *pTrans_ = pTrans;
+}
+
+/* PCGStep_Kernel0 / applyJDevice: Jp[c] = wS (J_i p_i - J_j p_j) of every correspondence (zero for invalid entries) */
+static void apply_j(const mat4* T, int n_corr, const EntryJ* corr, const pose6* p, real wS, vec3* Jp) {
+	for (int c = 0; c < n_corr; c++) {
+		const EntryJ* e = &corr[c];
+		vec3 b = v3(0,0,0);
+		if (e->imgIdx_i != 0xFFFFFFFFu) {
+			if (e->imgIdx_i > 0) {
+				const vec3 wp = mat_mul_p(&T[e->imgIdx_i], v3((real)e->pos_i[0], (real)e->pos_i[1], (real)e->pos_i[2]));
+				vec3 da, db, dc; lie_d(wp, &da, &db, &dc);
+				const vec3 pp = p[e->imgIdx_i].rot;
+				b = vadd(b, vadd(vadd(vadd(vscale(da, pp.x), vscale(db, pp.y)), vscale(dc, pp.z)), p[e->imgIdx_i].trans));
+			}
+			if (e->imgIdx_j > 0) {
+				const vec3 wp = mat_mul_p(&T[e->imgIdx_j], v3((real)e->pos_j[0], (real)e->pos_j[1], (real)e->pos_j[2]));
+				vec3 da, db, dc; lie_d(wp, &da, &db, &dc);
+				const vec3 pp = p[e->imgIdx_j].rot;
+				b = vsub(b, vadd(vadd(vadd(vscale(da, pp.x), vscale(db, pp.y)), vscale(dc, pp.z)), p[e->imgIdx_j].trans));
+			}
+			b = vscale(b, wS);
+		}
+		Jp[c] = b;
+	}
+}
+
+/* PCGStep_Kernel1a / applyJTDevice: Ap[v] += J_v^T Jp (with the sign of v's side) for frames 1..N-1 */
+static void apply_jt(int N, const mat4* T, int n_corr, const EntryJ* corr, const vec3* Jp, pose6* Ap) {
+	for (int v = 1; v < N; v++) {
+		vec3 oR = v3(0,0,0), oT = v3(0,0,0);
+		for (int c = 0; c < n_corr; c++) {
+			const EntryJ* e = &corr[c];
+			if (e->imgIdx_i == 0xFFFFFFFFu) continue;
+			if ((int)e->imgIdx_i != v && (int)e->imgIdx_j != v) continue;
+			real sign = 1; vec3 wp;
+			if ((unsigned)v != e->imgIdx_i) { sign = -1; wp = mat_mul_p(&T[e->imgIdx_j], v3((real)e->pos_j[0], (real)e->pos_j[1], (real)e->pos_j[2])); }
+			else wp = mat_mul_p(&T[e->imgIdx_i], v3((real)e->pos_i[0], (real)e->pos_i[1], (real)e->pos_i[2]));
+			vec3 da, db, dc; lie_d(wp, &da, &db, &dc);
+			oR = vadd(oR, vscale(v3(vdot(da, Jp[c]), vdot(db, Jp[c]), vdot(dc, Jp[c])), sign));
+			oT = vadd(oT, vscale(Jp[c], sign));
+		}
+		Ap[v].rot = vadd(Ap[v].rot, oR); Ap[v].trans = vadd(Ap[v].trans, oT);
+	}
 }
 
 int oracle_solve_window(int N, int H, int W, const float* depth, const float* normal,
@@ -411,32 +533,16 @@ int oracle_solve_window(int N, int H, int W, const float* depth, const float* no
 		for (int f = 0; f < N; f++) { T[f] = poseToMatrix(x[f].rot, x[f].trans); Tinv[f] = mat_inverse(&T[f]); } /* :890-897 */
 		int useDense = use_dense_any;
 		if (useDense) {
-			build_dense_system(&fc, N, T, Tinv, dense_pairs, n_pairs, prm, JtJ, Jtr, NULL);
+			build_dense_system(&fc, N, T, Tinv, dense_pairs, n_pairs, prm, JtJ, Jtr, NULL, NULL);
 			if (it == 0 && dbg_JtJ0) for (int k = 0; k < dim * dim; k++) dbg_JtJ0[k] = (double)JtJ[k];
 			if (it == 0 && dbg_Jtr0) for (int k = 0; k < dim; k++) dbg_Jtr0[k] = (double)Jtr[k];
 		}
 		/* PCGInit_Kernel1 / evalMinusJTFDevice (frames 1..N-1; frame 0 is the gauge) */
 		real rDotzOld = 0;
 		for (int v = 1; v < N; v++) {
-			vec3 rRot = v3(0,0,0), rTrans = v3(0,0,0), pRot = v3(0,0,0), pTrans = v3(0,0,0);
+			vec3 rRot, rTrans, pRot, pTrans;
 			delta[v].rot = v3(0,0,0); delta[v].trans = v3(0,0,0);
-			for (int c = 0; c < n_corr; c++) {
-				const EntryJ* e = &corr[c];
-				if (e->imgIdx_i == 0xFFFFFFFFu) continue;
-				if ((int)e->imgIdx_i != v && (int)e->imgIdx_j != v) continue;
-				const vec3 pi_ = v3((real)e->pos_i[0], (real)e->pos_i[1], (real)e->pos_i[2]);
-				const vec3 pj_ = v3((real)e->pos_j[0], (real)e->pos_j[1], (real)e->pos_j[2]);
-				const vec3 wi = mat_mul_p(&T[e->imgIdx_i], pi_), wj = mat_mul_p(&T[e->imgIdx_j], pj_);
-				real sign = 1; vec3 worldP = wi;
-				if ((unsigned)v != e->imgIdx_i) { sign = -1; worldP = wj; }
-				vec3 da, db, dc; lie_d(worldP, &da, &db, &dc);
-				const vec3 res = vsub(wi, wj);
-				const real rho = huber_weight(vdot(res, res), (real)prm->robust_delta);
-				rRot = vadd(rRot, vscale(v3(vdot(da, res), vdot(db, res), vdot(dc, res)), rho * sign));
-				rTrans = vadd(rTrans, vscale(res, rho * sign));
-				pRot = vadd(pRot, vscale(v3(vdot(da, da), vdot(db, db), vdot(dc, dc)), rho));
-				pTrans = vadd(pTrans, vscale(v3(1, 1, 1), rho));
-			}
+			sparse_jtf(v, T, n_corr, corr, (real)prm->robust_delta, &rRot, &rTrans, &pRot, &pTrans, NULL, NULL);
 			vec3 resRot = vscale(rRot, -wS), resTrans = vscale(rTrans, -wS);
 			if (useDense) { /* dense ordering: trans 0-2, rot 3-5 (SolverBundlingEquationsLie.h:113-118) */
 				resRot = vsub(resRot, v3(Jtr[v * 6 + 3], Jtr[v * 6 + 4], Jtr[v * 6 + 5]));
@@ -456,41 +562,8 @@ int oracle_solve_window(int N, int H, int W, const float* depth, const float* no
 		}
 		for (int lin = 0; lin < prm->num_iter_inner; lin++) { /* PCGIteration<useSparse,useDense>, :820-887 */
 			if (wS > 0) {
-				for (int c = 0; c < n_corr; c++) { /* PCGStep_Kernel0 / applyJDevice */
-					const EntryJ* e = &corr[c];
-					vec3 b = v3(0,0,0);
-					if (e->imgIdx_i != 0xFFFFFFFFu) {
-						if (e->imgIdx_i > 0) {
-							const vec3 wp = mat_mul_p(&T[e->imgIdx_i], v3((real)e->pos_i[0], (real)e->pos_i[1], (real)e->pos_i[2]));
-							vec3 da, db, dc; lie_d(wp, &da, &db, &dc);
-							const vec3 pp = p[e->imgIdx_i].rot;
-							b = vadd(b, vadd(vadd(vadd(vscale(da, pp.x), vscale(db, pp.y)), vscale(dc, pp.z)), p[e->imgIdx_i].trans));
-						}
-						if (e->imgIdx_j > 0) {
-							const vec3 wp = mat_mul_p(&T[e->imgIdx_j], v3((real)e->pos_j[0], (real)e->pos_j[1], (real)e->pos_j[2]));
-							vec3 da, db, dc; lie_d(wp, &da, &db, &dc);
-							const vec3 pp = p[e->imgIdx_j].rot;
-							b = vsub(b, vadd(vadd(vadd(vscale(da, pp.x), vscale(db, pp.y)), vscale(dc, pp.z)), p[e->imgIdx_j].trans));
-						}
-						b = vscale(b, wS);
-					}
-					Jp[c] = b;
-				}
-				for (int v = 1; v < N; v++) { /* PCGStep_Kernel1a / applyJTDevice */
-					vec3 oR = v3(0,0,0), oT = v3(0,0,0);
-					for (int c = 0; c < n_corr; c++) {
-						const EntryJ* e = &corr[c];
-						if (e->imgIdx_i == 0xFFFFFFFFu) continue;
-						if ((int)e->imgIdx_i != v && (int)e->imgIdx_j != v) continue;
-						real sign = 1; vec3 wp;
-						if ((unsigned)v != e->imgIdx_i) { sign = -1; wp = mat_mul_p(&T[e->imgIdx_j], v3((real)e->pos_j[0], (real)e->pos_j[1], (real)e->pos_j[2])); }
-						else wp = mat_mul_p(&T[e->imgIdx_i], v3((real)e->pos_i[0], (real)e->pos_i[1], (real)e->pos_i[2]));
-						vec3 da, db, dc; lie_d(wp, &da, &db, &dc);
-						oR = vadd(oR, vscale(v3(vdot(da, Jp[c]), vdot(db, Jp[c]), vdot(dc, Jp[c])), sign));
-						oT = vadd(oT, vscale(Jp[c], sign));
-					}
-					Ap[v].rot = vadd(Ap[v].rot, oR); Ap[v].trans = vadd(Ap[v].trans, oT);
-				}
+				apply_j(T, n_corr, corr, p, wS, Jp);
+				apply_jt(N, T, n_corr, corr, Jp, Ap);
 			}
 			if (useDense) { /* PCGStep_Kernel_Dense / applyJTJDenseDevice (SolverBundlingDenseUtil.h:349-385) */
 				for (int v = 1; v < N; v++) {
@@ -554,24 +627,107 @@ int oracle_build_cache(int N, int H, int W, const float* depth, const float* nor
 	return 0;
 }
 
-int oracle_dense_system(int N, int H, int W, const float* depth, const float* normal, float fx, float fy, float cx, float cy,
-                        const uint32_t* dense_pairs, int n_pairs, const oracle_params* prm, const float* poses /*[N][16]*/,
-                        double* JtJ_out, double* Jtr_out, int* n_found_per_pair) {
+/* the round trip the solver applies to its input poses: matrix -> se(3) -> matrix */
+static void load_poses(int N, const float* poses, mat4* T, mat4* Tinv) {
+	for (int f = 0; f < N; f++) {
+		mat4 Tm; vec3 rot, trans;
+		for (int k = 0; k < 16; k++) Tm.m[k] = (real)poses[f * 16 + k];
+		matrixToPose(&Tm, &rot, &trans);
+		T[f] = poseToMatrix(rot, trans);
+		if (Tinv) Tinv[f] = mat_inverse(&T[f]);
+	}
+}
+
+/* One dense system at given poses.  flip = 0 returns the raw addToLocalSystem sums (no FlipJtJ); the optional outputs are those of
+ * dense_extra (JtJ_abs_out / Jtr_abs_out as doubles, margin / accepted / contrib per (pair, quarter-res source pixel)). */
+int oracle_dense_system_ex(int N, int H, int W, const float* depth, const float* normal, float fx, float fy, float cx, float cy,
+                           const uint32_t* dense_pairs, int n_pairs, const oracle_params* prm, const float* poses /*[N][16]*/, int flip,
+                           double* JtJ_out, double* Jtr_out, int* n_found_per_pair, double* JtJ_abs_out, double* Jtr_abs_out,
+                           float* margin_out, unsigned char* accepted_out, float* contrib_out) {
 	const int dim = 6 * N;
 	frame_cache fc;
 	cache_build(&fc, N, H, W, depth, normal, fx, fy, cx, cy, prm->image_downscale);
 	mat4* T = (mat4*)malloc(sizeof(mat4) * N), *Tinv = (mat4*)malloc(sizeof(mat4) * N);
-	for (int f = 0; f < N; f++) { /* same round trip the solver applies: matrix -> se(3) -> matrix */
-		mat4 Tm; vec3 rot, trans;
-		for (int k = 0; k < 16; k++) Tm.m[k] = (real)poses[f * 16 + k];
-		matrixToPose(&Tm, &rot, &trans);
-		T[f] = poseToMatrix(rot, trans); Tinv[f] = mat_inverse(&T[f]);
-	}
+	load_poses(N, poses, T, Tinv);
 	real* JtJ = (real*)calloc((size_t)dim * dim, sizeof(real)), *Jtr = (real*)calloc(dim, sizeof(real));
-	build_dense_system(&fc, N, T, Tinv, dense_pairs, n_pairs, prm, JtJ, Jtr, n_found_per_pair);
+	real* JtJa = JtJ_abs_out ? (real*)calloc((size_t)dim * dim, sizeof(real)) : NULL, *Jtra = Jtr_abs_out ? (real*)calloc(dim, sizeof(real)) : NULL;
+	dense_extra ex = { JtJa, Jtra, margin_out, accepted_out, contrib_out, flip };
+	build_dense_system(&fc, N, T, Tinv, dense_pairs, n_pairs, prm, JtJ, Jtr, n_found_per_pair, &ex);
 	for (int k = 0; k < dim * dim; k++) JtJ_out[k] = (double)JtJ[k];
 	for (int k = 0; k < dim; k++) Jtr_out[k] = (double)Jtr[k];
-	cache_free(&fc); free(T); free(Tinv); free(JtJ); free(Jtr);
+	if (JtJa) for (int k = 0; k < dim * dim; k++) JtJ_abs_out[k] = (double)JtJa[k];
+	if (Jtra) for (int k = 0; k < dim; k++) Jtr_abs_out[k] = (double)Jtra[k];
+	cache_free(&fc); free(T); free(Tinv); free(JtJ); free(Jtr); free(JtJa); free(Jtra);
+	return 0;
+}
+
+int oracle_dense_system(int N, int H, int W, const float* depth, const float* normal, float fx, float fy, float cx, float cy,
+                        const uint32_t* dense_pairs, int n_pairs, const oracle_params* prm, const float* poses /*[N][16]*/,
+                        double* JtJ_out, double* Jtr_out, int* n_found_per_pair) {
+	return oracle_dense_system_ex(N, H, W, depth, normal, fx, fy, cx, cy, dense_pairs, n_pairs, prm, poses, 1, JtJ_out, Jtr_out, n_found_per_pair,
+	                              NULL, NULL, NULL, NULL, NULL);
+}
+
+/* The sparse term at given poses as the PCG of oracle_solve_window uses it, over the free frames 1..N-1 (dim = 6(N-1), per frame
+ * trans 0-2 / rot 3-5 like the dense system): A_out = the explicit matrix of applyJT(applyJ(.)), column by column from unit vectors;
+ * rhs_out = -wS J^T F (evalMinusJTF without the dense term); minv_out = the Jacobi preconditioner; rhs_abs_out (optional) = the
+ * gradient sums over |term|, scaled by wS. */
+int oracle_sparse_system(int N, int n_corr, const EntryJ* corr, const oracle_params* prm, const float* poses /*[N][16]*/,
+                         double* A_out, double* rhs_out, double* minv_out, double* rhs_abs_out) {
+	if (N < 2) return -1;
+	const int dimp = 6 * (N - 1);
+	const real wS = (real)prm->w_sparse;
+	mat4* T = (mat4*)malloc(sizeof(mat4) * N);
+	load_poses(N, poses, T, NULL);
+	pose6* p = (pose6*)calloc(N, sizeof(pose6)), *Ap = (pose6*)calloc(N, sizeof(pose6));
+	vec3* Jp = (vec3*)malloc(sizeof(vec3) * (n_corr > 0 ? n_corr : 1));
+	for (int u = 0; u < dimp; u++) {
+		memset(p, 0, sizeof(pose6) * N); memset(Ap, 0, sizeof(pose6) * N);
+		const int fu = 1 + u / 6, cu = u % 6;
+		real* pu = (cu < 3) ? &p[fu].trans.x : &p[fu].rot.x;
+		pu[cu % 3] = R_(1);
+		apply_j(T, n_corr, corr, p, wS, Jp);
+		apply_jt(N, T, n_corr, corr, Jp, Ap);
+		for (int v = 1; v < N; v++) {
+			const real col[6] = { Ap[v].trans.x, Ap[v].trans.y, Ap[v].trans.z, Ap[v].rot.x, Ap[v].rot.y, Ap[v].rot.z };
+			for (int r = 0; r < 6; r++) A_out[(size_t)((v - 1) * 6 + r) * dimp + u] = (double)col[r];
+		}
+	}
+	for (int v = 1; v < N; v++) {
+		vec3 rRot, rTrans, pRot, pTrans, aRot, aTrans;
+		sparse_jtf(v, T, n_corr, corr, (real)prm->robust_delta, &rRot, &rTrans, &pRot, &pTrans, &aRot, &aTrans);
+		const vec3 resRot = vscale(rRot, -wS), resTrans = vscale(rTrans, -wS);
+		const real rr[6] = { resTrans.x, resTrans.y, resTrans.z, resRot.x, resRot.y, resRot.z };
+		const real pc[6] = { pTrans.x, pTrans.y, pTrans.z, pRot.x, pRot.y, pRot.z };
+		const real ra[6] = { aTrans.x, aTrans.y, aTrans.z, aRot.x, aRot.y, aRot.z };
+		for (int r = 0; r < 6; r++) {
+			rhs_out[(v - 1) * 6 + r] = (double)rr[r];
+			minv_out[(v - 1) * 6 + r] = (double)(pc[r] > FLOAT_EPSILON ? R_(1) / pc[r] : R_(1));
+			if (rhs_abs_out) rhs_abs_out[(v - 1) * 6 + r] = (double)(ra[r] * wS);
+		}
+	}
+	free(T); free(p); free(Ap); free(Jp);
+	return 0;
+}
+
+/* The matrix-free sparse operator itself: y = applyJT(applyJ(x)) over frames 1..N-1, x and y in the layout of oracle_sparse_system. */
+int oracle_sparse_apply(int N, int n_corr, const EntryJ* corr, const oracle_params* prm, const float* poses, const double* x, double* y) {
+	if (N < 2) return -1;
+	mat4* T = (mat4*)malloc(sizeof(mat4) * N);
+	load_poses(N, poses, T, NULL);
+	pose6* p = (pose6*)calloc(N, sizeof(pose6)), *Ap = (pose6*)calloc(N, sizeof(pose6));
+	vec3* Jp = (vec3*)malloc(sizeof(vec3) * (n_corr > 0 ? n_corr : 1));
+	for (int v = 1; v < N; v++) {
+		const double* xv = x + (v - 1) * 6;
+		p[v].trans = v3((real)xv[0], (real)xv[1], (real)xv[2]); p[v].rot = v3((real)xv[3], (real)xv[4], (real)xv[5]);
+	}
+	apply_j(T, n_corr, corr, p, (real)prm->w_sparse, Jp);
+	apply_jt(N, T, n_corr, corr, Jp, Ap);
+	for (int v = 1; v < N; v++) {
+		const real o[6] = { Ap[v].trans.x, Ap[v].trans.y, Ap[v].trans.z, Ap[v].rot.x, Ap[v].rot.y, Ap[v].rot.z };
+		for (int r = 0; r < 6; r++) y[(v - 1) * 6 + r] = (double)o[r];
+	}
+	free(T); free(p); free(Ap); free(Jp);
 	return 0;
 }
 
