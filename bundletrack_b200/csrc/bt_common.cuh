@@ -137,6 +137,7 @@ struct PruneState;    // prune.cu
 struct MatchCache;    // prune.cu
 struct TracksDev;     // tracks_dev.cu
 struct MetricsState;  // metrics.cu
+struct NocsState;     // metrics.cu
 
 // The context owns the module states; each module defines the deleter of its state next to it, so the states stay private to their files.
 struct StateDeleter {
@@ -148,6 +149,7 @@ struct StateDeleter {
 	void operator()(MatchCache*) const;
 	void operator()(TracksDev*) const;
 	void operator()(MetricsState*) const;
+	void operator()(NocsState*) const;
 };
 template <class T> using StatePtr = std::unique_ptr<T, StateDeleter>;
 
@@ -165,6 +167,7 @@ struct bt_ctx {
 	bt::StatePtr<bt::MatchCache> mcache;
 	bt::StatePtr<bt::TracksDev> tracks;
 	bt::StatePtr<bt::MetricsState> metrics;
+	bt::StatePtr<bt::NocsState> nocs;
 };
 
 namespace bt {

@@ -305,3 +305,278 @@ extern "C" int bt_vocap(const double* err, int n, double max_err, double* auc_ou
 	*auc_out = area * (1.0 / max_err);      // the reference multiplies by 10 for its 0.1 m; 1.0 / 0.1 rounds to exactly 10
 	return BT_OK;
 }
+
+// ---- NOCS-REAL275: the 6-PACK benchmark (the reference's scripts/benchmark.py) -------------------------------------------------------
+// Per record, in float64, statement by statement as compute_RT_degree_cm_symmetry and compute_3d_iou_new state it (DESIGN.md §3.8):
+//  - columns 0..2 of both 4 x 4 poses are divided by their norms over all four rows (normalizeRotation);
+//  - a bottom row other than [0,0,0,1] on either pose gives theta = shift = 10000;
+//  - R = M[:3,:3] / cbrt(det M[:3,:3]), negative determinants included;
+//  - theta = arccos of the y-axis cosine (symmetric classes) or of (trace(R1 R2^T) - 1) / 2, NOT clipped: an argument beyond +-1 is NaN;
+//  - shift = |T1 - T2|;
+//  - IoU of the two transformed corner sets, with the box extents taken PER CORNER over x, y and z (np.amax(bbox, axis=0) of a [3, 8]
+//    array) and the division by the homogeneous row; for symmetric classes the maximum over 20 rotations of the ground truth about its y
+//    axis (gt @ Y(2 pi i / 20)), starting at 0 and skipping NaN as Python's max(max_iou, v) does.
+// Operation order, pinned (numpy's dot / norm / det / matmul go through BLAS and LAPACK, whose rounding is not): every sum of products is
+// ((a0 b0 + a1 b1) + a2 b2) + a3 b3 left to right, without fused multiply-adds (__dmul_rn / __dadd_rn); det = a(ei - fh) - b(di - fg) +
+// c(dh - eg); products over the 8 corners run in corner order.  cbrt and acos are CUDA's (1 ulp / 2 ulp), the 20 (cos, sin) pairs are the
+// host's libm of ((2 pi) i) / 20.0.
+namespace bt {
+namespace {
+
+constexpr int kNocsWarps = 4;                      // records per block
+constexpr int kNocsRot = 20;                       // the benchmark's rotations about y
+constexpr double kRadToDeg = 180.0 / 3.141592653589793;
+
+struct NocsRecord {
+	double pred[16], gt[16];     // row-major 4 x 4, translations in mm
+	double corners[24];          // 8 rows x, y, z of model_scales/<model>.txt
+	int32_t sym, pad;
+};
+
+__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ double dot3(double a0, double a1, double a2, double b0, double b1, double b2) {
+	return add(add(mul(a0, b0), mul(a1, b1)), mul(a2, b2));
+}
+// numpy's maximum / minimum: a NaN on either side is the result
+__device__ __forceinline__ double nmax(double a, double b) { return (a > b || isnan(a)) ? a : b; }
+__device__ __forceinline__ double nmin(double a, double b) { return (a < b || isnan(a)) ? a : b; }
+
+__device__ __forceinline__ void normalize_columns(double* M) {
+#pragma unroll
+	for (int c = 0; c < 3; c++) {
+		const double n = sqrt(add(add(add(mul(M[c], M[c]), mul(M[4 + c], M[4 + c])), mul(M[8 + c], M[8 + c])), mul(M[12 + c], M[12 + c])));
+#pragma unroll
+		for (int r = 0; r < 4; r++) M[4 * r + c] = __ddiv_rn(M[4 * r + c], n);
+	}
+}
+
+__device__ __forceinline__ double det3(const double* M) {
+	const double a = mul(M[0], sub(mul(M[5], M[10]), mul(M[6], M[9])));
+	const double b = mul(M[1], sub(mul(M[4], M[10]), mul(M[6], M[8])));
+	const double c = mul(M[2], sub(mul(M[4], M[9]), mul(M[5], M[8])));
+	return add(sub(a, b), c);
+}
+
+// transform_coordinates_3d of one corner: row r of M [x y z 1]^T over the homogeneous row, then the corner's max / min over x, y, z
+__device__ __forceinline__ void corner_extent(const double* M, double x, double y, double z, double& hi, double& lo) {
+	double w[4];
+#pragma unroll
+	for (int r = 0; r < 4; r++) w[r] = add(add(add(mul(M[4 * r], x), mul(M[4 * r + 1], y)), mul(M[4 * r + 2], z)), M[4 * r + 3]);
+	const double u0 = __ddiv_rn(w[0], w[3]), u1 = __ddiv_rn(w[1], w[3]), u2 = __ddiv_rn(w[2], w[3]);
+	hi = nmax(nmax(u0, u1), u2);
+	lo = nmin(nmin(u0, u1), u2);
+}
+
+// grid ceil(n / kNocsWarps) x (32 kNocsWarps): one warp per record.  Lane r < 20 of a symmetric record evaluates rotation r, lane 0 of any
+// other record the asymmetric IoU (rotation 0: cos 1, sin 0 reproduces gt exactly).
+__global__ void __launch_bounds__(32 * kNocsWarps) k_nocs_metrics(const NocsRecord* __restrict__ recs, const double2* __restrict__ rot, int n,
+                                                                  double* __restrict__ theta_out, double* __restrict__ shift_out,
+                                                                  double* __restrict__ iou_out) {
+	const int lane = threadIdx.x & 31;
+	const int i = blockIdx.x * kNocsWarps + (threadIdx.x >> 5);
+	if (i >= n) return;                                // whole warps leave together
+	const NocsRecord& rec = recs[i];
+	double P[16], G[16];
+#pragma unroll
+	for (int k = 0; k < 16; k++) { P[k] = rec.pred[k]; G[k] = rec.gt[k]; }
+	const bool sym = rec.sym != 0;
+	normalize_columns(P);
+	normalize_columns(G);
+
+	if (lane == 0) {
+		double theta = 10000.0, shift = 10000.0;
+		const bool bottom = P[12] == 0.0 && P[13] == 0.0 && P[14] == 0.0 && P[15] == 1.0 && G[12] == 0.0 && G[13] == 0.0 && G[14] == 0.0 && G[15] == 1.0;
+		if (bottom) {
+			const double c1 = cbrt(det3(P)), c2 = cbrt(det3(G));
+			double R1[9], R2[9];
+#pragma unroll
+			for (int r = 0; r < 3; r++)
+#pragma unroll
+				for (int c = 0; c < 3; c++) { R1[3 * r + c] = __ddiv_rn(P[4 * r + c], c1); R2[3 * r + c] = __ddiv_rn(G[4 * r + c], c2); }
+			double arg;
+			if (sym) {
+				// y1 = R1 [0 1 0]^T, y2 = R2 [0 1 0]^T: the middle columns
+				const double d = dot3(R1[1], R1[4], R1[7], R2[1], R2[4], R2[7]);
+				const double n1 = sqrt(dot3(R1[1], R1[4], R1[7], R1[1], R1[4], R1[7]));
+				const double n2 = sqrt(dot3(R2[1], R2[4], R2[7], R2[1], R2[4], R2[7]));
+				arg = __ddiv_rn(d, mul(n1, n2));
+			} else {
+				// trace(R1 R2^T) = sum_r R1[r,:] . R2[r,:]
+				const double t0 = dot3(R1[0], R1[1], R1[2], R2[0], R2[1], R2[2]);
+				const double t1 = dot3(R1[3], R1[4], R1[5], R2[3], R2[4], R2[5]);
+				const double t2 = dot3(R1[6], R1[7], R1[8], R2[6], R2[7], R2[8]);
+				arg = __ddiv_rn(sub(add(add(t0, t1), t2), 1.0), 2.0);
+			}
+			theta = mul(acos(arg), kRadToDeg);
+			const double dx = sub(P[3], G[3]), dy = sub(P[7], G[7]), dz = sub(P[11], G[11]);
+			shift = sqrt(dot3(dx, dy, dz, dx, dy, dz));
+		}
+		theta_out[i] = theta;
+		shift_out[i] = shift;
+	}
+
+	double iou = 0.0;
+	if (lane < (sym ? kNocsRot : 1)) {
+		// gt @ Y(t): columns 0 and 2 mix, 1 and 3 stay
+		const double2 cs = rot[lane];
+#pragma unroll
+		for (int r = 0; r < 4; r++) {
+			const double g0 = G[4 * r], g2 = G[4 * r + 2];
+			G[4 * r] = add(mul(g0, cs.x), mul(g2, -cs.y));
+			G[4 * r + 2] = add(mul(g0, cs.y), mul(g2, cs.x));
+		}
+		double dmin = INFINITY, inter = 1.0, v1 = 1.0, v2 = 1.0;
+#pragma unroll 1
+		for (int c = 0; c < 8; c++) {
+			const double x = rec.corners[3 * c], y = rec.corners[3 * c + 1], z = rec.corners[3 * c + 2];
+			double hi1, lo1, hi2, lo2;
+			corner_extent(G, x, y, z, hi1, lo1);
+			corner_extent(P, x, y, z, hi2, lo2);
+			const double d = sub(nmin(hi1, hi2), nmax(lo1, lo2));
+			dmin = c == 0 ? d : nmin(dmin, d);
+			inter = c == 0 ? d : mul(inter, d);
+			v1 = c == 0 ? sub(hi1, lo1) : mul(v1, sub(hi1, lo1));
+			v2 = c == 0 ? sub(hi2, lo2) : mul(v2, sub(hi2, lo2));
+		}
+		if (dmin < 0.0) inter = 0.0;
+		iou = __ddiv_rn(inter, sub(add(v1, v2), inter));
+	}
+	if (sym) {
+		// max(max_iou, v) from 0 in rotation order: a value enters only if it is greater, so NaN never does
+		double best = (iou > 0.0) ? iou : 0.0;
+		for (int o = 16; o > 0; o >>= 1) {
+			const double v = __shfl_xor_sync(0xffffffffu, best, o);
+			if (v > best) best = v;
+		}
+		iou = best;
+	}
+	if (lane == 0) iou_out[i] = iou;
+}
+
+}  // namespace
+
+struct NocsState {
+	int max_records = 0;
+	DevBuf recs;
+	UploadBuf h_recs;
+};
+void StateDeleter::operator()(NocsState* s) const { delete s; }
+
+}  // namespace bt
+
+extern "C" int bt_nocs_reserve(bt_ctx* ctx, int max_records) {
+	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_nocs_reserve: ctx is NULL");
+	BT_REQUIRE(max_records >= 1, BT_ERR_INVALID_ARG, "bt_nocs_reserve: max_records %d must be >= 1", max_records);
+	BT_CUDA(cudaSetDevice(ctx->device));
+	if (!ctx->nocs) ctx->nocs.reset(new NocsState());
+	NocsState* s = ctx->nocs.get();
+	const size_t bytes = kNocsRot * sizeof(double2) + sizeof(NocsRecord) * (size_t)max_records;
+	BT_TRY(s->recs.alloc(bytes));
+	BT_TRY(s->h_recs.reserve(bytes));
+	s->max_records = max_records;
+	return BT_OK;
+}
+
+extern "C" int bt_nocs_metrics(bt_ctx* ctx, const double* pred, const double* gt, const double* corners, const int32_t* symmetric, int n,
+                               double* theta_deg_out, double* shift_out, double* iou_out, void* stream_) {
+	BT_REQUIRE(n >= 1, BT_ERR_INVALID_ARG, "bt_nocs_metrics: n %d must be >= 1", n);
+	BT_REQUIRE(pred && gt && corners && symmetric && theta_deg_out && shift_out && iou_out, BT_ERR_INVALID_ARG, "bt_nocs_metrics: NULL argument");
+	for (size_t k = 0; k < 16 * (size_t)n; k++)
+		BT_REQUIRE(isfinite(pred[k]) && isfinite(gt[k]), BT_ERR_INVALID_ARG, "bt_nocs_metrics: record %d has a non-finite pose element", (int)(k / 16));
+	for (size_t k = 0; k < 24 * (size_t)n; k++)
+		BT_REQUIRE(isfinite(corners[k]), BT_ERR_INVALID_ARG, "bt_nocs_metrics: record %d has a non-finite corner", (int)(k / 24));
+	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_nocs_metrics: ctx is NULL");
+	NocsState* s = ctx->nocs.get();
+	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_nocs_metrics: call bt_nocs_reserve first");
+	BT_REQUIRE(n <= s->max_records, BT_ERR_CAPACITY, "bt_nocs_metrics: %d records exceed the reserved %d", n, s->max_records);
+	cudaStream_t stream = (cudaStream_t)stream_;
+	BT_CUDA(cudaSetDevice(ctx->device));
+	char* h;
+	BT_TRY(s->h_recs.acquire(0, &h));
+	double2* hrot = reinterpret_cast<double2*>(h);
+	for (int r = 0; r < kNocsRot; r++) {
+		const double t = ((2.0 * 3.141592653589793) * r) / 20.0;      // 2 * math.pi * i / float(n), Python's order
+		hrot[r] = make_double2(cos(t), sin(t));
+	}
+	NocsRecord* hr = reinterpret_cast<NocsRecord*>(h + kNocsRot * sizeof(double2));
+	for (int i = 0; i < n; i++) {
+		memcpy(hr[i].pred, pred + 16 * (size_t)i, sizeof(hr[i].pred));
+		memcpy(hr[i].gt, gt + 16 * (size_t)i, sizeof(hr[i].gt));
+		memcpy(hr[i].corners, corners + 24 * (size_t)i, sizeof(hr[i].corners));
+		hr[i].sym = symmetric[i] != 0;
+		hr[i].pad = 0;
+	}
+	const size_t bytes = kNocsRot * sizeof(double2) + sizeof(NocsRecord) * (size_t)n;
+	BT_CUDA(cudaMemcpyAsync(s->recs.p, h, bytes, cudaMemcpyHostToDevice, stream));
+	BT_TRY(s->h_recs.in_flight(stream));
+	const double2* d_rot = s->recs.as<double2>();
+	const NocsRecord* d_recs = reinterpret_cast<const NocsRecord*>(s->recs.as<char>() + kNocsRot * sizeof(double2));
+	k_nocs_metrics<<<(n + kNocsWarps - 1) / kNocsWarps, 32 * kNocsWarps, 0, stream>>>(d_recs, d_rot, n, theta_deg_out, shift_out, iou_out);
+	BT_CUDA(cudaGetLastError());
+	return BT_OK;
+}
+
+// numpy's pairwise summation (pairwise_sum in loops_utils.h): below 8 terms in order, up to 128 through 8 accumulators, above that split
+// at a multiple of 8 near the middle.  np.add.reduce feeds it all terms of a contiguous array, np.mean divides the result by the count.
+static double np_pairwise_sum(const double* a, size_t n) {
+	if (n < 8) {
+		double res = -0.0;
+		for (size_t i = 0; i < n; i++) res += a[i];
+		return res;
+	}
+	if (n <= 128) {
+		double r[8];
+		for (int j = 0; j < 8; j++) r[j] = a[j];
+		size_t i = 8;
+		for (; i < n - (n % 8); i += 8)
+			for (int j = 0; j < 8; j++) r[j] += a[i + j];
+		double res = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
+		for (; i < n; i++) res += a[i];
+		return res;
+	}
+	size_t n2 = n / 2;
+	n2 -= n2 % 8;
+	return np_pairwise_sum(a, n2) + np_pairwise_sum(a + n2, n - n2);
+}
+
+static double np_mean(const std::vector<double>& v) {
+	if (v.empty()) return NAN;                       // np.mean([])
+	return np_pairwise_sum(v.data(), v.size()) / (double)v.size();
+}
+
+// benchmark.py main's aggregation: per class the 5 deg 5 cm and IoU25 fractions of all its records, the mean theta over IoU > 0.25 and
+// theta < 360, the mean shift over IoU > 0.25; overall x += v / 6 in class order.
+extern "C" int bt_nocs_score(const int32_t* cls, const int32_t* scored, const double* theta_deg, const double* shift, const double* iou, int n,
+                             double* per_class_out, double* overall_out) {
+	BT_REQUIRE(n >= 1, BT_ERR_INVALID_ARG, "bt_nocs_score: n %d must be >= 1", n);
+	BT_REQUIRE(cls && scored && theta_deg && shift && iou && per_class_out && overall_out, BT_ERR_INVALID_ARG, "bt_nocs_score: NULL argument");
+	int cls_num[6] = {0, 0, 0, 0, 0, 0};
+	for (int i = 0; i < n; i++) {
+		BT_REQUIRE(cls[i] >= 1 && cls[i] <= 6, BT_ERR_INVALID_ARG, "bt_nocs_score: record %d has class %d outside 1..6", i, cls[i]);
+		cls_num[cls[i] - 1]++;
+	}
+	for (int c = 0; c < 6; c++)
+		BT_REQUIRE(cls_num[c] > 0, BT_ERR_INVALID_ARG, "bt_nocs_score: class %d has no record (the benchmark divides by its count)", c + 1);
+	double overall[4] = {0.0, 0.0, 0.0, 0.0};
+	std::vector<double> rot, trans;
+	for (int c = 0; c < 6; c++) {
+		int in55 = 0, iou25 = 0;
+		rot.clear();
+		trans.clear();
+		for (int i = 0; i < n; i++) {
+			if (cls[i] != c + 1 || !scored[i]) continue;
+			if (iou[i] > 0.25 && theta_deg[i] < 360) rot.push_back(theta_deg[i]);
+			if (iou[i] > 0.25) { trans.push_back(shift[i]); iou25++; }
+			if (theta_deg[i] < 5 && shift[i] < 50) in55++;
+		}
+		const double v[4] = {(double)in55 / (double)cls_num[c], (double)iou25 / (double)cls_num[c], np_mean(rot), np_mean(trans)};
+		for (int k = 0; k < 4; k++) {
+			per_class_out[4 * c + k] = v[k];
+			overall[k] += v[k] / 6;
+		}
+	}
+	for (int k = 0; k < 4; k++) overall_out[k] = overall[k];
+	return BT_OK;
+}

@@ -174,6 +174,34 @@ inline double voCap(const std::vector<double>& err, double max_err = 0.1) {
 	return auc;
 }
 
+// scripts/benchmark.py (6-PACK, NOCS-REAL275) per record in one device call: theta (degrees), shift and IoU into device double [n] arrays,
+// asynchronous on `stream`.  pred / gt as the benchmark compares them (translations in mm); corners: 24 doubles per record (the 8 rows of
+// model_scales/<model>.txt); symmetric: bottle, bowl and can.  The context needs bt_nocs_reserve(ctx, >= pred.size()).
+template <class Mat4>
+inline void nocsMetrics(bt_ctx* ctx, const std::vector<Mat4>& pred, const std::vector<Mat4>& gt, const std::vector<double>& corners,
+                        const std::vector<int32_t>& symmetric, double* theta_gpu, double* shift_gpu, double* iou_gpu, void* stream = nullptr) {
+	if (pred.size() != gt.size() || symmetric.size() != pred.size() || corners.size() != 24 * pred.size())
+		throw std::runtime_error("nocsMetrics: pred, gt, corners and symmetric differ in length");
+	std::vector<double> p(16 * pred.size()), g(16 * gt.size());
+	for (size_t f = 0; f < pred.size(); f++)
+		for (int r = 0; r < 4; r++)
+			for (int c = 0; c < 4; c++) { p[16 * f + 4 * r + c] = pred[f](r, c); g[16 * f + 4 * r + c] = gt[f](r, c); }
+	if (bt_nocs_metrics(ctx, p.data(), g.data(), corners.data(), symmetric.data(), (int)pred.size(), theta_gpu, shift_gpu, iou_gpu, stream) != BT_OK)
+		throw std::runtime_error(std::string("bt_nocs_metrics: ") + bt_last_error());
+}
+
+// benchmark.py's aggregation: per class (bottle .. mug) and overall {5 deg 5 cm fraction, IoU25 fraction, mean theta, mean shift (mm)}.
+struct NocsScore { double per_class[6][4]; double overall[4]; };
+inline NocsScore nocsScore(const std::vector<int32_t>& cls, const std::vector<int32_t>& scored, const std::vector<double>& theta_deg,
+                           const std::vector<double>& shift, const std::vector<double>& iou) {
+	const size_t n = cls.size();
+	if (scored.size() != n || theta_deg.size() != n || shift.size() != n || iou.size() != n) throw std::runtime_error("nocsScore: lengths differ");
+	NocsScore s;
+	if (bt_nocs_score(cls.data(), scored.data(), theta_deg.data(), shift.data(), iou.data(), (int)n, &s.per_class[0][0], s.overall) != BT_OK)
+		throw std::runtime_error(std::string("bt_nocs_score: ") + bt_last_error());
+	return s;
+}
+
 // ransacMultiPairGPU with the reference's argument list (device float4 arrays per pair, host result vectors).  The device result
 // buffers and the library's scratch belong to the object: nothing is allocated per call (the reference allocates six arrays and a
 // stream per pair per call, cuda_ransac.cu:1240-1275).

@@ -545,6 +545,34 @@ BT_API int bt_pose_metrics(bt_ctx* ctx, const double* model_pts_dev, int n_pts, 
  * as below max_err.  BT_ERR_INVALID_ARG for n < 0, err NULL with n > 0, auc_out NULL or max_err not positive and finite. */
 BT_API int bt_vocap(const double* err, int n, double max_err, double* auc_out);
 
+/* ---- NOCS-REAL275 scoring: the reference's 6-PACK benchmark (scripts/benchmark.py) -----------------------------------------------------
+ * bt_nocs_metrics: per record i, theta (degrees), shift and IoU as compute_RT_degree_cm_symmetry(pred, gt) and compute_3d_iou_new(gt, pred)
+ * return them, in float64, with the benchmark's quirks kept (DESIGN.md §3.8): columns normalised over all four rows, a bottom row other
+ * than [0,0,0,1] gives theta = shift = 10000, the rotation is divided by cbrt(det), arccos is not clipped (an argument beyond +-1 gives a
+ * NaN theta), the "box" extents are taken per corner over x, y and z, and for a symmetric record theta uses the y axes and the IoU is the
+ * maximum (from 0, NaN skipped) over 20 rotations of gt about its y axis.  The operation order is fixed, so results do not depend on n.
+ *   pred / gt   HOST row-major 4 x 4 per record, translations in mm, as the benchmark compares them (before normalizeRotation).
+ *   corners     HOST n x 8 x 3: the rows of model_scales/<model>.txt.
+ *   symmetric   HOST n flags: the y-axis rule (bottle, bowl and can; the benchmark never applies it to mugs).
+ *   theta_deg_out / shift_out / iou_out  DEVICE float64 [n].
+ * Asynchronous on `stream`: the inputs are copied before the call returns, the results are ready when the stream is.  BT_ERR_INVALID_ARG
+ * for n < 1, a NULL pointer, a non-finite input element, or a context without bt_nocs_reserve; BT_ERR_CAPACITY above max_records.
+ * bt_nocs_reserve: room for max_records records per call, 456 B each on the device and in pinned host memory. */
+BT_API int bt_nocs_reserve(bt_ctx* ctx, int max_records);
+BT_API int bt_nocs_metrics(bt_ctx* ctx, const double* pred, const double* gt, const double* corners, const int32_t* symmetric, int n,
+                           double* theta_deg_out, double* shift_out, double* iou_out, void* stream);
+/* The benchmark's aggregation (benchmark.py main), host code, no GPU.  Records in the order given; cls[i] in 1..6 (bottle, bowl, camera, can,
+ * laptop, mug); scored[i] = 0 for a record that is counted but not scored.  per_class_out[4 c + k] for class c + 1 and overall_out[k]:
+ *   k = 0  5 deg 5 cm fraction: theta < 5 and shift < 50, over the class's record count
+ *   k = 1  IoU25 fraction: IoU > 0.25, over the same count
+ *   k = 2  mean theta over IoU > 0.25 and theta < 360 (NaN when empty)
+ *   k = 3  mean shift over IoU > 0.25 (NaN when empty)
+ * Means are numpy's (pairwise sum, then / count); overall is x += v / 6 in class order, so NaN class means reach it.  Fed the benchmark's
+ * own per-record values, every number equals what it prints (x 100 for fractions, / 10 for the shift in cm).  BT_ERR_INVALID_ARG for
+ * n < 1, a NULL pointer, a class outside 1..6 or a class without records. */
+BT_API int bt_nocs_score(const int32_t* cls, const int32_t* scored, const double* theta_deg, const double* shift, const double* iou, int n,
+                         double* per_class_out, double* overall_out);
+
 /* Small device-memory helpers so non-CUDA hosts (ctypes, cgo, JNI) can drive the library without another runtime. */
 BT_API int bt_dev_alloc(void** out, size_t bytes);
 BT_API int bt_dev_free(void* p);
