@@ -20,7 +20,10 @@ BT_FRAME_OTHER, BT_FRAME_FAIL, BT_FRAME_NO_BA = 0, 1, 2      # Frame::_status as
 
 
 class BtError(RuntimeError):
-    pass
+    """A library call failed; rc is its BT_* status (None when the error was raised on the Python side)."""
+    def __init__(self, msg: str, rc: int = None):
+        super().__init__(msg)
+        self.rc = rc
 
 
 class SolverParams(ctypes.Structure):
@@ -150,12 +153,12 @@ EXPORTS = [
     "bt_solve_windows", "bt_solve_windows_begin", "bt_solve_windows_end", "bt_solve_stage", "bt_solve_run", "bt_solve_fetch", "bt_solve_get_stats",
     "bt_solve_enable_debug", "bt_solve_debug_dense", "bt_solve_debug_counts", "bt_solve_debug_system", "bt_solve_enable_timing", "bt_solve_get_timing", "bt_solve_get_host_timing", "bt_solve_enable_profile", "bt_solve_get_profile",
     "bt_matcher_reserve", "bt_desc_pool_reserve", "bt_desc_pool_store", "bt_knn_match_slots", "bt_match_pairs_pool", "bt_match_pairs_ex", "bt_match_cache_reserve", "bt_match_cache_reserve_entries", "bt_match_cache_usage", "bt_match_cache_put", "bt_match_cache_has", "bt_match_cache_status", "bt_match_cache_gather", "bt_match_cache_forget_frame", "bt_knn_match_pairs", "bt_knn_enable_timing", "bt_knn_get_timing", "bt_knn_debug_force_fallback", "bt_ransac_reserve", "bt_ransac_pairs", "bt_ransac_debug",
-    "bt_pipeline_reserve", "bt_prune_mutual_pairs", "bt_match_pairs", "bt_frames_preprocess", "bt_frames_preprocess_masked", "bt_lfnet_request",
+    "bt_pipeline_reserve", "bt_prune_mutual_pairs", "bt_match_pairs", "bt_frames_preprocess", "bt_frames_preprocess_masked", "bt_frames_preprocess_masked_u16", "bt_lfnet_request",
     "bt_frame_cache_reserve", "bt_frame_cache_store",
     "bt_rotation_geodesic", "bt_keyframe_check", "bt_select_keyframes", "bt_rigid_transform", "bt_lfnet_parse_reply", "bt_ba_gate", "bt_pose_format", "bt_pose_write_txt",
     "bt_tracks_create", "bt_tracks_destroy", "bt_tracks_update_pair", "bt_tracks_propagate", "bt_tracks_forget_frame", "bt_tracks_stats",
     "bt_tracks_dev_reserve", "bt_tracks_dev_reserve_ex", "bt_tracks_dev_update_pair", "bt_tracks_dev_propagate", "bt_tracks_dev_forget_frame", "bt_tracks_dev_stats", "bt_find_corres_pairs",
-    "bt_pose_init", "bt_tracker_create", "bt_tracker_destroy", "bt_tracker_begin_frame", "bt_tracker_end_frame", "bt_tracker_drop_frame", "bt_tracker_state", "bt_tracker_usage",
+    "bt_pose_init", "bt_tracker_create", "bt_tracker_destroy", "bt_tracker_begin_frame", "bt_tracker_begin_frame_u16", "bt_tracker_end_frame", "bt_tracker_drop_frame", "bt_tracker_state", "bt_tracker_usage",
     "bt_metrics_reserve", "bt_pose_metrics", "bt_vocap", "bt_nocs_reserve", "bt_nocs_metrics", "bt_nocs_score",
     "bt_dev_alloc", "bt_dev_free", "bt_memcpy_h2d", "bt_memcpy_d2h", "bt_host_alloc_pinned", "bt_host_free_pinned",
     "bt_stream_sync", "bt_debug_live_resources",
@@ -191,4 +194,4 @@ def load() -> ctypes.CDLL:
 def check(rc: int, what: str = "") -> None:
     if rc != BT_OK:
         msg = load().bt_last_error().decode("utf-8", "replace")
-        raise BtError(f"{what} failed with status {rc}: {msg}")
+        raise BtError(f"{what} failed with status {rc}: {msg}", rc)

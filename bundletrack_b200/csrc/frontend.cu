@@ -5,7 +5,7 @@
 // pair around each group and two device->host copies of the maps for PCL.  Here ONE kernel does the whole chain per
 // output tile: the raw depth of the tile plus its halo (erode radius + 2 x filter radius + 1 for the normal stencil) is
 // staged in shared memory once and the four stencils ping-pong between two shared arrays, so the image is read ~1.6x
-// and the three results (filtered depth, points, normals) are written once.  HBM-bound: 4 B in, 4 + 16 + 16 B out per
+// and the three results (filtered depth, points, normals) are written once.  HBM-bound: 4 B in (2 B from a depth PNG), 4 + 16 + 16 B out per
 // pixel.  Arithmetic follows the reference statement by statement (loop order of the float accumulations, float vs
 // double comparisons, the hole-filling behaviour of the filter on invalid centre pixels).
 #include "bt_common.cuh"
@@ -16,7 +16,7 @@ static constexpr int FE_TW = 64, FE_TH = 32, FE_THREADS = 256;
 static constexpr int FE_MAX_HALO = 12;
 
 struct FrontArgs {
-	const float* const* depth_in;   // [n] device pointers, H x W
+	const void* const* depth_in;    // [n] device pointers, H x W: float metres, or uint16 millimetres (the _u16 instantiation)
 	float* const* depth_out;        // [n]
 	float4* const* xyz_out;         // [n] or nullptr entries
 	float4* const* normal_out;      // [n]
@@ -90,7 +90,15 @@ struct MaskArgs {
 };
 static constexpr int FE_MW = FE_TW + 4, FE_MH = FE_TH + 4;
 
-template <bool MASKED>
+// One raw depth sample in metres.  uint16: Utils::readDepthImage (Utils.cpp:57-66) on the depth PNG's millimetres: (float)s * 0.001 is a
+// double multiply (0.001 is a double literal) rounded to float, and values below 0.1 m (compared in double) become 0.
+__device__ __forceinline__ float depth_sample(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float depth_sample(const uint16_t* p) {
+	const float d = __double2float_rn(__dmul_rn((double)__ldg(p), 0.001));
+	return ((double)d < 0.1) ? 0.f : d;
+}
+
+template <bool MASKED, class DIn>
 __device__ __forceinline__ void frontend_tile(const FrontArgs& a, const MaskArgs& mk) {
 	extern __shared__ float fe_smem[];
 	const int er = a.er, br = a.br, halo = er + 2 * br + 1;
@@ -100,11 +108,11 @@ __device__ __forceinline__ void frontend_tile(const FrontArgs& a, const MaskArgs
 	const int f = blockIdx.z;
 	const int x0 = blockIdx.x * FE_TW - halo, y0 = blockIdx.y * FE_TH - halo;   // image coordinates of region cell (0,0)
 	const int W = a.W, H = a.H;
-	const float* __restrict__ din = a.depth_in[f];
+	const DIn* __restrict__ din = static_cast<const DIn*>(a.depth_in[f]);
 	// ---- stage 0: raw depth of the region; cells outside the image hold 0 here and after every later stage
 	for (int c = threadIdx.x; c < RW * RH; c += FE_THREADS) {
 		const int cx = c % RW, cy = c / RW, x = x0 + cx, y = y0 + cy;
-		A[c] = (x >= 0 && x < W && y >= 0 && y < H) ? __ldg(din + (size_t)y * W + x) : 0.f;
+		A[c] = (x >= 0 && x < W && y >= 0 && y < H) ? depth_sample(din + (size_t)y * W + x) : 0.f;
 	}
 	uint8_t* Ms = reinterpret_cast<uint8_t*>(fe_smem + 2 * RW * RH + 3 * (2 * br + 1) * (2 * br + 1));   // [FE_MH][FE_MW] mask, halo 2
 	if constexpr (MASKED) {
@@ -246,8 +254,9 @@ __device__ __forceinline__ void frontend_tile(const FrontArgs& a, const MaskArgs
 	}
 }
 
-__global__ void __launch_bounds__(FE_THREADS) k_frame_frontend(FrontArgs a) { frontend_tile<false>(a, MaskArgs{}); }
-__global__ void __launch_bounds__(FE_THREADS) k_frame_frontend_masked(FrontArgs a, MaskArgs m) { frontend_tile<true>(a, m); }
+__global__ void __launch_bounds__(FE_THREADS) k_frame_frontend(FrontArgs a) { frontend_tile<false, float>(a, MaskArgs{}); }
+__global__ void __launch_bounds__(FE_THREADS) k_frame_frontend_masked(FrontArgs a, MaskArgs m) { frontend_tile<true, float>(a, m); }
+__global__ void __launch_bounds__(FE_THREADS) k_frame_frontend_masked_u16(FrontArgs a, MaskArgs m) { frontend_tile<true, uint16_t>(a, m); }
 
 struct FrontState {
 	DevBuf tables;
@@ -273,7 +282,8 @@ struct MaskSpec {
 	int32_t* roi_out;               // device [n][4]
 };
 
-static int frames_preprocess(bt_ctx* ctx, const char* who, int n_frames, const float* const* depth_raw_dev, int H, int W, float fx, float fy, float cx, float cy,
+// depth_raw_dev: float metres, or uint16 millimetres when u16 (masked calls only)
+static int frames_preprocess(bt_ctx* ctx, const char* who, int n_frames, const void* const* depth_raw_dev, bool u16, int H, int W, float fx, float fy, float cx, float cy,
                              const bt_depth_params* prm, float* const* depth_out_dev, float* const* xyz_out_dev, float* const* normal_out_dev,
                              const MaskSpec* mask, void* stream_) {
 	BT_REQUIRE(ctx && depth_raw_dev && prm && depth_out_dev && normal_out_dev, BT_ERR_INVALID_ARG, "%s: NULL argument", who);
@@ -330,7 +340,7 @@ static int frames_preprocess(bt_ctx* ctx, const char* who, int n_frames, const f
 	BT_TRY(s->h_tables.in_flight(stream));
 	FrontArgs a;
 	const void** dt = s->tables.as<const void*>();
-	a.depth_in = (const float* const*)dt; a.depth_out = (float* const*)(dt + n_frames);
+	a.depth_in = dt; a.depth_out = (float* const*)(dt + n_frames);
 	a.xyz_out = any_xyz ? (float4* const*)(dt + 2 * n_frames) : nullptr; a.normal_out = (float4* const*)(dt + 3 * n_frames);
 	a.H = H; a.W = W;
 	{   // Eigen::Matrix3f::inverse() of [[fx,0,cx],[0,fy,cy],[0,0,1]] (Frame.cpp:189): cofactors times 1/det, in float
@@ -351,8 +361,9 @@ static int frames_preprocess(bt_ctx* ctx, const char* who, int n_frames, const f
 		                                       s->seg_best.as<unsigned long long>(), s->seg_fill.as<uint8_t>(), stream)) != BT_OK) return rc;
 		MaskArgs m;
 		m.mask_in = (const uint8_t* const*)(dt + 6 * n_frames); m.fg_out = (uint8_t* const*)(dt + 5 * n_frames); m.roi = mask->roi_out;
-		if (smem > 48 * 1024) BT_CUDA(cudaFuncSetAttribute(k_frame_frontend_masked, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-		k_frame_frontend_masked<<<grid, FE_THREADS, smem, stream>>>(a, m);
+		auto* k = u16 ? k_frame_frontend_masked_u16 : k_frame_frontend_masked;
+		if (smem > 48 * 1024) BT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+		k<<<grid, FE_THREADS, smem, stream>>>(a, m);
 	}
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;
@@ -365,7 +376,7 @@ using namespace bt;
 extern "C" int bt_frames_preprocess(bt_ctx* ctx, int n_frames, const float* const* depth_raw_dev, int H, int W, float fx, float fy, float cx, float cy,
                                     const bt_depth_params* prm, float* const* depth_out_dev, float* const* xyz_out_dev, float* const* normal_out_dev,
                                     void* stream_) {
-	return frames_preprocess(ctx, "bt_frames_preprocess", n_frames, depth_raw_dev, H, W, fx, fy, cx, cy, prm, depth_out_dev, xyz_out_dev, normal_out_dev,
+	return frames_preprocess(ctx, "bt_frames_preprocess", n_frames, (const void* const*)depth_raw_dev, false, H, W, fx, fy, cx, cy, prm, depth_out_dev, xyz_out_dev, normal_out_dev,
 	                         nullptr, stream_);
 }
 
@@ -374,8 +385,17 @@ extern "C" int bt_frames_preprocess_masked(bt_ctx* ctx, int n_frames, const floa
                                            float* const* xyz_out_dev, float* const* normal_out_dev, uint8_t* const* fg_out_dev, int32_t* roi_out_dev,
                                            void* stream_) {
 	const MaskSpec m{mask_dev, mask_mode, fg_out_dev, roi_out_dev};
-	return frames_preprocess(ctx, "bt_frames_preprocess_masked", n_frames, depth_raw_dev, H, W, fx, fy, cx, cy, prm, depth_out_dev, xyz_out_dev, normal_out_dev,
+	return frames_preprocess(ctx, "bt_frames_preprocess_masked", n_frames, (const void* const*)depth_raw_dev, false, H, W, fx, fy, cx, cy, prm, depth_out_dev, xyz_out_dev, normal_out_dev,
 	                         &m, stream_);
+}
+
+extern "C" int bt_frames_preprocess_masked_u16(bt_ctx* ctx, int n_frames, const uint16_t* const* depth_mm_dev, const uint8_t* const* mask_dev, int mask_mode,
+                                               int H, int W, float fx, float fy, float cx, float cy, const bt_depth_params* prm, float* const* depth_out_dev,
+                                               float* const* xyz_out_dev, float* const* normal_out_dev, uint8_t* const* fg_out_dev, int32_t* roi_out_dev,
+                                               void* stream_) {
+	const MaskSpec m{mask_dev, mask_mode, fg_out_dev, roi_out_dev};
+	return frames_preprocess(ctx, "bt_frames_preprocess_masked_u16", n_frames, (const void* const*)depth_mm_dev, true, H, W, fx, fy, cx, cy, prm, depth_out_dev,
+	                         xyz_out_dev, normal_out_dev, &m, stream_);
 }
 
 extern "C" int bt_lfnet_request(bt_ctx* ctx, int n_frames, const uint8_t* const* colour_dev, const uint8_t* const* fg_dev, const int32_t* roi_dev,

@@ -1,7 +1,7 @@
 // tracker.cu — the whole tracking step, Bundler::processNewFrame (the reference's src/Bundler.cpp:56-183), as one library object over the
 // existing entry points, plus k_pose_init: SiftManager::procrustesByCorrespondence (FeatureManager.cpp:523-557) on the device.
 //
-// The tracker is host code: it calls bt_frames_preprocess_masked, bt_lfnet_request, bt_desc_pool_store, bt_find_corres_pairs, bt_pose_init,
+// The tracker is host code: it calls bt_frames_preprocess_masked (or _u16), bt_lfnet_request, bt_desc_pool_store, bt_find_corres_pairs, bt_pose_init,
 // bt_match_cache_*, bt_tracks_dev_forget_frame, bt_select_keyframes, bt_ba_gate, bt_frame_cache_store, bt_solve_windows and bt_keyframe_check
 // in the reference's order.  Its own state is the frame deque, the keyframe list and which slot of its reserved buffers each frame holds.
 // Synchronisations per frame: the ROI read-back in begin_frame; in end_frame the initial pose (with the neighbour pair's count and status),
@@ -239,10 +239,11 @@ extern "C" void bt_tracker_destroy(bt_tracker* t) {
 	bt_ctx_destroy(ctx);
 }
 
-extern "C" int bt_tracker_begin_frame(bt_tracker* t, int loader_id, const float* first_pose, const float* depth_raw_dev, const uint8_t* mask_dev,
-                                      const uint8_t* colour_dev, uint8_t* request_out_dev, int32_t* roi_out, int* status_out, void* stream_) {
-	BT_REQUIRE(t && depth_raw_dev && mask_dev && colour_dev && request_out_dev && status_out, BT_ERR_INVALID_ARG, "bt_tracker_begin_frame: NULL argument");
-	BT_REQUIRE(!t->pending, BT_ERR_INVALID_ARG, "bt_tracker_begin_frame: frame %d is pending: finish it with end_frame or drop_frame first", t->pend.id);
+// both begin_frame entry points: depth_raw_dev is float metres, or uint16 millimetres when u16
+static int tr_begin(bt_tracker* t, const char* who, int loader_id, const float* first_pose, const void* depth_raw_dev, bool u16, const uint8_t* mask_dev,
+                    const uint8_t* colour_dev, uint8_t* request_out_dev, int32_t* roi_out, int* id_out, float* pose_out, int* status_out, void* stream_) {
+	BT_REQUIRE(t && depth_raw_dev && mask_dev && colour_dev && request_out_dev && status_out, BT_ERR_INVALID_ARG, "%s: NULL argument", who);
+	BT_REQUIRE(!t->pending, BT_ERR_INVALID_ARG, "%s: frame %d is pending: finish it with end_frame or drop_frame first", who, t->pend.id);
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(t->ctx->device));
 	const bt_tracker_params& p = t->p;
@@ -255,14 +256,23 @@ extern "C" int bt_tracker_begin_frame(bt_tracker* t, int loader_id, const float*
 		f.id = loader_id;
 		for (int i = 0; i < 16; i++) f.pose[i] = first_pose ? first_pose[i] : ((i % 5 == 0) ? 1.f : 0.f);
 	}
+	if (id_out) *id_out = f.id;
+	if (pose_out) memcpy(pose_out, f.pose, sizeof f.pose);
 	f.slot = t->free_slots.back();                         // (one slot more than frames alive: never empty here)
-	const float* din[1] = { depth_raw_dev };
 	const uint8_t* msk[1] = { mask_dev };
 	float* dout[1] = { tr_depth(t, f.slot) };
 	float* nout[1] = { tr_normal(t, f.slot) };
 	uint8_t* fg[1] = { tr_fg(t, f.slot) };
-	int rc = bt_frames_preprocess_masked(t->ctx, 1, din, msk, p.mask_mode, p.H, p.W, p.fx, p.fy, p.cx, p.cy, &p.depth, dout, nullptr, nout, fg,
-	                                     t->roi.as<int32_t>(), stream);
+	int rc;
+	if (u16) {
+		const uint16_t* din[1] = { static_cast<const uint16_t*>(depth_raw_dev) };
+		rc = bt_frames_preprocess_masked_u16(t->ctx, 1, din, msk, p.mask_mode, p.H, p.W, p.fx, p.fy, p.cx, p.cy, &p.depth, dout, nullptr, nout, fg,
+		                                     t->roi.as<int32_t>(), stream);
+	} else {
+		const float* din[1] = { static_cast<const float*>(depth_raw_dev) };
+		rc = bt_frames_preprocess_masked(t->ctx, 1, din, msk, p.mask_mode, p.H, p.W, p.fx, p.fy, p.cx, p.cy, &p.depth, dout, nullptr, nout, fg,
+		                                 t->roi.as<int32_t>(), stream);
+	}
 	if (rc != BT_OK) return rc;
 	int32_t* roi = t->h_meta.as<int32_t>();
 	if ((rc = tr_read(roi, t->roi.p, 4 * sizeof(int32_t), stream)) != BT_OK) return rc;
@@ -280,6 +290,19 @@ extern "C" int bt_tracker_begin_frame(bt_tracker* t, int loader_id, const float*
 	t->pending = true;
 	*status_out = BT_FRAME_OTHER;
 	return BT_OK;
+}
+
+extern "C" int bt_tracker_begin_frame(bt_tracker* t, int loader_id, const float* first_pose, const float* depth_raw_dev, const uint8_t* mask_dev,
+                                      const uint8_t* colour_dev, uint8_t* request_out_dev, int32_t* roi_out, int* status_out, void* stream) {
+	return tr_begin(t, "bt_tracker_begin_frame", loader_id, first_pose, depth_raw_dev, false, mask_dev, colour_dev, request_out_dev, roi_out, nullptr, nullptr,
+	                status_out, stream);
+}
+
+extern "C" int bt_tracker_begin_frame_u16(bt_tracker* t, int loader_id, const float* first_pose, const uint16_t* depth_mm_dev, const uint8_t* mask_dev,
+                                          const uint8_t* colour_dev, uint8_t* request_out_dev, int32_t* roi_out, int* id_out, float* pose_out, int* status_out,
+                                          void* stream) {
+	return tr_begin(t, "bt_tracker_begin_frame_u16", loader_id, first_pose, depth_mm_dev, true, mask_dev, colour_dev, request_out_dev, roi_out, id_out, pose_out,
+	                status_out, stream);
 }
 
 extern "C" int bt_tracker_drop_frame(bt_tracker* t, float* pose_out) {

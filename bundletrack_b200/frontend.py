@@ -58,7 +58,9 @@ class FrameFrontEnd:
 
     def process_masked(self, depth_raw: Sequence, mask: Sequence, H: int, W: int, K, depth_out: Sequence, normal_out: Sequence,
                        fg_out: Sequence, xyz_out: Sequence = None, mode: int = None, roi_out=None, fetch_roi: bool = True):
-        """`process` plus the object mask (Frame::segmentationByMaskFile + invalidatePixelsByMask): mask/fg_out are per-frame device
+        """`process` plus the object mask (Frame::segmentationByMaskFile + invalidatePixelsByMask): depth_raw is per-frame device float32
+        metres, or uint16 millimetres as the depth PNG holds them (bt_frames_preprocess_masked_u16 converts them as Utils::readDepthImage does;
+        every frame of a call has the same dtype); mask/fg_out are per-frame device
         uint8 [H,W] (fg_out = Frame::_fg_mask, not the mask's own buffer); the maps are zeroed where fg == 0.  mode: _lib.BT_MASK_*
         (default: config.mask_mode of this object's yml).  roi_out: device int32 [n,4] (default: a buffer this object keeps, which
         `lfnet_request` reads by default).  Returns the ROI (umin, umax, vmin, vmax) per frame as numpy int32 [n,4], read back with
@@ -68,12 +70,17 @@ class FrameFrontEnd:
         fx, fy, cx, cy = (Kn[0, 0], Kn[1, 1], Kn[0, 2], Kn[1, 2]) if Kn.ndim == 2 else Kn
         n = len(depth_raw)
         arr = lambda seq: (ctypes.c_void_p * n)(*[_ptr(t) for t in seq])
+        dtypes = {str(getattr(t, "dtype", "float32")).replace("torch.", "") for t in depth_raw}
+        if len(dtypes) != 1 or not dtypes <= {"float32", "uint16"}:
+            raise _lib.BtError(f"process_masked: depth frames must all be float32 or all uint16, got {sorted(dtypes)}")
+        u16 = dtypes == {"uint16"}
+        fn = self.lib.bt_frames_preprocess_masked_u16 if u16 else self.lib.bt_frames_preprocess_masked
         roi = _ptr(roi_out) if roi_out is not None else self._roi_buffer(n)
         self._last_roi = roi
-        _lib.check(self.lib.bt_frames_preprocess_masked(
+        _lib.check(fn(
             self.ctx, ctypes.c_int(n), arr(depth_raw), arr(mask), ctypes.c_int(self.mask_mode if mode is None else mode), ctypes.c_int(H), ctypes.c_int(W),
             ctypes.c_float(fx), ctypes.c_float(fy), ctypes.c_float(cx), ctypes.c_float(cy), ctypes.byref(self.params), arr(depth_out),
-            arr(xyz_out) if xyz_out is not None else None, arr(normal_out), arr(fg_out), ctypes.c_void_p(roi), self.stream), "bt_frames_preprocess_masked")
+            arr(xyz_out) if xyz_out is not None else None, arr(normal_out), arr(fg_out), ctypes.c_void_p(roi), self.stream), "bt_frames_preprocess_masked" + ("_u16" if u16 else ""))
         if not fetch_roi:
             return None
         out = np.empty((n, 4), np.int32)

@@ -290,6 +290,23 @@ inline void processDepthNormalsAndMask(bt_ctx* ctx, const float* depth_raw_gpu, 
 	if (bt_memcpy_d2h(r, roi_gpu, sizeof r, stream) != BT_OK) throw std::runtime_error(std::string("bt_memcpy_d2h: ") + bt_last_error());
 	for (int i = 0; i < 4; i++) roi(i) = r[i];
 }
+// The same on the depth PNG's samples (device uint16 H*W millimetres, cv::imread(path, IMREAD_ANYDEPTH)): Utils::readDepthImage's
+// conversion runs in the front-end kernel (bt_frames_preprocess_masked_u16).
+template <class Float4T, class Mat3, class Vec4>
+inline void processDepthNormalsAndMask(bt_ctx* ctx, const uint16_t* depth_mm_gpu, const uint8_t* mask_gpu, int mode, float* depth_gpu, Float4T* normal_gpu,
+                                       Float4T* xyz_gpu, uint8_t* fg_gpu, int32_t* roi_gpu, int H, int W, const Mat3& K, const BtDepthConfig& cfg, Vec4& roi,
+                                       void* stream = nullptr) {
+	const bt_depth_params prm = cfg.to_params();
+	const uint16_t* in[1] = { depth_mm_gpu }; float* out[1] = { depth_gpu };
+	float* nrm[1] = { reinterpret_cast<float*>(normal_gpu) }; float* xyz[1] = { reinterpret_cast<float*>(xyz_gpu) };
+	const uint8_t* msk[1] = { mask_gpu }; uint8_t* fg[1] = { fg_gpu };
+	if (bt_frames_preprocess_masked_u16(ctx, 1, in, msk, mode, H, W, K(0, 0), K(1, 1), K(0, 2), K(1, 2), &prm, out, xyz_gpu ? xyz : nullptr, nrm, fg, roi_gpu,
+	                                    stream) != BT_OK)
+		throw std::runtime_error(std::string("bt_frames_preprocess_masked_u16: ") + bt_last_error());
+	int32_t r[4];
+	if (bt_memcpy_d2h(r, roi_gpu, sizeof r, stream) != BT_OK) throw std::runtime_error(std::string("bt_memcpy_d2h: ") + bt_last_error());
+	for (int i = 0; i < 4; i++) roi(i) = r[i];
+}
 // Lfnet::detectFeature's request image (FeatureManager.cpp:813-858, rot_deg = 0) from processDepthNormalsAndMask's fg / roi:
 // request_gpu (device uint8 400*400*3) receives the BGR bytes of the second message part; untouched when the ROI fails the gate.
 inline void lfnetRequest(bt_ctx* ctx, const uint8_t* color_gpu, const uint8_t* fg_gpu, const int32_t* roi_gpu, int H, int W, uint8_t* request_gpu,
@@ -369,6 +386,19 @@ public:
 		if (first_pose) to_flat(*first_pose, fp);
 		int st = -1;
 		check(bt_tracker_begin_frame(t_, loader_id, first_pose ? fp : nullptr, depth_raw_gpu, mask_gpu, color_gpu, request_gpu, roi, &st, stream), "bt_tracker_begin_frame");
+		return st;
+	}
+	// beginFrame on the depth PNG's uint16 millimetres; also returns the new frame's id and initial pose, for every status (a frame that fails
+	// the ROI gate is recorded with that pose)
+	template <class Mat4>
+	int beginFrame(int loader_id, const Mat4* first_pose, const uint16_t* depth_mm_gpu, const uint8_t* mask_gpu, const uint8_t* color_gpu, uint8_t* request_gpu,
+	               int& frame_id, Mat4& pose, int32_t* roi = nullptr, void* stream = nullptr) {
+		float fp[16], po[16];
+		if (first_pose) to_flat(*first_pose, fp);
+		int st = -1;
+		check(bt_tracker_begin_frame_u16(t_, loader_id, first_pose ? fp : nullptr, depth_mm_gpu, mask_gpu, color_gpu, request_gpu, roi, &frame_id, po, &st, stream),
+		      "bt_tracker_begin_frame_u16");
+		from_flat(po, pose);
 		return st;
 	}
 	// kpts: n x (x, y) image pixels; desc_gpu: n x 256 device floats, desc_step bytes per row (GpuMat::step; 0 = packed)

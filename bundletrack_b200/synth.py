@@ -435,3 +435,26 @@ def make_sequence(seed: int, n_frames: int, H: int = 480, W: int = 640, K=None, 
         if k in detect_fail:
             feats[k] = None
     return Sequence(raw, mask, colour, feats, poses_gt, K, tuple(roi_fail), tuple(neighbour_fail), tuple(detect_fail), radii, ob_in_cam[0].copy())
+
+
+def write_png(path: str, img: np.ndarray) -> None:
+    """A PNG of img with the standard library's zlib: uint8 [H,W] (grey), uint8 [H,W,3] BGR (stored as RGB, as cv2.imwrite does) or uint16
+    [H,W] (16-bit grey, big-endian samples).  Filter type 0 on every row; no ancillary chunks."""
+    import struct
+    import zlib
+    a = np.asarray(img)
+    if a.dtype == np.uint8 and a.ndim == 2:
+        depth, ctype, rows = 8, 0, a
+    elif a.dtype == np.uint8 and a.ndim == 3 and a.shape[2] == 3:
+        depth, ctype, rows = 8, 2, a[..., ::-1].reshape(a.shape[0], -1)
+    elif a.dtype == np.uint16 and a.ndim == 2:
+        depth, ctype, rows = 16, 0, a.astype(">u2").view(np.uint8).reshape(a.shape[0], -1)
+    else:
+        raise ValueError(f"write_png: unsupported array {a.dtype} {a.shape}")
+    raw = np.concatenate([np.zeros((rows.shape[0], 1), np.uint8), np.ascontiguousarray(rows)], 1).tobytes()
+
+    def chunk(tag: bytes, data: bytes) -> bytes:
+        return struct.pack(">I", len(data)) + tag + data + struct.pack(">I", zlib.crc32(tag + data) & 0xFFFFFFFF)
+    with open(path, "wb") as f:
+        f.write(b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", a.shape[1], a.shape[0], depth, ctype, 0, 0, 0))
+                + chunk(b"IDAT", zlib.compress(raw, 1)) + chunk(b"IEND", b""))

@@ -73,6 +73,20 @@ class Tracker:
                    "bt_tracker_begin_frame")
         return st.value, roi
 
+    def begin_frame_mm(self, depth_mm, mask, colour, request_out, loader_id: int = 0, first_pose=None):
+        """`begin_frame` on the depth PNG's samples: depth_mm is device uint16 [H,W] millimetres (the library converts them as
+        Utils::readDepthImage does).  Returns (status, roi, frame_id, pose [4,4] float32 cam->model): the new frame's id and initial pose,
+        for every status (a frame that fails the ROI gate is recorded with this pose)."""
+        roi = np.zeros(4, np.int32)
+        st, fid = ctypes.c_int(-1), ctypes.c_int(-1)
+        pose = np.zeros((4, 4), np.float32)
+        fp = None if first_pose is None else np.ascontiguousarray(first_pose, np.float32).reshape(16)
+        _lib.check(self.lib.bt_tracker_begin_frame_u16(self.t, ctypes.c_int(loader_id), None if fp is None else fp.ctypes.data_as(ctypes.c_void_p),
+                                                       ctypes.c_void_p(_ptr(depth_mm)), ctypes.c_void_p(_ptr(mask)), ctypes.c_void_p(_ptr(colour)),
+                                                       ctypes.c_void_p(_ptr(request_out)), roi.ctypes.data_as(ctypes.c_void_p), ctypes.byref(fid),
+                                                       pose.ctypes.data_as(ctypes.c_void_p), ctypes.byref(st), self.stream), "bt_tracker_begin_frame_u16")
+        return st.value, roi, fid.value, pose
+
     def end_frame(self, kpts, desc):
         """kpts: numpy [n,2] float32 image pixels; desc: device float32 [n,256].  Returns (pose [4,4] float32 cam->model, status)."""
         k = np.ascontiguousarray(kpts, np.float32).reshape(-1, 2)

@@ -356,6 +356,13 @@ enum { BT_MASK_AS_IS = 0, BT_MASK_LARGEST_HULL = 1 };
 BT_API int bt_frames_preprocess_masked(bt_ctx* ctx, int n_frames, const float* const* depth_raw_dev, const uint8_t* const* mask_dev, int mask_mode,
                          int H, int W, float fx, float fy, float cx, float cy, const bt_depth_params* prm, float* const* depth_out_dev,
                          float* const* xyz_out_dev, float* const* normal_out_dev, uint8_t* const* fg_out_dev, int32_t* roi_out_dev, void* stream);
+/* bt_frames_preprocess_masked on the depth PNG's samples: depth_mm_dev is DEVICE uint16 H*W per frame as cv::imread(path, IMREAD_ANYDEPTH)
+ * returns a 16-bit depth PNG (millimetres).  The kernel converts each sample as Utils::readDepthImage does (Utils.cpp:57-66):
+ * d = (float)((double)s * 0.001), 0 where (double)d < 0.1.  Every output is bit for bit what bt_frames_preprocess_masked gives on that float
+ * image; the upload is half the bytes and the host does no per-pixel work. */
+BT_API int bt_frames_preprocess_masked_u16(bt_ctx* ctx, int n_frames, const uint16_t* const* depth_mm_dev, const uint8_t* const* mask_dev, int mask_mode,
+                         int H, int W, float fx, float fy, float cx, float cy, const bt_depth_params* prm, float* const* depth_out_dev,
+                         float* const* xyz_out_dev, float* const* normal_out_dev, uint8_t* const* fg_out_dev, int32_t* roi_out_dev, void* stream);
 /* Lfnet::detectFeature's request image (src/FeatureManager.cpp:813-873, rot_deg = 0): the colour zeroed where fg == 0, cropped to
  * [vmin, vmax) x [umin, umax) of roi_dev (the reference's crop drops the last row and column), padded with zeros to a square and
  * resized to 400 x 400 as cv::resize(INTER_LINEAR) does on 8-bit images.  colour_dev: DEVICE uint8 H*W*3 BGR (cv::Mat CV_8UC3 data);
@@ -510,6 +517,12 @@ BT_API void bt_tracker_destroy(bt_tracker* t);
  * request image and *status_out = BT_FRAME_OTHER; finish the frame with end_frame or drop_frame. */
 BT_API int bt_tracker_begin_frame(bt_tracker* t, int loader_id, const float* first_pose, const float* depth_raw_dev, const uint8_t* mask_dev,
                                   const uint8_t* colour_dev, uint8_t* request_out_dev, int32_t* roi_out, int* status_out, void* stream);
+/* bt_tracker_begin_frame on the depth PNG's uint16 millimetres (DEVICE H*W; converted as bt_frames_preprocess_masked_u16 does).  Also writes
+ * the new frame's id to id_out and its initial pose (cam->model, 16 floats) to pose_out, for every status (both host, optional).  A frame
+ * that fails the ROI gate still has that pose: Bundler::saveNewframeResult records it (Bundler.cpp:362-377). */
+BT_API int bt_tracker_begin_frame_u16(bt_tracker* t, int loader_id, const float* first_pose, const uint16_t* depth_mm_dev, const uint8_t* mask_dev,
+                                      const uint8_t* colour_dev, uint8_t* request_out_dev, int32_t* roi_out, int* id_out, float* pose_out, int* status_out,
+                                      void* stream);
 /* kpts_host: n_kpts x (x, y) image pixels (bt_lfnet_parse_reply's output); desc: the n_kpts x 256 descriptors on the device.  Writes the frame's
  * pose as Bundler::saveNewframeResult would record it and its status.  BT_ERR_INVALID_ARG without a pending begin_frame, for n_kpts > max_feats
  * or a NULL argument.  BT_ERR_CAPACITY when max_keyframes = 0 and the frames alive plus the new one exceed max_frames_alive, or when

@@ -1,0 +1,42 @@
+#!/usr/bin/env python3
+"""Tracks one model in one NOCS-REAL275 scene, as the reference's scripts/run_nocs.py + bundle_track_nocs do, and writes one pose file per
+frame to <out_dir>/<model>_<scene>/poses/<id>.txt, the layout scripts/eval_nocs.py reads.  Features come from a running LF-Net server
+(lf-net-release/run_server.py) at tcp://127.0.0.1:<port>.  Frames follow the 6-PACK data list (bundletrack_b200.sequence.NocsScene); the
+masks are <mask_dir>/<id>.png.  Nothing under out_dir is removed.
+
+    python scripts/run_nocs.py --nocs_dir NOCS --scene_id 1 --model_name can_arizona_tea_norm --mask_dir masks/scene_1_model_can_arizona_tea_norm \\
+        --out_dir results --port 5555
+    python scripts/eval_nocs.py --nocs_dir NOCS --results_dir results
+"""
+from __future__ import annotations
+
+import argparse
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def main():
+    from bundletrack_b200.sequence import LfnetClient, NocsScene, run_sequence, summary
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--nocs_dir", required=True)
+    ap.add_argument("--scene_id", type=int, default=1)
+    ap.add_argument("--model_name", default="can_arizona_tea_norm")
+    ap.add_argument("--port", type=int, default=5555, help="the LF-Net server's port")
+    ap.add_argument("--mask_dir", required=True, help="the scene's and model's masks, <id>.png")
+    ap.add_argument("--out_dir", required=True)
+    ap.add_argument("--config", default=None, help="a config_nocs.yml (default: its values, bundletrack_b200.config.NOCS_DEFAULTS)")
+    ap.add_argument("--device", type=int, default=0)
+    a = ap.parse_args()
+    loader = NocsScene(a.nocs_dir, a.scene_id, a.model_name, a.mask_dir)
+    client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
+    try:
+        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, f"{a.model_name}_{a.scene_id}"), device=a.device)
+    finally:
+        client.close()
+    print(summary(res))
+
+
+if __name__ == "__main__":
+    main()

@@ -1,0 +1,42 @@
+#!/usr/bin/env python3
+"""Tracks one YCBInEOAT video, as the reference's scripts/run_ycbineoat.py + bundle_track_ycbineoat do, and writes one pose file per frame to
+<out_dir>/<video>/poses/<id>.txt, the layout scripts/eval_poses.py reads.  Features come from a running LF-Net server
+(lf-net-release/run_server.py) at tcp://127.0.0.1:<port>.  The video directory holds rgb/, depth/, masks/, annotated_poses/ and cam_K.txt
+(bundletrack_b200.sequence.YcbineoatVideo).  Nothing under out_dir is removed.
+
+    python scripts/run_ycbineoat.py --data_dir YCBInEOAT/bleach0 --config config_ycbineoat.yml --out_dir results --port 5555
+    python scripts/eval_poses.py --dataset_dir YCBInEOAT --model_dir YCB_Video_Dataset/models --results_dir results
+"""
+from __future__ import annotations
+
+import argparse
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def main():
+    from bundletrack_b200.sequence import LfnetClient, YcbineoatVideo, run_sequence, summary
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--data_dir", required=True, help="one video's directory")
+    ap.add_argument("--port", type=int, default=5555, help="the LF-Net server's port")
+    ap.add_argument("--out_dir", required=True)
+    ap.add_argument("--config", default=None, help="the reference's config_ycbineoat.yml (default: the config_nocs.yml values, "
+                                                    "bundletrack_b200.config.NOCS_DEFAULTS)")
+    ap.add_argument("--device", type=int, default=0)
+    a = ap.parse_args()
+    if not os.path.isdir(a.data_dir):
+        raise SystemExit(f"--data_dir {a.data_dir} is not a directory")
+    loader = YcbineoatVideo(a.data_dir)
+    video = os.path.basename(os.path.normpath(a.data_dir))
+    client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
+    try:
+        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, video), device=a.device)
+    finally:
+        client.close()
+    print(summary(res))
+
+
+if __name__ == "__main__":
+    main()
