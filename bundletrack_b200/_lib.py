@@ -158,8 +158,9 @@ EXPORTS = [
     "bt_rotation_geodesic", "bt_keyframe_check", "bt_select_keyframes", "bt_rigid_transform", "bt_lfnet_parse_reply", "bt_ba_gate", "bt_pose_format", "bt_pose_write_txt",
     "bt_tracks_create", "bt_tracks_destroy", "bt_tracks_update_pair", "bt_tracks_propagate", "bt_tracks_forget_frame", "bt_tracks_stats",
     "bt_tracks_dev_reserve", "bt_tracks_dev_reserve_ex", "bt_tracks_dev_update_pair", "bt_tracks_dev_propagate", "bt_tracks_dev_forget_frame", "bt_tracks_dev_stats", "bt_find_corres_pairs",
-    "bt_pose_init", "bt_tracker_create", "bt_tracker_destroy", "bt_tracker_begin_frame", "bt_tracker_begin_frame_u16", "bt_tracker_end_frame", "bt_tracker_drop_frame", "bt_tracker_state", "bt_tracker_usage",
+    "bt_pose_init", "bt_tracker_create", "bt_tracker_destroy", "bt_tracker_begin_frame", "bt_tracker_begin_frame_u16", "bt_tracker_end_frame", "bt_tracker_drop_frame", "bt_tracker_state", "bt_tracker_usage", "bt_tracker_last_fg",
     "bt_metrics_reserve", "bt_pose_metrics", "bt_vocap", "bt_nocs_reserve", "bt_nocs_metrics", "bt_nocs_score",
+    "bt_overlay_reserve", "bt_voxel_downsample", "bt_pose_overlay",
     "bt_dev_alloc", "bt_dev_free", "bt_memcpy_h2d", "bt_memcpy_d2h", "bt_host_alloc_pinned", "bt_host_free_pinned",
     "bt_stream_sync", "bt_debug_live_resources",
 ]

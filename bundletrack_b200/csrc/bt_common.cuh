@@ -138,6 +138,7 @@ struct MatchCache;    // prune.cu
 struct TracksDev;     // tracks_dev.cu
 struct MetricsState;  // metrics.cu
 struct NocsState;     // metrics.cu
+struct OverlayState;  // overlay.cu
 
 // The context owns the module states; each module defines the deleter of its state next to it, so the states stay private to their files.
 struct StateDeleter {
@@ -150,6 +151,7 @@ struct StateDeleter {
 	void operator()(TracksDev*) const;
 	void operator()(MetricsState*) const;
 	void operator()(NocsState*) const;
+	void operator()(OverlayState*) const;
 };
 template <class T> using StatePtr = std::unique_ptr<T, StateDeleter>;
 
@@ -168,9 +170,12 @@ struct bt_ctx {
 	bt::StatePtr<bt::TracksDev> tracks;
 	bt::StatePtr<bt::MetricsState> metrics;
 	bt::StatePtr<bt::NocsState> nocs;
+	bt::StatePtr<bt::OverlayState> overlay;
 };
 
 namespace bt {
+// policy.cu: the float cofactor inverse of a row-major 4 x 4 (Eigen's Matrix4f::inverse()); false when it is singular
+bool inverse4(const float* m, float* inv);
 // segment.cu: largest-hull mode for the masked front end, and the LF-Net request
 size_t hull_fill_smem(int H);
 int segment_largest_hull(const uint8_t* const* mask_tbl_dev, int n, int H, int W, int32_t* label, int32_t* count, unsigned long long* best,

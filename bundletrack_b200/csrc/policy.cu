@@ -98,8 +98,9 @@ extern "C" int bt_ba_gate(int n_edges_newframe, int min_fm_edges_newframe) {
 	return n_edges_newframe > min_fm_edges_newframe ? 1 : 0;      // `if (n_edges_newframe<=min_fm_edges_newframe) { NO_BA; return; }`, Bundler.cpp:343
 }
 
-// inverse of a 4x4 in float, by cofactors (what Eigen's Matrix4f::inverse() evaluates); row-major in and out
-static bool inverse4(const float* m, float* inv) {
+// inverse of a 4x4 in float, by cofactors (what Eigen's Matrix4f::inverse() evaluates); row-major in and out.  bt_pose_format and
+// bt_pose_overlay (overlay.cu) share it, so the overlay draws with the ob_in_cam the pose file holds.
+bool bt::inverse4(const float* m, float* inv) {
 	float t[16];
 	t[0] = m[5] * m[10] * m[15] - m[5] * m[11] * m[14] - m[9] * m[6] * m[15] + m[9] * m[7] * m[14] + m[13] * m[6] * m[11] - m[13] * m[7] * m[10];
 	t[4] = -m[4] * m[10] * m[15] + m[4] * m[11] * m[14] + m[8] * m[6] * m[15] - m[8] * m[7] * m[14] - m[12] * m[6] * m[11] + m[12] * m[7] * m[10];
@@ -127,7 +128,7 @@ static bool inverse4(const float* m, float* inv) {
 extern "C" int bt_pose_format(const float* cur_in_model, char* text, int cap) {
 	BT_REQUIRE(cur_in_model && text && cap > 0, BT_ERR_INVALID_ARG, "bt_pose_format: NULL argument");
 	float ob[16];
-	BT_REQUIRE(inverse4(cur_in_model, ob), BT_ERR_INVALID_ARG, "bt_pose_format: the pose is singular");
+	BT_REQUIRE(bt::inverse4(cur_in_model, ob), BT_ERR_INVALID_ARG, "bt_pose_format: the pose is singular");
 	// Eigen's default IOFormat with the stream's precision: every coefficient printed like `os << std::setprecision(10) << float`
 	// (= %.10g), padded on the left to the widest one, coefficients separated by one blank, rows by a newline, `endl` after the matrix
 	char cell[16][40];

@@ -108,6 +108,7 @@ struct bt_tracker {
 	std::vector<int> keyframes;            // Bundler::_keyframes (ids, admission order = id order)
 	bool pending = false;
 	TFrame pend;
+	int last_fg_slot = -1;                 // the slot whose fg map the last begin_frame wrote (bt_tracker_last_fg)
 };
 
 static int tr_forget(bt_tracker* t, int id, cudaStream_t stream) {
@@ -274,6 +275,7 @@ static int tr_begin(bt_tracker* t, const char* who, int loader_id, const float* 
 		                                 t->roi.as<int32_t>(), stream);
 	}
 	if (rc != BT_OK) return rc;
+	t->last_fg_slot = f.slot;
 	int32_t* roi = t->h_meta.as<int32_t>();
 	if ((rc = tr_read(roi, t->roi.p, 4 * sizeof(int32_t), stream)) != BT_OK) return rc;
 	if (roi_out) memcpy(roi_out, roi, 4 * sizeof(int32_t));
@@ -468,6 +470,15 @@ extern "C" int bt_tracker_state(bt_tracker* t, int32_t* ids, float* poses, int32
 		if (is_keyframe) is_keyframe[k] = kv.second.keyframe ? 1 : 0;
 		k++;
 	}
+	return BT_OK;
+}
+
+// Frame::_fg_mask of the frame the last begin_frame segmented.  Its slot is taken again only by a later begin_frame: a frame that failed the
+// ROI gate never took it, a dropped or failed frame gave it back, a tracked frame keeps it until a later step forgets the frame.
+extern "C" int bt_tracker_last_fg(bt_tracker* t, const uint8_t** fg_dev) {
+	BT_REQUIRE(t && fg_dev, BT_ERR_INVALID_ARG, "bt_tracker_last_fg: NULL argument");
+	BT_REQUIRE(t->last_fg_slot >= 0, BT_ERR_INVALID_ARG, "bt_tracker_last_fg: no frame has been segmented yet");
+	*fg_dev = tr_fg(t, t->last_fg_slot);
 	return BT_OK;
 }
 

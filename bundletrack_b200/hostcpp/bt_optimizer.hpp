@@ -152,6 +152,29 @@ inline void saveNewframePose(const std::string& path, const Mat4& cur_in_model) 
 	if (bt_pose_write_txt(path.c_str(), flat) != BT_OK) throw std::runtime_error(std::string("bt_pose_write_txt: ") + bt_last_error());
 }
 
+// Utils::downsamplePointCloud (Utils.cpp:134-140) for many device clouds in one asynchronous call: PCL's VoxelGrid at `leaf`, points of a
+// voxel summed in input order (bt_voxel_downsample).  clouds_gpu[c]: float n_pts[c] x 3; out_gpu[c]: room for as many; n_out_gpu: device int32
+// [clouds], the counts.  The context needs bt_overlay_reserve.
+inline void downsamplePointClouds(bt_ctx* ctx, const std::vector<const float*>& clouds_gpu, const std::vector<int>& n_pts, float leaf,
+                                  const std::vector<float*>& out_gpu, int32_t* n_out_gpu, void* stream = nullptr) {
+	if (bt_voxel_downsample(ctx, (int)clouds_gpu.size(), clouds_gpu.data(), n_pts.data(), leaf, out_gpu.data(), n_out_gpu, stream) != BT_OK)
+		throw std::runtime_error(std::string("bt_voxel_downsample: ") + bt_last_error());
+}
+
+// Utils::drawProjectPoints (Utils.cpp:216-226) with Bundler::saveNewframeResult's dimming (Bundler.cpp:379-399), for one frame: viz_gpu
+// (uint8 H x W x 3) receives the colour dimmed where fg == 0 with the model (device float n_model x 3, the loader's 1.5 cm cloud) stamped
+// under ob_in_cam = cur_in_model^-1; raw_gpu (optional) the colour zeroed where fg == 0.  The label (cv::putText) is the caller's.
+template <class Mat4, class Mat3>
+inline void drawProjectPoints(bt_ctx* ctx, const float* model_gpu, int n_model, const Mat4& cur_in_model, const Mat3& K, const uint8_t* color_gpu,
+                              const uint8_t* fg_gpu, int H, int W, uint8_t* viz_gpu, uint8_t* raw_gpu = nullptr, void* stream = nullptr) {
+	float P[16];
+	for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) P[4 * r + c] = cur_in_model(r, c);
+	uint8_t* raw[1] = { raw_gpu };
+	if (bt_pose_overlay(ctx, 1, model_gpu, n_model, P, K(0, 0), K(1, 1), K(0, 2), K(1, 2), &color_gpu, &fg_gpu, H, W, &viz_gpu, raw_gpu ? raw : nullptr,
+	                    stream) != BT_OK)
+		throw std::runtime_error(std::string("bt_pose_overlay: ") + bt_last_error());
+}
+
 // scripts/Utils.py add / adi for a whole sequence in one device call: ADD and ADD-S per frame (metres) into add_gpu / adds_gpu (device double
 // [n_frames]), asynchronous on `stream`.  model_pts_gpu: device double n_pts x 3 (points.xyz); pred / gt: ob_in_cam per frame as the
 // reference's poses/<id>.txt hold them.  The context needs bt_metrics_reserve(ctx, >= n_pts, >= pred.size()).

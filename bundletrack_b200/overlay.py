@@ -1,0 +1,178 @@
+"""Tracking overlays: the reference's LOG frames (Bundler::saveNewframeResult with `LOG: 1`, src/Bundler.cpp:379-411) drawn on the device.  A
+thin ctypes mirror of bt_overlay_reserve / bt_voxel_downsample / bt_pose_overlay (include/bundletrack_b200.h):
+
+- load_obj_points: the model's points as pcl::io::loadOBJFile reads them (the `v` lines, in file order);
+- Overlay: the model voxel-gridded once at 1.5 cm (DataLoader.cpp:92, 316), then per frame the model under the tracked pose, voxel-gridded at
+  1 cm, projected and stamped onto the frame's colour dimmed outside the object mask (Utils::drawProjectPoints, Utils.cpp:216-226), plus the
+  masked colour_raw image;
+- write_log_frame: the frame id label (cv::putText) and the three files the reference writes, through OpenCV as the reference does."""
+from __future__ import annotations
+
+import ctypes
+import os
+
+import numpy as np
+
+from . import _lib
+
+MODEL_LEAF = 0.015          # DataLoader.cpp:92, 316
+TILE = 2048                 # points per tile of the device grid (overlay.cu kTile): clouds of TILE +- 1 points cross a tile boundary
+
+
+def load_obj_points(path: str) -> np.ndarray:
+    """float32 [n,3]: x, y, z of every `v` line of the OBJ file in file order.  Values after the third on a `v` line (vertex colours) are
+    ignored; `vn`, `vt`, `f`, comments and every other line add no points."""
+    pts = []
+    with open(path) as f:
+        for k, line in enumerate(f, 1):
+            t = line.split()
+            if not t or t[0] != "v":
+                continue
+            if len(t) < 4:
+                raise ValueError(f"{path}:{k}: a vertex line needs x, y and z")
+            pts.append((float(t[1]), float(t[2]), float(t[3])))
+    if not pts:
+        raise ValueError(f"{path}: no vertex")
+    return np.asarray(pts, np.float64).astype(np.float32)
+
+
+def _ptrs(xs) -> "ctypes.Array":
+    a = (ctypes.c_void_p * len(xs))()
+    for i, x in enumerate(xs):
+        a[i] = int(x.data_ptr()) if hasattr(x, "data_ptr") else int(x)
+    return a
+
+
+class VoxelGrid:
+    """bt_voxel_downsample: PCL's VoxelGrid of many float32 [n,3] device clouds in one asynchronous call.  Scratch for max_frames clouds of
+    max_pts points is reserved here (or on `ctx`, shared with an Overlay)."""
+
+    def __init__(self, max_pts: int, max_frames: int = 1, device: int = 0, stream: int = 0, ctx=None):
+        self.lib = _lib.load()
+        self.device, self.stream = device, ctypes.c_void_p(stream)
+        self._own = ctx is None
+        self.ctx = ctypes.c_void_p() if ctx is None else ctx
+        if self._own:
+            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
+        self.reserve(max_pts, max_frames)
+
+    def reserve(self, max_pts: int, max_frames: int) -> None:
+        _lib.check(self.lib.bt_overlay_reserve(self.ctx, ctypes.c_int(max_pts), ctypes.c_int(max_frames)), "bt_overlay_reserve")
+
+    def close(self):
+        if self._own and self.ctx:
+            self.lib.bt_ctx_destroy(self.ctx)
+            self.ctx = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def enqueue(self, clouds, leaf: float, outs, n_out) -> None:
+        """clouds / outs: float32 [n_c,3] CUDA tensors (outs with room for n_c rows); n_out: int32 CUDA tensor [len(clouds)].  Asynchronous."""
+        n = (ctypes.c_int * len(clouds))(*[int(c.shape[0]) for c in clouds])
+        _lib.check(self.lib.bt_voxel_downsample(self.ctx, ctypes.c_int(len(clouds)), _ptrs(clouds), n, ctypes.c_float(leaf), _ptrs(outs),
+                                                ctypes.c_void_p(n_out.data_ptr()), self.stream), "bt_voxel_downsample")
+
+    def __call__(self, clouds, leaf: float):
+        """Each cloud (numpy or CUDA, [n,3]) voxel-gridded at leaf: a list of float32 numpy [m,3]; synchronises the stream."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        cl = [(c if isinstance(c, torch.Tensor) else torch.from_numpy(np.asarray(c, np.float32))).to(device=dev, dtype=torch.float32).reshape(-1, 3).contiguous()
+              for c in clouds]
+        outs = [torch.empty_like(c) for c in cl]
+        n_out = torch.empty(len(cl), dtype=torch.int32, device=dev)
+        torch.cuda.current_stream(dev).synchronize()        # the uploads are done before the library's stream reads them
+        self.enqueue(cl, leaf, outs, n_out)
+        _lib.check(self.lib.bt_stream_sync(self.stream), "bt_stream_sync")
+        counts = n_out.cpu().numpy()
+        return [o[:int(k)].cpu().numpy() for o, k in zip(outs, counts)]
+
+
+class Overlay:
+    """The LOG frame of a tracked object.  model_pts: the OBJ's points (load_obj_points), voxel-gridded here once at MODEL_LEAF on the device;
+    K: 3 x 3 or (fx, fy, cx, cy); frames of H x W; up to max_frames frames per render call.  leaf=None draws model_pts as given.  Device
+    work runs on `stream`."""
+
+    def __init__(self, model_pts, K, H: int, W: int, max_frames: int = 1, device: int = 0, stream: int = 0, ctx=None, leaf: float = MODEL_LEAF):
+        import torch
+        raw = np.ascontiguousarray(np.asarray(model_pts, np.float32).reshape(-1, 3))
+        if len(raw) == 0:
+            raise ValueError("the model has no point")
+        Kn = np.asarray(K, np.float64)
+        self.K = tuple(float(v) for v in ((Kn[0, 0], Kn[1, 1], Kn[0, 2], Kn[1, 2]) if Kn.ndim == 2 else Kn))
+        self.H, self.W, self.max_frames, self.device = int(H), int(W), int(max_frames), device
+        self.grid = VoxelGrid(len(raw), 1, device=device, stream=stream, ctx=ctx)
+        self.lib, self.ctx, self.stream = self.grid.lib, self.grid.ctx, self.grid.stream
+        self.model = raw if leaf is None else self.grid([raw], leaf)[0]
+        self.grid.reserve(max(len(self.model), 1), self.max_frames)
+        dev = torch.device("cuda", device)
+        self.model_dev = torch.from_numpy(self.model).to(dev)
+        torch.cuda.current_stream(dev).synchronize()
+
+    def close(self):
+        self.grid.close()
+
+    def render(self, cur_in_model, colour, fg, viz_out, raw_out=None) -> None:
+        """Draw len(colour) frames in one asynchronous call on the stream.  cur_in_model: [F,4,4] (or [4,4]) the tracker's cam -> model poses;
+        colour: device uint8 [H,W,3] BGR per frame (the original colour); fg: device uint8 [H,W] per frame (Frame::_fg_mask, or a device
+        address); viz_out / raw_out: device uint8 [H,W,3] per frame (raw_out may be None)."""
+        P = np.ascontiguousarray(np.asarray(cur_in_model, np.float32).reshape(-1, 16))
+        F = len(colour)
+        if len(P) != F or len(fg) != F or len(viz_out) != F or (raw_out is not None and len(raw_out) != F):
+            raise ValueError(f"{len(P)} poses, {F} colour images, {len(fg)} masks, {len(viz_out)} viz outputs: they must agree")
+        if self.model.shape[0] == 0:
+            raise ValueError("the voxel-gridded model is empty (no finite point)")
+        fx, fy, cx, cy = self.K
+        _lib.check(self.lib.bt_pose_overlay(self.ctx, ctypes.c_int(F), ctypes.c_void_p(self.model_dev.data_ptr()), ctypes.c_int(len(self.model)),
+                                            P.ctypes.data_as(ctypes.c_void_p), ctypes.c_float(fx), ctypes.c_float(fy), ctypes.c_float(cx), ctypes.c_float(cy),
+                                            _ptrs(colour), _ptrs(fg), ctypes.c_int(self.H), ctypes.c_int(self.W), _ptrs(viz_out),
+                                            None if raw_out is None else _ptrs(raw_out), self.stream), "bt_pose_overlay")
+
+    def render_host(self, cur_in_model, colour, fg):
+        """render() on host or device images; returns (viz, raw) as uint8 numpy [F,H,W,3] and synchronises the stream."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        to = lambda a: (a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))).to(dev)
+        col = [to(c) for c in colour]
+        m = [to(f) for f in fg]
+        viz = [torch.empty((self.H, self.W, 3), dtype=torch.uint8, device=dev) for _ in col]
+        raw = [torch.empty_like(v) for v in viz]
+        torch.cuda.current_stream(dev).synchronize()
+        self.render(cur_in_model, col, m, viz, raw)
+        _lib.check(self.lib.bt_stream_sync(self.stream), "bt_stream_sync")
+        return np.stack([v.cpu().numpy() for v in viz]), np.stack([r.cpu().numpy() for r in raw])
+
+
+def _cv2():
+    try:
+        import cv2
+    except ImportError as e:
+        raise RuntimeError("writing LOG frames needs OpenCV's Python module (cv2): the reference draws the label and encodes the JPEG and PNG "
+                           "files with OpenCV, and no other encoder gives the same bytes") from e
+    return cv2
+
+
+def label(viz: np.ndarray, id_str: str) -> np.ndarray:
+    """A copy of viz with the frame id drawn as the reference draws it: cv::putText(id, {5, 30}, FONT_HERSHEY_PLAIN, 2, {255, 0, 0}, 1, 8)."""
+    cv2 = _cv2()
+    img = np.ascontiguousarray(viz, np.uint8).copy()
+    cv2.putText(img, id_str, (5, 30), cv2.FONT_HERSHEY_PLAIN, 2, (255, 0, 0), 1, 8, False)
+    return img
+
+
+def write_log_frame(debug_dir: str, id_str: str, viz: np.ndarray, raw: np.ndarray) -> None:
+    """The label on viz, then <debug_dir>/<id>/color_viz.jpg and <debug_dir>/color_viz/<id>_color_viz.jpg (JPEG quality 80) and
+    <debug_dir>/color_raw/<id>_color_raw.png (the masked colour).  Directories are created, color_viz/ included (the reference never creates
+    it, so its write there fails on a fresh debug_dir)."""
+    cv2 = _cv2()
+    img = label(viz, id_str)
+    jobs = ((os.path.join(debug_dir, id_str, "color_viz.jpg"), img, [cv2.IMWRITE_JPEG_QUALITY, 80]),
+            (os.path.join(debug_dir, "color_viz", f"{id_str}_color_viz.jpg"), img, [cv2.IMWRITE_JPEG_QUALITY, 80]),
+            (os.path.join(debug_dir, "color_raw", f"{id_str}_color_raw.png"), np.ascontiguousarray(raw, np.uint8), []))
+    for path, a, params in jobs:
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        if not cv2.imwrite(path, a, params):
+            raise OSError(f"cv2.imwrite could not write {path}")

@@ -8,7 +8,8 @@ library.  The pieces:
 - a prefetching frame reader: a worker thread decodes frames ahead into pinned host buffers and uploads them on a copy stream, and the
   16-bit depth goes to the device as it is (bt_tracker_begin_frame_u16 converts it in the front-end kernel);
 - the LF-Net client (Lfnet::detectFeature's ZMQ round trip, FeatureManager.cpp:861-908);
-- run_sequence: Bundler::processNewFrame + saveNewframeResult for every frame, one pose file per frame.
+- run_sequence: Bundler::processNewFrame + saveNewframeResult for every frame, one pose file per frame and, with log > 0, the LOG frame's
+  images (overlay.py), encoded on a writer thread.
 
 Deliberate difference: the reference finds the ground-truth directory and decides the mask mode by searching data_dir for "NOCS" (DataLoader.cpp:
 68-72, Frame.cpp:251,267).  Here the loader's type decides both, so the dataset root may have any name."""
@@ -74,11 +75,13 @@ def initial_pose(ob_in_cam0) -> np.ndarray:
 
 
 class _Loader:
-    """Shared by both loaders: frames (FrameFiles, in the reference's order), K (3 x 3 float32), ob_in_cam0 (4 x 4 float32), mask_mode."""
+    """Shared by both loaders: frames (FrameFiles, in the reference's order), K (3 x 3 float32), ob_in_cam0 (4 x 4 float32), mask_mode, and
+    model_path, the object's OBJ file the LOG frames draw (None: not known)."""
     frames: list
     K: np.ndarray
     ob_in_cam0: np.ndarray
     mask_mode: int
+    model_path: str = None
 
     def __len__(self) -> int:
         return len(self.frames)
@@ -99,6 +102,7 @@ class NocsScene(_Loader):
         data_dir = f"{nocs_dir}/real_test/scene_{scene_id}/"
         self.data_dir, self.scene_id, self.model_name, self.mask_dir = data_dir, int(scene_id), model_name, mask_dir
         self.K = NOCS_K.copy()
+        self.model_path = f"{nocs_dir}/obj_models/real_test/{model_name}.obj"    # DataLoader.cpp:68-70
         gt_dir = f"{nocs_dir}/gts/real_test_text/scene_{scene_id}/model_{model_name}/"
         gts = _listdir(gt_dir)
         if not gts:
@@ -128,11 +132,13 @@ class NocsScene(_Loader):
 
 
 class YcbineoatVideo(_Loader):
-    """DataLoaderYcbineoat (DataLoader.cpp:303-380) for one video directory."""
+    """DataLoaderYcbineoat (DataLoader.cpp:303-380) for one video directory.  model_dir: the object's OBJ file (the yml's model_dir key,
+    DataLoader.cpp:292), needed only for LOG frames."""
 
-    def __init__(self, data_dir: str):
+    def __init__(self, data_dir: str, model_dir: str = None):
         from ._lib import BT_MASK_AS_IS
         self.data_dir = data_dir
+        self.model_path = model_dir
         self.K = _read_matrix(f"{data_dir}/cam_K.txt", 3, 3)                 # DataLoader.cpp:310
         gt_dir = f"{data_dir}/annotated_poses/"
         gts = _listdir(gt_dir)
@@ -347,15 +353,81 @@ class LfnetClient:
             self.sock = None
 
 
+# ---- LOG frames -----------------------------------------------------------------------------------------------------------------------------
+
+class LogWriter:
+    """Writes LOG frames (overlay.write_log_frame) on a thread of its own, so the JPEG and PNG encodes stay off the tracking thread.
+    submit() copies the device images into one of `depth` pinned slots behind the work already on `stream` and returns; it blocks only while
+    every slot is still being written.  An error on the writer thread is raised by the next submit() or by close()."""
+
+    def __init__(self, debug_dir: str, H: int, W: int, depth: int = 4):
+        import torch
+        from .overlay import _cv2
+        _cv2()                                           # no OpenCV: fail before the run starts
+        self.torch, self.debug_dir = torch, debug_dir
+        self.slots = [(torch.empty((H, W, 3), dtype=torch.uint8, pin_memory=True), torch.empty((H, W, 3), dtype=torch.uint8, pin_memory=True),
+                       torch.cuda.Event()) for _ in range(depth)]
+        self._free = queue.Queue()
+        for k in range(depth):
+            self._free.put(k)
+        self._q = queue.Queue()
+        self._err = None
+        self._thread = threading.Thread(target=self._run, daemon=True)
+        self._thread.start()
+
+    def _raise(self):
+        if self._err is not None:
+            e, self._err = self._err, None
+            raise RuntimeError(f"writing a LOG frame failed: {e}") from e
+
+    def _run(self):
+        from .overlay import write_log_frame
+        while True:
+            item = self._q.get()
+            if item is None:
+                return
+            k, id_str = item
+            hv, hr, ev = self.slots[k]
+            try:
+                if self._err is None:
+                    ev.synchronize()
+                    write_log_frame(self.debug_dir, id_str, hv.numpy(), hr.numpy())
+            except BaseException as e:      # handed to the tracking thread
+                self._err = e
+            finally:
+                self._free.put(k)
+
+    def submit(self, id_str: str, viz_dev, raw_dev, stream) -> None:
+        self._raise()
+        k = self._free.get()
+        hv, hr, ev = self.slots[k]
+        with self.torch.cuda.stream(stream):
+            hv.copy_(viz_dev, non_blocking=True)
+            hr.copy_(raw_dev, non_blocking=True)
+            ev.record(stream)
+        self._q.put((k, id_str))
+
+    def close(self) -> None:
+        """Waits for every frame submitted, then raises the writer's error if there was one."""
+        if self._thread is not None:
+            self._q.put(None)
+            self._thread.join()
+            self._thread = None
+        self._raise()
+
+
 # ---- the run --------------------------------------------------------------------------------------------------------------------------------
 
-def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max_keyframes: int = None, device: int = 0, prefetch: int = 2):
+def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max_keyframes: int = None, device: int = 0, prefetch: int = 2,
+                 log: int = 0):
     """Tracks every frame the loader yields (Bundler::processNewFrame) and writes <out_dir>/poses/<id_str>.txt for each one with
     policy.save_pose_txt (Bundler::saveNewframeResult runs after every frame): the initial pose of a frame that fails the ROI gate, the
     pose drop_frame reports when detection fails, otherwise end_frame's.  features(id_str, request uint8 [400,400,3] host, roi) returns
     (kpts [n,2] image pixels, desc [n,256] float32) or raises DetectionFailed; a reply with more than max_feats rows or descriptors that are
     not 256-dimensional is dropped too.  Sizing as INTEGRATION.md §7: max_frames_alive = bundle.window_size + 4, max_keyframes defaults to
-    min(1024, ceil(n_frames / 2)).  Nothing under out_dir is removed.  Returns [(id_str, status, wall seconds)] per frame."""
+    min(1024, ceil(n_frames / 2)).  Nothing under out_dir is removed.  Returns [(id_str, status, wall seconds)] per frame.
+    log > 0 (the yml's LOG): every frame's LOG images under out_dir (the reference's debug_dir), drawn on the device with the pose its pose
+    file holds (overlay.Overlay over loader.model_path) and written by a LogWriter thread; needs cv2.  log = 0 runs none of it."""
     import torch
     from .tracker import Tracker
     n = len(loader)
@@ -370,9 +442,17 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
     stream = torch.cuda.Stream(dev)
     trk = Tracker(y, H, W, loader.K, max_feats, int(y["bundle"]["window_size"]) + 4, device=device, stream=stream.cuda_stream,
                   mode=loader.mask_mode, max_keyframes=max_keyframes)
-    reader = None
+    reader = ovl = writer = None
     out = []
     try:
+        if log > 0:
+            from .overlay import Overlay, load_obj_points
+            if not loader.model_path:
+                raise ValueError("log > 0 draws the object model: the loader has no model path (YcbineoatVideo needs model_dir)")
+            writer = LogWriter(out_dir, H, W)
+            ovl = Overlay(load_obj_points(loader.model_path), loader.K, H, W, device=device, stream=stream.cuda_stream)
+            with torch.cuda.device(dev):
+                viz, raw = (torch.empty((H, W, 3), dtype=torch.uint8, device=dev) for _ in range(2))
         reader = FrameReader(loader, H, W, device, stream, prefetch)
         with torch.cuda.device(dev):
             request = torch.empty((LFNET_SIDE, LFNET_SIDE, 3), dtype=torch.uint8, device=dev)
@@ -380,7 +460,8 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
             t0 = time.perf_counter()
             depth, mask, colour = reader.get(i)
             st, roi, _, pose = trk.begin_frame_mm(depth, mask, colour, request, loader_id=i, first_pose=loader.initial_pose(i))
-            reader.release(i)
+            if ovl is None:
+                reader.release(i)
             if st == _lib.BT_FRAME_OTHER:
                 with torch.cuda.device(dev), torch.cuda.stream(stream):
                     req = request.cpu()
@@ -405,11 +486,25 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
                         raise _lib.BtError(f"frame {ff.id_str}: the tracker is full ({e}); raise max_keyframes (now {max_keyframes})",
                                            _lib.BT_ERR_CAPACITY) from e
             policy.save_pose_txt(os.path.join(out_dir, "poses", f"{ff.id_str}.txt"), pose)
+            if ovl is not None:
+                # the frame's colour slot and the tracker's fg map are read on `stream` before the slot is released and the next begin_frame
+                ovl.render(pose, [colour], [trk.last_fg()], [viz], [raw])
+                reader.release(i)
+                writer.submit(ff.id_str, viz, raw, stream)
             out.append((ff.id_str, st, time.perf_counter() - t0))
+        if writer is not None:
+            writer.close()
     finally:
         if reader is not None:
             reader.close()
         stream.synchronize()
+        if writer is not None:
+            try:
+                writer.close()
+            except Exception:
+                pass                # (the run is already failing: its own error is the one raised)
+        if ovl is not None:
+            ovl.close()
         trk.close()
     return out
 

@@ -458,3 +458,11 @@ def write_png(path: str, img: np.ndarray) -> None:
     with open(path, "wb") as f:
         f.write(b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", a.shape[1], a.shape[0], depth, ctype, 0, 0, 0))
                 + chunk(b"IDAT", zlib.compress(raw, 1)) + chunk(b"IEND", b""))
+
+
+def make_ellipsoid_model(seed: int, n: int, radii=(0.05, 0.04, 0.03)) -> np.ndarray:
+    """float32 [n,3]: n points on the surface of an ellipsoid with the given semi-axes (metres), the stand-in for an OBJ model's vertices."""
+    rng = np.random.default_rng(seed)
+    u = rng.normal(size=(n, 3))
+    u /= np.linalg.norm(u, axis=1, keepdims=True)
+    return (u * np.asarray(radii, np.float64)).astype(np.float32)

@@ -116,6 +116,13 @@ class Tracker:
                                              ctypes.c_int(cap), ctypes.byref(n)), "bt_tracker_state")
         return ids[:n.value].copy(), poses[:n.value].copy(), kf[:n.value].astype(bool)
 
+    def last_fg(self) -> int:
+        """Device address of Frame::_fg_mask (uint8 [H,W]) of the frame the last begin_frame segmented, ROI failures and dropped frames
+        included; valid until the next begin_frame on the tracker's stream."""
+        p = ctypes.c_void_p()
+        _lib.check(self.lib.bt_tracker_last_fg(self.t, ctypes.byref(p)), "bt_tracker_last_fg")
+        return int(p.value)
+
     def usage(self):
         """(map points alive, pairs in the match cache, entries of their blocks); synchronises the tracker's stream."""
         pts, pairs, ents = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_longlong(0)

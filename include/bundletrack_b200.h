@@ -536,6 +536,10 @@ BT_API int bt_tracker_drop_frame(bt_tracker* t, float* pose_out);
 BT_API int bt_tracker_state(bt_tracker* t, int32_t* ids, float* poses, int32_t* is_keyframe, int cap, int* n);
 /* What the tracker's tables hold now: map points alive, pairs in the match cache and the entries of their blocks.  Synchronises `stream`. */
 BT_API int bt_tracker_usage(bt_tracker* t, int* n_points, int* n_pairs_cached, long long* n_entries_cached, void* stream);
+/* Frame::_fg_mask (DEVICE uint8 H*W, 0 = background) of the frame the last begin_frame segmented, whatever became of it: a frame that failed
+ * the ROI gate or was dropped included.  Valid until the next begin_frame on the tracker's stream; read it with work enqueued on that stream
+ * before then (bt_pose_overlay for the reference's LOG frames).  BT_ERR_INVALID_ARG before the first begin_frame. */
+BT_API int bt_tracker_last_fg(bt_tracker* t, const uint8_t** fg_dev);
 
 /* ---- pose accuracy: the reference's evaluation (scripts/Utils.py add / adi, scripts/eval_ycbineoat.py VOCap) -------------------------
  * bt_pose_metrics: per frame f, ADD = mean_i |gt_f p_i - pred_f p_i| and ADD-S = mean_i min_j |gt_f p_i - pred_f p_j| over the model points p,
@@ -585,6 +589,39 @@ BT_API int bt_nocs_metrics(bt_ctx* ctx, const double* pred, const double* gt, co
  * n < 1, a NULL pointer, a class outside 1..6 or a class without records. */
 BT_API int bt_nocs_score(const int32_t* cls, const int32_t* scored, const double* theta_deg, const double* shift, const double* iou, int n,
                          double* per_class_out, double* overall_out);
+
+/* ---- tracking overlays: the reference's LOG frames (Bundler::saveNewframeResult, Bundler.cpp:379-411) ---------------------------------
+ * bt_voxel_downsample: PCL's VoxelGrid (Utils::downsamplePointCloud, Utils.cpp:134-140; pcl::VoxelGrid::applyFilter with every field
+ * averaged and no minimum count) of n_clouds clouds in one call, float32 (DESIGN.md §3.10): the voxel bounds from each cloud's finite
+ * points, one centroid per occupied voxel in ascending voxel index, non-finite points skipped, and a cloud whose grid would exceed INT32_MAX
+ * cells returned unchanged (non-finite points included).  Deliberate difference: the points of a voxel are summed in input order (PCL's
+ * std::sort leaves that order open; DESIGN.md §4).  Results do not depend on how clouds are batched.
+ *   pts_dev    HOST array of n_clouds DEVICE pointers, float32 n_pts[c] x 3 each.  n_pts: HOST, each >= 1.
+ *   leaf       the voxel side (metres), positive and finite; the same for every cloud.
+ *   out_dev    HOST array of n_clouds DEVICE pointers with room for n_pts[c] x 3 floats; n_out_dev: DEVICE int32 [n_clouds], the counts.
+ * Asynchronous on `stream`: no host synchronisation; the counts stay on the device.  BT_ERR_INVALID_ARG for a NULL pointer, n_clouds < 1,
+ * an empty cloud, a bad leaf or a context without bt_overlay_reserve; BT_ERR_CAPACITY for more than max_frames clouds or more than
+ * max_pts x max_frames points in all. */
+BT_API int bt_voxel_downsample(bt_ctx* ctx, int n_clouds, const float* const* pts_dev, const int* n_pts, float leaf, float* const* out_dev, int32_t* n_out_dev,
+                               void* stream);
+/* bt_pose_overlay: Bundler::saveNewframeResult's color_viz without the label, for n_frames frames in one call (Utils::drawProjectPoints,
+ * Utils.cpp:216-226): the model moved by ob_in_cam = inverse(cur_in_model) (the float inverse bt_pose_format prints; each coordinate
+ * ((m0 x + m1 y) + m2 z) + m3, every operation rounded), voxel-gridded at 0.01 as bt_voxel_downsample does, each centroid projected to
+ * u = roundf(x fx / z + cx), v = roundf(y fy / z + cy) and, inside the image, stamped as cv::circle(r = 1, filled) in BGR (0, 255, 255): the
+ * pixel and its four neighbours, clipped.  Under the stamps: the colour, each channel (uint8)(c * 0.2) where fg == 0.  raw: the colour with
+ * fg == 0 pixels zeroed (the color_raw image, Frame::_color after invalidatePixelsByMask).
+ *   model_dev   DEVICE float32 n_model x 3 (the model as the loader keeps it, voxel-gridded at 0.015).
+ *   cur_in_model HOST row-major 4 x 4 cam->model per frame (the tracker's pose), n_frames back to back.
+ *   colour_dev / fg_dev / viz_out_dev / raw_out_dev  HOST arrays of n_frames DEVICE pointers: uint8 H*W*3 BGR, H*W, H*W*3, H*W*3.  raw_out_dev
+ *               may be NULL.
+ * Asynchronous on `stream`.  BT_ERR_INVALID_ARG for a NULL pointer, sizes < 1, a singular pose or a context without bt_overlay_reserve;
+ * BT_ERR_CAPACITY for more than max_frames frames or max_pts model points.
+ * bt_overlay_reserve: scratch for max_frames clouds of max_pts points (max_pts x max_frames <= 2^30): 44 B per point on the device, about
+ * 1 KB per 2048 points in pinned host memory. */
+BT_API int bt_overlay_reserve(bt_ctx* ctx, int max_pts, int max_frames);
+BT_API int bt_pose_overlay(bt_ctx* ctx, int n_frames, const float* model_dev, int n_model, const float* cur_in_model, float fx, float fy, float cx, float cy,
+                           const uint8_t* const* colour_dev, const uint8_t* const* fg_dev, int H, int W, uint8_t* const* viz_out_dev,
+                           uint8_t* const* raw_out_dev, void* stream);
 
 /* Small device-memory helpers so non-CUDA hosts (ctypes, cgo, JNI) can drive the library without another runtime. */
 BT_API int bt_dev_alloc(void** out, size_t bytes);

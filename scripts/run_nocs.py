@@ -2,7 +2,8 @@
 """Tracks one model in one NOCS-REAL275 scene, as the reference's scripts/run_nocs.py + bundle_track_nocs do, and writes one pose file per
 frame to <out_dir>/<model>_<scene>/poses/<id>.txt, the layout scripts/eval_nocs.py reads.  Features come from a running LF-Net server
 (lf-net-release/run_server.py) at tcp://127.0.0.1:<port>.  Frames follow the 6-PACK data list (bundletrack_b200.sequence.NocsScene); the
-masks are <mask_dir>/<id>.png.  Nothing under out_dir is removed.
+masks are <mask_dir>/<id>.png.  With --log 1 the
+reference's LOG images are written next to the poses (bundletrack_b200.overlay).  Nothing under out_dir is removed.
 
     python scripts/run_nocs.py --nocs_dir NOCS --scene_id 1 --model_name can_arizona_tea_norm --mask_dir masks/scene_1_model_can_arizona_tea_norm \\
         --out_dir results --port 5555
@@ -28,11 +29,13 @@ def main():
     ap.add_argument("--out_dir", required=True)
     ap.add_argument("--config", default=None, help="a config_nocs.yml (default: its values, bundletrack_b200.config.NOCS_DEFAULTS)")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--log", type=int, default=0, help="the config's LOG: > 0 also writes every frame's overlay images under the output "
+                                                       "directory (<id>/color_viz.jpg, color_viz/, color_raw/); needs cv2")
     a = ap.parse_args()
     loader = NocsScene(a.nocs_dir, a.scene_id, a.model_name, a.mask_dir)
     client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
     try:
-        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, f"{a.model_name}_{a.scene_id}"), device=a.device)
+        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, f"{a.model_name}_{a.scene_id}"), device=a.device, log=a.log)
     finally:
         client.close()
     print(summary(res))

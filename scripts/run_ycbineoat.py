@@ -2,7 +2,8 @@
 """Tracks one YCBInEOAT video, as the reference's scripts/run_ycbineoat.py + bundle_track_ycbineoat do, and writes one pose file per frame to
 <out_dir>/<video>/poses/<id>.txt, the layout scripts/eval_poses.py reads.  Features come from a running LF-Net server
 (lf-net-release/run_server.py) at tcp://127.0.0.1:<port>.  The video directory holds rgb/, depth/, masks/, annotated_poses/ and cam_K.txt
-(bundletrack_b200.sequence.YcbineoatVideo).  Nothing under out_dir is removed.
+(bundletrack_b200.sequence.YcbineoatVideo).  With --log 1 the
+reference's LOG images are written next to the poses (bundletrack_b200.overlay).  Nothing under out_dir is removed.
 
     python scripts/run_ycbineoat.py --data_dir YCBInEOAT/bleach0 --config config_ycbineoat.yml --out_dir results --port 5555
     python scripts/eval_poses.py --dataset_dir YCBInEOAT --model_dir YCB_Video_Dataset/models --results_dir results
@@ -25,14 +26,17 @@ def main():
     ap.add_argument("--config", default=None, help="the reference's config_ycbineoat.yml (default: the config_nocs.yml values, "
                                                     "bundletrack_b200.config.NOCS_DEFAULTS)")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--log", type=int, default=0, help="the config's LOG: > 0 also writes every frame's overlay images under the output "
+                                                       "directory (<id>/color_viz.jpg, color_viz/, color_raw/); needs cv2")
+    ap.add_argument("--model_dir", default=None, help="the object's OBJ file (the config's model_dir), drawn by --log")
     a = ap.parse_args()
     if not os.path.isdir(a.data_dir):
         raise SystemExit(f"--data_dir {a.data_dir} is not a directory")
-    loader = YcbineoatVideo(a.data_dir)
+    loader = YcbineoatVideo(a.data_dir, a.model_dir)
     video = os.path.basename(os.path.normpath(a.data_dir))
     client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
     try:
-        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, video), device=a.device)
+        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, video), device=a.device, log=a.log)
     finally:
         client.close()
     print(summary(res))
