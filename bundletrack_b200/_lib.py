@@ -138,6 +138,14 @@ class MatchExtra(ctypes.Structure):
     _fields_ = [("uv", ctypes.c_void_p), ("n", ctypes.c_int)]
 
 
+class MatchVizDesc(ctypes.Structure):
+    _fields_ = [
+        ("colour_a", ctypes.c_void_p), ("H_a", ctypes.c_int), ("W_a", ctypes.c_int), ("roi_a", ctypes.c_int32 * 4),
+        ("colour_b", ctypes.c_void_p), ("H_b", ctypes.c_int), ("W_b", ctypes.c_int), ("roi_b", ctypes.c_int32 * 4),
+        ("uv", ctypes.c_void_p), ("n", ctypes.c_int), ("rng_state", ctypes.c_uint64),
+    ]
+
+
 class DescView(ctypes.Structure):
     _fields_ = [
         ("dev", ctypes.c_void_p),
@@ -161,6 +169,7 @@ EXPORTS = [
     "bt_pose_init", "bt_tracker_create", "bt_tracker_destroy", "bt_tracker_begin_frame", "bt_tracker_begin_frame_u16", "bt_tracker_end_frame", "bt_tracker_drop_frame", "bt_tracker_state", "bt_tracker_usage", "bt_tracker_last_fg",
     "bt_metrics_reserve", "bt_pose_metrics", "bt_vocap", "bt_nocs_reserve", "bt_nocs_metrics", "bt_nocs_score",
     "bt_overlay_reserve", "bt_voxel_downsample", "bt_pose_overlay",
+    "bt_match_viz_shape", "bt_match_viz_reserve", "bt_match_viz",
     "bt_dev_alloc", "bt_dev_free", "bt_memcpy_h2d", "bt_memcpy_d2h", "bt_host_alloc_pinned", "bt_host_free_pinned",
     "bt_stream_sync", "bt_debug_live_resources",
 ]

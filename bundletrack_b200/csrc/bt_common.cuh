@@ -139,6 +139,7 @@ struct TracksDev;     // tracks_dev.cu
 struct MetricsState;  // metrics.cu
 struct NocsState;     // metrics.cu
 struct OverlayState;  // overlay.cu
+struct MatchVizState; // matchviz.cu
 
 // The context owns the module states; each module defines the deleter of its state next to it, so the states stay private to their files.
 struct StateDeleter {
@@ -152,6 +153,7 @@ struct StateDeleter {
 	void operator()(MetricsState*) const;
 	void operator()(NocsState*) const;
 	void operator()(OverlayState*) const;
+	void operator()(MatchVizState*) const;
 };
 template <class T> using StatePtr = std::unique_ptr<T, StateDeleter>;
 
@@ -171,6 +173,7 @@ struct bt_ctx {
 	bt::StatePtr<bt::MetricsState> metrics;
 	bt::StatePtr<bt::NocsState> nocs;
 	bt::StatePtr<bt::OverlayState> overlay;
+	bt::StatePtr<bt::MatchVizState> matchviz;
 };
 
 namespace bt {

@@ -5,6 +5,7 @@
 // Everything is integer arithmetic (the resize's coefficients come from the same double -> float expressions as OpenCV's, with no
 // contraction), so the results do not depend on scheduling.  oracle/segment_oracle.py is the CPU statement of the same rules.
 #include "bt_common.cuh"
+#include "resize.cuh"
 
 namespace bt {
 
@@ -203,23 +204,6 @@ struct ReqArgs {
 	int H, W;
 };
 
-// cv::resize's INTER_LINEAR source index and 11-bit weights for destination index d (resize.cpp: fx = (float)((d + 0.5) * scale - 0.5),
-// scale = 1 / (dst / src) in double; the weights are saturate_cast<short>(w * 2048), i.e. rounded half to even).  Only the horizontal
-// direction moves the weight onto the edge sample; both clamp the indices.
-__device__ __forceinline__ void lin_coeffs(int d, int src, bool clamp_weights, int& s0, int& s1, int& w0, int& w1) {
-	const double scale = __ddiv_rn(1.0, __ddiv_rn((double)REQ_SIDE, (double)src));
-	float fx = __double2float_rn(__dadd_rn(__dmul_rn((double)d + 0.5, scale), -0.5));
-	int s = (int)floorf(fx);
-	fx = __fsub_rn(fx, (float)s);
-	if (clamp_weights) {
-		if (s < 0) { fx = 0.f; s = 0; }
-		if (s >= src - 1) { fx = 0.f; s = src - 1; }
-	}
-	w0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, fx), 2048.f));
-	w1 = __float2int_rn(__fmul_rn(fx, 2048.f));
-	s0 = min(max(s, 0), src - 1); s1 = min(max(s + 1, 0), src - 1);
-}
-
 __global__ void __launch_bounds__(256) k_lfnet_request(ReqArgs a) {
 	const int f = blockIdx.z, dx = blockIdx.x * 32 + threadIdx.x, dy = blockIdx.y * 8 + threadIdx.y;
 	if (dx >= REQ_SIDE || dy >= REQ_SIDE) return;
@@ -239,16 +223,11 @@ __global__ void __launch_bounds__(256) k_lfnet_request(ReqArgs a) {
 	uchar3 c00;
 	if (side == REQ_SIDE) { px(dy, dx, c00); o[0] = c00.x; o[1] = c00.y; o[2] = c00.z; return; }
 	int x0, x1, a0, a1, y0, y1, b0, b1;
-	lin_coeffs(dx, side, true, x0, x1, a0, a1);
-	lin_coeffs(dy, side, false, y0, y1, b0, b1);
+	lin_coeffs(dx, REQ_SIDE, side, true, x0, x1, a0, a1);
+	lin_coeffs(dy, REQ_SIDE, side, false, y0, y1, b0, b1);
 	uchar3 c01, c10, c11;
 	px(y0, x0, c00); px(y0, x1, c01); px(y1, x0, c10); px(y1, x1, c11);
-	// horizontal pass exact; vertical pass as OpenCV's vector path rounds it: ((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16), then (t + 2) >> 2
-	auto v = [&](int p00, int p01, int p10, int p11) {
-		const int h0 = p00 * a0 + p01 * a1, h1 = p10 * a0 + p11 * a1;
-		const int t = ((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16);
-		return (uint8_t)min(max((t + 2) >> 2, 0), 255);
-	};
+	auto v = [&](int p00, int p01, int p10, int p11) { return lin_blend(p00, p01, p10, p11, a0, a1, b0, b1); };
 	o[0] = v(c00.x, c01.x, c10.x, c11.x);
 	o[1] = v(c00.y, c01.y, c10.y, c11.y);
 	o[2] = v(c00.z, c01.z, c10.z, c11.z);

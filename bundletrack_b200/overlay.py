@@ -176,3 +176,123 @@ def write_log_frame(debug_dir: str, id_str: str, viz: np.ndarray, raw: np.ndarra
         os.makedirs(os.path.dirname(path), exist_ok=True)
         if not cv2.imwrite(path, a, params):
             raise OSError(f"cv2.imwrite could not write {path}")
+
+
+# ---- match images: the reference's LOG correspondence drawings (SiftManager::vizCorresBetween, src/FeatureManager.cpp:760-796)
+
+RNG_DEFAULT = 0xFFFFFFFF            # cv::theRNG()'s state when a process starts
+JPEG_MAX_SIDE = 65500               # libjpeg's limit: cv2.imwrite returns False past it
+
+
+def rng_after(state: int, n_matches: int) -> int:
+    """cv::RNG's state after the colours of an image of n_matches matches (three draws per match)."""
+    for _ in range(3 * int(n_matches)):
+        state = ((state & 0xFFFFFFFF) * 4164903690 + (state >> 32)) & 0xFFFFFFFFFFFFFFFF
+    return state
+
+
+def match_image_shape(roi_a, roi_b):
+    """(rows, cols) of the match image of two ROIs (umin, umax, vmin, vmax)."""
+    lib = _lib.load()
+    ra, rb = (ctypes.c_int32 * 4)(*[int(v) for v in roi_a]), (ctypes.c_int32 * 4)(*[int(v) for v in roi_b])
+    rows, cols = ctypes.c_int(), ctypes.c_int()
+    _lib.check(lib.bt_match_viz_shape(ra, rb, ctypes.byref(rows), ctypes.byref(cols)), "bt_match_viz_shape")
+    return rows.value, cols.value
+
+
+def match_image_path(debug_dir: str, new_id: str, id_a: str, id_b: str, stage: str) -> str:
+    """<debug_dir>/<new frame id>/<A id>_match_<B id>_<stage>.jpg, the reference's name for a match image."""
+    return os.path.join(debug_dir, new_id, f"{id_a}_match_{id_b}_{stage}.jpg")
+
+
+class MatchViz:
+    """bt_match_viz: match images drawn on the device, many per asynchronous call.  Scratch for max_images images and max_matches matches
+    per call is reserved here (or on `ctx`)."""
+
+    def __init__(self, max_images: int = 1, max_matches: int = 4096, device: int = 0, stream: int = 0, ctx=None):
+        self.lib = _lib.load()
+        self.device, self.stream = device, ctypes.c_void_p(stream)
+        self._own = ctx is None
+        self.ctx = ctypes.c_void_p() if ctx is None else ctx
+        if self._own:
+            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
+        _lib.check(self.lib.bt_match_viz_reserve(self.ctx, ctypes.c_int(max_images), ctypes.c_int(max_matches)), "bt_match_viz_reserve")
+
+    def close(self):
+        if self._own and self.ctx:
+            self.lib.bt_ctx_destroy(self.ctx)
+            self.ctx = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def draw(self, images, outs) -> None:
+        """images: (colour_a, roi_a, colour_b, roi_b, uv, rng_state) per image; colours are device uint8 [H,W,3], uv a device float32 [n,4]
+        (uA, vA, uB, vB) or None; outs: device uint8 [rows, cols, 3] per image (match_image_shape).  Asynchronous on the stream."""
+        n = len(images)
+        if len(outs) != n:
+            raise ValueError(f"{n} images and {len(outs)} outputs")
+        descs = (_lib.MatchVizDesc * n)()
+        for k, (d, (ca, ra, cb, rb, uv, st), o) in enumerate(zip(descs, images, outs)):
+            self._check(k, ca, ra, cb, rb, uv, o)
+            d.colour_a, d.H_a, d.W_a = ca.data_ptr(), ca.shape[0], ca.shape[1]
+            d.colour_b, d.H_b, d.W_b = cb.data_ptr(), cb.shape[0], cb.shape[1]
+            d.roi_a[:] = [int(v) for v in ra]
+            d.roi_b[:] = [int(v) for v in rb]
+            d.uv, d.n = (None, 0) if uv is None or uv.shape[0] == 0 else (uv.data_ptr(), uv.shape[0])
+            d.rng_state = int(st)
+        _lib.check(self.lib.bt_match_viz(self.ctx, ctypes.c_int(n), descs, _ptrs(outs), self.stream), "bt_match_viz")
+
+    def _check(self, k, ca, ra, cb, rb, uv, out) -> None:
+        """The library reads these through raw device pointers: each must be a contiguous CUDA tensor on this device, of the dtype and
+        shape the call expects."""
+        import torch
+
+        def dev_tensor(x, what, dtype):
+            if not isinstance(x, torch.Tensor) or not x.is_cuda or x.device.index != self.device:
+                raise ValueError(f"image {k}: {what} must be a CUDA tensor on device {self.device}")
+            if x.dtype != dtype or not x.is_contiguous():
+                raise ValueError(f"image {k}: {what} must be a contiguous {dtype} tensor, not {x.dtype}{'' if x.is_contiguous() else ' (strided)'}")
+
+        for c, what in ((ca, "colour_a"), (cb, "colour_b")):
+            dev_tensor(c, what, torch.uint8)
+            if c.dim() != 3 or c.shape[2] != 3:
+                raise ValueError(f"image {k}: {what} must be [H, W, 3], not {list(c.shape)}")
+        if uv is not None:
+            dev_tensor(uv, "uv", torch.float32)
+            if uv.dim() != 2 or uv.shape[1] != 4:
+                raise ValueError(f"image {k}: uv must be [n, 4] (uA, vA, uB, vB), not {list(uv.shape)}")
+        dev_tensor(out, "out", torch.uint8)
+        want = (*match_image_shape(ra, rb), 3)
+        if tuple(out.shape) != want:
+            raise ValueError(f"image {k}: out must be {list(want)}, not {list(out.shape)}")
+
+    def draw_host(self, images):
+        """draw() on host or device inputs; returns uint8 numpy images and synchronises the stream."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        to = lambda a, dt: (a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a, dt))).to(dev).contiguous()
+        ims = []
+        for ca, ra, cb, rb, uv, st in images:
+            u = None if uv is None or len(uv) == 0 else to(np.asarray(uv, np.float32).reshape(-1, 4), np.float32)
+            ims.append((to(ca, np.uint8), ra, to(cb, np.uint8), rb, u, st))
+        outs = [torch.empty((*match_image_shape(ra, rb), 3), dtype=torch.uint8, device=dev) for _, ra, _, rb, _, _ in ims]
+        torch.cuda.current_stream(dev).synchronize()
+        self.draw(ims, outs)
+        _lib.check(self.lib.bt_stream_sync(self.stream), "bt_stream_sync")
+        return [o.cpu().numpy() for o in outs]
+
+
+def write_match_image(path: str, img: np.ndarray) -> bool:
+    """imwrite(path, img, JPEG quality 80) as vizCorresBetween does.  An image wider or taller than JPEG allows is not written, as
+    cv::imwrite writes nothing for it: returns False (the caller reports it) instead of failing the run."""
+    cv2 = _cv2()
+    if max(img.shape[:2]) > JPEG_MAX_SIDE:
+        return False
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    if not cv2.imwrite(path, np.ascontiguousarray(img, np.uint8), [cv2.IMWRITE_JPEG_QUALITY, 80]):
+        raise OSError(f"cv2.imwrite could not write {path}")
+    return True

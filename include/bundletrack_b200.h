@@ -623,6 +623,39 @@ BT_API int bt_pose_overlay(bt_ctx* ctx, int n_frames, const float* model_dev, in
                            const uint8_t* const* colour_dev, const uint8_t* const* fg_dev, int H, int W, uint8_t* const* viz_out_dev,
                            uint8_t* const* raw_out_dev, void* stream);
 
+/* ---- match images: the reference's LOG correspondence drawings (SiftManager::vizCorresBetween, FeatureManager.cpp:760-796) ----------
+ * One image per desc, exactly as cv::drawMatches(NOT_DRAW_SINGLE_POINTS) of OpenCV 4.x draws it (DESIGN.md §3.11): the two ROI crops,
+ * each resized by scale = min(900 / rows_a, 900 / rows_b) (integer division; 8-bit INTER_LINEAR, a copy at 1) and placed side by side on a
+ * zero canvas of max(rows) x (cols_a + cols_b) pixels; then per match, in list order, a colour from cv::RNG, an anti-aliased circle of
+ * radius 3 at the A keypoint clipped to the A half, one at the B keypoint clipped to the B half, and an anti-aliased line between them
+ * (LINE_AA, 1/16-pixel coordinates).  Keypoints are ((u - umin) scale, (v - vmin) scale) in float32.
+ *   colour_a / colour_b  DEVICE uint8 H x W x 3 BGR (the masked colour); roi_*: umin, umax, vmin, vmax, the crop is rows [vmin, vmax) and
+ *               columns [umin, umax) and must lie inside the image, at most 900 rows tall.
+ *   uv          DEVICE float4 (uA, vA, uB, vB) per match in full-image pixels, 16-byte aligned; may be NULL when n == 0.
+ *   rng_state   cv::theRNG()'s state before the image (OpenCV's default is 0xffffffff).  A match draws three values, so the next image
+ *               of a run starts from the state advanced by 3 n draws. */
+typedef struct {
+	const uint8_t* colour_a;
+	int H_a, W_a;
+	int32_t roi_a[4];
+	const uint8_t* colour_b;
+	int H_b, W_b;
+	int32_t roi_b[4];
+	const float* uv;
+	int n;
+	uint64_t rng_state;
+} bt_match_viz_desc;
+/* bt_match_viz_shape: the output rows and cols of the image of two ROIs (each at least 1 x 1 and at most 900 rows tall). */
+BT_API int bt_match_viz_shape(const int32_t* roi_a, const int32_t* roi_b, int* rows, int* cols);
+/* bt_match_viz_reserve: scratch for max_images images (1 to 65535) and max_matches matches over a call: 2052 B of device memory and 4 B
+ * of pinned host memory per match (25 segment records of 80 B, 3 boxes, a colour), 112 B per image on each side. */
+BT_API int bt_match_viz_reserve(bt_ctx* ctx, int max_images, int max_matches);
+/* bt_match_viz: draws n_images images in one asynchronous call on `stream`; out_dev is a HOST array of n_images DEVICE pointers to
+ * rows x cols x 3 uint8 (bt_match_viz_shape).  Results do not depend on how images are batched.  BT_ERR_INVALID_ARG for a NULL pointer,
+ * a bad ROI, n < 0, more than 2^31 - 1 tiles of 32 x 32 output pixels in all, or a context without bt_match_viz_reserve;
+ * BT_ERR_CAPACITY beyond the reserved images or matches. */
+BT_API int bt_match_viz(bt_ctx* ctx, int n_images, const bt_match_viz_desc* desc, uint8_t* const* out_dev, void* stream);
+
 /* Small device-memory helpers so non-CUDA hosts (ctypes, cgo, JNI) can drive the library without another runtime. */
 BT_API int bt_dev_alloc(void** out, size_t bytes);
 BT_API int bt_dev_free(void* p);
