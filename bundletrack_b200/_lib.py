@@ -6,6 +6,8 @@ from __future__ import annotations
 import ctypes
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # BT_B200_LIB selects another BUILD of the same library (kernel experiments); there is still no non-CUDA path behind it
 LIB_PATH = os.environ.get("BT_B200_LIB") or os.path.join(_HERE, "lib", "libbundletrack_b200.so")
@@ -155,24 +157,117 @@ class DescView(ctypes.Structure):
     ]
 
 
-# every symbol include/bundletrack_b200.h declares (tests/test_abi.py checks the .so exports all of them)
-EXPORTS = [
-    "bt_last_error", "bt_version", "bt_ctx_create", "bt_ctx_destroy", "bt_solver_reserve",
-    "bt_solve_windows", "bt_solve_windows_begin", "bt_solve_windows_end", "bt_solve_stage", "bt_solve_run", "bt_solve_fetch", "bt_solve_get_stats",
-    "bt_solve_enable_debug", "bt_solve_debug_dense", "bt_solve_debug_counts", "bt_solve_debug_system", "bt_solve_enable_timing", "bt_solve_get_timing", "bt_solve_get_host_timing", "bt_solve_enable_profile", "bt_solve_get_profile",
-    "bt_matcher_reserve", "bt_desc_pool_reserve", "bt_desc_pool_store", "bt_knn_match_slots", "bt_match_pairs_pool", "bt_match_pairs_ex", "bt_match_cache_reserve", "bt_match_cache_reserve_entries", "bt_match_cache_usage", "bt_match_cache_put", "bt_match_cache_has", "bt_match_cache_status", "bt_match_cache_gather", "bt_match_cache_forget_frame", "bt_knn_match_pairs", "bt_knn_enable_timing", "bt_knn_get_timing", "bt_knn_debug_force_fallback", "bt_ransac_reserve", "bt_ransac_pairs", "bt_ransac_debug",
-    "bt_pipeline_reserve", "bt_prune_mutual_pairs", "bt_match_pairs", "bt_frames_preprocess", "bt_frames_preprocess_masked", "bt_frames_preprocess_masked_u16", "bt_lfnet_request",
-    "bt_frame_cache_reserve", "bt_frame_cache_store",
-    "bt_rotation_geodesic", "bt_keyframe_check", "bt_select_keyframes", "bt_rigid_transform", "bt_lfnet_parse_reply", "bt_ba_gate", "bt_pose_format", "bt_pose_write_txt",
-    "bt_tracks_create", "bt_tracks_destroy", "bt_tracks_update_pair", "bt_tracks_propagate", "bt_tracks_forget_frame", "bt_tracks_stats",
-    "bt_tracks_dev_reserve", "bt_tracks_dev_reserve_ex", "bt_tracks_dev_update_pair", "bt_tracks_dev_propagate", "bt_tracks_dev_forget_frame", "bt_tracks_dev_stats", "bt_find_corres_pairs",
-    "bt_pose_init", "bt_tracker_create", "bt_tracker_destroy", "bt_tracker_begin_frame", "bt_tracker_begin_frame_u16", "bt_tracker_end_frame", "bt_tracker_drop_frame", "bt_tracker_state", "bt_tracker_usage", "bt_tracker_last_fg",
-    "bt_metrics_reserve", "bt_pose_metrics", "bt_vocap", "bt_nocs_reserve", "bt_nocs_metrics", "bt_nocs_score",
-    "bt_overlay_reserve", "bt_voxel_downsample", "bt_pose_overlay",
-    "bt_match_viz_shape", "bt_match_viz_reserve", "bt_match_viz",
-    "bt_dev_alloc", "bt_dev_free", "bt_memcpy_h2d", "bt_memcpy_d2h", "bt_host_alloc_pinned", "bt_host_free_pinned",
-    "bt_stream_sync", "bt_debug_live_resources",
-]
+# Every entry point of include/bundletrack_b200.h as (restype, argtypes), in the header's order; load() applies it, so a call site passes
+# plain Python values and ctypes converts each to the C type declared here (tests/test_abi.py checks the table against the header).
+# int / int32_t -> c_int, float -> c_float, double -> c_double, long long -> c_longlong, size_t -> c_size_t, uint64_t -> c_uint64, a pointer
+# to a struct mirrored above -> POINTER(<Structure>), any other pointer or handle -> c_void_p; bt_last_error's string -> c_char_p.
+_i, _f, _d, _ll, _sz, _u64, _p, _P = (ctypes.c_int, ctypes.c_float, ctypes.c_double, ctypes.c_longlong, ctypes.c_size_t, ctypes.c_uint64,
+                                     ctypes.c_void_p, ctypes.POINTER)
+PROTOTYPES = {
+    "bt_last_error": (ctypes.c_char_p, ()),
+    "bt_version": (_i, ()),
+    "bt_ctx_create": (_i, (_p, _i)),
+    "bt_ctx_destroy": (None, (_p,)),
+    "bt_solver_reserve": (_i, (_p, _P(SolverLimits))),
+    "bt_solve_windows": (_i, (_p, _i, _P(Window), _P(SolverParams), _p, _p)),
+    "bt_solve_windows_begin": (_i, (_p, _i, _P(Window), _P(SolverParams), _p, _p)),
+    "bt_solve_windows_end": (_i, (_p, _p)),
+    "bt_solve_stage": (_i, (_p, _i, _P(Window), _P(SolverParams), _p, _p)),
+    "bt_solve_run": (_i, (_p, _p)),
+    "bt_solve_fetch": (_i, (_p, _p, _p)),
+    "bt_solve_get_stats": (_i, (_p, _P(SolveStats))),
+    "bt_solve_enable_timing": (_i, (_p, _i)),
+    "bt_solve_get_timing": (_i, (_p, _p)),
+    "bt_solve_get_host_timing": (_i, (_p, _p)),
+    "bt_solve_enable_profile": (_i, (_p, _i)),
+    "bt_solve_get_profile": (_i, (_p, _p, _i)),
+    "bt_solve_enable_debug": (_i, (_p, _i)),
+    "bt_solve_debug_dense": (_i, (_p, _i, _p, _p)),
+    "bt_solve_debug_counts": (_i, (_p, _i, _i, _p)),
+    "bt_solve_debug_system": (_i, (_p, _i, _i, _p, _p, _p, _p)),
+    "bt_matcher_reserve": (_i, (_p, _i, _i, _i)),
+    "bt_knn_match_pairs": (_i, (_p, _i, _P(DescView), _P(DescView), _i, _p, _p, _p, _p, _p)),
+    "bt_desc_pool_reserve": (_i, (_p, _i)),
+    "bt_desc_pool_store": (_i, (_p, _i, _P(DescView), _p)),
+    "bt_knn_match_slots": (_i, (_p, _i, _p, _p, _i, _p, _p, _p, _p, _p)),
+    "bt_knn_enable_timing": (_i, (_p, _i)),
+    "bt_knn_debug_force_fallback": (_i, (_p, _i)),
+    "bt_knn_get_timing": (_i, (_p, _p, _p)),
+    "bt_ransac_reserve": (_i, (_p, _i, _i, _i)),
+    "bt_ransac_pairs": (_i, (_p, _i, _p, _p, _p, _i, _f, _u64, _p, _p, _p)),
+    "bt_ransac_debug": (_i, (_p, _p, _i, _p, _i)),
+    "bt_pipeline_reserve": (_i, (_p, _i, _i, _i, _i)),
+    "bt_prune_mutual_pairs": (_i, (_p, _i, _P(MatchFrame), _P(MatchFrame), _i, _i, _f, _f, _f, _f, _p, _p, _i, _P(PruneParams), _p, _p, _p)),
+    "bt_match_pairs": (_i, (_p, _i, _P(MatchFrame), _P(MatchFrame), _P(DescView), _P(DescView), _i, _i, _f, _f, _f, _f, _P(PruneParams), _i, _f, _u64, _p, _i, _p, _p, _p, _p)),
+    "bt_match_pairs_pool": (_i, (_p, _i, _P(MatchFrame), _P(MatchFrame), _p, _p, _i, _i, _f, _f, _f, _f, _P(PruneParams), _i, _f, _u64, _p, _i, _p, _p, _p, _p)),
+    "bt_match_pairs_ex": (_i, (_p, _i, _P(MatchFrame), _P(MatchFrame), _P(DescView), _P(DescView), _p, _p, _i, _i, _f, _f, _f, _f, _P(PruneParams), _i, _f, _u64, _P(MatchExtra), _p, _i, _p, _p, _p, _p, _p, _p)),
+    "bt_match_cache_reserve": (_i, (_p, _i, _i)),
+    "bt_match_cache_reserve_entries": (_i, (_p, _i, _ll)),
+    "bt_match_cache_usage": (_i, (_p, _p, _p)),
+    "bt_match_cache_put": (_i, (_p, _i, _p, _p, _p, _p, _p, _p, _p)),
+    "bt_match_cache_has": (_i, (_p, _i, _i)),
+    "bt_match_cache_status": (_i, (_p, _i, _i, _p, _p)),
+    "bt_match_cache_gather": (_i, (_p, _i, _p, _p, _p, _p, _p, _i, _p, _p, _p)),
+    "bt_match_cache_forget_frame": (_i, (_p, _i)),
+    "bt_frames_preprocess": (_i, (_p, _i, _p, _i, _i, _f, _f, _f, _f, _P(DepthParams), _p, _p, _p, _p)),
+    "bt_frames_preprocess_masked": (_i, (_p, _i, _p, _p, _i, _i, _i, _f, _f, _f, _f, _P(DepthParams), _p, _p, _p, _p, _p, _p)),
+    "bt_frames_preprocess_masked_u16": (_i, (_p, _i, _p, _p, _i, _i, _i, _f, _f, _f, _f, _P(DepthParams), _p, _p, _p, _p, _p, _p)),
+    "bt_lfnet_request": (_i, (_p, _i, _p, _p, _p, _i, _i, _p, _p)),
+    "bt_frame_cache_reserve": (_i, (_p, _i, _i, _i, _f)),
+    "bt_frame_cache_store": (_i, (_p, _i, _p, _p, _p, _i, _i, _f, _f, _f, _f, _f, _f, _p)),
+    "bt_rotation_geodesic": (_f, (_p, _p)),
+    "bt_keyframe_check": (_i, (_p, _i, _i, _p, _i, _i, _f)),
+    "bt_select_keyframes": (_i, (_p, _p, _i, _i, _p, _p)),
+    "bt_rigid_transform": (_i, (_p, _p, _i, _p)),
+    "bt_ba_gate": (_i, (_i, _i)),
+    "bt_pose_format": (_i, (_p, _p, _i)),
+    "bt_pose_write_txt": (_i, (_p, _p)),
+    "bt_lfnet_parse_reply": (_i, (_p, _sz, _p, _sz, _sz, _p, _p, _i, _p, _p)),
+    "bt_tracks_create": (_i, (_p,)),
+    "bt_tracks_destroy": (None, (_p,)),
+    "bt_tracks_update_pair": (_i, (_p, _i, _i, _p, _p, _i)),
+    "bt_tracks_propagate": (_i, (_p, _i, _i, _p, _i, _p, _i, _p)),
+    "bt_tracks_forget_frame": (_i, (_p, _i)),
+    "bt_tracks_stats": (_i, (_p, _p, _p)),
+    "bt_tracks_dev_reserve": (_i, (_p, _i, _i, _i)),
+    "bt_tracks_dev_reserve_ex": (_i, (_p, _i, _i, _i)),
+    "bt_tracks_dev_update_pair": (_i, (_p, _i, _i, _p, _p, _i, _p)),
+    "bt_tracks_dev_propagate": (_i, (_p, _i, _i, _p, _i, _p, _i, _p, _p)),
+    "bt_tracks_dev_forget_frame": (_i, (_p, _i, _p)),
+    "bt_tracks_dev_stats": (_i, (_p, _p, _p, _p)),
+    "bt_find_corres_pairs": (_i, (_p, _i, _P(MatchFrame), _P(MatchFrame), _P(DescView), _P(DescView), _p, _p, _i, _i, _f, _f, _f, _f, _P(PruneParams), _i, _f, _u64, _p, _i, _p, _p, _p, _p, _p, _p)),
+    "bt_pose_init": (_i, (_p, _p, _p, _p, _p, _p, _p, _p)),
+    "bt_tracker_create": (_i, (_p, _i, _P(TrackerParams))),
+    "bt_tracker_destroy": (None, (_p,)),
+    "bt_tracker_begin_frame": (_i, (_p, _i, _p, _p, _p, _p, _p, _p, _p, _p)),
+    "bt_tracker_begin_frame_u16": (_i, (_p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p)),
+    "bt_tracker_end_frame": (_i, (_p, _p, _i, _P(DescView), _p, _p, _p)),
+    "bt_tracker_drop_frame": (_i, (_p, _p)),
+    "bt_tracker_state": (_i, (_p, _p, _p, _p, _i, _p)),
+    "bt_tracker_usage": (_i, (_p, _p, _p, _p, _p)),
+    "bt_tracker_last_fg": (_i, (_p, _p)),
+    "bt_metrics_reserve": (_i, (_p, _i, _i)),
+    "bt_pose_metrics": (_i, (_p, _p, _i, _p, _p, _i, _p, _p, _p)),
+    "bt_vocap": (_i, (_p, _i, _d, _p)),
+    "bt_nocs_reserve": (_i, (_p, _i)),
+    "bt_nocs_metrics": (_i, (_p, _p, _p, _p, _p, _i, _p, _p, _p, _p)),
+    "bt_nocs_score": (_i, (_p, _p, _p, _p, _p, _i, _p, _p)),
+    "bt_voxel_downsample": (_i, (_p, _i, _p, _p, _f, _p, _p, _p)),
+    "bt_overlay_reserve": (_i, (_p, _i, _i)),
+    "bt_pose_overlay": (_i, (_p, _i, _p, _i, _p, _f, _f, _f, _f, _p, _p, _i, _i, _p, _p, _p)),
+    "bt_match_viz_shape": (_i, (_p, _p, _p, _p)),
+    "bt_match_viz_reserve": (_i, (_p, _i, _i)),
+    "bt_match_viz": (_i, (_p, _i, _P(MatchVizDesc), _p, _p)),
+    "bt_dev_alloc": (_i, (_p, _sz)),
+    "bt_dev_free": (_i, (_p,)),
+    "bt_memcpy_h2d": (_i, (_p, _p, _sz, _p)),
+    "bt_memcpy_d2h": (_i, (_p, _p, _sz, _p)),
+    "bt_host_alloc_pinned": (_i, (_p, _sz)),
+    "bt_host_free_pinned": (_i, (_p,)),
+    "bt_stream_sync": (_i, (_p,)),
+    "bt_debug_live_resources": (_i, (_p, _p, _p)),
+}
+EXPORTS = list(PROTOTYPES)
 
 _lib = None
 
@@ -188,15 +283,9 @@ def load() -> ctypes.CDLL:
             "(nvcc, sm_90a). bundletrack_b200 has no CPU fallback."
         )
     lib = ctypes.CDLL(LIB_PATH)
-    lib.bt_last_error.restype = ctypes.c_char_p
-    for name in EXPORTS:
+    for name, (restype, argtypes) in PROTOTYPES.items():
         fn = getattr(lib, name)
-        if name not in ("bt_last_error", "bt_ctx_destroy", "bt_rotation_geodesic", "bt_tracks_destroy", "bt_tracker_destroy"):
-            fn.restype = ctypes.c_int
-    lib.bt_ctx_destroy.restype = None
-    lib.bt_rotation_geodesic.restype = ctypes.c_float
-    lib.bt_tracks_destroy.restype = None
-    lib.bt_tracker_destroy.restype = None
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 
@@ -205,3 +294,83 @@ def check(rc: int, what: str = "") -> None:
     if rc != BT_OK:
         msg = load().bt_last_error().decode("utf-8", "replace")
         raise BtError(f"{what} failed with status {rc}: {msg}", rc)
+
+
+class Handle:
+    """A library object made by the entry point `create` (which writes it to its first argument) and freed once by `destroy`.  Pass it
+    straight to any lib.bt_* call: its _as_parameter_ is one c_void_p, which close() frees and sets to NULL in place.  Every holder of the
+    Handle then passes NULL, which the library refuses with BT_ERR_INVALID_ARG, instead of the freed address.  The object is freed when the
+    last holder lets the Handle go, or by close()."""
+
+    def __init__(self, create: str, destroy: str, *args):
+        self._as_parameter_ = ctypes.c_void_p()
+        lib = load()
+        self._destroy = getattr(lib, destroy)
+        check(getattr(lib, create)(ctypes.byref(self._as_parameter_), *args), create)
+
+    def close(self) -> None:
+        if self._as_parameter_:
+            self._destroy(self._as_parameter_)
+            self._as_parameter_.value = None
+
+    def __del__(self):
+        self.close()
+
+
+class Context(Handle):
+    """A bt_ctx on CUDA device `device`: the scratch every facade of the package works in."""
+
+    def __init__(self, device: int = 0):
+        super().__init__("bt_ctx_create", "bt_ctx_destroy", device)
+
+
+class Facade:
+    """Base of the objects that work on a context.  ctx=None makes a Context this object owns, and close() destroys it; a given Context is
+    shared, and close() only lets it go.  .ctx, .stream and .lib are valid arguments for raw lib.bt_* calls."""
+
+    def __init__(self, ctx=None, device: int = 0, stream: int = 0):
+        self.lib = load()
+        self.stream = ctypes.c_void_p(stream)
+        self._own = ctx is None
+        self.ctx = Context(device) if ctx is None else ctx
+
+    def close(self) -> None:
+        if self._own and self.ctx is not None:
+            self.ctx.close()
+        self.ctx = None
+
+
+# ---- marshalling: what every facade hands the library -------------------------------------------------------------------------------
+def ptr(x):
+    """The address argument of x: a tensor's data_ptr(), a numpy array as a c_void_p that keeps the array alive; anything else (None, an
+    int address, a Handle) as it is.  A tensor's address does not keep the tensor alive: hold it in a local across the call, and for an
+    asynchronous call until the stream has read it."""
+    if isinstance(x, np.ndarray):
+        return x.ctypes.data_as(ctypes.c_void_p)
+    return x.data_ptr() if hasattr(x, "data_ptr") else x
+
+
+def ptrs(xs) -> "ctypes.Array":
+    """A host array of the addresses of xs (tensors, ints or None), for the library's `T* const*` arguments."""
+    return (ctypes.c_void_p * len(xs))(*[ptr(x) for x in xs])
+
+
+def i32s(xs) -> "ctypes.Array":
+    return (ctypes.c_int32 * len(xs))(*[int(v) for v in xs])
+
+
+def intrinsics(K) -> tuple:
+    """(fx, fy, cx, cy) of a 3 x 3 camera matrix or of a 4-vector that already holds them."""
+    K = np.asarray(K, np.float64)
+    return tuple(float(v) for v in ((K[0, 0], K[1, 1], K[0, 2], K[1, 2]) if K.ndim == 2 else K))
+
+
+def prepared(fn, *args) -> tuple:
+    """fn's arguments with every Python number converted to its declared type once, for a call made many times with the same
+    arguments: ctypes passes an instance of the declared type without converting it again."""
+    return tuple(t(a) if isinstance(a, (int, float)) else a for t, a in zip(fn.argtypes, args))
+
+
+def desc_view(t) -> DescView:
+    """The bt_desc_view of a [n, dim] float32 CUDA tensor whose rows may be pitched (stride(1) == 1)."""
+    return DescView(t.data_ptr(), t.shape[0], t.shape[1], t.stride(0) * 4 if t.shape[0] > 1 else t.shape[1] * 4)

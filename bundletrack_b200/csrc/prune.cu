@@ -600,7 +600,8 @@ extern "C" int bt_match_cache_put(bt_ctx* ctx, int n_pairs, const int32_t* idA, 
 }
 
 extern "C" int bt_match_cache_has(bt_ctx* ctx, int idA, int idB) {
-	if (!ctx || !ctx->mcache) return 0;
+	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_match_cache_has: ctx is NULL");
+	if (!ctx->mcache) return 0;
 	return ctx->mcache->recs.count(std::make_pair(idA, idB)) ? 1 : 0;
 }
 

@@ -8,94 +8,64 @@ from typing import List, Sequence, Tuple
 from . import _lib
 
 
-class KnnMatcher:
+class _DescPool(_lib.Facade):
+    """The context's persistent descriptor pool: a frame's descriptors are converted once (Lfnet::detectFeature, FeatureManager.cpp:907)."""
+
+    def pool_reserve(self, n_slots: int):
+        _lib.check(self.lib.bt_desc_pool_reserve(self.ctx, n_slots), "bt_desc_pool_reserve")
+
+    def pool_store(self, slot: int, desc: "torch.Tensor"):
+        _lib.check(self.lib.bt_desc_pool_store(self.ctx, slot, _lib.desc_view(desc), self.stream), "bt_desc_pool_store")
+
+
+class KnnMatcher(_DescPool):
     """knnMatch(query, train, k) for many (A, B) pairs at once; ONE tensor-core contraction per pair serves both directions."""
 
     def __init__(self, device: int = 0, max_pairs: int = 64, max_feats: int = 4096, dim: int = 256, stream: int = 0, ctx=None):
-        self.lib = _lib.load()
-        self.stream = ctypes.c_void_p(stream)
-        self._own = ctx is None
-        self.ctx = ctypes.c_void_p() if ctx is None else ctx
-        if self._own:
-            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
-        _lib.check(self.lib.bt_matcher_reserve(self.ctx, ctypes.c_int(max_pairs), ctypes.c_int(max_feats), ctypes.c_int(dim)), "bt_matcher_reserve")
+        super().__init__(ctx, device, stream)
+        _lib.check(self.lib.bt_matcher_reserve(self.ctx, max_pairs, max_feats, dim), "bt_matcher_reserve")
         self.dim = dim
-
-    def close(self):
-        if self._own and self.ctx:
-            self.lib.bt_ctx_destroy(self.ctx)
-            self.ctx = ctypes.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def knn_match_pairs(self, pairs: Sequence[Tuple["torch.Tensor", "torch.Tensor"]], k: int = 5):
         """pairs: list of (A [nA,dim] fp32 cuda, B [nB,dim] fp32 cuda); rows may be pitched (stride(0) >= dim).
         Returns (idxAB, distAB, idxBA, distBA): lists (one entry per pair) of [n,k] int32 / float32 cuda tensors.
         distance = sqrt(sum (a-b)^2) ascending, ties -> lower train index (cv::DMatch semantics)."""
         import torch
+        for t in (t for p in pairs for t in p):
+            assert t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1
         n = len(pairs)
-        A = (_lib.DescView * n)()
-        B = (_lib.DescView * n)()
-        na = nb = 0
-        for i, (a, b) in enumerate(pairs):
-            for view, t in ((A[i], a), (B[i], b)):
-                assert t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1
-                view.dev, view.n, view.dim, view.pitch_bytes = t.data_ptr(), t.shape[0], t.shape[1], t.stride(0) * 4 if t.shape[0] > 1 else t.shape[1] * 4
-            na += a.shape[0]
-            nb += b.shape[0]
-        dev = pairs[0][0].device
-        idxAB = torch.empty((max(na, 1), k), dtype=torch.int32, device=dev)
-        distAB = torch.empty((max(na, 1), k), dtype=torch.float32, device=dev)
-        idxBA = torch.empty((max(nb, 1), k), dtype=torch.int32, device=dev)
-        distBA = torch.empty((max(nb, 1), k), dtype=torch.float32, device=dev)
-        _lib.check(self.lib.bt_knn_match_pairs(self.ctx, ctypes.c_int(n), A, B, ctypes.c_int(k),
-                                               ctypes.c_void_p(idxAB.data_ptr()), ctypes.c_void_p(distAB.data_ptr()),
-                                               ctypes.c_void_p(idxBA.data_ptr()), ctypes.c_void_p(distBA.data_ptr()), self.stream), "bt_knn_match_pairs")
-        oAB, oBA, ia, ib = [], [], 0, 0
-        for a, b in pairs:
-            oAB.append((idxAB[ia:ia + a.shape[0]], distAB[ia:ia + a.shape[0]]))
-            oBA.append((idxBA[ib:ib + b.shape[0]], distBA[ib:ib + b.shape[0]]))
-            ia += a.shape[0]
-            ib += b.shape[0]
-        return [x[0] for x in oAB], [x[1] for x in oAB], [x[0] for x in oBA], [x[1] for x in oBA]
-
-    # ---- persistent descriptor pool: a frame's descriptors are converted once (Lfnet::detectFeature, FeatureManager.cpp:907) ----
-    def pool_reserve(self, n_slots: int):
-        _lib.check(self.lib.bt_desc_pool_reserve(self.ctx, ctypes.c_int(n_slots)), "bt_desc_pool_reserve")
-
-    def pool_store(self, slot: int, desc: "torch.Tensor"):
-        v = _lib.DescView()
-        v.dev, v.n, v.dim, v.pitch_bytes = desc.data_ptr(), desc.shape[0], desc.shape[1], (desc.stride(0) * 4 if desc.shape[0] > 1 else desc.shape[1] * 4)
-        _lib.check(self.lib.bt_desc_pool_store(self.ctx, ctypes.c_int(slot), ctypes.byref(v), self.stream), "bt_desc_pool_store")
+        A = (_lib.DescView * n)(*[_lib.desc_view(a) for a, _ in pairs])
+        B = (_lib.DescView * n)(*[_lib.desc_view(b) for _, b in pairs])
+        return self._knn(self.lib.bt_knn_match_pairs, "bt_knn_match_pairs", A, B, [(a.shape[0], b.shape[0]) for a, b in pairs], k, pairs[0][0].device)
 
     def knn_match_slots(self, slot_pairs: Sequence[Tuple[int, int]], sizes: Sequence[Tuple[int, int]], k: int = 5, device=None):
         """slot_pairs: (slotA, slotB) per pair; sizes: (nA, nB) per pair (what was stored).  Same outputs as knn_match_pairs."""
         import torch
-        n = len(slot_pairs)
-        sa = (ctypes.c_int32 * n)(*[int(a) for a, _ in slot_pairs])
-        sb = (ctypes.c_int32 * n)(*[int(b) for _, b in slot_pairs])
+        sa, sb = _lib.i32s([a for a, _ in slot_pairs]), _lib.i32s([b for _, b in slot_pairs])
+        return self._knn(self.lib.bt_knn_match_slots, "bt_knn_match_slots", sa, sb, sizes, k, device or torch.device("cuda", torch.cuda.current_device()))
+
+    def _knn(self, fn, what, A, B, sizes, k, dev):
+        import torch
         na, nb = sum(a for a, _ in sizes), sum(b for _, b in sizes)
-        dev = device or torch.device("cuda", torch.cuda.current_device())
-        idxAB = torch.empty((max(na, 1), k), dtype=torch.int32, device=dev); distAB = torch.empty((max(na, 1), k), dtype=torch.float32, device=dev)
-        idxBA = torch.empty((max(nb, 1), k), dtype=torch.int32, device=dev); distBA = torch.empty((max(nb, 1), k), dtype=torch.float32, device=dev)
-        _lib.check(self.lib.bt_knn_match_slots(self.ctx, ctypes.c_int(n), sa, sb, ctypes.c_int(k), ctypes.c_void_p(idxAB.data_ptr()), ctypes.c_void_p(distAB.data_ptr()),
-                                               ctypes.c_void_p(idxBA.data_ptr()), ctypes.c_void_p(distBA.data_ptr()), self.stream), "bt_knn_match_slots")
+        idxAB = torch.empty((max(na, 1), k), dtype=torch.int32, device=dev)
+        distAB = torch.empty((max(na, 1), k), dtype=torch.float32, device=dev)
+        idxBA = torch.empty((max(nb, 1), k), dtype=torch.int32, device=dev)
+        distBA = torch.empty((max(nb, 1), k), dtype=torch.float32, device=dev)
+        _lib.check(fn(self.ctx, len(sizes), A, B, k, *(_lib.ptr(t) for t in (idxAB, distAB, idxBA, distBA)), self.stream), what)
         oAB, oBA, ia, ib = [], [], 0, 0
         for a, b in sizes:
-            oAB.append((idxAB[ia:ia + a], distAB[ia:ia + a])); oBA.append((idxBA[ib:ib + b], distBA[ib:ib + b]))
-            ia += a; ib += b
+            oAB.append((idxAB[ia:ia + a], distAB[ia:ia + a]))
+            oBA.append((idxBA[ib:ib + b], distBA[ib:ib + b]))
+            ia += a
+            ib += b
         return [x[0] for x in oAB], [x[1] for x in oAB], [x[0] for x in oBA], [x[1] for x in oBA]
 
     def force_fallback(self, every_nth: int):
         """Test knob: every n-th query row goes through the exact brute-force kernel (0 = off)."""
-        _lib.check(self.lib.bt_knn_debug_force_fallback(self.ctx, ctypes.c_int(every_nth)), "bt_knn_debug_force_fallback")
+        _lib.check(self.lib.bt_knn_debug_force_fallback(self.ctx, every_nth), "bt_knn_debug_force_fallback")
 
     def enable_timing(self, on=True):
-        _lib.check(self.lib.bt_knn_enable_timing(self.ctx, ctypes.c_int(1 if on else 0)), "bt_knn_enable_timing")
+        _lib.check(self.lib.bt_knn_enable_timing(self.ctx, 1 if on else 0), "bt_knn_enable_timing")
 
     def timing(self):
         ms = (ctypes.c_float * 4)()
@@ -104,37 +74,24 @@ class KnnMatcher:
         return {"prep_ms": ms[0], "tc_ms": ms[1], "rerank_ms": ms[2], "fallback_ms": ms[3], "units": info[0], "rows": info[1], "fallback_rows": info[2]}
 
 
-class Ransac:
+class Ransac(_lib.Facade):
     """ransacMultiPairGPU (/root/reference/src/cuda/cuda_ransac.h:50) for a batch of pairs."""
 
     def __init__(self, device: int = 0, max_pairs: int = 64, max_pts: int = 8192, max_trials: int = 2000, stream: int = 0, ctx=None):
-        self.lib = _lib.load()
-        self.stream = ctypes.c_void_p(stream)
-        self._own = ctx is None
-        self.ctx = ctypes.c_void_p() if ctx is None else ctx
-        if self._own:
-            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
-        _lib.check(self.lib.bt_ransac_reserve(self.ctx, ctypes.c_int(max_pairs), ctypes.c_int(max_pts), ctypes.c_int(max_trials)), "bt_ransac_reserve")
+        super().__init__(ctx, device, stream)
+        _lib.check(self.lib.bt_ransac_reserve(self.ctx, max_pairs, max_pts, max_trials), "bt_ransac_reserve")
         self.max_trials = max_trials
-
-    def close(self):
-        if self._own and self.ctx:
-            self.lib.bt_ctx_destroy(self.ctx)
-            self.ctx = ctypes.c_void_p()
 
     def ransac_pairs(self, ptsA: List["torch.Tensor"], ptsB: List["torch.Tensor"], n_trials: int, dist_thresh: float, seed: int = 0):
         """ptsA[p], ptsB[p]: [n_p,4] float32 cuda (w ignored).  Returns list of int32 cuda tensors of inlier ids (ascending)."""
         import torch
         n = len(ptsA)
-        pa = (ctypes.c_void_p * n)(*[t.data_ptr() for t in ptsA])
-        pb = (ctypes.c_void_p * n)(*[t.data_ptr() for t in ptsB])
-        cnt = (ctypes.c_int * n)(*[t.shape[0] for t in ptsA])
         total = sum(t.shape[0] for t in ptsA)
         dev = ptsA[0].device
         ids = torch.empty(max(total, 1), dtype=torch.int32, device=dev)
         nin = torch.empty(n, dtype=torch.int32, device=dev)
-        _lib.check(self.lib.bt_ransac_pairs(self.ctx, ctypes.c_int(n), pa, pb, cnt, ctypes.c_int(n_trials), ctypes.c_float(dist_thresh), ctypes.c_uint64(seed),
-                                            ctypes.c_void_p(ids.data_ptr()), ctypes.c_void_p(nin.data_ptr()), self.stream), "bt_ransac_pairs")
+        _lib.check(self.lib.bt_ransac_pairs(self.ctx, n, _lib.ptrs(ptsA), _lib.ptrs(ptsB), _lib.i32s([t.shape[0] for t in ptsA]), n_trials, dist_thresh, seed,
+                                            _lib.ptr(ids), _lib.ptr(nin), self.stream), "bt_ransac_pairs")
         nin_h = nin.cpu().numpy()
         out, o = [], 0
         for p in range(n):
@@ -146,33 +103,25 @@ class Ransac:
         import numpy as np
         u3 = np.zeros((n_trials, 3), np.float32)
         bt = np.zeros(n_pairs, np.int32)
-        _lib.check(self.lib.bt_ransac_debug(self.ctx, u3.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(n_trials), bt.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(n_pairs)), "bt_ransac_debug")
+        _lib.check(self.lib.bt_ransac_debug(self.ctx, _lib.ptr(u3), n_trials, _lib.ptr(bt), n_pairs), "bt_ransac_debug")
         return u3, bt
 
 
-class MatchPipeline:
+class MatchPipeline(_DescPool):
     """The matcher half of the hot path, device-resident: SiftManager::findCorres for a batch of frame pairs
     (kNN both directions -> pruneMatches -> collectMutualMatches -> runRansacBetween) ending in the EntryJ records
     Bundler::optimizeGPU would build (/root/reference/src/FeatureManager.cpp:173-368,561-741; src/Bundler.cpp:298-324)."""
 
-    def __init__(self, yml=None, device: int = 0, max_pairs: int = 64, max_feats: int = 4096, dim: int = 256, stream: int = 0):
+    def __init__(self, yml=None, device: int = 0, max_pairs: int = 64, max_feats: int = 4096, dim: int = 256, stream: int = 0, ctx=None):
         from .config import load_yml, prune_params
-        self.lib = _lib.load()
-        self.stream = ctypes.c_void_p(stream)
-        self.ctx = ctypes.c_void_p()
-        _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
+        super().__init__(ctx, device, stream)
         y = load_yml(yml)
         rs = y["ransac"]
         self.prune = prune_params(y)
         self.ransac_trials = int(rs["max_iter"])
         self.ransac_inlier_dist = float(rs["inlier_dist"])
-        _lib.check(self.lib.bt_pipeline_reserve(self.ctx, ctypes.c_int(max_pairs), ctypes.c_int(max_feats), ctypes.c_int(dim), ctypes.c_int(max(self.ransac_trials, 1))), "bt_pipeline_reserve")
+        _lib.check(self.lib.bt_pipeline_reserve(self.ctx, max_pairs, max_feats, dim, max(self.ransac_trials, 1)), "bt_pipeline_reserve")
         self.max_pairs, self.max_feats = max_pairs, max_feats
-
-    def close(self):
-        if self.ctx:
-            self.lib.bt_ctx_destroy(self.ctx)
-            self.ctx = ctypes.c_void_p()
 
     @staticmethod
     def _frame(fr) -> "_lib.MatchFrame":
@@ -189,15 +138,11 @@ class MatchPipeline:
 
     def _views(self, pairs):
         n = len(pairs)
-        A = (_lib.MatchFrame * n)()
-        B = (_lib.MatchFrame * n)()
-        dA = (_lib.DescView * n)()
-        dB = (_lib.DescView * n)()
-        for i, (fa, fb) in enumerate(pairs):
-            A[i], B[i] = self._frame(fa), self._frame(fb)
-            for view, t in ((dA[i], fa.get("desc")), (dB[i], fb.get("desc"))):
-                if t is not None:      # (frames whose descriptors live in the pool need no view)
-                    view.dev, view.n, view.dim, view.pitch_bytes = t.data_ptr(), t.shape[0], t.shape[1], (t.stride(0) * 4 if t.shape[0] > 1 else t.shape[1] * 4)
+        A = (_lib.MatchFrame * n)(*[self._frame(fa) for fa, _ in pairs])
+        B = (_lib.MatchFrame * n)(*[self._frame(fb) for _, fb in pairs])
+        # (frames whose descriptors live in the pool need no view)
+        dA = (_lib.DescView * n)(*[_lib.desc_view(fa["desc"]) if fa.get("desc") is not None else _lib.DescView() for fa, _ in pairs])
+        dB = (_lib.DescView * n)(*[_lib.desc_view(fb["desc"]) if fb.get("desc") is not None else _lib.DescView() for _, fb in pairs])
         return A, B, dA, dB
 
     def prune_mutual(self, pairs, idxAB, idxBA, H, W, K, k=5):
@@ -210,24 +155,14 @@ class MatchPipeline:
         dev = pairs[0][0]["kpts"].device
         corr = torch.empty((max(cap, 1), 10), dtype=torch.float32, device=dev)
         cnt = torch.empty(n, dtype=torch.int32, device=dev)
-        _lib.check(self.lib.bt_prune_mutual_pairs(self.ctx, ctypes.c_int(n), A, B, ctypes.c_int(H), ctypes.c_int(W),
-                                                  ctypes.c_float(K[0]), ctypes.c_float(K[1]), ctypes.c_float(K[2]), ctypes.c_float(K[3]),
-                                                  ctypes.c_void_p(idxAB.data_ptr()), ctypes.c_void_p(idxBA.data_ptr()), ctypes.c_int(k), ctypes.byref(self.prune),
-                                                  ctypes.c_void_p(corr.data_ptr()), ctypes.c_void_p(cnt.data_ptr()), self.stream), "bt_prune_mutual_pairs")
+        _lib.check(self.lib.bt_prune_mutual_pairs(self.ctx, n, A, B, H, W, *_lib.intrinsics(K), _lib.ptr(idxAB), _lib.ptr(idxBA), k, self.prune,
+                                                  _lib.ptr(corr), _lib.ptr(cnt), self.stream), "bt_prune_mutual_pairs")
         ch = cnt.cpu().numpy()
         out, o = [], 0
         for p, (fa, fb) in enumerate(pairs):
             out.append(corr[o:o + int(ch[p])])
             o += fa["kpts"].shape[0] + fb["kpts"].shape[0]
         return out
-
-    def pool_reserve(self, n_slots: int):
-        _lib.check(self.lib.bt_desc_pool_reserve(self.ctx, ctypes.c_int(n_slots)), "bt_desc_pool_reserve")
-
-    def pool_store(self, slot: int, desc: "torch.Tensor"):
-        v = _lib.DescView()
-        v.dev, v.n, v.dim, v.pitch_bytes = desc.data_ptr(), desc.shape[0], desc.shape[1], (desc.stride(0) * 4 if desc.shape[0] > 1 else desc.shape[1] * 4)
-        _lib.check(self.lib.bt_desc_pool_store(self.ctx, ctypes.c_int(slot), ctypes.byref(v), self.stream), "bt_desc_pool_store")
 
     def match_pairs(self, pairs, H, W, K, seed: int = 0, capacity: int = 0, keep_on_device: bool = False, slots=None):
         """Fused pipeline.  slots: optional list of (slotA, slotB) naming descriptor sets stored with pool_store (the frames' "desc" entries
@@ -245,15 +180,13 @@ class MatchPipeline:
         n_ent = torch.empty(n, dtype=torch.int32, device=dev)
         off = torch.empty(n, dtype=torch.int32, device=dev)
         tot = torch.zeros(4, dtype=torch.int32, device=dev)
-        tail = (ctypes.c_int(H), ctypes.c_int(W), ctypes.c_float(K[0]), ctypes.c_float(K[1]), ctypes.c_float(K[2]), ctypes.c_float(K[3]),
-                ctypes.byref(self.prune), ctypes.c_int(self.ransac_trials), ctypes.c_float(self.ransac_inlier_dist), ctypes.c_uint64(seed),
-                ctypes.c_void_p(ent.data_ptr()), ctypes.c_int(cap), ctypes.c_void_p(n_ent.data_ptr()), ctypes.c_void_p(off.data_ptr()),
-                ctypes.c_void_p(tot.data_ptr()), self.stream)
+        tail = (H, W, *_lib.intrinsics(K), self.prune, self.ransac_trials, self.ransac_inlier_dist, seed,
+                _lib.ptr(ent), cap, _lib.ptr(n_ent), _lib.ptr(off), _lib.ptr(tot), self.stream)
         if slots is None:
-            _lib.check(self.lib.bt_match_pairs(self.ctx, ctypes.c_int(n), A, B, dA, dB, *tail), "bt_match_pairs")
+            _lib.check(self.lib.bt_match_pairs(self.ctx, n, A, B, dA, dB, *tail), "bt_match_pairs")
         else:
-            sa = (ctypes.c_int32 * n)(*[int(a) for a, _ in slots]); sb = (ctypes.c_int32 * n)(*[int(b) for _, b in slots])
-            _lib.check(self.lib.bt_match_pairs_pool(self.ctx, ctypes.c_int(n), A, B, sa, sb, *tail), "bt_match_pairs_pool")
+            _lib.check(self.lib.bt_match_pairs_pool(self.ctx, n, A, B, _lib.i32s([a for a, _ in slots]), _lib.i32s([b for _, b in slots]), *tail),
+                       "bt_match_pairs_pool")
         self.last = (ent, n_ent, off, tot)
         if keep_on_device:
             cnt = torch.stack([n_ent, off]).cpu().numpy()      # one small D2H (2 x n_pairs ints), no entry leaves the device
@@ -272,7 +205,7 @@ class MatchPipeline:
         return np.asarray(entry_off, np.int32), np.asarray(n_entry, np.int32), bi, bj
 
 
-class DeviceTracks:
+class DeviceTracks(_lib.Facade):
     """The map-point table on the device (bt_tracks_dev_*), owned by a context: the methods of policy.Tracks with the same results,
     host arrays in and out.  FindCorres keeps one; bt_find_corres_pairs reads and updates it without leaving the device.
     Capacities: frames alive (<= 64 + 1024, bt_tracks_dev_reserve_ex), keys per frame (<= 8192), map points alive (default
@@ -281,27 +214,10 @@ class DeviceTracks:
     All work, including the uploads and read-backs of the methods below, runs on `stream`."""
 
     def __init__(self, ctx=None, device: int = 0, max_frames: int = 64, max_keys_per_frame: int = 4096, max_points: int = 0, stream: int = 0):
-        self.lib = _lib.load()
-        self.stream = ctypes.c_void_p(stream)
-        self._own = ctx is None
-        self.ctx = ctypes.c_void_p() if ctx is None else ctx
-        if self._own:
-            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
+        super().__init__(ctx, device, stream)
         self.device = device
         max_points = max_points or 16 * max_keys_per_frame * -(-max_frames // 64)
-        _lib.check(self.lib.bt_tracks_dev_reserve_ex(self.ctx, ctypes.c_int(max_frames), ctypes.c_int(max_keys_per_frame), ctypes.c_int(max_points)),
-                   "bt_tracks_dev_reserve_ex")
-
-    def close(self):
-        if self._own and self.ctx:
-            self.lib.bt_ctx_destroy(self.ctx)
-            self.ctx = ctypes.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        _lib.check(self.lib.bt_tracks_dev_reserve_ex(self.ctx, max_frames, max_keys_per_frame, max_points), "bt_tracks_dev_reserve_ex")
 
     def _on_stream(self):
         """torch work (allocation, upload, read-back) on the table's stream: the kernels then see the uploads complete, the read-backs
@@ -322,8 +238,8 @@ class DeviceTracks:
         with self._on_stream():
             d_uv = torch.from_numpy(uv).to(dev) if len(uv) else torch.zeros((1, 4), dtype=torch.float32, device=dev)
             d_n = torch.tensor([len(uv)], dtype=torch.int32, device=dev)
-            _lib.check(self.lib.bt_tracks_dev_update_pair(self.ctx, ctypes.c_int(frame_a), ctypes.c_int(frame_b), ctypes.c_void_p(d_uv.data_ptr()),
-                                                          ctypes.c_void_p(d_n.data_ptr()), ctypes.c_int(len(uv)), self.stream), "bt_tracks_dev_update_pair")
+            _lib.check(self.lib.bt_tracks_dev_update_pair(self.ctx, frame_a, frame_b, _lib.ptr(d_uv), _lib.ptr(d_n), len(uv), self.stream),
+                       "bt_tracks_dev_update_pair")
 
     def propagate(self, frame_a: int, frame_b: int, existing_uv, capacity: int = 65536):
         import numpy as np
@@ -334,15 +250,14 @@ class DeviceTracks:
             d_ex = torch.from_numpy(ex).to(dev) if len(ex) else None
             out = torch.empty((max(capacity, 1), 4), dtype=torch.float32, device=dev)
             n = torch.zeros(1, dtype=torch.int32, device=dev)
-            _lib.check(self.lib.bt_tracks_dev_propagate(self.ctx, ctypes.c_int(frame_a), ctypes.c_int(frame_b), None if d_ex is None else ctypes.c_void_p(d_ex.data_ptr()),
-                                                        ctypes.c_int(len(ex)), ctypes.c_void_p(out.data_ptr()), ctypes.c_int(capacity), ctypes.c_void_p(n.data_ptr()),
-                                                        self.stream), "bt_tracks_dev_propagate")
+            _lib.check(self.lib.bt_tracks_dev_propagate(self.ctx, frame_a, frame_b, _lib.ptr(d_ex), len(ex), _lib.ptr(out), capacity, _lib.ptr(n), self.stream),
+                       "bt_tracks_dev_propagate")
             self.stats()                # synchronises the stream; a propagation longer than `capacity` is an error, as on the host
             k = int(n.item())
             return out[:k].cpu().numpy()
 
     def forget_frame(self, frame: int):
-        _lib.check(self.lib.bt_tracks_dev_forget_frame(self.ctx, ctypes.c_int(frame), self.stream), "bt_tracks_dev_forget_frame")
+        _lib.check(self.lib.bt_tracks_dev_forget_frame(self.ctx, frame, self.stream), "bt_tracks_dev_forget_frame")
 
     def stats(self):
         a, b = ctypes.c_int(0), ctypes.c_int(0)
@@ -366,14 +281,16 @@ class FindCorres:
         self.tracks = DeviceTracks(ctx=pipeline.ctx, max_frames=max_frames, max_keys_per_frame=pipeline.max_feats, max_points=max_points, stream=pipeline.stream.value or 0)
         self.slot_entries = max_entries_per_pair or 3 * pipeline.max_feats
         if max_entries_total is None:
-            _lib.check(self.lib.bt_match_cache_reserve(self.ctx, ctypes.c_int(max_pairs_cached), ctypes.c_int(self.slot_entries)), "bt_match_cache_reserve")
+            _lib.check(self.lib.bt_match_cache_reserve(self.ctx, max_pairs_cached, self.slot_entries), "bt_match_cache_reserve")
         else:
-            _lib.check(self.lib.bt_match_cache_reserve_entries(self.ctx, ctypes.c_int(max_pairs_cached), ctypes.c_longlong(max_entries_total)),
-                       "bt_match_cache_reserve_entries")
+            _lib.check(self.lib.bt_match_cache_reserve_entries(self.ctx, max_pairs_cached, max_entries_total), "bt_match_cache_reserve_entries")
         self.failed = set()          # ids of frames the reference would mark Frame::FAIL
 
     def has(self, id_a: int, id_b: int) -> bool:
-        return bool(self.lib.bt_match_cache_has(self.ctx, ctypes.c_int(id_a), ctypes.c_int(id_b)))
+        rc = self.lib.bt_match_cache_has(self.ctx, id_a, id_b)
+        if rc < 0:
+            _lib.check(rc, "bt_match_cache_has")
+        return bool(rc)
 
     def find_corres(self, pairs, slots, H, W, K, seed: int = 0):
         """pairs: list of (frameA newer, frameB older) dicts as for MatchPipeline.match_pairs; slots: their descriptor-pool slots.
@@ -396,19 +313,15 @@ class FindCorres:
         ent = torch.empty((max(cap, 1), 8), dtype=torch.int32, device=dev)
         meta = torch.zeros((3, n), dtype=torch.int32, device=dev)              # n_entry, entry_off, status
         tot = torch.zeros(4, dtype=torch.int32, device=dev)
-        sa = (ctypes.c_int32 * n)(*[int(a) for a, _ in sl]); sb = (ctypes.c_int32 * n)(*[int(b) for _, b in sl])
         mp = self.mp
-        _lib.check(self.lib.bt_find_corres_pairs(self.ctx, ctypes.c_int(n), A, B, None, None, sa, sb, ctypes.c_int(H), ctypes.c_int(W),
-                                                 ctypes.c_float(K[0]), ctypes.c_float(K[1]), ctypes.c_float(K[2]), ctypes.c_float(K[3]), ctypes.byref(mp.prune),
-                                                 ctypes.c_int(mp.ransac_trials), ctypes.c_float(mp.ransac_inlier_dist), ctypes.c_uint64(seed),
-                                                 ctypes.c_void_p(ent.data_ptr()), ctypes.c_int(cap), ctypes.c_void_p(meta[0].data_ptr()), ctypes.c_void_p(meta[1].data_ptr()),
-                                                 ctypes.c_void_p(tot.data_ptr()), ctypes.c_void_p(meta[2].data_ptr()), None, mp.stream), "bt_find_corres_pairs")
+        _lib.check(self.lib.bt_find_corres_pairs(self.ctx, n, A, B, None, None, _lib.i32s([a for a, _ in sl]), _lib.i32s([b for _, b in sl]), H, W,
+                                                 *_lib.intrinsics(K), mp.prune, mp.ransac_trials, mp.ransac_inlier_dist, seed, _lib.ptr(ent), cap,
+                                                 _lib.ptr(meta[0]), _lib.ptr(meta[1]), _lib.ptr(tot), _lib.ptr(meta[2]), None, mp.stream), "bt_find_corres_pairs")
         m = meta.cpu().numpy()                                                  # 3 x n ints: the call's only read-back
         self.tracks.stats()                                                     # (the stream is idle: raises if the table ran out of room)
-        ida = (ctypes.c_int32 * n)(*[int(a["id"]) for a, _ in prs]); idb = (ctypes.c_int32 * n)(*[int(b["id"]) for _, b in prs])
         n_h = np.ascontiguousarray(m[0]); off_h = np.ascontiguousarray(m[1]); st_h = np.ascontiguousarray(m[2])
-        _lib.check(self.lib.bt_match_cache_put(self.ctx, ctypes.c_int(n), ida, idb, ctypes.c_void_p(ent.data_ptr()), n_h.ctypes.data_as(ctypes.c_void_p),
-                                               off_h.ctypes.data_as(ctypes.c_void_p), st_h.ctypes.data_as(ctypes.c_void_p), mp.stream), "bt_match_cache_put")
+        _lib.check(self.lib.bt_match_cache_put(self.ctx, n, _lib.i32s([a["id"] for a, _ in prs]), _lib.i32s([b["id"] for _, b in prs]), _lib.ptr(ent),
+                                               _lib.ptr(n_h), _lib.ptr(off_h), _lib.ptr(st_h), mp.stream), "bt_match_cache_put")
         out = {}
         for i, (a, b) in enumerate(prs):
             if st_h[i] == 2:
@@ -424,16 +337,14 @@ class FindCorres:
         import torch
         prs = [(frames[j]["id"], frames[i]["id"], i, j) for i in range(len(frames)) for j in range(i + 1, len(frames))]
         n = len(prs)
-        ida = (ctypes.c_int32 * n)(*[p[0] for p in prs]); idb = (ctypes.c_int32 * n)(*[p[1] for p in prs])
         wi = np.array([p[2] for p in prs], np.uint32); wj = np.array([p[3] for p in prs], np.uint32)
         cap = n * self.slot_entries
         dst = torch.empty((max(min(cap, 1 << 22), 1), 8), dtype=torch.int32, device=device)
         off = np.zeros(n, np.int32); cnt = np.zeros(n, np.int32)
-        _lib.check(self.lib.bt_match_cache_gather(self.ctx, ctypes.c_int(n), ida, idb, wi.ctypes.data_as(ctypes.c_void_p), wj.ctypes.data_as(ctypes.c_void_p),
-                                                  ctypes.c_void_p(dst.data_ptr()), ctypes.c_int(dst.shape[0]), off.ctypes.data_as(ctypes.c_void_p), cnt.ctypes.data_as(ctypes.c_void_p),
-                                                  self.mp.stream), "bt_match_cache_gather")
+        _lib.check(self.lib.bt_match_cache_gather(self.ctx, n, _lib.i32s([p[0] for p in prs]), _lib.i32s([p[1] for p in prs]), _lib.ptr(wi), _lib.ptr(wj),
+                                                  _lib.ptr(dst), dst.shape[0], _lib.ptr(off), _lib.ptr(cnt), self.mp.stream), "bt_match_cache_gather")
         return dst, (off, cnt, wi, wj)
 
     def forget_frame(self, frame_id: int):
-        _lib.check(self.lib.bt_match_cache_forget_frame(self.ctx, ctypes.c_int(frame_id)), "bt_match_cache_forget_frame")
+        _lib.check(self.lib.bt_match_cache_forget_frame(self.ctx, frame_id), "bt_match_cache_forget_frame")
         self.tracks.forget_frame(frame_id)

@@ -20,7 +20,7 @@ def vocap(err, max_err: float = 0.1) -> float:
     """Area under the accuracy-threshold curve of the errors up to max_err, divided by max_err (the paper's tables print it x 100)."""
     e = np.ascontiguousarray(np.asarray(err, np.float64).reshape(-1))
     out = ctypes.c_double(0.0)
-    _lib.check(_lib.load().bt_vocap(e.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(e.size), ctypes.c_double(max_err), ctypes.byref(out)), "bt_vocap")
+    _lib.check(_lib.load().bt_vocap(_lib.ptr(e), e.size, max_err, ctypes.byref(out)), "bt_vocap")
     return out.value
 
 
@@ -31,29 +31,13 @@ def _poses(p, what: str) -> np.ndarray:
     return a.reshape(-1, 4, 4)
 
 
-class PoseMetrics:
+class PoseMetrics(_lib.Facade):
     """ADD / ADD-S of many frames in one device call.  Scratch for max_pts model points and max_frames frames per call is reserved here."""
 
     def __init__(self, max_pts: int, max_frames: int, device: int = 0, stream: int = 0, ctx=None):
-        self.lib = _lib.load()
-        self.stream = ctypes.c_void_p(stream)
+        super().__init__(ctx, device, stream)
         self.device = device
-        self._own = ctx is None
-        self.ctx = ctypes.c_void_p() if ctx is None else ctx
-        if self._own:
-            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
-        _lib.check(self.lib.bt_metrics_reserve(self.ctx, ctypes.c_int(max_pts), ctypes.c_int(max_frames)), "bt_metrics_reserve")
-
-    def close(self):
-        if self._own and self.ctx:
-            self.lib.bt_ctx_destroy(self.ctx)
-            self.ctx = ctypes.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        _lib.check(self.lib.bt_metrics_reserve(self.ctx, max_pts, max_frames), "bt_metrics_reserve")
 
     def __call__(self, model_pts, pred, gt):
         """model_pts: [N,3] float64 (numpy, or a CUDA tensor kept on the device between calls); pred, gt: [F,4,4] ob_in_cam.
@@ -68,9 +52,8 @@ class PoseMetrics:
         F = len(P)
         add = torch.empty(F, dtype=torch.float64, device=dev)
         adds = torch.empty(F, dtype=torch.float64, device=dev)
-        _lib.check(self.lib.bt_pose_metrics(self.ctx, ctypes.c_void_p(pts.data_ptr()), ctypes.c_int(pts.shape[0]), P.ctypes.data_as(ctypes.c_void_p),
-                                            G.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(F), ctypes.c_void_p(add.data_ptr()),
-                                            ctypes.c_void_p(adds.data_ptr()), self.stream), "bt_pose_metrics")
+        _lib.check(self.lib.bt_pose_metrics(self.ctx, _lib.ptr(pts), pts.shape[0], _lib.ptr(P), _lib.ptr(G), F, _lib.ptr(add), _lib.ptr(adds), self.stream),
+                   "bt_pose_metrics")
         _lib.check(self.lib.bt_stream_sync(self.stream), "bt_stream_sync")
         return add.cpu().numpy(), adds.cpu().numpy()
 
@@ -106,29 +89,13 @@ def _f64(a, n: int, what: str) -> np.ndarray:
     return v
 
 
-class NocsMetrics:
+class NocsMetrics(_lib.Facade):
     """theta (degrees), shift (mm) and IoU of many NOCS records in one device call (bt_nocs_metrics); room for max_records per call."""
 
     def __init__(self, max_records: int, device: int = 0, stream: int = 0, ctx=None):
-        self.lib = _lib.load()
-        self.stream = ctypes.c_void_p(stream)
+        super().__init__(ctx, device, stream)
         self.device = device
-        self._own = ctx is None
-        self.ctx = ctypes.c_void_p() if ctx is None else ctx
-        if self._own:
-            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
-        _lib.check(self.lib.bt_nocs_reserve(self.ctx, ctypes.c_int(max_records)), "bt_nocs_reserve")
-
-    def close(self):
-        if self._own and self.ctx:
-            self.lib.bt_ctx_destroy(self.ctx)
-            self.ctx = ctypes.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        _lib.check(self.lib.bt_nocs_reserve(self.ctx, max_records), "bt_nocs_reserve")
 
     def __call__(self, pred, gt, corners, symmetric):
         """pred, gt: [N,4,4] with translations in mm, as the benchmark compares them; corners: [N,8,3] (or [8,3] for all); symmetric: [N]
@@ -145,9 +112,8 @@ class NocsMetrics:
         C = _f64(C, 24 * N, "corners")
         S = _i32(symmetric, N, "symmetric")
         out = torch.empty((3, N), dtype=torch.float64, device=dev)
-        _lib.check(self.lib.bt_nocs_metrics(self.ctx, P.ctypes.data_as(ctypes.c_void_p), G.ctypes.data_as(ctypes.c_void_p), C.ctypes.data_as(ctypes.c_void_p),
-                                            S.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(N), ctypes.c_void_p(out[0].data_ptr()),
-                                            ctypes.c_void_p(out[1].data_ptr()), ctypes.c_void_p(out[2].data_ptr()), self.stream), "bt_nocs_metrics")
+        _lib.check(self.lib.bt_nocs_metrics(self.ctx, _lib.ptr(P), _lib.ptr(G), _lib.ptr(C), _lib.ptr(S), N, *(_lib.ptr(o) for o in out), self.stream),
+                   "bt_nocs_metrics")
         _lib.check(self.lib.bt_stream_sync(self.stream), "bt_stream_sync")
         o = out.cpu().numpy()
         return o[0].copy(), o[1].copy(), o[2].copy()
@@ -172,6 +138,6 @@ def nocs_score(cls, scored, theta_deg, shift, iou):
     t, d, u = _f64(theta_deg, n, "theta_deg"), _f64(shift, n, "shift"), _f64(iou, n, "iou")
     per = np.zeros((6, 4), np.float64)
     ov = np.zeros(4, np.float64)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    _lib.check(_lib.load().bt_nocs_score(p(c), p(s), p(t), p(d), p(u), ctypes.c_int(n), p(per), p(ov)), "bt_nocs_score")
+    p = _lib.ptr
+    _lib.check(_lib.load().bt_nocs_score(p(c), p(s), p(t), p(d), p(u), n, p(per), p(ov)), "bt_nocs_score")
     return per, ov

@@ -18,13 +18,6 @@ from .config import solver_params
 from .synth import ENTRYJ_DTYPE
 
 
-def _ptr(x) -> int:
-    """Device pointer of a torch tensor / anything with data_ptr(), or a raw integer address."""
-    if hasattr(x, "data_ptr"):
-        return int(x.data_ptr())
-    return int(x)
-
-
 class SolveWindow:
     """One window's inputs: device frame maps + host correspondences/poses (the reference's argument list)."""
 
@@ -38,11 +31,10 @@ class SolveWindow:
         # host correspondences: optional per-pair counts (Bundler::optimizeGPU's n_match_per_pair): the library then skips its grouping pass
         self.corr_block_n = None if corr_block_n is None else np.ascontiguousarray(corr_block_n, np.int32)
         self.H, self.W = int(H), int(W)
-        self.depths = [_ptr(d) for d in (depths_gpu or [])]
-        self.normals = [_ptr(n) for n in (normals_gpu or [])]
+        self.depths = [_lib.ptr(d) for d in (depths_gpu or [])]
+        self.normals = [_lib.ptr(n) for n in (normals_gpu or [])]
         self.poses = np.ascontiguousarray(poses, np.float32).reshape(-1, 4, 4)
-        K = np.asarray(K, np.float64)
-        self.K = (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])) if K.ndim == 2 else tuple(float(v) for v in K)
+        self.K = _lib.intrinsics(K)
         self.dense_pairs = None if dense_pairs is None else np.ascontiguousarray(dense_pairs, np.uint32).reshape(-1, 2)
         self.compat_flip = bool(compat_flip)
         self.cache_slots = None if cache_slots is None else np.ascontiguousarray(cache_slots, np.int32)
@@ -83,7 +75,7 @@ class SolveWindow:
                 cw.cache_slots = self.cache_slots.ctypes.data
             if self.corr_dev is not None:
                 off, nb, bi, bj = self.blocks
-                cw.corr_dev = _ptr(self.corr_dev)
+                cw.corr_dev = _lib.ptr(self.corr_dev)
                 cw.n_blocks = len(off)
                 cw.block_off, cw.block_n, cw.block_i, cw.block_j = off.ctypes.data, nb.ctypes.data, bi.ctypes.data, bj.ctypes.data
             elif self.corr_block_n is not None and len(self.corr_block_n):
@@ -115,56 +107,32 @@ class _PreparedBatch:
         self.arr, self.poses, self.keep, self.off = arr, poses, keep, off
 
 
-class OptimizerGpu:
+class OptimizerGpu(_lib.Facade):
     def __init__(self, yml=None, device: int = 0, max_windows: int = 1, max_frames: int = 15, max_corr: int = 65536,
-                 H: int = 480, W: int = 640, stream: int = 0):
-        self.lib = _lib.load()
+                 H: int = 480, W: int = 640, stream: int = 0, ctx=None):
+        super().__init__(ctx, device, stream)
         self.params = solver_params(yml)
-        self.stream = ctypes.c_void_p(stream)
-        self.ctx = ctypes.c_void_p()
-        _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
-        self.limits = _lib.SolverLimits(max_windows, max_frames, max_corr, H, W, self.params.image_downscale)
-        _lib.check(self.lib.bt_solver_reserve(self.ctx, ctypes.byref(self.limits)), "bt_solver_reserve")
+        self.reserve(max_windows, max_frames, max_corr, H, W)
         self._staged = None
 
-    def close(self):
-        if self.ctx:
-            self.lib.bt_ctx_destroy(self.ctx)
-            self.ctx = ctypes.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def reserve(self, max_windows: int, max_frames: int, max_corr: int, H: int, W: int):
+        """Size the context's solver: windows per call, frames per window, correspondences per window and the largest frame."""
+        self.limits = _lib.SolverLimits(max_windows, max_frames, max_corr, H, W, self.params.image_downscale)
+        _lib.check(self.lib.bt_solver_reserve(self.ctx, self.limits), "bt_solver_reserve")
 
     # ---- frame cache: quarter-res maps built once per keyframe instead of once per call (CUDACache.cpp:76-88) ----------
     def reserve_frame_cache(self, capacity: int, H: int = None, W: int = None):
-        _lib.check(self.lib.bt_frame_cache_reserve(self.ctx, ctypes.c_int(capacity), ctypes.c_int(H or self.limits.H), ctypes.c_int(W or self.limits.W),
-                                                   ctypes.c_float(self.params.image_downscale)), "bt_frame_cache_reserve")
+        _lib.check(self.lib.bt_frame_cache_reserve(self.ctx, capacity, H or self.limits.H, W or self.limits.W, self.params.image_downscale),
+                   "bt_frame_cache_reserve")
 
     def store_frames(self, slots: Sequence[int], depths_gpu: Sequence, normals_gpu: Sequence, H: int, W: int, K):
-        n = len(slots)
-        K = np.asarray(K, np.float64)
-        fx, fy, cx, cy = (K[0, 0], K[1, 1], K[0, 2], K[1, 2]) if K.ndim == 2 else K
-        sl = (ctypes.c_int32 * n)(*[int(v) for v in slots])
-        dp = (ctypes.c_void_p * n)(*[_ptr(d) for d in depths_gpu])
-        nq = (ctypes.c_void_p * n)(*[_ptr(d) for d in normals_gpu])
-        _lib.check(self.lib.bt_frame_cache_store(self.ctx, ctypes.c_int(n), sl, dp, nq, ctypes.c_int(H), ctypes.c_int(W), ctypes.c_float(fx), ctypes.c_float(fy),
-                                                 ctypes.c_float(cx), ctypes.c_float(cy), ctypes.c_float(self.params.depth_min), ctypes.c_float(self.params.depth_max),
-                                                 self.stream), "bt_frame_cache_store")
+        self.store_prepared(self.prepare_store(slots, depths_gpu, normals_gpu, H, W, K))
 
     def prepare_store(self, slots: Sequence[int], depths_gpu: Sequence, normals_gpu: Sequence, H: int, W: int, K):
         """The argument block of one bt_frame_cache_store call, marshalled ONCE (a C / C++ caller hands the library plain arrays; from Python
         the per-frame pointer extraction costs more than the library call itself).  Pass the result to store_prepared()."""
-        n = len(slots)
-        K = np.asarray(K, np.float64)
-        fx, fy, cx, cy = (K[0, 0], K[1, 1], K[0, 2], K[1, 2]) if K.ndim == 2 else K
-        sl = (ctypes.c_int32 * n)(*[int(v) for v in slots])
-        dp = (ctypes.c_void_p * n)(*[_ptr(d) for d in depths_gpu])
-        nq = (ctypes.c_void_p * n)(*[_ptr(d) for d in normals_gpu])
-        args = (self.ctx, ctypes.c_int(n), sl, dp, nq, ctypes.c_int(H), ctypes.c_int(W), ctypes.c_float(fx), ctypes.c_float(fy), ctypes.c_float(cx), ctypes.c_float(cy),
-                ctypes.c_float(self.params.depth_min), ctypes.c_float(self.params.depth_max), self.stream)
+        args = _lib.prepared(self.lib.bt_frame_cache_store, self.ctx, len(slots), _lib.i32s(slots), _lib.ptrs(depths_gpu), _lib.ptrs(normals_gpu), H, W,
+                             *_lib.intrinsics(K), self.params.depth_min, self.params.depth_max, self.stream)
         return args, (depths_gpu, normals_gpu)      # (the tensors are kept alive with the block)
 
     def store_prepared(self, prepared):
@@ -178,22 +146,21 @@ class OptimizerGpu:
         return _PreparedBatch(arr, np.ascontiguousarray(poses, np.float32), keep, off)
 
     def begin_prepared(self, batch):
-        _lib.check(self.lib.bt_solve_windows_begin(self.ctx, ctypes.c_int(len(batch.keep)), batch.arr, ctypes.byref(self.params),
-                                                   batch.poses.ctypes.data_as(ctypes.c_void_p), self.stream), "bt_solve_windows_begin")
+        _lib.check(self.lib.bt_solve_windows_begin(self.ctx, len(batch.keep), batch.arr, self.params, _lib.ptr(batch.poses), self.stream),
+                   "bt_solve_windows_begin")
 
     def end_prepared(self, batch, out: np.ndarray = None) -> np.ndarray:
         """Poses of the oldest batch in flight as one [sum n_frames, 4, 4] array (batch.off gives the windows' first frames)."""
         if out is None:
             out = np.empty((batch.poses.shape[0], 4, 4), np.float32)
-        _lib.check(self.lib.bt_solve_windows_end(self.ctx, out.ctypes.data_as(ctypes.c_void_p)), "bt_solve_windows_end")
+        _lib.check(self.lib.bt_solve_windows_end(self.ctx, _lib.ptr(out)), "bt_solve_windows_end")
         return out
 
     def solve_prepared(self, batch, out: np.ndarray = None) -> np.ndarray:
         if out is None:
             out = np.empty((batch.poses.shape[0], 4, 4), np.float32)
         np.copyto(out.reshape(-1, 16), batch.poses)
-        _lib.check(self.lib.bt_solve_windows(self.ctx, ctypes.c_int(len(batch.keep)), batch.arr, ctypes.byref(self.params),
-                                             out.ctypes.data_as(ctypes.c_void_p), self.stream), "bt_solve_windows")
+        _lib.check(self.lib.bt_solve_windows(self.ctx, len(batch.keep), batch.arr, self.params, _lib.ptr(out), self.stream), "bt_solve_windows")
         return out
 
     # ---- reference-shaped single-window call (LossGPU.h:50) -------------------------------------------------
@@ -220,26 +187,24 @@ class OptimizerGpu:
 
     def optimizeWindows(self, windows: List[SolveWindow]) -> List[np.ndarray]:
         arr, poses, keep = self._marshal(windows)
-        _lib.check(self.lib.bt_solve_windows(self.ctx, ctypes.c_int(len(windows)), arr, ctypes.byref(self.params),
-                                             poses.ctypes.data_as(ctypes.c_void_p), self.stream), "bt_solve_windows")
+        _lib.check(self.lib.bt_solve_windows(self.ctx, len(windows), arr, self.params, _lib.ptr(poses), self.stream), "bt_solve_windows")
         del keep
         return self._split(windows, poses)
 
     # ---- streaming form: up to two batches in flight, the host side of batch k+1 overlaps the GPU side of batch k ----------------
     def begin(self, windows: List[SolveWindow]):
         arr, poses, keep = self._marshal(windows)
-        _lib.check(self.lib.bt_solve_windows_begin(self.ctx, ctypes.c_int(len(windows)), arr, ctypes.byref(self.params),
-                                                   poses.ctypes.data_as(ctypes.c_void_p), self.stream), "bt_solve_windows_begin")
+        _lib.check(self.lib.bt_solve_windows_begin(self.ctx, len(windows), arr, self.params, _lib.ptr(poses), self.stream), "bt_solve_windows_begin")
         if not hasattr(self, "_inflight"):
             self._inflight = []
         self._inflight.append((windows, poses, keep, arr))
 
     def end(self) -> List[np.ndarray]:
         if not getattr(self, "_inflight", None):      # nothing begun: let the library say so
-            _lib.check(self.lib.bt_solve_windows_end(self.ctx, ctypes.c_void_p(0)), "bt_solve_windows_end")
+            _lib.check(self.lib.bt_solve_windows_end(self.ctx, None), "bt_solve_windows_end")
         windows, poses, _, _ = self._inflight.pop(0)
         out = np.empty_like(poses)
-        _lib.check(self.lib.bt_solve_windows_end(self.ctx, out.ctypes.data_as(ctypes.c_void_p)), "bt_solve_windows_end")
+        _lib.check(self.lib.bt_solve_windows_end(self.ctx, _lib.ptr(out)), "bt_solve_windows_end")
         return self._split(windows, out)
 
     @staticmethod
@@ -254,8 +219,7 @@ class OptimizerGpu:
     # split API used by bench.py to time the resident-input kernel path separately from staging
     def stage(self, windows: List[SolveWindow]):
         arr, poses, keep = self._marshal(windows)
-        _lib.check(self.lib.bt_solve_stage(self.ctx, ctypes.c_int(len(windows)), arr, ctypes.byref(self.params),
-                                           poses.ctypes.data_as(ctypes.c_void_p), self.stream), "bt_solve_stage")
+        _lib.check(self.lib.bt_solve_stage(self.ctx, len(windows), arr, self.params, _lib.ptr(poses), self.stream), "bt_solve_stage")
         self._staged = (windows, poses, keep, arr)
 
     def run(self):
@@ -264,17 +228,17 @@ class OptimizerGpu:
     def fetch(self) -> List[np.ndarray]:
         windows, poses, _, _ = self._staged
         out = np.empty_like(poses)
-        _lib.check(self.lib.bt_solve_fetch(self.ctx, out.ctypes.data_as(ctypes.c_void_p), self.stream), "bt_solve_fetch")
+        _lib.check(self.lib.bt_solve_fetch(self.ctx, _lib.ptr(out), self.stream), "bt_solve_fetch")
         return self._split(windows, out)
 
     def stats(self) -> dict:
         st = _lib.SolveStats()
-        _lib.check(self.lib.bt_solve_get_stats(self.ctx, ctypes.byref(st)), "bt_solve_get_stats")
+        _lib.check(self.lib.bt_solve_get_stats(self.ctx, st), "bt_solve_get_stats")
         return {"n_windows": st.n_windows, "n_tiles_total": st.n_tiles_total, "n_kernel_launches": st.n_kernel_launches,
                 "n_src_pixels": int(st.n_src_pixels)}
 
     def enable_timing(self, on=True):
-        _lib.check(self.lib.bt_solve_enable_timing(self.ctx, ctypes.c_int(1 if on else 0)), "bt_solve_enable_timing")
+        _lib.check(self.lib.bt_solve_enable_timing(self.ctx, 1 if on else 0), "bt_solve_enable_timing")
 
     def timing_ms(self):
         ms = (ctypes.c_float * 3)()
@@ -287,29 +251,29 @@ class OptimizerGpu:
         return {"tables_upload": us[0], "prep_launch": us[1], "scan_stage_upload": us[2], "solve_launch": us[3], "fetch_wait": us[4], "total": us[5]}
 
     def enable_profile(self, max_records=200000):
-        _lib.check(self.lib.bt_solve_enable_profile(self.ctx, ctypes.c_int(max_records)), "bt_solve_enable_profile")
+        _lib.check(self.lib.bt_solve_enable_profile(self.ctx, max_records), "bt_solve_enable_profile")
         self._prof_cap = max_records
 
     def get_profile(self):
         out = np.zeros((self._prof_cap, 12), np.int64)
-        n = self.lib.bt_solve_get_profile(self.ctx, out.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(self._prof_cap))
+        n = self.lib.bt_solve_get_profile(self.ctx, _lib.ptr(out), self._prof_cap)
         if n < 0:
             _lib.check(n, "bt_solve_get_profile")
         return out[:n]
 
     def enable_debug(self, on=True):
-        _lib.check(self.lib.bt_solve_enable_debug(self.ctx, ctypes.c_int(1 if on else 0)), "bt_solve_enable_debug")
+        _lib.check(self.lib.bt_solve_enable_debug(self.ctx, 1 if on else 0), "bt_solve_enable_debug")
 
     def debug_counts(self, w: int, n_pairs: int):
         c = np.zeros(n_pairs, np.float32)
-        _lib.check(self.lib.bt_solve_debug_counts(self.ctx, ctypes.c_int(w), ctypes.c_int(n_pairs), c.ctypes.data_as(ctypes.c_void_p)), "bt_solve_debug_counts")
+        _lib.check(self.lib.bt_solve_debug_counts(self.ctx, w, n_pairs, _lib.ptr(c)), "bt_solve_debug_counts")
         return c
 
     def debug_dense(self, w: int, n_frames: int):
         dim = 6 * n_frames
         J = np.zeros((dim, dim), np.float32)
         r = np.zeros(dim, np.float32)
-        _lib.check(self.lib.bt_solve_debug_dense(self.ctx, ctypes.c_int(w), J.ctypes.data_as(ctypes.c_void_p), r.ctypes.data_as(ctypes.c_void_p)), "bt_solve_debug_dense")
+        _lib.check(self.lib.bt_solve_debug_dense(self.ctx, w, _lib.ptr(J), _lib.ptr(r)), "bt_solve_debug_dense")
         return J, r
 
     def debug_system(self, w: int, n_frames: int):
@@ -317,6 +281,5 @@ class OptimizerGpu:
         dim = 6 * (n_frames - 1)
         A = np.zeros((dim, dim), np.float32)
         rhs, minv, delta = (np.zeros(dim, np.float32) for _ in range(3))
-        _lib.check(self.lib.bt_solve_debug_system(self.ctx, ctypes.c_int(w), ctypes.c_int(n_frames), *(v.ctypes.data_as(ctypes.c_void_p) for v in (A, rhs, minv, delta))),
-                   "bt_solve_debug_system")
+        _lib.check(self.lib.bt_solve_debug_system(self.ctx, w, n_frames, *(_lib.ptr(v) for v in (A, rhs, minv, delta))), "bt_solve_debug_system")
         return A, rhs, minv, delta

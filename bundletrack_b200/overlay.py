@@ -36,45 +36,22 @@ def load_obj_points(path: str) -> np.ndarray:
     return np.asarray(pts, np.float64).astype(np.float32)
 
 
-def _ptrs(xs) -> "ctypes.Array":
-    a = (ctypes.c_void_p * len(xs))()
-    for i, x in enumerate(xs):
-        a[i] = int(x.data_ptr()) if hasattr(x, "data_ptr") else int(x)
-    return a
-
-
-class VoxelGrid:
+class VoxelGrid(_lib.Facade):
     """bt_voxel_downsample: PCL's VoxelGrid of many float32 [n,3] device clouds in one asynchronous call.  Scratch for max_frames clouds of
     max_pts points is reserved here (or on `ctx`, shared with an Overlay)."""
 
     def __init__(self, max_pts: int, max_frames: int = 1, device: int = 0, stream: int = 0, ctx=None):
-        self.lib = _lib.load()
-        self.device, self.stream = device, ctypes.c_void_p(stream)
-        self._own = ctx is None
-        self.ctx = ctypes.c_void_p() if ctx is None else ctx
-        if self._own:
-            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
+        super().__init__(ctx, device, stream)
+        self.device = device
         self.reserve(max_pts, max_frames)
 
     def reserve(self, max_pts: int, max_frames: int) -> None:
-        _lib.check(self.lib.bt_overlay_reserve(self.ctx, ctypes.c_int(max_pts), ctypes.c_int(max_frames)), "bt_overlay_reserve")
-
-    def close(self):
-        if self._own and self.ctx:
-            self.lib.bt_ctx_destroy(self.ctx)
-            self.ctx = ctypes.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        _lib.check(self.lib.bt_overlay_reserve(self.ctx, max_pts, max_frames), "bt_overlay_reserve")
 
     def enqueue(self, clouds, leaf: float, outs, n_out) -> None:
         """clouds / outs: float32 [n_c,3] CUDA tensors (outs with room for n_c rows); n_out: int32 CUDA tensor [len(clouds)].  Asynchronous."""
-        n = (ctypes.c_int * len(clouds))(*[int(c.shape[0]) for c in clouds])
-        _lib.check(self.lib.bt_voxel_downsample(self.ctx, ctypes.c_int(len(clouds)), _ptrs(clouds), n, ctypes.c_float(leaf), _ptrs(outs),
-                                                ctypes.c_void_p(n_out.data_ptr()), self.stream), "bt_voxel_downsample")
+        _lib.check(self.lib.bt_voxel_downsample(self.ctx, len(clouds), _lib.ptrs(clouds), _lib.i32s([c.shape[0] for c in clouds]), leaf, _lib.ptrs(outs),
+                                                _lib.ptr(n_out), self.stream), "bt_voxel_downsample")
 
     def __call__(self, clouds, leaf: float):
         """Each cloud (numpy or CUDA, [n,3]) voxel-gridded at leaf: a list of float32 numpy [m,3]; synchronises the stream."""
@@ -101,8 +78,7 @@ class Overlay:
         raw = np.ascontiguousarray(np.asarray(model_pts, np.float32).reshape(-1, 3))
         if len(raw) == 0:
             raise ValueError("the model has no point")
-        Kn = np.asarray(K, np.float64)
-        self.K = tuple(float(v) for v in ((Kn[0, 0], Kn[1, 1], Kn[0, 2], Kn[1, 2]) if Kn.ndim == 2 else Kn))
+        self.K = _lib.intrinsics(K)
         self.H, self.W, self.max_frames, self.device = int(H), int(W), int(max_frames), device
         self.grid = VoxelGrid(len(raw), 1, device=device, stream=stream, ctx=ctx)
         self.lib, self.ctx, self.stream = self.grid.lib, self.grid.ctx, self.grid.stream
@@ -125,11 +101,8 @@ class Overlay:
             raise ValueError(f"{len(P)} poses, {F} colour images, {len(fg)} masks, {len(viz_out)} viz outputs: they must agree")
         if self.model.shape[0] == 0:
             raise ValueError("the voxel-gridded model is empty (no finite point)")
-        fx, fy, cx, cy = self.K
-        _lib.check(self.lib.bt_pose_overlay(self.ctx, ctypes.c_int(F), ctypes.c_void_p(self.model_dev.data_ptr()), ctypes.c_int(len(self.model)),
-                                            P.ctypes.data_as(ctypes.c_void_p), ctypes.c_float(fx), ctypes.c_float(fy), ctypes.c_float(cx), ctypes.c_float(cy),
-                                            _ptrs(colour), _ptrs(fg), ctypes.c_int(self.H), ctypes.c_int(self.W), _ptrs(viz_out),
-                                            None if raw_out is None else _ptrs(raw_out), self.stream), "bt_pose_overlay")
+        _lib.check(self.lib.bt_pose_overlay(self.ctx, F, _lib.ptr(self.model_dev), len(self.model), _lib.ptr(P), *self.K, _lib.ptrs(colour), _lib.ptrs(fg),
+                                            self.H, self.W, _lib.ptrs(viz_out), None if raw_out is None else _lib.ptrs(raw_out), self.stream), "bt_pose_overlay")
 
     def render_host(self, cur_in_model, colour, fg):
         """render() on host or device images; returns (viz, raw) as uint8 numpy [F,H,W,3] and synchronises the stream."""
@@ -193,10 +166,8 @@ def rng_after(state: int, n_matches: int) -> int:
 
 def match_image_shape(roi_a, roi_b):
     """(rows, cols) of the match image of two ROIs (umin, umax, vmin, vmax)."""
-    lib = _lib.load()
-    ra, rb = (ctypes.c_int32 * 4)(*[int(v) for v in roi_a]), (ctypes.c_int32 * 4)(*[int(v) for v in roi_b])
     rows, cols = ctypes.c_int(), ctypes.c_int()
-    _lib.check(lib.bt_match_viz_shape(ra, rb, ctypes.byref(rows), ctypes.byref(cols)), "bt_match_viz_shape")
+    _lib.check(_lib.load().bt_match_viz_shape(_lib.i32s(roi_a), _lib.i32s(roi_b), ctypes.byref(rows), ctypes.byref(cols)), "bt_match_viz_shape")
     return rows.value, cols.value
 
 
@@ -205,29 +176,14 @@ def match_image_path(debug_dir: str, new_id: str, id_a: str, id_b: str, stage: s
     return os.path.join(debug_dir, new_id, f"{id_a}_match_{id_b}_{stage}.jpg")
 
 
-class MatchViz:
+class MatchViz(_lib.Facade):
     """bt_match_viz: match images drawn on the device, many per asynchronous call.  Scratch for max_images images and max_matches matches
     per call is reserved here (or on `ctx`)."""
 
     def __init__(self, max_images: int = 1, max_matches: int = 4096, device: int = 0, stream: int = 0, ctx=None):
-        self.lib = _lib.load()
-        self.device, self.stream = device, ctypes.c_void_p(stream)
-        self._own = ctx is None
-        self.ctx = ctypes.c_void_p() if ctx is None else ctx
-        if self._own:
-            _lib.check(self.lib.bt_ctx_create(ctypes.byref(self.ctx), ctypes.c_int(device)), "bt_ctx_create")
-        _lib.check(self.lib.bt_match_viz_reserve(self.ctx, ctypes.c_int(max_images), ctypes.c_int(max_matches)), "bt_match_viz_reserve")
-
-    def close(self):
-        if self._own and self.ctx:
-            self.lib.bt_ctx_destroy(self.ctx)
-            self.ctx = ctypes.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().__init__(ctx, device, stream)
+        self.device = device
+        _lib.check(self.lib.bt_match_viz_reserve(self.ctx, max_images, max_matches), "bt_match_viz_reserve")
 
     def draw(self, images, outs) -> None:
         """images: (colour_a, roi_a, colour_b, roi_b, uv, rng_state) per image; colours are device uint8 [H,W,3], uv a device float32 [n,4]
@@ -244,7 +200,7 @@ class MatchViz:
             d.roi_b[:] = [int(v) for v in rb]
             d.uv, d.n = (None, 0) if uv is None or uv.shape[0] == 0 else (uv.data_ptr(), uv.shape[0])
             d.rng_state = int(st)
-        _lib.check(self.lib.bt_match_viz(self.ctx, ctypes.c_int(n), descs, _ptrs(outs), self.stream), "bt_match_viz")
+        _lib.check(self.lib.bt_match_viz(self.ctx, n, descs, _lib.ptrs(outs), self.stream), "bt_match_viz")
 
     def _check(self, k, ca, ra, cb, rb, uv, out) -> None:
         """The library reads these through raw device pointers: each must be a contiguous CUDA tensor on this device, of the dtype and

@@ -10,20 +10,15 @@ import numpy as np
 from . import _lib
 
 
-def _p(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
-
-
 def rotation_geodesic(pose_a, pose_b) -> float:
     a, b = np.ascontiguousarray(pose_a, np.float32), np.ascontiguousarray(pose_b, np.float32)
-    return float(_lib.load().bt_rotation_geodesic(_p(a), _p(b)))
+    return float(_lib.load().bt_rotation_geodesic(_lib.ptr(a), _lib.ptr(b)))
 
 
 def keyframe_check(pose_new, frame_id: int, n_keypts: int, keyframe_poses, min_feat_num: int = 0, min_rot_deg: float = 10.0) -> bool:
     kp = np.ascontiguousarray(keyframe_poses, np.float32).reshape(-1, 4, 4)
     pn = np.ascontiguousarray(pose_new, np.float32)
-    return bool(_lib.load().bt_keyframe_check(_p(pn), ctypes.c_int(frame_id), ctypes.c_int(n_keypts), _p(kp), ctypes.c_int(len(kp)), ctypes.c_int(min_feat_num),
-                                              ctypes.c_float(min_rot_deg)))
+    return bool(_lib.load().bt_keyframe_check(_lib.ptr(pn), frame_id, n_keypts, _lib.ptr(kp), len(kp), min_feat_num, min_rot_deg))
 
 
 def select_keyframes(pose_new, keyframe_poses, max_BA_frames: int = 15) -> np.ndarray:
@@ -31,14 +26,14 @@ def select_keyframes(pose_new, keyframe_poses, max_BA_frames: int = 15) -> np.nd
     pn = np.ascontiguousarray(pose_new, np.float32)
     out = np.zeros(max(len(kp), 1), np.int32)
     n = ctypes.c_int(0)
-    _lib.check(_lib.load().bt_select_keyframes(_p(pn), _p(kp), ctypes.c_int(len(kp)), ctypes.c_int(max_BA_frames), _p(out), ctypes.byref(n)), "bt_select_keyframes")
+    _lib.check(_lib.load().bt_select_keyframes(_lib.ptr(pn), _lib.ptr(kp), len(kp), max_BA_frames, _lib.ptr(out), ctypes.byref(n)), "bt_select_keyframes")
     return out[:n.value].copy()
 
 
 def rigid_transform(pts1, pts2) -> np.ndarray:
     a, b = np.ascontiguousarray(pts1, np.float32).reshape(-1, 3), np.ascontiguousarray(pts2, np.float32).reshape(-1, 3)
     out = np.zeros((4, 4), np.float32)
-    _lib.check(_lib.load().bt_rigid_transform(_p(a), _p(b), ctypes.c_int(len(a)), _p(out)), "bt_rigid_transform")
+    _lib.check(_lib.load().bt_rigid_transform(_lib.ptr(a), _lib.ptr(b), len(a), _lib.ptr(out)), "bt_rigid_transform")
     return out
 
 
@@ -49,9 +44,8 @@ def lfnet_parse_reply(parts, roi):
     n_guess = max(len(kp) // 8, 1)
     out = np.zeros((n_guess, 2), np.float32)
     n, dim = ctypes.c_int(0), ctypes.c_int(0)
-    r = (ctypes.c_int * 4)(*[int(v) for v in roi])
-    _lib.check(_lib.load().bt_lfnet_parse_reply(info, ctypes.c_size_t(len(info)), kp, ctypes.c_size_t(len(kp)), ctypes.c_size_t(len(desc)), r, _p(out),
-                                                ctypes.c_int(n_guess), ctypes.byref(n), ctypes.byref(dim)), "bt_lfnet_parse_reply")
+    _lib.check(_lib.load().bt_lfnet_parse_reply(info, len(info), kp, len(kp), len(desc), _lib.i32s(roi), _lib.ptr(out), n_guess, ctypes.byref(n),
+                                                ctypes.byref(dim)), "bt_lfnet_parse_reply")
     return out[:n.value], np.frombuffer(desc, np.float32).reshape(n.value, dim.value)
 
 
@@ -60,36 +54,26 @@ class Tracks:
 
     def __init__(self):
         self.lib = _lib.load()
-        self.h = ctypes.c_void_p()
-        _lib.check(self.lib.bt_tracks_create(ctypes.byref(self.h)), "bt_tracks_create")
+        self.h = _lib.Handle("bt_tracks_create", "bt_tracks_destroy")
 
     def close(self):
-        if self.h:
-            self.lib.bt_tracks_destroy(self.h)
-            self.h = ctypes.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self.h.close()
 
     def update_pair(self, frame_a: int, frame_b: int, uv, is_inlier=None):
         uv = np.ascontiguousarray(uv, np.float32).reshape(-1, 4)
         inl = None if is_inlier is None else np.ascontiguousarray(is_inlier, np.uint8)
-        _lib.check(self.lib.bt_tracks_update_pair(self.h, ctypes.c_int(frame_a), ctypes.c_int(frame_b), _p(uv), None if inl is None else _p(inl), ctypes.c_int(len(uv))),
-                   "bt_tracks_update_pair")
+        _lib.check(self.lib.bt_tracks_update_pair(self.h, frame_a, frame_b, _lib.ptr(uv), _lib.ptr(inl), len(uv)), "bt_tracks_update_pair")
 
     def propagate(self, frame_a: int, frame_b: int, existing_uv, capacity: int = 65536) -> np.ndarray:
         ex = np.ascontiguousarray(existing_uv, np.float32).reshape(-1, 4)
         out = np.zeros((capacity, 4), np.float32)
         n = ctypes.c_int(0)
-        _lib.check(self.lib.bt_tracks_propagate(self.h, ctypes.c_int(frame_a), ctypes.c_int(frame_b), _p(ex), ctypes.c_int(len(ex)), _p(out), ctypes.c_int(capacity),
-                                                ctypes.byref(n)), "bt_tracks_propagate")
+        _lib.check(self.lib.bt_tracks_propagate(self.h, frame_a, frame_b, _lib.ptr(ex), len(ex), _lib.ptr(out), capacity, ctypes.byref(n)),
+                   "bt_tracks_propagate")
         return out[:n.value].copy()
 
     def forget_frame(self, frame: int):
-        _lib.check(self.lib.bt_tracks_forget_frame(self.h, ctypes.c_int(frame)), "bt_tracks_forget_frame")
+        _lib.check(self.lib.bt_tracks_forget_frame(self.h, frame), "bt_tracks_forget_frame")
 
     def stats(self):
         a, b = ctypes.c_int(0), ctypes.c_int(0)
@@ -99,17 +83,17 @@ class Tracks:
 
 def ba_gate(n_edges_newframe: int, min_fm_edges_newframe: int = 10) -> bool:
     """Bundler::optimizeGPU's gate (/root/reference/src/Bundler.cpp:343-347): False = Frame::NO_BA, the optimizer is not called."""
-    return bool(_lib.load().bt_ba_gate(ctypes.c_int(n_edges_newframe), ctypes.c_int(min_fm_edges_newframe)))
+    return bool(_lib.load().bt_ba_gate(n_edges_newframe, min_fm_edges_newframe))
 
 
 def pose_text(cur_in_model) -> str:
     """Bundler::saveNewframeResult's pose record (Bundler.cpp:362-378): ob_in_cam = inverse(cur_in_model), printed like Eigen prints it."""
     p = np.ascontiguousarray(cur_in_model, np.float32)
     buf = ctypes.create_string_buffer(1024)
-    _lib.check(_lib.load().bt_pose_format(_p(p), buf, ctypes.c_int(1024)), "bt_pose_format")
+    _lib.check(_lib.load().bt_pose_format(_lib.ptr(p), buf, 1024), "bt_pose_format")
     return buf.value.decode()
 
 
 def save_pose_txt(path: str, cur_in_model) -> None:
     p = np.ascontiguousarray(cur_in_model, np.float32)
-    _lib.check(_lib.load().bt_pose_write_txt(path.encode(), _p(p)), "bt_pose_write_txt")
+    _lib.check(_lib.load().bt_pose_write_txt(path.encode(), _lib.ptr(p)), "bt_pose_write_txt")

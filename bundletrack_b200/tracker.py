@@ -18,11 +18,10 @@ def tracker_params(yml, H: int, W: int, K, max_feats: int, max_frames_alive: int
     keyframe.min_feat_num / min_rot, ransac.max_iter / inlier_dist and those config.py maps).  mode: _lib.BT_MASK_* (default: config.mask_mode).
     max_keyframes > 0 holds that many keyframes apart from max_frames_alive (the header's bt_tracker_params)."""
     y = load_yml(yml)
-    Kn = np.asarray(K, np.float64)
-    fx, fy, cx, cy = (Kn[0, 0], Kn[1, 1], Kn[0, 2], Kn[1, 2]) if Kn.ndim == 2 else Kn
+    fx, fy, cx, cy = _lib.intrinsics(K)
     b, kf, rs = y["bundle"], y["keyframe"], y["ransac"]
     p = _lib.TrackerParams()
-    p.H, p.W, p.fx, p.fy, p.cx, p.cy = int(H), int(W), float(fx), float(fy), float(cx), float(cy)
+    p.H, p.W, p.fx, p.fy, p.cx, p.cy = int(H), int(W), fx, fy, cx, cy
     p.max_feats, p.max_frames_alive, p.max_keyframes = int(max_feats), int(max_frames_alive), int(max_keyframes)
     p.mask_mode = mask_mode(yml) if mode is None else int(mode)
     p.depth, p.solver, p.prune = depth_params(y), solver_params(y), prune_params(y)
@@ -30,10 +29,6 @@ def tracker_params(yml, H: int, W: int, K, max_feats: int, max_frames_alive: int
     p.window_size, p.max_BA_frames, p.min_fm_edges_newframe = int(b["window_size"]), int(b["max_BA_frames"]), int(b["min_fm_edges_newframe"])
     p.min_feat_num, p.min_rot_deg = int(kf["min_feat_num"]), float(kf["min_rot"])
     return p
-
-
-def _ptr(x) -> int:
-    return int(x.data_ptr()) if hasattr(x, "data_ptr") else int(x)
 
 
 class Tracker:
@@ -47,19 +42,10 @@ class Tracker:
         self.lib = _lib.load()
         self.params = tracker_params(yml, H, W, K, max_feats, max_frames_alive, mode, max_keyframes)
         self.stream = ctypes.c_void_p(stream)
-        self.t = ctypes.c_void_p()
-        _lib.check(self.lib.bt_tracker_create(ctypes.byref(self.t), ctypes.c_int(device), ctypes.byref(self.params)), "bt_tracker_create")
+        self.t = _lib.Handle("bt_tracker_create", "bt_tracker_destroy", device, self.params)
 
     def close(self):
-        if self.t:
-            self.lib.bt_tracker_destroy(self.t)
-            self.t = ctypes.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self.t.close()
 
     def begin_frame(self, depth_raw, mask, colour, request_out, loader_id: int = 0, first_pose=None):
         """depth_raw float32 [H,W], mask uint8 [H,W], colour uint8 [H,W,3] BGR, request_out uint8 [400,400,3]: device.  loader_id / first_pose
@@ -67,10 +53,8 @@ class Tracker:
         roi = np.zeros(4, np.int32)
         st = ctypes.c_int(-1)
         fp = None if first_pose is None else np.ascontiguousarray(first_pose, np.float32).reshape(16)
-        _lib.check(self.lib.bt_tracker_begin_frame(self.t, ctypes.c_int(loader_id), None if fp is None else fp.ctypes.data_as(ctypes.c_void_p),
-                                                   ctypes.c_void_p(_ptr(depth_raw)), ctypes.c_void_p(_ptr(mask)), ctypes.c_void_p(_ptr(colour)),
-                                                   ctypes.c_void_p(_ptr(request_out)), roi.ctypes.data_as(ctypes.c_void_p), ctypes.byref(st), self.stream),
-                   "bt_tracker_begin_frame")
+        _lib.check(self.lib.bt_tracker_begin_frame(self.t, loader_id, _lib.ptr(fp), *(_lib.ptr(x) for x in (depth_raw, mask, colour, request_out, roi)),
+                                                   ctypes.byref(st), self.stream), "bt_tracker_begin_frame")
         return st.value, roi
 
     def begin_frame_mm(self, depth_mm, mask, colour, request_out, loader_id: int = 0, first_pose=None):
@@ -81,28 +65,23 @@ class Tracker:
         st, fid = ctypes.c_int(-1), ctypes.c_int(-1)
         pose = np.zeros((4, 4), np.float32)
         fp = None if first_pose is None else np.ascontiguousarray(first_pose, np.float32).reshape(16)
-        _lib.check(self.lib.bt_tracker_begin_frame_u16(self.t, ctypes.c_int(loader_id), None if fp is None else fp.ctypes.data_as(ctypes.c_void_p),
-                                                       ctypes.c_void_p(_ptr(depth_mm)), ctypes.c_void_p(_ptr(mask)), ctypes.c_void_p(_ptr(colour)),
-                                                       ctypes.c_void_p(_ptr(request_out)), roi.ctypes.data_as(ctypes.c_void_p), ctypes.byref(fid),
-                                                       pose.ctypes.data_as(ctypes.c_void_p), ctypes.byref(st), self.stream), "bt_tracker_begin_frame_u16")
+        _lib.check(self.lib.bt_tracker_begin_frame_u16(self.t, loader_id, _lib.ptr(fp), *(_lib.ptr(x) for x in (depth_mm, mask, colour, request_out, roi)),
+                                                       ctypes.byref(fid), _lib.ptr(pose), ctypes.byref(st), self.stream), "bt_tracker_begin_frame_u16")
         return st.value, roi, fid.value, pose
 
     def end_frame(self, kpts, desc):
         """kpts: numpy [n,2] float32 image pixels; desc: device float32 [n,256].  Returns (pose [4,4] float32 cam->model, status)."""
         k = np.ascontiguousarray(kpts, np.float32).reshape(-1, 2)
-        v = _lib.DescView()
-        v.dev, v.n, v.dim = _ptr(desc), int(desc.shape[0]), int(desc.shape[1])
-        v.pitch_bytes = desc.stride(0) * 4 if desc.shape[0] > 1 else desc.shape[1] * 4
         pose = np.zeros((4, 4), np.float32)
         st = ctypes.c_int(-1)
-        _lib.check(self.lib.bt_tracker_end_frame(self.t, k.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(len(k)), ctypes.byref(v),
-                                                 pose.ctypes.data_as(ctypes.c_void_p), ctypes.byref(st), self.stream), "bt_tracker_end_frame")
+        _lib.check(self.lib.bt_tracker_end_frame(self.t, _lib.ptr(k), len(k), _lib.desc_view(desc), _lib.ptr(pose), ctypes.byref(st), self.stream),
+                   "bt_tracker_end_frame")
         return pose, st.value
 
     def drop_frame(self):
         """Feature detection failed: the pending frame is FAIL and forgotten.  Returns its pose."""
         pose = np.zeros((4, 4), np.float32)
-        _lib.check(self.lib.bt_tracker_drop_frame(self.t, pose.ctypes.data_as(ctypes.c_void_p)), "bt_tracker_drop_frame")
+        _lib.check(self.lib.bt_tracker_drop_frame(self.t, _lib.ptr(pose)), "bt_tracker_drop_frame")
         return pose
 
     def state(self):
@@ -112,8 +91,7 @@ class Tracker:
         ids = np.zeros(cap, np.int32)
         poses = np.zeros((cap, 4, 4), np.float32)
         kf = np.zeros(cap, np.int32)
-        _lib.check(self.lib.bt_tracker_state(self.t, ids.ctypes.data_as(ctypes.c_void_p), poses.ctypes.data_as(ctypes.c_void_p), kf.ctypes.data_as(ctypes.c_void_p),
-                                             ctypes.c_int(cap), ctypes.byref(n)), "bt_tracker_state")
+        _lib.check(self.lib.bt_tracker_state(self.t, _lib.ptr(ids), _lib.ptr(poses), _lib.ptr(kf), cap, ctypes.byref(n)), "bt_tracker_state")
         return ids[:n.value].copy(), poses[:n.value].copy(), kf[:n.value].astype(bool)
 
     def last_fg(self) -> int:

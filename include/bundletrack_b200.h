@@ -301,7 +301,7 @@ BT_API int bt_match_pairs_ex(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, 
 /* Per-pair result cache: SiftManager::_matches (findCorres returns at once for a pair it has seen, FeatureManager.cpp:176;
  * forgetFrame drops a frame's pairs, :131-148).  Entries stay on the device; frames are named by Frame::_id.
  *   put     stores the blocks a bt_match_pairs* call produced (host copies of its n_entry / entry_off / status arrays).
- *   has     1 / 0.
+ *   has     1 / 0 (BT_ERR_INVALID_ARG for a NULL ctx).
  *   gather  writes the cached blocks of the listed pairs back to back into dst_dev with imgIdx_i / imgIdx_j rewritten to the given
  *           window indices (a frame's index changes from window to window) and fills block_off / block_n for bt_window::corr_dev;
  *           pairs with no cached matches contribute empty blocks.

@@ -8,7 +8,6 @@ import numpy as np
 import pytest
 
 from bundletrack_b200 import _lib, synth
-from bundletrack_b200.config import solver_params
 from bundletrack_b200.optimizer import OptimizerGpu, SolveWindow
 
 pytestmark = pytest.mark.gpu
@@ -36,21 +35,6 @@ def before(cuda_device):
 
 def _grew(now, base):
     return all(n > b for n, b in zip(now, base))
-
-
-class _Solver(OptimizerGpu):
-    """OptimizerGpu's calls on a context another object owns."""
-
-    def __init__(self, ctx, max_windows, max_frames, max_corr, H, W):
-        self.lib, self.params, self.stream, self.ctx, self._staged = _lib.load(), solver_params(None), ctypes.c_void_p(0), ctx, None
-        self.reserve(max_windows, max_frames, max_corr, H, W)
-
-    def reserve(self, max_windows, max_frames, max_corr, H, W):
-        self.limits = _lib.SolverLimits(max_windows, max_frames, max_corr, H, W, self.params.image_downscale)
-        _lib.check(self.lib.bt_solver_reserve(self.ctx, ctypes.byref(self.limits)), "bt_solver_reserve")
-
-    def close(self):
-        pass
 
 
 def _feature_frames(dev, n=3, n_feats=300):
@@ -89,7 +73,7 @@ def test_context_destroy_frees_every_module(before, cuda_device, grow):
     sw = synth.make_window(7, n_frames=4, n_corr=400)
     depth = [torch.from_numpy(sw.depth[k]).to(dev) for k in range(4)]
     normal = [torch.from_numpy(sw.normal[k]).to(dev) for k in range(4)]
-    opt = _Solver(ctx, 1, 8, 4096, sw.H, sw.W)
+    opt = OptimizerGpu(ctx=ctx, max_windows=1, max_frames=8, max_corr=4096, H=sw.H, W=sw.W)
     opt.enable_timing()
     opt.enable_profile(1000)
     opt.reserve_frame_cache(4)
@@ -140,6 +124,45 @@ def test_context_destroy_frees_every_module(before, cuda_device, grow):
         o.close()                                            # (borrowed context: none of these frees it)
     assert _live() == grown
     mp.close()
+    assert _live() == before
+
+
+def _front_end_run(fe, dev):
+    """One bt_frames_preprocess call through fe; returns its depth and normal maps."""
+    import torch
+    raw, K = synth.make_raw_depth(5, 120, 160)
+    d, n = torch.empty((120, 160), device=dev), torch.empty((120, 160, 4), device=dev)
+    fe.process([torch.from_numpy(raw).to(dev)], 120, 160, K, [d], [n])
+    torch.cuda.synchronize()
+    return d.cpu().numpy(), n.cpu().numpy()
+
+
+def test_borrower_after_owner_close_is_refused(before, cuda_device):
+    """bench.py's sharing: a front end on the optimizer's context.  Once the owner closes the context, the borrower's call passes NULL and
+    the library refuses it; no call reaches the destroyed context."""
+    from bundletrack_b200.frontend import FrameFrontEnd
+    opt = OptimizerGpu(max_windows=1, max_frames=4, max_corr=1024, H=120, W=160)
+    fe = FrameFrontEnd(ctx=opt.ctx)
+    _front_end_run(fe, cuda_device)
+    opt.close()
+    assert _live() == before
+    with pytest.raises(_lib.BtError) as e:
+        _front_end_run(fe, cuda_device)
+    assert e.value.rc == _lib.BT_ERR_INVALID_ARG
+    fe.close()
+
+
+def test_borrower_outlives_its_owner(before, cuda_device):
+    """Deleting the owner leaves the shared context to the borrower, which keeps working; the context goes with the last holder."""
+    from bundletrack_b200.frontend import FrameFrontEnd
+    opt = OptimizerGpu(max_windows=1, max_frames=4, max_corr=1024, H=120, W=160)
+    fe = FrameFrontEnd(ctx=opt.ctx)
+    want = _front_end_run(fe, cuda_device)
+    del opt
+    assert _grew(_live()[:1], before[:1])
+    got = _front_end_run(fe, cuda_device)
+    assert all(np.array_equal(a, b) for a, b in zip(got, want))
+    del fe
     assert _live() == before
 
 
