@@ -878,6 +878,14 @@ __device__ __forceinline__ float skew(const float* v, int a, int b) {   // [v]x 
 	const float s = ((b - a + 3) % 3 == 1) ? -1.f : 1.f;    // (0,1):-vz (1,2):-vx (2,0):-vy ; transposed: +
 	return s * v[k];
 }
+// skew() of the vector (x, y, z) without an array: an array indexed at run time would live in local memory, and the compiler may
+// then keep other small arrays of the kernel there too (the pixel loop's bilinear sums)
+__device__ __forceinline__ float skew3(float x, float y, float z, int a, int b) {
+	if (a == b) return 0.f;
+	const int k = 3 - a - b;
+	const float s = ((b - a + 3) % 3 == 1) ? -1.f : 1.f;
+	return s * (k == 0 ? x : (k == 1 ? y : z));
+}
 __device__ __forceinline__ void unpack_sym(int e, int& r, int& c) {
 	r = 0;
 	while (e >= 6 - r) { e -= 6 - r; r++; }
@@ -1344,13 +1352,54 @@ template <int HALF> __device__ __forceinline__ void butterfly_step(float (&v)[32
 	}
 	if constexpr (HALF > 1) butterfly_step<HALF / 2>(v, lane);
 }
+// Entry e of a dense tile's constants, from the current poses of its frames: e < 12: transform = T_i^-1 T_j (rigid inverse), row r,
+// col c; 12 <= e < 48: X_i = [[R,0],[[t]x R, R]] of the TARGET frame, which maps the tile's sums to the model frame; e == 48: the
+// window's projection / texel geometry, read by the pixel loop where it is used.
+__device__ __forceinline__ void tile_const(const SolveArgs& a, const Tile& tl, int e, float* sM, float* sX, float* sG) {
+	if (e < 12) {
+		const float* Ti = a.T + (size_t)tl.tgt_slot * 12;
+		const float* Tj = a.T + (size_t)tl.src_slot * 12;
+		const int r = e >> 2, c = e & 3;
+		float v = 0.f;
+		for (int k = 0; k < 3; k++) {
+			const float rik = __ldcg(Ti + k * 4 + r);          // R_i^T (r,k) = R_i(k,r)
+			v += rik * ((c < 3) ? __ldcg(Tj + k * 4 + c) : (__ldcg(Tj + k * 4 + 3) - __ldcg(Ti + k * 4 + 3)));
+		}
+		sM[e] = v;
+	} else if (e < 48) {
+		const float* Ti = a.T + (size_t)tl.tgt_slot * 12;
+		const int x = e - 12, r = x / 6, c = x - r * 6;
+		float v;
+		if (r < 3) v = (c < 3) ? __ldcg(Ti + r * 4 + c) : 0.f;
+		else if (c >= 3) v = __ldcg(Ti + (r - 3) * 4 + (c - 3));
+		else { const float tx = __ldcg(Ti + 3), ty = __ldcg(Ti + 7), tz = __ldcg(Ti + 11); v = 0.f; for (int kk = 0; kk < 3; kk++) v += skew3(tx, ty, tz, r - 3, kk) * __ldcg(Ti + kk * 4 + c); }
+		sX[x] = v;
+	} else if (e == 48) {
+		const WinDesc& wd = a.wins[tl.win];
+		sG[0] = wd.fx; sG[1] = wd.fy; sG[2] = wd.cx; sG[3] = wd.cy;
+		sG[4] = wd.tg.ifx; sG[5] = wd.tg.ify; sG[6] = wd.tg.icx; sG[7] = wd.tg.icy;
+		sG[8] = wd.tg.scaleW; sG[9] = wd.tg.scaleH; sG[10] = __int_as_float(wd.w); sG[11] = __int_as_float(wd.h);
+	}
+}
+// Thread tid's entry of tile_const: in the CTA-wide set-up tid < 12, 32..67 and 96; while warp 0 finishes the previous tile the
+// transform moves to 128..139.  -1: none.  Each entry takes a few dependent L2 loads, so they are spread over warps.
+__device__ __forceinline__ int tile_const_entry(int tid, bool warp0_busy) {
+	if (tid >= 32 && tid < 68) return 12 + (tid - 32);
+	if (tid == 96) return 48;
+	const int m = warp0_busy ? tid - 128 : tid;
+	return (m >= 0 && m < 12) ? m : -1;
+}
 template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(SolveArgs a) {
 	extern __shared__ __align__(16) float dyn_smem[];
 	__shared__ int s_tile, s_it, s_idx;
 	__shared__ Tile s_tl[2];      // the tile being processed and the one claimed for the next round (thread 0 fetches its record a tile ahead)
+	// the tile's constants.  s_pre[] = 1: written (and the tile's iteration flag acquired) by warps 1.. while warp 0 finished the previous
+	// tile, so the tile starts on its pixels at once.  Only X, which warp 0's epilogue reads, needs a second buffer; the pixel loop reads
+	// s_M and s_G at fixed addresses.
 	__shared__ __align__(16) float s_M[12];
 	__shared__ __align__(16) float s_G[12];
-	__shared__ float s_X[36];
+	__shared__ float s_X[2][36];
+	__shared__ int s_pre[2], s_nxt;
 	__shared__ float s_red[kTileVals];
 	__shared__ float s_part[(NT / 32)][kTileVals];
 	__shared__ int s_is_last, s_p2_claim;
@@ -1365,7 +1414,7 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 	if (fixed && (int)blockIdx.x >= total) return;
 	if (tid == 0) {
 		const int t0 = fixed ? (int)blockIdx.x : atomicAdd(a.queue, 1);
-		s_tile = t0; s_p2_claim = 0;
+		s_tile = t0; s_p2_claim = 0; s_pre[0] = 0;
 		if (t0 < all) { const int it0 = t0 / total; s_it = it0; s_idx = t0 - it0 * total; s_tl[0] = a.tiles[t0 - it0 * total]; }
 	}
 	int cur = 0;
@@ -1380,7 +1429,8 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 		if (tid == 0) nxt = fixed ? s_tile + total : atomicAdd(a.queue, 1);
 		ProfRec prf; PROF_T(0);
 		const WinDesc& wd = a.wins[tl.win];      // (fields are read where they are used: geometry in the pixel loop, the rest in the tail)
-		if (it > 0) {   // this window's previous GN iteration must have published its poses
+		const bool pre = s_pre[cur] != 0;
+		if (it > 0 && !pre) {   // this window's previous GN iteration must have published its poses
 			if (tid == 0) { while (ld_relaxed(a.iter_done + tl.win) < it) __nanosleep(64); (void)ld_acquire(a.iter_done + tl.win); }
 			__syncthreads();
 		}
@@ -1397,6 +1447,7 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 				s_is_last = (done == (it + 1) * tl.n_tiles_win);
 				s_tile = nxt;
 				if (nxt < all) { s_it = itn; s_idx = idxn; }
+				s_pre[cur ^ 1] = 0;
 				tile_fetch_wait();
 			}
 			PROF_T(4);
@@ -1406,30 +1457,11 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 #pragma unroll
 		for (int k = 0; k < kTileVals; k++) acc.v[k] = 0.f;
 		if (tl.pair >= 0) {
-			if (tid < 12) {   // transform = T_i^-1 T_j (rigid inverse), row r, col c
-				const float* Ti = a.T + (size_t)tl.tgt_slot * 12;
-				const float* Tj = a.T + (size_t)tl.src_slot * 12;
-				const int r = tid >> 2, c = tid & 3;
-				float v = 0.f;
-				for (int k = 0; k < 3; k++) {
-					const float rik = __ldcg(Ti + k * 4 + r);          // R_i^T (r,k) = R_i(k,r)
-					v += rik * ((c < 3) ? __ldcg(Tj + k * 4 + c) : (__ldcg(Tj + k * 4 + 3) - __ldcg(Ti + k * 4 + 3)));
-				}
-				s_M[tid] = v;
-			} else if (tid >= 32 && tid < 68) {   // X_i = [[R,0],[[t]x R, R]] of the TARGET frame: maps the tile's sums to the model frame
-				const float* Ti = a.T + (size_t)tl.tgt_slot * 12;
-				const int e = tid - 32, r = e / 6, c = e - r * 6;
-				float v;
-				if (r < 3) v = (c < 3) ? __ldcg(Ti + r * 4 + c) : 0.f;
-				else if (c >= 3) v = __ldcg(Ti + (r - 3) * 4 + (c - 3));
-				else { const float t3[3] = { __ldcg(Ti + 3), __ldcg(Ti + 7), __ldcg(Ti + 11) }; v = 0.f; for (int kk = 0; kk < 3; kk++) v += skew(t3, r - 3, kk) * __ldcg(Ti + kk * 4 + c); }
-				s_X[e] = v;
-			} else if (tid == 96) {   // the window's projection / texel geometry, read by the pixel loop where it is used
-				s_G[0] = wd.fx; s_G[1] = wd.fy; s_G[2] = wd.cx; s_G[3] = wd.cy;
-				s_G[4] = wd.tg.ifx; s_G[5] = wd.tg.ify; s_G[6] = wd.tg.icx; s_G[7] = wd.tg.icy;
-				s_G[8] = wd.tg.scaleW; s_G[9] = wd.tg.scaleH; s_G[10] = __int_as_float(wd.w); s_G[11] = __int_as_float(wd.h);
+			if (!pre) {
+				const int e = tile_const_entry(tid, false);
+				if (e >= 0) tile_const(a, tl, e, s_M, s_X[cur], s_G);
 			}
-			__syncthreads();
+			if (!pre) __syncthreads();
 			PROF_T(2);
 			tile_pixels<NT>(a, tl.src, tl.tex, s_M, s_G, tl.start, tl.count, acc);
 		}
@@ -1445,6 +1477,7 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 			butterfly_step<16>(v, lane);
 			if (lane < kTileVals) s_part[wid][lane] = v[0];
 		}
+		if (tid == 0) { s_nxt = nxt; if (!fixed) tile_fetch_wait(); }      // (warps 1.. read the next tile's record after the barrier)
 		__syncthreads();
 		if (wid == 0) {   // warp 0 finishes the tile: cross-warp sum, model-frame transform, store, ticket
 			float red = 0.f;
@@ -1462,7 +1495,7 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 						const int r = c_sym_r[lane], c = c_sym_c[lane];
 						float xr[6], xc[6];
 #pragma unroll
-						for (int u = 0; u < 6; u++) { xr[u] = s_X[r * 6 + u]; xc[u] = s_X[c * 6 + u]; }   // zero entries make the short rows exact
+						for (int u = 0; u < 6; u++) { xr[u] = s_X[cur][r * 6 + u]; xc[u] = s_X[cur][c * 6 + u]; }   // zero entries make the short rows exact
 #pragma unroll
 						for (int u = 0; u < 6; u++) {
 							float tsum = 0.f;
@@ -1473,7 +1506,7 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 					} else {
 						const int r = lane - 21;
 #pragma unroll
-						for (int u = 0; u < 6; u++) out += s_X[r * 6 + u] * s_red[21 + u];
+						for (int u = 0; u < 6; u++) out += s_X[cur][r * 6 + u] * s_red[21 + u];
 					}
 				}
 				__stcg(a.partial + (size_t)tl_idx * kTileVals + lane, out);
@@ -1484,7 +1517,26 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 				s_is_last = (done == (it + 1) * tl.n_tiles_win);
 				s_tile = nxt;
 				if (nxt < all) { s_it = itn; s_idx = idxn; }
-				tile_fetch_wait();
+				if (fixed) tile_fetch_wait();
+			}
+		} else if (fixed) {   // (the next tile is this window's next iteration: its flag waits for this tile's ticket)
+			if (tid == 32) s_pre[cur ^ 1] = 0;
+		} else {   // warps 1..: the next tile's set-up while warp 0 finishes this one, when its iteration flag is already set
+			const int nx = s_nxt;
+			const Tile& tn = s_tl[cur ^ 1];
+			if (tid == 32) {
+				int ok = 0;
+				if (nx < all) {
+					const int itx = nx / total;
+					ok = itx == 0 || ld_relaxed(a.iter_done + tn.win) >= itx;
+					if (ok && itx > 0) (void)ld_acquire(a.iter_done + tn.win);
+				}
+				s_pre[cur ^ 1] = ok;
+			}
+			asm volatile("bar.sync 2, %0;" ::"r"(NT - 32) : "memory");      // (barrier 1 belongs to the tail's PCG)
+			if (s_pre[cur ^ 1] && tn.pair >= 0) {
+				const int e = tile_const_entry(tid, true);
+				if (e >= 0) tile_const(a, tn, e, s_M, s_X[cur ^ 1], s_G);      // (every warp is past its pixels)
 			}
 		}
 		PROF_T(4);
