@@ -62,22 +62,23 @@ struct TexelGeom {
 	float scaleW, scaleH;             // (W-1)/(w-1), (H-1)/(h-1)  (CUDAImageUtil.cu:57-58)
 };
 
+// What the frame preparation needs of a window: uploaded before k_prep_frames is launched.
 struct WinDesc {
-	int n_frames, n_corr, n_groups, n_pairs;
-	int corr_off, grp_off, pair_off, frame_off;
+	int n_frames, n_pairs, pair_off, frame_off;
 	int tile_off, n_tiles;            // per GN iteration; written by the tile plan (last CTA of k_prep_frames)
 	int H, W, w, h;                   // full / quarter resolution
 	float fx, fy, cx, cy;             // quarter-res intrinsics (CUDACache.cpp:20-24)
 	TexelGeom tg;
 	int compat_flip;
-	int mem_off;                      // per-frame membership CSR of this window (see SolveArgs::mem)
-	int unique_blocks;                // 1: no two groups / no two dense pairs share an unordered frame pair => cross blocks need no atomics
 	int pad[3];
 };
 
-// The correspondence-side fields of a window, uploaded AFTER the frame preparation has been launched (the host scans the
-// correspondences while the GPU already works); window_tail reads them from here, the copies inside WinDesc are unused.
-struct WinSparse { int n_corr, n_groups, corr_off, grp_off, mem_off, unique_blocks, pad0, pad1; };
+// What arrives with a window's correspondences: uploaded AFTER the frame preparation has been launched (the host scans the
+// correspondences while the GPU already works).
+struct WinSparse {
+	int n_corr, n_groups, corr_off, grp_off, mem_off;      // mem_off: per-frame membership CSR of this window (see SolveArgs::mem)
+	int unique_blocks, pad0, pad1;    // 1: no two groups / no two dense pairs share an unordered frame pair => cross blocks need no atomics
+};
 
 // One unit of work of k_solve.  Everything the tile's prologue needs travels in the record (frame slots, map pointers, the window's
 // tile count), so that claiming a tile costs ONE dependent load - and that one is issued a whole tile ahead (k_solve keeps the next
@@ -952,16 +953,15 @@ template <int NT> __device__ void sparse_sums(const SolveArgs& a, int w, int par
 	}
 }
 
-template <int NT> __device__ void window_tail(const SolveArgs& a, const WinDesc& wd_in, int w, int it, float* smem_base, int* p2_claim) {
-	WinDesc wd = wd_in;
-	{ const WinSparse ws = a.wsp[w]; wd.n_corr = ws.n_corr; wd.n_groups = ws.n_groups; wd.corr_off = ws.corr_off; wd.grp_off = ws.grp_off; wd.mem_off = ws.mem_off; wd.unique_blocks = ws.unique_blocks; }
+// (wd and ws by value: every field is loaded once, not again behind each barrier)
+template <int NT> __device__ void window_tail(const SolveArgs& a, const WinDesc wd, const WinSparse ws, int w, int it, float* smem_base, int* p2_claim) {
 	const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
 	static_assert(NT >= 6 * (kMaxFrames - 1), "the PCG runs one thread per unknown");
-	const int N = wd.n_frames, P = wd.n_pairs, G = wd.n_groups;
+	const int N = wd.n_frames, P = wd.n_pairs, G = ws.n_groups;
 	TailSmem s;
 	const bool gsm = a.grp_in_smem != 0;
 	tail_carve(smem_base, N, P, G, s, gsm);
-	const float* grp_g = a.grp_sums + (size_t)wd.grp_off * kGrpVals;      // the same sums in global memory (written with st.cg by the sparse tile)
+	const float* grp_g = a.grp_sums + (size_t)ws.grp_off * kGrpVals;      // the same sums in global memory (written with st.cg by the sparse tile)
 	const int dimp = s.dimp, ld = s.ld;
 	const float wS = a.prm.w_sparse;
 	const bool use_dense = a.prm.w_dense > 0.f && P > 0;
@@ -1030,15 +1030,15 @@ template <int NT> __device__ void window_tail(const SolveArgs& a, const WinDesc&
 			const float4* Gg = reinterpret_cast<const float4*>(grp_g);
 			for (int k = tid; k < G * (kGrpVals / 4); k += H) cp_async16_cg(reinterpret_cast<float4*>(s.grp) + k, Gg + k);
 		}
-		for (int k = tid; k < G; k += H) { cp_async4(s.gi + k, a.grp_i + wd.grp_off + k); cp_async4(s.gj + k, a.grp_j + wd.grp_off + k); }
-		for (int k = tid; k <= G; k += H) cp_async4(s.gstart + k, a.grp_start + wd.grp_off + w + k);
+		for (int k = tid; k < G; k += H) { cp_async4(s.gi + k, a.grp_i + ws.grp_off + k); cp_async4(s.gj + k, a.grp_j + ws.grp_off + k); }
+		for (int k = tid; k <= G; k += H) cp_async4(s.gstart + k, a.grp_start + ws.grp_off + w + k);
 		for (int k = tid; k < P; k += H) {
 			const uint2* pr = a.pairs + wd.pair_off + k;
 			cp_async4(s.pt + k, &pr->x); cp_async4(s.ps + k, &pr->y);
 			cp_async4(s.pt0 + k, a.pair_tile0 + wd.pair_off + k); cp_async4(s.pnt + k, a.pair_ntile + wd.pair_off + k);
 		}
 		{
-			const int* mem = a.mem + wd.mem_off;     // fg_start[N+1] fp_start[N+1] fg_items[2G] fp_items[2P], contiguous like the smem copy
+			const int* mem = a.mem + ws.mem_off;     // fg_start[N+1] fp_start[N+1] fg_items[2G] fp_items[2P], contiguous like the smem copy
 			const int nmem = 2 * (N + 1) + 2 * G + 2 * P;
 			for (int k = tid; k < nmem; k += H) cp_async4(s.fg_start + k, mem + k);
 		}
@@ -1147,7 +1147,7 @@ template <int NT> __device__ void window_tail(const SolveArgs& a, const WinDesc&
 	PROF_T(5);
 	// ---- P4a: sparse cross blocks (i,j): J_i^T J_j, both frames free.  One thread per (group, 3x3 sub-block): uniform code per
 	//      thread, 9 entries each.  Sub-blocks: 0 = TT (-n I), 1 = TR ([sum s]x), 2 = RT (-[sum q]x), 3 = RR (-((q.s) I - s q^T)).
-	const bool uniq = wd.unique_blocks != 0;
+	const bool uniq = ws.unique_blocks != 0;
 	for (int k = tid; k < G * 4; k += NT) {
 		const int g = k >> 2, sb = k & 3;
 		const int gi = s.gi[g], gj = s.gj[g];
@@ -1545,7 +1545,7 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 		PROF_T(5);
 		if (a.prof && tid == 0) { prf.kind_cta = blockIdx.x; prf.tile_win = ((long long)tl_idx << 32) | ((long long)it << 16) | tl.count; prf.t[6] = prf.t[7] = prf.t[8] = prf.t[9] = 0; prof_emit(a, prf); }
 		if (s_is_last) {
-			window_tail<NT>(a, wd, tl.win, it, dyn_smem, &s_p2_claim);
+			window_tail<NT>(a, wd, a.wsp[tl.win], tl.win, it, dyn_smem, &s_p2_claim);
 			__threadfence();
 			__syncthreads();
 			if (tid == 0) st_release(a.iter_done + tl.win, it + 1);
@@ -1603,6 +1603,7 @@ struct SolverState {
 	// last staged batch
 	int n_windows = 0, frames_total = 0, smem_bytes = 0, chunk = 1024;
 	bt_solver_params prm{};
+	float d2max = 0.f;                   // SolveArgs::d2max of prm.dense_dist_thresh
 	std::vector<int> frame_off;
 	std::vector<int> n_frames;
 	bool staged = false, debug = false, timing = false;
@@ -1699,28 +1700,22 @@ static FrameGeom frame_geom(int H, int W, float fx, float fy, float cx, float cy
 	return g;
 }
 
-static SolveArgs make_args(bt_ctx* ctx);
 static int launch_prep(bt_ctx* ctx, cudaStream_t stream);
+static double us_since(std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count(); }
 
-// Staging order (what makes the fused call fast): everything the frame preparation needs (window descriptors, frame
-// pointers, poses, pair tables - ~100 KB) is built and uploaded first and, in the fused call, k_prep_frames is launched
-// right there; only then are the correspondences (the bulk: 32 B each) copied into pinned memory and uploaded in
-// chunks on a private copy stream, overlapping the kernel.  k_solve waits on the last chunk's event.
-static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, const bt_solver_params* params,
-                      const float* poses_in, void* stream_, bool early_prep) {
-	BT_REQUIRE(ctx && windows && params && poses_in, BT_ERR_INVALID_ARG, "bt_solve_stage: NULL argument");
-	BT_REQUIRE(ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_stage: call bt_solver_reserve first");
-	SolverState* s = ctx->solver.get();
-	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
-	BT_REQUIRE(n_windows > 0 && n_windows <= s->lim.max_windows, BT_ERR_CAPACITY, "bt_solve_stage: %d windows > reserved %d", n_windows, s->lim.max_windows);
-	BT_REQUIRE(params->num_iter_outer > 0 && params->num_iter_inner > 0 && params->image_downscale == s->lim.image_downscale, BT_ERR_INVALID_ARG,
-	           "bt_solve_stage: iteration counts must be positive and image_downscale must equal the reserved value");
-	s->staged = false; s->prep_launched = false;
-	const auto t_h0 = std::chrono::steady_clock::now();
-	auto us_since = [](std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count(); };
-	// ---- sizes
-	size_t F = 0, C = 0;
+// Largest float d2max with `sqrtf(d2) <= dist_t` <=> `d2 <= d2max` for every float d2 (sqrtf is correctly rounded and monotonic)
+static float dense_d2max(float th) {
+	if (!(th > 0.f)) return (th == 0.f) ? 0.f : -1.f;
+	auto nextf = [](float v, int d) { int32_t b; memcpy(&b, &v, 4); b += d; float r; memcpy(&r, &b, 4); return r; };
+	float d2max = th * th;
+	while (d2max > 0.f && sqrtf(d2max) > th) d2max = nextf(d2max, -1);
+	while (sqrtf(nextf(d2max, 1)) <= th) d2max = nextf(d2max, 1);
+	return d2max;
+}
+
+// Every window against what was reserved; F / C = frames / correspondences of the batch.
+static int validate_windows(const SolverState* s, int n_windows, const bt_window* windows, const bt_solver_params* params, size_t* F, size_t* C) {
+	*F = 0; *C = 0;
 	for (int w = 0; w < n_windows; w++) {
 		const bt_window& bw = windows[w];
 		BT_REQUIRE(bw.n_frames >= 2 && bw.n_frames <= s->lim.max_frames, BT_ERR_CAPACITY, "window %d: n_frames %d outside [2,%d]", w, bw.n_frames, s->lim.max_frames);
@@ -1741,26 +1736,23 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 		BT_REQUIRE((int)(bw.W / params->image_downscale) >= 2 && (int)(bw.H / params->image_downscale) >= 2, BT_ERR_INVALID_ARG, "window %d: image too small", w);
 		BT_REQUIRE(bw.corr_dev || bw.n_corr == 0 || bw.corr, BT_ERR_INVALID_ARG, "window %d: corr is NULL", w);
 		BT_REQUIRE(params->w_dense <= 0.f || bw.cache_slots || (bw.depth_dev && bw.normal_dev), BT_ERR_INVALID_ARG, "window %d: depth/normal pointers are NULL and no cache slots given", w);
-		F += bw.n_frames; C += (size_t)nc;
+		*F += bw.n_frames; *C += (size_t)nc;
 	}
-	// ---- host staging: one pinned block mirrored by one device block
-	const size_t maxP = (size_t)s->max_pairs, maxG = (size_t)s->max_groups;
-	const StageLayout L = stage_layout(n_windows, F, C, s->lim.max_frames, maxG, maxP);
-	BT_REQUIRE(L.total <= s->stage_buf[0].bytes, BT_ERR_CAPACITY, "bt_solve_stage: staging block %zu > reserved %zu bytes", L.total, s->stage_buf[0].bytes);
-	int rc;
-	char* hb;
-	BT_TRY(s->h_stage.acquire(L.total, &hb));
+	return BT_OK;
+}
+
+// What the frame preparation needs, with no look at the correspondences: window geometry, where each frame slot's maps live (a cache
+// slot or the call's own pointers), poses, the dense pair list with each pair's window and source slot.  *n_pairs = pairs of the batch.
+static int fill_frame_tables(SolverState* s, int n_windows, const bt_window* windows, const bt_solver_params* params, const float* poses_in,
+                             char* hb, const StageLayout& L, size_t* n_pairs) {
 	WinDesc* hw = (WinDesc*)(hb + L.wins);
 	const void** hdp = (const void**)(hb + L.dp); const void** hnp = (const void**)(hb + L.np);
 	const void** htex = (const void**)(hb + L.texp); const void** hsrc = (const void**)(hb + L.srcp); const void** hnsrc = (const void**)(hb + L.nsrcp);
-	int* hfw = (int*)(hb + L.fw); float* hpose = (float*)(hb + L.pose); bt_entryj* hcorr = (bt_entryj*)(hb + L.corr);
-	WinSparse* hws = (WinSparse*)(hb + L.wsp);
-	int* hgi = (int*)(hb + L.gi); int* hgj = (int*)(hb + L.gj); int* hgs = (int*)(hb + L.gs); uint2* hpairs = (uint2*)(hb + L.pairs);
-	int* hpwin = (int*)(hb + L.pwin); int* hpsrc = (int*)(hb + L.psrc); int* hmem = (int*)(hb + L.mem);
+	int* hfw = (int*)(hb + L.fw); float* hpose = (float*)(hb + L.pose);
+	uint2* hpairs = (uint2*)(hb + L.pairs); int* hpwin = (int*)(hb + L.pwin); int* hpsrc = (int*)(hb + L.psrc);
+	const bool dense = params->w_dense > 0.f;
 	s->frame_off.assign(n_windows, 0); s->n_frames.assign(n_windows, 0);
-
 	s->any_uncached = false;
-	// ==== phase 1: what the frame preparation needs - geometry, frame tables, poses, dense pair tables (no look at the correspondences)
 	size_t f_off = 0, p_off = 0;
 	for (int w = 0; w < n_windows; w++) {
 		const bt_window& bw = windows[w];
@@ -1776,7 +1768,7 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 		s->frame_off[w] = (int)f_off; s->n_frames[w] = N;
 		for (int f = 0; f < N; f++) {
 			const size_t fs = f_off + f;
-			if (bw.cache_slots && params->w_dense > 0.f) {     // maps built earlier by bt_frame_cache_store
+			if (bw.cache_slots && dense) {     // maps built earlier by bt_frame_cache_store
 				const int cs = bw.cache_slots[f];
 				BT_REQUIRE(cs >= 0 && cs < s->c_capacity && s->c_meta[cs].valid, BT_ERR_INVALID_ARG, "window %d frame %d: cache slot %d is empty or out of range", w, f, cs);
 				const SolverState::CacheMeta& m = s->c_meta[cs];
@@ -1787,17 +1779,16 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 				htex[fs] = s->c_texel.as<float4>() + (size_t)cs * s->c_npix; hsrc[fs] = s->c_src.as<float4>() + (size_t)cs * 2 * s->c_npix;
 				hnsrc[fs] = s->c_nsrc.as<int>() + cs;
 			} else {
-				hdp[fs] = (params->w_dense > 0.f) ? bw.depth_dev[f] : nullptr;
-				hnp[fs] = (params->w_dense > 0.f) ? bw.normal_dev[f] : nullptr;
+				hdp[fs] = dense ? bw.depth_dev[f] : nullptr; hnp[fs] = dense ? bw.normal_dev[f] : nullptr;
 				htex[fs] = s->texel.as<float4>() + fs * (size_t)s->npix_max; hsrc[fs] = s->src.as<float4>() + fs * 2 * (size_t)s->npix_max;
 				hnsrc[fs] = nullptr;
-				if (params->w_dense > 0.f) s->any_uncached = true;
+				if (dense) s->any_uncached = true;
 			}
 			hfw[fs] = w;
 			memcpy(hpose + fs * 16, poses_in + fs * 16, sizeof(float) * 16);
 		}
 		int np = 0;
-		if (params->w_dense > 0.f) {
+		if (dense) {
 			if (bw.dense_pairs) {
 				BT_REQUIRE(bw.n_dense_pairs >= 0 && bw.n_dense_pairs <= s->max_pairs, BT_ERR_CAPACITY, "window %d: %d dense pairs > %d", w, bw.n_dense_pairs, s->max_pairs);
 				for (int p = 0; p < bw.n_dense_pairs; p++) {
@@ -1813,208 +1804,232 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 		for (int p = 0; p < np; p++) { hpwin[p_off + p] = w; hpsrc[p_off + p] = (int)f_off + (int)hpairs[p_off + p].y; }
 		f_off += N; p_off += np;
 	}
-	s->n_windows = n_windows; s->frames_total = (int)f_off; s->prm = *params;
-	// chunk: aim for >= 4 tiles per SM-resident CTA over the batch, between 256 and 2048 source pixels
-	{
-		const long long est_px = (long long)p_off * (s->npix_max / 8);   // ~12 % valid
+	*n_pairs = p_off;
+	return BT_OK;
+}
+
+// How a window's entries reach the device block: through the pinned block (or none to move), in place from page-locked caller memory, from corr_dev
+enum class CorrFrom { Staged, InPlace, Device };
+
+// Groups one window's correspondences by (i,j): gi / gj / gs[ng + 1] (starts relative to the window's first entry), *n_valid entries kept,
+// and how they reach the device (*src: where they are, unless that is `staged`, the window's slice of the pinned block).  Four input forms:
+// blocks on the device; host entries in blocks the caller names; host entries already grouped; anything else.  Issues no CUDA copy.
+static int group_window(const bt_window& bw, int w, bt_entryj* staged, int* gi, int* gj, int* gs, std::vector<int>& bin,
+                        int* ng_out, int* n_valid_out, CorrFrom* how, const bt_entryj** src) {
+	static_assert(offsetof(bt_entryj, imgIdx_i) == 0 && offsetof(bt_entryj, imgIdx_j) == 4, "EntryJ header layout");
+	const int N = bw.n_frames;
+	int n_valid = 0, ng = 0; bool grouped = true;    // keys (i*N+j) non-decreasing and no invalid entries => groups are runs, the entries stay in their order
+	*how = CorrFrom::Staged; *src = nullptr;
+	if (bw.corr_dev) {      // every non-empty block is a group
+		for (int b = 0; b < bw.n_blocks; b++) {
+			if (bw.block_n[b] == 0) continue;
+			gi[ng] = (int)bw.block_i[b]; gj[ng] = (int)bw.block_j[b]; gs[ng] = n_valid; ng++;
+			n_valid += bw.block_n[b];
+		}
+		if (n_valid) { *how = CorrFrom::Device; *src = bw.corr_dev + bw.block_off[0]; }      // nothing to copy on the host
+	} else if (bw.block_n && bw.n_blocks > 0) {
+		// the caller names the blocks (Bundler::optimizeGPU emits the entries pair by pair and hands n_match_per_pair along,
+		// /root/reference/src/Bundler.cpp:298-351): only the first entry of every block is read - no pass over the 64 KB of a window
+		long long off = 0;
+		for (int b = 0; b < bw.n_blocks; b++) {
+			const int nb = bw.block_n[b];
+			BT_REQUIRE(nb >= 0 && off + nb <= bw.n_corr, BT_ERR_INVALID_ARG, "window %d: correspondence block %d overruns n_corr", w, b);
+			if (nb == 0) continue;
+			const uint32_t ei = bw.block_i ? bw.block_i[b] : bw.corr[off].imgIdx_i, ej = bw.block_j ? bw.block_j[b] : bw.corr[off].imgIdx_j;
+			BT_REQUIRE(ei < (uint32_t)N && ej < (uint32_t)N, BT_ERR_INVALID_ARG, "window %d: correspondence block %d references a frame outside [0,%d)", w, b, N);
+			gi[ng] = (int)ei; gj[ng] = (int)ej; gs[ng] = (int)off; ng++;
+			off += nb;
+		}
+		BT_REQUIRE(off == bw.n_corr, BT_ERR_INVALID_ARG, "window %d: the correspondence blocks cover %lld of %d entries", w, off, bw.n_corr);
+	} else {
+		// one 8-byte compare per entry (imgIdx_i | imgIdx_j << 32, little endian); range and order are only checked where a run ends
+		unsigned long long prev_raw = 0ull; long long prev_key = -1; bool have_prev = false;
+		for (int c = 0; c < bw.n_corr; c++) {
+			unsigned long long raw; memcpy(&raw, &bw.corr[c], sizeof raw);
+			if (have_prev && raw == prev_raw) continue;
+			const uint32_t ei = (uint32_t)raw, ej = (uint32_t)(raw >> 32);
+			if (ei >= (uint32_t)N || ej >= (uint32_t)N) { grouped = false; break; }
+			const long long key = (long long)ei * N + ej;
+			if (key < prev_key) { grouped = false; break; }
+			gi[ng] = (int)ei; gj[ng] = (int)ej; gs[ng] = c; ng++;
+			prev_raw = raw; prev_key = key; have_prev = true;
+		}
+	}
+	if (!bw.corr_dev && grouped) {
+		n_valid = bw.n_corr;
+		if (n_valid) {
+			// Caller's buffer page-locked (cudaHostAlloc / cudaHostRegister / bt_host_alloc_pinned)?  Then the copy engine reads it in
+			// place - no staging copy - and windows whose buffers follow each other in memory share one transfer.
+			cudaPointerAttributes pa;
+			if (cudaPointerGetAttributes(&pa, bw.corr) == cudaSuccess && pa.type == cudaMemoryTypeHost) { *how = CorrFrom::InPlace; *src = bw.corr; }
+			else memcpy(staged, bw.corr, sizeof(bt_entryj) * (size_t)n_valid);      // the window's entries are still in cache from the scan
+		}
+	} else if (!bw.corr_dev) {
+		// stable counting sort by (i,j) so each pair's entries are contiguous (Bundler::optimizeGPU already emits them that way,
+		// /root/reference/src/Bundler.cpp:298-324); invalid entries are dropped
+		ng = 0;
+		bin.assign((size_t)N * N + 1, 0);
+		for (int c = 0; c < bw.n_corr; c++) {
+			const bt_entryj& e = bw.corr[c];
+			if (e.imgIdx_i == 0xFFFFFFFFu) continue;
+			BT_REQUIRE(e.imgIdx_i < (uint32_t)N && e.imgIdx_j < (uint32_t)N, BT_ERR_INVALID_ARG, "window %d: correspondence %d references frame outside [0,%d)", w, c, N);
+			bin[(size_t)e.imgIdx_i * N + e.imgIdx_j + 1]++;
+			n_valid++;
+		}
+		for (size_t b = 0; b < (size_t)N * N; b++) {      // counts -> starts; every non-empty bin is a group
+			if (bin[b + 1] > 0) { gi[ng] = (int)(b / N); gj[ng] = (int)(b % N); gs[ng] = bin[b]; ng++; }
+			bin[b + 1] += bin[b];
+		}
+		for (int c = 0; c < bw.n_corr; c++) {
+			const bt_entryj& e = bw.corr[c];
+			if (e.imgIdx_i == 0xFFFFFFFFu) continue;
+			staged[bin[(size_t)e.imgIdx_i * N + e.imgIdx_j]++] = e;
+		}
+	}
+	gs[ng] = n_valid;
+	// a group that pairs a frame with itself has no counterpart in the moment form of the sparse term (DESIGN.md §4): refused
+	for (int g = 0; g < ng; g++) BT_REQUIRE(gi[g] != gj[g], BT_ERR_INVALID_ARG, "window %d: correspondences pair frame %d with itself", w, gi[g]);
+	*ng_out = ng; *n_valid_out = n_valid; return BT_OK;
+}
+
+// A window's per-frame membership CSR at `mem` (layout: SolveArgs::mem): the groups, then the dense pairs, touching each frame, in increasing index
+// order (fixed summation order); returns its length in ints.  *unique_blocks: every unordered frame pair occurs at most once per table.
+static size_t window_membership(int N, int ng, int np, const int* gi, const int* gj, const uint2* pairs, int* mem, std::vector<char>& seen, int* unique_blocks) {
+	bool uq = true; seen.assign((size_t)N * N, 0);
+	for (int g = 0; g < ng && uq; g++) { const int a2 = std::min(gi[g], gj[g]), b2 = std::max(gi[g], gj[g]); if (seen[(size_t)a2 * N + b2]) uq = false; seen[(size_t)a2 * N + b2] = 1; }
+	std::fill(seen.begin(), seen.end(), 0);
+	for (int p = 0; p < np && uq; p++) { const int a2 = (int)std::min(pairs[p].x, pairs[p].y), b2 = (int)std::max(pairs[p].x, pairs[p].y); if (seen[(size_t)a2 * N + b2]) uq = false; seen[(size_t)a2 * N + b2] = 1; }
+	*unique_blocks = uq ? 1 : 0;
+	int* fg_start = mem; int* fp_start = fg_start + (N + 1); int* fg_items = fp_start + (N + 1); int* fp_items = fg_items + 2 * ng;
+	auto csr = [N](int* start, int* items, int n, auto first, auto second) {      // per frame f: the k with first(k) == f, or (role 1) second(k) == f
+		int q = 0;
+		for (int f = 0; f < N; f++) {
+			start[f] = q;
+			for (int k = 0; k < n; k++) {
+				if (first(k) == f) items[q++] = k;
+				else if (second(k) == f) items[q++] = k | (1 << 16);
+			}
+		}
+		start[N] = q;
+	};
+	csr(fg_start, fg_items, ng, [gi](int g) { return gi[g]; }, [gj](int g) { return gj[g]; });
+	csr(fp_start, fp_items, np, [pairs](int p) { return (int)pairs[p].x; }, [pairs](int p) { return (int)pairs[p].y; });
+	return (size_t)(2 * (N + 1) + 2 * ng + 2 * np);
+}
+
+// The correspondence uploads of one batch, in order on the copy stream.  Entries staged in the pinned block go up in pieces of >= 256 KB;
+// entries in page-locked caller memory are read in place, buffers that follow each other in memory as one transfer; blocks on the device are
+// copied device -> device.  The last two leave a hole in the pinned block, so whatever is staged below the hole is flushed first.
+struct CorrUpload {
+	char* dev; const bt_entryj* pinned; cudaStream_t stream;      // entry 0 of the device block and of the pinned block
+	size_t sent = 0;                  // entries [0, sent) are uploaded or belong to the pending run
+	const bt_entryj* run_src = nullptr; size_t run_dst = 0, run_n = 0;      // pending in-place transfer
+	int staged(size_t upto) { return (upto - sent) * sizeof(bt_entryj) >= 256 * 1024 ? flush(upto) : BT_OK; }      // host entries now fill the pinned block up to `upto`
+	int in_place(const bt_entryj* src, size_t at, size_t n) {
+		BT_TRY(flush(at));
+		if (run_n && run_src + run_n == src && run_dst + run_n == at) run_n += n;      // extends the pending run
+		else { BT_TRY(send_run()); run_src = src; run_dst = at; run_n = n; }
+		sent = at + n; return BT_OK;
+	}
+	int from_device(const bt_entryj* src, size_t at, size_t n) {
+		BT_TRY(flush(at));
+		BT_CUDA(cudaMemcpyAsync(dev + at * sizeof(bt_entryj), src, n * sizeof(bt_entryj), cudaMemcpyDeviceToDevice, stream));
+		sent = at + n; return BT_OK;
+	}
+	int finish(size_t upto) { BT_TRY(flush(upto)); return send_run(); }
+private:
+	int flush(size_t upto) {
+		if (upto > sent) BT_CUDA(cudaMemcpyAsync(dev + sent * sizeof(bt_entryj), pinned + sent, (upto - sent) * sizeof(bt_entryj), cudaMemcpyHostToDevice, stream));
+		sent = upto; return BT_OK;
+	}
+	int send_run() {
+		if (run_n) BT_CUDA(cudaMemcpyAsync(dev + run_dst * sizeof(bt_entryj), run_src, run_n * sizeof(bt_entryj), cudaMemcpyHostToDevice, stream));
+		run_n = 0; return BT_OK;
+	}
+};
+
+// Staging order (what makes the fused call fast): everything the frame preparation needs (window descriptors, frame
+// pointers, poses, pair tables - ~100 KB) is built and uploaded first and, in the fused call, k_prep_frames is launched
+// right there; only then are the correspondences (the bulk: 32 B each) grouped and uploaded on a private copy stream,
+// overlapping the kernel.  k_solve waits on the last copy's event.
+static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, const bt_solver_params* params,
+                      const float* poses_in, void* stream_, bool early_prep) {
+	BT_REQUIRE(ctx && windows && params && poses_in, BT_ERR_INVALID_ARG, "bt_solve_stage: NULL argument");
+	BT_REQUIRE(ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_stage: call bt_solver_reserve first");
+	SolverState* s = ctx->solver.get();
+	cudaStream_t stream = (cudaStream_t)stream_;
+	BT_CUDA(cudaSetDevice(ctx->device));
+	BT_REQUIRE(n_windows > 0 && n_windows <= s->lim.max_windows, BT_ERR_CAPACITY, "bt_solve_stage: %d windows > reserved %d", n_windows, s->lim.max_windows);
+	BT_REQUIRE(params->num_iter_outer > 0 && params->num_iter_inner > 0 && params->image_downscale == s->lim.image_downscale, BT_ERR_INVALID_ARG,
+	           "bt_solve_stage: iteration counts must be positive and image_downscale must equal the reserved value");
+	s->staged = false; s->prep_launched = false;
+	const auto t_h0 = std::chrono::steady_clock::now();
+	size_t F, C, n_pairs;
+	BT_TRY(validate_windows(s, n_windows, windows, params, &F, &C));
+	// ---- lay out the pinned block (mirrored by one device block) and fill what the frame preparation needs
+	const StageLayout L = stage_layout(n_windows, F, C, s->lim.max_frames, (size_t)s->max_groups, (size_t)s->max_pairs);
+	BT_REQUIRE(L.total <= s->stage_buf[0].bytes, BT_ERR_CAPACITY, "bt_solve_stage: staging block %zu > reserved %zu bytes", L.total, s->stage_buf[0].bytes);
+	char* hb; BT_TRY(s->h_stage.acquire(L.total, &hb));
+	BT_TRY(fill_frame_tables(s, n_windows, windows, params, poses_in, hb, L, &n_pairs));
+	s->n_windows = n_windows; s->frames_total = (int)F; s->prm = *params; s->d2max = dense_d2max(params->dense_dist_thresh); s->layout = L;
+	{   // chunk: aim for >= 4 tiles per SM-resident CTA over the batch, between 256 and 2048 source pixels
+		const long long est_px = (long long)n_pairs * (s->npix_max / 8);   // ~12 % valid
 		long long c = est_px / ((long long)ctx->sm_count * 2 * 4);
 		c = std::max(256LL, std::min(2048LL, c));
 		s->chunk = s->force_chunk ? s->force_chunk : (int)((c + 255) / 256 * 256);
 	}
-	s->layout = L;
+	// ---- early upload.  Two device staging blocks, used alternately: every upload of this batch runs on the private copy stream and only waits for
+	// the k_solve that last read THIS block (two batches ago), so with the streaming form the 2 MB of batch k+1 cross PCIe while batch k is being solved.
 	BT_TRY(s->copy_stream.create());
-	// Two device staging blocks, used alternately: every upload of this batch runs on the private copy stream and only waits for the
-	// k_solve that last read THIS block (two batches ago) - so with the streaming form the 2 MB of batch k+1 cross PCIe while batch k is
-	// still being solved.  (With one block the uploads would queue behind the previous k_solve.)
 	s->stage_cur ^= 1;
 	DevBuf& stage_dev = s->stage_buf[s->stage_cur];
 	if (s->ev_stage_free[s->stage_cur]) BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_stage_free[s->stage_cur], 0));
-	{   // correspondence blocks produced on the device (bt_match_pairs on the caller's stream) are copied device -> device on the copy stream: order them
-		bool any_dev = false;
-		for (int w = 0; w < n_windows && !any_dev; w++) any_dev = windows[w].corr_dev != nullptr;
-		if (any_dev) { BT_TRY(s->ev_prev.record(stream)); BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_prev, 0)); }
+	// correspondence blocks produced on the device (bt_match_pairs on the caller's stream) are copied device -> device on the copy stream: order them
+	if (std::any_of(windows, windows + n_windows, [](const bt_window& bw) { return bw.corr_dev != nullptr; })) {
+		BT_TRY(s->ev_prev.record(stream)); BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_prev, 0));
 	}
-	// early tables first; the caller's stream (frame prep in the fused call) waits for them only
 	BT_CUDA(cudaMemcpyAsync(stage_dev.p, hb, L.late, cudaMemcpyHostToDevice, s->copy_stream));
 	BT_TRY(s->ev_early.record(s->copy_stream));
-	BT_CUDA(cudaStreamWaitEvent(stream, s->ev_early, 0));
+	BT_CUDA(cudaStreamWaitEvent(stream, s->ev_early, 0));      // the caller's stream (frame prep in the fused call) waits for the early tables only
 	s->host_us[0] = us_since(t_h0);
-	if (early_prep) { if ((rc = launch_prep(ctx, stream)) != BT_OK) return rc; }
+	if (early_prep) BT_TRY(launch_prep(ctx, stream));
 	s->host_us[1] = us_since(t_h0) - s->host_us[0];
-
-	// ==== phase 2 (the GPU is already busy in the fused call): correspondences -> groups, membership CSR, pinned copy, chunked upload
-	size_t c_off = 0, g_off = 0, m_off = 0, smem_need = 0, smem_lean = 0, sent = 0;
-	const bt_entryj* run_src = nullptr; size_t run_dst = 0, run_n = 0;      // pending in-place transfer from page-locked caller memory
-	std::vector<int> bin;
-	std::vector<char> seen;
-	p_off = 0;
+	// ---- per window (the GPU is already busy in the fused call): group the correspondences, upload them, membership CSR
+	const WinDesc* hw = (const WinDesc*)(hb + L.wins); WinSparse* hws = (WinSparse*)(hb + L.wsp);
+	int* hgi = (int*)(hb + L.gi); int* hgj = (int*)(hb + L.gj); int* hgs = (int*)(hb + L.gs); int* hmem = (int*)(hb + L.mem);
+	const uint2* hpairs = (const uint2*)(hb + L.pairs); bt_entryj* hcorr = (bt_entryj*)(hb + L.corr);
+	CorrUpload up{stage_dev.as<char>() + L.corr, hcorr, s->copy_stream};
+	size_t c_off = 0, g_off = 0, m_off = 0, p_off = 0, smem_need = 0, smem_lean = 0;
+	std::vector<int> bin; std::vector<char> seen;
 	for (int w = 0; w < n_windows; w++) {
-		const bt_window& bw = windows[w];
-		const int N = bw.n_frames, np = hw[w].n_pairs;
-		const size_t f_off_w = (size_t)hw[w].frame_off;
-		(void)f_off_w;
-		// correspondences: stable counting sort by (i,j) so each pair's entries are contiguous (Bundler::optimizeGPU
-		// already emits them that way, /root/reference/src/Bundler.cpp:298-324); invalid entries are dropped.
-		int n_valid = 0, ng = 0;
-		bool grouped = true;    // fast path: keys (i*N+j) non-decreasing and no invalid entries => groups are runs, plain copy
-		if (bw.corr_dev) {      // blocks produced on the device: every non-empty block is a group, the entries move device -> device
-			for (int b = 0; b < bw.n_blocks; b++) {
-				if (bw.block_n[b] == 0) continue;
-				hgi[g_off + ng] = (int)bw.block_i[b]; hgj[g_off + ng] = (int)bw.block_j[b]; hgs[g_off + w + ng] = n_valid; ng++;
-				n_valid += bw.block_n[b];
-			}
-			hgs[g_off + w + ng] = n_valid;
-			if (n_valid) {
-				if (c_off > sent) {     // flush what the host path has staged so far: the pinned block has a hole where this window's entries would be
-					BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.corr + sent * sizeof(bt_entryj), hcorr + sent, (c_off - sent) * sizeof(bt_entryj), cudaMemcpyHostToDevice, s->copy_stream));
-				}
-				BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.corr + c_off * sizeof(bt_entryj), bw.corr_dev + bw.block_off[0], (size_t)n_valid * sizeof(bt_entryj),
-				                        cudaMemcpyDeviceToDevice, s->copy_stream));
-				sent = c_off + n_valid;
-			}
-		} else {
-			static_assert(offsetof(bt_entryj, imgIdx_i) == 0 && offsetof(bt_entryj, imgIdx_j) == 4, "EntryJ header layout");
-			if (bw.block_n && bw.n_blocks > 0) {
-				// the caller names the blocks (Bundler::optimizeGPU emits the entries pair by pair and hands n_match_per_pair along,
-				// /root/reference/src/Bundler.cpp:298-351): only the first entry of every block is read - no pass over the 64 KB of a window
-				long long off = 0;
-				for (int b = 0; b < bw.n_blocks; b++) {
-					const int nb = bw.block_n[b];
-					BT_REQUIRE(nb >= 0 && off + nb <= bw.n_corr, BT_ERR_INVALID_ARG, "window %d: correspondence block %d overruns n_corr", w, b);
-					if (nb == 0) continue;
-					const uint32_t ei = bw.block_i ? bw.block_i[b] : bw.corr[off].imgIdx_i, ej = bw.block_j ? bw.block_j[b] : bw.corr[off].imgIdx_j;
-					BT_REQUIRE(ei < (uint32_t)N && ej < (uint32_t)N, BT_ERR_INVALID_ARG, "window %d: correspondence block %d references a frame outside [0,%d)", w, b, N);
-					hgi[g_off + ng] = (int)ei; hgj[g_off + ng] = (int)ej; hgs[g_off + w + ng] = (int)off; ng++;
-					off += nb;
-				}
-				BT_REQUIRE(off == bw.n_corr, BT_ERR_INVALID_ARG, "window %d: the correspondence blocks cover %lld of %d entries", w, off, bw.n_corr);
-			} else {
-			// one 8-byte compare per entry (imgIdx_i | imgIdx_j << 32, little endian); range and order are only checked where a run ends
-			unsigned long long prev_raw = 0ull;
-			bool have_prev = false;
-			long long prev_key = -1;
-			for (int c = 0; c < bw.n_corr; c++) {
-				unsigned long long raw;
-				memcpy(&raw, &bw.corr[c], sizeof raw);
-				if (have_prev && raw == prev_raw) continue;
-				const uint32_t ei = (uint32_t)raw, ej = (uint32_t)(raw >> 32);
-				if (ei >= (uint32_t)N || ej >= (uint32_t)N) { grouped = false; break; }
-				const long long key = (long long)ei * N + ej;
-				if (key < prev_key) { grouped = false; break; }
-				hgi[g_off + ng] = (int)ei; hgj[g_off + ng] = (int)ej; hgs[g_off + w + ng] = c; ng++;
-				prev_raw = raw; prev_key = key; have_prev = true;
-			}
-			}
-		}
-		if (bw.corr_dev) {
-			// nothing to copy on the host
-		} else if (grouped) {
-			n_valid = bw.n_corr;
-			hgs[g_off + w + ng] = n_valid;
-			if (n_valid) {
-				// Caller's buffer page-locked (cudaHostAlloc / cudaHostRegister / bt_host_alloc_pinned)?  Then the copy engine reads it in
-				// place - no staging copy - and windows whose buffers follow each other in memory share one transfer.
-				cudaPointerAttributes pa;
-				const bool pinned_src = cudaPointerGetAttributes(&pa, bw.corr) == cudaSuccess && pa.type == cudaMemoryTypeHost;
-				if (pinned_src) {
-					if (c_off > sent) {      // flush what was staged so far: the staging block has a hole where this window's entries would be
-						BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.corr + sent * sizeof(bt_entryj), hcorr + sent, (c_off - sent) * sizeof(bt_entryj), cudaMemcpyHostToDevice, s->copy_stream));
-					}
-					if (run_n && run_src + run_n == bw.corr && run_dst + run_n == c_off) run_n += (size_t)n_valid;      // extends the pending run
-					else {
-						if (run_n) BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.corr + run_dst * sizeof(bt_entryj), run_src, run_n * sizeof(bt_entryj), cudaMemcpyHostToDevice, s->copy_stream));
-						run_src = bw.corr; run_dst = c_off; run_n = (size_t)n_valid;
-					}
-					sent = c_off + n_valid;
-				} else {
-					memcpy(hcorr + c_off, bw.corr, sizeof(bt_entryj) * (size_t)n_valid);      // the window's entries are still in cache from the scan
-				}
-			}
-		} else {
-			ng = 0;
-			bin.assign((size_t)N * N + 1, 0);
-			for (int c = 0; c < bw.n_corr; c++) {
-				const bt_entryj& e = bw.corr[c];
-				if (e.imgIdx_i == 0xFFFFFFFFu) continue;
-				BT_REQUIRE(e.imgIdx_i < (uint32_t)N && e.imgIdx_j < (uint32_t)N, BT_ERR_INVALID_ARG, "window %d: correspondence %d references frame outside [0,%d)", w, c, N);
-				bin[(size_t)e.imgIdx_i * N + e.imgIdx_j + 1]++;
-				n_valid++;
-			}
-			for (size_t b = 0; b < (size_t)N * N; b++) {
-				if (bin[b + 1] > 0) { hgi[g_off + ng] = (int)(b / N); hgj[g_off + ng] = (int)(b % N); ng++; }
-			}
-			for (size_t b = 0; b < (size_t)N * N; b++) bin[b + 1] += bin[b];
-			{   // group starts (relative to corr_off); stored at grp_off + w + g to leave room for the extra end entry
-				int gg = 0;
-				for (size_t b = 0; b < (size_t)N * N; b++) if (bin[b + 1] > bin[b]) hgs[g_off + w + gg++] = bin[b];
-				hgs[g_off + w + ng] = n_valid;
-			}
-			for (int c = 0; c < bw.n_corr; c++) {
-				const bt_entryj& e = bw.corr[c];
-				if (e.imgIdx_i == 0xFFFFFFFFu) continue;
-				hcorr[c_off + bin[(size_t)e.imgIdx_i * N + e.imgIdx_j]++] = e;
-			}
-		}
-		// a group that pairs a frame with itself has no counterpart in the moment form of the sparse term (DESIGN.md §4): refused
-		for (int g = 0; g < ng; g++)
-			BT_REQUIRE(hgi[g_off + g] != hgj[g_off + g], BT_ERR_INVALID_ARG, "window %d: correspondences pair frame %d with itself", w, hgi[g_off + g]);
+		const int N = windows[w].n_frames, np = hw[w].n_pairs;
+		int* gi = hgi + g_off; int* gj = hgj + g_off; int* gs = hgs + g_off + w;      // every window's group starts have one extra end entry
+		int ng, n_valid; CorrFrom how; const bt_entryj* src;
+		BT_TRY(group_window(windows[w], w, hcorr + c_off, gi, gj, gs, bin, &ng, &n_valid, &how, &src));
+		if (how == CorrFrom::Device) BT_TRY(up.from_device(src, c_off, (size_t)n_valid));
+		else if (how == CorrFrom::InPlace) BT_TRY(up.in_place(src, c_off, (size_t)n_valid));
 		WinSparse& ws = hws[w];
 		memset(&ws, 0, sizeof ws);
 		ws.n_corr = n_valid; ws.n_groups = ng; ws.corr_off = (int)c_off; ws.grp_off = (int)g_off; ws.mem_off = (int)m_off;
-		{   // cross blocks are written without atomics when every unordered frame pair occurs at most once per table
-			seen.assign((size_t)N * N, 0);
-			bool uq = true;
-			for (int g = 0; g < ng && uq; g++) { const int a2 = std::min(hgi[g_off + g], hgj[g_off + g]), b2 = std::max(hgi[g_off + g], hgj[g_off + g]); if (seen[(size_t)a2 * N + b2]) uq = false; seen[(size_t)a2 * N + b2] = 1; }
-			std::fill(seen.begin(), seen.end(), 0);
-			for (int p = 0; p < np && uq; p++) { const int a2 = (int)std::min(hpairs[p_off + p].x, hpairs[p_off + p].y), b2 = (int)std::max(hpairs[p_off + p].x, hpairs[p_off + p].y); if (seen[(size_t)a2 * N + b2]) uq = false; seen[(size_t)a2 * N + b2] = 1; }
-			ws.unique_blocks = uq ? 1 : 0;
-		}
-		{   // per-frame membership CSR: groups then pairs touching each frame, in increasing index order (fixed summation order)
-			int* fg_start = hmem + m_off; int* fp_start = fg_start + (N + 1); int* fg_items = fp_start + (N + 1); int* fp_items = fg_items + 2 * ng;
-			int q = 0;
-			for (int f = 0; f < N; f++) {
-				fg_start[f] = q;
-				for (int g = 0; g < ng; g++) {
-					if (hgi[g_off + g] == f) fg_items[q++] = g;
-					else if (hgj[g_off + g] == f) fg_items[q++] = g | (1 << 16);
-				}
-			}
-			fg_start[N] = q;
-			q = 0;
-			for (int f = 0; f < N; f++) {
-				fp_start[f] = q;
-				for (int p = 0; p < np; p++) {
-					if ((int)hpairs[p_off + p].x == f) fp_items[q++] = p;
-					else if ((int)hpairs[p_off + p].y == f) fp_items[q++] = p | (1 << 16);
-				}
-			}
-			fp_start[N] = q;
-			m_off += (size_t)(2 * (N + 1) + 2 * ng + 2 * np);
-		}
+		m_off += window_membership(N, ng, np, gi, gj, hpairs + p_off, hmem + m_off, seen, &ws.unique_blocks);
 		smem_need = std::max(smem_need, tail_smem_floats(N, np, ng) * sizeof(float));
 		smem_lean = std::max(smem_lean, tail_smem_floats(N, np, ng, false) * sizeof(float));
 		c_off += n_valid; g_off += ng; p_off += np;
-		// upload what has accumulated once it is worth a copy (>= 256 KB), and whatever is left after the last window
-		if ((c_off - sent) * sizeof(bt_entryj) >= 256 * 1024 || (w + 1 == n_windows && c_off > sent)) {
-			BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.corr + sent * sizeof(bt_entryj), hcorr + sent, (c_off - sent) * sizeof(bt_entryj), cudaMemcpyHostToDevice, s->copy_stream));
-			sent = c_off;
-		}
+		BT_TRY(up.staged(c_off));
 	}
-	if (run_n) BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.corr + run_dst * sizeof(bt_entryj), run_src, run_n * sizeof(bt_entryj), cudaMemcpyHostToDevice, s->copy_stream));
-	s->grp_in_smem = smem_need <= kTailSmemMax;
-	if (!s->grp_in_smem) smem_need = smem_lean;
+	BT_TRY(up.finish(c_off));
+	s->grp_in_smem = smem_need <= kTailSmemMax; if (!s->grp_in_smem) smem_need = smem_lean;
 	BT_REQUIRE(smem_need <= kTailSmemMax, BT_ERR_CAPACITY, "bt_solve_stage: window needs %zu bytes of shared memory (> %d KB)", smem_need, (int)(kTailSmemMax / 1024));
 	s->smem_bytes = (int)smem_need;
-	BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.late, hb + L.late, L.corr - L.late, cudaMemcpyHostToDevice, s->copy_stream));      // group tables, CSR, WinSparse
+	BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.late, hb + L.late, L.corr - L.late, cudaMemcpyHostToDevice, s->copy_stream));      // ---- late upload: group tables, CSR, WinSparse
 	BT_TRY(s->h_stage.in_flight(s->copy_stream));
 	BT_CUDA(cudaStreamWaitEvent(stream, s->h_stage.ev, 0));     // everything later on the caller's stream sees the correspondences
 	if (s->debug) {
-		const int st = 6 * s->lim.max_frames;
-		if ((rc = s->dbgJ.alloc(sizeof(float) * (size_t)st * st * s->lim.max_windows)) != BT_OK) return rc;
-		if ((rc = s->dbgR.alloc(sizeof(float) * (size_t)st * s->lim.max_windows)) != BT_OK) return rc;
-		if ((rc = s->dbgC.alloc(sizeof(float) * (size_t)s->max_pairs * s->lim.max_windows)) != BT_OK) return rc;
-		const int sp = 6 * (s->lim.max_frames - 1);
-		if ((rc = s->dbgS.alloc(sizeof(float) * (size_t)sp * (sp + 3) * s->lim.max_windows)) != BT_OK) return rc;
+		const int st = 6 * s->lim.max_frames, sp = 6 * (s->lim.max_frames - 1);
+		BT_TRY(s->dbgJ.alloc(sizeof(float) * (size_t)st * st * s->lim.max_windows));
+		BT_TRY(s->dbgR.alloc(sizeof(float) * (size_t)st * s->lim.max_windows));
+		BT_TRY(s->dbgC.alloc(sizeof(float) * (size_t)s->max_pairs * s->lim.max_windows));
+		BT_TRY(s->dbgS.alloc(sizeof(float) * (size_t)sp * (sp + 3) * s->lim.max_windows));
 	}
 	s->staged = true;
 	s->host_us[2] = us_since(t_h0) - s->host_us[0] - s->host_us[1];
@@ -2058,17 +2073,7 @@ static SolveArgs make_args(bt_ctx* ctx) {
 	a.pair_tile0 = s->pair_tile0.as<int>(); a.pair_ntile = s->pair_ntile.as<int>();
 	a.n_tiles_total = s->scalars.as<int>(); a.queue = s->scalars.as<int>() + 1; a.n_src_px = (long long*)(s->scalars.as<char>() + 16);
 	a.tiles_done = s->tiles_done.as<int>(); a.iter_done = s->iter_done.as<int>();
-	a.chunk = s->chunk; a.grp_in_smem = s->grp_in_smem ? 1 : 0; a.prm = s->prm; a.grid_ctas = ctx->sm_count * s->occ;
-	{   // `sqrtf(d2) <= dist_t` <=> `d2 <= d2max` for every float d2 (sqrtf is correctly rounded and monotonic)
-		const float th = s->prm.dense_dist_thresh;
-		float d2max = th * th;
-		auto nextf = [](float v, int d) { int32_t b; memcpy(&b, &v, 4); b += d; float r; memcpy(&r, &b, 4); return r; };
-		if (th > 0.f) {
-			while (d2max > 0.f && sqrtf(d2max) > th) d2max = nextf(d2max, -1);
-			while (sqrtf(nextf(d2max, 1)) <= th) d2max = nextf(d2max, 1);
-		} else d2max = (th == 0.f) ? 0.f : -1.f;
-		a.d2max = d2max;
-	}
+	a.chunk = s->chunk; a.grp_in_smem = s->grp_in_smem ? 1 : 0; a.prm = s->prm; a.d2max = s->d2max; a.grid_ctas = ctx->sm_count * s->occ;
 	if (s->prof_cap > 0) { a.prof = s->prof.as<long long>(); a.prof_cap = s->prof_cap; }
 	if (s->debug) { a.dbg_JtJ = s->dbgJ.as<float>(); a.dbg_Jtr = s->dbgR.as<float>(); a.dbg_stride = 6 * s->lim.max_frames; a.dbg_cnt = s->dbgC.as<float>(); a.dbg_cnt_stride = s->max_pairs;
 	                a.dbg_sys = s->dbgS.as<float>(); a.dbg_sys_stride = 6 * (s->lim.max_frames - 1); }
@@ -2077,7 +2082,7 @@ static SolveArgs make_args(bt_ctx* ctx) {
 
 static int launch_prep(bt_ctx* ctx, cudaStream_t stream) {
 	SolverState* s = ctx->solver.get();
-	// (in the fused call the tail's shared-memory size is not known yet: the tile plan then aims at the occupancy of the last batch)
+	// make_args again at run time: grid_ctas and grp_in_smem are only final there (in the fused call the tile plan aims at the last batch's occupancy)
 	SolveArgs a = make_args(ctx);
 	if (s->timing) BT_CUDA(cudaEventRecord(s->ev[0], stream));
 	// frames whose maps come from the frame cache need one block each (source count + pose); a batch of cached frames only skips the count kernel
@@ -2095,7 +2100,7 @@ extern "C" int bt_solve_run(bt_ctx* ctx, void* stream_) {
 	SolverState* s = ctx->solver.get();
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
-	{ int rco = ensure_occupancy(ctx); if (rco != BT_OK) return rco; }
+	BT_TRY(ensure_occupancy(ctx));
 	SolveArgs a = make_args(ctx);
 	if (s->debug) {
 		BT_CUDA(cudaMemsetAsync(s->dbgJ.p, 0, s->dbgJ.bytes, stream));
@@ -2103,7 +2108,7 @@ extern "C" int bt_solve_run(bt_ctx* ctx, void* stream_) {
 		BT_CUDA(cudaMemsetAsync(s->dbgS.p, 0, s->dbgS.bytes, stream));
 	}
 	if (s->prof_cap > 0) BT_CUDA(cudaMemsetAsync(s->prof.p, 0, 8, stream));
-	if (!s->prep_launched) { int rcp = launch_prep(ctx, stream); if (rcp != BT_OK) return rcp; }
+	if (!s->prep_launched) BT_TRY(launch_prep(ctx, stream));
 	s->prep_launched = false;       // a second bt_solve_run on the same staged batch prepares again (poses restart from the staged input)
 	if (s->timing) BT_CUDA(cudaEventRecord(s->ev[2], stream));
 	const int occ = s->occ;
@@ -2116,35 +2121,41 @@ extern "C" int bt_solve_run(bt_ctx* ctx, void* stream_) {
 	return BT_OK;
 }
 
+// Queues, on `stream`, the download of the staged batch's poses and - behind them - the 32 bytes of scalars (tile count first) into `h`.
+static int queue_pose_download(SolverState* s, PinnedBuf& h, cudaStream_t stream) {
+	const size_t bytes = sizeof(float) * 16 * (size_t)s->frames_total;
+	BT_TRY(h.alloc(bytes + 64));
+	BT_CUDA(cudaMemcpyAsync(h.p, s->pose_out.p, bytes, cudaMemcpyDeviceToHost, stream));
+	BT_CUDA(cudaMemcpyAsync(h.as<char>() + bytes, s->scalars.p, 32, cudaMemcpyDeviceToHost, stream));
+	return BT_OK;
+}
+// Hands out the poses of a completed download, unless the tile plan reported an overflow.
+static int take_poses(const PinnedBuf& h, int frames, float* poses_out, const char* who) {
+	const size_t bytes = sizeof(float) * 16 * (size_t)frames;
+	const int n_tiles_total = *(const int*)(h.as<char>() + bytes);
+	BT_REQUIRE(n_tiles_total >= 0, BT_ERR_CAPACITY, "%s: tile list overflow (more dense tiles than reserved)", who);
+	memcpy(poses_out, h.p, bytes);
+	return BT_OK;
+}
+
 extern "C" int bt_solve_fetch(bt_ctx* ctx, float* poses_out, void* stream_) {
 	BT_REQUIRE(ctx && ctx->solver && ctx->solver->staged && poses_out, BT_ERR_INVALID_ARG, "bt_solve_fetch: nothing staged / NULL output");
 	SolverState* s = ctx->solver.get();
-	cudaStream_t stream = (cudaStream_t)stream_;
-	const size_t bytes = sizeof(float) * 16 * (size_t)s->frames_total;
-	int rc = s->h_poses.alloc(bytes + 64);
-	if (rc != BT_OK) return rc;
-	BT_CUDA(cudaMemcpyAsync(s->h_poses.p, s->pose_out.p, bytes, cudaMemcpyDeviceToHost, stream));
-	BT_CUDA(cudaMemcpyAsync(s->h_poses.as<char>() + bytes, s->scalars.p, 32, cudaMemcpyDeviceToHost, stream));
-	BT_CUDA(cudaStreamSynchronize(stream));
-	const int total = *(int*)(s->h_poses.as<char>() + bytes);
-	BT_REQUIRE(total >= 0, BT_ERR_CAPACITY, "bt_solve_fetch: tile list overflow (more dense tiles than reserved)");
-	memcpy(poses_out, s->h_poses.p, bytes);
-	return BT_OK;
+	BT_TRY(queue_pose_download(s, s->h_poses, (cudaStream_t)stream_));
+	BT_CUDA(cudaStreamSynchronize((cudaStream_t)stream_));
+	return take_poses(s->h_poses, s->frames_total, poses_out, "bt_solve_fetch");
 }
 
 extern "C" int bt_solve_windows(bt_ctx* ctx, int n_windows, const bt_window* windows, const bt_solver_params* params,
                                 float* poses_inout, void* stream) {
 	const auto t0 = std::chrono::steady_clock::now();
-	auto us = [&]() { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count(); };
-	int rc = stage_impl(ctx, n_windows, windows, params, poses_inout, stream, true);
-	if (rc != BT_OK) return rc;
-	const double t1 = us();
-	rc = bt_solve_run(ctx, stream);
-	if (rc != BT_OK) return rc;
-	const double t2 = us();
-	rc = bt_solve_fetch(ctx, poses_inout, stream);
+	BT_TRY(stage_impl(ctx, n_windows, windows, params, poses_inout, stream, true));
+	const double t1 = us_since(t0);
+	BT_TRY(bt_solve_run(ctx, stream));
+	const double t2 = us_since(t0);
+	const int rc = bt_solve_fetch(ctx, poses_inout, stream);
 	SolverState* s = ctx->solver.get();
-	s->host_us[3] = t2 - t1; s->host_us[4] = us() - t2; s->host_us[5] = us();
+	s->host_us[3] = t2 - t1; s->host_us[4] = us_since(t0) - t2; s->host_us[5] = us_since(t0);
 	return rc;
 }
 
@@ -2156,16 +2167,10 @@ extern "C" int bt_solve_windows_begin(bt_ctx* ctx, int n_windows, const bt_windo
 	SolverState* s = ctx->solver.get();
 	const int slot = s->pipe_head;
 	BT_REQUIRE(!s->pipe_pending[slot], BT_ERR_INVALID_ARG, "bt_solve_windows_begin: two batches are already in flight - call bt_solve_windows_end first");
-	int rc = stage_impl(ctx, n_windows, windows, params, poses_in, stream_, true);
-	if (rc != BT_OK) return rc;
-	rc = bt_solve_run(ctx, stream_);
-	if (rc != BT_OK) return rc;
-	cudaStream_t stream = (cudaStream_t)stream_;
-	const size_t bytes = sizeof(float) * 16 * (size_t)s->frames_total;
-	BT_TRY(s->h_pipe[slot].alloc(bytes + 64));
-	BT_CUDA(cudaMemcpyAsync(s->h_pipe[slot].p, s->pose_out.p, bytes, cudaMemcpyDeviceToHost, stream));
-	BT_CUDA(cudaMemcpyAsync(s->h_pipe[slot].as<char>() + bytes, s->scalars.p, 32, cudaMemcpyDeviceToHost, stream));
-	BT_TRY(s->ev_pipe[slot].record(stream));
+	BT_TRY(stage_impl(ctx, n_windows, windows, params, poses_in, stream_, true));
+	BT_TRY(bt_solve_run(ctx, stream_));
+	BT_TRY(queue_pose_download(s, s->h_pipe[slot], (cudaStream_t)stream_));
+	BT_TRY(s->ev_pipe[slot].record((cudaStream_t)stream_));
 	s->pipe_pending[slot] = true; s->pipe_frames[slot] = s->frames_total; s->pipe_head ^= 1;
 	return BT_OK;
 }
@@ -2176,11 +2181,7 @@ extern "C" int bt_solve_windows_end(bt_ctx* ctx, float* poses_out) {
 	BT_REQUIRE(s->pipe_pending[slot], BT_ERR_INVALID_ARG, "bt_solve_windows_end: no batch in flight");
 	BT_CUDA(cudaEventSynchronize(s->ev_pipe[slot]));
 	s->pipe_pending[slot] = false; s->pipe_tail ^= 1;
-	const size_t bytes = sizeof(float) * 16 * (size_t)s->pipe_frames[slot];
-	const int total = *(int*)(s->h_pipe[slot].as<char>() + bytes);
-	BT_REQUIRE(total >= 0, BT_ERR_CAPACITY, "bt_solve_windows_end: tile list overflow (more dense tiles than reserved)");
-	memcpy(poses_out, s->h_pipe[slot].p, bytes);
-	return BT_OK;
+	return take_poses(s->h_pipe[slot], s->pipe_frames[slot], poses_out, "bt_solve_windows_end");
 }
 
 // Host time of the last bt_solve_windows call, microseconds: {window tables + first upload, frame-prep launch, correspondence scan +
@@ -2198,11 +2199,10 @@ extern "C" int bt_frame_cache_reserve(bt_ctx* ctx, int capacity, int H, int W, f
 	BT_CUDA(cudaSetDevice(ctx->device));
 	const int w = (int)(W / image_downscale), h = (int)(H / image_downscale);
 	BT_REQUIRE(w >= 2 && h >= 2, BT_ERR_INVALID_ARG, "bt_frame_cache_reserve: image too small");
-	int rc;
-	if ((rc = s->c_texel.alloc(sizeof(float4) * (size_t)w * h * capacity)) != BT_OK) return rc;
-	if ((rc = s->c_src.alloc(sizeof(float4) * 2 * (size_t)w * h * capacity)) != BT_OK) return rc;
-	if ((rc = s->c_nsrc.alloc(sizeof(int) * (size_t)capacity)) != BT_OK) return rc;
-	if ((rc = s->c_blk.alloc(sizeof(int) * (size_t)capacity * ((w * h + 1023) / 1024))) != BT_OK) return rc;
+	BT_TRY(s->c_texel.alloc(sizeof(float4) * (size_t)w * h * capacity));
+	BT_TRY(s->c_src.alloc(sizeof(float4) * 2 * (size_t)w * h * capacity));
+	BT_TRY(s->c_nsrc.alloc(sizeof(int) * (size_t)capacity));
+	BT_TRY(s->c_blk.alloc(sizeof(int) * (size_t)capacity * ((w * h + 1023) / 1024)));
 	s->c_capacity = capacity; s->c_npix = w * h; s->c_downscale = image_downscale;
 	s->c_meta.assign(capacity, SolverState::CacheMeta());
 	return BT_OK;
@@ -2268,7 +2268,7 @@ extern "C" int bt_solve_get_stats(bt_ctx* ctx, bt_solve_stats* out) {
 extern "C" int bt_solve_enable_profile(bt_ctx* ctx, int max_records) {
 	BT_REQUIRE(ctx && ctx->solver && max_records >= 0, BT_ERR_INVALID_ARG, "bt_solve_enable_profile: call bt_solver_reserve first");
 	SolverState* s = ctx->solver.get();
-	if (max_records > 0) { int rc = s->prof.alloc(8 + (size_t)max_records * 96); if (rc != BT_OK) return rc; }
+	if (max_records > 0) BT_TRY(s->prof.alloc(8 + (size_t)max_records * 96));
 	s->prof_cap = max_records;
 	return BT_OK;
 }
