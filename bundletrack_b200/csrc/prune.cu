@@ -267,118 +267,145 @@ extern "C" int bt_pipeline_reserve(bt_ctx* ctx, int max_pairs, int max_feats, in
 	return s->h_pairs.reserve(sizeof(PrunePair) * max_pairs);
 }
 
-// prop_room > 0 (bt_find_corres_pairs): no host extras; pair p keeps room for prop_room propagated matches behind its mutual ones, and its
-// candidates go to extra[p * prop_room, ...) when the device table writes them
-static int fill_pairs(PruneState* s, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, cudaStream_t stream, const bt_match_extra* extra = nullptr,
-                      int prop_room = 0) {
-	PrunePair* hp;
-	float4* hx;
-	BT_TRY(s->h_pairs.acquire(0, &hp));
-	BT_TRY(s->h_extra.acquire(0, &hx));
-	int offA = 0, offB = 0, out = 0, xoff = 0;
-	for (int p = 0; p < n_pairs; p++) {
-		const bt_match_frame* fr[2] = { &A[p], &B[p] };
-		PruneFrame* dst[2] = { &hp[p].A, &hp[p].B };
-		for (int s2 = 0; s2 < 2; s2++) {
-			BT_REQUIRE(fr[s2]->n >= 0 && fr[s2]->n <= s->max_feats, BT_ERR_CAPACITY, "pair %d: %d features > reserved %d", p, fr[s2]->n, s->max_feats);
-			BT_REQUIRE(fr[s2]->n == 0 || (fr[s2]->kpts_dev && fr[s2]->depth_dev && fr[s2]->normal_dev), BT_ERR_INVALID_ARG, "pair %d: NULL frame pointer", p);
-			dst[s2]->kpts = reinterpret_cast<const float2*>(fr[s2]->kpts_dev); dst[s2]->n = fr[s2]->n; dst[s2]->frame_id = fr[s2]->frame_id;
-			dst[s2]->depth = fr[s2]->depth_dev; dst[s2]->normal = reinterpret_cast<const float4*>(fr[s2]->normal_dev);
-			memcpy(dst[s2]->T, fr[s2]->pose, sizeof(float) * 12);
+namespace {
+// One findCorres call on the context's scratch: each stage of kNN -> prune -> mutual union (+ propagated matches) -> RANSAC -> EntryJ is
+// launched by one method.  prune() reads knn()'s lists and writes corr / n_corr; bt_prune_mutual_pairs points both at the caller's arrays.
+struct Chain {
+	bt_ctx* ctx;
+	PruneState* s;
+	const char* who;                    // the entry point, for its messages
+	int n, trials;                      // pairs, RANSAC trials
+	const bt_match_frame *A, *B;
+	PruneCam cam;
+	const bt_prune_params* prm;
+	float inlier_dist;
+	uint64_t seed;
+	cudaStream_t stream;
+	const int32_t *idxAB = nullptr, *idxBA = nullptr;
+	int k = 0;
+	bt_correspondence* corr;
+	int32_t* n_corr;
+	Chain(bt_ctx* ctx_, const char* who_, int n_pairs, const bt_match_frame* A_, const bt_match_frame* B_, int H, int W, float fx, float fy, float cx, float cy,
+	      const bt_prune_params* prm_, int trials_, float inlier_dist_, uint64_t seed_, void* stream_)
+	    : ctx(ctx_), s(ctx_->prune.get()), who(who_), n(n_pairs), trials(trials_), A(A_), B(B_), cam{ H, W, 1.0f / fx, 1.0f / fy, -cx / fx, -cy / fy },
+	      prm(prm_), inlier_dist(inlier_dist_), seed(seed_), stream((cudaStream_t)stream_), corr(s->corr.as<bt_correspondence>()), n_corr(s->n_corr.as<int32_t>()) {}
+	// both directions, from descriptor views or from descriptor-pool slots: exactly one of the two is given
+	int knn(const bt_desc_view* dA, const bt_desc_view* dB, const int32_t* slotA, const int32_t* slotB) {
+		BT_REQUIRE(((dA && dB) ? 1 : 0) + ((slotA && slotB) ? 1 : 0) == 1, BT_ERR_INVALID_ARG, "%s: give either descriptor views or pool slots", who);
+		k = 5;   // k_near, FeatureManager.cpp:264
+		idxAB = s->idxAB.as<int32_t>(); idxBA = s->idxBA.as<int32_t>();
+		return dA ? bt_knn_match_pairs(ctx, n, dA, dB, k, s->idxAB.as<int32_t>(), s->distAB.as<float>(), s->idxBA.as<int32_t>(), s->distBA.as<float>(), stream)
+		          : bt_knn_match_slots(ctx, n, slotA, slotB, k, s->idxAB.as<int32_t>(), s->distAB.as<float>(), s->idxBA.as<int32_t>(), s->distBA.as<float>(), stream);
+	}
+	// the pair table, uploaded with the host extras.  prop_room > 0 (bt_find_corres_pairs): no host extras; pair p keeps room for prop_room
+	// propagated matches behind its mutual ones, and its candidates go to extra[p * prop_room, ...) when the device table writes them
+	int pairs(const bt_match_extra* extra, int prop_room) {
+		PrunePair* hp;
+		float4* hx;
+		BT_TRY(s->h_pairs.acquire(0, &hp));
+		BT_TRY(s->h_extra.acquire(0, &hx));
+		int offA = 0, offB = 0, out = 0, xoff = 0;
+		for (int p = 0; p < n; p++) {
+			const bt_match_frame* fr[2] = { &A[p], &B[p] };
+			PruneFrame* dst[2] = { &hp[p].A, &hp[p].B };
+			for (int s2 = 0; s2 < 2; s2++) {
+				BT_REQUIRE(fr[s2]->n >= 0 && fr[s2]->n <= s->max_feats, BT_ERR_CAPACITY, "pair %d: %d features > reserved %d", p, fr[s2]->n, s->max_feats);
+				BT_REQUIRE(fr[s2]->n == 0 || (fr[s2]->kpts_dev && fr[s2]->depth_dev && fr[s2]->normal_dev), BT_ERR_INVALID_ARG, "pair %d: NULL frame pointer", p);
+				dst[s2]->kpts = reinterpret_cast<const float2*>(fr[s2]->kpts_dev); dst[s2]->n = fr[s2]->n; dst[s2]->frame_id = fr[s2]->frame_id;
+				dst[s2]->depth = fr[s2]->depth_dev; dst[s2]->normal = reinterpret_cast<const float4*>(fr[s2]->normal_dev);
+				memcpy(dst[s2]->T, fr[s2]->pose, sizeof(float) * 12);
+			}
+			hp[p].idx_off_A = offA; hp[p].idx_off_B = offB; hp[p].out_off = out;
+			hp[p].win_idx_A = A[p].window_index; hp[p].win_idx_B = B[p].window_index;
+			const int nx = (extra && extra[p].n > 0 && abs(A[p].frame_id - B[p].frame_id) != 1) ? extra[p].n : 0;
+			BT_REQUIRE(nx == 0 || extra[p].uv, BT_ERR_INVALID_ARG, "pair %d: NULL propagated-match array", p);
+			BT_REQUIRE(nx <= s->max_feats && (size_t)(xoff + nx) <= s->extra_cap, BT_ERR_CAPACITY, "pair %d: %d propagated matches exceed the reserved room", p, nx);
+			hp[p].n_extra = nx; hp[p].extra_off = prop_room ? p * prop_room : xoff;
+			if (nx) memcpy(hx + xoff, extra[p].uv, sizeof(float4) * (size_t)nx);
+			xoff += nx;
+			offA += A[p].n; offB += B[p].n; out += A[p].n + B[p].n + nx + prop_room;
 		}
-		hp[p].idx_off_A = offA; hp[p].idx_off_B = offB; hp[p].out_off = out;
-		hp[p].win_idx_A = A[p].window_index; hp[p].win_idx_B = B[p].window_index;
-		const int nx = (extra && extra[p].n > 0 && abs(A[p].frame_id - B[p].frame_id) != 1) ? extra[p].n : 0;
-		BT_REQUIRE(nx == 0 || extra[p].uv, BT_ERR_INVALID_ARG, "pair %d: NULL propagated-match array", p);
-		BT_REQUIRE(nx <= s->max_feats && (size_t)(xoff + nx) <= s->extra_cap, BT_ERR_CAPACITY, "pair %d: %d propagated matches exceed the reserved room", p, nx);
-		hp[p].n_extra = nx; hp[p].extra_off = prop_room ? p * prop_room : xoff;
-		if (nx) memcpy(hx + xoff, extra[p].uv, sizeof(float4) * (size_t)nx);
-		xoff += nx;
-		offA += A[p].n; offB += B[p].n; out += A[p].n + B[p].n + nx + prop_room;
+		if (xoff) {
+			BT_CUDA(cudaMemcpyAsync(s->extra.p, hx, sizeof(float4) * (size_t)xoff, cudaMemcpyHostToDevice, stream));
+			BT_TRY(s->h_extra.in_flight(stream));
+		}
+		BT_CUDA(cudaMemcpyAsync(s->pairs.p, hp, sizeof(PrunePair) * n, cudaMemcpyHostToDevice, stream));
+		return s->h_pairs.in_flight(stream);
 	}
-	if (xoff) {
-		BT_CUDA(cudaMemcpyAsync(s->extra.p, hx, sizeof(float4) * (size_t)xoff, cudaMemcpyHostToDevice, stream));
-		BT_TRY(s->h_extra.in_flight(stream));
+	int prune() {
+		k_prune_mutual<<<n, 512, 0, stream>>>(s->pairs.as<PrunePair>(), cam, idxAB, idxBA, k, *prm, corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr);
+		BT_CUDA(cudaGetLastError());
+		return BT_OK;
 	}
-	BT_CUDA(cudaMemcpyAsync(s->pairs.p, hp, sizeof(PrunePair) * n_pairs, cudaMemcpyHostToDevice, stream));
-	return s->h_pairs.in_flight(stream);
-}
-
-static int prune_mutual_impl(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, int H, int W, float fx, float fy, float cx, float cy,
-                             const int32_t* idxAB, const int32_t* idxBA, int k, const bt_prune_params* prm,
-                             bt_correspondence* corr_out, int32_t* n_corr_out, void* stream_, const bt_match_extra* extra) {
-	PruneState* s = ctx ? ctx->prune.get() : nullptr;
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_prune_mutual_pairs: call bt_pipeline_reserve first");
-	BT_REQUIRE(A && B && idxAB && idxBA && prm && corr_out && n_corr_out && n_pairs > 0 && n_pairs <= s->max_pairs && k >= 1 && k <= 8, BT_ERR_INVALID_ARG, "bt_prune_mutual_pairs: bad argument");
-	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
-	int rc = fill_pairs(s, n_pairs, A, B, stream, extra);
-	if (rc != BT_OK) return rc;
-	PruneCam cam; cam.H = H; cam.W = W; cam.ifx = 1.0f / fx; cam.ify = 1.0f / fy; cam.icx = -cx / fx; cam.icy = -cy / fy;
-	k_prune_mutual<<<n_pairs, 512, 0, stream>>>(s->pairs.as<PrunePair>(), cam, idxAB, idxBA, k, *prm, corr_out, s->PA.as<float4>(), s->PB.as<float4>(), n_corr_out);
-	// findCorresByMapPoints for the non-neighbour pairs; also records the matches the two knnMatch directions gave (n_nn)
-	k_append_propagated<<<n_pairs, 256, 0, stream>>>(s->pairs.as<PrunePair>(), cam, s->extra.as<float4>(), corr_out, s->PA.as<float4>(), s->PB.as<float4>(), n_corr_out, s->n_nn.as<int32_t>(), nullptr);
-	BT_CUDA(cudaGetLastError());
-	return BT_OK;
-}
+	// findCorresByMapPoints for pairs [p0, p0 + np), with the pair table's counts or, given n_extra_dev, the ones the device table wrote
+	int append(int p0, int np, const int32_t* n_extra_dev) {
+		k_append_propagated<<<np, 256, 0, stream>>>(s->pairs.as<PrunePair>() + p0, cam, s->extra.as<float4>(), corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr + p0,
+		                                            s->n_nn.as<int32_t>() + p0, n_extra_dev);
+		BT_CUDA(cudaGetLastError());
+		return BT_OK;
+	}
+	int ransac(int p0, int np) {
+		RansacPair* rp = s->rpairs.as<RansacPair>() + p0;
+		k_ransac_table_from_counts<<<(np + 127) / 128, 128, 0, stream>>>(s->pairs.as<PrunePair>() + p0, np, n_corr + p0, s->PA.as<float4>(), s->PB.as<float4>(), rp);
+		BT_CUDA(cudaGetLastError());
+		return ransac_run_device(ctx, rp, np, trials, inlier_dist, seed, s->inl.as<int32_t>(), s->n_inl.as<int32_t>() + p0, stream);
+	}
+	int emit(bt_entryj* entry_out, int capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, int32_t* status_out, float* uv_out) {
+		k_emit_entryj<<<1, 1024, 0, stream>>>(s->pairs.as<PrunePair>(), n, corr, s->inl.as<int32_t>(), s->n_inl.as<int32_t>(), entry_out, n_entry_out, entry_off_out, total_out, capacity, status_out);
+		k_emit_fill<<<n, 256, 0, stream>>>(s->pairs.as<PrunePair>(), corr, s->inl.as<int32_t>(), n_entry_out, entry_off_out, entry_out, capacity, reinterpret_cast<float4*>(uv_out));
+		BT_CUDA(cudaGetLastError());
+		return BT_OK;
+	}
+};
+}  // namespace
 
 extern "C" int bt_prune_mutual_pairs(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, int H, int W, float fx, float fy, float cx, float cy,
                                      const int32_t* idxAB, const int32_t* idxBA, int k, const bt_prune_params* prm,
                                      bt_correspondence* corr_out, int32_t* n_corr_out, void* stream_) {
-	return prune_mutual_impl(ctx, n_pairs, A, B, H, W, fx, fy, cx, cy, idxAB, idxBA, k, prm, corr_out, n_corr_out, stream_, nullptr);
-}
-
-// The whole matcher half of the hot path for a batch of frame pairs, device-resident end to end:
-// kNN (both directions) -> prune -> mutual union -> RANSAC -> EntryJ.  Pair p's entries are contiguous in entry_out.
-static int match_pairs_impl(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, const bt_desc_view* dA, const bt_desc_view* dB,
-                            const int32_t* slotA, const int32_t* slotB, int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune, int ransac_trials,
-                            float ransac_inlier_dist, uint64_t ransac_seed, bt_entryj* entry_out, int entry_capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, void* stream_,
-                            const bt_match_extra* extra = nullptr, int32_t* status_out = nullptr, float* uv_out = nullptr) {
 	PruneState* s = ctx ? ctx->prune.get() : nullptr;
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_match_pairs: call bt_pipeline_reserve first");
-	BT_REQUIRE(A && B && ((dA && dB) || (slotA && slotB)) && prune && entry_out && n_entry_out && entry_off_out && total_out && n_pairs > 0 && n_pairs <= s->max_pairs, BT_ERR_INVALID_ARG, "bt_match_pairs: bad argument");
-	cudaStream_t stream = (cudaStream_t)stream_;
+	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_prune_mutual_pairs: call bt_pipeline_reserve first");
+	BT_REQUIRE(A && B && idxAB && idxBA && prm && corr_out && n_corr_out && n_pairs > 0 && n_pairs <= s->max_pairs && k >= 1 && k <= 8, BT_ERR_INVALID_ARG, "bt_prune_mutual_pairs: bad argument");
 	BT_CUDA(cudaSetDevice(ctx->device));
-	const int k = 5;   // k_near, FeatureManager.cpp:264
-	int rc = dA ? bt_knn_match_pairs(ctx, n_pairs, dA, dB, k, s->idxAB.as<int32_t>(), s->distAB.as<float>(), s->idxBA.as<int32_t>(), s->distBA.as<float>(), stream_)
-	            : bt_knn_match_slots(ctx, n_pairs, slotA, slotB, k, s->idxAB.as<int32_t>(), s->distAB.as<float>(), s->idxBA.as<int32_t>(), s->distBA.as<float>(), stream_);
-	if (rc != BT_OK) return rc;
-	rc = prune_mutual_impl(ctx, n_pairs, A, B, H, W, fx, fy, cx, cy, s->idxAB.as<int32_t>(), s->idxBA.as<int32_t>(), k, prune, s->corr.as<bt_correspondence>(), s->n_corr.as<int32_t>(), stream_, extra);
-	if (rc != BT_OK) return rc;
-	k_ransac_table_from_counts<<<(n_pairs + 127) / 128, 128, 0, stream>>>(s->pairs.as<PrunePair>(), n_pairs, s->n_corr.as<int32_t>(), s->PA.as<float4>(), s->PB.as<float4>(), s->rpairs.as<RansacPair>());
-	rc = ransac_run_device(ctx, s->rpairs.as<RansacPair>(), n_pairs, ransac_trials, ransac_inlier_dist, ransac_seed, s->inl.as<int32_t>(), s->n_inl.as<int32_t>(), stream);
-	if (rc != BT_OK) return rc;
-	k_emit_entryj<<<1, 1024, 0, stream>>>(s->pairs.as<PrunePair>(), n_pairs, s->corr.as<bt_correspondence>(), s->inl.as<int32_t>(), s->n_inl.as<int32_t>(), entry_out, n_entry_out, entry_off_out, total_out, entry_capacity, status_out);
-	k_emit_fill<<<n_pairs, 256, 0, stream>>>(s->pairs.as<PrunePair>(), s->corr.as<bt_correspondence>(), s->inl.as<int32_t>(), n_entry_out, entry_off_out, entry_out, entry_capacity,
-	                                        reinterpret_cast<float4*>(uv_out));
-	BT_CUDA(cudaGetLastError());
-	return BT_OK;
+	Chain c(ctx, "bt_prune_mutual_pairs", n_pairs, A, B, H, W, fx, fy, cx, cy, prm, 0, 0.f, 0, stream_);
+	c.idxAB = idxAB; c.idxBA = idxBA; c.k = k;
+	c.corr = corr_out; c.n_corr = n_corr_out;
+	BT_TRY(c.pairs(nullptr, 0));
+	BT_TRY(c.prune());
+	return c.append(0, n_pairs, nullptr);
 }
 
 extern "C" int bt_match_pairs(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, const bt_desc_view* dA, const bt_desc_view* dB,
                               int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune, int ransac_trials, float ransac_inlier_dist,
                               uint64_t ransac_seed, bt_entryj* entry_out, int entry_capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, void* stream_) {
 	BT_REQUIRE(dA && dB, BT_ERR_INVALID_ARG, "bt_match_pairs: NULL descriptor views");
-	return match_pairs_impl(ctx, n_pairs, A, B, dA, dB, nullptr, nullptr, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, entry_out, entry_capacity, n_entry_out, entry_off_out, total_out, stream_);
+	return bt_match_pairs_ex(ctx, n_pairs, A, B, dA, dB, nullptr, nullptr, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, nullptr, entry_out, entry_capacity, n_entry_out, entry_off_out, total_out, nullptr, nullptr, stream_);
 }
 
 extern "C" int bt_match_pairs_pool(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, const int32_t* slotA, const int32_t* slotB,
                                    int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune, int ransac_trials, float ransac_inlier_dist,
                                    uint64_t ransac_seed, bt_entryj* entry_out, int entry_capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, void* stream_) {
 	BT_REQUIRE(slotA && slotB, BT_ERR_INVALID_ARG, "bt_match_pairs_pool: NULL slot arrays");
-	return match_pairs_impl(ctx, n_pairs, A, B, nullptr, nullptr, slotA, slotB, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, entry_out, entry_capacity, n_entry_out, entry_off_out, total_out, stream_);
+	return bt_match_pairs_ex(ctx, n_pairs, A, B, nullptr, nullptr, slotA, slotB, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, nullptr, entry_out, entry_capacity, n_entry_out, entry_off_out, total_out, nullptr, nullptr, stream_);
 }
 
-// bt_match_pairs / bt_match_pairs_pool with the rest of SiftManager::findCorres (FeatureManager.cpp:173-242): propagated map-point
-// matches for the non-neighbour pairs, the pair status (OK / cleared / Frame::FAIL) and the (uA, vA, uB, vB) of every emitted entry
-// (what updateFramePairMapPoints needs).  Exactly one of (dA, dB) and (slotA, slotB) is given.
+// SiftManager::findCorres (FeatureManager.cpp:173-242) for a batch of pairs, device-resident end to end, with the propagated map-point matches
+// of the non-neighbour pairs, the pair status (OK / cleared / Frame::FAIL) and the (uA, vA, uB, vB) of every emitted entry (what
+// updateFramePairMapPoints needs).  Pair p's entries are contiguous in entry_out.  bt_match_pairs and bt_match_pairs_pool are this call.
 extern "C" int bt_match_pairs_ex(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, const bt_desc_view* dA, const bt_desc_view* dB,
                                  const int32_t* slotA, const int32_t* slotB, int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune,
                                  int ransac_trials, float ransac_inlier_dist, uint64_t ransac_seed, const bt_match_extra* extra,
                                  bt_entryj* entry_out, int entry_capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, int32_t* status_out, float* uv_out, void* stream_) {
-	BT_REQUIRE(((dA && dB) ? 1 : 0) + ((slotA && slotB) ? 1 : 0) == 1, BT_ERR_INVALID_ARG, "bt_match_pairs_ex: give either descriptor views or pool slots");
-	return match_pairs_impl(ctx, n_pairs, A, B, dA, dB, slotA, slotB, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, entry_out, entry_capacity, n_entry_out, entry_off_out, total_out,
-	                        stream_, extra, status_out, uv_out);
+	PruneState* s = ctx ? ctx->prune.get() : nullptr;
+	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_match_pairs: call bt_pipeline_reserve first");
+	BT_REQUIRE(A && B && prune && entry_out && n_entry_out && entry_off_out && total_out && n_pairs > 0 && n_pairs <= s->max_pairs, BT_ERR_INVALID_ARG, "bt_match_pairs: bad argument");
+	BT_CUDA(cudaSetDevice(ctx->device));
+	Chain c(ctx, "bt_match_pairs_ex", n_pairs, A, B, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, stream_);
+	BT_TRY(c.knn(dA, dB, slotA, slotB));
+	BT_TRY(c.pairs(extra, 0));
+	BT_TRY(c.prune());
+	BT_TRY(c.append(0, n_pairs, nullptr));
+	BT_TRY(c.ransac(0, n_pairs));
+	return c.emit(entry_out, entry_capacity, n_entry_out, entry_off_out, total_out, status_out, uv_out);
 }
 
 // Bundler::optimizeGPU's findCorres loop (/root/reference/src/Bundler.cpp:298-305) in one asynchronous call: the pairs are matched in the
@@ -391,63 +418,43 @@ extern "C" int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_fra
                                     int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, int32_t* status_out, float* uv_out, void* stream_) {
 	PruneState* s = ctx ? ctx->prune.get() : nullptr;
 	BT_REQUIRE(s && ctx->tracks, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: call bt_pipeline_reserve and bt_tracks_dev_reserve first");
-	BT_REQUIRE(((dA && dB) ? 1 : 0) + ((slotA && slotB) ? 1 : 0) == 1, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: give either descriptor views or pool slots");
 	BT_REQUIRE(A && B && prune && entry_out && entry_capacity >= 0 && n_entry_out && entry_off_out && total_out && n_pairs > 0 && n_pairs <= s->max_pairs,
 	           BT_ERR_INVALID_ARG, "bt_find_corres_pairs: bad argument");
-	{   // frame A is the newer frame of every pair; the frames that are new to the table must fit before anything is queued
-		std::vector<int> fresh;
-		for (int p = 0; p < n_pairs; p++) {
-			BT_REQUIRE(A[p].frame_id > B[p].frame_id, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: pair %d: frame A must be the newer frame (id %d <= %d)", p, A[p].frame_id, B[p].frame_id);
-			for (int id : { A[p].frame_id, B[p].frame_id }) {
-				int sl;
-				tracks_slot(ctx, id, false, &sl);
-				if (sl < 0 && std::find(fresh.begin(), fresh.end(), id) == fresh.end()) fresh.push_back(id);
-			}
+	std::vector<int> fresh;   // frame A is the newer frame of every pair; the frames that are new to the table must fit before anything is queued
+	for (int p = 0; p < n_pairs; p++) {
+		BT_REQUIRE(A[p].frame_id > B[p].frame_id, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: pair %d: frame A must be the newer frame (id %d <= %d)", p, A[p].frame_id, B[p].frame_id);
+		for (int id : { A[p].frame_id, B[p].frame_id }) {
+			int sl;
+			tracks_slot(ctx, id, false, &sl);
+			if (sl < 0 && std::find(fresh.begin(), fresh.end(), id) == fresh.end()) fresh.push_back(id);
 		}
-		BT_REQUIRE((int)fresh.size() <= tracks_free_slots(ctx), BT_ERR_CAPACITY, "bt_find_corres_pairs: %d new frames do not fit the map-point table", (int)fresh.size());
 	}
-	cudaStream_t stream = (cudaStream_t)stream_;
+	BT_REQUIRE((int)fresh.size() <= tracks_free_slots(ctx), BT_ERR_CAPACITY, "bt_find_corres_pairs: %d new frames do not fit the map-point table", (int)fresh.size());
 	BT_CUDA(cudaSetDevice(ctx->device));
-	const int k = 5;   // k_near, FeatureManager.cpp:264
-	int rc = dA ? bt_knn_match_pairs(ctx, n_pairs, dA, dB, k, s->idxAB.as<int32_t>(), s->distAB.as<float>(), s->idxBA.as<int32_t>(), s->distBA.as<float>(), stream_)
-	            : bt_knn_match_slots(ctx, n_pairs, slotA, slotB, k, s->idxAB.as<int32_t>(), s->distAB.as<float>(), s->idxBA.as<int32_t>(), s->distBA.as<float>(), stream_);
-	if (rc != BT_OK) return rc;
-	if ((rc = fill_pairs(s, n_pairs, A, B, stream, nullptr, s->max_feats)) != BT_OK) return rc;
-	PruneCam cam; cam.H = H; cam.W = W; cam.ifx = 1.0f / fx; cam.ify = 1.0f / fy; cam.icx = -cx / fx; cam.icy = -cy / fy;
-	PrunePair* dp = s->pairs.as<PrunePair>();
-	bt_correspondence* corr = s->corr.as<bt_correspondence>();
-	int32_t* n_corr = s->n_corr.as<int32_t>();
-	k_prune_mutual<<<n_pairs, 512, 0, stream>>>(dp, cam, s->idxAB.as<int32_t>(), s->idxBA.as<int32_t>(), k, *prune, corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr);
-	BT_CUDA(cudaGetLastError());
-	const PrunePair* hp = s->h_pairs.buf.as<PrunePair>();   // (fill_pairs' host copy: out_off per pair)
+	Chain c(ctx, "bt_find_corres_pairs", n_pairs, A, B, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, stream_);
+	BT_TRY(c.knn(dA, dB, slotA, slotB));
+	BT_TRY(c.pairs(nullptr, s->max_feats));
+	BT_TRY(c.prune());
 	for (int p = 0; p < n_pairs; p++) {
 		int sa, sb;
 		if (abs(A[p].frame_id - B[p].frame_id) != 1) {       // findCorresByMapPoints
 			tracks_slot(ctx, A[p].frame_id, false, &sa);
 			tracks_slot(ctx, B[p].frame_id, false, &sb);
 			if (sa >= 0 && sb >= 0) {
-				float4* cand = s->extra.as<float4>() + (size_t)p * s->max_feats;
-				if ((rc = tracks_launch_propagate(ctx, sa, sb, nullptr, 0, cand, s->max_feats, s->n_prop.as<int32_t>() + p, stream)) != BT_OK) return rc;
-				k_append_propagated<<<1, 256, 0, stream>>>(dp + p, cam, s->extra.as<float4>(), corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr + p,
-				                                           s->n_nn.as<int32_t>() + p, s->n_prop.as<int32_t>() + p);
+				int32_t* n_prop = s->n_prop.as<int32_t>() + p;
+				BT_TRY(tracks_launch_propagate(ctx, sa, sb, nullptr, 0, s->extra.as<float4>() + (size_t)p * s->max_feats, s->max_feats, n_prop, c.stream));
+				BT_TRY(c.append(p, 1, n_prop));
 			}
 		}
-		k_ransac_table_from_counts<<<1, 128, 0, stream>>>(dp + p, 1, n_corr + p, s->PA.as<float4>(), s->PB.as<float4>(), s->rpairs.as<RansacPair>() + p);
-		BT_CUDA(cudaGetLastError());
-		rc = ransac_run_device(ctx, s->rpairs.as<RansacPair>() + p, 1, ransac_trials, ransac_inlier_dist, ransac_seed, s->inl.as<int32_t>(), s->n_inl.as<int32_t>() + p, stream);
-		if (rc != BT_OK) return rc;
+		BT_TRY(c.ransac(p, 1));
 		// updateFramePairMapPoints on the entries the pair emits (none unless its status is OK)
-		if ((rc = tracks_slot(ctx, A[p].frame_id, true, &sa)) != BT_OK) return rc;
-		if ((rc = tracks_slot(ctx, B[p].frame_id, true, &sb)) != BT_OK) return rc;
-		const int off = hp[p].out_off;
-		TrkSrc src{ reinterpret_cast<const float*>(corr + off), (int)(sizeof(bt_correspondence) / sizeof(float)), s->inl.as<int32_t>() + off, nullptr, 0,
-		            s->n_inl.as<int32_t>(), p, entry_capacity };
-		if ((rc = tracks_launch_update(ctx, sa, sb, src, stream)) != BT_OK) return rc;
+		BT_TRY(tracks_slot(ctx, A[p].frame_id, true, &sa));
+		BT_TRY(tracks_slot(ctx, B[p].frame_id, true, &sb));
+		const int off = s->h_pairs.buf.as<PrunePair>()[p].out_off;      // (the host copy of the pair table)
+		BT_TRY(tracks_launch_update(ctx, sa, sb, TrkSrc{ reinterpret_cast<const float*>(c.corr + off), (int)(sizeof(bt_correspondence) / sizeof(float)),
+		                                                 s->inl.as<int32_t>() + off, nullptr, 0, s->n_inl.as<int32_t>(), p, entry_capacity }, c.stream));
 	}
-	k_emit_entryj<<<1, 1024, 0, stream>>>(dp, n_pairs, corr, s->inl.as<int32_t>(), s->n_inl.as<int32_t>(), entry_out, n_entry_out, entry_off_out, total_out, entry_capacity, status_out);
-	k_emit_fill<<<n_pairs, 256, 0, stream>>>(dp, corr, s->inl.as<int32_t>(), n_entry_out, entry_off_out, entry_out, entry_capacity, reinterpret_cast<float4*>(uv_out));
-	BT_CUDA(cudaGetLastError());
-	return BT_OK;
+	return c.emit(entry_out, entry_capacity, n_entry_out, entry_off_out, total_out, status_out, uv_out);
 }
 
 // ------------------------------------------------------------------------------------------------ per-pair result cache
@@ -590,8 +597,7 @@ extern "C" int bt_match_cache_put(bt_ctx* ctx, int n_pairs, const int32_t* idA, 
 	}
 	if (mv.empty()) return BT_OK;
 	cudaStream_t stream = (cudaStream_t)stream_;
-	int rc = cache_upload(c, mv, stream);
-	if (rc != BT_OK) return rc;
+	BT_TRY(cache_upload(c, mv, stream));
 	if (n_compact > 0) k_cache_compact<<<1, kCompactThreads, 0, stream>>>(c->tab.as<CacheMove>(), n_compact, c->arena.as<bt_entryj>());
 	if ((int)mv.size() > n_compact)
 		k_cache_move<<<(unsigned)mv.size() - n_compact, 128, 0, stream>>>(c->tab.as<CacheMove>() + n_compact, entry_dev, c->arena.as<bt_entryj>(), 0);
@@ -640,8 +646,7 @@ extern "C" int bt_match_cache_gather(bt_ctx* ctx, int n_pairs, const int32_t* id
 	}
 	if (mv.empty()) return BT_OK;
 	cudaStream_t stream = (cudaStream_t)stream_;
-	int rc = cache_upload(c, mv, stream);
-	if (rc != BT_OK) return rc;
+	BT_TRY(cache_upload(c, mv, stream));
 	k_cache_move<<<(unsigned)mv.size(), 128, 0, stream>>>(c->tab.as<CacheMove>(), c->arena.as<bt_entryj>(), dst_dev, 1);
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;

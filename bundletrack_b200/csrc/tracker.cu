@@ -91,6 +91,7 @@ struct TFrame {
 	bool keyframe = false;
 	float pose[16];
 };
+struct TPair { const TFrame *a, *b; int wa, wb; };   // a findCorres pair (a newer) and the two frames' window indices
 // device scratch in int32 units: the neighbour pair's initial pose and (count, offset, status), then the window call's counts
 enum { M_POSE = 0, M_N = 16, M_OFF = 17, M_STATUS = 18, M_TOTAL = 20, M_WIN = 24 };
 }  // namespace
@@ -111,14 +112,12 @@ struct bt_tracker {
 	int last_fg_slot = -1;                 // the slot whose fg map the last begin_frame wrote (bt_tracker_last_fg)
 };
 
-static int tr_forget(bt_tracker* t, int id, cudaStream_t stream) {
-	int rc = bt_match_cache_forget_frame(t->ctx, id);
-	if (rc != BT_OK) return rc;
-	return bt_tracks_dev_forget_frame(t->ctx, id, stream);
-}
-static void tr_release(bt_tracker* t, const TFrame& f) {
+static int tr_forget(bt_tracker* t, const TFrame& f, cudaStream_t stream) {
+	BT_TRY(bt_match_cache_forget_frame(t->ctx, f.id));
+	BT_TRY(bt_tracks_dev_forget_frame(t->ctx, f.id, stream));
 	t->free_slots.push_back(f.slot);
 	if (f.cslot >= 0) t->free_cslots.push_back(f.cslot);
+	return BT_OK;
 }
 static float* tr_depth(bt_tracker* t, int slot) { return t->depth.as<float>() + t->hw * slot; }
 static float* tr_normal(bt_tracker* t, int slot) { return t->normal.as<float>() + 4 * t->hw * slot; }
@@ -141,8 +140,7 @@ static int tr_cache(bt_tracker* t, TFrame& f, cudaStream_t stream) {
 	const float* d[1] = { tr_depth(t, f.slot) };
 	const float* n[1] = { tr_normal(t, f.slot) };
 	const bt_tracker_params& p = t->p;
-	int rc = bt_frame_cache_store(t->ctx, 1, &cs, d, n, p.H, p.W, p.fx, p.fy, p.cx, p.cy, p.solver.depth_min, p.solver.depth_max, stream);
-	if (rc != BT_OK) return rc;
+	BT_TRY(bt_frame_cache_store(t->ctx, 1, &cs, d, n, p.H, p.W, p.fx, p.fy, p.cx, p.cy, p.solver.depth_min, p.solver.depth_max, stream));
 	t->free_cslots.pop_back();
 	f.cslot = cs;
 	return BT_OK;
@@ -153,15 +151,14 @@ static int tr_read(void* dst, const void* src, size_t bytes, cudaStream_t stream
 	return BT_OK;
 }
 // findCorres on an ordered pair list (A newer) in one asynchronous call: (count, offset, status) of the n pairs go to meta_dev[0, 3n)
-static int tr_find_corres(bt_tracker* t, const std::vector<std::pair<const TFrame*, const TFrame*>>& prs, const std::vector<std::pair<int, int>>& widx,
-                          int32_t* meta_dev, cudaStream_t stream) {
+static int tr_find_corres(bt_tracker* t, const std::vector<TPair>& prs, int32_t* meta_dev, cudaStream_t stream) {
 	const int n = (int)prs.size();
 	std::vector<bt_match_frame> A(n), B(n);
 	std::vector<int32_t> sa(n), sb(n);
 	int cap = n * t->p.max_feats;                         // room for every propagated match: never truncates
 	for (int k = 0; k < n; k++) {
-		A[k] = tr_match_frame(t, *prs[k].first, widx[k].first); B[k] = tr_match_frame(t, *prs[k].second, widx[k].second);
-		sa[k] = prs[k].first->slot; sb[k] = prs[k].second->slot;
+		A[k] = tr_match_frame(t, *prs[k].a, prs[k].wa); B[k] = tr_match_frame(t, *prs[k].b, prs[k].wb);
+		sa[k] = prs[k].a->slot; sb[k] = prs[k].b->slot;
 		cap += A[k].n + B[k].n;
 	}
 	const bt_tracker_params& p = t->p;
@@ -170,20 +167,53 @@ static int tr_find_corres(bt_tracker* t, const std::vector<std::pair<const TFram
 	                            nullptr, stream);
 }
 // after the counts are read back: the table's overflow flag, then the _matches cache (SiftManager::_matches) for the same pairs
-static int tr_put(bt_tracker* t, const std::vector<std::pair<const TFrame*, const TFrame*>>& prs, const int32_t* h, cudaStream_t stream) {
+static int tr_put(bt_tracker* t, const std::vector<TPair>& prs, const int32_t* h, cudaStream_t stream) {
 	const int n = (int)prs.size();
 	int pts, obs;
-	int rc = bt_tracks_dev_stats(t->ctx, &pts, &obs, stream);     // (the stream is idle: reports a map-point table overflow)
-	if (rc != BT_OK) return rc;
+	BT_TRY(bt_tracks_dev_stats(t->ctx, &pts, &obs, stream));     // (the stream is idle: reports a map-point table overflow)
 	std::vector<int32_t> ia(n), ib(n);
-	for (int k = 0; k < n; k++) { ia[k] = prs[k].first->id; ib[k] = prs[k].second->id; }
+	for (int k = 0; k < n; k++) { ia[k] = prs[k].a->id; ib[k] = prs[k].b->id; }
 	return bt_match_cache_put(t->ctx, n, ia.data(), ib.data(), t->entries.as<bt_entryj>(), h, h + n, h + 2 * n, stream);
 }
+// the keyframes' poses, 16 floats each in admission order, for the policy calls (one row at least)
+static std::vector<float> tr_keyframe_poses(const bt_tracker* t) {
+	const int K = (int)t->keyframes.size();
+	std::vector<float> kp(16 * (size_t)std::max(K, 1));
+	for (int k = 0; k < K; k++) memcpy(&kp[16 * (size_t)k], t->alive.at(t->keyframes[k]).pose, 64);
+	return kp;
+}
 
-// the keyframe pool's match-cache budget (the header states it): max_BA_frames / 2 worst-case blocks of 3 x max_feats entries per frame slot.
-// A frame's cached pairs are those of the windows it was new in, with at most max_BA_frames - 1 older frames each.
-static long long tr_cache_budget(const bt_tracker_params* p) {
-	return (long long)(p->max_frames_alive + p->max_keyframes) * p->max_BA_frames * 3 * p->max_feats / 2;
+// the tracker's own context and every buffer and table it uses; the caller destroys the tracker when one of them fails
+static int tr_reserve(bt_tracker* t, int device, const bt_tracker_params* p) {
+	BT_TRY(bt_ctx_create(&t->ctx, device));
+	const int F = p->max_frames_alive + p->max_keyframes;    // frames with maps at once (max_keyframes = 0: max_frames_alive counts keyframes too)
+	t->n_slots = F + 1;                                    // + the frame between begin_frame and end_frame
+	t->max_pairs = p->max_BA_frames * (p->max_BA_frames - 1) / 2;
+	t->slot_entries = 3 * p->max_feats;
+	t->win_entries = t->max_pairs * t->slot_entries;
+	t->hw = (size_t)p->H * p->W;
+	const bt_solver_limits lim = { 1, p->max_BA_frames, t->win_entries, p->H, p->W, p->solver.image_downscale };
+	BT_TRY(bt_solver_reserve(t->ctx, &lim));
+	BT_TRY(bt_frame_cache_reserve(t->ctx, F, p->H, p->W, p->solver.image_downscale));
+	BT_TRY(bt_pipeline_reserve(t->ctx, t->max_pairs, p->max_feats, kDescDim, p->ransac_trials));
+	BT_TRY(bt_desc_pool_reserve(t->ctx, t->n_slots));
+	BT_TRY(bt_tracks_dev_reserve_ex(t->ctx, F, p->max_feats, 16 * p->max_feats * ((F + 63) / 64)));
+	// the keyframe pool's match-cache budget (the header states it): max_BA_frames / 2 worst-case blocks of 3 x max_feats entries per frame slot.
+	// A frame's cached pairs are those of the windows it was new in, with at most max_BA_frames - 1 older frames each.
+	BT_TRY(p->max_keyframes == 0 ? bt_match_cache_reserve(t->ctx, F * (F - 1) / 2, t->slot_entries)
+	                             : bt_match_cache_reserve_entries(t->ctx, F * (F - 1) / 2, (long long)F * p->max_BA_frames * 3 * p->max_feats / 2));
+	BT_TRY(t->depth.alloc(sizeof(float) * t->hw * t->n_slots));
+	BT_TRY(t->normal.alloc(4 * sizeof(float) * t->hw * t->n_slots));
+	BT_TRY(t->fg.alloc(t->hw * t->n_slots));
+	BT_TRY(t->kpts.alloc(2 * sizeof(float) * (size_t)p->max_feats * t->n_slots));
+	BT_TRY(t->roi.alloc(4 * sizeof(int32_t)));
+	BT_TRY(t->entries.alloc(sizeof(bt_entryj) * (size_t)t->win_entries));
+	BT_TRY(t->gather.alloc(sizeof(bt_entryj) * (size_t)t->win_entries));
+	BT_TRY(t->meta.alloc(sizeof(int32_t) * (M_WIN + 3 * (size_t)t->max_pairs)));
+	BT_TRY(t->h_meta.alloc(sizeof(int32_t) * (M_WIN + 3 * (size_t)t->max_pairs)));
+	for (int s = t->n_slots - 1; s >= 0; s--) t->free_slots.push_back(s);
+	for (int s = F - 1; s >= 0; s--) t->free_cslots.push_back(s);
+	return BT_OK;
 }
 
 extern "C" int bt_tracker_create(bt_tracker** out, int device, const bt_tracker_params* p) {
@@ -195,41 +225,12 @@ extern "C" int bt_tracker_create(bt_tracker** out, int device, const bt_tracker_
 	BT_REQUIRE(p->max_BA_frames >= 2 && p->max_BA_frames <= 32 && p->window_size >= 0 && p->ransac_trials >= 1 &&
 	           (p->mask_mode == BT_MASK_AS_IS || p->mask_mode == BT_MASK_LARGEST_HULL), BT_ERR_INVALID_ARG,
 	           "bt_tracker_create: bad parameters (max_BA_frames 2..32, window_size >= 0, ransac_trials >= 1, mask_mode)");
-	bt_ctx* ctx = nullptr;
-	int rc = bt_ctx_create(&ctx, device);
-	if (rc != BT_OK) return rc;
 	bt_tracker* t = new bt_tracker();
-	t->ctx = ctx;
 	t->p = *p;
-	const int F = p->max_frames_alive + p->max_keyframes;    // frames with maps at once (max_keyframes = 0: max_frames_alive counts keyframes too)
-	t->n_slots = F + 1;                                    // + the frame between begin_frame and end_frame
-	t->max_pairs = p->max_BA_frames * (p->max_BA_frames - 1) / 2;
-	t->slot_entries = 3 * p->max_feats;
-	t->win_entries = t->max_pairs * t->slot_entries;
-	t->hw = (size_t)p->H * p->W;
-	const bt_solver_limits lim = { 1, p->max_BA_frames, t->win_entries, p->H, p->W, p->solver.image_downscale };
-#define TRY(x) if ((rc = (x)) != BT_OK) { bt_tracker_destroy(t); return rc; }
-	TRY(bt_solver_reserve(ctx, &lim));
-	TRY(bt_frame_cache_reserve(ctx, F, p->H, p->W, p->solver.image_downscale));
-	TRY(bt_pipeline_reserve(ctx, t->max_pairs, p->max_feats, kDescDim, p->ransac_trials));
-	TRY(bt_desc_pool_reserve(ctx, t->n_slots));
-	TRY(bt_tracks_dev_reserve_ex(ctx, F, p->max_feats, 16 * p->max_feats * ((F + 63) / 64)));
-	TRY(p->max_keyframes == 0 ? bt_match_cache_reserve(ctx, F * (F - 1) / 2, t->slot_entries)
-	                          : bt_match_cache_reserve_entries(ctx, F * (F - 1) / 2, tr_cache_budget(p)));
-	TRY(t->depth.alloc(sizeof(float) * t->hw * t->n_slots));
-	TRY(t->normal.alloc(4 * sizeof(float) * t->hw * t->n_slots));
-	TRY(t->fg.alloc(t->hw * t->n_slots));
-	TRY(t->kpts.alloc(2 * sizeof(float) * (size_t)p->max_feats * t->n_slots));
-	TRY(t->roi.alloc(4 * sizeof(int32_t)));
-	TRY(t->entries.alloc(sizeof(bt_entryj) * (size_t)t->win_entries));
-	TRY(t->gather.alloc(sizeof(bt_entryj) * (size_t)t->win_entries));
-	TRY(t->meta.alloc(sizeof(int32_t) * (M_WIN + 3 * (size_t)t->max_pairs)));
-	TRY(t->h_meta.alloc(sizeof(int32_t) * (M_WIN + 3 * (size_t)t->max_pairs)));
-#undef TRY
-	for (int s = t->n_slots - 1; s >= 0; s--) t->free_slots.push_back(s);
-	for (int s = F - 1; s >= 0; s--) t->free_cslots.push_back(s);
-	*out = t;
-	return BT_OK;
+	const int rc = tr_reserve(t, device, p);
+	if (rc == BT_OK) *out = t;
+	else bt_tracker_destroy(t);
+	return rc;
 }
 
 extern "C" void bt_tracker_destroy(bt_tracker* t) {
@@ -264,20 +265,13 @@ static int tr_begin(bt_tracker* t, const char* who, int loader_id, const float* 
 	float* dout[1] = { tr_depth(t, f.slot) };
 	float* nout[1] = { tr_normal(t, f.slot) };
 	uint8_t* fg[1] = { tr_fg(t, f.slot) };
-	int rc;
-	if (u16) {
-		const uint16_t* din[1] = { static_cast<const uint16_t*>(depth_raw_dev) };
-		rc = bt_frames_preprocess_masked_u16(t->ctx, 1, din, msk, p.mask_mode, p.H, p.W, p.fx, p.fy, p.cx, p.cy, &p.depth, dout, nullptr, nout, fg,
-		                                     t->roi.as<int32_t>(), stream);
-	} else {
-		const float* din[1] = { static_cast<const float*>(depth_raw_dev) };
-		rc = bt_frames_preprocess_masked(t->ctx, 1, din, msk, p.mask_mode, p.H, p.W, p.fx, p.fy, p.cx, p.cy, &p.depth, dout, nullptr, nout, fg,
-		                                 t->roi.as<int32_t>(), stream);
-	}
-	if (rc != BT_OK) return rc;
+	const uint16_t* din_mm[1] = { static_cast<const uint16_t*>(depth_raw_dev) };
+	const float* din[1] = { static_cast<const float*>(depth_raw_dev) };
+	BT_TRY(u16 ? bt_frames_preprocess_masked_u16(t->ctx, 1, din_mm, msk, p.mask_mode, p.H, p.W, p.fx, p.fy, p.cx, p.cy, &p.depth, dout, nullptr, nout, fg, t->roi.as<int32_t>(), stream)
+	           : bt_frames_preprocess_masked(t->ctx, 1, din, msk, p.mask_mode, p.H, p.W, p.fx, p.fy, p.cx, p.cy, &p.depth, dout, nullptr, nout, fg, t->roi.as<int32_t>(), stream));
 	t->last_fg_slot = f.slot;
 	int32_t* roi = t->h_meta.as<int32_t>();
-	if ((rc = tr_read(roi, t->roi.p, 4 * sizeof(int32_t), stream)) != BT_OK) return rc;
+	BT_TRY(tr_read(roi, t->roi.p, 4 * sizeof(int32_t), stream));
 	if (roi_out) memcpy(roi_out, roi, 4 * sizeof(int32_t));
 	if (roi[1] - roi[0] < 10 || roi[3] - roi[2] < 10) {   // Bundler.cpp:88-93: FAIL, nothing is kept or forgotten
 		*status_out = BT_FRAME_FAIL;
@@ -286,7 +280,7 @@ static int tr_begin(bt_tracker* t, const char* who, int loader_id, const float* 
 	const uint8_t* col[1] = { colour_dev };
 	const uint8_t* fgc[1] = { fg[0] };
 	uint8_t* req[1] = { request_out_dev };
-	if ((rc = bt_lfnet_request(t->ctx, 1, col, fgc, t->roi.as<int32_t>(), p.H, p.W, req, stream)) != BT_OK) return rc;
+	BT_TRY(bt_lfnet_request(t->ctx, 1, col, fgc, t->roi.as<int32_t>(), p.H, p.W, req, stream));
 	t->free_slots.pop_back();
 	t->pend = f;
 	t->pending = true;
@@ -311,11 +305,119 @@ extern "C" int bt_tracker_drop_frame(bt_tracker* t, float* pose_out) {
 	BT_REQUIRE(t, BT_ERR_INVALID_ARG, "bt_tracker_drop_frame: NULL tracker");
 	BT_REQUIRE(t->pending, BT_ERR_INVALID_ARG, "bt_tracker_drop_frame: no frame is pending");
 	BT_CUDA(cudaSetDevice(t->ctx->device));
-	int rc = tr_forget(t, t->pend.id, nullptr);
-	if (rc != BT_OK) return rc;
-	tr_release(t, t->pend);
+	BT_TRY(tr_forget(t, t->pend, nullptr));
 	t->pending = false;
 	if (pose_out) memcpy(pose_out, t->pend.pose, sizeof t->pend.pose);
+	return BT_OK;
+}
+
+// Bundler.cpp:119-138: findCorres on (new, last), the initial pose from its inliers, the pair into the match cache; a FAIL pair fails the frame
+static int tr_neighbour(bt_tracker* t, TFrame& f, int* status, cudaStream_t stream) {
+	if (t->frames.empty()) return BT_OK;
+	int32_t* md = t->meta.as<int32_t>();
+	int32_t* mh = t->h_meta.as<int32_t>();
+	const TFrame& last = t->alive.at(t->frames.back());
+	const std::vector<TPair> prs = { { &f, &last, 1, 0 } };
+	BT_TRY(tr_find_corres(t, prs, md + M_N, stream));
+	BT_TRY(bt_pose_init(t->ctx, t->entries.as<bt_entryj>(), md + M_N, md + M_STATUS, f.pose, last.pose, reinterpret_cast<float*>(md + M_POSE), stream));
+	BT_TRY(tr_read(mh, md, sizeof(int32_t) * (M_STATUS + 1), stream));     // the pose, count, offset and status
+	BT_TRY(tr_put(t, prs, mh + M_N, stream));
+	if (mh[M_STATUS] == BT_PAIR_FAIL) *status = BT_FRAME_FAIL;
+	else memcpy(f.pose, mh + M_POSE, sizeof f.pose);
+	return BT_OK;
+}
+// Bundler.cpp:149-157: the oldest frame leaves a full deque (a keyframe stays alive), the new one joins
+static int tr_slide(bt_tracker* t, const TFrame& f, cudaStream_t stream) {
+	if ((int)t->frames.size() >= t->p.window_size + 3) {
+		const TFrame& o = t->alive.at(t->frames.front());
+		if (!o.keyframe) {
+			BT_TRY(tr_forget(t, o, stream));
+			t->alive.erase(t->frames.front());
+		}
+		t->frames.pop_front();
+	}
+	t->frames.push_back(f.id);
+	t->alive[f.id] = f;
+	return BT_OK;
+}
+// selectKeyFramesForBA + optimizeGPU (Bundler.cpp:222-358): the uncached pairs matched, all gathered, the BA gate, the solve
+static int tr_window(bt_tracker* t, TFrame& nf, int* status, cudaStream_t stream) {
+	const bt_tracker_params& p = t->p;
+	const int K = (int)t->keyframes.size();
+	std::vector<int32_t> chosen(std::max(K, 1));
+	int n_chosen = 0;
+	BT_TRY(bt_select_keyframes(nf.pose, tr_keyframe_poses(t).data(), K, p.max_BA_frames, chosen.data(), &n_chosen));
+	std::vector<TFrame*> win;
+	for (int k = 0; k < n_chosen; k++) win.push_back(&t->alive.at(t->keyframes[chosen[k]]));
+	win.push_back(&nf);                                    // the newest frame sorts last
+	const int N = (int)win.size();
+	std::vector<TPair> todo;
+	std::vector<int32_t> ga, gb;
+	std::vector<uint32_t> wi, wj;
+	for (int i = 0; i < N; i++)
+		for (int j = i + 1; j < N; j++) {
+			ga.push_back(win[j]->id); gb.push_back(win[i]->id); wi.push_back(i); wj.push_back(j);
+			if (!bt_match_cache_has(t->ctx, win[j]->id, win[i]->id)) todo.push_back({ win[j], win[i], j, i });
+		}
+	if (!todo.empty()) {
+		const int n = (int)todo.size();
+		int32_t* md = t->meta.as<int32_t>() + M_WIN;
+		int32_t* mh = t->h_meta.as<int32_t>() + M_WIN;
+		BT_TRY(tr_find_corres(t, todo, md, stream));
+		BT_TRY(tr_read(mh, md, sizeof(int32_t) * 3 * n, stream));
+		BT_TRY(tr_put(t, todo, mh, stream));
+		for (int k = 0; k < n; k++)
+			if (mh[2 * n + k] == BT_PAIR_FAIL && todo[k].a == &nf) *status = BT_FRAME_FAIL;
+	}
+	int n_edges = 0;
+	const int np = (int)ga.size();
+	std::vector<int32_t> boff(std::max(np, 1)), bn(std::max(np, 1));
+	if (np > 0) BT_TRY(bt_match_cache_gather(t->ctx, np, ga.data(), gb.data(), wi.data(), wj.data(), t->gather.as<bt_entryj>(), t->win_entries, boff.data(), bn.data(), stream));
+	for (int k = 0; k < np; k++) if ((int)wj[k] == N - 1) n_edges += bn[k];
+	if (*status != BT_FRAME_FAIL && !bt_ba_gate(n_edges, p.min_fm_edges_newframe)) *status = BT_FRAME_NO_BA;
+	if (*status != BT_FRAME_OTHER || N < 2) return BT_OK;
+	BT_TRY(tr_cache(t, nf, stream));
+	std::vector<const float*> dptr(N), nptr(N);
+	std::vector<int32_t> cs(N);
+	std::vector<float> poses(16 * (size_t)N);
+	for (int k = 0; k < N; k++) {
+		dptr[k] = tr_depth(t, win[k]->slot); nptr[k] = tr_normal(t, win[k]->slot); cs[k] = win[k]->cslot;
+		memcpy(&poses[16 * (size_t)k], win[k]->pose, 64);
+	}
+	bt_window w{};
+	w.n_frames = N; w.H = p.H; w.W = p.W;
+	w.depth_dev = dptr.data(); w.normal_dev = nptr.data();
+	w.fx = p.fx; w.fy = p.fy; w.cx = p.cx; w.cy = p.cy;
+	w.compat_flip = 1;
+	w.cache_slots = cs.data();
+	w.corr_dev = t->gather.as<bt_entryj>();
+	w.n_blocks = np; w.block_off = boff.data(); w.block_n = bn.data(); w.block_i = wi.data(); w.block_j = wj.data();
+	BT_TRY(bt_solve_windows(t->ctx, 1, &w, &p.solver, poses.data(), stream));
+	for (int k = 0; k < N; k++) memcpy(win[k]->pose, &poses[16 * (size_t)k], 64);     // every frame of the window, keyframes included
+	return BT_OK;
+}
+// a FAIL frame is forgotten, and popped when the deque holds it (Bundler.cpp:173-179); the reported pose is the one the frame has
+static int tr_fail(bt_tracker* t, TFrame f, bool in_deque, float* pose_out, int* status_out, cudaStream_t stream) {
+	BT_TRY(tr_forget(t, f, stream));
+	if (in_deque) { t->frames.pop_back(); t->alive.erase(f.id); }
+	memcpy(pose_out, f.pose, sizeof f.pose);
+	*status_out = BT_FRAME_FAIL;
+	return BT_OK;
+}
+// closing the frame (Bundler.cpp:173-221): FAIL, or checkAndAddKeyframe
+static int tr_close(bt_tracker* t, TFrame& nf, int status, float* pose_out, int* status_out, cudaStream_t stream) {
+	if (status == BT_FRAME_FAIL) return tr_fail(t, nf, true, pose_out, status_out, stream);
+	if (status == BT_FRAME_OTHER && bt_keyframe_check(nf.pose, nf.id, nf.n_kpts, tr_keyframe_poses(t).data(), (int)t->keyframes.size(), t->p.min_feat_num,
+	                                                  t->p.min_rot_deg) == 1) {
+		BT_TRY(tr_cache(t, nf, stream));
+		nf.keyframe = true;
+		t->keyframes.push_back(nf.id);
+	} else if (nf.cslot >= 0) {                            // only keyframes take part in later windows
+		t->free_cslots.push_back(nf.cslot);
+		nf.cslot = -1;
+	}
+	memcpy(pose_out, nf.pose, sizeof nf.pose);
+	*status_out = status;
 	return BT_OK;
 }
 
@@ -339,124 +441,16 @@ extern "C" int bt_tracker_end_frame(bt_tracker* t, const float* kpts_host, int n
 	BT_CUDA(cudaSetDevice(t->ctx->device));
 	TFrame f = t->pend;
 	f.n_kpts = n_kpts;
-	int rc;
 	if (n_kpts) BT_CUDA(cudaMemcpyAsync(tr_kpts(t, f.slot), kpts_host, 2 * sizeof(float) * (size_t)n_kpts, cudaMemcpyHostToDevice, stream));
-	if ((rc = bt_desc_pool_store(t->ctx, f.slot, desc, stream)) != BT_OK) return rc;
+	BT_TRY(bt_desc_pool_store(t->ctx, f.slot, desc, stream));
 	t->pending = false;                                    // from here on the frame is the tracker's
 	int status = BT_FRAME_OTHER;
-	int32_t* md = t->meta.as<int32_t>();
-	int32_t* mh = t->h_meta.as<int32_t>();
-	auto finish_fail = [&](bool in_deque) -> int {         // forgetFrame (+ pop_back); the reported pose is the one the frame has
-		if ((rc = tr_forget(t, f.id, stream)) != BT_OK) return rc;
-		if (in_deque) { t->frames.pop_back(); t->alive.erase(f.id); }
-		tr_release(t, f);
-		memcpy(pose_out, f.pose, sizeof f.pose);
-		*status_out = BT_FRAME_FAIL;
-		return BT_OK;
-	};
-	if (!t->frames.empty()) {                              // Bundler.cpp:119-138
-		const TFrame& last = t->alive.at(t->frames.back());
-		std::vector<std::pair<const TFrame*, const TFrame*>> prs = { { &f, &last } };
-		if ((rc = tr_find_corres(t, prs, { { 1, 0 } }, md + M_N, stream)) != BT_OK) return rc;
-		if ((rc = bt_pose_init(t->ctx, t->entries.as<bt_entryj>(), md + M_N, md + M_STATUS, f.pose, last.pose, reinterpret_cast<float*>(md + M_POSE), stream)) != BT_OK) return rc;
-		if ((rc = tr_read(mh, md, sizeof(int32_t) * (M_STATUS + 1), stream)) != BT_OK) return rc;     // the pose, count, offset and status
-		if ((rc = tr_put(t, prs, mh + M_N, stream)) != BT_OK) return rc;
-		if (mh[M_STATUS] == BT_PAIR_FAIL) return finish_fail(false);
-		memcpy(f.pose, mh + M_POSE, sizeof f.pose);
-	}
-	if ((int)t->frames.size() >= p.window_size + 3) {      // Bundler.cpp:149-157
-		const int old = t->frames.front();
-		TFrame& o = t->alive.at(old);
-		if (!o.keyframe) {
-			if ((rc = tr_forget(t, old, stream)) != BT_OK) return rc;
-			tr_release(t, o);
-			t->alive.erase(old);
-		}
-		t->frames.pop_front();
-	}
-	t->frames.push_back(f.id);
-	t->alive[f.id] = f;
+	BT_TRY(tr_neighbour(t, f, &status, stream));
+	if (status == BT_FRAME_FAIL) return tr_fail(t, f, false, pose_out, status_out, stream);
+	BT_TRY(tr_slide(t, f, stream));
 	TFrame& nf = t->alive.at(f.id);
-	if (f.id != 0) {                                       // selectKeyFramesForBA + optimizeGPU (Bundler.cpp:222-358)
-		const int K = (int)t->keyframes.size();
-		std::vector<float> kp(16 * (size_t)std::max(K, 1));
-		for (int k = 0; k < K; k++) memcpy(&kp[16 * (size_t)k], t->alive.at(t->keyframes[k]).pose, 64);
-		std::vector<int32_t> chosen(std::max(K, 1));
-		int n_chosen = 0;
-		if ((rc = bt_select_keyframes(nf.pose, kp.data(), K, p.max_BA_frames, chosen.data(), &n_chosen)) != BT_OK) return rc;
-		std::vector<TFrame*> win;
-		for (int k = 0; k < n_chosen; k++) win.push_back(&t->alive.at(t->keyframes[chosen[k]]));
-		win.push_back(&nf);                                // the newest frame sorts last
-		const int N = (int)win.size();
-		std::vector<std::pair<const TFrame*, const TFrame*>> todo;
-		std::vector<std::pair<int, int>> widx;
-		std::vector<int32_t> ga, gb;
-		std::vector<uint32_t> wi, wj;
-		for (int i = 0; i < N; i++)
-			for (int j = i + 1; j < N; j++) {
-				ga.push_back(win[j]->id); gb.push_back(win[i]->id); wi.push_back(i); wj.push_back(j);
-				if (!bt_match_cache_has(t->ctx, win[j]->id, win[i]->id)) { todo.push_back({ win[j], win[i] }); widx.push_back({ j, i }); }
-			}
-		if (!todo.empty()) {
-			const int n = (int)todo.size();
-			if ((rc = tr_find_corres(t, todo, widx, md + M_WIN, stream)) != BT_OK) return rc;
-			if ((rc = tr_read(mh + M_WIN, md + M_WIN, sizeof(int32_t) * 3 * n, stream)) != BT_OK) return rc;
-			if ((rc = tr_put(t, todo, mh + M_WIN, stream)) != BT_OK) return rc;
-			for (int k = 0; k < n; k++)
-				if (mh[M_WIN + 2 * n + k] == BT_PAIR_FAIL && todo[k].first == &nf) status = BT_FRAME_FAIL;
-		}
-		int n_edges = 0;
-		const int np = (int)ga.size();
-		std::vector<int32_t> boff(std::max(np, 1)), bn(std::max(np, 1));
-		if (np > 0) {
-			if ((rc = bt_match_cache_gather(t->ctx, np, ga.data(), gb.data(), wi.data(), wj.data(), t->gather.as<bt_entryj>(), t->win_entries, boff.data(), bn.data(), stream)) != BT_OK)
-				return rc;
-			for (int k = 0; k < np; k++) if ((int)wj[k] == N - 1) n_edges += bn[k];
-		}
-		if (status != BT_FRAME_FAIL) {
-			if (!bt_ba_gate(n_edges, p.min_fm_edges_newframe)) status = BT_FRAME_NO_BA;
-			else if (N >= 2) {
-				if ((rc = tr_cache(t, nf, stream)) != BT_OK) return rc;
-				std::vector<const float*> dptr(N), nptr(N);
-				std::vector<int32_t> cs(N);
-				std::vector<float> poses(16 * (size_t)N);
-				for (int k = 0; k < N; k++) {
-					dptr[k] = tr_depth(t, win[k]->slot); nptr[k] = tr_normal(t, win[k]->slot); cs[k] = win[k]->cslot;
-					memcpy(&poses[16 * (size_t)k], win[k]->pose, 64);
-				}
-				bt_window w{};
-				w.n_frames = N; w.H = p.H; w.W = p.W;
-				w.depth_dev = dptr.data(); w.normal_dev = nptr.data();
-				w.fx = p.fx; w.fy = p.fy; w.cx = p.cx; w.cy = p.cy;
-				w.compat_flip = 1;
-				w.cache_slots = cs.data();
-				w.corr_dev = t->gather.as<bt_entryj>();
-				w.n_blocks = np; w.block_off = boff.data(); w.block_n = bn.data(); w.block_i = wi.data(); w.block_j = wj.data();
-				if ((rc = bt_solve_windows(t->ctx, 1, &w, &p.solver, poses.data(), stream)) != BT_OK) return rc;
-				for (int k = 0; k < N; k++) memcpy(win[k]->pose, &poses[16 * (size_t)k], 64);     // every frame of the window, keyframes included
-			}
-		}
-	}
-	f = nf;
-	if (status == BT_FRAME_FAIL) return finish_fail(true);   // Bundler.cpp:173-179
-	bool admit = false;                                    // checkAndAddKeyframe (Bundler.cpp:185-221)
-	if (status == BT_FRAME_OTHER) {
-		const int K = (int)t->keyframes.size();
-		std::vector<float> kp(16 * (size_t)std::max(K, 1));
-		for (int k = 0; k < K; k++) memcpy(&kp[16 * (size_t)k], t->alive.at(t->keyframes[k]).pose, 64);
-		admit = bt_keyframe_check(nf.pose, nf.id, nf.n_kpts, kp.data(), K, p.min_feat_num, p.min_rot_deg) == 1;
-	}
-	if (admit) {
-		if ((rc = tr_cache(t, nf, stream)) != BT_OK) return rc;
-		nf.keyframe = true;
-		t->keyframes.push_back(nf.id);
-	} else if (nf.cslot >= 0) {                            // only keyframes take part in later windows
-		t->free_cslots.push_back(nf.cslot);
-		nf.cslot = -1;
-	}
-	memcpy(pose_out, nf.pose, sizeof nf.pose);
-	*status_out = status;
-	return BT_OK;
+	if (nf.id != 0) BT_TRY(tr_window(t, nf, &status, stream));
+	return tr_close(t, nf, status, pose_out, status_out, stream);
 }
 
 extern "C" int bt_tracker_state(bt_tracker* t, int32_t* ids, float* poses, int32_t* is_keyframe, int cap, int* n) {
@@ -485,7 +479,6 @@ extern "C" int bt_tracker_last_fg(bt_tracker* t, const uint8_t** fg_dev) {
 extern "C" int bt_tracker_usage(bt_tracker* t, int* n_points, int* n_pairs_cached, long long* n_entries_cached, void* stream) {
 	BT_REQUIRE(t && n_points && n_pairs_cached && n_entries_cached, BT_ERR_INVALID_ARG, "bt_tracker_usage: NULL argument");
 	BT_CUDA(cudaSetDevice(t->ctx->device));
-	int rc = tracks_points_alive(t->ctx, (cudaStream_t)stream, n_points);
-	if (rc != BT_OK) return rc;
+	BT_TRY(tracks_points_alive(t->ctx, (cudaStream_t)stream, n_points));
 	return bt_match_cache_usage(t->ctx, n_pairs_cached, n_entries_cached);
 }
