@@ -136,6 +136,10 @@ struct SolveArgs {
 	float* dbg_cnt; int dbg_cnt_stride;               // optional per-pair #correspondences found (last GN iteration)
 	float* dbg_sys; int dbg_sys_stride;               // optional PCG system dump (last GN iteration): per window A [st][st], rhs, Jacobi diagonal, delta [st] each
 	long long* prof; int prof_cap;                    // optional phase timestamps: [0] = record count, then 12 x int64 per record
+	// optional device times (bt_solve_enable_timing), %globaltimer ns: [0] prep start (first prep kernel's block 0), [1] prep end (tile
+	// plan written), [2] k_solve start (block 0), [3] k_solve end (last CTA).  Stamped inside the kernels: an event recorded between two
+	// kernels would cut the step's launch chain.  with_count: k_prep_count runs before k_prep_frames (it stamps [0] then).
+	long long* tstamp; int with_count;
 };
 
 // ------------------------------------------------------------------------------------------------ device math
@@ -276,6 +280,15 @@ __device__ __forceinline__ float texel_depth(const TexelGeom& g, int W, int H, i
 
 struct FrameGeom { int W, H, w, h; TexelGeom tg; };
 
+// Programmatic dependent launch (DESIGN §3.4): a step's kernels are launched as one chain, each one allowed to start while its
+// predecessor on the stream finishes.  chain_wait() returns once the predecessor has completed and its writes are visible; before it a
+// kernel only reads memory that no kernel still in flight writes.  chain_release() lets the successor's CTAs launch (they then sit in
+// their own chain_wait); a grid whose CTAs exit without it releases the successor at exit.  Without a programmatic predecessor (a
+// plain launch, a copy or an event wait in between) both are no-ops.
+__device__ __forceinline__ void chain_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void chain_release() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ long long global_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return (long long)t; }
+
 // A frame's maps are built one CTA per 1024 quarter-res pixels (block b, 1024 threads) in two launches.  The compacted source list
 // keeps pixel order (fixed summation order downstream), so each block needs the number of valid pixels before it: the first launch
 // counts the valid pixels of every block (frame_block_count), the second turns the counts of the blocks before it into the block's
@@ -299,13 +312,19 @@ __device__ __forceinline__ void frame_block_count(const FrameGeom& g, const floa
 		if (threadIdx.x == 0) blk_cnt[b] = t;
 	}
 }
-// The frame's last block also writes the source count to *nsrc.  Blocks past the end of the frame do nothing.
+// The frame's last block also writes the source count to *nsrc.  Blocks past the end of the frame do nothing.  The pixel's depth and
+// normal samples are loaded before chain_wait(): in k_cache_build that runs under the previous kernels' last CTAs, because the maps
+// are the call's inputs, complete before the chain's first kernel passed its own wait.  blk_cnt and every write come after it.
 __device__ __forceinline__ void frame_block_build(const FrameGeom& g, const float* __restrict__ depth, const float4* __restrict__ normal, float dmin, float dmax, int b,
                                                   const int* __restrict__ blk_cnt, float4* texel, float4* src, int* nsrc) {
 	__shared__ int s_w[32];
 	__shared__ int s_base;
 	const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
 	const int npix = g.w * g.h;
+	const int idx = b * 1024 + tid;
+	float4 rec, cp, nr;
+	if (idx < npix) rec = texel_build(g.tg, g.W, g.H, g.w, depth, normal, idx, cp, nr);
+	chain_wait();
 	if (b * 1024 >= npix) return;
 	if (wid == 0) {      // offset of this block = valid pixels of the blocks before it (at most a few dozen)
 		int t = 0;
@@ -314,11 +333,9 @@ __device__ __forceinline__ void frame_block_build(const FrameGeom& g, const floa
 		for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
 		if (lane == 0) s_base = t;
 	}
-	const int idx = b * 1024 + tid;
-	float4 cp, nr;
 	bool valid = false;
 	if (idx < npix) {
-		texel[idx] = texel_build(g.tg, g.W, g.H, g.w, depth, normal, idx, cp, nr);
+		texel[idx] = rec;
 		valid = (cp.z > dmin && cp.z < dmax);
 	}
 	const unsigned bal = __ballot_sync(0xffffffffu, valid);
@@ -404,7 +421,7 @@ __device__ __forceinline__ void prof_emit(const SolveArgs& a, const ProfRec& r) 
 	}
 }
 #ifdef BT_PROF_GLOBALTIMER      // (variant build: nanoseconds of the device-wide timer, comparable across SMs, instead of the SM's own cycle counter)
-__device__ __forceinline__ long long prof_now() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return (long long)t; }
+__device__ __forceinline__ long long prof_now() { return global_ns(); }
 #else
 __device__ __forceinline__ long long prof_now() { return clock64(); }
 #endif
@@ -487,8 +504,13 @@ __device__ int build_frame_maps(const FrameGeom& g, const float* __restrict__ de
 
 // Frame preparation of the frames a call rebuilds itself, one CTA per 1024 quarter-res pixels of a (window, frame) slot:
 // frame_block_count, then frame_block_build.  (One CTA per frame would walk 19 rounds serially.)
+// Every CTA of a chained kernel passes chain_wait() before it exits, so that the grid's completion orders everything after it behind
+// the predecessor.
 __global__ void __launch_bounds__(1024, 2) k_prep_count(SolveArgs a, int* __restrict__ blk_cnt) {
 	const int fs = blockIdx.y, b = blockIdx.x;
+	chain_wait();
+	chain_release();
+	if (a.tstamp && fs == 0 && b == 0 && threadIdx.x == 0) a.tstamp[0] = global_ns();
 	if (a.nsrc_cached[fs] || !(a.prm.w_dense > 0.0f)) return;
 	const WinDesc wd = a.wins[a.frame_win[fs]];
 	const FrameGeom g = {wd.W, wd.H, wd.w, wd.h, wd.tg};
@@ -497,8 +519,11 @@ __global__ void __launch_bounds__(1024, 2) k_prep_count(SolveArgs a, int* __rest
 
 __global__ void __launch_bounds__(1024, 2) k_prep_frames(SolveArgs a, WinDesc* wins_rw, int* prep_ticket, const int* __restrict__ blk_cnt) {
 	const int fs = blockIdx.y, b = blockIdx.x;
-	const WinDesc wd = a.wins[a.frame_win[fs]];
 	const int tid = threadIdx.x;
+	chain_wait();
+	chain_release();
+	if (a.tstamp && !a.with_count && fs == 0 && b == 0 && tid == 0) a.tstamp[0] = global_ns();
+	const WinDesc wd = a.wins[a.frame_win[fs]];
 	const int* cached = a.nsrc_cached[fs];
 	if (cached) { if (b == 0 && tid == 0) a.nsrc[fs] = *cached; }      // maps and source list were built by bt_frame_cache_store
 	else if (!(a.prm.w_dense > 0.0f)) { if (b == 0 && tid == 0) a.nsrc[fs] = 0; }
@@ -525,34 +550,50 @@ __global__ void __launch_bounds__(1024, 2) k_prep_frames(SolveArgs a, WinDesc* w
 	__syncthreads();
 	if (tid == 0) { const int t = atomicAdd(prep_ticket, 1); s_last = (t == (int)(gridDim.x * gridDim.y) - 1); if (s_last) { *prep_ticket = 0; __threadfence(); } }
 	__syncthreads();
-	if (s_last) plan_body(a, wins_rw);
+	if (s_last) {
+		plan_body(a, wins_rw);
+		if (a.tstamp && tid == 0) { a.tstamp[1] = global_ns(); a.tstamp[3] = 0; }      // ([3]: k_solve's CTAs take the maximum of their end times)
+	}
 }
 
 // bt_frame_cache_store: the same maps, built once per keyframe into a slot of the context's frame cache.
+// A store of up to kStoreInline frames carries its map pointers and slots in the kernel parameters (no table upload between the
+// previous kernel and the store's, which would cut the launch chain); a larger one reads them from the uploaded tables.
+static constexpr int kStoreInline = 64;
 struct CacheStoreArgs {
 	FrameGeom g;
-	const float* const* depth; const float4* const* normal; const int* slots;
+	const float* const* depth; const float4* const* normal; const int* slots;   // the uploaded tables, or nullptr: the arrays below
 	float4* texel; float4* src; int* nsrc; size_t slot_npix;   // quarter-res pixels per slot: texel map slot_npix float4, source list 2 * slot_npix
 	float dmin, dmax;
+	const float* depth_in[kStoreInline]; const float4* normal_in[kStoreInline]; int slot_in[kStoreInline];
 };
-__global__ void __launch_bounds__(1024, 2) k_frame_cache_store(CacheStoreArgs c) {
+__device__ __forceinline__ const float* store_depth(const CacheStoreArgs& c, int f) { return c.depth ? c.depth[f] : c.depth_in[f]; }
+__device__ __forceinline__ const float4* store_normal(const CacheStoreArgs& c, int f) { return c.normal ? c.normal[f] : c.normal_in[f]; }
+__device__ __forceinline__ int store_slot(const CacheStoreArgs& c, int f) { return c.slots ? c.slots[f] : c.slot_in[f]; }
+__global__ void __launch_bounds__(1024, 2) k_frame_cache_store(const __grid_constant__ CacheStoreArgs c) {
 	__shared__ int s_cnt[kPrepRounds * 32];
 	__shared__ int s_wt[32];
-	const int slot = c.slots[blockIdx.x];
-	const int n = build_frame_maps(c.g, c.depth[blockIdx.x], c.normal[blockIdx.x], c.texel + (size_t)slot * c.slot_npix, c.src + (size_t)slot * 2 * c.slot_npix,
+	const int slot = store_slot(c, blockIdx.x);
+	const int n = build_frame_maps(c.g, store_depth(c, blockIdx.x), store_normal(c, blockIdx.x), c.texel + (size_t)slot * c.slot_npix, c.src + (size_t)slot * 2 * c.slot_npix,
 	                               c.dmin, c.dmax, s_cnt, s_wt);
 	if (threadIdx.x == 0) c.nsrc[slot] = n;
 }
 
 // The same store spread over one CTA per 1024 quarter-res pixels (count + build, like k_prep_count / k_prep_frames): a handful of new
 // frames per step - one per tracked window - otherwise runs on a handful of CTAs walking 19 rounds each.
-__global__ void __launch_bounds__(1024, 2) k_cache_count(CacheStoreArgs c, int* __restrict__ blk_cnt) {
+// k_cache_count reads nothing before its wait (the caller's maps may come from the kernel right before the store) and releases
+// k_cache_build only after it: k_cache_build then loads its samples while the last count CTAs finish.  k_cache_build's writes wait for
+// k_cache_count's completion, which follows the previous kernel's - in a tracking step, the k_solve that read the slot being rewritten.
+__global__ void __launch_bounds__(1024, 2) k_cache_count(const __grid_constant__ CacheStoreArgs c, int* __restrict__ blk_cnt) {
 	const int f = blockIdx.y;
-	frame_block_count(c.g, c.depth[f], c.dmin, c.dmax, blockIdx.x, blk_cnt + f * gridDim.x);
+	chain_wait();
+	chain_release();
+	frame_block_count(c.g, store_depth(c, f), c.dmin, c.dmax, blockIdx.x, blk_cnt + f * gridDim.x);
 }
-__global__ void __launch_bounds__(1024, 2) k_cache_build(CacheStoreArgs c, const int* __restrict__ blk_cnt) {
-	const int f = blockIdx.y, slot = c.slots[f];
-	frame_block_build(c.g, c.depth[f], c.normal[f], c.dmin, c.dmax, blockIdx.x, blk_cnt + f * gridDim.x,
+__global__ void __launch_bounds__(1024, 2) k_cache_build(const __grid_constant__ CacheStoreArgs c, const int* __restrict__ blk_cnt) {
+	const int f = blockIdx.y, slot = store_slot(c, f);
+	chain_release();      // (the successor waits before it reads anything)
+	frame_block_build(c.g, store_depth(c, f), store_normal(c, f), c.dmin, c.dmax, blockIdx.x, blk_cnt + f * gridDim.x,
 	                  c.texel + (size_t)slot * c.slot_npix, c.src + (size_t)slot * 2 * c.slot_npix, c.nsrc + slot);
 }
 
@@ -1404,14 +1445,17 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 	__shared__ float s_part[(NT / 32)][kTileVals];
 	__shared__ int s_is_last, s_p2_claim;
 	const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+	chain_wait();
+	if (a.tstamp && blockIdx.x == 0 && tid == 0) a.tstamp[2] = global_ns();
+	const auto stamp_end = [&]() { if (a.tstamp && tid == 0) atomicMax((unsigned long long*)a.tstamp + 3, (unsigned long long)global_ns()); };
 	const int total = *a.n_tiles_total;
-	if (total <= 0) return;
+	if (total <= 0) { stamp_end(); return; }
 	const int all = total * a.prm.num_iter_outer;      // (the tile plan reports an overflow when this does not fit 31 bits)
 	// One iteration's tiles fit the grid (a single window, a handful of windows): STATIC assignment - CTA c runs tile c of every GN
 	// iteration.  With the queue the CTAs claim one tile ahead, i.e. into the NEXT iteration, and then sit on the iteration flag while
 	// the current iteration's last tiles wait for a CTA that finishes its first one, and an iteration's tile phase takes up to two tiles' time.
 	const bool fixed = total <= (int)gridDim.x;
-	if (fixed && (int)blockIdx.x >= total) return;
+	if (fixed && (int)blockIdx.x >= total) { stamp_end(); return; }
 	if (tid == 0) {
 		const int t0 = fixed ? (int)blockIdx.x : atomicAdd(a.queue, 1);
 		s_tile = t0; s_p2_claim = 0; s_pre[0] = 0;
@@ -1544,6 +1588,10 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 		}      // dense tile
 		PROF_T(5);
 		if (a.prof && tid == 0) { prf.kind_cta = blockIdx.x; prf.tile_win = ((long long)tl_idx << 32) | ((long long)it << 16) | tl.count; prf.t[6] = prf.t[7] = prf.t[8] = prf.t[9] = 0; prof_emit(a, prf); }
+		// this CTA's look-ahead claim found no tile left: the next kernel on the stream may launch into the SMs this CTA and the others
+		// that are done leave idle, while the windows' last tails run.  It only waits for k_solve's completion, and every CTA of k_solve is
+		// resident before any of its CTAs (the grid never exceeds one wave), so the persistent kernel's progress argument holds (DESIGN §3.1).
+		if (s_tile >= all) chain_release();
 		if (s_is_last) {
 			window_tail<NT>(a, wd, a.wsp[tl.win], tl.win, it, dyn_smem, &s_p2_claim);
 			__threadfence();
@@ -1552,6 +1600,7 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 		}
 		cur ^= 1;
 	}
+	stamp_end();
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -1617,7 +1666,11 @@ struct SolverState {
 	Event ev_prev, ev_early;
 	Event ev_stage_free[2];              // behind the k_solve that last read staging block 0 / 1
 	int stage_cur = 0;
-	Event ev[4];
+	// ev_stage_free of the current block is recorded when the next batch is staged, on the stream of the last bt_solve_run, not right
+	// behind k_solve: there it would sit between k_solve and the next step's store and cut the launch chain
+	cudaStream_t run_stream = nullptr;
+	bool run_pending = false;
+	DevBuf tstamp;                       // SolveArgs::tstamp (timing on)
 };
 void StateDeleter::operator()(SolverState* s) const { delete s; }
 
@@ -1675,18 +1728,22 @@ extern "C" int bt_solve_enable_debug(bt_ctx* ctx, int on) {
 extern "C" int bt_solve_enable_timing(bt_ctx* ctx, int on) {
 	BT_REQUIRE(ctx && ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_enable_timing: call bt_solver_reserve first");
 	SolverState* s = ctx->solver.get();
-	if (on) for (Event& e : s->ev) BT_TRY(e.create(true));
+	if (on && !s->tstamp.p) { BT_TRY(s->tstamp.alloc(4 * sizeof(long long))); BT_CUDA(cudaMemset(s->tstamp.p, 0, 4 * sizeof(long long))); }
 	s->timing = on != 0;
 	return BT_OK;
 }
 
-// Device time of the LAST bt_solve_run as (prep incl. the tile plan, gap, solve), from CUDA events recorded on the
-// launching stream.  Synchronises on the last event.
+// Device time of the LAST bt_solve_run as (prep incl. the tile plan, gap, solve), from %globaltimer stamps the kernels write: prep =
+// first prep kernel's start to the tile plan's end, gap = from there to k_solve's start, solve = k_solve's start to its last CTA's end.
+// Synchronises the device.
 extern "C" int bt_solve_get_timing(bt_ctx* ctx, float* ms3) {
 	BT_REQUIRE(ctx && ctx->solver && ctx->solver->timing && ms3, BT_ERR_INVALID_ARG, "bt_solve_get_timing: timing not enabled");
 	SolverState* s = ctx->solver.get();
-	BT_CUDA(cudaEventSynchronize(s->ev[3]));
-	for (int k = 0; k < 3; k++) BT_CUDA(cudaEventElapsedTime(ms3 + k, s->ev[k], s->ev[k + 1]));
+	BT_CUDA(cudaSetDevice(ctx->device));
+	BT_CUDA(cudaDeviceSynchronize());
+	long long t[4];
+	BT_CUDA(cudaMemcpy(t, s->tstamp.p, sizeof t, cudaMemcpyDeviceToHost));
+	for (int k = 0; k < 3; k++) ms3[k] = (float)((double)(t[k + 1] - t[k]) * 1e-6);
 	return BT_OK;
 }
 
@@ -1981,6 +2038,7 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 	// ---- early upload.  Two device staging blocks, used alternately: every upload of this batch runs on the private copy stream and only waits for
 	// the k_solve that last read THIS block (two batches ago), so with the streaming form the 2 MB of batch k+1 cross PCIe while batch k is being solved.
 	BT_TRY(s->copy_stream.create());
+	if (s->run_pending) { BT_TRY(s->ev_stage_free[s->stage_cur].record(s->run_stream)); s->run_pending = false; }     // behind the runs of the block being left
 	s->stage_cur ^= 1;
 	DevBuf& stage_dev = s->stage_buf[s->stage_cur];
 	if (s->ev_stage_free[s->stage_cur]) BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_stage_free[s->stage_cur], 0));
@@ -2055,6 +2113,20 @@ static int ensure_occupancy(bt_ctx* ctx) {
 	return BT_OK;
 }
 
+// Launches `kern` as the next link of the stream's dependent-launch chain: it may start while the kernel before it on the stream
+// finishes, and its chain_wait() orders it behind that kernel (DESIGN §3.4).  Behind a copy or an event wait it starts as a plain launch.
+template <typename... KArgs, typename... Args>
+static int launch_chained(void (*kern)(KArgs...), dim3 grid, int threads, size_t smem, cudaStream_t stream, Args&&... args) {
+	cudaLaunchAttribute attr;
+	attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+	attr.val.programmaticStreamSerializationAllowed = 1;
+	cudaLaunchConfig_t cfg = {};
+	cfg.gridDim = grid; cfg.blockDim = dim3((unsigned)threads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+	cfg.attrs = &attr; cfg.numAttrs = 1;
+	BT_CUDA(cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...));
+	return BT_OK;
+}
+
 static SolveArgs make_args(bt_ctx* ctx) {
 	SolverState* s = ctx->solver.get();
 	SolveArgs a;
@@ -2075,6 +2147,8 @@ static SolveArgs make_args(bt_ctx* ctx) {
 	a.tiles_done = s->tiles_done.as<int>(); a.iter_done = s->iter_done.as<int>();
 	a.chunk = s->chunk; a.grp_in_smem = s->grp_in_smem ? 1 : 0; a.prm = s->prm; a.d2max = s->d2max; a.grid_ctas = ctx->sm_count * s->occ;
 	if (s->prof_cap > 0) { a.prof = s->prof.as<long long>(); a.prof_cap = s->prof_cap; }
+	if (s->timing) a.tstamp = s->tstamp.as<long long>();
+	a.with_count = s->any_uncached ? 1 : 0;
 	if (s->debug) { a.dbg_JtJ = s->dbgJ.as<float>(); a.dbg_Jtr = s->dbgR.as<float>(); a.dbg_stride = 6 * s->lim.max_frames; a.dbg_cnt = s->dbgC.as<float>(); a.dbg_cnt_stride = s->max_pairs;
 	                a.dbg_sys = s->dbgS.as<float>(); a.dbg_sys_stride = 6 * (s->lim.max_frames - 1); }
 	return a;
@@ -2084,13 +2158,10 @@ static int launch_prep(bt_ctx* ctx, cudaStream_t stream) {
 	SolverState* s = ctx->solver.get();
 	// make_args again at run time: grid_ctas and grp_in_smem are only final there (in the fused call the tile plan aims at the last batch's occupancy)
 	SolveArgs a = make_args(ctx);
-	if (s->timing) BT_CUDA(cudaEventRecord(s->ev[0], stream));
 	// frames whose maps come from the frame cache need one block each (source count + pose); a batch of cached frames only skips the count kernel
 	const dim3 pgrid(s->any_uncached ? (unsigned)((s->npix_max + 1023) / 1024) : 1u, (unsigned)s->frames_total);
-	if (s->any_uncached) k_prep_count<<<pgrid, 1024, 0, stream>>>(a, s->blk_cnt.as<int>());
-	k_prep_frames<<<pgrid, 1024, 0, stream>>>(a, const_cast<WinDesc*>(a.wins), s->scalars.as<int>() + 8, s->blk_cnt.as<int>());
-	BT_CUDA(cudaGetLastError());
-	if (s->timing) BT_CUDA(cudaEventRecord(s->ev[1], stream));
+	if (s->any_uncached) BT_TRY(launch_chained(k_prep_count, pgrid, 1024, 0, stream, a, s->blk_cnt.as<int>()));
+	BT_TRY(launch_chained(k_prep_frames, pgrid, 1024, 0, stream, a, const_cast<WinDesc*>(a.wins), s->scalars.as<int>() + 8, (const int*)s->blk_cnt.as<int>()));
 	s->prep_launched = true;
 	return BT_OK;
 }
@@ -2110,13 +2181,10 @@ extern "C" int bt_solve_run(bt_ctx* ctx, void* stream_) {
 	if (s->prof_cap > 0) BT_CUDA(cudaMemsetAsync(s->prof.p, 0, 8, stream));
 	if (!s->prep_launched) BT_TRY(launch_prep(ctx, stream));
 	s->prep_launched = false;       // a second bt_solve_run on the same staged batch prepares again (poses restart from the staged input)
-	if (s->timing) BT_CUDA(cudaEventRecord(s->ev[2], stream));
 	const int occ = s->occ;
 	const int grid = ctx->sm_count * occ;
-	k_solve<256, BT_SOLVE_MIN_CTAS><<<grid, 256, s->smem_bytes, stream>>>(a);
-	BT_CUDA(cudaGetLastError());
-	BT_TRY(s->ev_stage_free[s->stage_cur].record(stream));      // this batch's staging block may be overwritten after this point
-	if (s->timing) BT_CUDA(cudaEventRecord(s->ev[3], stream));
+	BT_TRY(launch_chained(k_solve<256, BT_SOLVE_MIN_CTAS>, dim3((unsigned)grid), 256, (size_t)s->smem_bytes, stream, a));
+	s->run_stream = stream; s->run_pending = true;      // (ev_stage_free: see SolverState)
 	s->launches = s->any_uncached ? 3 : 2;
 	return BT_OK;
 }
@@ -2218,34 +2286,40 @@ extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* sl
 	BT_REQUIRE(H > 0 && W > 0 && geom.w >= 2 && geom.h >= 2 && geom.w * geom.h <= s->c_npix, BT_ERR_CAPACITY, "bt_frame_cache_store: image %dx%d does not fit the reserved cache", W, H);
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
-	const size_t b_ptr = sizeof(void*) * (size_t)n_frames, bytes = 2 * b_ptr + sizeof(int) * (size_t)n_frames;
-	BT_TRY(s->c_tables.alloc(bytes));
-	UploadBuf& up = s->c_htables[s->c_flip];
-	s->c_flip ^= 1;
-	char* hb;
-	BT_TRY(up.acquire(bytes, &hb));
-	const void** hd = (const void**)hb; const void** hn = (const void**)(hb + b_ptr); int* hs = (int*)(hb + 2 * b_ptr);
 	for (int f = 0; f < n_frames; f++) {
 		BT_REQUIRE(slots[f] >= 0 && slots[f] < s->c_capacity, BT_ERR_INVALID_ARG, "bt_frame_cache_store: slot %d out of range [0,%d)", slots[f], s->c_capacity);
 		BT_REQUIRE(depth_dev[f] && normal_dev[f], BT_ERR_INVALID_ARG, "bt_frame_cache_store: frame %d has a NULL map", f);
 		for (int g = 0; g < f; g++) BT_REQUIRE(slots[g] != slots[f], BT_ERR_INVALID_ARG, "bt_frame_cache_store: slot %d listed twice", slots[f]);
-		hd[f] = depth_dev[f]; hn[f] = normal_dev[f]; hs[f] = slots[f];
 	}
-	BT_CUDA(cudaMemcpyAsync(s->c_tables.p, hb, bytes, cudaMemcpyHostToDevice, stream));
-	BT_TRY(up.in_flight(stream));
 	CacheStoreArgs c;
+	memset(&c, 0, sizeof c);
 	c.g = geom;
-	char* db = s->c_tables.as<char>();
-	c.depth = (const float* const*)db; c.normal = (const float4* const*)(db + b_ptr); c.slots = (const int*)(db + 2 * b_ptr);
 	c.texel = s->c_texel.as<float4>(); c.src = s->c_src.as<float4>(); c.nsrc = s->c_nsrc.as<int>(); c.slot_npix = (size_t)s->c_npix;
 	c.dmin = depth_min; c.dmax = depth_max;
-	if (n_frames >= 2 * ctx->sm_count) k_frame_cache_store<<<n_frames, 1024, 0, stream>>>(c);      // many frames: one CTA per frame fills the machine (faster than count + build there, DESIGN §9.6)
-	else {
-		const dim3 grid((unsigned)((geom.w * geom.h + 1023) / 1024), (unsigned)n_frames);
-		k_cache_count<<<grid, 1024, 0, stream>>>(c, s->c_blk.as<int>());
-		k_cache_build<<<grid, 1024, 0, stream>>>(c, s->c_blk.as<int>());
+	if (n_frames <= kStoreInline) {
+		for (int f = 0; f < n_frames; f++) { c.depth_in[f] = depth_dev[f]; c.normal_in[f] = (const float4*)normal_dev[f]; c.slot_in[f] = slots[f]; }
+	} else {
+		const size_t b_ptr = sizeof(void*) * (size_t)n_frames, bytes = 2 * b_ptr + sizeof(int) * (size_t)n_frames;
+		BT_TRY(s->c_tables.alloc(bytes));
+		UploadBuf& up = s->c_htables[s->c_flip];
+		s->c_flip ^= 1;
+		char* hb;
+		BT_TRY(up.acquire(bytes, &hb));
+		const void** hd = (const void**)hb; const void** hn = (const void**)(hb + b_ptr); int* hs = (int*)(hb + 2 * b_ptr);
+		for (int f = 0; f < n_frames; f++) { hd[f] = depth_dev[f]; hn[f] = normal_dev[f]; hs[f] = slots[f]; }
+		BT_CUDA(cudaMemcpyAsync(s->c_tables.p, hb, bytes, cudaMemcpyHostToDevice, stream));
+		BT_TRY(up.in_flight(stream));
+		char* db = s->c_tables.as<char>();
+		c.depth = (const float* const*)db; c.normal = (const float4* const*)(db + b_ptr); c.slots = (const int*)(db + 2 * b_ptr);
 	}
-	BT_CUDA(cudaGetLastError());
+	if (n_frames >= 2 * ctx->sm_count) {      // many frames: one CTA per frame fills the machine (faster than count + build there, DESIGN §9.6)
+		k_frame_cache_store<<<n_frames, 1024, 0, stream>>>(c);
+		BT_CUDA(cudaGetLastError());
+	} else {
+		const dim3 grid((unsigned)((geom.w * geom.h + 1023) / 1024), (unsigned)n_frames);
+		BT_TRY(launch_chained(k_cache_count, grid, 1024, 0, stream, c, s->c_blk.as<int>()));
+		BT_TRY(launch_chained(k_cache_build, grid, 1024, 0, stream, c, (const int*)s->c_blk.as<int>()));
+	}
 	for (int f = 0; f < n_frames; f++) {
 		SolverState::CacheMeta& m = s->c_meta[slots[f]];
 		m.valid = true; m.H = H; m.W = W; m.fx = fx; m.fy = fy; m.cx = cx; m.cy = cy; m.dmin = depth_min; m.dmax = depth_max;

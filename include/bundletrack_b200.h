@@ -162,8 +162,8 @@ typedef struct {
 BT_API int bt_solve_get_stats(bt_ctx* ctx, bt_solve_stats* out);
 /* Copies the dense system (6N x 6N JtJ, row-major, reference ordering trans 0-2 / rot 3-5, and 6N Jtr) that the
  * LAST Gauss-Newton iteration of window `w` assembled; debugging/parity aid. */
-/* Per-kernel device time of the last bt_solve_run (ms3 = {frame cache, plan, persistent solve}), CUDA events on the
- * launching stream; opt-in because it adds four event records per run. */
+/* Per-kernel device time of the last bt_solve_run (ms3 = {frame preparation incl. the tile plan, gap to the solve, persistent
+ * solve}), from device-timer stamps the kernels write; opt-in.  bt_solve_get_timing synchronises the device. */
 BT_API int bt_solve_enable_timing(bt_ctx* ctx, int on);
 BT_API int bt_solve_get_timing(bt_ctx* ctx, float* ms3);
 /* Host-side time of the last bt_solve_windows call, microseconds: us6 = {window tables + first upload, frame-preparation launch,
