@@ -157,6 +157,23 @@ class DescView(ctypes.Structure):
     ]
 
 
+class LfnetParams(ctypes.Structure):
+    _fields_ = [
+        ("top_k", ctypes.c_int),
+        ("net_channel", ctypes.c_int), ("net_block", ctypes.c_int), ("conv_ksize", ctypes.c_int), ("net_num_scales", ctypes.c_int),
+        ("net_min_scale", ctypes.c_double), ("net_max_scale", ctypes.c_double),
+        ("leaky_alpha", ctypes.c_float),
+        ("sm_ksize", ctypes.c_int),
+        ("com_strength", ctypes.c_float), ("score_com_strength", ctypes.c_float), ("scale_com_strength", ctypes.c_float),
+        ("kp_loc_size", ctypes.c_int),
+        ("kp_com_strength", ctypes.c_float),
+        ("nms_ksize", ctypes.c_int),
+        ("nms_thresh", ctypes.c_float),
+        ("crop_radius", ctypes.c_int), ("patch_size", ctypes.c_int),
+        ("desc_net_channel", ctypes.c_int), ("desc_net_depth", ctypes.c_int), ("desc_conv_ksize", ctypes.c_int), ("desc_dim", ctypes.c_int),
+    ]
+
+
 # Every entry point of include/bundletrack_b200.h as (restype, argtypes), in the header's order; load() applies it, so a call site passes
 # plain Python values and ctypes converts each to the C type declared here (tests/test_abi.py checks the table against the header).
 # int / int32_t -> c_int, float -> c_float, double -> c_double, long long -> c_longlong, size_t -> c_size_t, uint64_t -> c_uint64, a pointer
@@ -258,6 +275,13 @@ PROTOTYPES = {
     "bt_match_viz_shape": (_i, (_p, _p, _p, _p)),
     "bt_match_viz_reserve": (_i, (_p, _i, _i)),
     "bt_match_viz": (_i, (_p, _i, _P(MatchVizDesc), _p, _p)),
+    "bt_lfnet_weights_size": (_i, (_p, _p)),
+    "bt_lfnet_reserve": (_i, (_p, _p, _i)),
+    "bt_lfnet_load_weights": (_i, (_p, _p, _sz)),
+    "bt_lfnet_detect": (_i, (_p, _i, _p, _p, _p, _p, _p)),
+    "bt_lfnet_enable_timing": (_i, (_p, _i)),
+    "bt_lfnet_get_timing": (_i, (_p, _p)),
+    "bt_lfnet_debug_maps": (_i, (_p, _i, _p, _p, _p, _p, _p)),
     "bt_dev_alloc": (_i, (_p, _sz)),
     "bt_dev_free": (_i, (_p,)),
     "bt_memcpy_h2d": (_i, (_p, _p, _sz, _p)),

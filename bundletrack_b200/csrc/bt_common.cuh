@@ -140,6 +140,7 @@ struct MetricsState;  // metrics.cu
 struct NocsState;     // metrics.cu
 struct OverlayState;  // overlay.cu
 struct MatchVizState; // matchviz.cu
+struct LfnetState;    // lfnet.cu
 
 // The context owns the module states; each module defines the deleter of its state next to it, so the states stay private to their files.
 struct StateDeleter {
@@ -154,6 +155,7 @@ struct StateDeleter {
 	void operator()(NocsState*) const;
 	void operator()(OverlayState*) const;
 	void operator()(MatchVizState*) const;
+	void operator()(LfnetState*) const;
 };
 template <class T> using StatePtr = std::unique_ptr<T, StateDeleter>;
 
@@ -174,6 +176,7 @@ struct bt_ctx {
 	bt::StatePtr<bt::NocsState> nocs;
 	bt::StatePtr<bt::OverlayState> overlay;
 	bt::StatePtr<bt::MatchVizState> matchviz;
+	bt::StatePtr<bt::LfnetState> lfnet;
 };
 
 namespace bt {

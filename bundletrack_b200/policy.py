@@ -41,12 +41,24 @@ def lfnet_parse_reply(parts, roi):
     """parts: the three byte strings of the LF-Net server's reply; roi = (umin, umax, vmin, vmax).  Returns (kpts [n,2] float32 in image
     pixels, desc [n,dim] float32 view of part 2)."""
     info, kp, desc = (bytes(p) for p in parts)
+    kpts, n, dim = _parse_reply(info, kp, len(desc), roi)
+    return kpts, np.frombuffer(desc, np.float32).reshape(n, dim)
+
+
+def lfnet_reply_keypoints(n: int, dim: int, kpts_400, roi) -> np.ndarray:
+    """The keypoints of a reply with n rows of dim-dimensional descriptors whose keypoint part is kpts_400 (n x (x, y) float32 in the
+    400 x 400 network input), in image pixels: lfnet_parse_reply's transform for a source whose descriptors never leave the device."""
+    kp = np.ascontiguousarray(kpts_400, np.float32).reshape(-1)
+    return _parse_reply(np.array([n, dim], np.int32).tobytes(), kp.tobytes(), 4 * n * dim, roi)[0]
+
+
+def _parse_reply(info: bytes, kp: bytes, desc_bytes: int, roi):
     n_guess = max(len(kp) // 8, 1)
     out = np.zeros((n_guess, 2), np.float32)
     n, dim = ctypes.c_int(0), ctypes.c_int(0)
-    _lib.check(_lib.load().bt_lfnet_parse_reply(info, len(info), kp, len(kp), len(desc), _lib.i32s(roi), _lib.ptr(out), n_guess, ctypes.byref(n),
+    _lib.check(_lib.load().bt_lfnet_parse_reply(info, len(info), kp, len(kp), desc_bytes, _lib.i32s(roi), _lib.ptr(out), n_guess, ctypes.byref(n),
                                                 ctypes.byref(dim)), "bt_lfnet_parse_reply")
-    return out[:n.value], np.frombuffer(desc, np.float32).reshape(n.value, dim.value)
+    return out[:n.value], n.value, dim.value
 
 
 class Tracks:

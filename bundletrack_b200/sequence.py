@@ -424,7 +424,9 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
     policy.save_pose_txt (Bundler::saveNewframeResult runs after every frame): the initial pose of a frame that fails the ROI gate, the
     pose drop_frame reports when detection fails, otherwise end_frame's.  features(id_str, request uint8 [400,400,3] host, roi) returns
     (kpts [n,2] image pixels, desc [n,256] float32) or raises DetectionFailed; a reply with more than max_feats rows or descriptors that are
-    not 256-dimensional is dropped too.  Sizing as INTEGRATION.md §7: max_frames_alive = bundle.window_size + 4, max_keyframes defaults to
+    not 256-dimensional is dropped too.  A source marked on_device (lfnet.LfnetDevice) is called as features.features_on_device(id_str,
+    request uint8 [400,400,3] on the device, roi, stream) instead and returns the keypoints on the host and the descriptors on the device, so
+    neither the request nor the descriptors cross the bus.  Sizing as INTEGRATION.md §7: max_frames_alive = bundle.window_size + 4, max_keyframes defaults to
     min(1024, ceil(n_frames / 2)).  Nothing under out_dir is removed.  Returns [(id_str, status, wall seconds)] per frame.
     log > 0 (the yml's LOG): every frame's LOG images under out_dir (the reference's debug_dir), drawn on the device with the pose its pose
     file holds (overlay.Overlay over loader.model_path) and written by a LogWriter thread; needs cv2.  log = 0 runs none of it."""
@@ -443,6 +445,7 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
     trk = Tracker(y, H, W, loader.K, max_feats, int(y["bundle"]["window_size"]) + 4, device=device, stream=stream.cuda_stream,
                   mode=loader.mask_mode, max_keyframes=max_keyframes)
     reader = ovl = writer = None
+    on_device = getattr(features, "on_device", False)
     out = []
     try:
         if log > 0:
@@ -463,20 +466,26 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
             if ovl is None:
                 reader.release(i)
             if st == _lib.BT_FRAME_OTHER:
-                with torch.cuda.device(dev), torch.cuda.stream(stream):
-                    req = request.cpu()
                 try:
-                    kpts, desc = features(ff.id_str, req.numpy(), roi)
-                    kpts = np.ascontiguousarray(kpts, np.float32).reshape(-1, 2)
-                    desc = np.ascontiguousarray(desc, np.float32)
+                    if on_device:
+                        kpts, desc = features.features_on_device(ff.id_str, request, roi, stream.cuda_stream)
+                    else:
+                        with torch.cuda.device(dev), torch.cuda.stream(stream):
+                            req = request.cpu()
+                        kpts, desc = features(ff.id_str, req.numpy(), roi)
+                        kpts = np.ascontiguousarray(kpts, np.float32).reshape(-1, 2)
+                        desc = np.ascontiguousarray(desc, np.float32)
                     if desc.ndim != 2 or desc.shape[1] != DESC_DIM or len(desc) != len(kpts) or len(kpts) > max_feats:
-                        raise DetectionFailed(f"frame {ff.id_str}: {len(kpts)} keypoints with descriptors {desc.shape}; the tracker takes at most "
-                                              f"{max_feats} rows of {DESC_DIM}")
+                        raise DetectionFailed(f"frame {ff.id_str}: {len(kpts)} keypoints with descriptors {tuple(desc.shape)}; the tracker takes at "
+                                              f"most {max_feats} rows of {DESC_DIM}")
                 except DetectionFailed:
                     pose, st = trk.drop_frame(), _lib.BT_FRAME_FAIL
                 else:
-                    with torch.cuda.device(dev), torch.cuda.stream(stream):
-                        desc_dev = torch.from_numpy(desc).to(dev)
+                    if on_device:
+                        desc_dev = desc
+                    else:
+                        with torch.cuda.device(dev), torch.cuda.stream(stream):
+                            desc_dev = torch.from_numpy(desc).to(dev)
                     try:
                         pose, st = trk.end_frame(kpts, desc_dev)
                     except _lib.BtError as e:

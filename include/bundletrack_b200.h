@@ -656,6 +656,54 @@ BT_API int bt_match_viz_reserve(bt_ctx* ctx, int max_images, int max_matches);
  * BT_ERR_CAPACITY beyond the reserved images or matches. */
 BT_API int bt_match_viz(bt_ctx* ctx, int n_images, const bt_match_viz_desc* desc, uint8_t* const* out_dev, void* stream);
 
+/* ---- LF-Net on the device: Lfnet::detectFeature's feature server (lf-net-release/run_server.py) without TensorFlow ----------------------
+ * The network run_server.py builds at train_lfnet.py's defaults (DESIGN.md §3.12): mso_resnet_detector with use_nms3d, soft_scale and
+ * soft_kpts, simple_desc on photo patches, l2-normalised descriptors, FP32 throughout.  bt_lfnet_params holds its numeric hyper-parameters;
+ * the kernels take net_channel 16 and conv_ksize 5 only (the orientation conv uses conv_ksize as the reference's does).
+ * bt_lfnet_weights_size: the float count of the weight blob for `p` (host code, no GPU).  Blob layout, float32, in this order (TF weight
+ * layouts [kh][kw][cin][cout] and [in][out]; BN = (scale, shift) with scale = gamma / sqrt(moving_variance + 1e-5), shift = beta -
+ * moving_mean scale, folded in float64 and rounded once; C = net_channel, k = conv_ksize):
+ *   init_conv W[k][k][1][C] b[C]; per block: pre-bn scale[C] shift[C], conv1 W[k][k][C][C] b[C], mid-bn scale shift, conv2 W b;
+ *   fin-bn scale[C] shift[C]; per scale i: score_conv_i W[k][k][C][1] b[1]; ori_conv W[k][k][C][2] b[2];
+ *   per descriptor conv l: W[kd][kd][cin][cout] scale[cout] shift[cout] (shift also holds the conv bias times scale);
+ *   fc1 W[F][512] scale[512] shift[512] (F = the flattened last conv output, HWC); fc2 W[512][desc_dim] b[desc_dim].
+ * bt_lfnet_reserve: everything bt_lfnet_detect uses for up to max_images requests per call (about 46 MB per image for the maps plus
+ * 122 KB per keypoint row at the defaults); a later call with other parameters drops the loaded weights.  BT_ERR_INVALID_ARG names a
+ * parameter the kernels do not take.
+ * bt_lfnet_load_weights: copies the blob (synchronously); refuses a size other than bt_lfnet_weights_size's and non-finite floats.
+ * bt_lfnet_detect: n requests (HOST array of DEVICE pointers to 400 x 400 x 3 uint8, bt_lfnet_request's output) in one asynchronous call:
+ *   kpts_out   DEVICE float [n][top_k][2]: (x, y) in the 400 x 400 input, the server's reply keypoints, row-major pixel order of the
+ *              integer peaks (tf.where); rows past n_out[i] are zero.
+ *   desc_out   DEVICE float [n][top_k][desc_dim]: the reply's descriptor rows (a bt_desc_view with pitch desc_dim * 4); rows past n_out[i]
+ *              are zero.
+ *   n_out      DEVICE int32 [n]: keypoints per request (top_k, or fewer when fewer NMS peaks are selected).
+ * Results do not depend on how requests are batched.  BT_ERR_CAPACITY above max_images.
+ * bt_lfnet_enable_timing / bt_lfnet_get_timing: device time of the last call per stage, ms5 = {trunk, score maps, detection, keypoints and
+ * patches, descriptor}; get_timing waits for that call.
+ * bt_lfnet_debug_maps (test aid): image `image` of the last call's max_heatmaps and max_scales (400 x 400 floats each), its integer
+ * keypoints (top_k x (x, y) int32) and orientations (top_k x (cos, sin)), each output optional; synchronises `stream`. */
+typedef struct {
+	int top_k;                 /* run_server.py --top_k (500) */
+	int net_channel, net_block, conv_ksize, net_num_scales;
+	double net_min_scale, net_max_scale;
+	float leaky_alpha;
+	int sm_ksize;
+	float com_strength, score_com_strength, scale_com_strength;
+	int kp_loc_size;
+	float kp_com_strength;
+	int nms_ksize;
+	float nms_thresh;
+	int crop_radius, patch_size;
+	int desc_net_channel, desc_net_depth, desc_conv_ksize, desc_dim;
+} bt_lfnet_params;
+BT_API int bt_lfnet_weights_size(const bt_lfnet_params* p, size_t* n_floats);
+BT_API int bt_lfnet_reserve(bt_ctx* ctx, const bt_lfnet_params* params, int max_images);
+BT_API int bt_lfnet_load_weights(bt_ctx* ctx, const float* blob, size_t n_floats);
+BT_API int bt_lfnet_detect(bt_ctx* ctx, int n, const uint8_t* const* request_dev, float* kpts_out, float* desc_out, int32_t* n_out, void* stream);
+BT_API int bt_lfnet_enable_timing(bt_ctx* ctx, int on);
+BT_API int bt_lfnet_get_timing(bt_ctx* ctx, float* ms5);
+BT_API int bt_lfnet_debug_maps(bt_ctx* ctx, int image, float* heat_host, float* scale_host, int32_t* kpts_int_host, float* ori_host, void* stream);
+
 /* Small device-memory helpers so non-CUDA hosts (ctypes, cgo, JNI) can drive the library without another runtime. */
 BT_API int bt_dev_alloc(void** out, size_t bytes);
 BT_API int bt_dev_free(void* p);

@@ -25,6 +25,8 @@ def main():
     ap.add_argument("--scene_id", type=int, default=1)
     ap.add_argument("--model_name", default="can_arizona_tea_norm")
     ap.add_argument("--port", type=int, default=5555, help="the LF-Net server's port")
+    ap.add_argument("--lfnet_model", default=None, help="instead of the server: a released LF-Net model directory (config.pkl and "
+                                                        "weights.npz from scripts/lfnet_export_weights.py), run on the device")
     ap.add_argument("--mask_dir", required=True, help="the scene's and model's masks, <id>.png")
     ap.add_argument("--out_dir", required=True)
     ap.add_argument("--config", default=None, help="a config_nocs.yml (default: its values, bundletrack_b200.config.NOCS_DEFAULTS)")
@@ -33,7 +35,11 @@ def main():
                                                        "directory (<id>/color_viz.jpg, color_viz/, color_raw/); needs cv2")
     a = ap.parse_args()
     loader = NocsScene(a.nocs_dir, a.scene_id, a.model_name, a.mask_dir)
-    client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
+    if a.lfnet_model:
+        from bundletrack_b200.lfnet import load_lfnet
+        client = load_lfnet(a.lfnet_model, device=a.device)
+    else:
+        client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
     try:
         res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, f"{a.model_name}_{a.scene_id}"), device=a.device, log=a.log)
     finally:

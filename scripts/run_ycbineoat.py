@@ -22,6 +22,8 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--data_dir", required=True, help="one video's directory")
     ap.add_argument("--port", type=int, default=5555, help="the LF-Net server's port")
+    ap.add_argument("--lfnet_model", default=None, help="instead of the server: a released LF-Net model directory (config.pkl and "
+                                                        "weights.npz from scripts/lfnet_export_weights.py), run on the device")
     ap.add_argument("--out_dir", required=True)
     ap.add_argument("--config", default=None, help="the reference's config_ycbineoat.yml (default: the config_nocs.yml values, "
                                                     "bundletrack_b200.config.NOCS_DEFAULTS)")
@@ -34,7 +36,11 @@ def main():
         raise SystemExit(f"--data_dir {a.data_dir} is not a directory")
     loader = YcbineoatVideo(a.data_dir, a.model_dir)
     video = os.path.basename(os.path.normpath(a.data_dir))
-    client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
+    if a.lfnet_model:
+        from bundletrack_b200.lfnet import load_lfnet
+        client = load_lfnet(a.lfnet_model, device=a.device)
+    else:
+        client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
     try:
         res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, video), device=a.device, log=a.log)
     finally:
