@@ -1,6 +1,7 @@
 // bt_common.cuh — shared declarations for the sm_90a hot-path library (no torch, no third-party headers).
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -33,6 +34,17 @@ void set_error(const char* fmt, ...);
 		const int rc_ = (x);                                                                         \
 		if (rc_ != BT_OK) return rc_;                                                                \
 	} while (0)
+
+// Largest float d2max with `sqrtf(d2) <= th` <=> `d2 <= d2max` for every float d2 (sqrtf is correctly rounded and monotonic), so a
+// kernel can compare squared distances.  -1 when no d2 qualifies (th < 0 or NaN); +inf for th = +inf.
+inline float sqrt_le_max(float th) {
+	if (!(th > 0.f)) return (th == 0.f) ? 0.f : -1.f;
+	auto nextf = [](float v, int d) { int32_t b; memcpy(&b, &v, 4); b += d; float r; memcpy(&r, &b, 4); return r; };
+	float d2max = th * th;
+	while (d2max > 0.f && sqrtf(d2max) > th) d2max = nextf(d2max, -1);
+	while (sqrtf(nextf(d2max, 1)) <= th) d2max = nextf(d2max, 1);
+	return d2max;
+}
 
 // What the handle types below hold right now, across the process (bt_debug_live_resources).
 struct LiveResources { std::atomic<long long> dev_bytes{0}, pinned_bytes{0}; std::atomic<int> handles{0}; };

@@ -750,13 +750,13 @@ struct MatcherState {
 	int slot_rows = 0;                      // rows per pool slot (max_feats padded to 256)
 	int n_transient = 0, n_persist = 0;     // transient slots [0, n_transient) serve bt_knn_match_pairs; persistent ones follow
 	std::vector<int> slot_n;                // persistent slots: number of rows stored, -1 = empty
-	DevBuf pool_h, pool_f, norms, errn, slot_meta, sets, pairs, pconst, G, jobs, blk_start, q_start, cand, cand_cnt, qjob, fb_rows, fb_count, fb_part_d, fb_part_i, fb_tickets;
-	UploadBuf h_stage;                      // the set and pair tables of a call
+	DevBuf pool_h, pool_f, norms, errn, slot_meta, sets, tables, pconst, G, cand, cand_cnt, qjob, fb_rows, fb_count, fb_part_d, fb_part_i, fb_tickets;
+	UploadBuf h_stage;                      // the set and work tables of a call
 	PFN_encodeTiled encode = nullptr;
 	CUtensorMap tmap_a, tmap_b;
 	bool maps_ready = false;
 	size_t g_halves_cap = 0;
-	int max_jobs = 0, max_q_total = 0, max_blocks = 0;
+	int max_q_total = 0, max_blocks = 0;
 	int last_units = 0, last_rows = 0;
 	Event ev[5];
 	bool timing = false;
@@ -778,43 +778,69 @@ static int make_tmap(MatcherState* m, CUtensorMap* out, void* base, uint64_t row
 // (re)allocates the descriptor pool for n_transient + n_persist slots and rebuilds the tensor maps over it
 static int pool_alloc(MatcherState* m) {
 	const size_t rows = (size_t)(m->n_transient + m->n_persist) * m->slot_rows + BN;
-	int rc;
-	if ((rc = m->pool_h.alloc(rows * KD * 2)) != BT_OK) return rc;
-	if ((rc = m->pool_f.alloc(rows * KD * 4)) != BT_OK) return rc;
-	if ((rc = m->norms.alloc(rows * 4)) != BT_OK) return rc;
-	if ((rc = m->errn.alloc(rows * 4)) != BT_OK) return rc;
-	if ((rc = m->slot_meta.alloc(sizeof(int) * 2 * (size_t)(m->n_transient + m->n_persist))) != BT_OK) return rc;
-	if ((rc = make_tmap(m, &m->tmap_a, m->pool_h.p, (uint64_t)rows, BM)) != BT_OK) return rc;
-	if ((rc = make_tmap(m, &m->tmap_b, m->pool_h.p, (uint64_t)rows, BN)) != BT_OK) return rc;
+	BT_TRY(m->pool_h.alloc(rows * KD * 2));
+	BT_TRY(m->pool_f.alloc(rows * KD * 4));
+	BT_TRY(m->norms.alloc(rows * 4));
+	BT_TRY(m->errn.alloc(rows * 4));
+	BT_TRY(m->slot_meta.alloc(sizeof(int) * 2 * (size_t)(m->n_transient + m->n_persist)));
+	BT_TRY(make_tmap(m, &m->tmap_a, m->pool_h.p, (uint64_t)rows, BM));
+	BT_TRY(make_tmap(m, &m->tmap_b, m->pool_h.p, (uint64_t)rows, BN));
 	m->maps_ready = true;
 	return BT_OK;
 }
 
+// timing event i, when timing is on: [ev0, ev1) = descriptor conversion + table upload + per-pair constants, [ev1, ev2) = k_knn_tc alone
+static int mark(MatcherState* m, int i, cudaStream_t stream) { if (m->timing) BT_CUDA(cudaEventRecord(m->ev[i], stream)); return BT_OK; }
+
+static size_t desc_pitch(const bt_desc_view& v) { return v.pitch_bytes ? v.pitch_bytes : (size_t)KD * 4; }
+
+// What the matcher requires of a descriptor set.  The error texts begin with `who`, or, for the view of pair `pair` >= 0, with "pair %d".
+static int check_desc(const bt_desc_view& v, const MatcherState* m, const char* who, int pair) {
+	char at[24];
+	auto where = [&]() -> const char* { if (pair < 0) return who; snprintf(at, sizeof at, "pair %d", pair); return at; };
+	BT_REQUIRE(v.dim == KD, BT_ERR_UNSUPPORTED, "%s: descriptor dim %d != %d", where(), v.dim, KD);
+	BT_REQUIRE(v.n >= 0 && v.n <= m->max_feats, BT_ERR_CAPACITY, "%s: %d features > reserved %d", where(), v.n, m->max_feats);
+	BT_REQUIRE(v.n == 0 || v.dev, BT_ERR_INVALID_ARG, "%s: NULL descriptor pointer", where());
+	BT_REQUIRE(((uintptr_t)v.dev & 15) == 0 && (desc_pitch(v) & 15) == 0, BT_ERR_INVALID_ARG, "%s: descriptors must be 16-byte aligned", where());
+	return BT_OK;
+}
+
+// the conversion of a checked descriptor set into pool slot `slot`, padded to whole 256-row B tiles
+static PrepSet prep_set(const MatcherState* m, const bt_desc_view& v, int slot) {
+	return PrepSet{ v.dev, desc_pitch(v), v.n, slot * m->slot_rows, (std::max(v.n, 1) + BN - 1) / BN * BN, slot };
+}
+
 struct PoolSetRef { int slot; int n; };      // a descriptor set in the pool: rows [slot * slot_rows, +n)
 
-static int launch_prep(bt_ctx* ctx, const std::vector<PrepSet>& sets, char* hb, size_t& hoff, cudaStream_t stream) {
-	MatcherState* m = ctx->matcher.get();
+// uploads the set table from the staging block at hb and moves hb past it.  `sets` take consecutive slots (one call's transient slots 0, 1,
+// ..., or the one slot a store writes): one memset clears their counters.
+static int launch_prep(MatcherState* m, const std::vector<PrepSet>& sets, char*& hb, cudaStream_t stream) {
 	if (sets.empty()) return BT_OK;
 	const size_t b_sets = sizeof(PrepSet) * sets.size();
-	memcpy(hb + hoff, sets.data(), b_sets);
-	BT_CUDA(cudaMemcpyAsync(m->sets.p, hb + hoff, b_sets, cudaMemcpyHostToDevice, stream));
-	hoff += (b_sets + 255) & ~(size_t)255;
+	memcpy(hb, sets.data(), b_sets);
+	BT_CUDA(cudaMemcpyAsync(m->sets.p, hb, b_sets, cudaMemcpyHostToDevice, stream));
+	hb += (b_sets + 255) & ~(size_t)255;
+	BT_CUDA(cudaMemsetAsync(m->slot_meta.as<int>() + 2 * sets[0].slot, 0, 2 * sizeof(int) * sets.size(), stream));
 	int max_padded = 0;
-	for (auto& s : sets) { max_padded = std::max(max_padded, s.rows_padded); BT_CUDA(cudaMemsetAsync(m->slot_meta.as<int>() + 2 * s.slot, 0, 2 * sizeof(int), stream)); }
+	for (auto& s : sets) max_padded = std::max(max_padded, s.rows_padded);
 	k_desc_prep<<<dim3((unsigned)std::max(1, std::min((max_padded + 7) / 8, 64)), (unsigned)sets.size()), 256, 0, stream>>>(
 	    m->sets.as<PrepSet>(), m->pool_h.as<__half>(), m->pool_f.as<float>(), m->norms.as<float>(), m->errn.as<float>(), m->slot_meta.as<int>());
 	return BT_OK;
 }
 
-// the matcher proper on descriptor sets that are already in the pool
-static int knn_run(bt_ctx* ctx, int n_pairs, const PoolSetRef* A, const PoolSetRef* B, int k, int32_t* idxAB, float* distAB, int32_t* idxBA, float* distBA,
-                   char* hb, size_t hoff, cudaStream_t stream) {
-	MatcherState* m = ctx->matcher.get();
-	std::vector<KnnPair> pairs;
-	std::vector<SelJob> jobs;
-	std::vector<int> blk_start, q_start;
-	long long units = 0, g_off = 0;
-	int q_total = 0, blocks = 0;
+// The work of one call on descriptor sets in the pool, as the kernels walk it.
+struct KnnPlan {
+	std::vector<KnnPair> pairs;             // the live pairs, then a guard entry: UnitWalk::next() may read one entry past the last pair
+	std::vector<SelJob> jobs;               // one per (pair, direction)
+	std::vector<int> blk_start, q_start;    // per job: its first k_knn_select block, its first query row
+	long long units = 0, g_off = 0;         // tensor-pass units; halves of G in use
+	int q_total = 0, blocks = 0;            // query rows; k_knn_select blocks
+};
+// the four tables lie back to back, in the pinned block and in MatcherState::tables alike
+static_assert(sizeof(KnnPair) % alignof(SelJob) == 0 && sizeof(SelJob) % alignof(int) == 0, "KnnPlan tables must stay aligned back to back");
+struct KnnTables { const KnnPair* pairs; const SelJob* jobs; const int* blk_start; const int* q_start; };
+
+static int plan_work(const MatcherState* m, const char* who, int n_pairs, const PoolSetRef* A, const PoolSetRef* B, KnnPlan& w) {
 	size_t off_dir[2] = { 0, 0 };
 	for (int p = 0; p < n_pairs; p++) {
 		const int nA = A[p].n, nB = B[p].n;
@@ -822,65 +848,88 @@ static int knn_run(bt_ctx* ctx, int n_pairs, const PoolSetRef* A, const PoolSetR
 		KnnPair pr; memset(&pr, 0, sizeof pr);
 		if (live) {
 			pr.a_row0 = A[p].slot * m->slot_rows; pr.b_row0 = B[p].slot * m->slot_rows; pr.nA = nA; pr.nB = nB;
-			pr.n_qt = (nA + BM - 1) / BM; pr.n_tt = (nB + BN - 1) / BN; pr.unit0 = (int)units;      // a unit = 128 A rows x 256 B rows
+			pr.n_qt = (nA + BM - 1) / BM; pr.n_tt = (nB + BN - 1) / BN; pr.unit0 = (int)w.units;      // a unit = 128 A rows x 256 B rows
 			pr.nA_pad = pr.n_qt * BM; pr.nB_pad = pr.n_tt * BN; pr.setA = A[p].slot; pr.setB = B[p].slot;
-			pr.g_row = g_off; g_off += (long long)(pr.nB_pad / GRP) * pr.nA_pad;
-			pr.g_col = g_off; g_off += (long long)(pr.nA_pad / GRP) * pr.nB_pad;
-			units += (long long)pr.n_qt * pr.n_tt;
-			pairs.push_back(pr);
+			pr.g_row = w.g_off; w.g_off += (long long)(pr.nB_pad / GRP) * pr.nA_pad;
+			pr.g_col = w.g_off; w.g_off += (long long)(pr.nA_pad / GRP) * pr.nB_pad;
+			w.units += (long long)pr.n_qt * pr.n_tt;
+			w.pairs.push_back(pr);
 		}
 		for (int dir = 0; dir < 2; dir++) {
 			SelJob jb; memset(&jb, 0, sizeof jb);
 			jb.nq = dir == 0 ? nA : nB; jb.nt = dir == 0 ? nB : nA; jb.n_groups = (jb.nt + 127) / 128 * (128 / GRP);      // whole blocks of 128 positions: a block's valid rows are spread over all of its groups
 			jb.q_pool_row0 = (dir == 0 ? A[p].slot : B[p].slot) * m->slot_rows; jb.t_pool_row0 = (dir == 0 ? B[p].slot : A[p].slot) * m->slot_rows;
-			jb.pconst = live ? (int)pairs.size() - 1 : -1;
+			jb.pconst = live ? (int)w.pairs.size() - 1 : -1;
 			if (live) {
 				jb.g_off = dir == 0 ? pr.g_row : pr.g_col; jb.x_off = dir == 0 ? pr.g_col : pr.g_row;
 				jb.q_stride = dir == 0 ? pr.nA_pad : pr.nB_pad; jb.x_stride = dir == 0 ? pr.nB_pad : pr.nA_pad;
 			}
-			jb.dir = dir; jb.out_off = (int)off_dir[dir]; jb.q_base = q_total; jb.blk0 = blocks;
-			jobs.push_back(jb);
-			blk_start.push_back(blocks); q_start.push_back(q_total);
-			blocks += (jb.nq + 127) / 128 * 2; q_total += jb.nq; off_dir[dir] += (size_t)jb.nq;
+			jb.dir = dir; jb.out_off = (int)off_dir[dir]; jb.q_base = w.q_total; jb.blk0 = w.blocks;
+			w.jobs.push_back(jb);
+			w.blk_start.push_back(w.blocks); w.q_start.push_back(w.q_total);
+			w.blocks += (jb.nq + 127) / 128 * 2; w.q_total += jb.nq; off_dir[dir] += (size_t)jb.nq;
 		}
 	}
-	BT_REQUIRE((size_t)g_off <= m->g_halves_cap && q_total <= m->max_q_total && blocks <= m->max_blocks && units < (1ll << 31), BT_ERR_CAPACITY, "bt_knn_match_pairs: work list overflow");
-	{ KnnPair guard; memset(&guard, 0, sizeof guard); guard.unit0 = (int)units; guard.n_qt = guard.n_tt = 1; pairs.push_back(guard); }   // UnitWalk::next() may read one entry past the last pair
-	const int n_live = (int)pairs.size() - 1;
-	// ---- upload tables (one pinned block; the caller holds the event guard)
-	const size_t b_pairs = sizeof(KnnPair) * pairs.size(), b_jobs = sizeof(SelJob) * jobs.size(), b_int = sizeof(int) * jobs.size();
-	char* h0 = hb + hoff;
-	memcpy(h0, pairs.data(), b_pairs);
-	memcpy(h0 + b_pairs, jobs.data(), b_jobs);
-	memcpy(h0 + b_pairs + b_jobs, blk_start.data(), b_int);
-	memcpy(h0 + b_pairs + b_jobs + b_int, q_start.data(), b_int);
-	BT_CUDA(cudaMemcpyAsync(m->pairs.p, h0, b_pairs, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaMemcpyAsync(m->jobs.p, h0 + b_pairs, b_jobs, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaMemcpyAsync(m->blk_start.p, h0 + b_pairs + b_jobs, b_int, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaMemcpyAsync(m->q_start.p, h0 + b_pairs + b_jobs + b_int, b_int, cudaMemcpyHostToDevice, stream));
-	BT_TRY(m->h_stage.in_flight(stream));
+	BT_REQUIRE((size_t)w.g_off <= m->g_halves_cap && w.q_total <= m->max_q_total && w.blocks <= m->max_blocks && w.units < (1ll << 31), BT_ERR_CAPACITY, "%s: work list overflow", who);
+	KnnPair guard; memset(&guard, 0, sizeof guard); guard.unit0 = (int)w.units; guard.n_qt = guard.n_tt = 1; w.pairs.push_back(guard);
+	return BT_OK;
+}
+
+// one copy of the plan's tables from the pinned block `hb` (the caller holds its event guard) to the device
+static int upload_plan(MatcherState* m, const KnnPlan& w, char* hb, cudaStream_t stream, KnnTables* dev) {
+	size_t off = 0;
+	auto put = [&](const auto& v) {      // appends table v; its place on the device
+		const size_t b = sizeof(v[0]) * v.size();
+		memcpy(hb + off, v.data(), b);
+		off += b;
+		return reinterpret_cast<decltype(v.data())>(m->tables.as<char>() + off - b);
+	};
+	*dev = KnnTables{ put(w.pairs), put(w.jobs), put(w.blk_start), put(w.q_start) };      // (a braced list is evaluated in order)
+	BT_CUDA(cudaMemcpyAsync(m->tables.p, hb, off, cudaMemcpyHostToDevice, stream));
+	return m->h_stage.in_flight(stream);
+}
+
+// The checks every matching entry point makes (A and B are its two input lists), then the device, the staging block and the first mark.
+static int begin_match(bt_ctx* ctx, const char* who, int n_pairs, const void* A, const void* B, int k, const KnnOut& out, cudaStream_t stream, char** hb) {
+	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready, BT_ERR_INVALID_ARG, "%s: call bt_matcher_reserve first", who);
+	BT_REQUIRE(A && B && out.idx[0] && out.dist[0] && out.idx[1] && out.dist[1], BT_ERR_INVALID_ARG, "%s: NULL argument", who);
+	BT_REQUIRE(k >= 1 && k <= 8, BT_ERR_UNSUPPORTED, "%s: k=%d outside [1,8]", who, k);
+	MatcherState* m = ctx->matcher.get();
+	BT_REQUIRE(n_pairs > 0 && n_pairs <= m->max_pairs, BT_ERR_CAPACITY, "%s: %d pairs > reserved %d", who, n_pairs, m->max_pairs);
+	BT_CUDA(cudaSetDevice(ctx->device));
+	BT_TRY(m->h_stage.acquire(0, hb));
+	return mark(m, 0, stream);
+}
+
+// the matcher proper on descriptor sets that are already in the pool; hb: the free part of the staging block
+static int knn_run(bt_ctx* ctx, const char* who, int n_pairs, const PoolSetRef* A, const PoolSetRef* B, int k, const KnnOut& out, char* hb,
+                   cudaStream_t stream) {
+	MatcherState* m = ctx->matcher.get();
+	KnnPlan w;
+	BT_TRY(plan_work(m, who, n_pairs, A, B, w));
+	KnnTables t;
+	BT_TRY(upload_plan(m, w, hb, stream, &t));
+	const int n_live = (int)w.pairs.size() - 1, n_jobs = (int)w.jobs.size();
 	BT_CUDA(cudaMemsetAsync(m->fb_count.p, 0, 16, stream));
-	if (n_live > 0) k_knn_pairconst<<<(n_live + 127) / 128, 128, 0, stream>>>(m->pairs.as<KnnPair>(), n_live, m->slot_meta.as<int>(), m->pconst.as<PairConst>());
-	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[1], stream));      // [ev0, ev1) = descriptor conversion + table upload + per-pair constants; [ev1, ev2) = k_knn_tc alone
-	// ---- kernels
+	if (n_live > 0) k_knn_pairconst<<<(n_live + 127) / 128, 128, 0, stream>>>(t.pairs, n_live, m->slot_meta.as<int>(), m->pconst.as<PairConst>());
+	BT_TRY(mark(m, 1, stream));
 	if (n_live > 0) {
-		const int grid = (int)std::min<long long>(units, ctx->sm_count);
-		k_knn_tc<<<grid, KNN_THREADS, SMEM_TOTAL, stream>>>(m->tmap_a, m->tmap_b, m->pairs.as<KnnPair>(), n_live, (int)units, m->norms.as<float>(), m->pconst.as<PairConst>(), m->G.as<__half>());
+		const int grid = (int)std::min<long long>(w.units, ctx->sm_count);
+		k_knn_tc<<<grid, KNN_THREADS, SMEM_TOTAL, stream>>>(m->tmap_a, m->tmap_b, t.pairs, n_live, (int)w.units, m->norms.as<float>(), m->pconst.as<PairConst>(), m->G.as<__half>());
 	}
-	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[2], stream));
-	KnnOut out; out.idx[0] = idxAB; out.idx[1] = idxBA; out.dist[0] = distAB; out.dist[1] = distBA;
-	if (q_total > 0) {
-		if (k <= 5) k_knn_select<5><<<blocks, 256, 0, stream>>>(m->jobs.as<SelJob>(), m->blk_start.as<int>(), (int)jobs.size(), m->G.as<__half>(), m->errn.as<float>(), m->pconst.as<PairConst>(), k, m->cand.as<int32_t>(), m->cand_cnt.as<int32_t>(), m->qjob.as<int>());
-		else k_knn_select<8><<<blocks, 256, 0, stream>>>(m->jobs.as<SelJob>(), m->blk_start.as<int>(), (int)jobs.size(), m->G.as<__half>(), m->errn.as<float>(), m->pconst.as<PairConst>(), k, m->cand.as<int32_t>(), m->cand_cnt.as<int32_t>(), m->qjob.as<int>());
-		k_knn_rerank<<<(q_total + 7) / 8, 256, 0, stream>>>(m->jobs.as<SelJob>(), m->qjob.as<int>(), q_total, m->cand.as<int32_t>(), m->cand_cnt.as<int32_t>(), m->pool_f.as<float>(),
-		                                                 k, out, m->fb_rows.as<int>(), m->fb_count.as<int>(), m->force_fallback);
-		if (m->timing) BT_CUDA(cudaEventRecord(m->ev[3], stream));
-		k_knn_exact<<<ctx->sm_count * 2, 256, 0, stream>>>(m->jobs.as<SelJob>(), m->q_start.as<int>(), (int)jobs.size(), m->pool_f.as<float>(), m->fb_rows.as<int>(), m->fb_count.as<int>(), k, out,
+	BT_TRY(mark(m, 2, stream));
+	if (w.q_total > 0) {
+		auto* sel = k <= 5 ? k_knn_select<5> : k_knn_select<8>;
+		sel<<<w.blocks, 256, 0, stream>>>(t.jobs, t.blk_start, n_jobs, m->G.as<__half>(), m->errn.as<float>(), m->pconst.as<PairConst>(), k, m->cand.as<int32_t>(), m->cand_cnt.as<int32_t>(), m->qjob.as<int>());
+		k_knn_rerank<<<(w.q_total + 7) / 8, 256, 0, stream>>>(t.jobs, m->qjob.as<int>(), w.q_total, m->cand.as<int32_t>(), m->cand_cnt.as<int32_t>(), m->pool_f.as<float>(),
+		                                                   k, out, m->fb_rows.as<int>(), m->fb_count.as<int>(), m->force_fallback);
+		BT_TRY(mark(m, 3, stream));
+		k_knn_exact<<<ctx->sm_count * 2, 256, 0, stream>>>(t.jobs, t.q_start, n_jobs, m->pool_f.as<float>(), m->fb_rows.as<int>(), m->fb_count.as<int>(), k, out,
 		                                              m->fb_part_d.as<double>(), m->fb_part_i.as<int>(), m->fb_tickets.as<int>());
-	} else if (m->timing) BT_CUDA(cudaEventRecord(m->ev[3], stream));
-	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[4], stream));
+	} else BT_TRY(mark(m, 3, stream));
+	BT_TRY(mark(m, 4, stream));
 	BT_CUDA(cudaGetLastError());
-	m->last_units = (int)units; m->last_rows = q_total;
+	m->last_units = (int)w.units; m->last_rows = w.q_total;
 	return BT_OK;
 }
 
@@ -909,15 +958,13 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 	BT_TRY(pool_alloc(m));
 	const int pad_a = (max_feats + BM - 1) / BM * BM;      // A sets are padded to whole 128-row tiles
 	m->g_halves_cap = (size_t)max_pairs * ((size_t)(slot_rows / GRP) * pad_a + (size_t)(pad_a / GRP) * slot_rows);
-	m->max_jobs = 2 * max_pairs;
 	m->max_q_total = 2 * max_pairs * max_feats;
 	m->max_blocks = 2 * max_pairs * ((max_feats + 127) / 128 * 2);      // k_knn_select covers whole 128-position blocks, 64 queries per CTA
 	BT_TRY(m->sets.alloc(sizeof(PrepSet) * (size_t)std::max(m->n_transient, 1)));
-	BT_TRY(m->pairs.alloc(sizeof(KnnPair) * ((size_t)max_pairs + 1)));
+	const size_t b_tables = sizeof(KnnPair) * ((size_t)max_pairs + 1) + (sizeof(SelJob) + 2 * sizeof(int)) * 2 * max_pairs;     // a KnnPlan's
+	BT_TRY(m->tables.alloc(b_tables));
 	BT_TRY(m->pconst.alloc(sizeof(PairConst) * (size_t)max_pairs));
 	BT_TRY(m->G.alloc(m->g_halves_cap * 2 + 64));
-	BT_TRY(m->jobs.alloc(sizeof(SelJob) * m->max_jobs));
-	BT_TRY(m->blk_start.alloc(sizeof(int) * m->max_jobs)); BT_TRY(m->q_start.alloc(sizeof(int) * m->max_jobs));
 	BT_TRY(m->cand.alloc(sizeof(int32_t) * SEL_MAXC * (size_t)m->max_q_total));
 	BT_TRY(m->cand_cnt.alloc(sizeof(int32_t) * (size_t)m->max_q_total));
 	BT_TRY(m->qjob.alloc(sizeof(int) * (size_t)m->max_q_total));
@@ -926,7 +973,7 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 	BT_TRY(m->fb_part_d.alloc(sizeof(double) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8)); BT_TRY(m->fb_part_i.alloc(sizeof(int) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8));
 	BT_TRY(m->fb_tickets.alloc(sizeof(int) * (size_t)FB_SPLIT_ROWS));
 	BT_CUDA(cudaMemset(m->fb_tickets.p, 0, sizeof(int) * (size_t)FB_SPLIT_ROWS));
-	BT_TRY(m->h_stage.reserve(sizeof(PrepSet) * 2 * max_pairs + sizeof(KnnPair) * ((size_t)max_pairs + 1) + (sizeof(SelJob) + 2 * sizeof(int)) * m->max_jobs + 4096));
+	BT_TRY(m->h_stage.reserve(sizeof(PrepSet) * 2 * max_pairs + b_tables + 4096));
 	BT_CUDA(cudaFuncSetAttribute(k_knn_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_TOTAL));
 	return BT_OK;
 }
@@ -949,18 +996,12 @@ extern "C" int bt_desc_pool_store(bt_ctx* ctx, int slot, const bt_desc_view* des
 	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready && desc, BT_ERR_INVALID_ARG, "bt_desc_pool_store: call bt_matcher_reserve / bt_desc_pool_reserve first");
 	MatcherState* m = ctx->matcher.get();
 	BT_REQUIRE(slot >= 0 && slot < m->n_persist, BT_ERR_INVALID_ARG, "bt_desc_pool_store: slot %d outside [0,%d)", slot, m->n_persist);
-	BT_REQUIRE(desc->dim == KD, BT_ERR_UNSUPPORTED, "bt_desc_pool_store: descriptor dim %d != %d", desc->dim, KD);
-	BT_REQUIRE(desc->n >= 0 && desc->n <= m->max_feats, BT_ERR_CAPACITY, "bt_desc_pool_store: %d features > reserved %d", desc->n, m->max_feats);
-	BT_REQUIRE(desc->n == 0 || desc->dev, BT_ERR_INVALID_ARG, "bt_desc_pool_store: NULL descriptor pointer");
-	BT_REQUIRE(((uintptr_t)desc->dev & 15) == 0 && ((desc->pitch_bytes ? desc->pitch_bytes : (size_t)KD * 4) & 15) == 0, BT_ERR_INVALID_ARG, "bt_desc_pool_store: descriptors must be 16-byte aligned");
+	BT_TRY(check_desc(*desc, m, __func__, -1));
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
 	char* hb;
 	BT_TRY(m->h_stage.acquire(0, &hb));
-	PrepSet s; s.src = desc->dev; s.pitch_bytes = desc->pitch_bytes ? desc->pitch_bytes : (size_t)KD * 4; s.n = desc->n;
-	s.slot = m->n_transient + slot; s.row0 = s.slot * m->slot_rows; s.rows_padded = (std::max(desc->n, 1) + BN - 1) / BN * BN;
-	size_t hoff = 0;
-	BT_TRY(launch_prep(ctx, std::vector<PrepSet>(1, s), hb, hoff, stream));
+	BT_TRY(launch_prep(m, { prep_set(m, *desc, m->n_transient + slot) }, hb, stream));
 	BT_TRY(m->h_stage.in_flight(stream));
 	BT_CUDA(cudaGetLastError());
 	m->slot_n[slot] = desc->n;
@@ -969,12 +1010,11 @@ extern "C" int bt_desc_pool_store(bt_ctx* ctx, int slot, const bt_desc_view* des
 
 extern "C" int bt_knn_match_slots(bt_ctx* ctx, int n_pairs, const int32_t* slotA, const int32_t* slotB, int k,
                                   int32_t* idxAB, float* distAB, int32_t* idxBA, float* distBA, void* stream_) {
-	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready, BT_ERR_INVALID_ARG, "bt_knn_match_slots: call bt_matcher_reserve first");
-	BT_REQUIRE(slotA && slotB && idxAB && distAB && idxBA && distBA, BT_ERR_INVALID_ARG, "bt_knn_match_slots: NULL argument");
-	BT_REQUIRE(k >= 1 && k <= 8, BT_ERR_UNSUPPORTED, "bt_knn_match_slots: k=%d outside [1,8]", k);
+	const KnnOut out{ { idxAB, idxBA }, { distAB, distBA } };
+	cudaStream_t stream = (cudaStream_t)stream_;
+	char* hb;
+	BT_TRY(begin_match(ctx, __func__, n_pairs, slotA, slotB, k, out, stream, &hb));
 	MatcherState* m = ctx->matcher.get();
-	BT_CUDA(cudaSetDevice(ctx->device));
-	BT_REQUIRE(n_pairs > 0 && n_pairs <= m->max_pairs, BT_ERR_CAPACITY, "bt_knn_match_slots: %d pairs > reserved %d", n_pairs, m->max_pairs);
 	std::vector<PoolSetRef> A(n_pairs), B(n_pairs);
 	for (int p = 0; p < n_pairs; p++) {
 		for (int s2 = 0; s2 < 2; s2++) {
@@ -983,11 +1023,7 @@ extern "C" int bt_knn_match_slots(bt_ctx* ctx, int n_pairs, const int32_t* slotA
 			(s2 == 0 ? A[p] : B[p]) = PoolSetRef{ m->n_transient + sl, m->slot_n[sl] };
 		}
 	}
-	char* hb;
-	BT_TRY(m->h_stage.acquire(0, &hb));
-	cudaStream_t stream = (cudaStream_t)stream_;
-	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[0], stream));
-	return knn_run(ctx, n_pairs, A.data(), B.data(), k, idxAB, distAB, idxBA, distBA, hb, 0, stream);
+	return knn_run(ctx, __func__, n_pairs, A.data(), B.data(), k, out, hb, stream);
 }
 
 extern "C" int bt_knn_debug_force_fallback(bt_ctx* ctx, int every_nth) {
@@ -1017,41 +1053,26 @@ extern "C" int bt_knn_get_timing(bt_ctx* ctx, float* ms4, int* info3) {
 
 extern "C" int bt_knn_match_pairs(bt_ctx* ctx, int n_pairs, const bt_desc_view* A, const bt_desc_view* B, int k,
                                   int32_t* idxAB, float* distAB, int32_t* idxBA, float* distBA, void* stream_) {
-	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready, BT_ERR_INVALID_ARG, "bt_knn_match_pairs: call bt_matcher_reserve first");
-	BT_REQUIRE(A && B && idxAB && distAB && idxBA && distBA, BT_ERR_INVALID_ARG, "bt_knn_match_pairs: NULL argument");
-	BT_REQUIRE(k >= 1 && k <= 8, BT_ERR_UNSUPPORTED, "bt_knn_match_pairs: k=%d outside [1,8]", k);
-	MatcherState* m = ctx->matcher.get();
+	const KnnOut out{ { idxAB, idxBA }, { distAB, distBA } };
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
-	BT_REQUIRE(n_pairs > 0 && n_pairs <= m->max_pairs, BT_ERR_CAPACITY, "bt_knn_match_pairs: %d pairs > reserved %d", n_pairs, m->max_pairs);
-	for (int p = 0; p < n_pairs; p++) {
-		for (const bt_desc_view* v : { &A[p], &B[p] }) {
-			BT_REQUIRE(v->dim == KD, BT_ERR_UNSUPPORTED, "pair %d: descriptor dim %d != %d", p, v->dim, KD);
-			BT_REQUIRE(v->n >= 0 && v->n <= m->max_feats, BT_ERR_CAPACITY, "pair %d: %d features > reserved %d", p, v->n, m->max_feats);
-			BT_REQUIRE(v->n == 0 || v->dev, BT_ERR_INVALID_ARG, "pair %d: NULL descriptor pointer", p);
-			BT_REQUIRE(((uintptr_t)v->dev & 15) == 0 && ((v->pitch_bytes ? v->pitch_bytes : (size_t)KD * 4) & 15) == 0, BT_ERR_INVALID_ARG, "pair %d: descriptors must be 16-byte aligned", p);
-		}
-	}
+	char* hb;
+	BT_TRY(begin_match(ctx, __func__, n_pairs, A, B, k, out, stream, &hb));
+	MatcherState* m = ctx->matcher.get();
 	// ---- unique descriptor sets (a keyframe appears in many pairs) -> transient pool slots, converted once per call
 	std::map<std::pair<const float*, int>, int> slot_of;
 	std::vector<PrepSet> sets;
 	auto slot = [&](const bt_desc_view& v) -> int {
-		const auto key = std::make_pair(v.dev, v.n);
-		auto it = slot_of.find(key);
-		if (it != slot_of.end()) return it->second;
-		PrepSet s; s.src = v.dev; s.pitch_bytes = v.pitch_bytes ? v.pitch_bytes : (size_t)v.dim * 4; s.n = v.n; s.slot = (int)sets.size();
-		s.row0 = s.slot * m->slot_rows; s.rows_padded = (std::max(v.n, 1) + BN - 1) / BN * BN;
-		sets.push_back(s);
-		slot_of[key] = s.slot;
-		return s.slot;
+		const auto it = slot_of.emplace(std::make_pair(v.dev, v.n), (int)sets.size());
+		if (it.second) sets.push_back(prep_set(m, v, it.first->second));
+		return it.first->second;
 	};
 	std::vector<PoolSetRef> sa(n_pairs), sb(n_pairs);
-	for (int p = 0; p < n_pairs; p++) { sa[p] = PoolSetRef{ slot(A[p]), A[p].n }; sb[p] = PoolSetRef{ slot(B[p]), B[p].n }; }
+	for (int p = 0; p < n_pairs; p++) {
+		BT_TRY(check_desc(A[p], m, __func__, p));
+		BT_TRY(check_desc(B[p], m, __func__, p));
+		sa[p] = PoolSetRef{ slot(A[p]), A[p].n }; sb[p] = PoolSetRef{ slot(B[p]), B[p].n };
+	}
 	BT_REQUIRE((int)sets.size() <= m->n_transient, BT_ERR_CAPACITY, "bt_knn_match_pairs: %d distinct descriptor sets in one call > %d (store them with bt_desc_pool_store and use bt_knn_match_slots)", (int)sets.size(), m->n_transient);
-	char* hb;
-	BT_TRY(m->h_stage.acquire(0, &hb));
-	if (m->timing) BT_CUDA(cudaEventRecord(m->ev[0], stream));
-	size_t hoff = 0;
-	BT_TRY(launch_prep(ctx, sets, hb, hoff, stream));
-	return knn_run(ctx, n_pairs, sa.data(), sb.data(), k, idxAB, distAB, idxBA, distBA, hb, hoff, stream);
+	BT_TRY(launch_prep(m, sets, hb, stream));
+	return knn_run(ctx, __func__, n_pairs, sa.data(), sb.data(), k, out, hb, stream);
 }

@@ -238,13 +238,7 @@ int ransac_run_device(bt_ctx* ctx, const RansacPair* d_pairs, int n_pairs, int n
 		r->table_seed = seed; r->table_trials = r->max_trials;
 	}
 	BT_CUDA(cudaMemsetAsync(r->best.p, 0, sizeof(unsigned long long) * n_pairs, stream));
-	// largest float d2 with sqrtf(d2) <= dist_thresh (both correctly rounded, host and device): lets the kernel compare squares
-	float d2_max = -1.0f;
-	if (dist_thresh >= 0.f) {
-		d2_max = dist_thresh * dist_thresh;
-		while (d2_max > 0.f && sqrtf(d2_max) > dist_thresh) d2_max = nextafterf(d2_max, 0.f);
-		while (sqrtf(nextafterf(d2_max, INFINITY)) <= dist_thresh) d2_max = nextafterf(d2_max, INFINITY);
-	}
+	const float d2_max = sqrt_le_max(dist_thresh);      // (sqrtf is correctly rounded on the device too: the kernel compares squares)
 	const dim3 grid((n_trials + 255) / 256, n_pairs);
 	k_ransac_model<<<grid, 256, 0, stream>>>(d_pairs, n_trials, r->table.as<float>(), r->poses.as<float>(), r->good.as<int>());
 	k_ransac_eval<<<grid, 256, 0, stream>>>(d_pairs, n_trials, r->poses.as<float>(), r->good.as<int>(), d2_max, r->best.as<unsigned long long>());

@@ -1760,16 +1760,6 @@ static FrameGeom frame_geom(int H, int W, float fx, float fy, float cx, float cy
 static int launch_prep(bt_ctx* ctx, cudaStream_t stream);
 static double us_since(std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count(); }
 
-// Largest float d2max with `sqrtf(d2) <= dist_t` <=> `d2 <= d2max` for every float d2 (sqrtf is correctly rounded and monotonic)
-static float dense_d2max(float th) {
-	if (!(th > 0.f)) return (th == 0.f) ? 0.f : -1.f;
-	auto nextf = [](float v, int d) { int32_t b; memcpy(&b, &v, 4); b += d; float r; memcpy(&r, &b, 4); return r; };
-	float d2max = th * th;
-	while (d2max > 0.f && sqrtf(d2max) > th) d2max = nextf(d2max, -1);
-	while (sqrtf(nextf(d2max, 1)) <= th) d2max = nextf(d2max, 1);
-	return d2max;
-}
-
 // Every window against what was reserved; F / C = frames / correspondences of the batch.
 static int validate_windows(const SolverState* s, int n_windows, const bt_window* windows, const bt_solver_params* params, size_t* F, size_t* C) {
 	*F = 0; *C = 0;
@@ -2028,7 +2018,7 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 	BT_REQUIRE(L.total <= s->stage_buf[0].bytes, BT_ERR_CAPACITY, "bt_solve_stage: staging block %zu > reserved %zu bytes", L.total, s->stage_buf[0].bytes);
 	char* hb; BT_TRY(s->h_stage.acquire(L.total, &hb));
 	BT_TRY(fill_frame_tables(s, n_windows, windows, params, poses_in, hb, L, &n_pairs));
-	s->n_windows = n_windows; s->frames_total = (int)F; s->prm = *params; s->d2max = dense_d2max(params->dense_dist_thresh); s->layout = L;
+	s->n_windows = n_windows; s->frames_total = (int)F; s->prm = *params; s->d2max = sqrt_le_max(params->dense_dist_thresh); s->layout = L;
 	{   // chunk: aim for >= 4 tiles per SM-resident CTA over the batch, between 256 and 2048 source pixels
 		const long long est_px = (long long)n_pairs * (s->npix_max / 8);   // ~12 % valid
 		long long c = est_px / ((long long)ctx->sm_count * 2 * 4);

@@ -140,6 +140,39 @@ def test_knn_matches_opencv(matcher, cuda_device):
     assert np.abs(dAB[0].cpu().numpy() - dc).max() < 1e-5
 
 
+@pytest.mark.parametrize("bad,code", [("dim", -5), ("n", -2), ("null", -1), ("offset", -1), ("pitch", -1)])
+def test_desc_view_refused_alike_by_store_and_match(matcher, cuda_device, bad, code):
+    """A descriptor set the matcher cannot take is refused with the same status by bt_desc_pool_store and bt_knn_match_pairs: dim 128,
+    more rows than reserved, a NULL pointer, a pointer off 16-byte alignment, a row pitch of 1028 bytes."""
+    import ctypes
+    import torch
+    from bundletrack_b200 import _lib
+    buf = torch.zeros((64, 320), device=cuda_device)
+    good = _lib.desc_view(buf[:, :256])                              # pitch 1280 B
+    v = _lib.DescView(good.dev, good.n, good.dim, good.pitch_bytes)
+    if bad == "dim":
+        v.dim = 128
+    elif bad == "n":
+        v.n = 5121                                                  # the fixture reserved 5120
+    elif bad == "null":
+        v.dev = None
+    elif bad == "offset":
+        v.dev = good.dev + 4
+    else:
+        v.pitch_bytes = 1028
+    lib = matcher.lib
+    matcher.pool_reserve(6)
+    assert lib.bt_desc_pool_store(matcher.ctx, 0, ctypes.byref(good), matcher.stream) == 0
+    assert lib.bt_desc_pool_store(matcher.ctx, 0, ctypes.byref(v), matcher.stream) == code
+    assert lib.bt_last_error().decode().startswith("bt_desc_pool_store: ")
+    out = [torch.empty((128, 5), dtype=t, device=cuda_device) for t in (torch.int32, torch.float32, torch.int32, torch.float32)]
+    A, B = (_lib.DescView * 2)(good, good), (_lib.DescView * 2)(good, v)      # the bad view is pair 1's B
+    assert lib.bt_knn_match_pairs(matcher.ctx, 2, A, B, 5, *(_lib.ptr(t) for t in out), matcher.stream) == code
+    assert lib.bt_last_error().decode().startswith("pair 1: ")
+    iAB, _, _, _ = matcher.knn_match_pairs([(buf[:, :256], buf[:, :256])])      # the matcher still works
+    assert iAB[0].shape == (64, 5)
+
+
 # ------------------------------------------------------------------------------------------------------------ RANSAC
 def _ransac_case(seed, n, inlier_frac=0.7, noise=0.0005, big=False):
     return synth.make_ransac_case(seed, n, inlier_frac, noise)
@@ -218,6 +251,20 @@ def test_ransac_edge_cases(cuda_device):
     A4, B4, _ = _ransac_case(2, 30, inlier_frac=0.0)   # all outliers: at most the 3 sampled points agree
     ids = r.ransac_pairs([torch.from_numpy(A4).to(cuda_device)], [torch.from_numpy(B4).to(cuda_device)], 500, 0.0005)
     assert len(ids[0]) <= 6
+    r.close()
+
+
+def test_ransac_infinite_threshold(cuda_device):
+    """dist_thresh = +inf: the squared threshold is +inf, so every point is an inlier of a pair that has a model; a pair of two points
+    still has none."""
+    from bundletrack_b200.matcher import Ransac
+    import torch
+    r = Ransac(max_pairs=2, max_pts=64, max_trials=500)
+    A4, B4, _ = _ransac_case(3, 50, inlier_frac=0.5)
+    A2, B2, _ = _ransac_case(4, 2)
+    t = lambda x: torch.from_numpy(x).to(cuda_device)
+    ids = r.ransac_pairs([t(A4), t(A2)], [t(B4), t(B2)], 500, float("inf"))
+    assert np.array_equal(ids[0].cpu().numpy(), np.arange(50)) and len(ids[1]) == 0
     r.close()
 
 
