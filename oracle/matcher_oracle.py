@@ -17,8 +17,26 @@ from __future__ import annotations
 import numpy as np
 
 
+def _d2_direct(qrow: np.ndarray, t: np.ndarray) -> np.ndarray:
+    """float64 sum of (q - t)^2 over the last axis: the distance both knn() and knn_direct() order by, computed alike."""
+    diff = qrow[None, :] - t
+    return (diff * diff).sum(1)
+
+
+def _top_k(c: np.ndarray, dd: np.ndarray, kk: int, idx_row: np.ndarray, dist_row: np.ndarray):
+    order = np.lexsort((c, dd))[:kk]
+    idx_row[:kk] = c[order]
+    dist_row[:kk] = np.sqrt(dd[order]).astype(np.float32)
+
+
 def knn(query: np.ndarray, train: np.ndarray, k: int = 5, block: int = 512):
-    """Exact kNN.  Returns (idx [nq,k] int32, dist [nq,k] float32); rows with fewer than k candidates pad with -1/inf."""
+    """Exact kNN.  Returns (idx [nq,k] int32, dist [nq,k] float32); rows with fewer than k candidates pad with -1/inf.
+
+    The float64 expansion |q|^2 + |t|^2 - 2 q.t only preselects: it cancels when descriptors share a large offset (|q|, |t| >> |q - t|).
+    Whatever the summation order, its error is below (dim + 2) 2^-53 (|q| + |t|)^2 (norms and dot product each to dim 2^-53 of their
+    magnitude, plus the two additions); `margin` is four times that for the row's largest train norm.  The k rows of smallest expanded d2
+    have exact d2 <= kth + margin, so every row whose exact d2 is at most that has expanded d2 <= kth + 2 margin: those rows are
+    recomputed by direct differences and ordered by (d2, index), as knn_direct() orders all of them."""
     q = np.asarray(query, np.float32)
     t = np.asarray(train, np.float32).astype(np.float64)
     nq, nt = q.shape[0], t.shape[0]
@@ -27,20 +45,31 @@ def knn(query: np.ndarray, train: np.ndarray, k: int = 5, block: int = 512):
     if nq == 0 or nt == 0:
         return idx, dist
     tn = (t * t).sum(1)
+    tmax = np.sqrt(tn.max())
     kk = min(k, nt)
     for s in range(0, nq, block):
         qb = q[s:s + block].astype(np.float64)
-        d2 = (qb * qb).sum(1)[:, None] + tn[None, :] - 2.0 * (qb @ t.T)
-        # exact differences for the short list (the expansion above loses ~1e-16 relative: irrelevant for ordering
-        # except exact ties, which the recomputation below settles identically for both orders)
-        cand = np.argpartition(d2, min(kk + 8, nt - 1), axis=1)[:, : min(kk + 9, nt)]
+        qn = (qb * qb).sum(1)
+        d2 = qn[:, None] + tn[None, :] - 2.0 * (qb @ t.T)
+        kth = np.partition(d2, kk - 1, axis=1)[:, kk - 1]
+        margin = 4.0 * 2.0 ** -53 * (q.shape[1] + 2) * (np.sqrt(qn) + tmax) ** 2
+        keep = d2 <= (kth + 2.0 * margin)[:, None]
         for r in range(qb.shape[0]):
-            c = np.sort(cand[r])
-            diff = qb[r][None, :] - t[c]
-            dd = (diff * diff).sum(1)
-            order = np.lexsort((c, dd))[:kk]
-            idx[s + r, :kk] = c[order]
-            dist[s + r, :kk] = np.sqrt(dd[order]).astype(np.float32)
+            c = np.nonzero(keep[r])[0]
+            _top_k(c, _d2_direct(qb[r], t[c]), kk, idx[s + r], dist[s + r])
+    return idx, dist
+
+
+def knn_direct(query: np.ndarray, train: np.ndarray, k: int = 5):
+    """Plain brute force: direct-difference float64 d2 to every train row, top k by (d2, index).  Slow; the check on knn()."""
+    q = np.asarray(query, np.float32).astype(np.float64)
+    t = np.asarray(train, np.float32).astype(np.float64)
+    nq, nt = q.shape[0], t.shape[0]
+    idx = np.full((nq, k), -1, np.int32)
+    dist = np.full((nq, k), np.inf, np.float32)
+    all_rows = np.arange(nt)
+    for r in range(nq if nt else 0):
+        _top_k(all_rows, _d2_direct(q[r], t), min(k, nt), idx[r], dist[r])
     return idx, dist
 
 

@@ -5,6 +5,7 @@ import pytest
 
 from bundletrack_b200 import synth
 from oracle import matcher_oracle as mo
+from oracle.knn_families import PLACEMENTS, cluster_case
 
 
 def test_knn_matches_opencv_bfmatcher():
@@ -33,6 +34,43 @@ def test_knn_ties_go_to_lower_index_and_padding():
     assert e_i.shape == (0, 5)
     z_i, z_d = mo.knn(a, b[:0])
     assert (z_i == -1).all() and np.isinf(z_d).all()
+
+
+@pytest.mark.parametrize("C", [1.0, 1e2, 1e3, 1e4])
+def test_knn_equals_direct_brute_force_under_common_offset(C):
+    """Descriptors sharing a large offset, C c + N(0, 1e-3) with c ~ N(0, 1): the expansion |q|^2 + |t|^2 - 2 q.t cancels, so knn() may only use it to
+    preselect (at C = 1e4 a fixed short list taken from it picks the wrong rows for most queries)."""
+    rng = np.random.default_rng(int(C))
+    c = rng.normal(size=256)
+    a = (C * c + rng.normal(0, 1e-3, (300, 256))).astype(np.float32)
+    b = (C * c + rng.normal(0, 1e-3, (400, 256))).astype(np.float32)
+    for q, t in ((a, b), (b, a)):
+        i1, d1 = mo.knn(q, t, 5)
+        i2, d2 = mo.knn_direct(q, t, 5)
+        assert np.array_equal(i1, i2)
+        assert np.array_equal(d1, d2)
+
+
+@pytest.mark.parametrize("family,placement", [("tie", "g17"), ("tie", "one_group"), ("near", "spread12"), ("near", "g5")])
+def test_knn_equals_direct_brute_force_on_ties_and_near_ties(family, placement):
+    """The adversarial families of the GPU tests (exact ties, near-ties 2^-20 apart in reverse index order), k = 1..8."""
+    qs, ts = cluster_case(family, PLACEMENTS[placement], seed=3)
+    for k in (1, 4, 8):
+        for q, t in ((qs, ts), (ts, qs)):
+            i1, d1 = mo.knn(q, t, k)
+            i2, d2 = mo.knn_direct(q, t, k)
+            assert np.array_equal(i1, i2) and np.array_equal(d1, d2)
+    rows = sorted(PLACEMENTS[placement], reverse=not family == "tie")     # near-ties: nearest member at the highest row; ties: lowest first
+    m = min(8, len(rows))
+    assert mo.knn(qs, ts, 8)[0][37, :m].tolist() == rows[:m]
+
+
+def test_knn_direct_pads_and_breaks_ties_by_index():
+    a = np.zeros((2, 256), np.float32)
+    b = np.zeros((3, 256), np.float32); b[:, 0] = [1, 1, 0.5]
+    idx, dist = mo.knn_direct(a, b, 5)
+    assert idx[0].tolist() == [2, 0, 1, -1, -1] and np.isinf(dist[0, 3:]).all()
+    assert (mo.knn_direct(a, b[:0], 3)[0] == -1).all() and mo.knn_direct(a[:0], b, 3)[0].shape == (0, 3)
 
 
 def test_ransac_oracle_against_reference_golden():
