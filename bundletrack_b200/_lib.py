@@ -174,6 +174,13 @@ class LfnetParams(ctypes.Structure):
     ]
 
 
+class VosParams(ctypes.Structure):
+    _fields_ = [
+        ("ref_num", ctypes.c_int), ("range", ctypes.c_int),
+        ("sigma1", ctypes.c_double), ("sigma2", ctypes.c_double), ("temperature", ctypes.c_double),
+    ]
+
+
 # Every entry point of include/bundletrack_b200.h as (restype, argtypes), in the header's order; load() applies it, so a call site passes
 # plain Python values and ctypes converts each to the C type declared here (tests/test_abi.py checks the table against the header).
 # int / int32_t -> c_int, float -> c_float, double -> c_double, long long -> c_longlong, size_t -> c_size_t, uint64_t -> c_uint64, a pointer
@@ -282,6 +289,15 @@ PROTOTYPES = {
     "bt_lfnet_enable_timing": (_i, (_p, _i)),
     "bt_lfnet_get_timing": (_i, (_p, _p)),
     "bt_lfnet_debug_maps": (_i, (_p, _i, _p, _p, _p, _p, _p)),
+    "bt_vos_schedule": (_i, (_i, _i, _i, _p, _p)),
+    "bt_vos_weights_size": (_i, (_p, _p)),
+    "bt_vos_reserve": (_i, (_p, _p, _i, _i)),
+    "bt_vos_load_weights": (_i, (_p, _p, _sz)),
+    "bt_vos_begin": (_i, (_p, _p, _p, _p, _p)),
+    "bt_vos_next": (_i, (_p, _p, _p, _p)),
+    "bt_vos_enable_timing": (_i, (_p, _i)),
+    "bt_vos_get_timing": (_i, (_p, _p)),
+    "bt_vos_debug": (_i, (_p, _i, _p, _p, _p, _p, _p)),
     "bt_dev_alloc": (_i, (_p, _sz)),
     "bt_dev_free": (_i, (_p,)),
     "bt_memcpy_h2d": (_i, (_p, _p, _sz, _p)),

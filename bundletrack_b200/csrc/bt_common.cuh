@@ -153,6 +153,7 @@ struct NocsState;     // metrics.cu
 struct OverlayState;  // overlay.cu
 struct MatchVizState; // matchviz.cu
 struct LfnetState;    // lfnet.cu
+struct VosState;      // vos.cu
 
 // The context owns the module states; each module defines the deleter of its state next to it, so the states stay private to their files.
 struct StateDeleter {
@@ -168,6 +169,7 @@ struct StateDeleter {
 	void operator()(OverlayState*) const;
 	void operator()(MatchVizState*) const;
 	void operator()(LfnetState*) const;
+	void operator()(VosState*) const;
 };
 template <class T> using StatePtr = std::unique_ptr<T, StateDeleter>;
 
@@ -189,6 +191,7 @@ struct bt_ctx {
 	bt::StatePtr<bt::OverlayState> overlay;
 	bt::StatePtr<bt::MatchVizState> matchviz;
 	bt::StatePtr<bt::LfnetState> lfnet;
+	bt::StatePtr<bt::VosState> vos;
 };
 
 namespace bt {

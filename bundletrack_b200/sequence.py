@@ -214,9 +214,11 @@ def read_image(path: str, kind: str, reader: str = None) -> np.ndarray:
     return np.ascontiguousarray(a)
 
 
-def read_frame(ff: FrameFiles, reader: str = None):
-    """(depth uint16 [H,W], mask uint8 [H,W], colour uint8 [H,W,3] BGR) of one frame; the three must have one size."""
-    d, m, c = read_image(ff.depth, "depth", reader), read_image(ff.mask, "mask", reader), read_image(ff.colour, "colour", reader)
+def read_frame(ff: FrameFiles, reader: str = None, with_mask: bool = True):
+    """(depth uint16 [H,W], mask uint8 [H,W], colour uint8 [H,W,3] BGR) of one frame; the three must have one size.  with_mask=False
+    leaves the mask file unread and gives zeros in its place (the masks come from elsewhere)."""
+    d, c = read_image(ff.depth, "depth", reader), read_image(ff.colour, "colour", reader)
+    m = read_image(ff.mask, "mask", reader) if with_mask else np.zeros(d.shape, np.uint8)
     if d.shape != m.shape or d.shape != c.shape[:2]:
         raise ValueError(f"frame {ff.id_str}: depth {d.shape}, mask {m.shape} and colour {c.shape[:2]} differ in size")
     return d, m, c
@@ -229,11 +231,13 @@ class FrameReader:
     (uint16 depth, mask, BGR colour) and uploads each on a copy stream; get(i) makes `stream` wait for frame i's upload and returns its
     device tensors.  release(i) records an event on `stream` behind the work that reads frame i; the copy stream waits for that event before
     it rewrites the slot, so work enqueued before release (bt_lfnet_request reads the colour after begin_frame's ROI synchronisation) is
-    covered.  prefetch=0 decodes and uploads in get(), in the calling thread."""
+    covered.  prefetch=0 decodes and uploads in get(), in the calling thread.  with_mask=False reads no mask files (get's mask is then
+    left as it was: the caller supplies the masks)."""
 
-    def __init__(self, loader, H: int, W: int, device: int, stream, prefetch: int = 2):
+    def __init__(self, loader, H: int, W: int, device: int, stream, prefetch: int = 2, with_mask: bool = True):
         import torch
         self.torch, self.loader, self.stream, self.prefetch = torch, loader, stream, int(prefetch)
+        self.with_mask = with_mask
         self.dev = torch.device("cuda", device)
         self.copy = torch.cuda.Stream(self.dev)
         R = self.prefetch + 1
@@ -257,7 +261,7 @@ class FrameReader:
         torch = self.torch
         s = i % self.R
         t0 = time.perf_counter()
-        arrays = read_frame(self.loader.frames[i])
+        arrays = read_frame(self.loader.frames[i], with_mask=self.with_mask)
         self.decode_s[i] = time.perf_counter() - t0
         self.uploaded[s].synchronize()                  # the slot's previous upload has read the pinned buffers
         for h, a in zip(self.host[s], arrays):
@@ -419,7 +423,7 @@ class LogWriter:
 # ---- the run --------------------------------------------------------------------------------------------------------------------------------
 
 def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max_keyframes: int = None, device: int = 0, prefetch: int = 2,
-                 log: int = 0):
+                 log: int = 0, masks=None):
     """Tracks every frame the loader yields (Bundler::processNewFrame) and writes <out_dir>/poses/<id_str>.txt for each one with
     policy.save_pose_txt (Bundler::saveNewframeResult runs after every frame): the initial pose of a frame that fails the ROI gate, the
     pose drop_frame reports when detection fails, otherwise end_frame's.  features(id_str, request uint8 [400,400,3] host, roi) returns
@@ -429,7 +433,9 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
     neither the request nor the descriptors cross the bus.  Sizing as INTEGRATION.md §7: max_frames_alive = bundle.window_size + 4, max_keyframes defaults to
     min(1024, ceil(n_frames / 2)).  Nothing under out_dir is removed.  Returns [(id_str, status, wall seconds)] per frame.
     log > 0 (the yml's LOG): every frame's LOG images under out_dir (the reference's debug_dir), drawn on the device with the pose its pose
-    file holds (overlay.Overlay over loader.model_path) and written by a LogWriter thread; needs cv2.  log = 0 runs none of it."""
+    file holds (overlay.Overlay over loader.model_path) and written by a LogWriter thread; needs cv2.  log = 0 runs none of it.
+    masks (vos.VosSource): each frame's object mask is propagated on the device from the first frame's, on the tracker's stream, over the
+    frames the loader yields in order; the loader's mask files are not read."""
     import torch
     from .tracker import Tracker
     n = len(loader)
@@ -456,12 +462,14 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
             ovl = Overlay(load_obj_points(loader.model_path), loader.K, H, W, device=device, stream=stream.cuda_stream)
             with torch.cuda.device(dev):
                 viz, raw = (torch.empty((H, W, 3), dtype=torch.uint8, device=dev) for _ in range(2))
-        reader = FrameReader(loader, H, W, device, stream, prefetch)
+        reader = FrameReader(loader, H, W, device, stream, prefetch, with_mask=masks is None)
         with torch.cuda.device(dev):
             request = torch.empty((LFNET_SIDE, LFNET_SIDE, 3), dtype=torch.uint8, device=dev)
         for i, ff in enumerate(loader.frames):
             t0 = time.perf_counter()
             depth, mask, colour = reader.get(i)
+            if masks is not None:
+                mask = masks.mask(i, ff.id_str, colour, stream.cuda_stream)
             st, roi, _, pose = trk.begin_frame_mm(depth, mask, colour, request, loader_id=i, first_pose=loader.initial_pose(i))
             if ovl is None:
                 reader.release(i)
@@ -503,6 +511,8 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
             out.append((ff.id_str, st, time.perf_counter() - t0))
         if writer is not None:
             writer.close()
+        if masks is not None:
+            masks.flush()
     finally:
         if reader is not None:
             reader.close()

@@ -704,6 +704,45 @@ BT_API int bt_lfnet_enable_timing(bt_ctx* ctx, int on);
 BT_API int bt_lfnet_get_timing(bt_ctx* ctx, float* ms5);
 BT_API int bt_lfnet_debug_maps(bt_ctx* ctx, int image, float* heat_host, float* scale_host, int32_t* kpts_int_host, float* ori_host, void* stream);
 
+/* ---- Object masks on the device: transductive-vos.pytorch's run_video.py (resnet50) without PyTorch ----------------------------------
+ * The first frame's mask is propagated through the video (DESIGN.md §3.13): a ResNet-50 to stride 8 (layer3 and layer4 at stride 1,
+ * layer4 with 256 planes) plus adjust_dim and bn256 gives 256 features per pixel of the (ceil(H / 8), ceil(W / 8)) grid; each frame's
+ * labels are a softmax over the selected earlier frames' pixels, spatially weighted, times their labels.  FP32 results from 3xTF32
+ * tensor-core products.  bt_vos_params holds run_video.py's --ref_num (5 to 64), --range (0 to 10000), --sigma1, --sigma2 (> 0) and
+ * --temperature.
+ * bt_vos_schedule (host code, no GPU): the history frames frame k >= 1 reads (lib/predict.py's sample_frames), n_out <= ref_num of them.
+ * bt_vos_weights_size: the float count of the weight blob (the same for every params).  Blob layout, float32: per conv, in the network's
+ * order, W[cout][ky][kx][cin] then BN scale[cout] and shift[cout] (scale = weight / sqrt(running_var + 1e-5), shift = bias - running_mean
+ * scale, folded in float64 and rounded once).  The order: conv1 (3 -> 64, 7 x 7) with bn1; for each bottleneck of layer1..layer4 (3, 4,
+ * 6, 3 blocks; planes 64, 128, 256, 256) conv1 (1 x 1) bn1, conv2 (3 x 3) bn2, conv3 (1 x 1) bn3, then, in the first block of layer1,
+ * layer2 and layer3, downsample.0 with downsample.1; last adjust_dim (1024 -> 256, 1 x 1) with bn256.
+ * bt_vos_reserve: the history ring of max(range + 5, ref_num + 1) frames of features (1 KB per low-resolution pixel) and labels, and the
+ * network's scratch, for H x W frames (8 to 4096 each).  It ends any sequence begun.
+ * bt_vos_load_weights: copies the blob (synchronously); refuses a size other than bt_vos_weights_size's and non-finite floats.
+ * bt_vos_begin: frame 0.  colour_dev DEVICE H x W x 3 uint8 BGR (cv2.imread's order), init_mask_dev DEVICE H x W uint8 label values,
+ *   mask_out_dev DEVICE H x W uint8 (the mask with > 0 -> 255).  The mask's distinct values become consecutive label channels, value 0
+ *   being channel 0 even when absent; more than 8 channels is BT_ERR_INVALID_ARG, naming the count.  Reads the value set back, so it
+ *   synchronises `stream`.
+ * bt_vos_next: the next frame, asynchronous on `stream`: mask_out_dev DEVICE H x W uint8, 255 where the label is not channel 0.
+ *   BT_ERR_INVALID_ARG before bt_vos_begin.  Both take frames of the reserved size.
+ * bt_vos_enable_timing / bt_vos_get_timing: device time of the last call, ms3 = {backbone, propagation, mask}; get_timing waits for it.
+ * bt_vos_debug (test aid): ring slot `slot`'s features (Hd x Wd x 256 floats) and label (Hd x Wd x 8 floats), the last bt_vos_next's
+ *   low-resolution prediction (8 x Hd x Wd floats, channels past the label count zero) and info5 = {frame index, label channels, ring
+ *   slots, Hd, Wd}; frame k lives in slot k mod ring slots.  Each output optional; synchronises `stream`. */
+typedef struct {
+	int ref_num, range;
+	double sigma1, sigma2, temperature;
+} bt_vos_params;
+BT_API int bt_vos_schedule(int k, int ref_num, int range, int32_t* idx_out, int* n_out);
+BT_API int bt_vos_weights_size(const bt_vos_params* p, size_t* n_floats);
+BT_API int bt_vos_reserve(bt_ctx* ctx, const bt_vos_params* params, int H, int W);
+BT_API int bt_vos_load_weights(bt_ctx* ctx, const float* blob, size_t n_floats);
+BT_API int bt_vos_begin(bt_ctx* ctx, const uint8_t* colour_dev, const uint8_t* init_mask_dev, uint8_t* mask_out_dev, void* stream);
+BT_API int bt_vos_next(bt_ctx* ctx, const uint8_t* colour_dev, uint8_t* mask_out_dev, void* stream);
+BT_API int bt_vos_enable_timing(bt_ctx* ctx, int on);
+BT_API int bt_vos_get_timing(bt_ctx* ctx, float* ms3);
+BT_API int bt_vos_debug(bt_ctx* ctx, int slot, float* feat_host, float* label_host, float* pred_host, int32_t* info5, void* stream);
+
 /* Small device-memory helpers so non-CUDA hosts (ctypes, cgo, JNI) can drive the library without another runtime. */
 BT_API int bt_dev_alloc(void** out, size_t bytes);
 BT_API int bt_dev_free(void* p);

@@ -25,6 +25,10 @@ def main():
     ap.add_argument("--lfnet_model", default=None, help="instead of the server: a released LF-Net model directory (config.pkl and "
                                                         "weights.npz from scripts/lfnet_export_weights.py), run on the device")
     ap.add_argument("--out_dir", required=True)
+    ap.add_argument("--vos_model", default=None, help="instead of the mask files: a transductive-vos checkpoint (run_video.py --resume) "
+                                                      "that propagates --init_mask through the video on the device")
+    ap.add_argument("--init_mask", default=None, help="with --vos_model: the first frame's mask (label values, 8-bit)")
+    ap.add_argument("--mask_save_dir", default=None, help="with --vos_model: also write each frame's mask there as <id>.png, 0 / 255")
     ap.add_argument("--config", default=None, help="the reference's config_ycbineoat.yml (default: the config_nocs.yml values, "
                                                     "bundletrack_b200.config.NOCS_DEFAULTS)")
     ap.add_argument("--device", type=int, default=0)
@@ -36,15 +40,27 @@ def main():
         raise SystemExit(f"--data_dir {a.data_dir} is not a directory")
     loader = YcbineoatVideo(a.data_dir, a.model_dir)
     video = os.path.basename(os.path.normpath(a.data_dir))
+    if (a.init_mask or a.mask_save_dir) and not a.vos_model:
+        raise SystemExit("--init_mask and --mask_save_dir go with --vos_model")
+    masks = None
+    if a.vos_model:
+        if not a.init_mask:
+            raise SystemExit("--vos_model needs --init_mask, the first frame's mask")
+        from bundletrack_b200.sequence import png_layout
+        from bundletrack_b200.vos import load_source
+        W, H = png_layout(loader.frames[0].colour)[:2]
+        masks = load_source(a.vos_model, a.init_mask, H, W, a.mask_save_dir, device=a.device)
     if a.lfnet_model:
         from bundletrack_b200.lfnet import load_lfnet
         client = load_lfnet(a.lfnet_model, device=a.device)
     else:
         client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
     try:
-        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, video), device=a.device, log=a.log)
+        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, video), device=a.device, log=a.log, masks=masks)
     finally:
         client.close()
+        if masks is not None:
+            masks.close()
     print(summary(res))
 
 
