@@ -306,6 +306,7 @@ PROTOTYPES = {
     "bt_host_free_pinned": (_i, (_p,)),
     "bt_stream_sync": (_i, (_p,)),
     "bt_debug_live_resources": (_i, (_p, _p, _p)),
+    "bt_debug_fail_alloc": (_i, (_i,)),
 }
 EXPORTS = list(PROTOTYPES)
 

@@ -55,6 +55,13 @@ extern "C" int bt_debug_live_resources(long long* device_bytes, long long* pinne
 	return BT_OK;
 }
 
+// Test aid: the nth allocation of a library-owned block from now fails with BT_ERR_CUDA without calling CUDA (0 disarms).
+extern "C" int bt_debug_fail_alloc(int nth) {
+	BT_REQUIRE(nth >= 0, BT_ERR_INVALID_ARG, "bt_debug_fail_alloc: nth %d < 0", nth);
+	bt::g_fail_alloc = nth;
+	return BT_OK;
+}
+
 extern "C" int bt_dev_alloc(void** out, size_t bytes) {
 	BT_REQUIRE(out != nullptr, BT_ERR_INVALID_ARG, "bt_dev_alloc: out is NULL");
 	BT_CUDA(cudaMalloc(out, bytes ? bytes : 1));

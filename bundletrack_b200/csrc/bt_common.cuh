@@ -15,11 +15,14 @@ namespace bt {
 
 void set_error(const char* fmt, ...);
 
+// Reports a failed runtime call and consumes it as the runtime's last error, so that a later, unrelated cudaGetLastError() does not
+// report it again (a sticky error stays sticky regardless).
 #define BT_CUDA(x)                                                                                   \
 	do {                                                                                             \
 		cudaError_t e_ = (x);                                                                        \
 		if (e_ != cudaSuccess) {                                                                     \
 			bt::set_error("%s:%d %s -> %s", __FILE__, __LINE__, #x, cudaGetErrorString(e_));         \
+			(void)cudaGetLastError();                                                                \
 			return BT_ERR_CUDA;                                                                      \
 		}                                                                                            \
 	} while (0)
@@ -49,10 +52,13 @@ inline float sqrt_le_max(float th) {
 // What the handle types below hold right now, across the process (bt_debug_live_resources).
 struct LiveResources { std::atomic<long long> dev_bytes{0}, pinned_bytes{0}; std::atomic<int> handles{0}; };
 inline LiveResources g_live;
+// Test aid (bt_debug_fail_alloc): when positive, the allocation that counts it down to 0 fails without calling CUDA.
+inline std::atomic<int> g_fail_alloc{0};
 
 // A growable block of device memory (DevBuf) or page-locked host memory (PinnedBuf), freed with its owner.  `alloc` only grows: a block
 // that is large enough is kept, a larger one replaces it (contents are not kept).  The contexts allocate in *_reserve, never on the
-// per-call path unless a call exceeds what was reserved, in which case the call fails with BT_ERR_CAPACITY.
+// per-call path unless a call exceeds what was reserved, in which case the call fails with BT_ERR_CAPACITY.  The old block is freed
+// before the new one is allocated, so a failed alloc leaves the block empty.
 template <bool Pinned>
 struct Block {
 	void* p = nullptr;
@@ -66,6 +72,7 @@ struct Block {
 	int alloc(size_t n) {
 		if (n <= bytes) return BT_OK;
 		free();
+		BT_REQUIRE(!(g_fail_alloc > 0 && --g_fail_alloc == 0), BT_ERR_CUDA, "Block::alloc: %zu bytes refused by bt_debug_fail_alloc", n);
 		if (Pinned) BT_CUDA(cudaMallocHost(&p, n));
 		else BT_CUDA(cudaMalloc(&p, n));
 		bytes = n;
@@ -195,6 +202,28 @@ struct bt_ctx {
 };
 
 namespace bt {
+// Every module state has `bool ready`.  A reserve checks its arguments, then takes its state with take_state (ready = false), allocates,
+// and sets its capacities and ready = true last; every other entry point looks its state up with state_of, which refuses a state that is
+// not ready.  So after a reserve fails partway, nothing runs on the blocks it freed until a later reserve succeeds.
+template <class T> int take_state(bt_ctx* ctx, StatePtr<T> bt_ctx::*member, T** out) {
+	BT_CUDA(cudaSetDevice(ctx->device));
+	StatePtr<T>& s = ctx->*member;
+	if (!s) s.reset(new T());
+	s->ready = false;
+	*out = s.get();
+	return BT_OK;
+}
+template <class T> int state_of(bt_ctx* ctx, StatePtr<T> bt_ctx::*member, const char* who, const char* reserve, T** out) {
+	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "%s: ctx is NULL", who);
+	T* s = (ctx->*member).get();
+	BT_REQUIRE(s && s->ready, BT_ERR_INVALID_ARG, "%s: call %s (successfully) first", who, reserve);
+	BT_CUDA(cudaSetDevice(ctx->device));
+	*out = s;
+	return BT_OK;
+}
+
+// knn.cu: the argument checks of bt_matcher_reserve, which bt_pipeline_reserve makes before it changes any state
+int matcher_reserve_args(int max_pairs, int max_feats, int dim);
 // policy.cu: the float cofactor inverse of a row-major 4 x 4 (Eigen's Matrix4f::inverse()); false when it is singular
 bool inverse4(const float* m, float* inv);
 // segment.cu: largest-hull mode for the masked front end, and the LF-Net request
@@ -203,7 +232,8 @@ int segment_largest_hull(const uint8_t* const* mask_tbl_dev, int n, int H, int W
                          uint8_t* fill, cudaStream_t stream);
 int launch_lfnet_request(const void* const* tbl_dev, const int32_t* roi_dev, int n, int H, int W, cudaStream_t stream);
 // tracks_dev.cu: the device map-point table, driven pair by pair from bt_find_corres_pairs (prune.cu).  Frames are named by slot;
-// tracks_slot maps a frame id to its slot (-1: the frame has no map yet, unless create is set).
+// tracks_slot maps a frame id to its slot (-1: the frame has no map yet, unless create is set).  tracks_state is state_of for the table.
+int tracks_state(bt_ctx* ctx, const char* who);
 int tracks_slot(bt_ctx* ctx, int frame_id, bool create, int* slot);
 int tracks_free_slots(bt_ctx* ctx);
 // map points alive now (created and not freed by forgets); synchronises `stream`

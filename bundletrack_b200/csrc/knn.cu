@@ -746,6 +746,7 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 struct MatcherState {
+	bool ready = false;
 	int max_pairs = 0, max_feats = 0, dim = 0;
 	int slot_rows = 0;                      // rows per pool slot (max_feats padded to 256)
 	int n_transient = 0, n_persist = 0;     // transient slots [0, n_transient) serve bt_knn_match_pairs; persistent ones follow
@@ -754,7 +755,6 @@ struct MatcherState {
 	UploadBuf h_stage;                      // the set and work tables of a call
 	PFN_encodeTiled encode = nullptr;
 	CUtensorMap tmap_a, tmap_b;
-	bool maps_ready = false;
 	size_t g_halves_cap = 0;
 	int max_q_total = 0, max_blocks = 0;
 	int last_units = 0, last_rows = 0;
@@ -776,17 +776,15 @@ static int make_tmap(MatcherState* m, CUtensorMap* out, void* base, uint64_t row
 }
 
 // (re)allocates the descriptor pool for n_transient + n_persist slots and rebuilds the tensor maps over it
-static int pool_alloc(MatcherState* m) {
-	const size_t rows = (size_t)(m->n_transient + m->n_persist) * m->slot_rows + BN;
+static int pool_alloc(MatcherState* m, int n_persist) {
+	const size_t rows = (size_t)(m->n_transient + n_persist) * m->slot_rows + BN;
 	BT_TRY(m->pool_h.alloc(rows * KD * 2));
 	BT_TRY(m->pool_f.alloc(rows * KD * 4));
 	BT_TRY(m->norms.alloc(rows * 4));
 	BT_TRY(m->errn.alloc(rows * 4));
-	BT_TRY(m->slot_meta.alloc(sizeof(int) * 2 * (size_t)(m->n_transient + m->n_persist)));
+	BT_TRY(m->slot_meta.alloc(sizeof(int) * 2 * (size_t)(m->n_transient + n_persist)));
 	BT_TRY(make_tmap(m, &m->tmap_a, m->pool_h.p, (uint64_t)rows, BM));
-	BT_TRY(make_tmap(m, &m->tmap_b, m->pool_h.p, (uint64_t)rows, BN));
-	m->maps_ready = true;
-	return BT_OK;
+	return make_tmap(m, &m->tmap_b, m->pool_h.p, (uint64_t)rows, BN);
 }
 
 // timing event i, when timing is on: [ev0, ev1) = descriptor conversion + table upload + per-pair constants, [ev1, ev2) = k_knn_tc alone
@@ -891,12 +889,11 @@ static int upload_plan(MatcherState* m, const KnnPlan& w, char* hb, cudaStream_t
 
 // The checks every matching entry point makes (A and B are its two input lists), then the device, the staging block and the first mark.
 static int begin_match(bt_ctx* ctx, const char* who, int n_pairs, const void* A, const void* B, int k, const KnnOut& out, cudaStream_t stream, char** hb) {
-	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready, BT_ERR_INVALID_ARG, "%s: call bt_matcher_reserve first", who);
+	MatcherState* m;
+	BT_TRY(state_of(ctx, &bt_ctx::matcher, who, "bt_matcher_reserve", &m));
 	BT_REQUIRE(A && B && out.idx[0] && out.dist[0] && out.idx[1] && out.dist[1], BT_ERR_INVALID_ARG, "%s: NULL argument", who);
 	BT_REQUIRE(k >= 1 && k <= 8, BT_ERR_UNSUPPORTED, "%s: k=%d outside [1,8]", who, k);
-	MatcherState* m = ctx->matcher.get();
 	BT_REQUIRE(n_pairs > 0 && n_pairs <= m->max_pairs, BT_ERR_CAPACITY, "%s: %d pairs > reserved %d", who, n_pairs, m->max_pairs);
-	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_TRY(m->h_stage.acquire(0, hb));
 	return mark(m, 0, stream);
 }
@@ -937,13 +934,17 @@ static int knn_run(bt_ctx* ctx, const char* who, int n_pairs, const PoolSetRef* 
 
 using namespace bt;
 
-extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int dim) {
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_matcher_reserve: NULL ctx");
+int bt::matcher_reserve_args(int max_pairs, int max_feats, int dim) {
 	BT_REQUIRE(dim == KD, BT_ERR_UNSUPPORTED, "bt_matcher_reserve: descriptor dim %d unsupported (the tensor path is built for %d)", dim, KD);
 	BT_REQUIRE(max_pairs > 0 && max_feats > 0, BT_ERR_INVALID_ARG, "bt_matcher_reserve: bad limits");
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->matcher) ctx->matcher.reset(new MatcherState());
-	MatcherState* m = ctx->matcher.get();
+	return BT_OK;
+}
+
+extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int dim) {
+	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_matcher_reserve: NULL ctx");
+	BT_TRY(matcher_reserve_args(max_pairs, max_feats, dim));
+	MatcherState* m;
+	BT_TRY(take_state(ctx, &bt_ctx::matcher, &m));
 	if (!m->encode) {
 		void* fn = nullptr;
 		cudaDriverEntryPointQueryResult qres;
@@ -953,52 +954,58 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 	}
 	const int slot_rows = (max_feats + BN - 1) / BN * BN;
 	if (slot_rows != m->slot_rows || std::min(2 * max_pairs, 128) != m->n_transient) std::fill(m->slot_n.begin(), m->slot_n.end(), -1);     // the persistent slots move: what they held is dropped
-	m->max_pairs = max_pairs; m->max_feats = max_feats; m->dim = dim; m->slot_rows = slot_rows;
+	m->slot_rows = slot_rows;
 	m->n_transient = std::min(2 * max_pairs, 128);       // distinct descriptor sets one bt_knn_match_pairs call may name (all pairs of K frames: K sets)
-	BT_TRY(pool_alloc(m));
+	BT_TRY(pool_alloc(m, m->n_persist));
 	const int pad_a = (max_feats + BM - 1) / BM * BM;      // A sets are padded to whole 128-row tiles
-	m->g_halves_cap = (size_t)max_pairs * ((size_t)(slot_rows / GRP) * pad_a + (size_t)(pad_a / GRP) * slot_rows);
-	m->max_q_total = 2 * max_pairs * max_feats;
-	m->max_blocks = 2 * max_pairs * ((max_feats + 127) / 128 * 2);      // k_knn_select covers whole 128-position blocks, 64 queries per CTA
+	const size_t g_halves_cap = (size_t)max_pairs * ((size_t)(slot_rows / GRP) * pad_a + (size_t)(pad_a / GRP) * slot_rows);
+	const int max_q_total = 2 * max_pairs * max_feats;
 	BT_TRY(m->sets.alloc(sizeof(PrepSet) * (size_t)std::max(m->n_transient, 1)));
 	const size_t b_tables = sizeof(KnnPair) * ((size_t)max_pairs + 1) + (sizeof(SelJob) + 2 * sizeof(int)) * 2 * max_pairs;     // a KnnPlan's
 	BT_TRY(m->tables.alloc(b_tables));
 	BT_TRY(m->pconst.alloc(sizeof(PairConst) * (size_t)max_pairs));
-	BT_TRY(m->G.alloc(m->g_halves_cap * 2 + 64));
-	BT_TRY(m->cand.alloc(sizeof(int32_t) * SEL_MAXC * (size_t)m->max_q_total));
-	BT_TRY(m->cand_cnt.alloc(sizeof(int32_t) * (size_t)m->max_q_total));
-	BT_TRY(m->qjob.alloc(sizeof(int) * (size_t)m->max_q_total));
-	BT_TRY(m->fb_rows.alloc(sizeof(int) * (size_t)m->max_q_total));
+	BT_TRY(m->G.alloc(g_halves_cap * 2 + 64));
+	BT_TRY(m->cand.alloc(sizeof(int32_t) * SEL_MAXC * (size_t)max_q_total));
+	BT_TRY(m->cand_cnt.alloc(sizeof(int32_t) * (size_t)max_q_total));
+	BT_TRY(m->qjob.alloc(sizeof(int) * (size_t)max_q_total));
+	BT_TRY(m->fb_rows.alloc(sizeof(int) * (size_t)max_q_total));
 	BT_TRY(m->fb_count.alloc(16));
 	BT_TRY(m->fb_part_d.alloc(sizeof(double) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8)); BT_TRY(m->fb_part_i.alloc(sizeof(int) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8));
 	BT_TRY(m->fb_tickets.alloc(sizeof(int) * (size_t)FB_SPLIT_ROWS));
 	BT_CUDA(cudaMemset(m->fb_tickets.p, 0, sizeof(int) * (size_t)FB_SPLIT_ROWS));
 	BT_TRY(m->h_stage.reserve(sizeof(PrepSet) * 2 * max_pairs + b_tables + 4096));
 	BT_CUDA(cudaFuncSetAttribute(k_knn_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_TOTAL));
+	m->max_pairs = max_pairs; m->max_feats = max_feats; m->dim = dim;
+	m->g_halves_cap = g_halves_cap; m->max_q_total = max_q_total;
+	m->max_blocks = 2 * max_pairs * ((max_feats + 127) / 128 * 2);      // k_knn_select covers whole 128-position blocks, 64 queries per CTA
+	m->ready = true;
 	return BT_OK;
 }
 
 // Persistent descriptor pool (SURVEY.md 8f rank 3): Lfnet::detectFeature uploads a frame's descriptors once (FeatureManager.cpp:907);
 // bt_desc_pool_store converts them once into a slot, bt_knn_match_slots / bt_match_pairs_pool then name slots.
 extern "C" int bt_desc_pool_reserve(bt_ctx* ctx, int n_slots) {
-	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready, BT_ERR_INVALID_ARG, "bt_desc_pool_reserve: call bt_matcher_reserve first");
+	MatcherState* m;
+	BT_TRY(state_of(ctx, &bt_ctx::matcher, "bt_desc_pool_reserve", "bt_matcher_reserve", &m));
 	BT_REQUIRE(n_slots > 0, BT_ERR_INVALID_ARG, "bt_desc_pool_reserve: bad slot count");
-	MatcherState* m = ctx->matcher.get();
-	BT_CUDA(cudaSetDevice(ctx->device));
 	if (n_slots <= m->n_persist) return BT_OK;
 	BT_CUDA(cudaDeviceSynchronize());          // the pool moves: nothing may still be reading the old one
-	m->n_persist = n_slots;
+	m->ready = false;                          // (the transient slots move too: until the pool is whole, the matcher refuses every call)
+	m->n_persist = 0;
 	m->slot_n.assign(n_slots, -1);             // (growing the pool re-allocates it: stored sets are dropped)
-	return pool_alloc(m);
+	BT_TRY(pool_alloc(m, n_slots));
+	m->n_persist = n_slots;
+	m->ready = true;
+	return BT_OK;
 }
 
 extern "C" int bt_desc_pool_store(bt_ctx* ctx, int slot, const bt_desc_view* desc, void* stream_) {
-	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->maps_ready && desc, BT_ERR_INVALID_ARG, "bt_desc_pool_store: call bt_matcher_reserve / bt_desc_pool_reserve first");
-	MatcherState* m = ctx->matcher.get();
+	MatcherState* m;
+	BT_TRY(state_of(ctx, &bt_ctx::matcher, "bt_desc_pool_store", "bt_matcher_reserve", &m));
+	BT_REQUIRE(desc, BT_ERR_INVALID_ARG, "bt_desc_pool_store: NULL descriptor view");
 	BT_REQUIRE(slot >= 0 && slot < m->n_persist, BT_ERR_INVALID_ARG, "bt_desc_pool_store: slot %d outside [0,%d)", slot, m->n_persist);
 	BT_TRY(check_desc(*desc, m, __func__, -1));
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	char* hb;
 	BT_TRY(m->h_stage.acquire(0, &hb));
 	BT_TRY(launch_prep(m, { prep_set(m, *desc, m->n_transient + slot) }, hb, stream));
@@ -1027,22 +1034,24 @@ extern "C" int bt_knn_match_slots(bt_ctx* ctx, int n_pairs, const int32_t* slotA
 }
 
 extern "C" int bt_knn_debug_force_fallback(bt_ctx* ctx, int every_nth) {
-	BT_REQUIRE(ctx && ctx->matcher, BT_ERR_INVALID_ARG, "bt_knn_debug_force_fallback: call bt_matcher_reserve first");
-	ctx->matcher->force_fallback = every_nth > 0 ? every_nth : 0;
+	MatcherState* m;
+	BT_TRY(state_of(ctx, &bt_ctx::matcher, "bt_knn_debug_force_fallback", "bt_matcher_reserve", &m));
+	m->force_fallback = every_nth > 0 ? every_nth : 0;
 	return BT_OK;
 }
 
 extern "C" int bt_knn_enable_timing(bt_ctx* ctx, int on) {
-	BT_REQUIRE(ctx && ctx->matcher, BT_ERR_INVALID_ARG, "bt_knn_enable_timing: call bt_matcher_reserve first");
-	MatcherState* m = ctx->matcher.get();
+	MatcherState* m;
+	BT_TRY(state_of(ctx, &bt_ctx::matcher, "bt_knn_enable_timing", "bt_matcher_reserve", &m));
 	if (on) for (Event& e : m->ev) BT_TRY(e.create(true));
 	m->timing = on != 0;
 	return BT_OK;
 }
 // ms4 = {descriptor prep, tensor-core pass, select + exact re-rank, exact fallback}; info3 = {units, query rows, fallback rows}
 extern "C" int bt_knn_get_timing(bt_ctx* ctx, float* ms4, int* info3) {
-	BT_REQUIRE(ctx && ctx->matcher && ctx->matcher->timing && ms4 && info3, BT_ERR_INVALID_ARG, "bt_knn_get_timing: timing not enabled");
-	MatcherState* m = ctx->matcher.get();
+	MatcherState* m;
+	BT_TRY(state_of(ctx, &bt_ctx::matcher, "bt_knn_get_timing", "bt_matcher_reserve", &m));
+	BT_REQUIRE(m->timing && ms4 && info3, BT_ERR_INVALID_ARG, "bt_knn_get_timing: timing not enabled");
 	BT_CUDA(cudaEventSynchronize(m->ev[4]));
 	for (int k = 0; k < 4; k++) BT_CUDA(cudaEventElapsedTime(ms4 + k, m->ev[k], m->ev[k + 1]));
 	int fb = 0;

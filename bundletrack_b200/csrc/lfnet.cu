@@ -574,8 +574,9 @@ constexpr int N_STAGES = 5;     // trunk, scales, detection, keypoints + patches
 
 struct LfnetState {
 	bt_lfnet_params p = {};
+	bool ready = false;
 	int max_images = 0;
-	bool loaded = false;
+	bool loaded = false;            // the weights in w are those of the network p
 	Layout L = {};
 	ScaleArgs sa = {};
 	size_t logit_stride = 0;
@@ -583,7 +584,6 @@ struct LfnetState {
 	UploadBuf h_tbl;
 	bool timing = false;
 	Event ev[N_STAGES + 1];
-	float ms[N_STAGES] = {};
 	bool timed = false;
 };
 void StateDeleter::operator()(LfnetState* s) const { delete s; }
@@ -624,16 +624,9 @@ extern "C" int bt_lfnet_reserve(bt_ctx* ctx, const bt_lfnet_params* p, int max_i
 	LF_FIELD(p->desc_dim >= 32 && p->desc_dim % 32 == 0 && p->desc_dim <= 4096, "desc_dim", "%d", p->desc_dim);
 	LF_FIELD(isfinite(p->leaky_alpha) && isfinite(p->com_strength) && isfinite(p->score_com_strength) && isfinite(p->scale_com_strength) &&
 	         isfinite(p->kp_com_strength) && isfinite(p->nms_thresh), "a strength, alpha or threshold", "%s", "non-finite");
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->lfnet) ctx->lfnet.reset(new LfnetState());
-	LfnetState* s = ctx->lfnet.get();
-	const bool same_net = s->loaded && memcmp(&s->p, p, sizeof *p) == 0;
-	s->p = *p;
-	s->loaded = same_net;
-	s->L = layout_of(*p);
 	// scale_factors = exp(linspace(log(max), log(min), n)) in float64 (mso_resnet_detector.py:106-110), numpy's linspace (start + i step,
 	// the last element set to stop); sizes int(float32(400) * float32(1 / s) + 0.5) (mso_resnet_detector.py:130-132)
-	ScaleArgs& a = s->sa;
+	ScaleArgs a = {};
 	a.n_scales = p->net_num_scales;
 	size_t off = 0;
 	for (int i = 0; i < a.n_scales; i++) {
@@ -649,11 +642,14 @@ extern "C" int bt_lfnet_reserve(bt_ctx* ctx, const bt_lfnet_params* p, int max_i
 		a.logit_off[i] = off;
 		off += (size_t)a.size[i] * a.size[i];
 	}
-	s->logit_stride = off;
+	LfnetState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::lfnet, &s));
+	s->loaded = s->loaded && memcmp(&s->p, p, sizeof *p) == 0;      // (the same network keeps its weights: w is not reallocated)
+	const Layout L = layout_of(*p);
 	const size_t n = (size_t)max_images, rows = n * p->top_k, ns = (size_t)a.n_scales;
 	size_t act = 0;
-	for (int l = 0; l < p->desc_net_depth; l++) act = std::max(act, (size_t)s->L.dl[l].Hout * s->L.dl[l].Hout * s->L.dl[l].Cout);
-	BT_TRY(s->w.alloc(sizeof(float) * s->L.total));
+	for (int l = 0; l < p->desc_net_depth; l++) act = std::max(act, (size_t)L.dl[l].Hout * L.dl[l].Hout * L.dl[l].Cout);
+	BT_TRY(s->w.alloc(sizeof(float) * L.total));
 	BT_TRY(s->tbl.alloc(sizeof(void*) * n));
 	BT_TRY(s->h_tbl.reserve(sizeof(void*) * n));
 	BT_TRY(s->grey.alloc(sizeof(float) * n * HW));
@@ -670,32 +666,31 @@ extern "C" int bt_lfnet_reserve(bt_ctx* ctx, const bt_lfnet_params* p, int max_i
 	const size_t per_row = std::max(std::max(act, (size_t)FC_HIDDEN), (size_t)p->desc_dim);
 	BT_TRY(s->act.alloc(sizeof(float) * rows * per_row));
 	BT_TRY(s->raw.alloc(sizeof(float) * rows * per_row));
+	s->p = *p; s->L = L; s->sa = a; s->logit_stride = off;
 	s->max_images = max_images;
+	s->ready = true;
 	return BT_OK;
 }
 
 extern "C" int bt_lfnet_load_weights(bt_ctx* ctx, const float* blob, size_t n_floats) {
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_lfnet_load_weights: ctx is NULL");
-	LfnetState* s = ctx->lfnet.get();
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_lfnet_load_weights: call bt_lfnet_reserve first");
+	LfnetState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::lfnet, "bt_lfnet_load_weights", "bt_lfnet_reserve", &s));
 	BT_REQUIRE(blob, BT_ERR_INVALID_ARG, "bt_lfnet_load_weights: blob is NULL");
 	BT_REQUIRE(n_floats == s->L.total, BT_ERR_INVALID_ARG, "bt_lfnet_load_weights: %zu floats, the network of these parameters has %zu", n_floats, s->L.total);
 	for (size_t i = 0; i < n_floats; i++)
 		BT_REQUIRE(isfinite(blob[i]), BT_ERR_INVALID_ARG, "bt_lfnet_load_weights: float %zu is not finite", i);
-	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_CUDA(cudaMemcpy(s->w.p, blob, sizeof(float) * n_floats, cudaMemcpyHostToDevice));
 	s->loaded = true;
 	return BT_OK;
 }
 
 extern "C" int bt_lfnet_detect(bt_ctx* ctx, int n, const uint8_t* const* request_dev, float* kpts_out, float* desc_out, int32_t* n_out, void* stream_) {
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_lfnet_detect: ctx is NULL");
-	LfnetState* s = ctx->lfnet.get();
-	BT_REQUIRE(s && s->loaded, BT_ERR_INVALID_ARG, "bt_lfnet_detect: call bt_lfnet_reserve and bt_lfnet_load_weights first");
+	LfnetState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::lfnet, "bt_lfnet_detect", "bt_lfnet_reserve", &s));
+	BT_REQUIRE(s->loaded, BT_ERR_INVALID_ARG, "bt_lfnet_detect: call bt_lfnet_load_weights first");
 	BT_REQUIRE(n >= 1 && request_dev && kpts_out && desc_out && n_out, BT_ERR_INVALID_ARG, "bt_lfnet_detect: n %d < 1 or a NULL pointer", n);
 	for (int i = 0; i < n; i++) BT_REQUIRE(request_dev[i], BT_ERR_INVALID_ARG, "bt_lfnet_detect: request %d is NULL", i);
 	BT_REQUIRE(n <= s->max_images, BT_ERR_CAPACITY, "bt_lfnet_detect: %d images > the reserved %d", n, s->max_images);
-	BT_CUDA(cudaSetDevice(ctx->device));
 	cudaStream_t st = (cudaStream_t)stream_;
 	const bt_lfnet_params& p = s->p;
 	const Layout& L = s->L;
@@ -788,28 +783,26 @@ extern "C" int bt_lfnet_detect(bt_ctx* ctx, int n, const uint8_t* const* request
 }
 
 extern "C" int bt_lfnet_enable_timing(bt_ctx* ctx, int on) {
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_lfnet_enable_timing: ctx is NULL");
-	BT_REQUIRE(ctx->lfnet, BT_ERR_INVALID_ARG, "bt_lfnet_enable_timing: call bt_lfnet_reserve first");
-	ctx->lfnet->timing = on != 0;
+	LfnetState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::lfnet, "bt_lfnet_enable_timing", "bt_lfnet_reserve", &s));
+	s->timing = on != 0;
 	return BT_OK;
 }
 
 extern "C" int bt_lfnet_get_timing(bt_ctx* ctx, float* ms5) {
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_lfnet_get_timing: ctx is NULL");
-	LfnetState* s = ctx->lfnet.get();
-	BT_REQUIRE(s && s->timed && ms5, BT_ERR_INVALID_ARG, "bt_lfnet_get_timing: no timed call (bt_lfnet_enable_timing) or ms5 is NULL");
-	BT_CUDA(cudaSetDevice(ctx->device));
+	LfnetState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::lfnet, "bt_lfnet_get_timing", "bt_lfnet_reserve", &s));
+	BT_REQUIRE(s->timed && ms5, BT_ERR_INVALID_ARG, "bt_lfnet_get_timing: no timed call (bt_lfnet_enable_timing) or ms5 is NULL");
 	BT_CUDA(cudaEventSynchronize(s->ev[N_STAGES]));
 	for (int i = 0; i < N_STAGES; i++) BT_CUDA(cudaEventElapsedTime(ms5 + i, s->ev[i], s->ev[i + 1]));
 	return BT_OK;
 }
 
 extern "C" int bt_lfnet_debug_maps(bt_ctx* ctx, int image, float* heat_host, float* scale_host, int32_t* kpts_int_host, float* ori_host, void* stream) {
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_lfnet_debug_maps: ctx is NULL");
-	LfnetState* s = ctx->lfnet.get();
-	BT_REQUIRE(s && s->loaded, BT_ERR_INVALID_ARG, "bt_lfnet_debug_maps: no network reserved and loaded");
+	LfnetState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::lfnet, "bt_lfnet_debug_maps", "bt_lfnet_reserve", &s));
+	BT_REQUIRE(s->loaded, BT_ERR_INVALID_ARG, "bt_lfnet_debug_maps: call bt_lfnet_load_weights first");
 	BT_REQUIRE(image >= 0 && image < s->max_images, BT_ERR_INVALID_ARG, "bt_lfnet_debug_maps: image %d outside [0, %d)", image, s->max_images);
-	BT_CUDA(cudaSetDevice(ctx->device));
 	cudaStream_t st = (cudaStream_t)stream;
 	const size_t k = (size_t)s->p.top_k, f = (size_t)image;
 	if (heat_host) BT_CUDA(cudaMemcpyAsync(heat_host, s->heat.as<float>() + f * HW, sizeof(float) * HW, cudaMemcpyDeviceToHost, st));

@@ -382,6 +382,7 @@ bool roi_ok(const int32_t* r, int H, int W) { return r[0] >= 0 && r[0] < r[1] &&
 }  // namespace
 
 struct MatchVizState {
+	bool ready = false;
 	int max_images = 0, max_matches = 0;
 	DevBuf imgs, segs, boxes, colours;
 	UploadBuf h;                                   // the image table and the colours of one call
@@ -410,9 +411,8 @@ extern "C" int bt_match_viz_reserve(bt_ctx* ctx, int max_images, int max_matches
 	// the images of a call are k_mv_setup's grid rows (at most 65535)
 	BT_REQUIRE(max_images >= 1 && max_images <= 65535 && max_matches >= 0 && max_matches < (1 << 28), BT_ERR_INVALID_ARG,
 	           "bt_match_viz_reserve: max_images %d must be in [1, 65535] and max_matches %d in [0, 2^28)", max_images, max_matches);
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->matchviz) ctx->matchviz.reset(new MatchVizState());
-	MatchVizState* s = ctx->matchviz.get();
+	MatchVizState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::matchviz, &s));
 	const size_t mm = (size_t)max(max_matches, 1);
 	BT_TRY(s->imgs.alloc(sizeof(MvImage) * (size_t)max_images));
 	BT_TRY(s->segs.alloc(sizeof(MvSeg) * kSegs * mm));
@@ -420,14 +420,15 @@ extern "C" int bt_match_viz_reserve(bt_ctx* ctx, int max_images, int max_matches
 	BT_TRY(s->colours.alloc(sizeof(uchar4) * mm));
 	BT_TRY(s->h.reserve(align16(sizeof(MvImage) * (size_t)max_images) + sizeof(uchar4) * mm));
 	s->max_images = max_images; s->max_matches = max_matches;
+	s->ready = true;
 	return BT_OK;
 }
 
 extern "C" int bt_match_viz(bt_ctx* ctx, int n_images, const bt_match_viz_desc* desc, uint8_t* const* out_dev, void* stream_) {
-	BT_REQUIRE(ctx && desc && out_dev, BT_ERR_INVALID_ARG, "bt_match_viz: NULL argument");
+	BT_REQUIRE(desc && out_dev, BT_ERR_INVALID_ARG, "bt_match_viz: NULL argument");
 	BT_REQUIRE(n_images >= 1, BT_ERR_INVALID_ARG, "bt_match_viz: n_images %d must be >= 1", n_images);
-	MatchVizState* s = ctx->matchviz.get();
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_match_viz: call bt_match_viz_reserve first");
+	MatchVizState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::matchviz, "bt_match_viz", "bt_match_viz_reserve", &s));
 	long long total = 0, tiles = 0;
 	for (int i = 0; i < n_images; i++) {
 		const bt_match_viz_desc& d = desc[i];
@@ -446,7 +447,6 @@ extern "C" int bt_match_viz(bt_ctx* ctx, int n_images, const bt_match_viz_desc* 
 	BT_REQUIRE(n_images <= s->max_images && total <= s->max_matches, BT_ERR_CAPACITY,
 	           "bt_match_viz: %d images / %lld matches exceed the reserved %d / %d", n_images, total, s->max_images, s->max_matches);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	char* h;
 	BT_TRY(s->h.acquire(0, &h));
 	const size_t ib = align16(sizeof(MvImage) * (size_t)n_images);

@@ -225,6 +225,7 @@ void frame_const(const double* pred, const double* gt, FrameConst& fc) {
 }  // namespace
 
 struct MetricsState {
+	bool ready = false;
 	int max_pts = 0, max_frames = 0;
 	DevBuf pts32, frames, part, pmax;
 	UploadBuf h_frames;
@@ -239,9 +240,8 @@ extern "C" int bt_metrics_reserve(bt_ctx* ctx, int max_pts, int max_frames) {
 	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_metrics_reserve: ctx is NULL");
 	BT_REQUIRE(max_pts >= 1 && max_frames >= 1, BT_ERR_INVALID_ARG, "bt_metrics_reserve: max_pts %d / max_frames %d must be >= 1", max_pts, max_frames);
 	BT_REQUIRE((max_pts + kChunk - 1) / kChunk <= 65535, BT_ERR_INVALID_ARG, "bt_metrics_reserve: max_pts %d > %d", max_pts, 65535 * kChunk);
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->metrics) ctx->metrics.reset(new MetricsState());
-	MetricsState* s = ctx->metrics.get();
+	MetricsState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::metrics, &s));
 	const size_t n_chunks = (size_t)(max_pts + kChunk - 1) / kChunk;
 	BT_TRY(s->pts32.alloc(sizeof(float4) * (size_t)max_pts));
 	BT_TRY(s->frames.alloc(sizeof(FrameConst) * (size_t)max_frames));
@@ -249,6 +249,7 @@ extern "C" int bt_metrics_reserve(bt_ctx* ctx, int max_pts, int max_frames) {
 	BT_TRY(s->pmax.alloc(sizeof(unsigned long long)));
 	BT_TRY(s->h_frames.reserve(sizeof(FrameConst) * (size_t)max_frames));
 	s->max_pts = max_pts; s->max_frames = max_frames;
+	s->ready = true;
 	return BT_OK;
 }
 
@@ -258,13 +259,11 @@ extern "C" int bt_pose_metrics(bt_ctx* ctx, const double* model_pts_dev, int n_p
 	BT_REQUIRE(model_pts_dev && pred_ob_in_cam && gt_ob_in_cam && add_out && adds_out, BT_ERR_INVALID_ARG, "bt_pose_metrics: NULL argument");
 	for (size_t k = 0; k < 16 * (size_t)n_frames; k++)
 		BT_REQUIRE(isfinite(pred_ob_in_cam[k]) && isfinite(gt_ob_in_cam[k]), BT_ERR_INVALID_ARG, "bt_pose_metrics: frame %d has a non-finite pose element", (int)(k / 16));
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_pose_metrics: ctx is NULL");
-	MetricsState* s = ctx->metrics.get();
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_pose_metrics: call bt_metrics_reserve first");
+	MetricsState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::metrics, "bt_pose_metrics", "bt_metrics_reserve", &s));
 	BT_REQUIRE(n_pts <= s->max_pts && n_frames <= s->max_frames, BT_ERR_CAPACITY, "bt_pose_metrics: %d points / %d frames exceed the reserved %d / %d",
 	           n_pts, n_frames, s->max_pts, s->max_frames);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	FrameConst* hf;
 	BT_TRY(s->h_frames.acquire(0, &hf));
 	for (int f = 0; f < n_frames; f++) frame_const(pred_ob_in_cam + 16 * (size_t)f, gt_ob_in_cam + 16 * (size_t)f, hf[f]);
@@ -458,6 +457,7 @@ __global__ void __launch_bounds__(32 * kNocsWarps) k_nocs_metrics(const NocsReco
 }  // namespace
 
 struct NocsState {
+	bool ready = false;
 	int max_records = 0;
 	DevBuf recs;
 	UploadBuf h_recs;
@@ -469,13 +469,13 @@ void StateDeleter::operator()(NocsState* s) const { delete s; }
 extern "C" int bt_nocs_reserve(bt_ctx* ctx, int max_records) {
 	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_nocs_reserve: ctx is NULL");
 	BT_REQUIRE(max_records >= 1, BT_ERR_INVALID_ARG, "bt_nocs_reserve: max_records %d must be >= 1", max_records);
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->nocs) ctx->nocs.reset(new NocsState());
-	NocsState* s = ctx->nocs.get();
+	NocsState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::nocs, &s));
 	const size_t bytes = kNocsRot * sizeof(double2) + sizeof(NocsRecord) * (size_t)max_records;
 	BT_TRY(s->recs.alloc(bytes));
 	BT_TRY(s->h_recs.reserve(bytes));
 	s->max_records = max_records;
+	s->ready = true;
 	return BT_OK;
 }
 
@@ -487,12 +487,10 @@ extern "C" int bt_nocs_metrics(bt_ctx* ctx, const double* pred, const double* gt
 		BT_REQUIRE(isfinite(pred[k]) && isfinite(gt[k]), BT_ERR_INVALID_ARG, "bt_nocs_metrics: record %d has a non-finite pose element", (int)(k / 16));
 	for (size_t k = 0; k < 24 * (size_t)n; k++)
 		BT_REQUIRE(isfinite(corners[k]), BT_ERR_INVALID_ARG, "bt_nocs_metrics: record %d has a non-finite corner", (int)(k / 24));
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_nocs_metrics: ctx is NULL");
-	NocsState* s = ctx->nocs.get();
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_nocs_metrics: call bt_nocs_reserve first");
+	NocsState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::nocs, "bt_nocs_metrics", "bt_nocs_reserve", &s));
 	BT_REQUIRE(n <= s->max_records, BT_ERR_CAPACITY, "bt_nocs_metrics: %d records exceed the reserved %d", n, s->max_records);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	char* h;
 	BT_TRY(s->h_recs.acquire(0, &h));
 	double2* hrot = reinterpret_cast<double2*>(h);

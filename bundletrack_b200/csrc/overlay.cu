@@ -348,6 +348,7 @@ __global__ void k_ovl_stamp(const float* __restrict__ cent, int stride, const in
 }  // namespace
 
 struct OverlayState {
+	bool ready = false;
 	int max_pts = 0, max_frames = 0, max_tiles = 0;
 	DevBuf a, b, cent, tiles, grid, hist, scan, cnt, tscan, tbl, nout;
 	UploadBuf h;                                   // tiles, pointer tables and poses of one call
@@ -404,9 +405,8 @@ extern "C" int bt_overlay_reserve(bt_ctx* ctx, int max_pts, int max_frames) {
 	const long long total = (long long)max_pts * max_frames;
 	const long long tiles = total / kTile + max_frames;
 	BT_REQUIRE(total <= (1LL << 30), BT_ERR_INVALID_ARG, "bt_overlay_reserve: max_pts x max_frames = %lld > 2^30", total);
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->overlay) ctx->overlay.reset(new OverlayState());
-	OverlayState* s = ctx->overlay.get();
+	OverlayState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::overlay, &s));
 	BT_TRY(s->a.alloc(sizeof(float4) * (size_t)total));
 	BT_TRY(s->b.alloc(sizeof(float4) * (size_t)total));
 	BT_TRY(s->cent.alloc(3 * sizeof(float) * (size_t)total));
@@ -421,16 +421,17 @@ extern "C" int bt_overlay_reserve(bt_ctx* ctx, int max_pts, int max_frames) {
 	BT_TRY(s->tbl.alloc(tbl));
 	BT_TRY(s->h.reserve(align16(sizeof(Tile) * (size_t)tiles) + tbl));
 	s->max_pts = max_pts; s->max_frames = max_frames; s->max_tiles = (int)tiles;
+	s->ready = true;
 	return BT_OK;
 }
 
 extern "C" int bt_voxel_downsample(bt_ctx* ctx, int n_clouds, const float* const* pts_dev, const int* n_pts, float leaf, float* const* out_dev, int32_t* n_out_dev,
                                    void* stream_) {
-	BT_REQUIRE(ctx && pts_dev && n_pts && out_dev && n_out_dev, BT_ERR_INVALID_ARG, "bt_voxel_downsample: NULL argument");
+	BT_REQUIRE(pts_dev && n_pts && out_dev && n_out_dev, BT_ERR_INVALID_ARG, "bt_voxel_downsample: NULL argument");
 	BT_REQUIRE(n_clouds >= 1, BT_ERR_INVALID_ARG, "bt_voxel_downsample: n_clouds %d must be >= 1", n_clouds);
 	BT_REQUIRE(leaf > 0.f && isfinite(leaf), BT_ERR_INVALID_ARG, "bt_voxel_downsample: leaf must be positive and finite");
-	OverlayState* s = ctx->overlay.get();
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_voxel_downsample: call bt_overlay_reserve first");
+	OverlayState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::overlay, "bt_voxel_downsample", "bt_overlay_reserve", &s));
 	long long total = 0;
 	for (int c = 0; c < n_clouds; c++) {
 		BT_REQUIRE(n_pts[c] >= 1 && pts_dev[c] && out_dev[c], BT_ERR_INVALID_ARG, "bt_voxel_downsample: cloud %d has %d points or a NULL pointer", c, n_pts[c]);
@@ -440,7 +441,6 @@ extern "C" int bt_voxel_downsample(bt_ctx* ctx, int n_clouds, const float* const
 	           "bt_voxel_downsample: %d clouds / %lld points exceed the reserved %d clouds / %lld points", n_clouds, total, s->max_frames,
 	           (long long)s->max_pts * s->max_frames);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	char* h;
 	BT_TRY(s->h.acquire(0, &h));
 	int n_tiles = 0;
@@ -463,17 +463,16 @@ extern "C" int bt_voxel_downsample(bt_ctx* ctx, int n_clouds, const float* const
 extern "C" int bt_pose_overlay(bt_ctx* ctx, int n_frames, const float* model_dev, int n_model, const float* cur_in_model, float fx, float fy, float cx, float cy,
                                const uint8_t* const* colour_dev, const uint8_t* const* fg_dev, int H, int W, uint8_t* const* viz_out_dev,
                                uint8_t* const* raw_out_dev, void* stream_) {
-	BT_REQUIRE(ctx && model_dev && cur_in_model && colour_dev && fg_dev && viz_out_dev, BT_ERR_INVALID_ARG, "bt_pose_overlay: NULL argument");
+	BT_REQUIRE(model_dev && cur_in_model && colour_dev && fg_dev && viz_out_dev, BT_ERR_INVALID_ARG, "bt_pose_overlay: NULL argument");
 	BT_REQUIRE(n_frames >= 1 && n_model >= 1 && H >= 1 && W >= 1, BT_ERR_INVALID_ARG, "bt_pose_overlay: n_frames %d / n_model %d / %d x %d must be >= 1",
 	           n_frames, n_model, W, H);
 	for (int f = 0; f < n_frames; f++)
 		BT_REQUIRE(colour_dev[f] && fg_dev[f] && viz_out_dev[f] && (!raw_out_dev || raw_out_dev[f]), BT_ERR_INVALID_ARG, "bt_pose_overlay: frame %d has a NULL image", f);
-	OverlayState* s = ctx->overlay.get();
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_pose_overlay: call bt_overlay_reserve first");
+	OverlayState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::overlay, "bt_pose_overlay", "bt_overlay_reserve", &s));
 	BT_REQUIRE(n_frames <= s->max_frames && n_model <= s->max_pts, BT_ERR_CAPACITY, "bt_pose_overlay: %d frames / %d model points exceed the reserved %d / %d",
 	           n_frames, n_model, s->max_frames, s->max_pts);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	char* h;
 	BT_TRY(s->h.acquire(0, &h));
 	const size_t fb = align16(sizeof(OverlayFrame) * (size_t)n_frames), pb = align16(sizeof(void*) * (size_t)n_frames);

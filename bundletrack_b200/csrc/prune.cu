@@ -233,6 +233,7 @@ __global__ void __launch_bounds__(256) k_emit_fill(const PrunePair* __restrict__
 }
 
 struct PruneState {
+	bool ready = false;
 	int max_pairs = 0, max_feats = 0;
 	DevBuf pairs, corr, PA, PB, n_corr, n_nn, rpairs, inl, n_inl, idxAB, distAB, idxBA, distBA, entry_off, total, extra, n_prop;
 	UploadBuf h_pairs, h_extra;
@@ -245,26 +246,29 @@ void StateDeleter::operator()(PruneState* s) const { delete s; }
 using namespace bt;
 
 extern "C" int bt_pipeline_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int dim, int max_trials) {
-	BT_REQUIRE(ctx && max_pairs > 0 && max_feats > 0, BT_ERR_INVALID_ARG, "bt_pipeline_reserve: bad arguments");
+	BT_REQUIRE(ctx && max_pairs > 0 && max_feats > 0 && max_trials > 0, BT_ERR_INVALID_ARG, "bt_pipeline_reserve: bad arguments");
+	BT_TRY(matcher_reserve_args(max_pairs, max_feats, dim));
+	PruneState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::prune, &s));
 	BT_TRY(bt_matcher_reserve(ctx, max_pairs, max_feats, dim));
 	BT_TRY(bt_ransac_reserve(ctx, max_pairs, 3 * max_feats, max_trials));
-	if (!ctx->prune) ctx->prune.reset(new PruneState());
-	PruneState* s = ctx->prune.get();
-	s->max_pairs = max_pairs; s->max_feats = max_feats;
 	const size_t cap = (size_t)3 * max_feats * max_pairs;      // nA + nB mutual candidates + up to max_feats propagated map-point matches per pair
-	s->extra_cap = (size_t)max_feats * max_pairs;
+	const size_t extra_cap = (size_t)max_feats * max_pairs;
 	BT_TRY(s->pairs.alloc(sizeof(PrunePair) * max_pairs));
 	BT_TRY(s->corr.alloc(sizeof(bt_correspondence) * cap));
 	BT_TRY(s->PA.alloc(sizeof(float4) * cap)); BT_TRY(s->PB.alloc(sizeof(float4) * cap));
 	BT_TRY(s->n_corr.alloc(sizeof(int32_t) * max_pairs)); BT_TRY(s->n_nn.alloc(sizeof(int32_t) * max_pairs));
-	BT_TRY(s->extra.alloc(sizeof(float4) * s->extra_cap));
+	BT_TRY(s->extra.alloc(sizeof(float4) * extra_cap));
 	BT_TRY(s->rpairs.alloc(sizeof(RansacPair) * max_pairs));
 	BT_TRY(s->inl.alloc(sizeof(int32_t) * cap)); BT_TRY(s->n_inl.alloc(sizeof(int32_t) * max_pairs));
 	BT_TRY(s->idxAB.alloc(sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs)); BT_TRY(s->distAB.alloc(sizeof(float) * 8 * (size_t)max_feats * max_pairs));
 	BT_TRY(s->idxBA.alloc(sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs)); BT_TRY(s->distBA.alloc(sizeof(float) * 8 * (size_t)max_feats * max_pairs));
 	BT_TRY(s->entry_off.alloc(sizeof(int32_t) * max_pairs)); BT_TRY(s->total.alloc(16)); BT_TRY(s->n_prop.alloc(sizeof(int32_t) * max_pairs));
-	BT_TRY(s->h_extra.reserve(sizeof(float4) * s->extra_cap));
-	return s->h_pairs.reserve(sizeof(PrunePair) * max_pairs);
+	BT_TRY(s->h_extra.reserve(sizeof(float4) * extra_cap));
+	BT_TRY(s->h_pairs.reserve(sizeof(PrunePair) * max_pairs));
+	s->max_pairs = max_pairs; s->max_feats = max_feats; s->extra_cap = extra_cap;
+	s->ready = true;
+	return BT_OK;
 }
 
 namespace {
@@ -362,10 +366,9 @@ struct Chain {
 extern "C" int bt_prune_mutual_pairs(bt_ctx* ctx, int n_pairs, const bt_match_frame* A, const bt_match_frame* B, int H, int W, float fx, float fy, float cx, float cy,
                                      const int32_t* idxAB, const int32_t* idxBA, int k, const bt_prune_params* prm,
                                      bt_correspondence* corr_out, int32_t* n_corr_out, void* stream_) {
-	PruneState* s = ctx ? ctx->prune.get() : nullptr;
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_prune_mutual_pairs: call bt_pipeline_reserve first");
+	PruneState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::prune, "bt_prune_mutual_pairs", "bt_pipeline_reserve", &s));
 	BT_REQUIRE(A && B && idxAB && idxBA && prm && corr_out && n_corr_out && n_pairs > 0 && n_pairs <= s->max_pairs && k >= 1 && k <= 8, BT_ERR_INVALID_ARG, "bt_prune_mutual_pairs: bad argument");
-	BT_CUDA(cudaSetDevice(ctx->device));
 	Chain c(ctx, "bt_prune_mutual_pairs", n_pairs, A, B, H, W, fx, fy, cx, cy, prm, 0, 0.f, 0, stream_);
 	c.idxAB = idxAB; c.idxBA = idxBA; c.k = k;
 	c.corr = corr_out; c.n_corr = n_corr_out;
@@ -395,10 +398,9 @@ extern "C" int bt_match_pairs_ex(bt_ctx* ctx, int n_pairs, const bt_match_frame*
                                  const int32_t* slotA, const int32_t* slotB, int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune,
                                  int ransac_trials, float ransac_inlier_dist, uint64_t ransac_seed, const bt_match_extra* extra,
                                  bt_entryj* entry_out, int entry_capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, int32_t* status_out, float* uv_out, void* stream_) {
-	PruneState* s = ctx ? ctx->prune.get() : nullptr;
-	BT_REQUIRE(s, BT_ERR_INVALID_ARG, "bt_match_pairs: call bt_pipeline_reserve first");
+	PruneState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::prune, "bt_match_pairs", "bt_pipeline_reserve", &s));
 	BT_REQUIRE(A && B && prune && entry_out && n_entry_out && entry_off_out && total_out && n_pairs > 0 && n_pairs <= s->max_pairs, BT_ERR_INVALID_ARG, "bt_match_pairs: bad argument");
-	BT_CUDA(cudaSetDevice(ctx->device));
 	Chain c(ctx, "bt_match_pairs_ex", n_pairs, A, B, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, stream_);
 	BT_TRY(c.knn(dA, dB, slotA, slotB));
 	BT_TRY(c.pairs(extra, 0));
@@ -416,8 +418,9 @@ extern "C" int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_fra
                                     const int32_t* slotA, const int32_t* slotB, int H, int W, float fx, float fy, float cx, float cy, const bt_prune_params* prune,
                                     int ransac_trials, float ransac_inlier_dist, uint64_t ransac_seed, bt_entryj* entry_out, int entry_capacity,
                                     int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, int32_t* status_out, float* uv_out, void* stream_) {
-	PruneState* s = ctx ? ctx->prune.get() : nullptr;
-	BT_REQUIRE(s && ctx->tracks, BT_ERR_INVALID_ARG, "bt_find_corres_pairs: call bt_pipeline_reserve and bt_tracks_dev_reserve first");
+	PruneState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::prune, "bt_find_corres_pairs", "bt_pipeline_reserve", &s));
+	BT_TRY(tracks_state(ctx, "bt_find_corres_pairs"));
 	BT_REQUIRE(A && B && prune && entry_out && entry_capacity >= 0 && n_entry_out && entry_off_out && total_out && n_pairs > 0 && n_pairs <= s->max_pairs,
 	           BT_ERR_INVALID_ARG, "bt_find_corres_pairs: bad argument");
 	std::vector<int> fresh;   // frame A is the newer frame of every pair; the frames that are new to the table must fit before anything is queued
@@ -430,7 +433,6 @@ extern "C" int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_fra
 		}
 	}
 	BT_REQUIRE((int)fresh.size() <= tracks_free_slots(ctx), BT_ERR_CAPACITY, "bt_find_corres_pairs: %d new frames do not fit the map-point table", (int)fresh.size());
-	BT_CUDA(cudaSetDevice(ctx->device));
 	Chain c(ctx, "bt_find_corres_pairs", n_pairs, A, B, H, W, fx, fy, cx, cy, prune, ransac_trials, ransac_inlier_dist, ransac_seed, stream_);
 	BT_TRY(c.knn(dA, dB, slotA, slotB));
 	BT_TRY(c.pairs(nullptr, s->max_feats));
@@ -498,6 +500,7 @@ __global__ void __launch_bounds__(kCompactThreads) k_cache_compact(const CacheMo
 	}
 }
 struct MatchCache {
+	bool ready = false;
 	int max_pairs = 0, max_block = 0;  // pairs cached at once; entries per block (the arena size for bt_match_cache_reserve_entries)
 	long long cap = 0, top = 0, live = 0;   // arena entries: size, end of the last block placed, entries in live blocks
 	DevBuf arena, tab;
@@ -517,9 +520,8 @@ static int cache_upload(MatchCache* c, const std::vector<CacheMove>& mv, cudaStr
 	return up.in_flight(stream);
 }
 static int cache_reserve(bt_ctx* ctx, int max_pairs_cached, int max_block, long long total) {
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->mcache) ctx->mcache.reset(new MatchCache());
-	MatchCache* c = ctx->mcache.get();
+	MatchCache* c;
+	BT_TRY(take_state(ctx, &bt_ctx::mcache, &c));
 	BT_TRY(c->arena.alloc(sizeof(bt_entryj) * (size_t)total));
 	// a put uploads the compaction (every live block) and its own blocks in one table
 	BT_TRY(c->tab.alloc(sizeof(CacheMove) * 2 * (size_t)max_pairs_cached));
@@ -527,6 +529,7 @@ static int cache_reserve(bt_ctx* ctx, int max_pairs_cached, int max_block, long 
 	c->max_pairs = max_pairs_cached; c->max_block = max_block;
 	c->cap = total; c->top = 0; c->live = 0;
 	c->recs.clear();
+	c->ready = true;
 	return BT_OK;
 }
 }  // namespace bt
@@ -544,10 +547,10 @@ extern "C" int bt_match_cache_reserve_entries(bt_ctx* ctx, int max_pairs_cached,
 
 extern "C" int bt_match_cache_put(bt_ctx* ctx, int n_pairs, const int32_t* idA, const int32_t* idB, const bt_entryj* entry_dev,
                                   const int32_t* n_entry_host, const int32_t* entry_off_host, const int32_t* status_host, void* stream_) {
-	BT_REQUIRE(ctx && ctx->mcache && idA && idB && n_entry_host && entry_off_host && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_match_cache_put: call bt_match_cache_reserve first / NULL argument");
-	MatchCache* c = ctx->mcache.get();
+	MatchCache* c;
+	BT_TRY(state_of(ctx, &bt_ctx::mcache, "bt_match_cache_put", "bt_match_cache_reserve", &c));
+	BT_REQUIRE(idA && idB && n_entry_host && entry_off_host && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_match_cache_put: NULL argument");
 	BT_REQUIRE(n_pairs <= c->max_pairs, BT_ERR_CAPACITY, "bt_match_cache_put: %d pairs > table of %d", n_pairs, c->max_pairs);
-	BT_CUDA(cudaSetDevice(ctx->device));
 	// check everything before changing anything: a refused put leaves the cache as it was.  A pair listed twice keeps its last block.
 	std::map<std::pair<int, int>, int> last;            // pair -> index of its last occurrence in the list
 	for (int p = 0; p < n_pairs; p++) {
@@ -607,32 +610,37 @@ extern "C" int bt_match_cache_put(bt_ctx* ctx, int n_pairs, const int32_t* idA, 
 
 extern "C" int bt_match_cache_has(bt_ctx* ctx, int idA, int idB) {
 	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_match_cache_has: ctx is NULL");
-	if (!ctx->mcache) return 0;
-	return ctx->mcache->recs.count(std::make_pair(idA, idB)) ? 1 : 0;
+	if (!ctx->mcache) return 0;        // (nothing cached before the first reserve)
+	MatchCache* c;
+	BT_TRY(state_of(ctx, &bt_ctx::mcache, "bt_match_cache_has", "bt_match_cache_reserve", &c));
+	return c->recs.count(std::make_pair(idA, idB)) ? 1 : 0;
 }
 
 extern "C" int bt_match_cache_status(bt_ctx* ctx, int idA, int idB, int* n_entry, int* status) {
-	BT_REQUIRE(ctx && ctx->mcache, BT_ERR_INVALID_ARG, "bt_match_cache_status: call bt_match_cache_reserve first");
-	const auto it = ctx->mcache->recs.find(std::make_pair(idA, idB));
-	BT_REQUIRE(it != ctx->mcache->recs.end(), BT_ERR_INVALID_ARG, "bt_match_cache_status: pair (%d, %d) is not cached", idA, idB);
+	MatchCache* c;
+	BT_TRY(state_of(ctx, &bt_ctx::mcache, "bt_match_cache_status", "bt_match_cache_reserve", &c));
+	const auto it = c->recs.find(std::make_pair(idA, idB));
+	BT_REQUIRE(it != c->recs.end(), BT_ERR_INVALID_ARG, "bt_match_cache_status: pair (%d, %d) is not cached", idA, idB);
 	if (n_entry) *n_entry = it->second.n;
 	if (status) *status = it->second.status;
 	return BT_OK;
 }
 
 extern "C" int bt_match_cache_usage(bt_ctx* ctx, int* n_pairs, long long* n_entries) {
-	BT_REQUIRE(ctx && ctx->mcache && n_pairs && n_entries, BT_ERR_INVALID_ARG, "bt_match_cache_usage: call bt_match_cache_reserve first / NULL argument");
-	*n_pairs = (int)ctx->mcache->recs.size();
-	*n_entries = ctx->mcache->live;
+	MatchCache* c;
+	BT_TRY(state_of(ctx, &bt_ctx::mcache, "bt_match_cache_usage", "bt_match_cache_reserve", &c));
+	BT_REQUIRE(n_pairs && n_entries, BT_ERR_INVALID_ARG, "bt_match_cache_usage: NULL argument");
+	*n_pairs = (int)c->recs.size();
+	*n_entries = c->live;
 	return BT_OK;
 }
 
 extern "C" int bt_match_cache_gather(bt_ctx* ctx, int n_pairs, const int32_t* idA, const int32_t* idB, const uint32_t* win_i, const uint32_t* win_j,
                                      bt_entryj* dst_dev, int capacity, int32_t* block_off_host, int32_t* block_n_host, void* stream_) {
-	BT_REQUIRE(ctx && ctx->mcache && idA && idB && win_i && win_j && dst_dev && block_off_host && block_n_host && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_match_cache_gather: NULL argument");
-	MatchCache* c = ctx->mcache.get();
+	MatchCache* c;
+	BT_TRY(state_of(ctx, &bt_ctx::mcache, "bt_match_cache_gather", "bt_match_cache_reserve", &c));
+	BT_REQUIRE(idA && idB && win_i && win_j && dst_dev && block_off_host && block_n_host && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_match_cache_gather: NULL argument");
 	BT_REQUIRE(n_pairs <= c->max_pairs, BT_ERR_CAPACITY, "bt_match_cache_gather: %d pairs > table of %d", n_pairs, c->max_pairs);
-	BT_CUDA(cudaSetDevice(ctx->device));
 	std::vector<CacheMove> mv;
 	int off = 0;
 	for (int p = 0; p < n_pairs; p++) {
@@ -653,8 +661,8 @@ extern "C" int bt_match_cache_gather(bt_ctx* ctx, int n_pairs, const int32_t* id
 }
 
 extern "C" int bt_match_cache_forget_frame(bt_ctx* ctx, int frame_id) {
-	BT_REQUIRE(ctx && ctx->mcache, BT_ERR_INVALID_ARG, "bt_match_cache_forget_frame: call bt_match_cache_reserve first");
-	MatchCache* c = ctx->mcache.get();
+	MatchCache* c;
+	BT_TRY(state_of(ctx, &bt_ctx::mcache, "bt_match_cache_forget_frame", "bt_match_cache_reserve", &c));
 	for (auto it = c->recs.begin(); it != c->recs.end();) {
 		if (it->first.first == frame_id || it->first.second == frame_id) { c->live -= it->second.n; it = c->recs.erase(it); }
 		else ++it;

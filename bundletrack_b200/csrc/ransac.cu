@@ -219,6 +219,7 @@ __global__ void __launch_bounds__(256) k_ransac_inliers(const RansacPair* __rest
 }
 
 struct RansacState {
+	bool ready = false;
 	int max_pairs = 0, max_pts = 0, max_trials = 0;
 	DevBuf pairs, table, poses, good, best, best_trial;
 	UploadBuf h_pairs;
@@ -231,7 +232,7 @@ void StateDeleter::operator()(RansacState* r) const { delete r; }
 int ransac_run_device(bt_ctx* ctx, const RansacPair* d_pairs, int n_pairs, int n_trials, float dist_thresh, uint64_t seed,
                       int32_t* inlier_ids_out, int32_t* n_inliers_out, cudaStream_t stream) {
 	RansacState* r = ctx->ransac.get();
-	BT_REQUIRE(r, BT_ERR_INVALID_ARG, "ransac: call bt_ransac_reserve first");
+	BT_REQUIRE(r && r->ready, BT_ERR_INVALID_ARG, "ransac: call bt_ransac_reserve (successfully) first");
 	BT_REQUIRE(n_pairs <= r->max_pairs && n_trials <= r->max_trials && n_trials > 0, BT_ERR_CAPACITY, "ransac: %d pairs / %d trials exceed the reserved %d / %d", n_pairs, n_trials, r->max_pairs, r->max_trials);
 	if (r->table_seed != seed || r->table_trials < n_trials) {
 		k_ransac_table<<<(r->max_trials + 255) / 256, 256, 0, stream>>>(r->table.as<float>(), r->max_trials, (unsigned long long)seed);
@@ -253,10 +254,8 @@ using namespace bt;
 
 extern "C" int bt_ransac_reserve(bt_ctx* ctx, int max_pairs, int max_pts, int max_trials) {
 	BT_REQUIRE(ctx && max_pairs > 0 && max_pts > 0 && max_trials > 0, BT_ERR_INVALID_ARG, "bt_ransac_reserve: bad arguments");
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->ransac) ctx->ransac.reset(new RansacState());
-	RansacState* r = ctx->ransac.get();
-	r->max_pairs = max_pairs; r->max_pts = max_pts; r->max_trials = max_trials;
+	RansacState* r;
+	BT_TRY(take_state(ctx, &bt_ctx::ransac, &r));
 	BT_TRY(r->pairs.alloc(sizeof(RansacPair) * max_pairs));
 	BT_TRY(r->table.alloc(sizeof(float) * 3 * max_trials));
 	BT_TRY(r->poses.alloc(sizeof(float) * 12 * (size_t)max_pairs * max_trials));
@@ -265,16 +264,17 @@ extern "C" int bt_ransac_reserve(bt_ctx* ctx, int max_pairs, int max_pts, int ma
 	BT_TRY(r->best_trial.alloc(sizeof(int32_t) * max_pairs));
 	BT_TRY(r->h_pairs.reserve(sizeof(RansacPair) * max_pairs));
 	r->table_seed = ~0ull; r->table_trials = 0;
+	r->max_pairs = max_pairs; r->max_pts = max_pts; r->max_trials = max_trials;
+	r->ready = true;
 	return BT_OK;
 }
 
 extern "C" int bt_ransac_pairs(bt_ctx* ctx, int n_pairs, const float* const* ptsA, const float* const* ptsB, const int* n_pts, int n_trials, float dist_thresh,
                                uint64_t seed, int32_t* inlier_ids_out, int32_t* n_inliers_out, void* stream_) {
-	BT_REQUIRE(ctx && ctx->ransac, BT_ERR_INVALID_ARG, "bt_ransac_pairs: call bt_ransac_reserve first");
+	RansacState* r;
+	BT_TRY(state_of(ctx, &bt_ctx::ransac, "bt_ransac_pairs", "bt_ransac_reserve", &r));
 	BT_REQUIRE(ptsA && ptsB && n_pts && inlier_ids_out && n_inliers_out && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_ransac_pairs: NULL argument");
-	RansacState* r = ctx->ransac.get();
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_REQUIRE(n_pairs <= r->max_pairs, BT_ERR_CAPACITY, "bt_ransac_pairs: %d pairs > reserved %d", n_pairs, r->max_pairs);
 	RansacPair* hp;
 	BT_TRY(r->h_pairs.acquire(0, &hp));
@@ -291,8 +291,8 @@ extern "C" int bt_ransac_pairs(bt_ctx* ctx, int n_pairs, const float* const* pts
 
 // Debug/parity aid: the 3 uniforms per trial the sampler uses (seed as in bt_ransac_pairs), and the winning trial ids of the last call.
 extern "C" int bt_ransac_debug(bt_ctx* ctx, float* u3_out, int n_trials, int32_t* best_trial_out, int n_pairs) {
-	BT_REQUIRE(ctx && ctx->ransac, BT_ERR_INVALID_ARG, "bt_ransac_debug: call bt_ransac_reserve first");
-	RansacState* r = ctx->ransac.get();
+	RansacState* r;
+	BT_TRY(state_of(ctx, &bt_ctx::ransac, "bt_ransac_debug", "bt_ransac_reserve", &r));
 	BT_CUDA(cudaDeviceSynchronize());
 	if (u3_out) BT_CUDA(cudaMemcpy(u3_out, r->table.p, sizeof(float) * 3 * std::min(n_trials, r->table_trials), cudaMemcpyDeviceToHost));
 	if (best_trial_out) BT_CUDA(cudaMemcpy(best_trial_out, r->best_trial.p, sizeof(int32_t) * std::min(n_pairs, r->max_pairs), cudaMemcpyDeviceToHost));

@@ -1627,6 +1627,7 @@ static StageLayout stage_layout(int n_windows, size_t F, size_t C, int max_frame
 }
 
 struct SolverState {
+	bool ready = false;
 	bt_solver_limits lim{};
 	int npix_max = 0, max_pairs = 0, max_frames_total = 0, max_tiles = 0, max_groups = 0;
 	DevBuf blk_cnt, grp_sums, stage_buf[2], texel, src, nsrc, x, T, pose_out, tiles, scalars, partial, tiles_done, iter_done, pair_tile0, pair_ntile, dbgJ, dbgR, dbgC, dbgS, prof;
@@ -1637,7 +1638,7 @@ struct SolverState {
 	UploadBuf c_htables[2];              // two pinned table blocks, used alternately: a store only waits for the upload of the store before last,
 	                                     // so back-to-back stores (one new frame per window per step) never stall the host behind the GPU
 	int c_flip = 0;
-	int c_capacity = 0, c_npix = 0;
+	int c_capacity = 0, c_npix = 0;      // (c_capacity 0 until bt_frame_cache_reserve completes)
 	float c_downscale = 0.f;
 	std::vector<CacheMeta> c_meta;
 	int prof_cap = 0;
@@ -1674,60 +1675,57 @@ struct SolverState {
 };
 void StateDeleter::operator()(SolverState* s) const { delete s; }
 
-static int reserve_impl(bt_ctx* ctx, const bt_solver_limits* lim) {
-	if (!ctx->solver) ctx->solver.reset(new SolverState());
-	SolverState* s = ctx->solver.get();
-	BT_REQUIRE(lim->max_windows > 0 && lim->max_frames >= 2 && lim->max_frames <= kMaxFrames && lim->max_corr >= 0 && lim->H > 0 && lim->W > 0 && lim->image_downscale >= 1.0f,
-	           BT_ERR_INVALID_ARG, "bt_solver_reserve: bad limits (max_frames must be 2..%d)", kMaxFrames);
-	s->lim = *lim;
-	{ const char* e = getenv("BT_SOLVE_CHUNK"); const int v = e ? atoi(e) : 0; s->force_chunk = (v >= 256 && v <= 16384) ? (v + 255) / 256 * 256 : 0; }
-	const int w = (int)(lim->W / lim->image_downscale), h = (int)(lim->H / lim->image_downscale);
-	s->npix_max = w * h;
-	const int F = lim->max_windows * lim->max_frames;
-	s->max_frames_total = F;
-	s->max_pairs = lim->max_frames * (lim->max_frames - 1);   // both directions allowed in custom lists
-	s->max_groups = lim->max_frames * lim->max_frames;
-	const int min_chunk = 256;   // worst case: every pixel valid at the smallest chunk the scheduler ever picks
-	s->max_tiles = lim->max_windows * (lim->max_frames * (lim->max_frames - 1) / 2) * ((s->npix_max + min_chunk - 1) / min_chunk + 1) + kSparseTiles * lim->max_windows;
-	{   // worst case over every window count <= max_windows (the table offsets grow with the count, so the maximum is at max_windows)
-		const StageLayout L = stage_layout(lim->max_windows, (size_t)F, (size_t)lim->max_corr * lim->max_windows, lim->max_frames, (size_t)s->max_groups, (size_t)s->max_pairs);
-		BT_TRY(s->stage_buf[0].alloc(L.total)); BT_TRY(s->stage_buf[1].alloc(L.total));
-	}
-	BT_TRY(s->texel.alloc(sizeof(float4) * (size_t)s->npix_max * F));
-	BT_TRY(s->src.alloc(sizeof(float4) * 2 * (size_t)s->npix_max * F));
-	BT_TRY(s->nsrc.alloc(sizeof(int) * F));
-	BT_TRY(s->grp_sums.alloc(sizeof(float) * kGrpVals * (size_t)s->max_groups * lim->max_windows));
-	BT_TRY(s->blk_cnt.alloc(sizeof(int) * (size_t)F * ((s->npix_max + 1023) / 1024)));
-	BT_TRY(s->x.alloc(sizeof(float) * 6 * F)); BT_TRY(s->T.alloc(sizeof(float) * 12 * F)); BT_TRY(s->pose_out.alloc(sizeof(float) * 16 * F));
-	BT_TRY(s->pair_tile0.alloc(sizeof(int) * (size_t)s->max_pairs * lim->max_windows));
-	BT_TRY(s->pair_ntile.alloc(sizeof(int) * (size_t)s->max_pairs * lim->max_windows));
-	BT_TRY(s->tiles.alloc(sizeof(Tile) * (size_t)s->max_tiles));
-	BT_TRY(s->partial.alloc(sizeof(float) * kTileVals * (size_t)s->max_tiles));
-	BT_TRY(s->scalars.alloc(64));
-	BT_CUDA(cudaMemset(s->scalars.p, 0, 64));
-	BT_TRY(s->tiles_done.alloc(sizeof(int) * lim->max_windows)); BT_TRY(s->iter_done.alloc(sizeof(int) * lim->max_windows));
-	return BT_OK;
-}
-
 }  // namespace bt
 
 using namespace bt;
 
 extern "C" int bt_solver_reserve(bt_ctx* ctx, const bt_solver_limits* lim) {
 	BT_REQUIRE(ctx && lim, BT_ERR_INVALID_ARG, "bt_solver_reserve: NULL argument");
-	BT_CUDA(cudaSetDevice(ctx->device));
-	return reserve_impl(ctx, lim);
+	BT_REQUIRE(lim->max_windows > 0 && lim->max_frames >= 2 && lim->max_frames <= kMaxFrames && lim->max_corr >= 0 && lim->H > 0 && lim->W > 0 && lim->image_downscale >= 1.0f,
+	           BT_ERR_INVALID_ARG, "bt_solver_reserve: bad limits (max_frames must be 2..%d)", kMaxFrames);
+	SolverState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::solver, &s));
+	{ const char* e = getenv("BT_SOLVE_CHUNK"); const int v = e ? atoi(e) : 0; s->force_chunk = (v >= 256 && v <= 16384) ? (v + 255) / 256 * 256 : 0; }
+	const int w = (int)(lim->W / lim->image_downscale), h = (int)(lim->H / lim->image_downscale);
+	const int npix_max = w * h;
+	const int F = lim->max_windows * lim->max_frames;
+	const int max_pairs = lim->max_frames * (lim->max_frames - 1);   // both directions allowed in custom lists
+	const int max_groups = lim->max_frames * lim->max_frames;
+	const int min_chunk = 256;   // worst case: every pixel valid at the smallest chunk the scheduler ever picks
+	const int max_tiles = lim->max_windows * (lim->max_frames * (lim->max_frames - 1) / 2) * ((npix_max + min_chunk - 1) / min_chunk + 1) + kSparseTiles * lim->max_windows;
+	{   // worst case over every window count <= max_windows (the table offsets grow with the count, so the maximum is at max_windows)
+		const StageLayout L = stage_layout(lim->max_windows, (size_t)F, (size_t)lim->max_corr * lim->max_windows, lim->max_frames, (size_t)max_groups, (size_t)max_pairs);
+		BT_TRY(s->stage_buf[0].alloc(L.total)); BT_TRY(s->stage_buf[1].alloc(L.total));
+	}
+	BT_TRY(s->texel.alloc(sizeof(float4) * (size_t)npix_max * F));
+	BT_TRY(s->src.alloc(sizeof(float4) * 2 * (size_t)npix_max * F));
+	BT_TRY(s->nsrc.alloc(sizeof(int) * F));
+	BT_TRY(s->grp_sums.alloc(sizeof(float) * kGrpVals * (size_t)max_groups * lim->max_windows));
+	BT_TRY(s->blk_cnt.alloc(sizeof(int) * (size_t)F * ((npix_max + 1023) / 1024)));
+	BT_TRY(s->x.alloc(sizeof(float) * 6 * F)); BT_TRY(s->T.alloc(sizeof(float) * 12 * F)); BT_TRY(s->pose_out.alloc(sizeof(float) * 16 * F));
+	BT_TRY(s->pair_tile0.alloc(sizeof(int) * (size_t)max_pairs * lim->max_windows));
+	BT_TRY(s->pair_ntile.alloc(sizeof(int) * (size_t)max_pairs * lim->max_windows));
+	BT_TRY(s->tiles.alloc(sizeof(Tile) * (size_t)max_tiles));
+	BT_TRY(s->partial.alloc(sizeof(float) * kTileVals * (size_t)max_tiles));
+	BT_TRY(s->scalars.alloc(64));
+	BT_CUDA(cudaMemset(s->scalars.p, 0, 64));
+	BT_TRY(s->tiles_done.alloc(sizeof(int) * lim->max_windows)); BT_TRY(s->iter_done.alloc(sizeof(int) * lim->max_windows));
+	s->lim = *lim;
+	s->npix_max = npix_max; s->max_frames_total = F; s->max_pairs = max_pairs; s->max_groups = max_groups; s->max_tiles = max_tiles;
+	s->ready = true;
+	return BT_OK;
 }
 
 extern "C" int bt_solve_enable_debug(bt_ctx* ctx, int on) {
-	BT_REQUIRE(ctx && ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_enable_debug: call bt_solver_reserve first");
-	ctx->solver->debug = on != 0;
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_enable_debug", "bt_solver_reserve", &s));
+	s->debug = on != 0;
 	return BT_OK;
 }
 
 extern "C" int bt_solve_enable_timing(bt_ctx* ctx, int on) {
-	BT_REQUIRE(ctx && ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_enable_timing: call bt_solver_reserve first");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_enable_timing", "bt_solver_reserve", &s));
 	if (on && !s->tstamp.p) { BT_TRY(s->tstamp.alloc(4 * sizeof(long long))); BT_CUDA(cudaMemset(s->tstamp.p, 0, 4 * sizeof(long long))); }
 	s->timing = on != 0;
 	return BT_OK;
@@ -1737,9 +1735,9 @@ extern "C" int bt_solve_enable_timing(bt_ctx* ctx, int on) {
 // first prep kernel's start to the tile plan's end, gap = from there to k_solve's start, solve = k_solve's start to its last CTA's end.
 // Synchronises the device.
 extern "C" int bt_solve_get_timing(bt_ctx* ctx, float* ms3) {
-	BT_REQUIRE(ctx && ctx->solver && ctx->solver->timing && ms3, BT_ERR_INVALID_ARG, "bt_solve_get_timing: timing not enabled");
-	SolverState* s = ctx->solver.get();
-	BT_CUDA(cudaSetDevice(ctx->device));
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_get_timing", "bt_solver_reserve", &s));
+	BT_REQUIRE(s->timing && ms3, BT_ERR_INVALID_ARG, "bt_solve_get_timing: timing not enabled");
 	BT_CUDA(cudaDeviceSynchronize());
 	long long t[4];
 	BT_CUDA(cudaMemcpy(t, s->tstamp.p, sizeof t, cudaMemcpyDeviceToHost));
@@ -2001,11 +1999,10 @@ private:
 // overlapping the kernel.  k_solve waits on the last copy's event.
 static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, const bt_solver_params* params,
                       const float* poses_in, void* stream_, bool early_prep) {
-	BT_REQUIRE(ctx && windows && params && poses_in, BT_ERR_INVALID_ARG, "bt_solve_stage: NULL argument");
-	BT_REQUIRE(ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_stage: call bt_solver_reserve first");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_stage", "bt_solver_reserve", &s));
+	BT_REQUIRE(windows && params && poses_in, BT_ERR_INVALID_ARG, "bt_solve_stage: NULL argument");
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_REQUIRE(n_windows > 0 && n_windows <= s->lim.max_windows, BT_ERR_CAPACITY, "bt_solve_stage: %d windows > reserved %d", n_windows, s->lim.max_windows);
 	BT_REQUIRE(params->num_iter_outer > 0 && params->num_iter_inner > 0 && params->image_downscale == s->lim.image_downscale, BT_ERR_INVALID_ARG,
 	           "bt_solve_stage: iteration counts must be positive and image_downscale must equal the reserved value");
@@ -2157,10 +2154,10 @@ static int launch_prep(bt_ctx* ctx, cudaStream_t stream) {
 }
 
 extern "C" int bt_solve_run(bt_ctx* ctx, void* stream_) {
-	BT_REQUIRE(ctx && ctx->solver && ctx->solver->staged, BT_ERR_INVALID_ARG, "bt_solve_run: nothing staged");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_run", "bt_solver_reserve", &s));
+	BT_REQUIRE(s->staged, BT_ERR_INVALID_ARG, "bt_solve_run: nothing staged");
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_TRY(ensure_occupancy(ctx));
 	SolveArgs a = make_args(ctx);
 	if (s->debug) {
@@ -2197,8 +2194,9 @@ static int take_poses(const PinnedBuf& h, int frames, float* poses_out, const ch
 }
 
 extern "C" int bt_solve_fetch(bt_ctx* ctx, float* poses_out, void* stream_) {
-	BT_REQUIRE(ctx && ctx->solver && ctx->solver->staged && poses_out, BT_ERR_INVALID_ARG, "bt_solve_fetch: nothing staged / NULL output");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_fetch", "bt_solver_reserve", &s));
+	BT_REQUIRE(s->staged && poses_out, BT_ERR_INVALID_ARG, "bt_solve_fetch: nothing staged / NULL output");
 	BT_TRY(queue_pose_download(s, s->h_poses, (cudaStream_t)stream_));
 	BT_CUDA(cudaStreamSynchronize((cudaStream_t)stream_));
 	return take_poses(s->h_poses, s->frames_total, poses_out, "bt_solve_fetch");
@@ -2221,8 +2219,8 @@ extern "C" int bt_solve_windows(bt_ctx* ctx, int n_windows, const bt_window* win
 // OLDEST batch begun and hands its poses out.  Up to two batches may be in flight, so the host side of batch k+1 (tables, grouping,
 // uploads, launches) overlaps the GPU side of batch k; everything is ordered on `stream`.
 extern "C" int bt_solve_windows_begin(bt_ctx* ctx, int n_windows, const bt_window* windows, const bt_solver_params* params, const float* poses_in, void* stream_) {
-	BT_REQUIRE(ctx && ctx->solver, BT_ERR_INVALID_ARG, "bt_solve_windows_begin: call bt_solver_reserve first");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_windows_begin", "bt_solver_reserve", &s));
 	const int slot = s->pipe_head;
 	BT_REQUIRE(!s->pipe_pending[slot], BT_ERR_INVALID_ARG, "bt_solve_windows_begin: two batches are already in flight - call bt_solve_windows_end first");
 	BT_TRY(stage_impl(ctx, n_windows, windows, params, poses_in, stream_, true));
@@ -2233,8 +2231,9 @@ extern "C" int bt_solve_windows_begin(bt_ctx* ctx, int n_windows, const bt_windo
 	return BT_OK;
 }
 extern "C" int bt_solve_windows_end(bt_ctx* ctx, float* poses_out) {
-	BT_REQUIRE(ctx && ctx->solver && poses_out, BT_ERR_INVALID_ARG, "bt_solve_windows_end: NULL argument");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_windows_end", "bt_solver_reserve", &s));
+	BT_REQUIRE(poses_out, BT_ERR_INVALID_ARG, "bt_solve_windows_end: NULL argument");
 	const int slot = s->pipe_tail;
 	BT_REQUIRE(s->pipe_pending[slot], BT_ERR_INVALID_ARG, "bt_solve_windows_end: no batch in flight");
 	BT_CUDA(cudaEventSynchronize(s->ev_pipe[slot]));
@@ -2245,18 +2244,20 @@ extern "C" int bt_solve_windows_end(bt_ctx* ctx, float* poses_out) {
 // Host time of the last bt_solve_windows call, microseconds: {window tables + first upload, frame-prep launch, correspondence scan +
 // staging + uploads, k_solve launch, pose download + wait for the GPU, whole call}.
 extern "C" int bt_solve_get_host_timing(bt_ctx* ctx, double* us6) {
-	BT_REQUIRE(ctx && ctx->solver && us6, BT_ERR_INVALID_ARG, "bt_solve_get_host_timing: NULL argument");
-	for (int k = 0; k < 6; k++) us6[k] = ctx->solver->host_us[k];
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_get_host_timing", "bt_solver_reserve", &s));
+	BT_REQUIRE(us6, BT_ERR_INVALID_ARG, "bt_solve_get_host_timing: NULL argument");
+	for (int k = 0; k < 6; k++) us6[k] = s->host_us[k];
 	return BT_OK;
 }
 
 extern "C" int bt_frame_cache_reserve(bt_ctx* ctx, int capacity, int H, int W, float image_downscale) {
-	BT_REQUIRE(ctx && ctx->solver, BT_ERR_INVALID_ARG, "bt_frame_cache_reserve: call bt_solver_reserve first");
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_frame_cache_reserve", "bt_solver_reserve", &s));
 	BT_REQUIRE(capacity > 0 && H > 0 && W > 0 && image_downscale >= 1.0f, BT_ERR_INVALID_ARG, "bt_frame_cache_reserve: bad arguments");
-	SolverState* s = ctx->solver.get();
-	BT_CUDA(cudaSetDevice(ctx->device));
 	const int w = (int)(W / image_downscale), h = (int)(H / image_downscale);
 	BT_REQUIRE(w >= 2 && h >= 2, BT_ERR_INVALID_ARG, "bt_frame_cache_reserve: image too small");
+	s->c_capacity = 0;
 	BT_TRY(s->c_texel.alloc(sizeof(float4) * (size_t)w * h * capacity));
 	BT_TRY(s->c_src.alloc(sizeof(float4) * 2 * (size_t)w * h * capacity));
 	BT_TRY(s->c_nsrc.alloc(sizeof(int) * (size_t)capacity));
@@ -2268,14 +2269,14 @@ extern "C" int bt_frame_cache_reserve(bt_ctx* ctx, int capacity, int H, int W, f
 
 extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* slots, const float* const* depth_dev, const float* const* normal_dev,
                                     int H, int W, float fx, float fy, float cx, float cy, float depth_min, float depth_max, void* stream_) {
-	BT_REQUIRE(ctx && ctx->solver && slots && depth_dev && normal_dev, BT_ERR_INVALID_ARG, "bt_frame_cache_store: NULL argument");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_frame_cache_store", "bt_solver_reserve", &s));
+	BT_REQUIRE(slots && depth_dev && normal_dev, BT_ERR_INVALID_ARG, "bt_frame_cache_store: NULL argument");
 	BT_REQUIRE(s->c_capacity > 0, BT_ERR_INVALID_ARG, "bt_frame_cache_store: call bt_frame_cache_reserve first");
 	BT_REQUIRE(n_frames > 0 && n_frames <= s->c_capacity, BT_ERR_CAPACITY, "bt_frame_cache_store: %d frames > capacity %d", n_frames, s->c_capacity);
 	const FrameGeom geom = frame_geom(H, W, fx, fy, cx, cy, s->c_downscale);
 	BT_REQUIRE(H > 0 && W > 0 && geom.w >= 2 && geom.h >= 2 && geom.w * geom.h <= s->c_npix, BT_ERR_CAPACITY, "bt_frame_cache_store: image %dx%d does not fit the reserved cache", W, H);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	for (int f = 0; f < n_frames; f++) {
 		BT_REQUIRE(slots[f] >= 0 && slots[f] < s->c_capacity, BT_ERR_INVALID_ARG, "bt_frame_cache_store: slot %d out of range [0,%d)", slots[f], s->c_capacity);
 		BT_REQUIRE(depth_dev[f] && normal_dev[f], BT_ERR_INVALID_ARG, "bt_frame_cache_store: frame %d has a NULL map", f);
@@ -2318,8 +2319,9 @@ extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* sl
 }
 
 extern "C" int bt_solve_get_stats(bt_ctx* ctx, bt_solve_stats* out) {
-	BT_REQUIRE(ctx && ctx->solver && out, BT_ERR_INVALID_ARG, "bt_solve_get_stats: NULL argument");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_get_stats", "bt_solver_reserve", &s));
+	BT_REQUIRE(out, BT_ERR_INVALID_ARG, "bt_solve_get_stats: NULL argument");
 	char h[32];
 	BT_CUDA(cudaMemcpy(h, s->scalars.p, 32, cudaMemcpyDeviceToHost));
 	out->n_windows = s->n_windows;
@@ -2330,15 +2332,17 @@ extern "C" int bt_solve_get_stats(bt_ctx* ctx, bt_solve_stats* out) {
 }
 
 extern "C" int bt_solve_enable_profile(bt_ctx* ctx, int max_records) {
-	BT_REQUIRE(ctx && ctx->solver && max_records >= 0, BT_ERR_INVALID_ARG, "bt_solve_enable_profile: call bt_solver_reserve first");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_enable_profile", "bt_solver_reserve", &s));
+	BT_REQUIRE(max_records >= 0, BT_ERR_INVALID_ARG, "bt_solve_enable_profile: max_records %d < 0", max_records);
 	if (max_records > 0) BT_TRY(s->prof.alloc(8 + (size_t)max_records * 96));
 	s->prof_cap = max_records;
 	return BT_OK;
 }
 extern "C" int bt_solve_get_profile(bt_ctx* ctx, long long* out, int max_records) {
-	BT_REQUIRE(ctx && ctx->solver && ctx->solver->prof_cap > 0 && out, BT_ERR_INVALID_ARG, "bt_solve_get_profile: profiling not enabled");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_get_profile", "bt_solver_reserve", &s));
+	BT_REQUIRE(s->prof_cap > 0 && out, BT_ERR_INVALID_ARG, "bt_solve_get_profile: profiling not enabled");
 	BT_CUDA(cudaDeviceSynchronize());
 	long long n = 0;
 	BT_CUDA(cudaMemcpy(&n, s->prof.p, 8, cudaMemcpyDeviceToHost));
@@ -2349,8 +2353,9 @@ extern "C" int bt_solve_get_profile(bt_ctx* ctx, long long* out, int max_records
 }
 
 extern "C" int bt_solve_debug_counts(bt_ctx* ctx, int w, int n_pairs, float* counts_out) {
-	BT_REQUIRE(ctx && ctx->solver && ctx->solver->debug && ctx->solver->staged && counts_out, BT_ERR_INVALID_ARG, "bt_solve_debug_counts: debug not enabled / nothing run");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_debug_counts", "bt_solver_reserve", &s));
+	BT_REQUIRE(s->debug && s->staged && counts_out, BT_ERR_INVALID_ARG, "bt_solve_debug_counts: debug not enabled / nothing run");
 	BT_REQUIRE(w >= 0 && w < s->n_windows && n_pairs >= 0 && n_pairs <= s->max_pairs, BT_ERR_INVALID_ARG, "bt_solve_debug_counts: bad index");
 	BT_CUDA(cudaDeviceSynchronize());
 	BT_CUDA(cudaMemcpy(counts_out, s->dbgC.as<float>() + (size_t)w * s->max_pairs, sizeof(float) * n_pairs, cudaMemcpyDeviceToHost));
@@ -2358,8 +2363,9 @@ extern "C" int bt_solve_debug_counts(bt_ctx* ctx, int w, int n_pairs, float* cou
 }
 
 extern "C" int bt_solve_debug_dense(bt_ctx* ctx, int w, float* JtJ_out, float* Jtr_out) {
-	BT_REQUIRE(ctx && ctx->solver && ctx->solver->debug && ctx->solver->staged, BT_ERR_INVALID_ARG, "bt_solve_debug_dense: debug not enabled / nothing run");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_debug_dense", "bt_solver_reserve", &s));
+	BT_REQUIRE(s->debug && s->staged, BT_ERR_INVALID_ARG, "bt_solve_debug_dense: debug not enabled / nothing run");
 	BT_REQUIRE(w >= 0 && w < s->n_windows, BT_ERR_INVALID_ARG, "bt_solve_debug_dense: window %d out of range", w);
 	const int st = 6 * s->lim.max_frames, dim = 6 * s->n_frames[w];
 	BT_CUDA(cudaDeviceSynchronize());
@@ -2369,8 +2375,9 @@ extern "C" int bt_solve_debug_dense(bt_ctx* ctx, int w, float* JtJ_out, float* J
 }
 
 extern "C" int bt_solve_debug_system(bt_ctx* ctx, int w, int n_frames, float* A_out, float* rhs_out, float* minv_out, float* delta_out) {
-	BT_REQUIRE(ctx && ctx->solver && ctx->solver->debug && ctx->solver->staged, BT_ERR_INVALID_ARG, "bt_solve_debug_system: debug not enabled / nothing run");
-	SolverState* s = ctx->solver.get();
+	SolverState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::solver, "bt_solve_debug_system", "bt_solver_reserve", &s));
+	BT_REQUIRE(s->debug && s->staged, BT_ERR_INVALID_ARG, "bt_solve_debug_system: debug not enabled / nothing run");
 	BT_REQUIRE(w >= 0 && w < s->n_windows, BT_ERR_INVALID_ARG, "bt_solve_debug_system: window %d out of range", w);
 	BT_REQUIRE(n_frames == s->n_frames[w], BT_ERR_INVALID_ARG, "bt_solve_debug_system: window %d has %d frames, the outputs are sized for %d", w, s->n_frames[w], n_frames);
 	const int st = 6 * (s->lim.max_frames - 1), dim = 6 * (s->n_frames[w] - 1);

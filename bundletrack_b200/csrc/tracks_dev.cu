@@ -357,6 +357,7 @@ __global__ void __launch_bounds__(256) k_trk_forget(TrkTable t, int slot) {
 }
 
 struct TracksDev {
+	bool ready = false;
 	TrkTable t{};
 	int list_cap = 0, scap = 0;
 	DevBuf keys, hkey, hidx, n_keys, obs, n_obs, last, free_pts, ctr, shk, smn, smx, ent;
@@ -367,6 +368,11 @@ struct TracksDev {
 };
 
 void StateDeleter::operator()(TracksDev* d) const { delete d; }
+
+int tracks_state(bt_ctx* ctx, const char* who) {
+	TracksDev* d;
+	return state_of(ctx, &bt_ctx::tracks, who, "bt_tracks_dev_reserve", &d);
+}
 
 int tracks_slot(bt_ctx* ctx, int frame_id, bool create, int* slot) {
 	TracksDev* d = ctx->tracks.get();
@@ -413,22 +419,21 @@ int tracks_launch_propagate(bt_ctx* ctx, int slot_a, int slot_b, const float4* e
 using namespace bt;
 
 static int tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_per_frame, int max_points) {
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->tracks) ctx->tracks.reset(new TracksDev());
-	TracksDev* d = ctx->tracks.get();
+	TracksDev* d;
+	BT_TRY(take_state(ctx, &bt_ctx::tracks, &d));
 	int hcap = 64;
 	while (hcap < 2 * max_keys_per_frame) hcap <<= 1;
-	d->list_cap = 4 * max_keys_per_frame;       // one pair's list: mutual matches of both directions plus propagated ones, duplicates kept
-	d->scap = 64;
-	while (d->scap < 2 * d->list_cap) d->scap <<= 1;
+	const int list_cap = 4 * max_keys_per_frame;       // one pair's list: mutual matches of both directions plus propagated ones, duplicates kept
+	int scap = 64;
+	while (scap < 2 * list_cap) scap <<= 1;
 	const size_t F = (size_t)max_frames, K = (size_t)max_keys_per_frame, Pn = (size_t)max_points;
 	BT_TRY(d->keys.alloc(sizeof(int4) * F * K)); BT_TRY(d->hkey.alloc(sizeof(unsigned long long) * F * hcap)); BT_TRY(d->hidx.alloc(sizeof(int) * F * hcap));
 	BT_TRY(d->n_keys.alloc(sizeof(int) * F));
 	BT_TRY(d->obs.alloc(sizeof(float2) * Pn * F)); BT_TRY(d->n_obs.alloc(sizeof(int) * Pn)); BT_TRY(d->last.alloc(sizeof(unsigned long long) * Pn));
 	BT_TRY(d->free_pts.alloc(sizeof(int) * Pn));
 	BT_TRY(d->ctr.alloc(sizeof(int) * C_N));
-	BT_TRY(d->shk.alloc(sizeof(unsigned long long) * 2 * d->scap)); BT_TRY(d->smn.alloc(sizeof(int) * 2 * d->scap)); BT_TRY(d->smx.alloc(sizeof(int) * d->scap));
-	BT_TRY(d->ent.alloc(sizeof(TrkEnt) * d->list_cap));
+	BT_TRY(d->shk.alloc(sizeof(unsigned long long) * 2 * scap)); BT_TRY(d->smn.alloc(sizeof(int) * 2 * scap)); BT_TRY(d->smx.alloc(sizeof(int) * scap));
+	BT_TRY(d->ent.alloc(sizeof(TrkEnt) * list_cap));
 	BT_CUDA(cudaMemset(d->hkey.p, 0xff, sizeof(unsigned long long) * F * hcap));
 	BT_CUDA(cudaMemset(d->n_keys.p, 0, sizeof(int) * F));
 	BT_CUDA(cudaMemset(d->obs.p, 0xff, sizeof(float2) * Pn * F));        // every observation empty
@@ -446,8 +451,10 @@ static int tracks_dev_reserve(bt_ctx* ctx, int max_frames, int max_keys_per_fram
 	d->slot_of.clear(); d->free_slots.clear();
 	for (int f = max_frames - 1; f >= 0; f--) d->free_slots.push_back(f);
 	d->epoch = 0;
+	d->list_cap = list_cap; d->scap = scap;
 	d->prop_smem = (size_t)t.sort_cap * (sizeof(unsigned long long) + 2 * sizeof(int) + 1);
 	BT_CUDA(cudaFuncSetAttribute(k_trk_propagate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d->prop_smem));
+	d->ready = true;
 	return BT_OK;
 }
 
@@ -465,12 +472,12 @@ extern "C" int bt_tracks_dev_reserve_ex(bt_ctx* ctx, int max_frames, int max_key
 }
 
 extern "C" int bt_tracks_dev_update_pair(bt_ctx* ctx, int frame_a, int frame_b, const float* uv_dev, const int32_t* n_dev, int uv_capacity, void* stream_) {
-	BT_REQUIRE(ctx && ctx->tracks, BT_ERR_INVALID_ARG, "bt_tracks_dev_update_pair: call bt_tracks_dev_reserve first");
+	TracksDev* d;
+	BT_TRY(state_of(ctx, &bt_ctx::tracks, "bt_tracks_dev_update_pair", "bt_tracks_dev_reserve", &d));
 	BT_REQUIRE(n_dev && uv_capacity >= 0 && (uv_capacity == 0 || uv_dev), BT_ERR_INVALID_ARG, "bt_tracks_dev_update_pair: bad arguments");
 	BT_REQUIRE(frame_a > frame_b, BT_ERR_INVALID_ARG, "bt_tracks_dev_update_pair: frame A must be the newer frame (id %d <= %d)", frame_a, frame_b);
-	BT_CUDA(cudaSetDevice(ctx->device));
-	const bool need_a = !ctx->tracks->slot_of.count(frame_a), need_b = !ctx->tracks->slot_of.count(frame_b);
-	BT_REQUIRE(tracks_free_slots(ctx) >= (int)need_a + (int)need_b, BT_ERR_CAPACITY, "bt_tracks_dev_update_pair: more than %d frames alive", ctx->tracks->t.max_frames);
+	const bool need_a = !d->slot_of.count(frame_a), need_b = !d->slot_of.count(frame_b);
+	BT_REQUIRE(tracks_free_slots(ctx) >= (int)need_a + (int)need_b, BT_ERR_CAPACITY, "bt_tracks_dev_update_pair: more than %d frames alive", d->t.max_frames);
 	int sa, sb, rc;
 	if ((rc = tracks_slot(ctx, frame_a, true, &sa)) != BT_OK) return rc;
 	if ((rc = tracks_slot(ctx, frame_b, true, &sb)) != BT_OK) return rc;
@@ -480,11 +487,11 @@ extern "C" int bt_tracks_dev_update_pair(bt_ctx* ctx, int frame_a, int frame_b, 
 
 extern "C" int bt_tracks_dev_propagate(bt_ctx* ctx, int frame_a, int frame_b, const float* existing_uv_dev, int n_existing, float* out_uv_dev, int capacity,
                                        int32_t* n_out_dev, void* stream_) {
-	BT_REQUIRE(ctx && ctx->tracks, BT_ERR_INVALID_ARG, "bt_tracks_dev_propagate: call bt_tracks_dev_reserve first");
+	TracksDev* d;
+	BT_TRY(state_of(ctx, &bt_ctx::tracks, "bt_tracks_dev_propagate", "bt_tracks_dev_reserve", &d));
 	BT_REQUIRE(n_out_dev && n_existing >= 0 && (n_existing == 0 || existing_uv_dev) && capacity >= 0 && (capacity == 0 || out_uv_dev), BT_ERR_INVALID_ARG,
 	           "bt_tracks_dev_propagate: bad arguments");
 	BT_REQUIRE(frame_a > frame_b, BT_ERR_INVALID_ARG, "bt_tracks_dev_propagate: frame A must be the newer frame (id %d <= %d)", frame_a, frame_b);
-	BT_CUDA(cudaSetDevice(ctx->device));
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int sa, sb;
 	tracks_slot(ctx, frame_a, false, &sa);
@@ -498,11 +505,10 @@ extern "C" int bt_tracks_dev_propagate(bt_ctx* ctx, int frame_a, int frame_b, co
 }
 
 extern "C" int bt_tracks_dev_forget_frame(bt_ctx* ctx, int frame, void* stream_) {
-	BT_REQUIRE(ctx && ctx->tracks, BT_ERR_INVALID_ARG, "bt_tracks_dev_forget_frame: call bt_tracks_dev_reserve first");
-	TracksDev* d = ctx->tracks.get();
+	TracksDev* d;
+	BT_TRY(state_of(ctx, &bt_ctx::tracks, "bt_tracks_dev_forget_frame", "bt_tracks_dev_reserve", &d));
 	const auto it = d->slot_of.find(frame);
 	if (it == d->slot_of.end()) return BT_OK;
-	BT_CUDA(cudaSetDevice(ctx->device));
 	const int slot = it->second;
 	k_trk_forget<<<ctx->sm_count > 0 ? ctx->sm_count : 132, 256, 0, (cudaStream_t)stream_>>>(d->t, slot);
 	BT_CUDA(cudaGetLastError());
@@ -513,9 +519,9 @@ extern "C" int bt_tracks_dev_forget_frame(bt_ctx* ctx, int frame, void* stream_)
 
 // Synchronises `stream`.  BT_ERR_CAPACITY when an earlier call overflowed a capacity (that call changed nothing); the flag is cleared.
 extern "C" int bt_tracks_dev_stats(bt_ctx* ctx, int* n_points, int* n_observations, void* stream_) {
-	BT_REQUIRE(ctx && ctx->tracks && n_points && n_observations, BT_ERR_INVALID_ARG, "bt_tracks_dev_stats: call bt_tracks_dev_reserve first / NULL argument");
-	TracksDev* d = ctx->tracks.get();
-	BT_CUDA(cudaSetDevice(ctx->device));
+	TracksDev* d;
+	BT_TRY(state_of(ctx, &bt_ctx::tracks, "bt_tracks_dev_stats", "bt_tracks_dev_reserve", &d));
+	BT_REQUIRE(n_points && n_observations, BT_ERR_INVALID_ARG, "bt_tracks_dev_stats: NULL argument");
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int c[C_N];
 	BT_CUDA(cudaMemcpyAsync(c, d->ctr.p, sizeof(c), cudaMemcpyDeviceToHost, stream));

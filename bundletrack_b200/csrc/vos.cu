@@ -508,7 +508,7 @@ constexpr int N_STAGES = 3;     // backbone, propagation, mask
 struct VosState {
 	bt_vos_params p = {};
 	int H = 0, W = 0, Hd = 0, Wd = 0, slots = 0;
-	bool reserved = false;          // every buffer holds the sizes below
+	bool ready = false;
 	bool loaded = false;
 	int frame = -1;                 // frames seen since bt_vos_begin; -1 before it
 	int n_labels = 0;
@@ -566,14 +566,6 @@ int run_backbone(VosState* s, const uint8_t* colour, int slot, cudaStream_t st) 
 	return launch_conv(W, n.adjust, x, H, Wd, nullptr, false, s->feat.as<float>() + (size_t)slot * s->Hd * s->Wd * FEAT, ho, wo, st);
 }
 
-// rc of a call that needs a reserved, loaded state
-int vos_state(bt_ctx* ctx, const char* fn, VosState** out) {
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "%s: ctx is NULL", fn);
-	*out = ctx->vos.get();
-	BT_REQUIRE(*out && (*out)->reserved && (*out)->loaded, BT_ERR_INVALID_ARG, "%s: call bt_vos_reserve (successfully) and bt_vos_load_weights first", fn);
-	return BT_OK;
-}
-
 }  // namespace
 
 // run_video.py's sample_frames: frames 0..k-1 up to ref_num, then numpy's linspace(ref_start, ref_end, ref_num - 3) truncated to int
@@ -609,42 +601,37 @@ extern "C" int bt_vos_reserve(bt_ctx* ctx, const bt_vos_params* p, int H, int W)
 	           BT_ERR_INVALID_ARG, "bt_vos_reserve: sigma1 %g, sigma2 %g must be finite and positive, temperature %g finite", p->sigma1, p->sigma2,
 	           p->temperature);
 	BT_REQUIRE(H >= 8 && W >= 8 && H <= 4096 && W <= 4096, BT_ERR_INVALID_ARG, "bt_vos_reserve: size %d x %d outside [8, 4096]", H, W);
-	BT_CUDA(cudaSetDevice(ctx->device));
-	if (!ctx->vos) ctx->vos.reset(new VosState());
-	VosState* s = ctx->vos.get();
-	// a failed allocation below can leave a buffer freed or smaller than the new sizes: the state is unusable until a reserve succeeds
-	s->reserved = false;
-	s->p = *p;
-	s->H = H; s->W = W;
-	s->Hd = (H + 7) / 8; s->Wd = (W + 7) / 8;
-	s->slots = std::max(p->range + 5, p->ref_num + 1);
-	s->frame = -1;
-	s->net = net_layout();
-	const size_t HW = (size_t)s->Hd * s->Wd;
+	VosState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::vos, &s));
+	const int Hd = (H + 7) / 8, Wd = (W + 7) / 8, slots = std::max(p->range + 5, p->ref_num + 1);
+	const Net net = net_layout();
+	const size_t HW = (size_t)Hd * Wd;
 	const int H1 = conv_out(H, 7, 2), W1 = conv_out(W, 7, 2), H2 = conv_out(H1, 3, 2), W2 = conv_out(W1, 3, 2);
 	const size_t act = std::max({(size_t)H1 * W1 * 64, (size_t)H2 * W2 * 256, HW * 1024});
-	BT_TRY(s->w.alloc(sizeof(float) * s->net.total));
+	BT_TRY(s->w.alloc(sizeof(float) * net.total));
 	for (DevBuf& b : s->act) BT_TRY(b.alloc(sizeof(float) * act));
-	BT_TRY(s->feat.alloc(sizeof(float) * s->slots * HW * FEAT));
-	BT_TRY(s->label.alloc(sizeof(float) * s->slots * HW * MAX_LABELS));
+	BT_TRY(s->feat.alloc(sizeof(float) * slots * HW * FEAT));
+	BT_TRY(s->label.alloc(sizeof(float) * slots * HW * MAX_LABELS));
 	BT_TRY(s->part.alloc(sizeof(float) * p->ref_num * HW * (2 + MAX_LABELS)));
 	BT_TRY(s->pred.alloc(sizeof(float) * MAX_LABELS * HW));
 	BT_TRY(s->chan.alloc(sizeof(int32_t) * 512));
 	BT_TRY(s->present.alloc(sizeof(int32_t) * 256));
 	BT_CUDA(cudaFuncSetAttribute(k_vos_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CB_SMEM));
 	BT_CUDA(cudaFuncSetAttribute(k_vos_propagate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PB_SMEM));
-	s->reserved = true;
+	s->p = *p;
+	s->H = H; s->W = W; s->Hd = Hd; s->Wd = Wd; s->slots = slots;
+	s->net = net;
+	s->frame = -1;
+	s->ready = true;
 	return BT_OK;
 }
 
 extern "C" int bt_vos_load_weights(bt_ctx* ctx, const float* blob, size_t n_floats) {
-	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_vos_load_weights: ctx is NULL");
-	VosState* s = ctx->vos.get();
-	BT_REQUIRE(s && s->reserved, BT_ERR_INVALID_ARG, "bt_vos_load_weights: call bt_vos_reserve (successfully) first");
+	VosState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::vos, "bt_vos_load_weights", "bt_vos_reserve", &s));
 	BT_REQUIRE(blob, BT_ERR_INVALID_ARG, "bt_vos_load_weights: blob is NULL");
 	BT_REQUIRE(n_floats == s->net.total, BT_ERR_INVALID_ARG, "bt_vos_load_weights: %zu floats, the network has %zu", n_floats, s->net.total);
 	for (size_t i = 0; i < n_floats; i++) BT_REQUIRE(std::isfinite(blob[i]), BT_ERR_INVALID_ARG, "bt_vos_load_weights: float %zu is not finite", i);
-	BT_CUDA(cudaSetDevice(ctx->device));
 	BT_CUDA(cudaMemcpy(s->w.p, blob, sizeof(float) * n_floats, cudaMemcpyHostToDevice));
 	s->loaded = true;
 	return BT_OK;
@@ -652,9 +639,9 @@ extern "C" int bt_vos_load_weights(bt_ctx* ctx, const float* blob, size_t n_floa
 
 extern "C" int bt_vos_begin(bt_ctx* ctx, const uint8_t* colour_dev, const uint8_t* init_mask_dev, uint8_t* mask_out_dev, void* stream_) {
 	VosState* s;
-	BT_TRY(vos_state(ctx, "bt_vos_begin", &s));
+	BT_TRY(state_of(ctx, &bt_ctx::vos, "bt_vos_begin", "bt_vos_reserve", &s));
+	BT_REQUIRE(s->loaded, BT_ERR_INVALID_ARG, "bt_vos_begin: call bt_vos_load_weights first");
 	BT_REQUIRE(colour_dev && init_mask_dev && mask_out_dev, BT_ERR_INVALID_ARG, "bt_vos_begin: NULL pointer");
-	BT_CUDA(cudaSetDevice(ctx->device));
 	cudaStream_t st = (cudaStream_t)stream_;
 	const int n = s->H * s->W, HW = s->Hd * s->Wd;
 	// the mask's distinct values, read back once: value 0 -> channel 0 (kept when absent), the others in increasing order
@@ -691,11 +678,11 @@ extern "C" int bt_vos_begin(bt_ctx* ctx, const uint8_t* colour_dev, const uint8_
 
 extern "C" int bt_vos_next(bt_ctx* ctx, const uint8_t* colour_dev, uint8_t* mask_out_dev, void* stream_) {
 	VosState* s;
-	BT_TRY(vos_state(ctx, "bt_vos_next", &s));
+	BT_TRY(state_of(ctx, &bt_ctx::vos, "bt_vos_next", "bt_vos_reserve", &s));
+	BT_REQUIRE(s->loaded, BT_ERR_INVALID_ARG, "bt_vos_next: call bt_vos_load_weights first");
 	BT_REQUIRE(s->frame >= 0, BT_ERR_INVALID_ARG, "bt_vos_next: no sequence begun (bt_vos_begin)");
 	BT_REQUIRE(colour_dev && mask_out_dev, BT_ERR_INVALID_ARG, "bt_vos_next: NULL pointer");
 	BT_REQUIRE(s->frame < (1 << 30), BT_ERR_CAPACITY, "bt_vos_next: sequence too long");
-	BT_CUDA(cudaSetDevice(ctx->device));
 	cudaStream_t st = (cudaStream_t)stream_;
 	const int k = s->frame + 1, HW = s->Hd * s->Wd, slot = k % s->slots;
 	PropArgs a = {};
@@ -730,16 +717,17 @@ extern "C" int bt_vos_next(bt_ctx* ctx, const uint8_t* colour_dev, uint8_t* mask
 }
 
 extern "C" int bt_vos_enable_timing(bt_ctx* ctx, int on) {
-	BT_REQUIRE(ctx && ctx->vos, BT_ERR_INVALID_ARG, "bt_vos_enable_timing: call bt_vos_reserve first");
-	ctx->vos->timing = on != 0;
+	VosState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::vos, "bt_vos_enable_timing", "bt_vos_reserve", &s));
+	s->timing = on != 0;
 	return BT_OK;
 }
 
 extern "C" int bt_vos_get_timing(bt_ctx* ctx, float* ms3) {
-	BT_REQUIRE(ctx && ms3, BT_ERR_INVALID_ARG, "bt_vos_get_timing: NULL argument");
-	VosState* s = ctx->vos.get();
-	BT_REQUIRE(s && s->timed, BT_ERR_INVALID_ARG, "bt_vos_get_timing: no timed call (bt_vos_enable_timing)");
-	BT_CUDA(cudaSetDevice(ctx->device));
+	VosState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::vos, "bt_vos_get_timing", "bt_vos_reserve", &s));
+	BT_REQUIRE(ms3, BT_ERR_INVALID_ARG, "bt_vos_get_timing: NULL argument");
+	BT_REQUIRE(s->timed, BT_ERR_INVALID_ARG, "bt_vos_get_timing: no timed call (bt_vos_enable_timing)");
 	BT_CUDA(cudaEventSynchronize(s->ev[N_STAGES]));
 	for (int i = 0; i < N_STAGES; i++) BT_CUDA(cudaEventElapsedTime(ms3 + i, s->ev[i], s->ev[i + 1]));
 	return BT_OK;
@@ -747,9 +735,9 @@ extern "C" int bt_vos_get_timing(bt_ctx* ctx, float* ms3) {
 
 extern "C" int bt_vos_debug(bt_ctx* ctx, int slot, float* feat_host, float* label_host, float* pred_host, int32_t* info5, void* stream) {
 	VosState* s;
-	BT_TRY(vos_state(ctx, "bt_vos_debug", &s));
+	BT_TRY(state_of(ctx, &bt_ctx::vos, "bt_vos_debug", "bt_vos_reserve", &s));
+	BT_REQUIRE(s->loaded, BT_ERR_INVALID_ARG, "bt_vos_debug: call bt_vos_load_weights first");
 	BT_REQUIRE(slot >= 0 && slot < s->slots, BT_ERR_INVALID_ARG, "bt_vos_debug: slot %d outside [0, %d)", slot, s->slots);
-	BT_CUDA(cudaSetDevice(ctx->device));
 	cudaStream_t st = (cudaStream_t)stream;
 	const size_t HW = (size_t)s->Hd * s->Wd;
 	if (feat_host) BT_CUDA(cudaMemcpyAsync(feat_host, s->feat.as<float>() + slot * HW * FEAT, sizeof(float) * HW * FEAT, cudaMemcpyDeviceToHost, st));

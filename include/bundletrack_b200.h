@@ -122,7 +122,8 @@ BT_API const char* bt_last_error(void);
 BT_API int bt_version(void);
 
 /* Create / destroy.  `device` is a CUDA ordinal.  The context owns every scratch buffer, so the per-call path does
- * no cudaMalloc/cudaFree (the reference does ~110 per call, SURVEY.md Q10). */
+ * no cudaMalloc/cudaFree (the reference does ~110 per call, SURVEY.md Q10).  A *_reserve refused for its arguments changes nothing; one
+ * that fails while allocating (BT_ERR_CUDA) leaves its module refusing every call with BT_ERR_INVALID_ARG until a reserve succeeds. */
 BT_API int bt_ctx_create(bt_ctx** out, int device);
 BT_API void bt_ctx_destroy(bt_ctx* ctx);
 BT_API int bt_solver_reserve(bt_ctx* ctx, const bt_solver_limits* lim);
@@ -205,7 +206,8 @@ BT_API int bt_knn_match_pairs(bt_ctx* ctx, int n_pairs, const bt_desc_view* A, c
  * (/root/reference/src/FeatureManager.cpp:876-908); bt_desc_pool_store converts them ONCE into pool slot `slot` (fp16 rows for the
  * tensor pass, fp32 copy for the exact stage, norms, measured rounding errors - the caller's buffer is not referenced afterwards) and
  * bt_knn_match_slots / bt_match_pairs_pool then name slots: no per-call conversion.  Slots stay valid until overwritten or until
- * bt_matcher_reserve / bt_desc_pool_reserve re-size the pool. */
+ * bt_matcher_reserve / bt_desc_pool_reserve re-size the pool.  The pool shares its blocks with the matcher's per-call slots: after a
+ * bt_desc_pool_reserve that fails, every matcher call is refused until bt_matcher_reserve (then bt_desc_pool_reserve) succeeds. */
 BT_API int bt_desc_pool_reserve(bt_ctx* ctx, int n_slots);
 BT_API int bt_desc_pool_store(bt_ctx* ctx, int slot, const bt_desc_view* desc, void* stream);
 BT_API int bt_knn_match_slots(bt_ctx* ctx, int n_pairs, const int32_t* slotA, const int32_t* slotB, int k,
@@ -756,6 +758,9 @@ BT_API int bt_stream_sync(void* stream);
  * streams.  Destroying a context or tracker returns all three to their values from before it was created.  Memory from bt_dev_alloc /
  * bt_host_alloc_pinned is the caller's and is not counted. */
 BT_API int bt_debug_live_resources(long long* device_bytes, long long* pinned_bytes, int* handles);
+/* Test aid: the nth allocation of a device or page-locked block by the library from now (a reserve's, typically) fails with BT_ERR_CUDA
+ * without calling CUDA, as an out-of-memory would; 0 disarms.  BT_ERR_INVALID_ARG for nth < 0. */
+BT_API int bt_debug_fail_alloc(int nth);
 
 #ifdef __cplusplus
 }
