@@ -289,6 +289,8 @@ PROTOTYPES = {
     "bt_lfnet_enable_timing": (_i, (_p, _i)),
     "bt_lfnet_get_timing": (_i, (_p, _p)),
     "bt_lfnet_debug_maps": (_i, (_p, _i, _p, _p, _p, _p, _p)),
+    "bt_lfnet_file_info": (_i, (_p, _p, _p)),
+    "bt_lfnet_load_file": (_i, (_p, _p, _i, _p)),
     "bt_vos_schedule": (_i, (_i, _i, _i, _p, _p)),
     "bt_vos_weights_size": (_i, (_p, _p)),
     "bt_vos_reserve": (_i, (_p, _p, _i, _i)),

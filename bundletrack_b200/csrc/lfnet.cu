@@ -2,6 +2,7 @@
 // desc_inputs = photos, use_nms3d), from the 400 x 400 request image to the keypoints and descriptors of the server's reply.
 // FP32 throughout; every reduction has a fixed order, so results do not depend on scheduling or on how requests are batched.
 // oracle/lfnet_oracle.py is the float64 statement of the same graph, written from the reference's Python.  DESIGN.md §3.12.
+#include <errno.h>
 #include <math.h>
 #include "bt_common.cuh"
 
@@ -598,6 +599,74 @@ extern "C" int bt_lfnet_weights_size(const bt_lfnet_params* p, size_t* n_floats)
 	           p->desc_net_depth >= 1 && p->desc_net_depth <= MAX_DESC && p->net_channel > 0 && p->conv_ksize > 0 && p->patch_size > 0 &&
 	           p->desc_net_channel > 0 && p->desc_conv_ksize > 0 && p->desc_dim > 0, BT_ERR_INVALID_ARG, "bt_lfnet_weights_size: parameters out of range");
 	*n_floats = layout_of(*p).total;
+	return BT_OK;
+}
+
+// ---- the weights file (layout: include/bundletrack_b200.h): plain host code, no GPU --------------------------------------------------------
+namespace {
+constexpr char kFileMagic[8] = {'B', 'T', 'L', 'F', 'N', 'E', 'T', 'W'};
+constexpr uint32_t kFileVersion = 1;
+struct FileCloser { void operator()(FILE* f) const { fclose(f); } };
+using File = std::unique_ptr<FILE, FileCloser>;
+
+// Opens `path` and checks its header against this library and its size against the header; on success `f` stands at the first float.
+// Refusals are BT_ERR_INVALID_ARG with a message that starts with `who` and names what differs.
+int open_weights_file(const char* who, const char* path, File& f, bt_lfnet_params* p, size_t* n_floats) {
+	BT_REQUIRE(path, BT_ERR_INVALID_ARG, "%s: path is NULL", who);
+	f.reset(fopen(path, "rb"));
+	BT_REQUIRE(f, BT_ERR_INVALID_ARG, "%s: %s: cannot open it: %s", who, path, strerror(errno));
+	BT_REQUIRE(fseek(f.get(), 0, SEEK_END) == 0, BT_ERR_INVALID_ARG, "%s: %s: cannot seek in it", who, path);
+	const long long size = ftell(f.get());
+	BT_REQUIRE(size >= 0 && fseek(f.get(), 0, SEEK_SET) == 0, BT_ERR_INVALID_ARG, "%s: %s: cannot seek in it", who, path);
+	const long long head = (long long)(sizeof kFileMagic + 2 * sizeof(uint32_t) + sizeof(bt_lfnet_params) + sizeof(uint64_t));
+	char magic[sizeof kFileMagic];
+	BT_REQUIRE(fread(magic, 1, sizeof magic, f.get()) == sizeof magic, BT_ERR_INVALID_ARG, "%s: %s: truncated: %lld bytes, the header takes %lld",
+	           who, path, size, head);
+	BT_REQUIRE(memcmp(magic, kFileMagic, sizeof magic) == 0, BT_ERR_INVALID_ARG, "%s: %s: bad magic: not an LF-Net weights file (lfnet.write_weights_file)",
+	           who, path);
+	uint32_t version = 0, params_bytes = 0;
+	uint64_t count = 0;
+	const bool whole = fread(&version, sizeof version, 1, f.get()) == 1 && fread(&params_bytes, sizeof params_bytes, 1, f.get()) == 1;
+	BT_REQUIRE(!whole || version == kFileVersion, BT_ERR_INVALID_ARG, "%s: %s: format version %u, this library reads version %u", who, path, version,
+	           kFileVersion);
+	BT_REQUIRE(!whole || params_bytes == sizeof(bt_lfnet_params), BT_ERR_INVALID_ARG,
+	           "%s: %s: a bt_lfnet_params struct size of %u bytes, this library's is %zu", who, path, params_bytes, sizeof(bt_lfnet_params));
+	BT_REQUIRE(whole && fread(p, sizeof *p, 1, f.get()) == 1 && fread(&count, sizeof count, 1, f.get()) == 1, BT_ERR_INVALID_ARG,
+	           "%s: %s: truncated: %lld bytes, the header takes %lld", who, path, size, head);
+	size_t want = 0;
+	BT_REQUIRE(bt_lfnet_weights_size(p, &want) == BT_OK, BT_ERR_INVALID_ARG, "%s: %s: its parameters are out of range", who, path);
+	BT_REQUIRE(count == want, BT_ERR_INVALID_ARG, "%s: %s: a float count of %llu, bt_lfnet_weights_size gives %zu for its parameters", who, path,
+	           (unsigned long long)count, want);
+	const long long total = head + (long long)(sizeof(float) * want);
+	BT_REQUIRE(size >= total, BT_ERR_INVALID_ARG, "%s: %s: truncated: %lld bytes, the header and %zu floats take %lld", who, path, size, want, total);
+	BT_REQUIRE(size == total, BT_ERR_INVALID_ARG, "%s: %s: %lld bytes, %lld more than the header and %zu floats take", who, path, size, size - total, want);
+	*n_floats = want;
+	return BT_OK;
+}
+}  // namespace
+
+extern "C" int bt_lfnet_file_info(const char* path, bt_lfnet_params* params_out, size_t* n_floats_out) {
+	File f;
+	bt_lfnet_params p;
+	size_t n = 0;
+	BT_TRY(open_weights_file("bt_lfnet_file_info", path, f, &p, &n));
+	if (params_out) *params_out = p;
+	if (n_floats_out) *n_floats_out = n;
+	return BT_OK;
+}
+
+extern "C" int bt_lfnet_load_file(bt_ctx* ctx, const char* path, int max_images, bt_lfnet_params* params_out) {
+	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_lfnet_load_file: ctx is NULL");
+	File f;
+	bt_lfnet_params p;
+	size_t n = 0;
+	BT_TRY(open_weights_file("bt_lfnet_load_file", path, f, &p, &n));
+	std::vector<float> blob(n);
+	BT_REQUIRE(fread(blob.data(), sizeof(float), n, f.get()) == n, BT_ERR_INVALID_ARG, "bt_lfnet_load_file: %s: reading the floats failed", path);
+	f.reset();
+	BT_TRY(bt_lfnet_reserve(ctx, &p, max_images));
+	BT_TRY(bt_lfnet_load_weights(ctx, blob.data(), n));
+	if (params_out) *params_out = p;
 	return BT_OK;
 }
 

@@ -8,6 +8,7 @@
 //   * knnMatchBothDirections            (the two cv::cuda::DescriptorMatcher::knnMatch calls of SiftManager::findCorresbyNN,
 //                                        /root/reference/src/FeatureManager.cpp:271-273)
 //   * processDepthAndNormals            (Frame::processDepth + Frame::depthToCloudAndNormals, /root/reference/src/Frame.cpp:152-233)
+//   * LfnetGpu::detectFeature           (Lfnet::detectFeature without the LF-Net server, the reference's src/FeatureManager.cpp:813-908)
 // Header-only, no Eigen/yaml-cpp/OpenCV dependency of its own: the pose and intrinsics types are template parameters
 // that only need operator()(row, col) (Eigen::Matrix4f / Matrix3f satisfy it), and the yml values arrive through
 // BtSolverConfig, which the caller fills from the UNCHANGED config_*.yml keys (see INTEGRATION.md for the 6-line
@@ -339,6 +340,93 @@ inline void lfnetRequest(bt_ctx* ctx, const uint8_t* color_gpu, const uint8_t* f
 		throw std::runtime_error(std::string("bt_lfnet_request: ") + bt_last_error());
 }
 
+// ---- Lfnet::detectFeature (FeatureManager.cpp:813-908) without the server: LF-Net on the device (bt_lfnet_detect) -------------------------
+// The network comes from a weights file (bt_lfnet_load_file; lfnet.write_weights_file or scripts/lfnet_export_blob.py writes it).  The object
+// owns its context, the output buffers and one pinned read-back block; nothing is allocated per call.  KeyPointT needs pt.x, pt.y and size
+// (cv::KeyPoint): each keypoint is made as the reference makes it, cv::KeyPoint(p, 1).  Streams are void* as elsewhere in this header; a
+// cudaStream_t passes as it is.
+class LfnetGpu {
+public:
+	explicit LfnetGpu(const std::string& weights_file, int max_images = 1, int device = 0) : max_images_(max_images) {
+		check(bt_ctx_create(&ctx_, device), "bt_ctx_create");
+		try {
+			check(bt_lfnet_load_file(ctx_, weights_file.c_str(), max_images, &p_), "bt_lfnet_load_file");
+			const size_t K = (size_t)p_.top_k, n = (size_t)max_images;
+			head_ = (sizeof(int32_t) * n + 15) / 16 * 16;            // the counts, then every image's keypoints: one read-back
+			check(bt_dev_alloc(&out_, head_ + sizeof(float) * 2 * K * n), "bt_dev_alloc");
+			check(bt_dev_alloc(&desc_, sizeof(float) * K * p_.desc_dim * n), "bt_dev_alloc");
+			check(bt_host_alloc_pinned(&host_, head_ + sizeof(float) * 2 * K * n), "bt_host_alloc_pinned");
+		} catch (...) { release(); throw; }
+	}
+	~LfnetGpu() { release(); }
+	LfnetGpu(const LfnetGpu&) = delete;
+	LfnetGpu& operator=(const LfnetGpu&) = delete;
+
+	// One request (beginFrame's request image, device uint8 400 x 400 x 3) with Frame::_roi (umin, umax, vmin, vmax): kpts receives the
+	// keypoints in image pixels, desc a view of the descriptors on the device (n rows of desc_dim floats, pitch desc_dim * 4, valid until the
+	// next call).  Returns the keypoint count.  Zero keypoints throw, as the reference's detectFeature fails: the caller's catch calls
+	// BundlerGpu::dropFrame (Bundler.cpp:103-117).  Reading the keypoints back is the call's one synchronisation of `stream`.
+	template <class KeyPointT>
+	int detectFeature(const uint8_t* request_gpu, const int32_t roi[4], std::vector<KeyPointT>& kpts, bt_desc_view& desc, void* stream = nullptr) {
+		std::vector<std::vector<KeyPointT>> k(1);
+		std::vector<bt_desc_view> d(1);
+		detectFeatures(1, &request_gpu, &roi, k, d, stream);
+		if (d[0].n == 0) throw std::runtime_error("LfnetGpu::detectFeature: LF-Net found no keypoints");
+		kpts.swap(k[0]);
+		desc = d[0];
+		return d[0].n;
+	}
+	// n requests in one bt_lfnet_detect (several objects or streams).  An image without keypoints gets an empty kpts[i] and desc[i].n = 0.
+	template <class KeyPointT>
+	void detectFeatures(int n, const uint8_t* const* requests_gpu, const int32_t* const* rois, std::vector<std::vector<KeyPointT>>& kpts,
+	                    std::vector<bt_desc_view>& desc, void* stream = nullptr) {
+		if (n < 1 || n > max_images_) throw std::runtime_error("LfnetGpu: " + std::to_string(n) + " requests, the object takes 1 to " + std::to_string(max_images_));
+		const size_t K = (size_t)p_.top_k, D = (size_t)p_.desc_dim;
+		float* kp_dev = reinterpret_cast<float*>(static_cast<char*>(out_) + head_);
+		check(bt_lfnet_detect(ctx_, n, requests_gpu, kp_dev, static_cast<float*>(desc_), static_cast<int32_t*>(out_), stream), "bt_lfnet_detect");
+		check(bt_memcpy_d2h(host_, out_, head_ + sizeof(float) * 2 * K * n, stream), "bt_memcpy_d2h");
+		const int32_t* cnt = static_cast<const int32_t*>(host_);
+		const float* kp = reinterpret_cast<const float*>(static_cast<const char*>(host_) + head_);
+		kpts.resize(n);
+		desc.resize(n);
+		for (int i = 0; i < n; i++) {
+			const int m = cnt[i];
+			kpts[i].clear();
+			xy_.resize(2 * (size_t)m + 1);
+			if (m > 0) {
+				// bt_lfnet_parse_reply's transform on the reply this image would have had
+				const int32_t info[2] = { m, (int32_t)D };
+				int n_out = 0, dim_out = 0;
+				check(bt_lfnet_parse_reply(info, sizeof info, kp + 2 * K * i, sizeof(float) * 2 * m, sizeof(float) * D * m, rois[i], xy_.data(), m, &n_out, &dim_out),
+				      "bt_lfnet_parse_reply");
+				kpts[i].resize(m);
+				for (int j = 0; j < m; j++) { KeyPointT& k = kpts[i][j]; k = KeyPointT(); k.pt.x = xy_[2 * j]; k.pt.y = xy_[2 * j + 1]; k.size = 1.f; }
+			}
+			bt_desc_view v{};
+			v.dev = static_cast<const float*>(desc_) + K * D * i; v.n = m; v.dim = (int)D; v.pitch_bytes = D * sizeof(float);
+			desc[i] = v;
+		}
+	}
+	const bt_lfnet_params& params() const { return p_; }
+	bt_ctx* ctx() { return ctx_; }
+
+private:
+	static void check(int rc, const char* what) { if (rc != BT_OK) throw std::runtime_error(std::string(what) + ": " + bt_last_error()); }
+	void release() {
+		if (host_) bt_host_free_pinned(host_);
+		if (desc_) bt_dev_free(desc_);
+		if (out_) bt_dev_free(out_);
+		bt_ctx_destroy(ctx_);
+		host_ = desc_ = out_ = nullptr; ctx_ = nullptr;
+	}
+	int max_images_;
+	bt_ctx* ctx_ = nullptr;
+	bt_lfnet_params p_{};
+	size_t head_ = 0;
+	void *out_ = nullptr, *desc_ = nullptr, *host_ = nullptr;
+	std::vector<float> xy_;
+};
+
 // ---- the two knnMatch calls of SiftManager::findCorresbyNN (/root/reference/src/FeatureManager.cpp:271-273) in one call --------
 // desA/desB: device CV_32F descriptor matrices (GpuMat::data, rows, step).  DMatchT needs queryIdx, trainIdx, distance (cv::DMatch).
 // The device result buffers belong to the object (sized once for max_feats x k), nothing is allocated per call.
@@ -391,8 +479,8 @@ inline void knnMatchBothDirections(bt_ctx* ctx, const float* desA, int nA, size_
 
 // ---- Bundler::processNewFrame (the reference's src/Bundler.cpp:56-183) as one object over bt_tracker_* -------------------------------------
 // The reference's call is split where it asks the LF-Net server for features (Lfnet::detectFeature, Bundler.cpp:108): beginFrame segments the
-// frame and returns the request image, the caller does the ZMQ round trip (bt_lfnet_parse_reply maps the keypoints back) and calls endFrame,
-// or dropFrame when detection threw.  Statuses are Frame::_status values (BT_FRAME_OTHER / FAIL / NO_BA); poses are cam->model through
+// frame and returns the request image, the caller runs LfnetGpu::detectFeature on it (or does the ZMQ round trip, bt_lfnet_parse_reply mapping
+// the keypoints back) and calls endFrame, or dropFrame when detection threw.  Statuses are Frame::_status values (BT_FRAME_OTHER / FAIL / NO_BA); poses are cam->model through
 // operator()(row, col) (Eigen::Matrix4f works); endFrame's pose is what Bundler::saveNewframeResult records for the frame.
 class BundlerGpu {
 public:

@@ -2,7 +2,8 @@
 
 load_lfnet(model_dir) reads a released model's config.pkl and weights.npz (scripts/lfnet_export_weights.py makes the latter from a TF
 checkpoint) and returns an LfnetDevice, a feature source run_sequence drives on the device: the request image never leaves the GPU and
-the descriptors go straight to the tracker.  DESIGN.md §3.12."""
+the descriptors go straight to the tracker.  write_weights_file turns the same directory into one weights file that bt_lfnet_load_file
+(LfnetDevice.from_file, the C++ LfnetGpu, scripts/lfnet_server.py) loads without Python.  DESIGN.md §3.12."""
 from __future__ import annotations
 
 import ctypes
@@ -161,19 +162,55 @@ def read_weights(path: str) -> dict:
         return {k: z[k] for k in z.files}
 
 
+FILE_MAGIC = b"BTLFNETW"
+FILE_VERSION = 1
+
+
+def weights_file_bytes(blob: np.ndarray, hp: dict) -> bytes:
+    """The weights file bt_lfnet_load_file reads (layout: include/bundletrack_b200.h): magic, version, sizeof(bt_lfnet_params), the params
+    struct and the float count, then the blob."""
+    p = params_struct(hp)
+    blob = np.ascontiguousarray(blob, np.float32)
+    return (FILE_MAGIC + np.array([FILE_VERSION, ctypes.sizeof(p)], "<u4").tobytes() + bytes(p) + np.array([blob.size], "<u8").tobytes()
+            + blob.astype("<f4").tobytes())
+
+
+def write_weights_file(model_dir: str, out_path: str, top_k: int = 500) -> dict:
+    """A released model directory (config.pkl + weights.npz, as load_lfnet reads it) as one weights file any host can load with
+    bt_lfnet_load_file, BN folded as make_blob folds it.  Returns the hyper-parameters written."""
+    hp = check_config(read_config(os.path.join(model_dir, "config.pkl")), top_k)
+    data = weights_file_bytes(make_blob(read_weights(os.path.join(model_dir, "weights.npz")), hp), hp)
+    with open(out_path, "wb") as f:
+        f.write(data)
+    return hp
+
+
+def file_info(path: str) -> tuple:
+    """(hyper-parameters, float count) of a weights file, checked as bt_lfnet_load_file checks it (no GPU)."""
+    p, n = _lib.LfnetParams(), ctypes.c_size_t(0)
+    _lib.check(_lib.load().bt_lfnet_file_info(os.fsencode(path), ctypes.byref(p), ctypes.byref(n)), "bt_lfnet_file_info")
+    return {f: getattr(p, f) for f, _ in p._fields_}, n.value
+
+
 class LfnetDevice(_lib.Facade):
     """The LF-Net server's network on the device.  detect() runs a batch of request images (bt_lfnet_request's output) in one call;
-    as a run_sequence feature source (on_device) it hands the tracker host keypoints in image pixels and the device descriptors."""
+    as a run_sequence feature source (on_device) it hands the tracker host keypoints in image pixels and the device descriptors.
+    LfnetDevice.from_file loads a weights file instead of TF variables."""
     on_device = True
 
-    def __init__(self, weights: dict, hp: dict, max_images: int = 1, device: int = 0, stream: int = 0, ctx=None):
+    def __init__(self, weights: dict, hp: dict, max_images: int = 1, device: int = 0, stream: int = 0, ctx=None, _file: str = None):
         super().__init__(ctx, device, stream)
+        if _file is None:
+            self.hp = dict(hp)
+            self.params = params_struct(self.hp)
+            blob = make_blob(weights, self.hp)
+            _lib.check(self.lib.bt_lfnet_reserve(self.ctx, ctypes.byref(self.params), max_images), "bt_lfnet_reserve")
+            _lib.check(self.lib.bt_lfnet_load_weights(self.ctx, _lib.ptr(blob), blob.size), "bt_lfnet_load_weights")
+        else:
+            self.params = _lib.LfnetParams()
+            _lib.check(self.lib.bt_lfnet_load_file(self.ctx, os.fsencode(_file), max_images, ctypes.byref(self.params)), "bt_lfnet_load_file")
+            self.hp = {f: getattr(self.params, f) for f, _ in self.params._fields_}
         import torch
-        self.hp = dict(hp)
-        self.params = params_struct(self.hp)
-        blob = make_blob(weights, self.hp)
-        _lib.check(self.lib.bt_lfnet_reserve(self.ctx, ctypes.byref(self.params), max_images), "bt_lfnet_reserve")
-        _lib.check(self.lib.bt_lfnet_load_weights(self.ctx, _lib.ptr(blob), blob.size), "bt_lfnet_load_weights")
         self.max_images = max_images
         dev = torch.device("cuda", device)
         K, D = self.hp["top_k"], self.hp["desc_dim"]
@@ -181,6 +218,12 @@ class LfnetDevice(_lib.Facade):
         self.desc = torch.empty((max_images, K, D), dtype=torch.float32, device=dev)
         self.n = torch.empty((max_images,), dtype=torch.int32, device=dev)
         self._host = torch.empty((K * 2 + 1,), dtype=torch.float32, pin_memory=True)
+
+    @classmethod
+    def from_file(cls, path: str, max_images: int = 1, device: int = 0, stream: int = 0, ctx=None) -> "LfnetDevice":
+        """The network of a weights file (write_weights_file), loaded by bt_lfnet_load_file: the same device state as the constructor
+        makes from the TF variables the file was written from."""
+        return cls(None, None, max_images, device, stream, ctx, _file=path)
 
     def detect(self, requests, stream=None):
         """requests: device uint8 [400, 400, 3] tensors.  Enqueues one bt_lfnet_detect on `stream` (default: the facade's) and returns

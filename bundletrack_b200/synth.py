@@ -460,6 +460,23 @@ def write_png(path: str, img: np.ndarray) -> None:
                 + chunk(b"IDAT", zlib.compress(raw, 1)) + chunk(b"IEND", b""))
 
 
+def write_ycbineoat_video(seq: Sequence, video_dir: str) -> None:
+    """seq as a YCBInEOAT video directory (sequence.YcbineoatVideo reads it): rgb/, depth/ (16-bit millimetres), masks/, cam_K.txt and
+    annotated_poses/ (ob_in_cam per frame), frames named %07d.png."""
+    import os
+    for sub in ("rgb", "depth", "masks", "annotated_poses"):
+        os.makedirs(os.path.join(video_dir, sub), exist_ok=True)
+    for k in range(seq.n_frames):
+        for sub, img in (("rgb", seq.colour[k]), ("depth", np.round(seq.depth_raw[k] * 1000).astype(np.uint16)), ("masks", seq.mask[k])):
+            write_png(os.path.join(video_dir, sub, f"{k:07d}.png"), img)
+        G = np.linalg.inv(np.asarray(seq.poses_gt[k], np.float64))
+        with open(os.path.join(video_dir, "annotated_poses", f"{k:07d}.txt"), "w") as f:
+            f.write("".join(" ".join(f"{v:.9g}" for v in row) + "\n" for row in G))
+    K = np.array([[seq.K[0], 0, seq.K[2]], [0, seq.K[1], seq.K[3]], [0, 0, 1]])
+    with open(os.path.join(video_dir, "cam_K.txt"), "w") as f:
+        f.write("".join(" ".join(f"{v:.9g}" for v in row) + "\n" for row in K))
+
+
 def make_ellipsoid_model(seed: int, n: int, radii=(0.05, 0.04, 0.03)) -> np.ndarray:
     """float32 [n,3]: n points on the surface of an ellipsoid with the given semi-axes (metres), the stand-in for an OBJ model's vertices."""
     rng = np.random.default_rng(seed)

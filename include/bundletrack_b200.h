@@ -683,7 +683,20 @@ BT_API int bt_match_viz(bt_ctx* ctx, int n_images, const bt_match_viz_desc* desc
  * bt_lfnet_enable_timing / bt_lfnet_get_timing: device time of the last call per stage, ms5 = {trunk, score maps, detection, keypoints and
  * patches, descriptor}; get_timing waits for that call.
  * bt_lfnet_debug_maps (test aid): image `image` of the last call's max_heatmaps and max_scales (400 x 400 floats each), its integer
- * keypoints (top_k x (x, y) int32) and orientations (top_k x (cos, sin)), each output optional; synchronises `stream`. */
+ * keypoints (top_k x (x, y) int32) and orientations (top_k x (cos, sin)), each output optional; synchronises `stream`.
+ * Weights file (lfnet.write_weights_file, scripts/lfnet_export_blob.py), so a host without Python can load a network; byte order of the
+ * host that wrote it (little-endian on x86-64 and aarch64), no padding:
+ *   offset 0        char     magic[8] = "BTLFNETW"
+ *   offset 8        uint32   format version = 1
+ *   offset 12       uint32   sizeof(bt_lfnet_params) = P (104 on x86-64 and aarch64)
+ *   offset 16       bt_lfnet_params, P bytes, as the struct is laid out in memory
+ *   offset 16 + P   uint64   n_floats = bt_lfnet_weights_size of those parameters
+ *   offset 24 + P   float32  the blob above, n_floats of them, and nothing after it.
+ * bt_lfnet_file_info (host code, no GPU): checks the file and writes its parameters and float count (each output optional).
+ *   BT_ERR_INVALID_ARG, naming what differs, for a file it cannot open, a bad magic, another format version or struct size, a truncated
+ *   file or trailing bytes, parameters bt_lfnet_weights_size refuses and a float count other than its.
+ * bt_lfnet_load_file: bt_lfnet_file_info's checks, then bt_lfnet_reserve(ctx, params, max_images) and bt_lfnet_load_weights with the
+ *   file's blob; their refusals come through unchanged.  params_out (optional) receives the file's parameters. */
 typedef struct {
 	int top_k;                 /* run_server.py --top_k (500) */
 	int net_channel, net_block, conv_ksize, net_num_scales;
@@ -705,6 +718,8 @@ BT_API int bt_lfnet_detect(bt_ctx* ctx, int n, const uint8_t* const* request_dev
 BT_API int bt_lfnet_enable_timing(bt_ctx* ctx, int on);
 BT_API int bt_lfnet_get_timing(bt_ctx* ctx, float* ms5);
 BT_API int bt_lfnet_debug_maps(bt_ctx* ctx, int image, float* heat_host, float* scale_host, int32_t* kpts_int_host, float* ori_host, void* stream);
+BT_API int bt_lfnet_file_info(const char* path, bt_lfnet_params* params_out, size_t* n_floats_out);
+BT_API int bt_lfnet_load_file(bt_ctx* ctx, const char* path, int max_images, bt_lfnet_params* params_out);
 
 /* ---- Object masks on the device: transductive-vos.pytorch's run_video.py (resnet50) without PyTorch ----------------------------------
  * The first frame's mask is propagated through the video (DESIGN.md §3.13): a ResNet-50 to stride 8 (layer3 and layer4 at stride 1,
