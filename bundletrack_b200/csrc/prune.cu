@@ -5,7 +5,7 @@
 //   k_prune_mutual   one CTA per frame pair.  Direction A->B then B->A: for every query feature the FIRST of its k
 //                    neighbours passing the gates of SiftManager::pruneMatches (/root/reference/src/FeatureManager.cpp:
 //                    290-336: both keypoints round()ed inside the image, both depths >= 0.1, model-frame distance <=
-//                    max_dist_*, cos(angle between model-frame normals) >= cos(max_normal_*), thresholds chosen by
+//                    max_dist_*, cos(angle between model-frame normals) >= cos(max_normal_*) or NaN (a zero normal), thresholds chosen by
 //                    |idA-idB|==1) is kept; survivors are appended in query order, A->B block first, duplicates NOT
 //                    removed — exactly collectMutualMatches (:338-368, a union, SURVEY.md D1).  Also emits the
 //                    model-frame points RANSAC consumes (runRansacMultiPairGPU :676-706).
@@ -14,7 +14,9 @@
 //                    inliers -> EntryJ {imgIdx_i = older frame, imgIdx_j = newer frame, pos_i = ptB_cam, pos_j = ptA_cam}
 //                    (Bundler::optimizeGPU, /root/reference/src/Bundler.cpp:308-317), < 5 inliers => pair dropped
 //                    (FeatureManager.cpp:233-241,727-730); pairs written back to back, which is the grouping the
-//                    solver's tail wants.
+//                    solver's tail wants.  A list longer than the caller's capacity is cut there; the pair status (OK /
+//                    cleared / Frame::FAIL) follows the match outcome, never the cut.
+//   tests/test_find_corres_adversarial_gpu.py holds all of these to a float64 restatement (oracle/corres_families.py).
 #include <algorithm>
 #include <climits>
 #include <map>
@@ -38,7 +40,7 @@ __device__ __forceinline__ bool prune_gate(const PruneFrame& Q, const PruneFrame
 	const int uq = (int)roundf(pq.x), vq = (int)roundf(pq.y), ut = (int)roundf(pt.x), vt = (int)roundf(pt.y);   // std::round
 	if (uq < 0 || vq < 0 || uq >= cam.W || vq >= cam.H || ut < 0 || vt < 0 || ut >= cam.W || vt >= cam.H) return false;   // Utils::isPixelInsideImage
 	const float dq = __ldg(Q.depth + (size_t)vq * cam.W + uq), dt = __ldg(Tn.depth + (size_t)vt * cam.W + ut);
-	if (dq < 0.1f || dt < 0.1f) return false;                    // organised cloud point: z < 0.1 (zeros when depth < 0.1)
+	if (!(dq >= 0.1f && dt >= 0.1f)) return false;              // the organised cloud holds zeros wherever !(depth >= 0.1), NaN included
 	// Frame::depthToCloudAndNormals: K^-1 (u d, v d, d)   (/root/reference/src/Frame.cpp:199-233, CUDAImageUtil.cu:310-326)
 	ptQ[0] = cam.ifx * ((float)uq * dq) + cam.icx * dq; ptQ[1] = cam.ify * ((float)vq * dq) + cam.icy * dq; ptQ[2] = dq;
 	ptT[0] = cam.ifx * ((float)ut * dt) + cam.icx * dt; ptT[1] = cam.ify * ((float)vt * dt) + cam.icy * dt; ptT[2] = dt;
@@ -196,6 +198,7 @@ __global__ void __launch_bounds__(1024) k_emit_entryj(const PrunePair* __restric
 		s_scan[tid] = cnt;
 		__syncthreads();
 		for (int o = 1; o < 1024; o <<= 1) { const int v = (tid >= o) ? s_scan[tid - o] : 0; __syncthreads(); s_scan[tid] += v; __syncthreads(); }
+		const int matched = cnt;
 		int excl = s_scan[tid] - cnt + s_carry;
 		// never describe more than the caller's buffer holds: a pair that does not fit is cut (or dropped), so the (offset, count)
 		// arrays a caller hands on as bt_window::block_off / block_n always stay inside entry_out
@@ -204,8 +207,9 @@ __global__ void __launch_bounds__(1024) k_emit_entryj(const PrunePair* __restric
 		if (p < n_pairs) {
 			n_entry_out[p] = cnt; entry_off_out[p] = excl;
 			// SiftManager::findCorres' outcome for the pair (FeatureManager.cpp:186-241,282-286): a pair left with fewer than 5 matches is
-			// cleared, and when the two frames are neighbours (|idA - idB| == 1) the newer frame is marked Frame::FAIL
-			if (status_out) status_out[p] = cnt > 0 ? BT_PAIR_OK : (abs(pairs[p].A.frame_id - pairs[p].B.frame_id) == 1 ? BT_PAIR_FAIL : BT_PAIR_EMPTY);
+			// cleared, and when the two frames are neighbours (|idA - idB| == 1) the newer frame is marked Frame::FAIL.  The outcome is the
+			// match's, not the buffer's: a pair cut by the capacity keeps its status and shows the cut only in its count
+			if (status_out) status_out[p] = matched > 0 ? BT_PAIR_OK : (abs(pairs[p].A.frame_id - pairs[p].B.frame_id) == 1 ? BT_PAIR_FAIL : BT_PAIR_EMPTY);
 		}
 		__syncthreads();
 		if (tid == 1023) s_carry += s_scan[1023];

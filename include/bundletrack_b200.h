@@ -287,8 +287,9 @@ BT_API int bt_match_pairs_pool(bt_ctx* ctx, int n_pairs, const bt_match_frame* A
  *    (A[p].frame_id, B[p].frame_id) called with n_existing = 0; the device drops the ones whose (uA,vA) or (uB,vB) already occurs among
  *    the pair's mutual matches, looks the 3-D points up at round(u), round(v) and appends the rest before RANSAC.  Ignored for
  *    neighbour pairs (|idA - idB| == 1), as in the reference.
- *  - status_out[p] (DEVICE, optional): BT_PAIR_OK (>= 5 inliers emitted), BT_PAIR_EMPTY (matches cleared, frame status unchanged) or
- *    BT_PAIR_FAIL (a neighbour pair ended with fewer than 5 matches: the reference marks frame A Frame::FAIL, :233-241,282-286).
+ *  - status_out[p] (DEVICE, optional): BT_PAIR_OK (>= 5 inliers), BT_PAIR_EMPTY (matches cleared, frame status unchanged) or
+ *    BT_PAIR_FAIL (a neighbour pair ended with fewer than 5 matches: the reference marks frame A Frame::FAIL, :233-241,282-286).  The
+ *    status is the match's outcome: a pair that entry_capacity cuts keeps it, and only n_entry_out[p] shows the cut.
  *  - uv_out (DEVICE float4 per emitted entry, optional): (uA, vA, uB, vB) of the entry - what updateFramePairMapPoints (:448-485) is fed
  *    through bt_tracks_update_pair. */
 typedef struct { const float* uv; int n; } bt_match_extra;   /* HOST: n x (uA, vA, uB, vB) */

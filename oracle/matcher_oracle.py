@@ -129,10 +129,11 @@ def ransac_pair(A, B, u3, dist_thresh):
 
 # ---------------------------------------------------------------------------------------------------------------------
 def _cloud_point(depth, K, u, v):
-    """Frame::depthToCloudAndNormals (/root/reference/src/Frame.cpp:199-233): K^-1 (u d, v d, d), zeros when d < 0.1."""
+    """Frame::depthToCloudAndNormals (/root/reference/src/Frame.cpp:199-233): K^-1 (u d, v d, d), zeros wherever !(d >= 0.1): below
+    0.1, negative, -inf and NaN alike (to_camera in frontend.cu)."""
     fx, fy, cx, cy = [np.float32(x) for x in K]
     d = np.float32(depth[v, u])
-    if d < np.float32(0.1):
+    if not d >= np.float32(0.1):
         return np.zeros(3, np.float32)
     ifx, ify, icx, icy = np.float32(1) / fx, np.float32(1) / fy, -cx / fx, -cy / fy
     return np.array([ifx * (np.float32(u) * d) + icx * d, ify * (np.float32(v) * d) + icy * d, d], np.float32)
@@ -170,6 +171,227 @@ def prune_matches(Q, T, knn_idx, K, max_dist, cos_max):
             out.append((q, int(t), pq, pt))
             break
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+GATE_FAIL, GATE_PASS, GATE_MARGINAL = "fail", "pass", "marginal"
+# A zero normal normalises to NaN (Eigen 3.2's normalized()), the dot is NaN and `dot < cos_max` is false: the candidate is kept.  Eigen
+# 3.3 returns the zero vector instead (dot 0, rejected whenever cos_max > 0); which one the reference ran is open (DESIGN.md §3.2).
+ZERO_NORMAL_KEEPS = True
+_U = 2.0 ** -24
+
+
+def _gamma(n):
+    return n * _U / (1.0 - n * _U)
+
+
+class _Exact:
+    """Float64 arithmetic that records whether every step was exact in float32 too: every result a float32 value and every float64
+    operation exact (TwoSum for additions; a product of two float32 values always is; sqrt and division checked by multiplying back).
+    When it stays exact, the kernel's float32 values - fused or not - equal these."""
+
+    def __init__(self):
+        self.ok = True
+
+    def _rep(self, x):
+        if np.isfinite(x) and float(np.float32(x)) != x:
+            self.ok = False
+        return x
+
+    def mul(self, a, b):
+        return self._rep(a * b)
+
+    def add(self, a, b):
+        s = a + b
+        bb = s - a
+        if np.isfinite(s) and (a - (s - bb)) + (b - bb) != 0.0:
+            self.ok = False
+        return self._rep(s)
+
+    def sqrt(self, s):
+        r = float(np.sqrt(s))
+        if r * r != s:
+            self.ok = False
+        return self._rep(r)
+
+    def div(self, a, b):
+        q = a / b
+        if q * b != a:
+            self.ok = False
+        return self._rep(q)
+
+
+def gate_pixels(Q, T, q, t):
+    """std::round (half away from zero) of both keypoints and Utils::isPixelInsideImage on both frames: (uq, vq, ut, vt) or None."""
+    H, W = Q["depth"].shape
+    uq, vq = _round_half_away(Q["kpts"][q, 0]), _round_half_away(Q["kpts"][q, 1])
+    ut, vt = _round_half_away(T["kpts"][t, 0]), _round_half_away(T["kpts"][t, 1])
+    if not (0 <= uq < W and 0 <= vq < H and 0 <= ut < W and 0 <= vt < H):
+        return None
+    return uq, vq, ut, vt
+
+
+def prune_gate64(Q, T, q, t, K, max_dist, cos_max):
+    """One candidate of SiftManager::pruneMatches (FeatureManager.cpp:290-336) in float64 with a float32 error bound.
+    Returns (GATE_PASS / GATE_FAIL / GATE_MARGINAL, ptQ_cam, ptT_cam as float32, detail dict).
+
+    Rounding, the in-image test and the depth test (!(d >= 0.1) rejects, NaN included) are exact decisions.  The rest is evaluated in
+    float64 in the kernel's operation order from the kernel's float32 inputs (ifx = 1/fx, icx = -cx/fx rounded to float32, the float32
+    pose, depth and normals).  When every step is exact in float32 as well (_Exact: dyadic geometry) the decision is exact; otherwise
+    a test within its bound E of the threshold is MARGINAL: the float32 kernel may decide it either way.
+
+    Bounds (u = 2^-24; a float32 operation, fused or not, rounds once; n roundings on a term stay within gamma_n = n u / (1 - n u)):
+      cloud point  x = ifx (u d) + icx d: at most 3 roundings per term, |dx| <= gamma_3 a_x with a_x = |ifx u d| + |icx d|; z = d exact.
+      model point  m_r = ((T_r0 x + T_r1 y) + T_r2 z) + T_r3: at most 4 roundings per term on top of the inputs' errors, so
+                   |dm_r| <= gamma_8 M_r with M_r = sum_i |T_ri| (|p_i| + a_i) + |T_r3|.
+      difference   |dd_r| <= |dmQ_r| + |dmT_r| + u |d_r|.
+      distance     sqrt((d0^2 + d1^2) + d2^2) is 1-Lipschitz in d (moves by <= sum_r |dd_r|); its own 3 squares, 2 additions and the sqrt
+                   add at most gamma_4 dist.   E_dist = sum_r (gamma_8 (MQ_r + MT_r) + u |d_r|) + gamma_4 dist.
+      normals      w_r = (T_r0 n_x + T_r1 n_y) + T_r2 n_z: |dw_r| <= gamma_3 N_r, N_r = sum_i |T_ri| |n_i|.  w / |w| moves by at most
+                   2 |dw|_2 / |w|; the norm (3 squares, 2 adds, sqrt) and the division add gamma_5 per unit component; the dot's 3 products
+                   and 2 additions add gamma_3 (its terms sum to <= 1 in magnitude).
+                   E_dot = 2 gamma_3 (|N_q|_2 / l_q + |N_t|_2 / l_t) + 2 gamma_5 + gamma_3.
+    Both bounds are doubled for the second-order terms and the float64 evaluation itself."""
+    H, W = Q["depth"].shape
+    px = gate_pixels(Q, T, q, t)
+    z3 = np.zeros(3, np.float32)
+    if px is None:
+        return GATE_FAIL, z3, z3, {"why": "outside"}
+    uq, vq, ut, vt = px
+    dq, dt = np.float32(Q["depth"][vq, uq]), np.float32(T["depth"][vt, ut])
+    if not (dq >= np.float32(0.1) and dt >= np.float32(0.1)):
+        return GATE_FAIL, z3, z3, {"why": "depth"}
+    pq, pt = _cloud_point(Q["depth"], K, uq, vq), _cloud_point(T["depth"], K, ut, vt)
+    fx, fy, cx, cy = [np.float32(x) for x in K]
+    ifx, ify, icx, icy = (float(v) for v in (np.float32(1) / fx, np.float32(1) / fy, -cx / fx, -cy / fy))
+    ex, exn = _Exact(), _Exact()          # the distance's chain and the normals' chain, each exact or bounded on its own
+    out = {}
+    for side, (fr, u, v, d) in (("q", (Q, uq, vq, float(dq))), ("t", (T, ut, vt, float(dt)))):
+        P = np.asarray(fr["pose"], np.float32).astype(np.float64)
+        p = [ex.add(ex.mul(ifx, ex.mul(float(u), d)), ex.mul(icx, d)), ex.add(ex.mul(ify, ex.mul(float(v), d)), ex.mul(icy, d)), d]
+        a = [abs(ifx * u * d) + abs(icx * d), abs(ify * v * d) + abs(icy * d), 0.0]
+        n = [float(x) for x in np.asarray(fr["normal"][v, u, :3], np.float32)]
+        m, M, w, N = [], [], [], []
+        for r in range(3):
+            m.append(ex.add(ex.add(ex.add(ex.mul(P[r, 0], p[0]), ex.mul(P[r, 1], p[1])), ex.mul(P[r, 2], p[2])), P[r, 3]))
+            M.append(sum(abs(P[r, i]) * (abs(p[i]) + a[i]) for i in range(3)) + abs(P[r, 3]))
+            w.append(exn.add(exn.add(exn.mul(P[r, 0], n[0]), exn.mul(P[r, 1], n[1])), exn.mul(P[r, 2], n[2])))
+            N.append(sum(abs(P[r, i]) * abs(n[i]) for i in range(3)))
+        out[side] = (m, M, w, N)
+    (mQ, MQ, wq, NQ), (mT, MT, wt, NT) = out["q"], out["t"]
+    dd = [ex.add(mQ[r], -mT[r]) for r in range(3)]
+    dist = ex.sqrt(ex.add(ex.add(ex.mul(dd[0], dd[0]), ex.mul(dd[1], dd[1])), ex.mul(dd[2], dd[2])))
+    e_dist = 2.0 * (sum(_gamma(8) * (MQ[r] + MT[r]) + _U * abs(dd[r]) for r in range(3)) + _gamma(4) * dist)
+    lq = exn.sqrt(exn.add(exn.add(exn.mul(wq[0], wq[0]), exn.mul(wq[1], wq[1])), exn.mul(wq[2], wq[2])))
+    lt = exn.sqrt(exn.add(exn.add(exn.mul(wt[0], wt[0]), exn.mul(wt[1], wt[1])), exn.mul(wt[2], wt[2])))
+    zero_normal = lq == 0.0 or lt == 0.0
+    if zero_normal:
+        dot, e_dot = float("nan"), 0.0
+    else:
+        uq3, ut3 = [exn.div(x, lq) for x in wq], [exn.div(x, lt) for x in wt]
+        dot = exn.add(exn.add(exn.mul(uq3[0], ut3[0]), exn.mul(uq3[1], ut3[1])), exn.mul(uq3[2], ut3[2]))
+        e_dot = 2.0 * (2.0 * _gamma(3) * (np.linalg.norm(NQ) / lq + np.linalg.norm(NT) / lt) + 2.0 * _gamma(5) + _gamma(3))
+    if ex.ok:
+        e_dist = 0.0
+    if exn.ok:
+        e_dot = 0.0
+    md, cm = float(np.float32(max_dist)), float(np.float32(cos_max))
+    detail = {"dist": dist, "e_dist": e_dist, "dot": dot, "e_dot": e_dot, "exact": ex.ok and exn.ok, "zero_normal": zero_normal}
+    if zero_normal and not ZERO_NORMAL_KEEPS:
+        return GATE_FAIL, pq, pt, detail
+    if dist > md + e_dist or (not zero_normal and dot < cm - e_dot):
+        return GATE_FAIL, pq, pt, detail
+    if dist > md - e_dist or (not zero_normal and dot < cm + e_dot):
+        return GATE_MARGINAL, pq, pt, detail
+    return GATE_PASS, pq, pt, detail
+
+
+def prune_options(Q, T, knn_idx, K, max_dist, cos_max):
+    """pruneMatches for one direction under prune_gate64: for every query, in order, the outcomes the kernel may produce - the train
+    index it keeps, or None - each with its (ptQ, ptT).  A query has one outcome unless a marginal candidate comes before the first
+    passing one.  Returns (options [per query: list of (t or None, ptQ, ptT)], marginals [(q, t, detail)])."""
+    nT = len(T["kpts"])
+    options, marginals = [], []
+    for q in range(len(Q["kpts"])):
+        opts = []
+        decided = False
+        for t in knn_idx[q]:
+            t = int(t)
+            if t < 0 or t >= nT:
+                continue
+            verdict, pq, pt, detail = prune_gate64(Q, T, q, t, K, max_dist, cos_max)
+            if verdict == GATE_FAIL:
+                continue
+            opts.append((t, pq, pt))
+            if verdict == GATE_PASS:
+                decided = True
+                break
+            marginals.append((q, t, detail))
+        if not decided:
+            opts.append((None, None, None))
+        options.append(opts)
+    return options, marginals
+
+
+def _mutual_row(A, B, q, t, pq, pt, direction):
+    if direction == 0:
+        return np.concatenate([A["kpts"][q], B["kpts"][t], pq, pt]).astype(np.float32)
+    return np.concatenate([A["kpts"][t], B["kpts"][q], pt, pq]).astype(np.float32)
+
+
+def mutual_rows_resolved(A, B, optAB, optBA, got=None, ulps=0):
+    """collectMutualMatches' rows under prune_options' outcomes (A->B block, then B->A).  A query with several possible outcomes takes the
+    one whose row is `got`'s next row (uv bit-equal, points within `ulps` float32 ulps), else its no-match outcome if it has one.
+    Returns (rows [m,10] float32, n_ambiguous_queries)."""
+    rows, amb = [], 0
+    for direction, opts_all in ((0, optAB), (1, optBA)):
+        for q, opts in enumerate(opts_all):
+            if len(opts) > 1:
+                amb += 1
+            pick = opts[-1] if len(opts) == 1 else None
+            if pick is None:
+                nxt = got[len(rows)] if got is not None and len(rows) < len(got) else None
+                pick = opts[-1]
+                for o in opts:
+                    if o[0] is not None and nxt is not None and rows_match(_mutual_row(A, B, q, o[0], o[1], o[2], direction)[None], nxt[None], ulps):
+                        pick = o
+                        break
+            if pick[0] is not None:
+                rows.append(_mutual_row(A, B, q, pick[0], pick[1], pick[2], direction))
+    return np.asarray(rows, np.float32).reshape(-1, 10), amb
+
+
+def rows_match(a, b, ulps=0):
+    """(uA, vA, uB, vB) bit-equal and the six point coordinates within `ulps` float32 ulps (0: bit-equal)."""
+    a = np.ascontiguousarray(a, np.float32).reshape(-1, 10)
+    b = np.ascontiguousarray(b, np.float32).reshape(-1, 10)
+    if a.shape != b.shape:
+        return False
+    if not np.array_equal(a[:, :4].view(np.uint32), b[:, :4].view(np.uint32)):
+        return False
+    return bool((ulp_distance(a[:, 4:], b[:, 4:]) <= ulps).all())
+
+
+def ulp_distance(a, b):
+    """|a - b| in float32 ulps along the ordered integer line (+0 and -0 are 0 apart); NaN against anything is far."""
+    def key(x):
+        i = np.ascontiguousarray(x, np.float32).view(np.int32).astype(np.int64)
+        return np.where(i < 0, -(i & 0x7FFFFFFF), i)
+    d = np.abs(key(a) - key(b))
+    return np.where(np.isnan(a) | np.isnan(b), np.int64(1) << 40, d)
+
+
+def emit_plan(n_inliers, neighbor, capacity):
+    """k_emit_entryj's contract for one call, from each pair's RANSAC inlier count: a pair with fewer than 5 is cleared
+    (FeatureManager.cpp:233-241); the pairs are written back to back and cut at `capacity`; the status is the match outcome, not the
+    cut's: OK when >= 5 inliers, else FAIL for a neighbour pair (Frame::FAIL, :282-286) and EMPTY otherwise.
+    Returns (n_entry, entry_off, total, status) with status 0 / 1 / 2 = BT_PAIR_OK / BT_PAIR_EMPTY / BT_PAIR_FAIL."""
+    kept = np.where(np.asarray(n_inliers, np.int64) >= 5, np.asarray(n_inliers, np.int64), 0)
+    off = np.concatenate([[0], np.cumsum(kept)[:-1]]).astype(np.int64)
+    off_c = np.minimum(off, capacity)
+    n_c = np.minimum(off + kept, capacity) - off_c
+    status = np.where(kept > 0, 0, np.where(np.asarray(neighbor, bool), 2, 1))
+    return n_c.astype(np.int32), off_c.astype(np.int32), int(min(kept.sum(), capacity)), status.astype(np.int32)
 
 
 def collect_mutual(A, B, mAB, mBA):
