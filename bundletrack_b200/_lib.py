@@ -220,6 +220,7 @@ PROTOTYPES = {
     "bt_ransac_reserve": (_i, (_p, _i, _i, _i)),
     "bt_ransac_pairs": (_i, (_p, _i, _p, _p, _p, _i, _f, _u64, _p, _p, _p)),
     "bt_ransac_debug": (_i, (_p, _p, _i, _p, _i)),
+    "bt_ransac_debug_trials": (_i, (_p, _i, _i, _p, _p, _p)),
     "bt_pipeline_reserve": (_i, (_p, _i, _i, _i, _i)),
     "bt_prune_mutual_pairs": (_i, (_p, _i, _P(MatchFrame), _P(MatchFrame), _i, _i, _f, _f, _f, _f, _p, _p, _i, _P(PruneParams), _p, _p, _p)),
     "bt_match_pairs": (_i, (_p, _i, _P(MatchFrame), _P(MatchFrame), _P(DescView), _P(DescView), _i, _i, _f, _f, _f, _f, _P(PruneParams), _i, _f, _u64, _p, _i, _p, _p, _p, _p)),

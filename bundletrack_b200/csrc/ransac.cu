@@ -149,7 +149,7 @@ __global__ void __launch_bounds__(256) k_ransac_eval(const RansacPair* __restric
 		const int m = min(kEvalPts, pr.n - base);
 		__syncthreads();
 		for (int k = threadIdx.x; k < ((m + 1) & ~1); k += blockDim.x) {
-			float4 a4 = make_float4(0.f, 0.f, 0.f, 0.f), b4 = make_float4(3e38f, 3e38f, 3e38f, 0.f);      // padding point of an odd tail: never an inlier (its squared distance overflows)
+			float4 a4 = make_float4(0.f, 0.f, 0.f, 0.f), b4 = make_float4(NAN, NAN, NAN, 0.f);      // padding point of an odd tail: its squared distance is NaN, never <= d2_max (+inf included)
 			if (k < m) { a4 = __ldg(pr.A + base + k); b4 = __ldg(pr.B + base + k); }
 			const int j = k >> 1, h = k & 1;
 			float* p0 = reinterpret_cast<float*>(&sP[0][j]); float* p1 = reinterpret_cast<float*>(&sP[1][j]); float* p2 = reinterpret_cast<float*>(&sP[2][j]);
@@ -225,6 +225,7 @@ struct RansacState {
 	UploadBuf h_pairs;
 	unsigned long long table_seed = ~0ull;
 	int table_trials = 0;
+	int last_pairs = 0, last_trials = 0;      // shape of the last run's per-trial poses, flags and keys (bt_ransac_debug_trials)
 };
 void StateDeleter::operator()(RansacState* r) const { delete r; }
 
@@ -245,6 +246,7 @@ int ransac_run_device(bt_ctx* ctx, const RansacPair* d_pairs, int n_pairs, int n
 	k_ransac_eval<<<grid, 256, 0, stream>>>(d_pairs, n_trials, r->poses.as<float>(), r->good.as<int>(), d2_max, r->best.as<unsigned long long>());
 	k_ransac_inliers<<<n_pairs, 256, 0, stream>>>(d_pairs, n_trials, r->poses.as<float>(), dist_thresh, r->best.as<unsigned long long>(), inlier_ids_out, n_inliers_out, r->best_trial.as<int32_t>());
 	BT_CUDA(cudaGetLastError());
+	r->last_pairs = n_pairs; r->last_trials = n_trials;
 	return BT_OK;
 }
 
@@ -263,7 +265,7 @@ extern "C" int bt_ransac_reserve(bt_ctx* ctx, int max_pairs, int max_pts, int ma
 	BT_TRY(r->best.alloc(sizeof(unsigned long long) * max_pairs));
 	BT_TRY(r->best_trial.alloc(sizeof(int32_t) * max_pairs));
 	BT_TRY(r->h_pairs.reserve(sizeof(RansacPair) * max_pairs));
-	r->table_seed = ~0ull; r->table_trials = 0;
+	r->table_seed = ~0ull; r->table_trials = 0; r->last_pairs = r->last_trials = 0;
 	r->max_pairs = max_pairs; r->max_pts = max_pts; r->max_trials = max_trials;
 	r->ready = true;
 	return BT_OK;
@@ -296,5 +298,25 @@ extern "C" int bt_ransac_debug(bt_ctx* ctx, float* u3_out, int n_trials, int32_t
 	BT_CUDA(cudaDeviceSynchronize());
 	if (u3_out) BT_CUDA(cudaMemcpy(u3_out, r->table.p, sizeof(float) * 3 * std::min(n_trials, r->table_trials), cudaMemcpyDeviceToHost));
 	if (best_trial_out) BT_CUDA(cudaMemcpy(best_trial_out, r->best_trial.p, sizeof(int32_t) * std::min(n_pairs, r->max_pairs), cudaMemcpyDeviceToHost));
+	return BT_OK;
+}
+
+// Debug/parity aid: one pair's per-trial poses ([n_trials][12], row-major [R | t]) and good flags of the last call (n_trials at most that
+// call's), and the inlier count its winning key holds (-1 when no trial finished).
+extern "C" int bt_ransac_debug_trials(bt_ctx* ctx, int pair, int n_trials, float* poses_out, int32_t* good_out, int32_t* best_count_out) {
+	RansacState* r;
+	BT_TRY(state_of(ctx, &bt_ctx::ransac, "bt_ransac_debug_trials", "bt_ransac_reserve", &r));
+	BT_REQUIRE(pair >= 0 && pair < r->last_pairs, BT_ERR_INVALID_ARG, "bt_ransac_debug_trials: pair %d of a last call with %d pairs", pair, r->last_pairs);
+	BT_REQUIRE(n_trials >= 0 && n_trials <= r->last_trials, BT_ERR_INVALID_ARG, "bt_ransac_debug_trials: %d trials, the last call ran %d", n_trials, r->last_trials);
+	BT_CUDA(cudaDeviceSynchronize());
+	const int nt = n_trials;
+	const size_t row = (size_t)pair * r->last_trials;
+	if (poses_out && nt) BT_CUDA(cudaMemcpy(poses_out, r->poses.as<float>() + row * 12, sizeof(float) * 12 * nt, cudaMemcpyDeviceToHost));
+	if (good_out && nt) BT_CUDA(cudaMemcpy(good_out, r->good.as<int>() + row, sizeof(int32_t) * nt, cudaMemcpyDeviceToHost));
+	if (best_count_out) {
+		unsigned long long key;
+		BT_CUDA(cudaMemcpy(&key, r->best.as<unsigned long long>() + pair, sizeof(key), cudaMemcpyDeviceToHost));
+		*best_count_out = key == 0ull ? -1 : (int32_t)(key >> 32);
+	}
 	return BT_OK;
 }

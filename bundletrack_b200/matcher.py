@@ -106,6 +106,20 @@ class Ransac(_lib.Facade):
         _lib.check(self.lib.bt_ransac_debug(self.ctx, _lib.ptr(u3), n_trials, _lib.ptr(bt), n_pairs), "bt_ransac_debug")
         return u3, bt
 
+    def debug_trials(self, pair: int, n_trials: int):
+        """Pair `pair` of the last call: (poses [n_trials, 3, 4] float32 [R | t], good [n_trials] int32, the winner's inlier count or -1)."""
+        return ransac_debug_trials(self.lib, self.ctx, pair, n_trials)
+
+
+def ransac_debug_trials(lib, ctx, pair: int, n_trials: int):
+    """bt_ransac_debug_trials on any context that ran RANSAC (a Ransac facade or the matcher chain of a MatchPipeline)."""
+    import numpy as np
+    poses = np.zeros((n_trials, 3, 4), np.float32)
+    good = np.zeros(n_trials, np.int32)
+    cnt = ctypes.c_int32(0)
+    _lib.check(lib.bt_ransac_debug_trials(ctx, pair, n_trials, _lib.ptr(poses), _lib.ptr(good), ctypes.byref(cnt)), "bt_ransac_debug_trials")
+    return poses, good, cnt.value
+
 
 class MatchPipeline(_DescPool):
     """The matcher half of the hot path, device-resident: SiftManager::findCorres for a batch of frame pairs

@@ -233,6 +233,10 @@ BT_API int bt_ransac_pairs(bt_ctx* ctx, int n_pairs, const float* const* ptsA, c
 /* Parity aid: the three uniforms per trial the sampler used (same values as curand_uniform after
  * curand_init(seed, trial, 0)) and the winning trial id of every pair of the last call. */
 BT_API int bt_ransac_debug(bt_ctx* ctx, float* u3_out, int n_trials, int32_t* best_trial_out, int n_pairs);
+/* Parity aid: for pair `pair` of the last call (bt_ransac_pairs or the matcher chain), every trial's pose (poses_out [n_trials][12],
+ * row-major [R | t]; a trial that is not good leaves its row as it was) and good flag (a model was fitted) of the first n_trials trials,
+ * and the inlier count the winner was chosen with (-1 when no trial finished).  n_trials above the last call's is refused (BT_ERR_INVALID_ARG).  NULL outputs are skipped. */
+BT_API int bt_ransac_debug_trials(bt_ctx* ctx, int pair, int n_trials, float* poses_out, int32_t* good_out, int32_t* best_count_out);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Geometric pruning + "mutual" union + the fused matcher pipeline.  Replaces SiftManager::pruneMatches and

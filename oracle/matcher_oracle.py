@@ -127,6 +127,254 @@ def ransac_pair(A, B, u3, dist_thresh):
     return np.nonzero(dist <= dist_thresh)[0].astype(np.int32), best, counts
 
 
+def ransac_sample_ids(u3, n):
+    """The ids every trial samples from n points: roundf(u * (float)(n - 1)), the product in float32 and rounded half away from zero
+    (k_ransac_model).  [n_trials, 3] int64; all zero when n < 1."""
+    p = np.asarray(u3, np.float32) * np.float32(max(n - 1, 0))
+    return np.floor(p.astype(np.float64) + 0.5).astype(np.int64)
+
+
+def ransac_expected_good(A, B, ids, n):
+    """good as k_ransac_model sets it for finite fits: n >= 3, three distinct ids, all six sample points finite."""
+    A = np.asarray(A, np.float32)[:, :3]
+    B = np.asarray(B, np.float32)[:, :3]
+    if n < 3:
+        return np.zeros(len(ids), bool)
+    distinct = (ids[:, 0] != ids[:, 1]) & (ids[:, 1] != ids[:, 2]) & (ids[:, 0] != ids[:, 2])
+    finite = np.isfinite(A[ids]).all((1, 2)) & np.isfinite(B[ids]).all((1, 2))
+    return distinct & finite
+
+
+def kabsch64(s, d):
+    """Float64 least-squares rigid fit of d ~ R s + t (det R = +1) and its residual sum of squares."""
+    s = np.asarray(s, np.float64)
+    d = np.asarray(d, np.float64)
+    sm, dm = s.mean(0), d.mean(0)
+    U, _, Vt = np.linalg.svd((s - sm).T @ (d - dm))
+    D = np.diag([1.0, 1.0, np.sign(np.linalg.det(Vt.T @ U.T)) or 1.0])
+    R = Vt.T @ D @ U.T
+    t = dm - R @ sm
+    return R, t, float(((d - (s @ R.T + t)) ** 2).sum())
+
+
+# ------------------------------------------------------------------------------ exact float32 arithmetic (round to nearest even)
+def f32_round(x):
+    """The float32 nearest to the rational x (ties to even; overflow to +-inf; subnormals kept), as a Python float."""
+    from fractions import Fraction
+    if x == 0:
+        return 0.0
+    x = Fraction(x)
+    sign, a = (-1.0, -x) if x < 0 else (1.0, x)
+    e = a.numerator.bit_length() - a.denominator.bit_length()
+    if Fraction(2) ** e > a:
+        e -= 1
+    q = max(e, -126) - 23                       # the unit in the last place at a's binade
+    m = a / Fraction(2) ** q
+    r = m.numerator // m.denominator
+    rem = m - r
+    if rem > Fraction(1, 2) or (rem == Fraction(1, 2) and r % 2 == 1):
+        r += 1
+    v = float(Fraction(r) * Fraction(2) ** q)
+    if v > float(np.finfo(np.float32).max):
+        return sign * float("inf")
+    return sign * v
+
+
+def f32_fma(a, b, c):
+    from fractions import Fraction
+    if not all(np.isfinite([a, b, c])):
+        return float(np.float32(np.float64(a) * np.float64(b) + np.float64(c)))
+    return f32_round(Fraction(a) * Fraction(b) + Fraction(c))
+
+
+def f32_mul(a, b):
+    return f32_fma(a, b, 0.0) if np.isfinite([a, b]).all() else float(np.float32(a) * np.float32(b))
+
+
+def f32_add(a, b):
+    from fractions import Fraction
+    if not np.isfinite([a, b]).all():
+        return float(np.float32(a) + np.float32(b))
+    return f32_round(Fraction(a) + Fraction(b))
+
+
+RANSAC_ORDERS = ("kernel", "plain", "plain_squares", "plain_model")
+
+
+def ransac_d2_exact(P, a, b, order="kernel"):
+    """One point's squared distance under the float32 pose P [3, 4] exactly as float32 code computes it.
+    order="kernel": k_ransac_eval's documented order, m = fma(P2, az, fma(P0, ax, P1 * ay)) + P3, d = b - m, d2 = fma(dz, dz, fma(dx, dx,
+    dy * dy)) (k_ransac_inliers is the same expression as nvcc contracts it).  Without contraction every product and sum rounds on its
+    own: m = ((P0 ax + P1 ay) + P2 az) + P3 and d2 = (dx^2 + dy^2) + dz^2.  order="plain" takes both uncontracted, "plain_squares" only
+    d2 and "plain_model" only m."""
+    P = [[float(v) for v in row] for row in np.asarray(P, np.float32)]
+    a = [float(v) for v in np.asarray(a, np.float32)[:3]]
+    b = [float(v) for v in np.asarray(b, np.float32)[:3]]
+    fused_m = order in ("kernel", "plain_squares")
+    fused_sq = order in ("kernel", "plain_model")
+    d = []
+    for r in range(3):
+        if fused_m:
+            m = f32_add(f32_fma(P[r][2], a[2], f32_fma(P[r][0], a[0], f32_mul(P[r][1], a[1]))), P[r][3])
+        else:
+            m = f32_add(f32_add(f32_add(f32_mul(P[r][0], a[0]), f32_mul(P[r][1], a[1])), f32_mul(P[r][2], a[2])), P[r][3])
+        d.append(f32_add(b[r], -m))
+    if fused_sq:
+        return f32_fma(d[2], d[2], f32_fma(d[0], d[0], f32_mul(d[1], d[1])))
+    return f32_add(f32_add(f32_mul(d[0], d[0]), f32_mul(d[1], d[1])), f32_mul(d[2], d[2]))
+
+
+def sqrt_le_max(th):
+    """bt_common.cuh's sqrt_le_max: the largest float32 d with sqrtf(d) <= th (sqrtf correctly rounded), -1 when none, +inf for +inf."""
+    th = np.float32(th)
+    if not th > 0:
+        return np.float32(0.0) if th == 0 else np.float32(-1.0)
+    if np.isinf(th):
+        return np.float32(np.inf)
+    with np.errstate(over="ignore"):
+        d = np.float32(th * th)
+    while d > 0 and np.sqrt(d) > th:
+        d = np.nextafter(d, np.float32(-np.inf))
+    while np.sqrt(np.nextafter(d, np.float32(np.inf))) <= th:
+        d = np.nextafter(d, np.float32(np.inf))
+    return d
+
+
+IN, OUT, MARGINAL = 1, 0, 2
+_U = 2.0 ** -24
+
+
+def ransac_classify(poses, A, B, thresh):
+    """Every point under each float32 pose (poses [T, 3, 4] or one [3, 4]): IN / OUT by the kernel's decision d2 <= sqrt_le_max(thresh),
+    MARGINAL when that decision depends on how the float32 expression is contracted (an order of RANSAC_ORDERS decides otherwise than
+    the kernel's).  Returns (decision [T, n] bool, the kernel's, and status [T, n] IN / OUT / MARGINAL), without the T axis for one pose.
+
+    A float64 evaluation from the float32 inputs decides every point outside a band around d2_max that bounds the float32 error: each
+    coordinate of m = P a + t rounds at most 4 times and d = b - m once more, so |d_float32 - d| <= E = 8 u (sum_i |P_ri a_i| + |t_r| + |b_r|),
+    and d2 moves by at most 2 |d| E + E^2 plus 4 u d2 for its own roundings (the band is twice that).  Points inside the band are evaluated
+    exactly (ransac_d2_exact) in every order.  At +inf every point whose d2 is not NaN passes, overflowed or not."""
+    one = np.asarray(poses).ndim == 2
+    P = np.asarray(poses, np.float32).reshape(-1, 3, 4)
+    d2_max = float(sqrt_le_max(thresh))
+    A = np.asarray(A, np.float32)[:, :3]
+    B = np.asarray(B, np.float32)[:, :3]
+    P64, A64, B64 = P.astype(np.float64), A.astype(np.float64), B.astype(np.float64)
+    with np.errstate(all="ignore"):
+        d = B64[None] - (np.einsum("tij,nj->tni", P64[:, :, :3], A64) + P64[:, None, :, 3])
+        d2 = (d * d).sum(2)
+        E = 8.0 * _U * (np.einsum("tij,nj->tni", np.abs(P64[:, :, :3]), np.abs(A64)) + np.abs(P64[:, None, :, 3]) + np.abs(B64)[None]).max(2)
+        band = 2.0 * (2.0 * np.sqrt(d2) * E + E * E + 4.0 * _U * d2)
+        if d2_max == float("inf"):
+            decision = ~np.isnan(d2)
+            near = np.zeros_like(decision)
+        else:
+            decision = d2 <= d2_max
+            near = np.isfinite(d2) & (np.abs(d2 - d2_max) <= band)
+    status = np.where(decision, IN, OUT).astype(np.int8)
+    for t, i in zip(*np.nonzero(near)):
+        k = ransac_d2_exact(P[t], A[i], B[i], "kernel") <= d2_max
+        alt = [ransac_d2_exact(P[t], A[i], B[i], o) <= d2_max for o in RANSAC_ORDERS[1:]]
+        decision[t, i] = k
+        status[t, i] = MARGINAL if any(x != k for x in alt) else (IN if k else OUT)
+    return (decision[0], status[0]) if one else (decision, status)
+
+
+def counts_from_poses(A, B, poses, good, thresh, batch=64):
+    """Every trial's inlier count restated under its own float32 pose (poses [T, 3, 4], good [T]): (counts [T] int64, counts of marginal
+    points [T] int64).  Trials that are not good count 0."""
+    T = len(good)
+    counts = np.zeros(T, np.int64)
+    marg = np.zeros(T, np.int64)
+    g = np.nonzero(np.asarray(good) != 0)[0]
+    if len(g) == 0:
+        return counts, marg
+    P = np.ascontiguousarray(np.asarray(poses, np.float32)[g]).reshape(len(g), 12)
+    uniq, inv = np.unique(P.view(np.uint32), axis=0, return_inverse=True)      # trials with bit-equal poses are restated once
+    uc, um = np.zeros(len(uniq), np.int64), np.zeros(len(uniq), np.int64)
+    for s in range(0, len(uniq), batch):
+        dec, st = ransac_classify(uniq[s:s + batch].view(np.float32).reshape(-1, 3, 4), A, B, thresh)
+        uc[s:s + batch] = dec.sum(1)
+        um[s:s + batch] = (st == MARGINAL).sum(1)
+    counts[g] = uc[inv.ravel()]
+    marg[g] = um[inv.ravel()]
+    return counts, marg
+
+
+def ransac_winner(counts, good):
+    """(max count, lowest trial among those with it) over the good trials, as the device's 64-bit key picks it; (-1, -1) without one."""
+    g = np.nonzero(np.asarray(good) != 0)[0]
+    if len(g) == 0:
+        return -1, -1
+    c = np.asarray(counts)[g]
+    return int(g[np.argmax(c)]), int(c.max())
+
+
+def ransac_model_f32(s, d, sweeps=8):
+    """k_ransac_model's fit in float32, operation by operation (no fused multiply-adds; rsqrtf and sqrtf correctly rounded): Horn's 4x4
+    profile matrix and `sweeps` cyclic Jacobi sweeps.  s, d: [3, 3] float32 samples.  Returns the [3, 4] pose or None (not finite)."""
+    f = np.float32
+    with np.errstate(all="ignore"):
+        s = np.asarray(s, f)
+        d = np.asarray(d, f)
+        sm = ((s[0] + s[1]) + s[2]) / f(3)
+        dm = ((d[0] + d[1]) + d[2]) / f(3)
+        S = np.zeros((3, 3), f)
+        for k in range(3):
+            a, b = s[k] - sm, d[k] - dm
+            for i in range(3):
+                for j in range(3):
+                    S[i, j] = f(S[i, j] + f(a[i] * b[j]))
+        N = np.zeros((4, 4), f)
+        N[0, 0] = (S[0, 0] + S[1, 1]) + S[2, 2]
+        N[0, 1] = N[1, 0] = S[1, 2] - S[2, 1]
+        N[0, 2] = N[2, 0] = S[2, 0] - S[0, 2]
+        N[0, 3] = N[3, 0] = S[0, 1] - S[1, 0]
+        N[1, 1] = (S[0, 0] - S[1, 1]) - S[2, 2]
+        N[1, 2] = N[2, 1] = S[0, 1] + S[1, 0]
+        N[1, 3] = N[3, 1] = S[2, 0] + S[0, 2]
+        N[2, 2] = (-S[0, 0] + S[1, 1]) - S[2, 2]
+        N[2, 3] = N[3, 2] = S[1, 2] + S[2, 1]
+        N[3, 3] = (-S[0, 0] - S[1, 1]) + S[2, 2]
+        V = np.eye(4, dtype=f)
+        for _ in range(sweeps):
+            off = f(0)
+            for p in range(4):
+                for r in range(p + 1, 4):
+                    off = f(off + f(N[p, r] * N[p, r]))
+            if off < f(1e-22):
+                break
+            for p in range(3):
+                for r in range(p + 1, 4):
+                    apq = N[p, r]
+                    if abs(apq) < f(1e-30):
+                        continue
+                    theta = f((N[r, r] - N[p, p]) / f(f(2) * apq))
+                    t = f((f(1) if theta >= 0 else f(-1)) / f(abs(theta) + np.sqrt(f(f(theta * theta) + f(1)))))
+                    c = f(f(1) / np.sqrt(f(f(t * t) + f(1))))
+                    sn = f(t * c)
+                    for M, rows in ((N, True), (N, False), (V, True)):
+                        if rows:      # columns p, r of every row
+                            x, y = M[:, p].copy(), M[:, r].copy()
+                            M[:, p], M[:, r] = f(c * x) - f(sn * y), f(sn * x) + f(c * y)
+                        else:
+                            x, y = M[p, :].copy(), M[r, :].copy()
+                            M[p, :], M[r, :] = f(c * x) - f(sn * y), f(sn * x) + f(c * y)
+        best = 0
+        for k in range(1, 4):
+            if N[k, k] > N[best, best]:
+                best = k
+        q = V[:, best]
+        qn = f(f(1) / np.sqrt(f(f(f(q[0] * q[0]) + f(q[1] * q[1])) + f(q[2] * q[2])) + f(q[3] * q[3])))
+        w, x, y, z = (f(v * qn) for v in q)
+        R = np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)],
+                      [2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)],
+                      [2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]], f)
+        if not np.isfinite(R).all():
+            return None
+        t = (dm - R @ sm).astype(f)
+    return np.concatenate([R, t[:, None]], 1).astype(f)
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 def _cloud_point(depth, K, u, v):
     """Frame::depthToCloudAndNormals (/root/reference/src/Frame.cpp:199-233): K^-1 (u d, v d, d), zeros wherever !(d >= 0.1): below

@@ -100,7 +100,7 @@ def _cases(dev):
     rng = np.random.default_rng(3)
     pa = rng.normal(size=(200, 4)).astype(np.float32)
     r = Ransac(ctx=ctx, max_pairs=2, max_pts=256, max_trials=100)
-    yield ("ransac", "bt_ransac_reserve", ["bt_ransac_pairs", "bt_ransac_debug"],
+    yield ("ransac", "bt_ransac_reserve", ["bt_ransac_pairs", "bt_ransac_debug", "bt_ransac_debug_trials"],
            lambda: host(r.ransac_pairs([t(pa)], [t(pa + 0.001)], n_trials=100, dist_thresh=0.01)), lambda: lib.bt_ransac_reserve(ctx, 4, 1024, 200))
     # pipeline, match cache, map-point table: one findCorres call on fresh state
     w = synth.make_window(31, n_frames=3, n_corr=10)
