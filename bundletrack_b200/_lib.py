@@ -148,6 +148,10 @@ class MatchVizDesc(ctypes.Structure):
     ]
 
 
+class TsdfParams(ctypes.Structure):
+    _fields_ = [("voxel", ctypes.c_float), ("trunc", ctypes.c_float)]
+
+
 class DescView(ctypes.Structure):
     _fields_ = [
         ("dev", ctypes.c_void_p),
@@ -271,6 +275,7 @@ PROTOTYPES = {
     "bt_tracker_state": (_i, (_p, _p, _p, _p, _i, _p)),
     "bt_tracker_usage": (_i, (_p, _p, _p, _p, _p)),
     "bt_tracker_last_fg": (_i, (_p, _p)),
+    "bt_tracker_frame_depth": (_i, (_p, _i, _p)),
     "bt_metrics_reserve": (_i, (_p, _i, _i)),
     "bt_pose_metrics": (_i, (_p, _p, _i, _p, _p, _i, _p, _p, _p)),
     "bt_vocap": (_i, (_p, _i, _d, _p)),
@@ -283,6 +288,10 @@ PROTOTYPES = {
     "bt_match_viz_shape": (_i, (_p, _p, _p, _p)),
     "bt_match_viz_reserve": (_i, (_p, _i, _i)),
     "bt_match_viz": (_i, (_p, _i, _P(MatchVizDesc), _p, _p)),
+    "bt_recon_reserve": (_i, (_p, _i, _i, _i, _ll, _i, _i)),
+    "bt_tsdf_fuse": (_i, (_p, _i, _p, _p, _f, _f, _f, _f, _i, _i, _p, _p)),
+    "bt_tsdf_mesh": (_i, (_p, _p, _p, _p, _p, _p)),
+    "bt_tsdf_grid": (_i, (_p, _p, _p, _p, _p, _p)),
     "bt_lfnet_weights_size": (_i, (_p, _p)),
     "bt_lfnet_reserve": (_i, (_p, _p, _i)),
     "bt_lfnet_load_weights": (_i, (_p, _p, _sz)),

@@ -161,6 +161,7 @@ struct OverlayState;  // overlay.cu
 struct MatchVizState; // matchviz.cu
 struct LfnetState;    // lfnet.cu
 struct VosState;      // vos.cu
+struct ReconState;    // recon.cu
 
 // The context owns the module states; each module defines the deleter of its state next to it, so the states stay private to their files.
 struct StateDeleter {
@@ -177,6 +178,7 @@ struct StateDeleter {
 	void operator()(MatchVizState*) const;
 	void operator()(LfnetState*) const;
 	void operator()(VosState*) const;
+	void operator()(ReconState*) const;
 };
 template <class T> using StatePtr = std::unique_ptr<T, StateDeleter>;
 
@@ -199,6 +201,7 @@ struct bt_ctx {
 	bt::StatePtr<bt::MatchVizState> matchviz;
 	bt::StatePtr<bt::LfnetState> lfnet;
 	bt::StatePtr<bt::VosState> vos;
+	bt::StatePtr<bt::ReconState> recon;
 };
 
 namespace bt {

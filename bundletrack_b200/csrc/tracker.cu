@@ -476,6 +476,14 @@ extern "C" int bt_tracker_last_fg(bt_tracker* t, const uint8_t** fg_dev) {
 	return BT_OK;
 }
 
+extern "C" int bt_tracker_frame_depth(bt_tracker* t, int frame_id, const float** depth_dev) {
+	BT_REQUIRE(t && depth_dev, BT_ERR_INVALID_ARG, "bt_tracker_frame_depth: NULL argument");
+	const auto it = t->alive.find(frame_id);
+	BT_REQUIRE(it != t->alive.end(), BT_ERR_INVALID_ARG, "bt_tracker_frame_depth: frame %d is not alive", frame_id);
+	*depth_dev = tr_depth(t, it->second.slot);
+	return BT_OK;
+}
+
 extern "C" int bt_tracker_usage(bt_tracker* t, int* n_points, int* n_pairs_cached, long long* n_entries_cached, void* stream) {
 	BT_REQUIRE(t && n_points && n_pairs_cached && n_entries_cached, BT_ERR_INVALID_ARG, "bt_tracker_usage: NULL argument");
 	BT_CUDA(cudaSetDevice(t->ctx->device));

@@ -423,7 +423,7 @@ class LogWriter:
 # ---- the run --------------------------------------------------------------------------------------------------------------------------------
 
 def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max_keyframes: int = None, device: int = 0, prefetch: int = 2,
-                 log: int = 0, masks=None):
+                 log: int = 0, masks=None, model_out: str = None):
     """Tracks every frame the loader yields (Bundler::processNewFrame) and writes <out_dir>/poses/<id_str>.txt for each one with
     policy.save_pose_txt (Bundler::saveNewframeResult runs after every frame): the initial pose of a frame that fails the ROI gate, the
     pose drop_frame reports when detection fails, otherwise end_frame's.  features(id_str, request uint8 [400,400,3] host, roi) returns
@@ -435,7 +435,10 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
     log > 0 (the yml's LOG): every frame's LOG images under out_dir (the reference's debug_dir), drawn on the device with the pose its pose
     file holds (overlay.Overlay over loader.model_path) and written by a LogWriter thread; needs cv2.  log = 0 runs none of it.
     masks (vos.VosSource): each frame's object mask is propagated on the device from the first frame's, on the tracker's stream, over the
-    frames the loader yields in order; the loader's mask files are not read."""
+    frames the loader yields in order; the loader's mask files are not read.
+    model_out (a path): after the last frame, the keyframes' depth maps are fused with their final poses into a TSDF on the tracker's stream
+    (recon.fuse_keyframes at recon.VOXEL / TRUNC) and its zero surface is written there as a binary PLY, in the model
+    frame (the object's frame when the loader's first pose is its ob_in_cam0).  None runs none of it; tracking is the same either way."""
     import torch
     from .tracker import Tracker
     n = len(loader)
@@ -513,6 +516,8 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
             writer.close()
         if masks is not None:
             masks.flush()
+        if model_out is not None:
+            _write_model(trk, loader.K, H, W, device, stream, model_out)
     finally:
         if reader is not None:
             reader.close()
@@ -526,6 +531,18 @@ def run_sequence(loader, yml, features, out_dir: str, max_feats: int = 2000, max
             ovl.close()
         trk.close()
     return out
+
+
+def _write_model(trk, K, H: int, W: int, device: int, stream, path: str) -> None:
+    """The keyframes fused and meshed on the tracker's stream, the mesh written to path (recon.py)."""
+    from . import recon
+    tsdf = recon.Tsdf(max(1, int(trk.state()[2].sum())), H, W, device=device, stream=stream.cuda_stream)
+    try:
+        recon.fuse_keyframes(trk, tsdf, K)
+        verts, faces = tsdf.mesh()
+    finally:
+        tsdf.close()
+    recon.write_ply(path, verts, faces)
 
 
 def summary(result) -> str:

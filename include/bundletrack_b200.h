@@ -547,6 +547,11 @@ BT_API int bt_tracker_usage(bt_tracker* t, int* n_points, int* n_pairs_cached, l
  * the ROI gate or was dropped included.  Valid until the next begin_frame on the tracker's stream; read it with work enqueued on that stream
  * before then (bt_pose_overlay for the reference's LOG frames).  BT_ERR_INVALID_ARG before the first begin_frame. */
 BT_API int bt_tracker_last_fg(bt_tracker* t, const uint8_t** fg_dev);
+/* The processed depth (DEVICE float32 H*W, metres, 0 = none or masked out: what the solver reads) of frame frame_id, which must be alive
+ * (bt_tracker_state lists it).  Valid until the frame is released: for a keyframe, until the tracker is destroyed; otherwise until a later
+ * end_frame slides it out of the deque.  Read it with work enqueued on the tracker's stream (bt_tsdf_fuse for an object model).
+ * BT_ERR_INVALID_ARG for a NULL argument or an id that is not alive. */
+BT_API int bt_tracker_frame_depth(bt_tracker* t, int frame_id, const float** depth_dev);
 
 /* ---- pose accuracy: the reference's evaluation (scripts/Utils.py add / adi, scripts/eval_ycbineoat.py VOCap) -------------------------
  * bt_pose_metrics: per frame f, ADD = mean_i |gt_f p_i - pred_f p_i| and ADD-S = mean_i min_j |gt_f p_i - pred_f p_j| over the model points p,
@@ -662,6 +667,43 @@ BT_API int bt_match_viz_reserve(bt_ctx* ctx, int max_images, int max_matches);
  * a bad ROI, n < 0, more than 2^31 - 1 tiles of 32 x 32 output pixels in all, or a context without bt_match_viz_reserve;
  * BT_ERR_CAPACITY beyond the reserved images or matches. */
 BT_API int bt_match_viz(bt_ctx* ctx, int n_images, const bt_match_viz_desc* desc, uint8_t* const* out_dev, void* stream);
+
+/* ---- object model from a tracking run: a TSDF of depth maps in the model frame, and its zero surface (DESIGN.md §3.14) -----------------
+ * bt_tsdf_fuse: fuses n_frames depth maps into a truncated signed distance field on a grid in the model frame, float32 with every operation
+ * rounded on its own, so the grid is bit-reproducible (oracle/recon_oracle.py restates it):
+ *   - the grid spans the axis-aligned box of every valid pixel (finite depth > 0) of every frame, back-projected and moved into the model frame,
+ *     with m = ceil(trunc / voxel) + 1 samples of margin on every side: origin = lo - m voxel, n_a = ceil((hi_a - lo_a) / voxel) + 1 + 2 m,
+ *     sample i at origin + i voxel;
+ *   - per sample, frames in the order given: c = R^T (p - t); skipped when c_z <= 0, when the nearest pixel (floor(u + 0.5), floor(v + 0.5))
+ *     is outside the image or has depth d <= 0 (masked-out pixels are 0 and never carve), or when sdf = d - c_z < -trunc; otherwise
+ *     sum += min(1, sdf / trunc) and count += 1.
+ *   depth_dev     HOST array of n_frames DEVICE pointers to float32 H*W depth (metres, 0 = none), e.g. bt_tracker_frame_depth's.
+ *   cam_in_model  HOST row-major 4 x 4 cam->model per frame (bt_tracker_state's poses), n_frames back to back, finite.
+ *   p             voxel (the sample spacing) and trunc, in metres, positive and finite.
+ * Synchronises `stream` once, to read the bounds back (the grid's size decides what runs); the integration is then enqueued on `stream`.
+ * BT_ERR_INVALID_ARG for a NULL pointer, n_frames < 1, sizes < 1, bad params or intrinsics, a non-finite pose element, no valid pixel in any
+ * frame, or a context without bt_recon_reserve.  BT_ERR_CAPACITY for more frames or a larger image than reserved, or a grid of more than
+ * max_voxels samples (the message names the dims and the bounds); both leave the previous grid as it was.
+ * bt_tsdf_mesh: the zero surface of f = sum / count over the samples with count >= 1 (f < 0 inside), by marching tetrahedra: every cube split
+ * into the six tets of its (0,0,0)-(1,1,1) diagonal, so the surface is closed wherever it is observed; a tet takes part when its four corners
+ * are observed.  A vertex lies on one of the 7 edge directions {x, y, z, xy, xz, yz, xyz} of its edge's lower sample and is stored once, at
+ * t = fa / (fa - fb) from that sample; vertices come in (sample, direction) order, faces in (cube, tet, triangle) order, wound so that their
+ * normals point to f > 0 (free space).  Two calls on one grid give the same bytes.
+ *   verts_dev     DEVICE float32 [max_vertices x 3]; faces_dev DEVICE int32 [max_faces x 3] (indices into verts).
+ *   n_verts / n_faces  HOST: the counts, written also when they exceed the reserve.
+ * Synchronises `stream` once, to read the counts back; the outputs are written on `stream` after it.  BT_ERR_INVALID_ARG for a NULL pointer
+ * or before a successful bt_tsdf_fuse; BT_ERR_CAPACITY, with the outputs untouched, for more than max_vertices vertices or max_faces faces.
+ * bt_tsdf_grid: the last fused grid (a parity aid): dims (3 ints), origin (3 floats), the bounds of the valid pixels (min x y z, max x y z)
+ * and the DEVICE sum (float32) and count (int32) arrays, sample (i, j, k) at i + n_x (j + n_y k), valid until the next fuse or reserve on the
+ * context.  Any output may be NULL.  BT_ERR_INVALID_ARG before a successful bt_tsdf_fuse.
+ * bt_recon_reserve: room for max_frames frames (1..65535) of up to H x W per fuse and a grid of max_voxels samples (8..2^27): 24 B per sample
+ * on the device.  max_vertices / max_faces bound a mesh call's outputs. */
+typedef struct { float voxel, trunc; } bt_tsdf_params;
+BT_API int bt_recon_reserve(bt_ctx* ctx, int max_frames, int H, int W, long long max_voxels, int max_vertices, int max_faces);
+BT_API int bt_tsdf_fuse(bt_ctx* ctx, int n_frames, const float* const* depth_dev, const float* cam_in_model, float fx, float fy, float cx, float cy,
+                        int H, int W, const bt_tsdf_params* p, void* stream);
+BT_API int bt_tsdf_mesh(bt_ctx* ctx, float* verts_dev, int32_t* faces_dev, int* n_verts, int* n_faces, void* stream);
+BT_API int bt_tsdf_grid(bt_ctx* ctx, int* dims, float* origin, float* bounds, const float** sum_dev, const int32_t** count_dev);
 
 /* ---- LF-Net on the device: Lfnet::detectFeature's feature server (lf-net-release/run_server.py) without TensorFlow ----------------------
  * The network run_server.py builds at train_lfnet.py's defaults (DESIGN.md §3.12): mso_resnet_detector with use_nms3d, soft_scale and

@@ -37,6 +37,8 @@ def main():
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--log", type=int, default=0, help="the config's LOG: > 0 also writes every frame's overlay images under the output "
                                                        "directory (<id>/color_viz.jpg, color_viz/, color_raw/); needs cv2")
+    ap.add_argument("--save_model", default=None, metavar="PATH", help="after the last frame, fuse the keyframes' depth into a TSDF on the "
+                                                                      "device and write its surface to PATH as a binary PLY, in the object's frame")
     a = ap.parse_args()
     loader = NocsScene(a.nocs_dir, a.scene_id, a.model_name, a.mask_dir)
     if (a.init_mask or a.mask_save_dir) and not a.vos_model:
@@ -55,7 +57,8 @@ def main():
     else:
         client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
     try:
-        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, f"{a.model_name}_{a.scene_id}"), device=a.device, log=a.log, masks=masks)
+        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, f"{a.model_name}_{a.scene_id}"), device=a.device, log=a.log, masks=masks,
+                           model_out=a.save_model)
     finally:
         client.close()
         if masks is not None:

@@ -35,6 +35,8 @@ def main():
     ap.add_argument("--log", type=int, default=0, help="the config's LOG: > 0 also writes every frame's overlay images under the output "
                                                        "directory (<id>/color_viz.jpg, color_viz/, color_raw/); needs cv2")
     ap.add_argument("--model_dir", default=None, help="the object's OBJ file (the config's model_dir), drawn by --log")
+    ap.add_argument("--save_model", default=None, metavar="PATH", help="after the last frame, fuse the keyframes' depth into a TSDF on the "
+                                                                      "device and write its surface to PATH as a binary PLY, in the object's frame")
     a = ap.parse_args()
     if not os.path.isdir(a.data_dir):
         raise SystemExit(f"--data_dir {a.data_dir} is not a directory")
@@ -56,7 +58,8 @@ def main():
     else:
         client = LfnetClient(f"tcp://127.0.0.1:{a.port}")
     try:
-        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, video), device=a.device, log=a.log, masks=masks)
+        res = run_sequence(loader, a.config, client, os.path.join(a.out_dir, video), device=a.device, log=a.log, masks=masks,
+                           model_out=a.save_model)
     finally:
         client.close()
         if masks is not None:
