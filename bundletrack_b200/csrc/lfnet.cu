@@ -5,6 +5,7 @@
 #include <errno.h>
 #include <math.h>
 #include "bt_common.cuh"
+#include "bt_scan.cuh"
 
 namespace bt {
 namespace {
@@ -299,28 +300,10 @@ __global__ void __launch_bounds__(256) k_nms(const float* __restrict__ heat, flo
 // row-major order (tf.where).  Each thread owns one contiguous run of pixels, so thread order is pixel order for both scans.
 constexpr int TOPK_THREADS = 1024;
 __device__ __forceinline__ unsigned okey(float v) { const unsigned u = __float_as_uint(v); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
-__device__ int block_excl_scan(int v, int* sh, int* total) {
-	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	int inc = v;
-	for (int o = 1; o < 32; o <<= 1) { const int n = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += n; }
-	if (lane == 31) sh[warp] = inc;
-	__syncthreads();
-	if (warp == 0) {
-		int w = lane < TOPK_THREADS / 32 ? sh[lane] : 0, wi = w;
-		for (int o = 1; o < 32; o <<= 1) { const int n = __shfl_up_sync(0xffffffffu, wi, o); if (lane >= o) wi += n; }
-		sh[lane] = wi - w;
-		if (lane == 31) sh[32] = wi;
-	}
-	__syncthreads();
-	const int r = sh[warp] + inc - v;
-	*total = sh[32];
-	__syncthreads();
-	return r;
-}
 __global__ void __launch_bounds__(TOPK_THREADS) k_topk(const float* __restrict__ score, const uint8_t* __restrict__ peak, int k, int2* __restrict__ kint,
                                                        int32_t* __restrict__ n_out) {
 	__shared__ int hist[256];
-	__shared__ int sh[33];
+	__shared__ int sh[TOPK_THREADS / 32];
 	__shared__ unsigned s_prefix;
 	__shared__ int s_remaining;
 	const int f = blockIdx.x;

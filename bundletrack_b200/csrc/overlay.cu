@@ -20,6 +20,7 @@
 #include <math.h>
 #include <limits.h>
 #include "bt_common.cuh"
+#include "bt_scan.cuh"
 
 namespace bt {
 
@@ -43,9 +44,6 @@ struct CloudGrid {
 
 struct OverlayFrame { float P[12]; };              // ob_in_cam rows 0..2
 
-// monotone map of a float to a signed int (and back): integer min / max order floats
-__device__ __forceinline__ int ord(float f) { const int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
-__device__ __forceinline__ float unord(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
 __device__ __forceinline__ bool finite3(float x, float y, float z) { return isfinite(x) && isfinite(y) && isfinite(z); }
 
 __global__ void k_vox_init(CloudGrid* __restrict__ g, int n_clouds) {
@@ -60,7 +58,7 @@ __device__ __forceinline__ void minmax_tile(float x, float y, float z, bool vali
 	if (threadIdx.x < 3) { s[threadIdx.x] = INT_MAX; s[3 + threadIdx.x] = INT_MIN; }
 	__syncthreads();
 	if (valid && finite3(x, y, z)) {
-		const int ox = ord(x), oy = ord(y), oz = ord(z);
+		const int ox = ordered_key(x), oy = ordered_key(y), oz = ordered_key(z);
 		atomicMin(&s[0], ox); atomicMin(&s[1], oy); atomicMin(&s[2], oz);
 		atomicMax(&s[3], ox); atomicMax(&s[4], oy); atomicMax(&s[5], oz);
 	}
@@ -121,7 +119,7 @@ __global__ void k_vox_grid(CloudGrid* __restrict__ g, int n_clouds, float inv) {
 	double cells = 1.0;
 	int div[3];
 	for (int a = 0; a < 3; a++) {
-		const float lo = unord(G.mn[a]), hi = unord(G.mx[a]);
+		const float lo = ordered_float(G.mn[a]), hi = ordered_float(G.mx[a]);
 		const float span = __fmul_rn(__fsub_rn(hi, lo), inv);
 		cells *= (span >= 9.2e18f ? 9.2e18 : (double)((long long)span + 1));
 		G.min_b[a] = (int)floorf(__fmul_rn(lo, inv));
@@ -180,21 +178,9 @@ __global__ void __launch_bounds__(kScanThreads) k_scan(const uint32_t* __restric
 	const int tid = threadIdx.x;
 	const int per = (n + kScanThreads - 1) / kScanThreads;
 	const int b = min(n, tid * per), e = min(n, b + per);
-	uint32_t sum = 0;
+	uint32_t sum = 0, total;
 	for (int i = b; i < e; i++) sum += in[i];
-	// block exclusive scan of the per-thread sums
-	const int lane = tid & 31, w = tid >> 5;
-	uint32_t v = sum;
-	for (int o = 1; o < 32; o <<= 1) { const uint32_t u = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += u; }
-	if (lane == 31) s_w[w] = v;
-	__syncthreads();
-	if (w == 0) {
-		uint32_t x = s_w[lane];
-		for (int o = 1; o < 32; o <<= 1) { const uint32_t u = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += u; }
-		s_w[lane] = x;
-	}
-	__syncthreads();
-	uint32_t run = v - sum + (w > 0 ? s_w[w - 1] : 0u);
+	uint32_t run = block_excl_scan(sum, s_w, &total);
 	for (int i = b; i < e; i++) { const uint32_t c = in[i]; out[i] = run; run += c; }
 	if (tid == kScanThreads - 1) out[n] = run;
 }

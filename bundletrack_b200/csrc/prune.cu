@@ -22,6 +22,7 @@
 #include <map>
 #include <vector>
 #include "bt_common.cuh"
+#include "bt_scan.cuh"
 
 namespace bt {
 
@@ -186,7 +187,7 @@ __global__ void __launch_bounds__(1024) k_emit_entryj(const PrunePair* __restric
                                                        const int32_t* __restrict__ inlier_ids, const int32_t* __restrict__ n_inliers,
                                                        bt_entryj* __restrict__ entry_out, int32_t* __restrict__ n_entry_out, int32_t* __restrict__ entry_off_out, int32_t* total_out, int capacity,
                                                        int32_t* __restrict__ status_out) {
-	__shared__ int s_scan[1024];
+	__shared__ int s_scan[32];
 	__shared__ int s_carry;
 	const int tid = threadIdx.x;
 	if (tid == 0) s_carry = 0;
@@ -195,11 +196,9 @@ __global__ void __launch_bounds__(1024) k_emit_entryj(const PrunePair* __restric
 		const int p = base + tid;
 		int cnt = 0;
 		if (p < n_pairs) { cnt = n_inliers[p]; if (cnt < 5) cnt = 0; }     // fewer than 5 matches => cleared
-		s_scan[tid] = cnt;
-		__syncthreads();
-		for (int o = 1; o < 1024; o <<= 1) { const int v = (tid >= o) ? s_scan[tid - o] : 0; __syncthreads(); s_scan[tid] += v; __syncthreads(); }
+		int total;
 		const int matched = cnt;
-		int excl = s_scan[tid] - cnt + s_carry;
+		int excl = block_excl_scan(cnt, s_scan, &total) + s_carry;
 		// never describe more than the caller's buffer holds: a pair that does not fit is cut (or dropped), so the (offset, count)
 		// arrays a caller hands on as bt_window::block_off / block_n always stay inside entry_out
 		if (excl > capacity) excl = capacity;
@@ -212,7 +211,7 @@ __global__ void __launch_bounds__(1024) k_emit_entryj(const PrunePair* __restric
 			if (status_out) status_out[p] = matched > 0 ? BT_PAIR_OK : (abs(pairs[p].A.frame_id - pairs[p].B.frame_id) == 1 ? BT_PAIR_FAIL : BT_PAIR_EMPTY);
 		}
 		__syncthreads();
-		if (tid == 1023) s_carry += s_scan[1023];
+		if (tid == 1023) s_carry += total;
 		__syncthreads();
 	}
 	if (tid == 0) *total_out = min(s_carry, capacity);

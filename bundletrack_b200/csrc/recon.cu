@@ -19,6 +19,7 @@
 #include <math.h>
 #include <limits.h>
 #include "bt_common.cuh"
+#include "bt_scan.cuh"
 
 namespace bt {
 
@@ -39,10 +40,6 @@ struct Grid {
 	float fx, fy, cx, cy;
 	int H, W;
 };
-
-// monotone map of a float to a signed int (and back): integer min / max order floats
-__device__ __forceinline__ int ord(float f) { const int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
-int unord_host(int i) { return i >= 0 ? i : i ^ 0x7fffffff; }
 
 __device__ __forceinline__ float coord(const Grid& g, int a, int i) { return __fadd_rn(g.origin[a], __fmul_rn((float)i, g.voxel)); }
 
@@ -66,8 +63,8 @@ __global__ void __launch_bounds__(kThreads) k_bounds(const float* const* __restr
 #pragma unroll
 			for (int a = 0; a < 3; a++) {
 				const float p = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(P.R[3 * a], c[0]), __fmul_rn(P.R[3 * a + 1], c[1])), __fmul_rn(P.R[3 * a + 2], c[2])), P.t[a]);
-				atomicMin(&s[a], ord(p));
-				atomicMax(&s[3 + a], ord(p));
+				atomicMin(&s[a], ordered_key(p));
+				atomicMax(&s[3 + a], ordered_key(p));
 			}
 		}
 	}
@@ -228,28 +225,12 @@ __global__ void __launch_bounds__(kThreads) k_mt_block_sums(const uint32_t* __re
 // exclusive scan of the block totals in one CTA; blk[n] = the totals
 __global__ void __launch_bounds__(kScanTopThreads) k_mt_scan_top(int2* __restrict__ blk, int n) {
 	__shared__ int2 s_w[kScanTopThreads / 32];
-	const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+	const int tid = threadIdx.x;
 	const int per = (n + kScanTopThreads - 1) / kScanTopThreads;
 	const int b = min(n, tid * per), e = min(n, b + per);
-	int2 sum = make_int2(0, 0);
+	int2 sum = make_int2(0, 0), total;
 	for (int i = b; i < e; i++) { sum.x += blk[i].x; sum.y += blk[i].y; }
-	int2 x = sum;
-	for (int o = 1; o < 32; o <<= 1) {
-		const int ux = __shfl_up_sync(0xffffffffu, x.x, o), uy = __shfl_up_sync(0xffffffffu, x.y, o);
-		if (lane >= o) { x.x += ux; x.y += uy; }
-	}
-	if (lane == 31) s_w[w] = x;
-	__syncthreads();
-	if (w == 0) {
-		int2 y = s_w[lane];
-		for (int o = 1; o < 32; o <<= 1) {
-			const int ux = __shfl_up_sync(0xffffffffu, y.x, o), uy = __shfl_up_sync(0xffffffffu, y.y, o);
-			if (lane >= o) { y.x += ux; y.y += uy; }
-		}
-		s_w[lane] = y;
-	}
-	__syncthreads();
-	int2 run = make_int2(x.x - sum.x + (w > 0 ? s_w[w - 1].x : 0), x.y - sum.y + (w > 0 ? s_w[w - 1].y : 0));
+	int2 run = block_excl_scan(sum, s_w, &total);
 	for (int i = b; i < e; i++) { const int2 c = blk[i]; blk[i] = run; run.x += c.x; run.y += c.y; }
 	if (tid == kScanTopThreads - 1) blk[n] = run;
 }
@@ -264,11 +245,8 @@ __global__ void __launch_bounds__(kThreads) k_mt_offsets(const uint32_t* __restr
 	for (int r = 0; r < kScanItems; r++) {
 		const long long v = base + r * kThreads + tid;
 		const int cv = v < nv ? __popc(mask[v]) : 0, cf = v < nv ? ntri[v] : 0;
-		int xv = cv, xf = cf;
-		for (int o = 1; o < 32; o <<= 1) {
-			const int uv = __shfl_up_sync(0xffffffffu, xv, o), uf = __shfl_up_sync(0xffffffffu, xf, o);
-			if (lane >= o) { xv += uv; xf += uf; }
-		}
+		const int2 x = warp_incl_scan(make_int2(cv, cf));
+		const int xv = x.x, xf = x.y;
 		if (lane == 31) { s_v[w] = xv; s_f[w] = xf; }
 		__syncthreads();
 		int bv = run.x, bf = run.y, tv = 0, tf = 0;
@@ -421,10 +399,7 @@ extern "C" int bt_tsdf_fuse(bt_ctx* ctx, int n_frames, const float* const* depth
 	BT_CUDA(cudaStreamSynchronize(stream));                 // the call's one synchronisation: the grid's size decides what runs next
 	BT_REQUIRE(hb[0] != INT_MAX, BT_ERR_INVALID_ARG, "bt_tsdf_fuse: no frame has a valid depth pixel");
 	float lo[3], hi[3];
-	for (int a = 0; a < 3; a++) {
-		const int l = unord_host(hb[a]), u = unord_host(hb[3 + a]);
-		memcpy(&lo[a], &l, 4); memcpy(&hi[a], &u, 4);
-	}
+	for (int a = 0; a < 3; a++) { lo[a] = ordered_float(hb[a]); hi[a] = ordered_float(hb[3 + a]); }
 	// float32 on the host, one rounding per operation (oracle/recon_oracle.py: grid)
 	const int m = (int)ceilf(p->trunc / p->voxel) + 1;
 	long long n[3], total = 1;

@@ -42,6 +42,7 @@
 #include <stdlib.h>
 #include <chrono>
 #include "bt_common.cuh"
+#include "bt_scan.cuh"
 
 namespace bt {
 
@@ -463,22 +464,11 @@ __device__ int build_frame_maps(const FrameGeom& g, const float* __restrict__ de
 		// ---- exclusive scan of the rounds*32 counts in (round, warp) order: two entries per thread
 		const int n = rounds * 32;
 		const int v0 = (2 * tid < n) ? s_cnt[2 * tid] : 0, v1 = (2 * tid + 1 < n) ? s_cnt[2 * tid + 1] : 0;
-		int incl = v0 + v1;
-#pragma unroll
-		for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
-		if (lane == 31) s_wt[wid] = incl;
-		__syncthreads();
-		if (wid == 0) {
-			int t = s_wt[lane];
-#pragma unroll
-			for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, t, o); if (lane >= o) t += u; }
-			s_wt[lane] = t;
-		}
-		__syncthreads();
-		const int excl = base + incl - (v0 + v1) + (wid ? s_wt[wid - 1] : 0);
+		int total;
+		const int excl = base + block_excl_scan(v0 + v1, s_wt, &total);
 		if (2 * tid < n) s_cnt[2 * tid] = excl;
 		if (2 * tid + 1 < n) s_cnt[2 * tid + 1] = excl + v0;
-		base += s_wt[31];
+		base += total;
 		__syncthreads();
 		// ---- sweep 2: texel map + source records at their final offsets
 #pragma unroll 2
@@ -607,7 +597,7 @@ __device__ __forceinline__ int chunks_for(int n, int chunk, int& per) {
 // Runs on the LAST CTA of k_prep_frames to finish (1024 threads): per-window tile counts -> scans -> flat tile list.
 __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw) {
 	__shared__ int s_cnt[1024];
-	__shared__ int s_scan[1024];
+	__shared__ int s_wtot[32];
 	__shared__ int s_carry;
 	__shared__ unsigned long long s_px;
 	const int tid = threadIdx.x;
@@ -669,26 +659,10 @@ __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw) {
 		// (2) exclusive scan of the per-window tile counts: the dense tiles plus ONE sparse tile (the window's moment sums), first in line
 		int cnt = 0;
 		if (tid < nw) { cnt = s_cnt[tid] + kSparseTiles; a.tiles_done[base + tid] = 0; a.iter_done[base + tid] = 0; }
-		{   // inclusive scan over the 1024 per-window counts: warp shuffles + one pass over the 32 warp totals
-			__shared__ int s_wtot[32];
-			int incl = cnt;
-#pragma unroll
-			for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, o); if ((tid & 31) >= o) incl += u; }
-			if ((tid & 31) == 31) s_wtot[tid >> 5] = incl;
-			__syncthreads();
-			if (tid < 32) {
-				int t = s_wtot[tid];
-#pragma unroll
-				for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, t, o); if (tid >= o) t += u; }
-				s_wtot[tid] = t;
-			}
-			__syncthreads();
-			s_scan[tid] = incl + ((tid >> 5) ? s_wtot[(tid >> 5) - 1] : 0);
-			__syncthreads();
-		}
+		int n_tiles;      // the tiles of this block of windows
+		const int excl = s_carry + block_excl_scan(cnt, s_wtot, &n_tiles);
 		PROF_T(2);
-		const int excl = s_scan[tid] - cnt + s_carry;
-		const bool fits = (s_carry + s_scan[1023] <= a.max_tiles);
+		const bool fits = (s_carry + n_tiles <= a.max_tiles);
 		// (3) per-window prefix over its pairs: one warp per window, lanes over pairs
 		if (tid < nw) {
 			wins_rw[base + tid].tile_off = excl;
@@ -696,6 +670,7 @@ __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw) {
 			s_cnt[tid] = excl;      // reuse: window -> tile_off for step (4)
 		}
 		__syncthreads();
+		if (tid == 0) s_carry += n_tiles;      // (every thread has read s_carry)
 		for (int wl = (tid >> 5); wl < nw; wl += 32) {
 			const int w = base + wl, lane = tid & 31;
 			const int poff = a.wins[w].pair_off, np = a.wins[w].n_pairs;
@@ -703,9 +678,7 @@ __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw) {
 			for (int p0 = 0; p0 < np; p0 += 32) {
 				const int p = p0 + lane;
 				const int v = (p < np) ? a.pair_ntile[poff + p] : 0;
-				int incl = v;
-#pragma unroll
-				for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
+				const int incl = warp_incl_scan(v);
 				if (p < np) a.pair_tile0[poff + p] = kSparseTiles + carry + incl - v;      // the first slots of the window are its sparse tiles
 				carry += __shfl_sync(0xffffffffu, incl, 31);
 			}
@@ -734,8 +707,6 @@ __device__ void plan_body(const SolveArgs& a, WinDesc* wins_rw) {
 		}
 		__syncthreads();
 		PROF_T(4);
-		if (tid == 0) s_carry += s_scan[1023];
-		__syncthreads();
 	}
 	if (tid == 0) {
 		*a.n_tiles_total = (s_carry <= a.max_tiles && (long long)s_carry * a.prm.num_iter_outer < 0x7fffff00ll) ? s_carry : -1;   // -1 => capacity error reported by the host

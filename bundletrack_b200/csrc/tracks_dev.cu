@@ -23,6 +23,7 @@
 #include <map>
 #include <vector>
 #include "bt_common.cuh"
+#include "bt_scan.cuh"
 
 namespace bt {
 
@@ -89,29 +90,6 @@ __device__ int scratch_slot(unsigned long long* hk, int cap, unsigned long long 
 	}
 }
 
-// exclusive scan over the block; *total = block sum.  Every thread calls it.
-__device__ int block_scan(int v, int* s /*[33]*/, int* total) {
-	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-	int x = v;
-#pragma unroll
-	for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-	if (lane == 31) s[wid] = x;
-	__syncthreads();
-	if (wid == 0) {
-		const int w = lane < nw ? s[lane] : 0;
-		int t = w;
-#pragma unroll
-		for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, t, o); if (lane >= o) t += y; }
-		s[lane] = t - w;
-		if (lane == 31) s[32] = t;
-	}
-	__syncthreads();
-	const int r = x - v + s[wid];
-	*total = s[32];
-	__syncthreads();
-	return r;
-}
-
 __device__ __forceinline__ float4 src_uv(const TrkSrc& s, int i) {
 	const int j = s.ids ? s.ids[i] : i;
 	const float* p = s.base + (size_t)s.stride * j;
@@ -120,7 +98,7 @@ __device__ __forceinline__ float4 src_uv(const TrkSrc& s, int i) {
 
 __global__ void __launch_bounds__(kTrkThreads) k_trk_update(TrkTable t, int sa, int sb, TrkSrc src, unsigned long long* __restrict__ shk, int* __restrict__ smn,
                                                           int* __restrict__ smx, int scap, TrkEnt* __restrict__ ent, int list_cap, unsigned epoch) {
-	__shared__ int s_scan[33];
+	__shared__ int s_scan[kTrkThreads / 32];
 	__shared__ int s_n, s_S, s_ok, s_nc, s_na, s_nfree, s_next, s_nkA, s_nkB;
 	const int tid = threadIdx.x;
 	if (tid == 0) {
@@ -173,8 +151,8 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_update(TrkTable t, int sa, 
 			fl = (inA && inB) ? E_SKIP : ((inB ? 0 : E_CREATE) | (inA ? 0 : E_NEWA));
 		}
 		int tc, ta;
-		const int rc = block_scan((fl & E_CREATE) ? 1 : 0, s_scan, &tc);
-		const int ra = block_scan((fl & E_NEWA) ? 1 : 0, s_scan, &ta);
+		const int rc = block_excl_scan((fl & E_CREATE) ? 1 : 0, s_scan, &tc);
+		const int ra = block_excl_scan((fl & E_NEWA) ? 1 : 0, s_scan, &ta);
 		if (i < n) { ent[i].flags = fl; ent[i].rc = carry_c + rc; ent[i].ra = carry_a + ra; }
 		carry_c += tc; carry_a += ta;
 	}
@@ -233,7 +211,7 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_update(TrkTable t, int sa, 
 		}
 	}
 	int tot;
-	block_scan(add_obs, s_scan, &tot);
+	block_excl_scan(add_obs, s_scan, &tot);
 	if (tid == 0) {
 		t.n_keys[sa] = s_nkA + s_na; t.n_keys[sb] = s_nkB + s_nc;
 		t.ctr[C_CREATED] += s_nc;
@@ -248,7 +226,7 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_update(TrkTable t, int sa, 
 __global__ void __launch_bounds__(kTrkThreads) k_trk_propagate(TrkTable t, int sa, int sb, const float4* __restrict__ existing, int n_existing,
                                                              float4* __restrict__ out, int capacity, int32_t* __restrict__ n_out) {
 	extern __shared__ unsigned long long s_key[];           // [sort_cap] sort keys, then int payload, int A-order index, uint8 drop of the same length
-	__shared__ int s_scan[33];
+	__shared__ int s_scan[kTrkThreads / 32];
 	__shared__ int s_m;
 	const int tid = threadIdx.x;
 	const int nk = t.n_keys[sa];
@@ -324,7 +302,7 @@ __global__ void __launch_bounds__(kTrkThreads) k_trk_propagate(TrkTable t, int s
 		const int k = base + tid;
 		const bool keep = k < m && !s_drop[k];
 		int tot;
-		const int r = carry + block_scan(keep ? 1 : 0, s_scan, &tot);
+		const int r = carry + block_excl_scan(keep ? 1 : 0, s_scan, &tot);
 		if (keep) {
 			if (r < capacity) {
 				const int4 e = t.keys[(size_t)sa * t.max_keys + s_ord[k]];
