@@ -162,6 +162,7 @@ struct MatchVizState; // matchviz.cu
 struct LfnetState;    // lfnet.cu
 struct VosState;      // vos.cu
 struct ReconState;    // recon.cu
+struct SurfaceState;  // metrics.cu
 
 // The context owns the module states; each module defines the deleter of its state next to it, so the states stay private to their files.
 struct StateDeleter {
@@ -179,6 +180,7 @@ struct StateDeleter {
 	void operator()(LfnetState*) const;
 	void operator()(VosState*) const;
 	void operator()(ReconState*) const;
+	void operator()(SurfaceState*) const;
 };
 template <class T> using StatePtr = std::unique_ptr<T, StateDeleter>;
 
@@ -202,6 +204,7 @@ struct bt_ctx {
 	bt::StatePtr<bt::LfnetState> lfnet;
 	bt::StatePtr<bt::VosState> vos;
 	bt::StatePtr<bt::ReconState> recon;
+	bt::StatePtr<bt::SurfaceState> surface;
 };
 
 namespace bt {

@@ -15,11 +15,13 @@
 //    true nearest neighbour is always reranked; the result is the float64 minimum over all candidates.
 // ADD is the same block's queries against themselves, so one kernel gives both; each block writes one partial sum per metric and a
 // second kernel adds a frame's partials in chunk order: the result depends on n_pts only, not on the grid or the number of frames.
+// The scan itself (nearest_scan) also serves the object model's surface distances, at the end of this file.
 #include <math.h>
 #include <stddef.h>
 #include <algorithm>
 #include <vector>
 #include "bt_common.cuh"
+#include "bt_scan.cuh"
 
 namespace bt {
 
@@ -77,47 +79,18 @@ __global__ void __launch_bounds__(kThreads) k_metrics_prep(const double* __restr
 	if ((threadIdx.x & 31) == 0) atomicMax(pmax_bits, (unsigned long long)__double_as_longlong(r));
 }
 
-// grid (n_frames, ceil(n / kChunk)): block (f, c) takes queries [c kChunk, (c + 1) kChunk) of frame f against the whole model
-__global__ void __launch_bounds__(kThreads) k_pose_metrics(const double* __restrict__ pts, const float4* __restrict__ pts32, int n,
-                                                           const FrameConst* __restrict__ frames, const unsigned long long* __restrict__ pmax_bits,
-                                                           double* __restrict__ part_add, double* __restrict__ part_adds) {
-	__shared__ float4 s_tile[kTile];
-	static_assert(kTile >= kChunk, "the queries pass through the tile buffer");
-	__shared__ double s_fr[kFrameDoubles];
-	__shared__ double s_red[2][kThreads / 32];
-	__shared__ double s_best[kQpt][kThreads];
-	__shared__ float s_m[kQpt][kThreads], s_a[kQpt][kThreads];
-	const int f = blockIdx.x, chunk = blockIdx.y, tid = threadIdx.x;
-	const double* src = reinterpret_cast<const double*>(frames + f);
-	for (int t = tid; t < kFrameDoubles; t += kThreads) s_fr[t] = src[t];
-	__syncthreads();
-	const FrameConst& fr = *reinterpret_cast<const FrameConst*>(s_fr);
-	const double pmax = __longlong_as_double((long long)*pmax_bits);
-	const float kappa = __double2float_ru(fr.kappa);
-	// Only the fp32 query and its threshold stay in registers through the scan.  What the rerank alone needs - the poses, the running minima,
-	// the rounding slack and the best squared float64 distance - lives in shared memory, one slot per thread and query.
-	const volatile double* v_pred = s_fr + offsetof(FrameConst, pred) / sizeof(double);
-	const volatile double* v_gt = s_fr + offsetof(FrameConst, gt) / sizeof(double);
-
-	double sa = 0.0;
-#pragma unroll 1
-	for (int k = 0; k < kQpt; k++) {
-		const int i = chunk * kChunk + k * kThreads + tid;
-		const int ii = min(i, n - 1);          // queries past n repeat the last point and are left out of the sums
-		const double x = pts[3 * (size_t)ii], y = pts[3 * (size_t)ii + 1], z = pts[3 * (size_t)ii + 2];
-		double gx, gy, gz, cx, cy, cz, ux, uy, uz;
-		xform(fr.gt, x, y, z, gx, gy, gz);
-		xform(fr.pred, x, y, z, cx, cy, cz);
-		xform(fr.M, x, y, z, ux, uy, uz);
-		const double d2 = (gx - cx) * (gx - cx) + (gy - cy) * (gy - cy) + (gz - cz) * (gz - cz);
-		if (i < n) sa += sqrt(d2);                         // ADD, in k order
-		// the query's own point is a candidate too: it seeds the running minima
-		s_best[k][tid] = d2;
-		const float4 q = make_float4((float)ux, (float)uy, (float)uz, 0.f);
-		s_tile[k * kThreads + tid] = q;         // the tile is loaded after the queries are in registers
-		s_a[k][tid] = __double2float_ru(2.0 * kU * (sqrt(ux * ux + uy * uy + uz * uz) + pmax) + fr.a_abs);
-		s_m[k][tid] = dist2_f32(q.x, q.y, q.z, pts32[ii]);
-	}
+// The exact nearest-distance scan that ADD-S and the surface distances share.  On entry each thread has seeded its kQpt queries: slot
+// k * kThreads + tid of s_tile holds query k in fp32, s_a[k][tid] its rounding slack a, and s_m[k][tid] / s_best[k][tid] the fp32 and float64
+// squared distances to one candidate.  The scan runs every target of pts32 through the fp32 filter and hands each survivor to `rr`:
+//   rr.target(j, cx, cy, cz)   target j's float64 point, as the rerank compares it;
+//   rr.dist2(k, cx, cy, cz)    the float64 squared distance from query k to that point.
+// On return s_best[k][tid] is the smallest rerank over all candidates.  The whole block calls it.
+template <class Rerank>
+__device__ __forceinline__ void nearest_scan(const float4* __restrict__ pts32, int n, float kappa, float4* s_tile, double (*s_best)[kThreads],
+                                             float (*s_m)[kThreads], float (*s_a)[kThreads], const Rerank& rr) {
+	const int tid = threadIdx.x;
+	// Only the fp32 query and its threshold stay in registers through the scan.  What the rerank alone needs - the running minima, the
+	// rounding slack and the best squared float64 distance - lives in shared memory, one slot per thread and query.
 	float qx[kQpt], qy[kQpt], qz[kQpt], T[kQpt];
 #pragma unroll
 	for (int k = 0; k < kQpt; k++) {
@@ -142,24 +115,78 @@ __global__ void __launch_bounds__(kThreads) k_pose_metrics(const double* __restr
 				hit |= s[k] <= T[k];
 			}
 			if (hit) {
-				const int j = base + t;
-				const double x = pts[3 * (size_t)j], y = pts[3 * (size_t)j + 1], z = pts[3 * (size_t)j + 2];
 				double cx, cy, cz;
-				xform(v_pred, x, y, z, cx, cy, cz);
+				rr.target(base + t, cx, cy, cz);
 #pragma unroll
 				for (int k = 0; k < kQpt; k++) {
 					if (s[k] <= T[k]) {
-						const int ii = min(chunk * kChunk + k * kThreads + tid, n - 1);
-						const double px = pts[3 * (size_t)ii], py = pts[3 * (size_t)ii + 1], pz = pts[3 * (size_t)ii + 2];
-						double gx, gy, gz;
-						xform(v_gt, px, py, pz, gx, gy, gz);
-						s_best[k][tid] = fmin(s_best[k][tid], (gx - cx) * (gx - cx) + (gy - cy) * (gy - cy) + (gz - cz) * (gz - cz));
+						s_best[k][tid] = fmin(s_best[k][tid], rr.dist2(k, cx, cy, cz));
 						if (s[k] < s_m[k][tid]) { s_m[k][tid] = s[k]; T[k] = rerank_threshold(s[k], s_a[k][tid], kappa); }
 					}
 				}
 			}
 		}
 	}
+}
+
+// ADD-S's rerank: |gt p_i - pred p_j|, the reference's expression, with the poses read from shared memory
+struct PoseRerank {
+	const double* pts;
+	const volatile double* pred;
+	const volatile double* gt;
+	int first, n;            // query k of this thread is point min(first + k kThreads, n - 1)
+	__device__ __forceinline__ void target(int j, double& cx, double& cy, double& cz) const {
+		const double x = pts[3 * (size_t)j], y = pts[3 * (size_t)j + 1], z = pts[3 * (size_t)j + 2];
+		xform(pred, x, y, z, cx, cy, cz);
+	}
+	__device__ __forceinline__ double dist2(int k, double cx, double cy, double cz) const {
+		const int ii = min(first + k * kThreads, n - 1);
+		const double px = pts[3 * (size_t)ii], py = pts[3 * (size_t)ii + 1], pz = pts[3 * (size_t)ii + 2];
+		double gx, gy, gz;
+		xform(gt, px, py, pz, gx, gy, gz);
+		return (gx - cx) * (gx - cx) + (gy - cy) * (gy - cy) + (gz - cz) * (gz - cz);
+	}
+};
+
+// grid (n_frames, ceil(n / kChunk)): block (f, c) takes queries [c kChunk, (c + 1) kChunk) of frame f against the whole model
+__global__ void __launch_bounds__(kThreads) k_pose_metrics(const double* __restrict__ pts, const float4* __restrict__ pts32, int n,
+                                                           const FrameConst* __restrict__ frames, const unsigned long long* __restrict__ pmax_bits,
+                                                           double* __restrict__ part_add, double* __restrict__ part_adds) {
+	__shared__ float4 s_tile[kTile];
+	static_assert(kTile >= kChunk, "the queries pass through the tile buffer");
+	__shared__ double s_fr[kFrameDoubles];
+	__shared__ double s_red[2][kThreads / 32];
+	__shared__ double s_best[kQpt][kThreads];
+	__shared__ float s_m[kQpt][kThreads], s_a[kQpt][kThreads];
+	const int f = blockIdx.x, chunk = blockIdx.y, tid = threadIdx.x;
+	const double* src = reinterpret_cast<const double*>(frames + f);
+	for (int t = tid; t < kFrameDoubles; t += kThreads) s_fr[t] = src[t];
+	__syncthreads();
+	const FrameConst& fr = *reinterpret_cast<const FrameConst*>(s_fr);
+	const double pmax = __longlong_as_double((long long)*pmax_bits);
+	const float kappa = __double2float_ru(fr.kappa);
+
+	double sa = 0.0;
+#pragma unroll 1
+	for (int k = 0; k < kQpt; k++) {
+		const int i = chunk * kChunk + k * kThreads + tid;
+		const int ii = min(i, n - 1);          // queries past n repeat the last point and are left out of the sums
+		const double x = pts[3 * (size_t)ii], y = pts[3 * (size_t)ii + 1], z = pts[3 * (size_t)ii + 2];
+		double gx, gy, gz, cx, cy, cz, ux, uy, uz;
+		xform(fr.gt, x, y, z, gx, gy, gz);
+		xform(fr.pred, x, y, z, cx, cy, cz);
+		xform(fr.M, x, y, z, ux, uy, uz);
+		const double d2 = (gx - cx) * (gx - cx) + (gy - cy) * (gy - cy) + (gz - cz) * (gz - cz);
+		if (i < n) sa += sqrt(d2);                         // ADD, in k order
+		// the query's own point is a candidate too: it seeds the running minima
+		s_best[k][tid] = d2;
+		const float4 q = make_float4((float)ux, (float)uy, (float)uz, 0.f);
+		s_tile[k * kThreads + tid] = q;         // the tile is loaded after the queries are in registers
+		s_a[k][tid] = __double2float_ru(2.0 * kU * (sqrt(ux * ux + uy * uy + uz * uz) + pmax) + fr.a_abs);
+		s_m[k][tid] = dist2_f32(q.x, q.y, q.z, pts32[ii]);
+	}
+	const PoseRerank rr{pts, s_fr + offsetof(FrameConst, pred) / sizeof(double), s_fr + offsetof(FrameConst, gt) / sizeof(double), chunk * kChunk + tid, n};
+	nearest_scan(pts32, n, kappa, s_tile, s_best, s_m, s_a, rr);
 
 	// fixed-order sums: the thread's queries in k order, then a shuffle tree per warp, then the warps in order
 	double ss = 0.0;
@@ -576,5 +603,287 @@ extern "C" int bt_nocs_score(const int32_t* cls, const int32_t* scored, const do
 		}
 	}
 	for (int k = 0; k < 4; k++) overall_out[k] = overall[k];
+	return BT_OK;
+}
+
+// ---- object model accuracy: surface samples and exact nearest distances both ways (DESIGN.md §3.15) --------------------------------------
+// Sampling, pinned so that oracle/surface_oracle.py restates it bit for bit:
+//  - per face, w = |(B - A) x (C - A)| (twice the area) in float64, every operation rounded on its own, sums left to right;
+//  - the weight q = floor(w / w_max 2^32), an integer, with w_max the largest w (an integer max of the bits of non-negative doubles);
+//  - the CDF is the 64-bit inclusive prefix sum of q, exact, so its order does not matter; total = the last entry;
+//  - sample k draws h_i = splitmix64 output i from state `seed`, i = 3k, 3k + 1, 3k + 2.  Its position in [0, total) is
+//    ((k 2^32 + (h_3k >> 32)) total) / (N 2^32), integer division, one per stratum of the CDF; its face is the first whose CDF exceeds it,
+//    so a face with q = 0 is never chosen;
+//  - u1, u2 = (h >> 11) 2^-53 of the other two, s = sqrt(u1), and the point is ((1 - s) A + s (1 - u2) B) + s u2 C per coordinate.
+// Distances: the ADD-S scan with the identity as the pose (kappa = 1), reranking |a_i - b_j| as sqrt(((dx dx + dy dy) + dz dz)).
+namespace bt {
+namespace {
+
+constexpr int kFaceThreads = 1024;                 // faces per CDF block
+constexpr int kMaxSurfaceFaces = 1 << 27;          // q <= 2^32 per face, so the total stays below 2^59
+constexpr int kMaxSurfaceSamples = 1 << 27;
+
+// what one sampling call reads back: the CDF's total, and n_faces - f of the lowest face f with a bad index or a non-finite vertex (0: none)
+struct SampleStatus {
+	unsigned long long total, wmax_bits;
+	int bad, pad;
+};
+
+__device__ __forceinline__ unsigned long long splitmix64(unsigned long long seed, unsigned long long i) {
+	unsigned long long z = seed + (i + 1) * 0x9E3779B97F4A7C15ull;
+	z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+	z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+	return z ^ (z >> 31);
+}
+
+__device__ __forceinline__ double3 vert(const double* v, int i) { return make_double3(v[3 * (size_t)i], v[3 * (size_t)i + 1], v[3 * (size_t)i + 2]); }
+
+__global__ void __launch_bounds__(kThreads) k_face_weight(const double* __restrict__ verts, int n_verts, const int32_t* __restrict__ faces, int n_faces,
+                                                          double* __restrict__ w_out, SampleStatus* __restrict__ st) {
+	const int f = blockIdx.x * kThreads + threadIdx.x;
+	if (f >= n_faces) return;
+	const int i0 = faces[3 * (size_t)f], i1 = faces[3 * (size_t)f + 1], i2 = faces[3 * (size_t)f + 2];
+	double w = 0.0;
+	bool ok = i0 >= 0 && i0 < n_verts && i1 >= 0 && i1 < n_verts && i2 >= 0 && i2 < n_verts;
+	if (ok) {
+		const double3 A = vert(verts, i0), B = vert(verts, i1), C = vert(verts, i2);
+		const double ux = sub(B.x, A.x), uy = sub(B.y, A.y), uz = sub(B.z, A.z);
+		const double vx = sub(C.x, A.x), vy = sub(C.y, A.y), vz = sub(C.z, A.z);
+		const double cx = sub(mul(uy, vz), mul(uz, vy)), cy = sub(mul(uz, vx), mul(ux, vz)), cz = sub(mul(ux, vy), mul(uy, vx));
+		w = sqrt(dot3(cx, cy, cz, cx, cy, cz));
+		ok = isfinite(w) && isfinite(A.x + A.y + A.z + B.x + B.y + B.z + C.x + C.y + C.z);
+	}
+	if (!ok) { atomicMax(&st->bad, n_faces - f); w = 0.0; }
+	w_out[f] = w;
+	atomicMax(&st->wmax_bits, (unsigned long long)__double_as_longlong(w));
+}
+
+// per block of kFaceThreads faces: q and its inclusive prefix within the block, and the block's total
+__global__ void __launch_bounds__(kFaceThreads) k_face_cdf(const double* __restrict__ w, int n_faces, const SampleStatus* __restrict__ st,
+                                                           unsigned long long* __restrict__ cdf, unsigned long long* __restrict__ block_tot) {
+	__shared__ unsigned long long s[kFaceThreads / 32];
+	const int f = blockIdx.x * kFaceThreads + threadIdx.x;
+	const double wmax = __longlong_as_double((long long)st->wmax_bits);
+	unsigned long long q = 0;
+	if (f < n_faces && wmax > 0.0) q = __double2ull_rz(__dmul_rn(__ddiv_rn(w[f], wmax), 4294967296.0));
+	unsigned long long tot;
+	const unsigned long long ex = block_excl_scan(q, s, &tot);
+	if (f < n_faces) cdf[f] = ex + q;
+	if (threadIdx.x == 0) block_tot[blockIdx.x] = tot;
+}
+
+// one block: the blocks' offsets (exclusive prefix of their totals, in rounds of kFaceThreads) and the CDF's total
+__global__ void __launch_bounds__(kFaceThreads) k_face_cdf_top(unsigned long long* __restrict__ block_tot, int n_blocks, SampleStatus* __restrict__ st) {
+	__shared__ unsigned long long s[kFaceThreads / 32];
+	unsigned long long carry = 0;
+	for (int base = 0; base < n_blocks; base += kFaceThreads) {
+		const int b = base + threadIdx.x;
+		const unsigned long long v = b < n_blocks ? block_tot[b] : 0;
+		unsigned long long tot;
+		const unsigned long long ex = block_excl_scan(v, s, &tot);
+		if (b < n_blocks) block_tot[b] = carry + ex;
+		carry += tot;
+	}
+	if (threadIdx.x == 0) st->total = carry;
+}
+
+__global__ void __launch_bounds__(kFaceThreads) k_face_cdf_add(unsigned long long* __restrict__ cdf, int n_faces, const unsigned long long* __restrict__ block_off) {
+	const int f = blockIdx.x * kFaceThreads + threadIdx.x;
+	if (f < n_faces) cdf[f] += block_off[blockIdx.x];
+}
+
+__global__ void __launch_bounds__(kThreads) k_mesh_sample(const double* __restrict__ verts, const int32_t* __restrict__ faces,
+                                                          const unsigned long long* __restrict__ cdf, int n_faces, const SampleStatus* __restrict__ st,
+                                                          int n_samples, unsigned long long seed, double* __restrict__ out) {
+	const int k = blockIdx.x * kThreads + threadIdx.x;
+	if (k >= n_samples) return;
+	const unsigned long long total = st->total;
+	const unsigned long long h0 = splitmix64(seed, 3ull * k), h1 = splitmix64(seed, 3ull * k + 1), h2 = splitmix64(seed, 3ull * k + 2);
+	const unsigned long long x = ((unsigned long long)k << 32) + (h0 >> 32);
+	const unsigned long long pos = (unsigned long long)(((unsigned __int128)x * total) / ((unsigned __int128)n_samples << 32));
+	int lo = 0, hi = n_faces - 1;
+	while (lo < hi) {                                  // the first face whose CDF exceeds pos
+		const int mid = (lo + hi) >> 1;
+		if (cdf[mid] > pos) hi = mid;
+		else lo = mid + 1;
+	}
+	const double u1 = (double)(h1 >> 11) * 0x1p-53, u2 = (double)(h2 >> 11) * 0x1p-53;
+	const double s = sqrt(u1);
+	const double b0 = sub(1.0, s), b1 = mul(s, sub(1.0, u2)), b2 = mul(s, u2);
+	const double3 A = vert(verts, faces[3 * (size_t)lo]), B = vert(verts, faces[3 * (size_t)lo + 1]), C = vert(verts, faces[3 * (size_t)lo + 2]);
+	out[3 * (size_t)k] = add(add(mul(b0, A.x), mul(b1, B.x)), mul(b2, C.x));
+	out[3 * (size_t)k + 1] = add(add(mul(b0, A.y), mul(b1, B.y)), mul(b2, C.y));
+	out[3 * (size_t)k + 2] = add(add(mul(b0, A.z), mul(b1, B.z)), mul(b2, C.z));
+}
+
+// The surface's rerank: |q_i - t_j| of two float64 point sets, every operation rounded on its own
+struct PointRerank {
+	const double* q;
+	const double* t;
+	int first, n;            // query k of this thread is point min(first + k kThreads, n - 1)
+	__device__ __forceinline__ void target(int j, double& cx, double& cy, double& cz) const {
+		cx = t[3 * (size_t)j]; cy = t[3 * (size_t)j + 1]; cz = t[3 * (size_t)j + 2];
+	}
+	__device__ __forceinline__ double dist2(int k, double cx, double cy, double cz) const {
+		const int ii = min(first + k * kThreads, n - 1);
+		const double dx = sub(q[3 * (size_t)ii], cx), dy = sub(q[3 * (size_t)ii + 1], cy), dz = sub(q[3 * (size_t)ii + 2], cz);
+		return dot3(dx, dy, dz, dx, dy, dz);
+	}
+};
+
+// grid ceil(n_q / kChunk): d_out[i] = min_j |q_i - t_j| for the block's kChunk queries
+__global__ void __launch_bounds__(kThreads) k_surface_nearest(const double* __restrict__ q, int n_q, const double* __restrict__ t,
+                                                              const float4* __restrict__ t32, int n_t, const unsigned long long* __restrict__ pmax_bits,
+                                                              double* __restrict__ d_out) {
+	__shared__ float4 s_tile[kTile];
+	__shared__ double s_best[kQpt][kThreads];
+	__shared__ float s_m[kQpt][kThreads], s_a[kQpt][kThreads];
+	const int tid = threadIdx.x, first = blockIdx.x * kChunk + tid;
+	const double pmax = __longlong_as_double((long long)*pmax_bits);
+	const PointRerank rr{q, t, first, n_q};
+#pragma unroll 1
+	for (int k = 0; k < kQpt; k++) {
+		const int ii = min(first + k * kThreads, n_q - 1);
+		const double x = q[3 * (size_t)ii], y = q[3 * (size_t)ii + 1], z = q[3 * (size_t)ii + 2];
+		// target min(i, n_t - 1) seeds the running minima (the same index of a set sampled alike lies close by)
+		const int js = min(ii, n_t - 1);
+		double cx, cy, cz;
+		rr.target(js, cx, cy, cz);
+		s_best[k][tid] = rr.dist2(k, cx, cy, cz);
+		const float4 qf = make_float4((float)x, (float)y, (float)z, 0.f);
+		s_tile[k * kThreads + tid] = qf;
+		s_a[k][tid] = __double2float_ru(2.0 * kU * (sqrt(x * x + y * y + z * z) + pmax));
+		s_m[k][tid] = dist2_f32(qf.x, qf.y, qf.z, t32[js]);
+	}
+	nearest_scan(t32, n_t, 1.0f, s_tile, s_best, s_m, s_a, rr);
+#pragma unroll
+	for (int k = 0; k < kQpt; k++) {
+		const int i = first + k * kThreads;
+		if (i < n_q) d_out[i] = sqrt(s_best[k][tid]);
+	}
+}
+
+}  // namespace
+
+struct SurfaceState {
+	bool ready = false;
+	int max_faces = 0, max_samples = 0;
+	DevBuf w, cdf, block, status, pts32, pmax;
+	PinnedBuf h_status;
+};
+void StateDeleter::operator()(SurfaceState* s) const { delete s; }
+
+}  // namespace bt
+
+extern "C" int bt_surface_reserve(bt_ctx* ctx, int max_faces, int max_samples) {
+	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_surface_reserve: ctx is NULL");
+	BT_REQUIRE(max_faces >= 1 && max_faces <= kMaxSurfaceFaces && max_samples >= 1 && max_samples <= kMaxSurfaceSamples, BT_ERR_INVALID_ARG,
+	           "bt_surface_reserve: max_faces %d / max_samples %d must be in 1..%d / 1..%d", max_faces, max_samples, kMaxSurfaceFaces, kMaxSurfaceSamples);
+	SurfaceState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::surface, &s));
+	const size_t nb = (size_t)(max_faces + kFaceThreads - 1) / kFaceThreads;
+	BT_TRY(s->w.alloc(sizeof(double) * (size_t)max_faces));
+	BT_TRY(s->cdf.alloc(sizeof(unsigned long long) * (size_t)max_faces));
+	BT_TRY(s->block.alloc(sizeof(unsigned long long) * nb));
+	BT_TRY(s->status.alloc(sizeof(SampleStatus)));
+	BT_TRY(s->pts32.alloc(2 * sizeof(float4) * (size_t)max_samples));
+	BT_TRY(s->pmax.alloc(2 * sizeof(unsigned long long)));
+	BT_TRY(s->h_status.alloc(sizeof(SampleStatus)));
+	s->max_faces = max_faces; s->max_samples = max_samples;
+	s->ready = true;
+	return BT_OK;
+}
+
+extern "C" int bt_mesh_sample(bt_ctx* ctx, const double* verts_dev, int n_verts, const int32_t* faces_dev, int n_faces, int n_samples, uint64_t seed,
+                              double* pts_out_dev, void* stream_) {
+	BT_REQUIRE(verts_dev && faces_dev && pts_out_dev, BT_ERR_INVALID_ARG, "bt_mesh_sample: NULL argument");
+	BT_REQUIRE(n_verts >= 1 && n_faces >= 1 && n_samples >= 1, BT_ERR_INVALID_ARG, "bt_mesh_sample: n_verts %d / n_faces %d / n_samples %d must be >= 1",
+	           n_verts, n_faces, n_samples);
+	SurfaceState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::surface, "bt_mesh_sample", "bt_surface_reserve", &s));
+	BT_REQUIRE(n_faces <= s->max_faces && n_samples <= s->max_samples, BT_ERR_CAPACITY, "bt_mesh_sample: %d faces / %d samples exceed the reserved %d / %d",
+	           n_faces, n_samples, s->max_faces, s->max_samples);
+	cudaStream_t stream = (cudaStream_t)stream_;
+	SampleStatus* st = s->status.as<SampleStatus>();
+	const int nb = (n_faces + kFaceThreads - 1) / kFaceThreads;
+	BT_CUDA(cudaMemsetAsync(st, 0, sizeof(SampleStatus), stream));
+	k_face_weight<<<(n_faces + kThreads - 1) / kThreads, kThreads, 0, stream>>>(verts_dev, n_verts, faces_dev, n_faces, s->w.as<double>(), st);
+	k_face_cdf<<<nb, kFaceThreads, 0, stream>>>(s->w.as<double>(), n_faces, st, s->cdf.as<unsigned long long>(), s->block.as<unsigned long long>());
+	k_face_cdf_top<<<1, kFaceThreads, 0, stream>>>(s->block.as<unsigned long long>(), nb, st);
+	k_face_cdf_add<<<nb, kFaceThreads, 0, stream>>>(s->cdf.as<unsigned long long>(), n_faces, s->block.as<unsigned long long>());
+	BT_CUDA(cudaGetLastError());
+	SampleStatus* h = s->h_status.as<SampleStatus>();
+	BT_CUDA(cudaMemcpyAsync(h, st, sizeof(SampleStatus), cudaMemcpyDeviceToHost, stream));
+	BT_CUDA(cudaStreamSynchronize(stream));                 // the call's one synchronisation: a bad mesh is refused before the output is touched
+	BT_REQUIRE(h->bad == 0, BT_ERR_INVALID_ARG, "bt_mesh_sample: face %d has a vertex index outside [0, %d) or a non-finite vertex", n_faces - h->bad, n_verts);
+	BT_REQUIRE(h->total > 0, BT_ERR_INVALID_ARG, "bt_mesh_sample: the mesh's %d faces have no area", n_faces);
+	k_mesh_sample<<<(n_samples + kThreads - 1) / kThreads, kThreads, 0, stream>>>(verts_dev, faces_dev, s->cdf.as<unsigned long long>(), n_faces, st,
+	                                                                              n_samples, seed, pts_out_dev);
+	BT_CUDA(cudaGetLastError());
+	return BT_OK;
+}
+
+extern "C" int bt_surface_distances(bt_ctx* ctx, const double* a_dev, int n_a, const double* b_dev, int n_b, double* d_ab_out, double* d_ba_out, void* stream_) {
+	BT_REQUIRE(a_dev && b_dev && d_ab_out && d_ba_out, BT_ERR_INVALID_ARG, "bt_surface_distances: NULL argument");
+	BT_REQUIRE(n_a >= 1 && n_b >= 1, BT_ERR_INVALID_ARG, "bt_surface_distances: n_a %d / n_b %d must be >= 1", n_a, n_b);
+	SurfaceState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::surface, "bt_surface_distances", "bt_surface_reserve", &s));
+	BT_REQUIRE(n_a <= s->max_samples && n_b <= s->max_samples, BT_ERR_CAPACITY, "bt_surface_distances: %d / %d points exceed the reserved %d",
+	           n_a, n_b, s->max_samples);
+	cudaStream_t stream = (cudaStream_t)stream_;
+	float4* a32 = s->pts32.as<float4>();
+	float4* b32 = a32 + s->max_samples;
+	unsigned long long* pmax = s->pmax.as<unsigned long long>();
+	BT_CUDA(cudaMemsetAsync(pmax, 0, 2 * sizeof(unsigned long long), stream));
+	k_metrics_prep<<<(n_a + kThreads - 1) / kThreads, kThreads, 0, stream>>>(a_dev, n_a, a32, pmax);
+	k_metrics_prep<<<(n_b + kThreads - 1) / kThreads, kThreads, 0, stream>>>(b_dev, n_b, b32, pmax + 1);
+	k_surface_nearest<<<(n_a + kChunk - 1) / kChunk, kThreads, 0, stream>>>(a_dev, n_a, b_dev, b32, n_b, pmax + 1, d_ab_out);
+	k_surface_nearest<<<(n_b + kChunk - 1) / kChunk, kThreads, 0, stream>>>(b_dev, n_b, a_dev, a32, n_a, pmax, d_ba_out);
+	BT_CUDA(cudaGetLastError());
+	return BT_OK;
+}
+
+// the p-quantile of sorted x: linear interpolation at position p (n - 1), x[lo] + (pos - lo) (x[lo + 1] - x[lo])
+static double quantile_sorted(const std::vector<double>& x, double p) {
+	const double pos = p * (double)(x.size() - 1);
+	const size_t lo = (size_t)pos;
+	if (lo + 1 >= x.size()) return x.back();
+	return x[lo] + (pos - (double)lo) * (x[lo + 1] - x[lo]);
+}
+
+extern "C" int bt_surface_score(const double* d_ab, int n_a, const double* d_ba, int n_b, const double* taus, int n_taus, double* out) {
+	BT_REQUIRE(d_ab && d_ba && out && (taus || n_taus == 0), BT_ERR_INVALID_ARG, "bt_surface_score: NULL argument");
+	BT_REQUIRE(n_a >= 1 && n_b >= 1 && n_taus >= 0, BT_ERR_INVALID_ARG, "bt_surface_score: n_a %d / n_b %d must be >= 1, n_taus %d >= 0", n_a, n_b, n_taus);
+	for (int t = 0; t < n_taus; t++)
+		BT_REQUIRE(taus[t] > 0.0 && isfinite(taus[t]), BT_ERR_INVALID_ARG, "bt_surface_score: tau %d (%g) must be positive and finite", t, taus[t]);
+	const double* d[2] = {d_ab, d_ba};
+	const int n[2] = {n_a, n_b};
+	double mean[2], med[2], p95[2];
+	for (int s = 0; s < 2; s++) {
+		std::vector<double> x(d[s], d[s] + n[s]);
+		double sum = 0.0;
+		for (int i = 0; i < n[s]; i++) {
+			BT_REQUIRE(x[i] >= 0.0 && isfinite(x[i]), BT_ERR_INVALID_ARG, "bt_surface_score: distance %d of %s (%g) must be finite and >= 0", i,
+			           s ? "d_ba" : "d_ab", x[i]);
+			sum += x[i];
+		}
+		mean[s] = sum / (double)n[s];
+		std::sort(x.begin(), x.end());
+		med[s] = quantile_sorted(x, 0.5);
+		p95[s] = quantile_sorted(x, 0.95);
+	}
+	out[0] = mean[0];
+	out[1] = mean[1];
+	out[2] = (mean[0] + mean[1]) / 2.0;
+	out[3] = med[0]; out[4] = p95[0]; out[5] = med[1]; out[6] = p95[1];
+	for (int t = 0; t < n_taus; t++) {
+		long long c[2] = {0, 0};
+		for (int s = 0; s < 2; s++)
+			for (int i = 0; i < n[s]; i++) c[s] += d[s][i] < taus[t];
+		const double P = (double)c[0] / (double)n_a, R = (double)c[1] / (double)n_b;
+		out[7 + 3 * t] = P;
+		out[8 + 3 * t] = R;
+		out[9 + 3 * t] = P + R > 0.0 ? 2.0 * P * R / (P + R) : 0.0;
+	}
 	return BT_OK;
 }

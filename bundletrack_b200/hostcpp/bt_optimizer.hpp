@@ -226,6 +226,43 @@ inline NocsScore nocsScore(const std::vector<int32_t>& cls, const std::vector<in
 	return s;
 }
 
+// An object model against a reference mesh (DESIGN.md §3.15): both sampled uniformly by area with n_samples points and the same seed, exact
+// nearest distances both ways, and the scores (metres; per tau precision, recall and F-score).  The meshes are compared in the frame they
+// are given in.  Vertices: device double [n x 3], faces: device int32 [m x 3].  The context needs bt_surface_reserve(ctx, >= both face counts,
+// >= n_samples); the samples and distances live in device memory allocated for the call.  Synchronises `stream`.
+struct SurfaceScore {
+	double accuracy, completeness, chamfer, median_model_to_ref, p95_model_to_ref, median_ref_to_model, p95_ref_to_model;
+	std::vector<double> precision, recall, fscore;
+};
+inline SurfaceScore surfaceScore(bt_ctx* ctx, const double* model_verts_gpu, int n_model_verts, const int32_t* model_faces_gpu, int n_model_faces,
+                                 const double* ref_verts_gpu, int n_ref_verts, const int32_t* ref_faces_gpu, int n_ref_faces, int n_samples,
+                                 const std::vector<double>& taus, uint64_t seed = 0, void* stream = nullptr) {
+	struct DevBlock {
+		void* p = nullptr;
+		~DevBlock() { if (p) bt_dev_free(p); }
+	} pts, dist;
+	auto check = [](int rc, const char* what) { if (rc != BT_OK) throw std::runtime_error(std::string(what) + ": " + bt_last_error()); };
+	const size_t n = n_samples > 0 ? (size_t)n_samples : 0;
+	check(bt_dev_alloc(&pts.p, 2 * 3 * sizeof(double) * n), "bt_dev_alloc");
+	check(bt_dev_alloc(&dist.p, 2 * sizeof(double) * n), "bt_dev_alloc");
+	double* a = static_cast<double*>(pts.p);
+	double* d = static_cast<double*>(dist.p);
+	check(bt_mesh_sample(ctx, model_verts_gpu, n_model_verts, model_faces_gpu, n_model_faces, n_samples, seed, a, stream), "bt_mesh_sample");
+	check(bt_mesh_sample(ctx, ref_verts_gpu, n_ref_verts, ref_faces_gpu, n_ref_faces, n_samples, seed, a + 3 * n, stream), "bt_mesh_sample");
+	check(bt_surface_distances(ctx, a, n_samples, a + 3 * n, n_samples, d, d + n, stream), "bt_surface_distances");
+	std::vector<double> h(2 * n), out(7 + 3 * taus.size());
+	check(bt_memcpy_d2h(h.data(), d, sizeof(double) * 2 * n, stream), "bt_memcpy_d2h");
+	check(bt_stream_sync(stream), "bt_stream_sync");
+	check(bt_surface_score(h.data(), n_samples, h.data() + n, n_samples, taus.data(), (int)taus.size(), out.data()), "bt_surface_score");
+	SurfaceScore s{out[0], out[1], out[2], out[3], out[4], out[5], out[6], {}, {}, {}};
+	for (size_t t = 0; t < taus.size(); t++) {
+		s.precision.push_back(out[7 + 3 * t]);
+		s.recall.push_back(out[8 + 3 * t]);
+		s.fscore.push_back(out[9 + 3 * t]);
+	}
+	return s;
+}
+
 // ransacMultiPairGPU with the reference's argument list (device float4 arrays per pair, host result vectors).  The device result
 // buffers and the library's scratch belong to the object: nothing is allocated per call (the reference allocates six arrays and a
 // stream per pair per call, cuda_ransac.cu:1240-1275).

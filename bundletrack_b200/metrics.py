@@ -1,5 +1,6 @@
 """Pose accuracy as BundleTrack is judged: ADD and ADD-S per frame (the reference's scripts/Utils.py add / adi) on the device, and their
 VOCap AUC (scripts/eval_ycbineoat.py) on the host.  A thin ctypes mirror of bt_pose_metrics / bt_vocap (include/bundletrack_b200.h).
+Also the NOCS-REAL275 scores, and an object model's accuracy against a reference mesh (SurfaceScore).
 Poses are ob_in_cam (model -> camera), the matrices poses/<id>.txt holds; `ob_in_cam` turns the tracker's cam -> model poses into them."""
 from __future__ import annotations
 
@@ -141,3 +142,70 @@ def nocs_score(cls, scored, theta_deg, shift, iou):
     p = _lib.ptr
     _lib.check(_lib.load().bt_nocs_score(p(c), p(s), p(t), p(d), p(u), n, p(per), p(ov)), "bt_nocs_score")
     return per, ov
+
+
+# Object model accuracy (DESIGN.md §3.15): both meshes sampled uniformly by area on the device, exact nearest distances both ways, and
+# the scores on the host.  The meshes are compared in the frame they are given in: nothing aligns them, so a tracking error shows.
+SCORE_KEYS = ("accuracy", "completeness", "chamfer", "median_model_to_ref", "p95_model_to_ref", "median_ref_to_model", "p95_ref_to_model")
+
+
+def surface_score(d_ab, d_ba, taus=(0.002, 0.005, 0.01)) -> dict:
+    """bt_surface_score (host code) of the model -> reference distances d_ab and the reference -> model distances d_ba (metres): accuracy
+    (mean d_ab), completeness (mean d_ba), chamfer, the median and p95 of each direction, and per tau precision, recall and F-score."""
+    a = np.ascontiguousarray(np.asarray(d_ab, np.float64).reshape(-1))
+    b = np.ascontiguousarray(np.asarray(d_ba, np.float64).reshape(-1))
+    t = np.ascontiguousarray(np.asarray(taus, np.float64).reshape(-1))
+    out = np.zeros(len(SCORE_KEYS) + 3 * t.size, np.float64)
+    _lib.check(_lib.load().bt_surface_score(_lib.ptr(a), a.size, _lib.ptr(b), b.size, _lib.ptr(t), t.size, _lib.ptr(out)), "bt_surface_score")
+    res = dict(zip(SCORE_KEYS, out[:len(SCORE_KEYS)].tolist()))
+    per = out[len(SCORE_KEYS):].reshape(-1, 3)
+    res.update(taus=t.tolist(), precision=per[:, 0].tolist(), recall=per[:, 1].tolist(), fscore=per[:, 2].tolist())
+    return res
+
+
+class SurfaceScore(_lib.Facade):
+    """A mesh scored against a reference mesh on the device.  Room for meshes of up to max_faces faces and max_samples samples per side
+    is reserved here."""
+
+    def __init__(self, max_faces: int, max_samples: int, device: int = 0, stream: int = 0, ctx=None):
+        super().__init__(ctx, device, stream)
+        self.device = device
+        _lib.check(self.lib.bt_surface_reserve(self.ctx, max_faces, max_samples), "bt_surface_reserve")
+
+    def _dev(self, x, dtype, what: str):
+        import torch
+        t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
+        t = t.to(device=torch.device("cuda", self.device), dtype=dtype).contiguous()
+        if t.dim() != 2 or t.shape[1] != 3:
+            raise ValueError(f"{what}: expected [n, 3], got {list(t.shape)}")
+        return t
+
+    def sample(self, verts, faces, n_samples: int, seed: int = 0):
+        """n_samples points uniform by area on the mesh (verts [V,3], faces [F,3] vertex indices; numpy or CUDA tensors): a float64 CUDA
+        tensor [n_samples, 3], bit-reproducible for a seed."""
+        import torch
+        v = self._dev(verts, torch.float64, "verts")
+        f = self._dev(faces, torch.int32, "faces")
+        out = torch.empty((int(n_samples), 3), dtype=torch.float64, device=v.device)
+        _lib.check(self.lib.bt_mesh_sample(self.ctx, _lib.ptr(v), v.shape[0], _lib.ptr(f), f.shape[0], int(n_samples), int(seed), _lib.ptr(out),
+                                           self.stream), "bt_mesh_sample")
+        return out
+
+    def distances(self, a, b):
+        """(d_ab, d_ba): float64 numpy, d_ab[i] = min_j |a_i - b_j| and d_ba[j] = min_i |b_j - a_i|, exact, for point sets a [n,3] and b [m,3]."""
+        import torch
+        A, B = self._dev(a, torch.float64, "a"), self._dev(b, torch.float64, "b")
+        d_ab = torch.empty(A.shape[0], dtype=torch.float64, device=A.device)
+        d_ba = torch.empty(B.shape[0], dtype=torch.float64, device=A.device)
+        _lib.check(self.lib.bt_surface_distances(self.ctx, _lib.ptr(A), A.shape[0], _lib.ptr(B), B.shape[0], _lib.ptr(d_ab), _lib.ptr(d_ba), self.stream),
+                   "bt_surface_distances")
+        _lib.check(self.lib.bt_stream_sync(self.stream), "bt_stream_sync")
+        return d_ab.cpu().numpy(), d_ba.cpu().numpy()
+
+    def score(self, model_verts, model_faces, ref_verts, ref_faces, n_samples: int = 100_000, taus=(0.002, 0.005, 0.01), seed: int = 0) -> dict:
+        """Both meshes sampled with n_samples points and the same seed, then surface_score of the distances both ways, plus n_samples."""
+        a = self.sample(model_verts, model_faces, n_samples, seed)
+        b = self.sample(ref_verts, ref_faces, n_samples, seed)
+        res = surface_score(*self.distances(a, b), taus)
+        res["n_samples"] = int(n_samples)
+        return res

@@ -3,10 +3,12 @@ tetrahedra.  A thin ctypes mirror of bt_recon_reserve / bt_tsdf_fuse / bt_tsdf_m
 
 - Tsdf: fuse(depths, poses, K, voxel, trunc) and mesh() on a context;
 - fuse_keyframes: a tracker's keyframes, with their current poses and their processed depth, fused on the tracker's stream;
-- write_ply: the mesh as binary little-endian PLY."""
+- write_ply: the mesh as binary little-endian PLY; read_mesh: that PLY, or a Wavefront OBJ (a reference mesh to score the model
+  against, bundletrack_b200.metrics.SurfaceScore)."""
 from __future__ import annotations
 
 import ctypes
+import os
 
 import numpy as np
 
@@ -109,3 +111,73 @@ def write_ply(path: str, verts, faces) -> None:
         out.write(head.encode("ascii"))
         out.write(v.tobytes())
         out.write(rows.tobytes())
+
+
+def _read_obj(path: str):
+    verts, faces = [], []
+    with open(path, "r", errors="replace") as fh:
+        for ln, line in enumerate(fh, 1):
+            tok = line.split()
+            if not tok:
+                continue
+            if tok[0] == "v":
+                verts.append([float(x) for x in tok[1:4]])
+            elif tok[0] == "f":
+                # a / b / c forms keep the vertex index; a negative index counts back from the last vertex so far; polygons are fanned
+                raw = [int(t.split("/")[0]) for t in tok[1:]]
+                idx = [i - 1 if i > 0 else len(verts) + i for i in raw]
+                if len(idx) < 3 or 0 in raw or min(idx) < 0 or max(idx) >= len(verts):
+                    raise ValueError(f"{path}:{ln}: bad face {line.strip()!r} ({len(verts)} vertices so far)")
+                faces += [(idx[0], idx[k], idx[k + 1]) for k in range(1, len(idx) - 1)]
+    return np.asarray(verts, np.float64).reshape(-1, 3), np.asarray(faces, np.int32).reshape(-1, 3)
+
+
+_PLY_TYPES = {"char": "i1", "uchar": "u1", "short": "<i2", "ushort": "<u2", "int": "<i4", "uint": "<u4", "float": "<f4", "double": "<f8",
+              "int8": "i1", "uint8": "u1", "int16": "<i2", "uint16": "<u2", "int32": "<i4", "uint32": "<u4", "float32": "<f4", "float64": "<f8"}
+
+
+def _read_ply(path: str):
+    with open(path, "rb") as fh:
+        data = fh.read()
+    end = data.find(b"end_header\n")
+    if not data.startswith(b"ply\n") or end < 0:
+        raise ValueError(f"{path}: not a PLY file")
+    lines = data[:end].decode("ascii", "replace").splitlines()
+    if "format binary_little_endian 1.0" not in lines:
+        fmt = next((l for l in lines if l.startswith("format")), "format ?")
+        raise ValueError(f"{path}: PLY '{fmt}' is not read, only binary_little_endian (what write_ply writes)")
+    elems = []                                   # (name, count, [(property, type or (count type, index type))])
+    for l in lines:
+        t = l.split()
+        if t and t[0] == "element":
+            elems.append((t[1], int(t[2]), []))
+        elif t and t[0] == "property":
+            elems[-1][2].append((t[-1], (t[2], t[3]) if t[1] == "list" else t[1]))
+    names = [e[0] for e in elems]
+    if names != ["vertex", "face"]:
+        raise ValueError(f"{path}: PLY elements {names} are not read, only vertex then face")
+    (_, nv, vprops), (_, nf, fprops) = elems
+    vdt = np.dtype([(n, _PLY_TYPES[t]) for n, t in vprops])
+    if len(fprops) != 1 or not isinstance(fprops[0][1], tuple) or fprops[0][1][0] not in ("uchar", "uint8"):
+        raise ValueError(f"{path}: the face element must be one 'list uchar <int type>' property")
+    fdt = np.dtype([("n", "u1"), ("i", _PLY_TYPES[fprops[0][1][1]], (3,))])
+    off = end + len(b"end_header\n")
+    v = np.frombuffer(data, vdt, nv, off)
+    rows = np.frombuffer(data, fdt, nf, off + vdt.itemsize * nv)
+    if nf and (rows["n"] != 3).any():
+        raise ValueError(f"{path}: only triangles are read from PLY")
+    f = rows["i"].astype(np.int64)
+    if nf and (f.min() < 0 or f.max() >= nv):
+        raise ValueError(f"{path}: face indices must lie in [0, {nv})")
+    return np.stack([v["x"], v["y"], v["z"]], 1).astype(np.float64), f.astype(np.int32).reshape(-1, 3)
+
+
+def read_mesh(path: str):
+    """(verts float64 [n,3], faces int32 [m,3]) of a Wavefront OBJ (`v` and `f` lines; `f a/b/c` forms, negative indices, polygons split
+    into fans from their first vertex) or of a binary little-endian PLY of triangles as write_ply writes it.  Other files are refused."""
+    ext = os.path.splitext(path)[1].lower()
+    if ext == ".obj":
+        return _read_obj(path)
+    if ext == ".ply":
+        return _read_ply(path)
+    raise ValueError(f"{path}: '{ext or path}' meshes are not read, only .obj and binary .ply")

@@ -602,6 +602,37 @@ BT_API int bt_nocs_metrics(bt_ctx* ctx, const double* pred, const double* gt, co
 BT_API int bt_nocs_score(const int32_t* cls, const int32_t* scored, const double* theta_deg, const double* shift, const double* iou, int n,
                          double* per_class_out, double* overall_out);
 
+/* ---- object model accuracy: a mesh against a reference mesh, in the frame both are given in (no alignment; DESIGN.md §3.15) ----------
+ * bt_mesh_sample: n_samples points on the mesh, uniform by area and reproducible bit for bit (oracle/surface_oracle.py restates it):
+ * per face w = |(B - A) x (C - A)| in float64, the integer weight q = floor(w / max w * 2^32), the exact 64-bit prefix sum of q as the CDF,
+ * and sample k at CDF position ((k 2^32 + (h_3k >> 32)) * total) / (n_samples 2^32) in integer arithmetic, where h_i is splitmix64 output i
+ * from state `seed`; its face is the first whose CDF exceeds the position (a face with q = 0, area 0 included, is never chosen).  The point is
+ * ((1 - s) A + s (1 - u2) B) + s u2 C with s = sqrt(u1), u1, u2 = (h_3k+1 >> 11, h_3k+2 >> 11) * 2^-53, every operation rounded on its own.
+ *   verts_dev     DEVICE float64 n_verts x 3.   faces_dev  DEVICE int32 n_faces x 3 (vertex indices).
+ *   pts_out_dev   DEVICE float64 n_samples x 3, in CDF order (sample k lies on a face no later than sample k + 1's).
+ * Synchronises `stream` once, to read back the face check and the CDF's total; the samples are then written on `stream`.  BT_ERR_INVALID_ARG,
+ * with the output untouched, for a NULL pointer, sizes < 1, a face index outside [0, n_verts) or a non-finite vertex on a face (the message
+ * names the lowest such face), a mesh whose weights are all 0, or a context without bt_surface_reserve; BT_ERR_CAPACITY for more faces or
+ * samples than reserved.
+ * bt_surface_distances: d_ab[i] = min_j |a_i - b_j| and d_ba[j] = min_i |b_j - a_i|, float64 and exact: the ADD-S scan (an fp32 filter with
+ * a proven bound, then |a_i - b_j| = sqrt((dx dx + dy dy) + dz dz) in float64 for every candidate it keeps).
+ *   a_dev / b_dev DEVICE float64 n_a x 3 / n_b x 3, finite.   d_ab_out / d_ba_out  DEVICE float64 [n_a] / [n_b].
+ * Asynchronous on `stream`.  BT_ERR_INVALID_ARG for a NULL pointer, sizes < 1 or a context without bt_surface_reserve; BT_ERR_CAPACITY for
+ * more than max_samples points on either side.
+ * bt_surface_reserve: room for meshes of up to max_faces faces (1..2^27) and point sets of up to max_samples points (1..2^27): 16 B per face
+ * and 32 B per sample on the device. */
+BT_API int bt_surface_reserve(bt_ctx* ctx, int max_faces, int max_samples);
+BT_API int bt_mesh_sample(bt_ctx* ctx, const double* verts_dev, int n_verts, const int32_t* faces_dev, int n_faces, int n_samples, uint64_t seed,
+                          double* pts_out_dev, void* stream);
+BT_API int bt_surface_distances(bt_ctx* ctx, const double* a_dev, int n_a, const double* b_dev, int n_b, double* d_ab_out, double* d_ba_out, void* stream);
+/* The scores of the two directions' distances, host code, no GPU (d_ab: model -> reference, d_ba: reference -> model).  out[0..6]: accuracy
+ * = mean d_ab, completeness = mean d_ba, chamfer = (accuracy + completeness) / 2, then the median and p95 of d_ab and of d_ba; then per
+ * threshold t: out[7 + 3 t] precision = #{d_ab < tau} / n_a, out[8 + 3 t] recall = #{d_ba < tau} / n_b (strictly less), out[9 + 3 t]
+ * F = 2 P R / (P + R), 0 when P + R = 0.  Means sum in index order; a quantile p is x[lo] + (pos - lo) (x[lo + 1] - x[lo]) at pos = p (n - 1)
+ * of the sorted values, lo = floor(pos).  BT_ERR_INVALID_ARG for a NULL pointer (taus may be NULL when n_taus = 0), n_a or n_b < 1,
+ * n_taus < 0, a distance that is negative or not finite, or a tau that is not positive and finite. */
+BT_API int bt_surface_score(const double* d_ab, int n_a, const double* d_ba, int n_b, const double* taus, int n_taus, double* out);
+
 /* ---- tracking overlays: the reference's LOG frames (Bundler::saveNewframeResult, Bundler.cpp:379-411) ---------------------------------
  * bt_voxel_downsample: PCL's VoxelGrid (Utils::downsamplePointCloud, Utils.cpp:134-140; pcl::VoxelGrid::applyFilter with every field
  * averaged and no minimum count) of n_clouds clouds in one call, float32 (DESIGN.md §3.10): the voxel bounds from each cloud's finite
