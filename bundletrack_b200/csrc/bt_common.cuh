@@ -128,24 +128,59 @@ struct Stream {
 	operator cudaStream_t() const { return s; }
 };
 
-// A page-locked block the host fills for an asynchronous upload, and the event recorded behind the copies that read it.  The entry
-// points return before those copies run, so the block is rewritten (acquire) or regrown (reserve) only once the event has passed.
-struct UploadBuf {
-	PinnedBuf buf;
-	Event ev;
-	// the block, at least `bytes` large (0: as reserved), once the last upload from it is done
-	template <class T> int acquire(size_t bytes, T** host) {
-		BT_TRY(ev.sync());
-		BT_TRY(buf.alloc(bytes));
-		*host = buf.as<T>();
+// The tables a call builds on the host for its kernels: typed slices of one block, added in order, each at a multiple of 256 bytes.
+// A module lays out each call shape in one function of its counts; its reserve calls that function with the worst-case counts and every
+// call with its real ones, so whether a call fits its reservation is decided by one piece of arithmetic (TableBlock::begin checks it).
+template <class T> struct Slice {
+	size_t off = 0, n = 0;
+	size_t end() const { return off + sizeof(T) * n; }
+};
+struct TableLayout {
+	size_t total = 0;
+	template <class T> Slice<T> add(size_t n) {
+		const Slice<T> s{total, n};
+		total += (sizeof(T) * n + 255) & ~(size_t)255;
+		return s;
+	}
+};
+
+// The block a call's tables are built in and its device mirror.  NH page-locked blocks used in turn (with 2, a call waits only for the
+// upload of the call before last), each with the event recorded behind the copies that read it, and NM device blocks at the same
+// offsets.  The entry points return before those copies run, so a pinned block is rewritten (begin) or regrown (reserve) only once its
+// event has passed.  The device blocks are allocated first: a reservation too large for the device fails there, before any pinning.
+template <int NH = 1, int NM = 1> struct TableBlock {
+	int reserve(size_t bytes) {
+		for (DevBuf& d : mirror) BT_TRY(d.alloc(bytes));
+		for (int k = 0; k < NH; k++) {
+			if (bytes > pinned[k].bytes) BT_TRY(ev[k].sync());
+			BT_TRY(pinned[k].alloc(bytes));
+		}
 		return BT_OK;
 	}
-	int reserve(size_t bytes) {
-		if (bytes > buf.bytes) BT_TRY(ev.sync());
-		return buf.alloc(bytes);
+	// the next pinned block, once its last upload is done, for tables laid out as L; BT_ERR_CAPACITY when L exceeds the reservation
+	int begin(const char* who, const TableLayout& L) {
+		cur = (cur + 1) % NH;
+		BT_TRY(ev[cur].sync());
+		size_t have = pinned[cur].bytes;
+		for (const DevBuf& d : mirror) have = d.bytes < have ? d.bytes : have;
+		BT_REQUIRE(L.total <= have, BT_ERR_CAPACITY, "%s: tables of %zu bytes exceed the %zu reserved", who, L.total, have);
+		return BT_OK;
 	}
-	// the copies from the block are queued on `stream`
-	int in_flight(cudaStream_t stream) { return ev.record(stream); }
+	template <class T> T* host(const Slice<T>& s) const { return reinterpret_cast<T*>(pinned[cur].template as<char>() + s.off); }
+	template <class T> T* dev(const Slice<T>& s, int m = 0) const { return reinterpret_cast<T*>(mirror[m].template as<char>() + s.off); }
+	// bytes [from, to) of the current pinned block to device block m
+	int send(size_t from, size_t to, cudaStream_t stream, int m = 0) {
+		BT_CUDA(cudaMemcpyAsync(mirror[m].template as<char>() + from, pinned[cur].template as<char>() + from, to - from, cudaMemcpyHostToDevice, stream));
+		return BT_OK;
+	}
+	// the copies from the current pinned block are queued on `stream`
+	int in_flight(cudaStream_t stream) { return ev[cur].record(stream); }
+	cudaEvent_t uploaded() const { return ev[cur]; }
+private:
+	PinnedBuf pinned[NH];
+	Event ev[NH];
+	DevBuf mirror[NM];
+	int cur = 0;
 };
 
 struct SolverState;   // solver.cu

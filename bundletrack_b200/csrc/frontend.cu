@@ -259,14 +259,11 @@ __global__ void __launch_bounds__(FE_THREADS) k_frame_frontend_masked(FrontArgs 
 __global__ void __launch_bounds__(FE_THREADS) k_frame_frontend_masked_u16(FrontArgs a, MaskArgs m) { frontend_tile<true, uint16_t>(a, m); }
 
 struct FrontState {
-	DevBuf tables;
-	UploadBuf h_tables;
-	int cap = 0;
+	TableBlock<> tables;
 	// largest-hull mode scratch (segment.cu), grown on demand: label / pixel-count maps, per-frame winner, the filled hull maps
 	DevBuf seg_label, seg_count, seg_best, seg_fill;
-	// bt_lfnet_request's own pointer tables, so it never waits on or overwrites the front end's
-	DevBuf req_tables;
-	UploadBuf h_req;
+	// bt_lfnet_request's own pointer table, so it never waits on or overwrites the front end's
+	TableBlock<> req_tables;
 };
 void StateDeleter::operator()(FrontState* s) const { delete s; }
 static FrontState* g_front(bt_ctx* ctx, bool create) {
@@ -281,6 +278,22 @@ struct MaskSpec {
 	uint8_t* const* fg_out;         // [n]
 	int32_t* roi_out;               // device [n][4]
 };
+
+// The pointer tables of a front-end call and, when masked, those of the mask and the ROI's initial (9999, 0, 9999, 0) per frame, which
+// goes to the caller's roi_out.  mask_in is the mask the front end dilates: the caller's, or the filled hull.
+struct FrontTables : TableLayout {
+	Slice<const void*> depth_in; Slice<float*> depth_out; Slice<float4*> xyz_out, normal_out;
+	Slice<const uint8_t*> mask, mask_in; Slice<uint8_t*> fg_out; Slice<int32_t> roi;
+};
+static FrontTables front_tables(size_t n_frames, bool masked) {
+	const size_t nm = masked ? n_frames : 0;
+	FrontTables t;
+	t.depth_in = t.add<const void*>(n_frames); t.depth_out = t.add<float*>(n_frames);
+	t.xyz_out = t.add<float4*>(n_frames); t.normal_out = t.add<float4*>(n_frames);
+	t.mask = t.add<const uint8_t*>(nm); t.fg_out = t.add<uint8_t*>(nm); t.mask_in = t.add<const uint8_t*>(nm);
+	t.roi = t.add<int32_t>(4 * nm);
+	return t;
+}
 
 // depth_raw_dev: float metres, or uint16 millimetres when u16 (masked calls only)
 static int frames_preprocess(bt_ctx* ctx, const char* who, int n_frames, const void* const* depth_raw_dev, bool u16, int H, int W, float fx, float fy, float cx, float cy,
@@ -301,47 +314,44 @@ static int frames_preprocess(bt_ctx* ctx, const char* who, int n_frames, const v
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
 	FrontState* s = g_front(ctx, true);
-	// pointer tables: [depth_in | depth_out | xyz_out | normal_out] (+ [mask | fg_out | mask the front end dilates] and the ROI's
-	// initial (9999, 0, 9999, 0) per frame when masked), one pinned block, one upload per destination
-	const int n_tbl = mask ? 7 : 4;
-	const size_t bytes = sizeof(void*) * n_tbl * (size_t)n_frames, roi_bytes = mask ? sizeof(int32_t) * 4 * (size_t)n_frames : 0;
+	const FrontTables t = front_tables(n_frames, mask != nullptr);
 	const size_t hw = (size_t)H * W * n_frames;
 	int rc;
-	if ((rc = s->tables.alloc(bytes)) != BT_OK) return rc;
+	BT_TRY(s->tables.reserve(t.total));
 	if (hull) {
 		if ((rc = s->seg_label.alloc(sizeof(int32_t) * hw)) != BT_OK) return rc;
 		if ((rc = s->seg_count.alloc(sizeof(int32_t) * hw)) != BT_OK) return rc;
 		if ((rc = s->seg_fill.alloc(hw)) != BT_OK) return rc;
 		if ((rc = s->seg_best.alloc(sizeof(unsigned long long) * n_frames)) != BT_OK) return rc;
 	}
-	const void** ht;
-	BT_TRY(s->h_tables.acquire(bytes + roi_bytes, &ht));
+	BT_TRY(s->tables.begin(who, t));
+	const void** h_in = s->tables.host(t.depth_in); float** h_out = s->tables.host(t.depth_out);
+	float4** h_xyz = s->tables.host(t.xyz_out); float4** h_normal = s->tables.host(t.normal_out);
 	bool any_xyz = false;
 	for (int f = 0; f < n_frames; f++) {
 		BT_REQUIRE(depth_raw_dev[f] && depth_out_dev[f] && normal_out_dev[f], BT_ERR_INVALID_ARG, "%s: frame %d has a NULL map", who, f);
 		BT_REQUIRE((const void*)depth_raw_dev[f] != (const void*)depth_out_dev[f], BT_ERR_INVALID_ARG, "%s: frame %d: in-place filtering is not supported (tiles read their neighbours' input)", who, f);
-		ht[f] = depth_raw_dev[f]; ht[n_frames + f] = depth_out_dev[f];
-		ht[2 * n_frames + f] = xyz_out_dev ? xyz_out_dev[f] : nullptr; ht[3 * n_frames + f] = normal_out_dev[f];
+		h_in[f] = depth_raw_dev[f]; h_out[f] = depth_out_dev[f];
+		h_xyz[f] = xyz_out_dev ? (float4*)xyz_out_dev[f] : nullptr; h_normal[f] = (float4*)normal_out_dev[f];
 		any_xyz = any_xyz || (xyz_out_dev && xyz_out_dev[f]);
 		if (mask) {
 			BT_REQUIRE(mask->mask[f] && mask->fg_out[f], BT_ERR_INVALID_ARG, "%s: frame %d has a NULL mask or fg map", who, f);
 			BT_REQUIRE((const void*)mask->mask[f] != (const void*)mask->fg_out[f], BT_ERR_INVALID_ARG, "%s: frame %d: fg_out aliases the mask (tiles read their neighbours' mask)", who, f);
-			ht[4 * n_frames + f] = mask->mask[f]; ht[5 * n_frames + f] = mask->fg_out[f];
-			ht[6 * n_frames + f] = hull ? (const void*)(s->seg_fill.as<uint8_t>() + (size_t)H * W * f) : (const void*)mask->mask[f];
+			s->tables.host(t.mask)[f] = mask->mask[f]; s->tables.host(t.fg_out)[f] = mask->fg_out[f];
+			s->tables.host(t.mask_in)[f] = hull ? s->seg_fill.as<uint8_t>() + (size_t)H * W * f : mask->mask[f];
 		}
 	}
 	if (xyz_out_dev) for (int f = 0; f < n_frames; f++) BT_REQUIRE(!any_xyz || xyz_out_dev[f], BT_ERR_INVALID_ARG, "%s: xyz outputs must be given for all frames or none", who);
-	BT_CUDA(cudaMemcpyAsync(s->tables.p, ht, bytes, cudaMemcpyHostToDevice, stream));
+	BT_TRY(s->tables.send(0, mask ? t.mask_in.end() : t.normal_out.end(), stream));
 	if (mask) {
-		int32_t* hr = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(ht) + bytes);
+		int32_t* hr = s->tables.host(t.roi);
 		for (int f = 0; f < n_frames; f++) { hr[4 * f] = 9999; hr[4 * f + 1] = 0; hr[4 * f + 2] = 9999; hr[4 * f + 3] = 0; }
-		BT_CUDA(cudaMemcpyAsync(mask->roi_out, hr, roi_bytes, cudaMemcpyHostToDevice, stream));
+		BT_CUDA(cudaMemcpyAsync(mask->roi_out, hr, sizeof(int32_t) * 4 * (size_t)n_frames, cudaMemcpyHostToDevice, stream));
 	}
-	BT_TRY(s->h_tables.in_flight(stream));
+	BT_TRY(s->tables.in_flight(stream));
 	FrontArgs a;
-	const void** dt = s->tables.as<const void*>();
-	a.depth_in = dt; a.depth_out = (float* const*)(dt + n_frames);
-	a.xyz_out = any_xyz ? (float4* const*)(dt + 2 * n_frames) : nullptr; a.normal_out = (float4* const*)(dt + 3 * n_frames);
+	a.depth_in = s->tables.dev(t.depth_in); a.depth_out = s->tables.dev(t.depth_out);
+	a.xyz_out = any_xyz ? s->tables.dev(t.xyz_out) : nullptr; a.normal_out = s->tables.dev(t.normal_out);
 	a.H = H; a.W = W;
 	{   // Eigen::Matrix3f::inverse() of [[fx,0,cx],[0,fy,cy],[0,0,1]] (Frame.cpp:189): cofactors times 1/det, in float
 		const float det = fx * fy, invdet = 1.0f / det;
@@ -357,10 +367,10 @@ static int frames_preprocess(bt_ctx* ctx, const char* who, int n_frames, const v
 		if (smem > 48 * 1024) BT_CUDA(cudaFuncSetAttribute(k_frame_frontend, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 		k_frame_frontend<<<grid, FE_THREADS, smem, stream>>>(a);
 	} else {
-		if (hull && (rc = segment_largest_hull((const uint8_t* const*)(dt + 4 * n_frames), n_frames, H, W, s->seg_label.as<int32_t>(), s->seg_count.as<int32_t>(),
+		if (hull && (rc = segment_largest_hull(s->tables.dev(t.mask), n_frames, H, W, s->seg_label.as<int32_t>(), s->seg_count.as<int32_t>(),
 		                                       s->seg_best.as<unsigned long long>(), s->seg_fill.as<uint8_t>(), stream)) != BT_OK) return rc;
 		MaskArgs m;
-		m.mask_in = (const uint8_t* const*)(dt + 6 * n_frames); m.fg_out = (uint8_t* const*)(dt + 5 * n_frames); m.roi = mask->roi_out;
+		m.mask_in = s->tables.dev(t.mask_in); m.fg_out = s->tables.dev(t.fg_out); m.roi = mask->roi_out;
 		auto* k = u16 ? k_frame_frontend_masked_u16 : k_frame_frontend_masked;
 		if (smem > 48 * 1024) BT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 		k<<<grid, FE_THREADS, smem, stream>>>(a, m);
@@ -405,16 +415,16 @@ extern "C" int bt_lfnet_request(bt_ctx* ctx, int n_frames, const uint8_t* const*
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_CUDA(cudaSetDevice(ctx->device));
 	FrontState* s = g_front(ctx, true);
-	const size_t bytes = sizeof(void*) * 3 * (size_t)n_frames;   // [colour | fg | out]
-	int rc;
-	if ((rc = s->req_tables.alloc(bytes)) != BT_OK) return rc;
-	const void** ht;
-	BT_TRY(s->h_req.acquire(bytes, &ht));
+	TableLayout L;
+	const Slice<const void*> tbl = L.add<const void*>(3 * (size_t)n_frames);   // [colour | fg | out]
+	BT_TRY(s->req_tables.reserve(L.total));
+	BT_TRY(s->req_tables.begin("bt_lfnet_request", L));
+	const void** ht = s->req_tables.host(tbl);
 	for (int f = 0; f < n_frames; f++) {
 		BT_REQUIRE(colour_dev[f] && fg_dev[f] && request_out_dev[f], BT_ERR_INVALID_ARG, "bt_lfnet_request: frame %d has a NULL image", f);
 		ht[f] = colour_dev[f]; ht[n_frames + f] = fg_dev[f]; ht[2 * n_frames + f] = request_out_dev[f];
 	}
-	BT_CUDA(cudaMemcpyAsync(s->req_tables.p, ht, bytes, cudaMemcpyHostToDevice, stream));
-	BT_TRY(s->h_req.in_flight(stream));
-	return launch_lfnet_request(s->req_tables.as<const void*>(), roi_dev, n_frames, H, W, stream);
+	BT_TRY(s->req_tables.send(0, tbl.end(), stream));
+	BT_TRY(s->req_tables.in_flight(stream));
+	return launch_lfnet_request(s->req_tables.dev(tbl), roi_dev, n_frames, H, W, stream);
 }

@@ -751,8 +751,8 @@ struct MatcherState {
 	int slot_rows = 0;                      // rows per pool slot (max_feats padded to 256)
 	int n_transient = 0, n_persist = 0;     // transient slots [0, n_transient) serve bt_knn_match_pairs; persistent ones follow
 	std::vector<int> slot_n;                // persistent slots: number of rows stored, -1 = empty
-	DevBuf pool_h, pool_f, norms, errn, slot_meta, sets, tables, pconst, G, cand, cand_cnt, qjob, fb_rows, fb_count, fb_part_d, fb_part_i, fb_tickets;
-	UploadBuf h_stage;                      // the set and work tables of a call
+	DevBuf pool_h, pool_f, norms, errn, slot_meta, pconst, G, cand, cand_cnt, qjob, fb_rows, fb_count, fb_part_d, fb_part_i, fb_tickets;
+	TableBlock<> tables;                    // the set and work tables of a call (KnnTables)
 	PFN_encodeTiled encode = nullptr;
 	CUtensorMap tmap_a, tmap_b;
 	size_t g_halves_cap = 0;
@@ -810,19 +810,28 @@ static PrepSet prep_set(const MatcherState* m, const bt_desc_view& v, int slot) 
 
 struct PoolSetRef { int slot; int n; };      // a descriptor set in the pool: rows [slot * slot_rows, +n)
 
-// uploads the set table from the staging block at hb and moves hb past it.  `sets` take consecutive slots (one call's transient slots 0, 1,
-// ..., or the one slot a store writes): one memset clears their counters.
-static int launch_prep(MatcherState* m, const std::vector<PrepSet>& sets, char*& hb, cudaStream_t stream) {
+// The tables of a call: the descriptor sets it converts, then the work plan (KnnPlan) on n_pairs pairs.  The sets go up first, in a copy
+// of their own, so that the conversion runs while the plan is made.
+struct KnnTables : TableLayout { Slice<PrepSet> sets; Slice<KnnPair> pairs; Slice<SelJob> jobs; Slice<int> blk_start, q_start; };
+static KnnTables knn_tables(size_t n_sets, size_t n_pairs) {
+	KnnTables t;
+	t.sets = t.add<PrepSet>(n_sets);
+	t.pairs = t.add<KnnPair>(n_pairs + 1);      // (the live pairs and the guard entry)
+	t.jobs = t.add<SelJob>(2 * n_pairs); t.blk_start = t.add<int>(2 * n_pairs); t.q_start = t.add<int>(2 * n_pairs);
+	return t;
+}
+
+// uploads the set table.  `sets` take consecutive slots (one call's transient slots 0, 1, ..., or the one slot a store writes): one memset
+// clears their counters.
+static int launch_prep(MatcherState* m, const KnnTables& t, const std::vector<PrepSet>& sets, cudaStream_t stream) {
 	if (sets.empty()) return BT_OK;
-	const size_t b_sets = sizeof(PrepSet) * sets.size();
-	memcpy(hb, sets.data(), b_sets);
-	BT_CUDA(cudaMemcpyAsync(m->sets.p, hb, b_sets, cudaMemcpyHostToDevice, stream));
-	hb += (b_sets + 255) & ~(size_t)255;
+	memcpy(m->tables.host(t.sets), sets.data(), sizeof(PrepSet) * sets.size());
+	BT_TRY(m->tables.send(t.sets.off, t.sets.end(), stream));
 	BT_CUDA(cudaMemsetAsync(m->slot_meta.as<int>() + 2 * sets[0].slot, 0, 2 * sizeof(int) * sets.size(), stream));
 	int max_padded = 0;
 	for (auto& s : sets) max_padded = std::max(max_padded, s.rows_padded);
 	k_desc_prep<<<dim3((unsigned)std::max(1, std::min((max_padded + 7) / 8, 64)), (unsigned)sets.size()), 256, 0, stream>>>(
-	    m->sets.as<PrepSet>(), m->pool_h.as<__half>(), m->pool_f.as<float>(), m->norms.as<float>(), m->errn.as<float>(), m->slot_meta.as<int>());
+	    m->tables.dev(t.sets), m->pool_h.as<__half>(), m->pool_f.as<float>(), m->norms.as<float>(), m->errn.as<float>(), m->slot_meta.as<int>());
 	return BT_OK;
 }
 
@@ -834,9 +843,6 @@ struct KnnPlan {
 	long long units = 0, g_off = 0;         // tensor-pass units; halves of G in use
 	int q_total = 0, blocks = 0;            // query rows; k_knn_select blocks
 };
-// the four tables lie back to back, in the pinned block and in MatcherState::tables alike
-static_assert(sizeof(KnnPair) % alignof(SelJob) == 0 && sizeof(SelJob) % alignof(int) == 0, "KnnPlan tables must stay aligned back to back");
-struct KnnTables { const KnnPair* pairs; const SelJob* jobs; const int* blk_start; const int* q_start; };
 
 static int plan_work(const MatcherState* m, const char* who, int n_pairs, const PoolSetRef* A, const PoolSetRef* B, KnnPlan& w) {
 	size_t off_dir[2] = { 0, 0 };
@@ -873,55 +879,54 @@ static int plan_work(const MatcherState* m, const char* who, int n_pairs, const 
 	return BT_OK;
 }
 
-// one copy of the plan's tables from the pinned block `hb` (the caller holds its event guard) to the device
-static int upload_plan(MatcherState* m, const KnnPlan& w, char* hb, cudaStream_t stream, KnnTables* dev) {
-	size_t off = 0;
-	auto put = [&](const auto& v) {      // appends table v; its place on the device
-		const size_t b = sizeof(v[0]) * v.size();
-		memcpy(hb + off, v.data(), b);
-		off += b;
-		return reinterpret_cast<decltype(v.data())>(m->tables.as<char>() + off - b);
-	};
-	*dev = KnnTables{ put(w.pairs), put(w.jobs), put(w.blk_start), put(w.q_start) };      // (a braced list is evaluated in order)
-	BT_CUDA(cudaMemcpyAsync(m->tables.p, hb, off, cudaMemcpyHostToDevice, stream));
-	return m->h_stage.in_flight(stream);
+// one copy of the plan's tables to the device
+static int upload_plan(MatcherState* m, const KnnTables& t, const KnnPlan& w, cudaStream_t stream) {
+	memcpy(m->tables.host(t.pairs), w.pairs.data(), sizeof(KnnPair) * w.pairs.size());
+	memcpy(m->tables.host(t.jobs), w.jobs.data(), sizeof(SelJob) * w.jobs.size());
+	memcpy(m->tables.host(t.blk_start), w.blk_start.data(), sizeof(int) * w.blk_start.size());
+	memcpy(m->tables.host(t.q_start), w.q_start.data(), sizeof(int) * w.q_start.size());
+	BT_TRY(m->tables.send(t.pairs.off, t.q_start.end(), stream));
+	return m->tables.in_flight(stream);
 }
 
-// The checks every matching entry point makes (A and B are its two input lists), then the device, the staging block and the first mark.
-static int begin_match(bt_ctx* ctx, const char* who, int n_pairs, const void* A, const void* B, int k, const KnnOut& out, cudaStream_t stream, char** hb) {
+// The checks every matching entry point makes (A and B are its two input lists), then the device and the first mark.
+static int begin_match(bt_ctx* ctx, const char* who, int n_pairs, const void* A, const void* B, int k, const KnnOut& out, cudaStream_t stream) {
 	MatcherState* m;
 	BT_TRY(state_of(ctx, &bt_ctx::matcher, who, "bt_matcher_reserve", &m));
 	BT_REQUIRE(A && B && out.idx[0] && out.dist[0] && out.idx[1] && out.dist[1], BT_ERR_INVALID_ARG, "%s: NULL argument", who);
 	BT_REQUIRE(k >= 1 && k <= 8, BT_ERR_UNSUPPORTED, "%s: k=%d outside [1,8]", who, k);
 	BT_REQUIRE(n_pairs > 0 && n_pairs <= m->max_pairs, BT_ERR_CAPACITY, "%s: %d pairs > reserved %d", who, n_pairs, m->max_pairs);
-	BT_TRY(m->h_stage.acquire(0, hb));
 	return mark(m, 0, stream);
 }
 
-// the matcher proper on descriptor sets that are already in the pool; hb: the free part of the staging block
-static int knn_run(bt_ctx* ctx, const char* who, int n_pairs, const PoolSetRef* A, const PoolSetRef* B, int k, const KnnOut& out, char* hb,
-                   cudaStream_t stream) {
+// the matcher proper, after the conversion of `sets` into the pool
+static int knn_run(bt_ctx* ctx, const char* who, int n_pairs, const std::vector<PrepSet>& sets, const PoolSetRef* A, const PoolSetRef* B, int k,
+                   const KnnOut& out, cudaStream_t stream) {
 	MatcherState* m = ctx->matcher.get();
+	const KnnTables t = knn_tables(sets.size(), n_pairs);
+	BT_TRY(m->tables.begin(who, t));
+	BT_TRY(launch_prep(m, t, sets, stream));
 	KnnPlan w;
 	BT_TRY(plan_work(m, who, n_pairs, A, B, w));
-	KnnTables t;
-	BT_TRY(upload_plan(m, w, hb, stream, &t));
+	BT_TRY(upload_plan(m, t, w, stream));
+	const KnnPair* d_pairs = m->tables.dev(t.pairs);
+	const SelJob* d_jobs = m->tables.dev(t.jobs);
 	const int n_live = (int)w.pairs.size() - 1, n_jobs = (int)w.jobs.size();
 	BT_CUDA(cudaMemsetAsync(m->fb_count.p, 0, 16, stream));
-	if (n_live > 0) k_knn_pairconst<<<(n_live + 127) / 128, 128, 0, stream>>>(t.pairs, n_live, m->slot_meta.as<int>(), m->pconst.as<PairConst>());
+	if (n_live > 0) k_knn_pairconst<<<(n_live + 127) / 128, 128, 0, stream>>>(d_pairs, n_live, m->slot_meta.as<int>(), m->pconst.as<PairConst>());
 	BT_TRY(mark(m, 1, stream));
 	if (n_live > 0) {
 		const int grid = (int)std::min<long long>(w.units, ctx->sm_count);
-		k_knn_tc<<<grid, KNN_THREADS, SMEM_TOTAL, stream>>>(m->tmap_a, m->tmap_b, t.pairs, n_live, (int)w.units, m->norms.as<float>(), m->pconst.as<PairConst>(), m->G.as<__half>());
+		k_knn_tc<<<grid, KNN_THREADS, SMEM_TOTAL, stream>>>(m->tmap_a, m->tmap_b, d_pairs, n_live, (int)w.units, m->norms.as<float>(), m->pconst.as<PairConst>(), m->G.as<__half>());
 	}
 	BT_TRY(mark(m, 2, stream));
 	if (w.q_total > 0) {
 		auto* sel = k <= 5 ? k_knn_select<5> : k_knn_select<8>;
-		sel<<<w.blocks, 256, 0, stream>>>(t.jobs, t.blk_start, n_jobs, m->G.as<__half>(), m->errn.as<float>(), m->pconst.as<PairConst>(), k, m->cand.as<int32_t>(), m->cand_cnt.as<int32_t>(), m->qjob.as<int>());
-		k_knn_rerank<<<(w.q_total + 7) / 8, 256, 0, stream>>>(t.jobs, m->qjob.as<int>(), w.q_total, m->cand.as<int32_t>(), m->cand_cnt.as<int32_t>(), m->pool_f.as<float>(),
+		sel<<<w.blocks, 256, 0, stream>>>(d_jobs, m->tables.dev(t.blk_start), n_jobs, m->G.as<__half>(), m->errn.as<float>(), m->pconst.as<PairConst>(), k, m->cand.as<int32_t>(), m->cand_cnt.as<int32_t>(), m->qjob.as<int>());
+		k_knn_rerank<<<(w.q_total + 7) / 8, 256, 0, stream>>>(d_jobs, m->qjob.as<int>(), w.q_total, m->cand.as<int32_t>(), m->cand_cnt.as<int32_t>(), m->pool_f.as<float>(),
 		                                                   k, out, m->fb_rows.as<int>(), m->fb_count.as<int>(), m->force_fallback);
 		BT_TRY(mark(m, 3, stream));
-		k_knn_exact<<<ctx->sm_count * 2, 256, 0, stream>>>(t.jobs, t.q_start, n_jobs, m->pool_f.as<float>(), m->fb_rows.as<int>(), m->fb_count.as<int>(), k, out,
+		k_knn_exact<<<ctx->sm_count * 2, 256, 0, stream>>>(d_jobs, m->tables.dev(t.q_start), n_jobs, m->pool_f.as<float>(), m->fb_rows.as<int>(), m->fb_count.as<int>(), k, out,
 		                                              m->fb_part_d.as<double>(), m->fb_part_i.as<int>(), m->fb_tickets.as<int>());
 	} else BT_TRY(mark(m, 3, stream));
 	BT_TRY(mark(m, 4, stream));
@@ -960,9 +965,7 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 	const int pad_a = (max_feats + BM - 1) / BM * BM;      // A sets are padded to whole 128-row tiles
 	const size_t g_halves_cap = (size_t)max_pairs * ((size_t)(slot_rows / GRP) * pad_a + (size_t)(pad_a / GRP) * slot_rows);
 	const int max_q_total = 2 * max_pairs * max_feats;
-	BT_TRY(m->sets.alloc(sizeof(PrepSet) * (size_t)std::max(m->n_transient, 1)));
-	const size_t b_tables = sizeof(KnnPair) * ((size_t)max_pairs + 1) + (sizeof(SelJob) + 2 * sizeof(int)) * 2 * max_pairs;     // a KnnPlan's
-	BT_TRY(m->tables.alloc(b_tables));
+	BT_TRY(m->tables.reserve(knn_tables(m->n_transient, max_pairs).total));
 	BT_TRY(m->pconst.alloc(sizeof(PairConst) * (size_t)max_pairs));
 	BT_TRY(m->G.alloc(g_halves_cap * 2 + 64));
 	BT_TRY(m->cand.alloc(sizeof(int32_t) * SEL_MAXC * (size_t)max_q_total));
@@ -973,7 +976,6 @@ extern "C" int bt_matcher_reserve(bt_ctx* ctx, int max_pairs, int max_feats, int
 	BT_TRY(m->fb_part_d.alloc(sizeof(double) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8)); BT_TRY(m->fb_part_i.alloc(sizeof(int) * (size_t)FB_SPLIT_ROWS * FB_SEG * 8));
 	BT_TRY(m->fb_tickets.alloc(sizeof(int) * (size_t)FB_SPLIT_ROWS));
 	BT_CUDA(cudaMemset(m->fb_tickets.p, 0, sizeof(int) * (size_t)FB_SPLIT_ROWS));
-	BT_TRY(m->h_stage.reserve(sizeof(PrepSet) * 2 * max_pairs + b_tables + 4096));
 	BT_CUDA(cudaFuncSetAttribute(k_knn_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_TOTAL));
 	m->max_pairs = max_pairs; m->max_feats = max_feats; m->dim = dim;
 	m->g_halves_cap = g_halves_cap; m->max_q_total = max_q_total;
@@ -1006,10 +1008,10 @@ extern "C" int bt_desc_pool_store(bt_ctx* ctx, int slot, const bt_desc_view* des
 	BT_REQUIRE(slot >= 0 && slot < m->n_persist, BT_ERR_INVALID_ARG, "bt_desc_pool_store: slot %d outside [0,%d)", slot, m->n_persist);
 	BT_TRY(check_desc(*desc, m, __func__, -1));
 	cudaStream_t stream = (cudaStream_t)stream_;
-	char* hb;
-	BT_TRY(m->h_stage.acquire(0, &hb));
-	BT_TRY(launch_prep(m, { prep_set(m, *desc, m->n_transient + slot) }, hb, stream));
-	BT_TRY(m->h_stage.in_flight(stream));
+	const KnnTables t = knn_tables(1, 0);
+	BT_TRY(m->tables.begin("bt_desc_pool_store", t));
+	BT_TRY(launch_prep(m, t, { prep_set(m, *desc, m->n_transient + slot) }, stream));
+	BT_TRY(m->tables.in_flight(stream));
 	BT_CUDA(cudaGetLastError());
 	m->slot_n[slot] = desc->n;
 	return BT_OK;
@@ -1019,8 +1021,7 @@ extern "C" int bt_knn_match_slots(bt_ctx* ctx, int n_pairs, const int32_t* slotA
                                   int32_t* idxAB, float* distAB, int32_t* idxBA, float* distBA, void* stream_) {
 	const KnnOut out{ { idxAB, idxBA }, { distAB, distBA } };
 	cudaStream_t stream = (cudaStream_t)stream_;
-	char* hb;
-	BT_TRY(begin_match(ctx, __func__, n_pairs, slotA, slotB, k, out, stream, &hb));
+	BT_TRY(begin_match(ctx, __func__, n_pairs, slotA, slotB, k, out, stream));
 	MatcherState* m = ctx->matcher.get();
 	std::vector<PoolSetRef> A(n_pairs), B(n_pairs);
 	for (int p = 0; p < n_pairs; p++) {
@@ -1030,7 +1031,7 @@ extern "C" int bt_knn_match_slots(bt_ctx* ctx, int n_pairs, const int32_t* slotA
 			(s2 == 0 ? A[p] : B[p]) = PoolSetRef{ m->n_transient + sl, m->slot_n[sl] };
 		}
 	}
-	return knn_run(ctx, __func__, n_pairs, A.data(), B.data(), k, out, hb, stream);
+	return knn_run(ctx, __func__, n_pairs, {}, A.data(), B.data(), k, out, stream);
 }
 
 extern "C" int bt_knn_debug_force_fallback(bt_ctx* ctx, int every_nth) {
@@ -1064,8 +1065,7 @@ extern "C" int bt_knn_match_pairs(bt_ctx* ctx, int n_pairs, const bt_desc_view* 
                                   int32_t* idxAB, float* distAB, int32_t* idxBA, float* distBA, void* stream_) {
 	const KnnOut out{ { idxAB, idxBA }, { distAB, distBA } };
 	cudaStream_t stream = (cudaStream_t)stream_;
-	char* hb;
-	BT_TRY(begin_match(ctx, __func__, n_pairs, A, B, k, out, stream, &hb));
+	BT_TRY(begin_match(ctx, __func__, n_pairs, A, B, k, out, stream));
 	MatcherState* m = ctx->matcher.get();
 	// ---- unique descriptor sets (a keyframe appears in many pairs) -> transient pool slots, converted once per call
 	std::map<std::pair<const float*, int>, int> slot_of;
@@ -1082,6 +1082,5 @@ extern "C" int bt_knn_match_pairs(bt_ctx* ctx, int n_pairs, const bt_desc_view* 
 		sa[p] = PoolSetRef{ slot(A[p]), A[p].n }; sb[p] = PoolSetRef{ slot(B[p]), B[p].n };
 	}
 	BT_REQUIRE((int)sets.size() <= m->n_transient, BT_ERR_CAPACITY, "bt_knn_match_pairs: %d distinct descriptor sets in one call > %d (store them with bt_desc_pool_store and use bt_knn_match_slots)", (int)sets.size(), m->n_transient);
-	BT_TRY(launch_prep(m, sets, hb, stream));
-	return knn_run(ctx, __func__, n_pairs, sa.data(), sb.data(), k, out, hb, stream);
+	return knn_run(ctx, __func__, n_pairs, sets, sa.data(), sb.data(), k, out, stream);
 }

@@ -564,13 +564,15 @@ struct LfnetState {
 	Layout L = {};
 	ScaleArgs sa = {};
 	size_t logit_stride = 0;
-	DevBuf w, tbl, grey, fa, fb, fc, logits, stats, Lm, Lmax, t1, t2, Es, heat, scl, nms, peak, kint, ori, patches, act, raw;
-	UploadBuf h_tbl;
+	DevBuf w, grey, fa, fb, fc, logits, stats, Lm, Lmax, t1, t2, Es, heat, scl, nms, peak, kint, ori, patches, act, raw;
+	TableBlock<> requests;          // the request pointers of a bt_lfnet_detect call
 	bool timing = false;
 	Event ev[N_STAGES + 1];
 	bool timed = false;
 };
 void StateDeleter::operator()(LfnetState* s) const { delete s; }
+struct RequestTable : TableLayout { Slice<const uint8_t*> req; };
+static RequestTable request_table(size_t n) { RequestTable t; t.req = t.add<const uint8_t*>(n); return t; }
 
 }  // namespace bt
 
@@ -702,8 +704,7 @@ extern "C" int bt_lfnet_reserve(bt_ctx* ctx, const bt_lfnet_params* p, int max_i
 	size_t act = 0;
 	for (int l = 0; l < p->desc_net_depth; l++) act = std::max(act, (size_t)L.dl[l].Hout * L.dl[l].Hout * L.dl[l].Cout);
 	BT_TRY(s->w.alloc(sizeof(float) * L.total));
-	BT_TRY(s->tbl.alloc(sizeof(void*) * n));
-	BT_TRY(s->h_tbl.reserve(sizeof(void*) * n));
+	BT_TRY(s->requests.reserve(request_table(n).total));
 	BT_TRY(s->grey.alloc(sizeof(float) * n * HW));
 	for (DevBuf* b : {&s->fa, &s->fb, &s->fc}) BT_TRY(b->alloc(sizeof(float) * n * TC * HW));
 	BT_TRY(s->logits.alloc(sizeof(float) * n * off));
@@ -754,13 +755,13 @@ extern "C" int bt_lfnet_detect(bt_ctx* ctx, int n, const uint8_t* const* request
 	auto mark = [&](int i) -> int { if (s->timing) BT_CUDA(cudaEventRecord(s->ev[i], st)); return BT_OK; };
 	BT_TRY(mark(0));
 	// request pointers
-	const uint8_t** h = nullptr;
-	BT_TRY(s->h_tbl.acquire(sizeof(void*) * N, &h));
-	for (int i = 0; i < n; i++) h[i] = request_dev[i];
-	BT_CUDA(cudaMemcpyAsync(s->tbl.p, h, sizeof(void*) * N, cudaMemcpyHostToDevice, st));
-	BT_TRY(s->h_tbl.in_flight(st));
+	const RequestTable rt = request_table(N);
+	BT_TRY(s->requests.begin("bt_lfnet_detect", rt));
+	memcpy(s->requests.host(rt.req), request_dev, sizeof(void*) * N);
+	BT_TRY(s->requests.send(0, rt.req.end(), st));
+	BT_TRY(s->requests.in_flight(st));
 	const dim3 gp((HW + 255) / 256, n);
-	k_grey<<<gp, 256, 0, st>>>(s->tbl.as<const uint8_t* const>(), s->grey.as<float>());
+	k_grey<<<gp, 256, 0, st>>>(s->requests.dev(rt.req), s->grey.as<float>());
 	// trunk: init conv, then per block x -> t = conv1(act(bn_pre x)) -> x' = conv2(act(bn_mid t)) + x, then act(bn_fin x)
 	const dim3 gc((SIDE + CT_W - 1) / CT_W, (SIDE + CT_H - 1) / CT_H, n);
 	float *x = s->fa.as<float>(), *t = s->fb.as<float>(), *y = s->fc.as<float>();

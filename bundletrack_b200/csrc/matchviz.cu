@@ -375,7 +375,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_mv_draw(const MvImage* __restri
 // cv::RNG::next
 inline uint64_t rng_next(uint64_t s) { return (uint64_t)(uint32_t)s * 4164903690ull + (s >> 32); }
 
-size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+struct VizTables : TableLayout { Slice<MvImage> images; Slice<uchar4> colours; };
+VizTables viz_tables(size_t n_images, size_t n_matches) {
+	VizTables t;
+	t.images = t.add<MvImage>(n_images); t.colours = t.add<uchar4>(n_matches);
+	return t;
+}
 
 bool roi_ok(const int32_t* r, int H, int W) { return r[0] >= 0 && r[0] < r[1] && r[1] <= W && r[2] >= 0 && r[2] < r[3] && r[3] <= H && r[3] - r[2] <= 900; }
 
@@ -384,8 +389,8 @@ bool roi_ok(const int32_t* r, int H, int W) { return r[0] >= 0 && r[0] < r[1] &&
 struct MatchVizState {
 	bool ready = false;
 	int max_images = 0, max_matches = 0;
-	DevBuf imgs, segs, boxes, colours;
-	UploadBuf h;                                   // the image table and the colours of one call
+	DevBuf segs, boxes;
+	TableBlock<> tables;                           // the image table and the colours of one call
 };
 void StateDeleter::operator()(MatchVizState* s) const { delete s; }
 
@@ -414,11 +419,9 @@ extern "C" int bt_match_viz_reserve(bt_ctx* ctx, int max_images, int max_matches
 	MatchVizState* s;
 	BT_TRY(take_state(ctx, &bt_ctx::matchviz, &s));
 	const size_t mm = (size_t)max(max_matches, 1);
-	BT_TRY(s->imgs.alloc(sizeof(MvImage) * (size_t)max_images));
 	BT_TRY(s->segs.alloc(sizeof(MvSeg) * kSegs * mm));
 	BT_TRY(s->boxes.alloc(sizeof(int4) * 3 * mm));
-	BT_TRY(s->colours.alloc(sizeof(uchar4) * mm));
-	BT_TRY(s->h.reserve(align16(sizeof(MvImage) * (size_t)max_images) + sizeof(uchar4) * mm));
+	BT_TRY(s->tables.reserve(viz_tables(max_images, mm).total));
 	s->max_images = max_images; s->max_matches = max_matches;
 	s->ready = true;
 	return BT_OK;
@@ -447,11 +450,10 @@ extern "C" int bt_match_viz(bt_ctx* ctx, int n_images, const bt_match_viz_desc* 
 	BT_REQUIRE(n_images <= s->max_images && total <= s->max_matches, BT_ERR_CAPACITY,
 	           "bt_match_viz: %d images / %lld matches exceed the reserved %d / %d", n_images, total, s->max_images, s->max_matches);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	char* h;
-	BT_TRY(s->h.acquire(0, &h));
-	const size_t ib = align16(sizeof(MvImage) * (size_t)n_images);
-	MvImage* im = reinterpret_cast<MvImage*>(h);
-	uchar4* col = reinterpret_cast<uchar4*>(h + ib);
+	const VizTables t = viz_tables(n_images, (size_t)total);
+	BT_TRY(s->tables.begin("bt_match_viz", t));
+	MvImage* im = s->tables.host(t.images);
+	uchar4* col = s->tables.host(t.colours);
 	int match_base = 0, tile_base = 0, max_n = 0;
 	for (int i = 0; i < n_images; i++) {
 		const bt_match_viz_desc& d = desc[i];
@@ -479,13 +481,12 @@ extern "C" int bt_match_viz(bt_ctx* ctx, int n_images, const bt_match_viz_desc* 
 		match_base += d.n;
 		max_n = max(max_n, d.n);
 	}
-	BT_CUDA(cudaMemcpyAsync(s->imgs.p, h, sizeof(MvImage) * (size_t)n_images, cudaMemcpyHostToDevice, stream));
-	if (total) BT_CUDA(cudaMemcpyAsync(s->colours.p, h + ib, sizeof(uchar4) * (size_t)total, cudaMemcpyHostToDevice, stream));
-	BT_TRY(s->h.in_flight(stream));
-	const MvImage* d_im = s->imgs.as<MvImage>();
+	BT_TRY(s->tables.send(0, t.colours.end(), stream));
+	BT_TRY(s->tables.in_flight(stream));
+	const MvImage* d_im = s->tables.dev(t.images);
 	if (total) k_mv_setup<<<dim3((3 * max_n + 127) / 128, n_images), 128, 0, stream>>>(d_im, s->segs.as<MvSeg>(), s->boxes.as<int4>());
 	k_mv_base<<<tile_base, kThreads, 0, stream>>>(d_im, n_images);
-	if (total) k_mv_draw<<<tile_base, kThreads, 0, stream>>>(d_im, n_images, s->segs.as<MvSeg>(), s->boxes.as<int4>(), s->colours.as<uchar4>());
+	if (total) k_mv_draw<<<tile_base, kThreads, 0, stream>>>(d_im, n_images, s->segs.as<MvSeg>(), s->boxes.as<int4>(), s->tables.dev(t.colours));
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;
 }

@@ -254,9 +254,11 @@ void frame_const(const double* pred, const double* gt, FrameConst& fc) {
 struct MetricsState {
 	bool ready = false;
 	int max_pts = 0, max_frames = 0;
-	DevBuf pts32, frames, part, pmax;
-	UploadBuf h_frames;
+	DevBuf pts32, part, pmax;
+	TableBlock<> frames;
 };
+struct FrameTable : TableLayout { Slice<FrameConst> frames; };
+static FrameTable frame_table(size_t n_frames) { FrameTable t; t.frames = t.add<FrameConst>(n_frames); return t; }
 void StateDeleter::operator()(MetricsState* s) const { delete s; }
 
 }  // namespace bt
@@ -271,10 +273,9 @@ extern "C" int bt_metrics_reserve(bt_ctx* ctx, int max_pts, int max_frames) {
 	BT_TRY(take_state(ctx, &bt_ctx::metrics, &s));
 	const size_t n_chunks = (size_t)(max_pts + kChunk - 1) / kChunk;
 	BT_TRY(s->pts32.alloc(sizeof(float4) * (size_t)max_pts));
-	BT_TRY(s->frames.alloc(sizeof(FrameConst) * (size_t)max_frames));
 	BT_TRY(s->part.alloc(2 * sizeof(double) * n_chunks * max_frames));
 	BT_TRY(s->pmax.alloc(sizeof(unsigned long long)));
-	BT_TRY(s->h_frames.reserve(sizeof(FrameConst) * (size_t)max_frames));
+	BT_TRY(s->frames.reserve(frame_table(max_frames).total));
 	s->max_pts = max_pts; s->max_frames = max_frames;
 	s->ready = true;
 	return BT_OK;
@@ -291,17 +292,18 @@ extern "C" int bt_pose_metrics(bt_ctx* ctx, const double* model_pts_dev, int n_p
 	BT_REQUIRE(n_pts <= s->max_pts && n_frames <= s->max_frames, BT_ERR_CAPACITY, "bt_pose_metrics: %d points / %d frames exceed the reserved %d / %d",
 	           n_pts, n_frames, s->max_pts, s->max_frames);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	FrameConst* hf;
-	BT_TRY(s->h_frames.acquire(0, &hf));
+	const FrameTable t = frame_table(n_frames);
+	BT_TRY(s->frames.begin("bt_pose_metrics", t));
+	FrameConst* hf = s->frames.host(t.frames);
 	for (int f = 0; f < n_frames; f++) frame_const(pred_ob_in_cam + 16 * (size_t)f, gt_ob_in_cam + 16 * (size_t)f, hf[f]);
-	BT_CUDA(cudaMemcpyAsync(s->frames.p, hf, sizeof(FrameConst) * (size_t)n_frames, cudaMemcpyHostToDevice, stream));
-	BT_TRY(s->h_frames.in_flight(stream));
+	BT_TRY(s->frames.send(0, t.frames.end(), stream));
+	BT_TRY(s->frames.in_flight(stream));
 	BT_CUDA(cudaMemsetAsync(s->pmax.p, 0, sizeof(unsigned long long), stream));
 	k_metrics_prep<<<(n_pts + kThreads - 1) / kThreads, kThreads, 0, stream>>>(model_pts_dev, n_pts, s->pts32.as<float4>(), s->pmax.as<unsigned long long>());
 	const int n_chunks = (n_pts + kChunk - 1) / kChunk;
 	double* part_add = s->part.as<double>();
 	double* part_adds = part_add + (size_t)n_chunks * n_frames;
-	k_pose_metrics<<<dim3(n_frames, n_chunks), kThreads, 0, stream>>>(model_pts_dev, s->pts32.as<float4>(), n_pts, s->frames.as<FrameConst>(),
+	k_pose_metrics<<<dim3(n_frames, n_chunks), kThreads, 0, stream>>>(model_pts_dev, s->pts32.as<float4>(), n_pts, s->frames.dev(t.frames),
 	                                                                  s->pmax.as<unsigned long long>(), part_add, part_adds);
 	k_metrics_final<<<(n_frames + 127) / 128, 128, 0, stream>>>(part_add, part_adds, n_chunks, n_pts, n_frames, add_out, adds_out);
 	BT_CUDA(cudaGetLastError());
@@ -486,9 +488,11 @@ __global__ void __launch_bounds__(32 * kNocsWarps) k_nocs_metrics(const NocsReco
 struct NocsState {
 	bool ready = false;
 	int max_records = 0;
-	DevBuf recs;
-	UploadBuf h_recs;
+	TableBlock<> recs;
 };
+// the rotation table (kNocsRot angles), then the records
+struct NocsTables : TableLayout { Slice<double2> rot; Slice<NocsRecord> recs; };
+static NocsTables nocs_tables(size_t n) { NocsTables t; t.rot = t.add<double2>(kNocsRot); t.recs = t.add<NocsRecord>(n); return t; }
 void StateDeleter::operator()(NocsState* s) const { delete s; }
 
 }  // namespace bt
@@ -498,9 +502,7 @@ extern "C" int bt_nocs_reserve(bt_ctx* ctx, int max_records) {
 	BT_REQUIRE(max_records >= 1, BT_ERR_INVALID_ARG, "bt_nocs_reserve: max_records %d must be >= 1", max_records);
 	NocsState* s;
 	BT_TRY(take_state(ctx, &bt_ctx::nocs, &s));
-	const size_t bytes = kNocsRot * sizeof(double2) + sizeof(NocsRecord) * (size_t)max_records;
-	BT_TRY(s->recs.alloc(bytes));
-	BT_TRY(s->h_recs.reserve(bytes));
+	BT_TRY(s->recs.reserve(nocs_tables(max_records).total));
 	s->max_records = max_records;
 	s->ready = true;
 	return BT_OK;
@@ -518,14 +520,14 @@ extern "C" int bt_nocs_metrics(bt_ctx* ctx, const double* pred, const double* gt
 	BT_TRY(state_of(ctx, &bt_ctx::nocs, "bt_nocs_metrics", "bt_nocs_reserve", &s));
 	BT_REQUIRE(n <= s->max_records, BT_ERR_CAPACITY, "bt_nocs_metrics: %d records exceed the reserved %d", n, s->max_records);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	char* h;
-	BT_TRY(s->h_recs.acquire(0, &h));
-	double2* hrot = reinterpret_cast<double2*>(h);
+	const NocsTables t = nocs_tables(n);
+	BT_TRY(s->recs.begin("bt_nocs_metrics", t));
+	double2* hrot = s->recs.host(t.rot);
 	for (int r = 0; r < kNocsRot; r++) {
 		const double t = ((2.0 * 3.141592653589793) * r) / 20.0;      // 2 * math.pi * i / float(n), Python's order
 		hrot[r] = make_double2(cos(t), sin(t));
 	}
-	NocsRecord* hr = reinterpret_cast<NocsRecord*>(h + kNocsRot * sizeof(double2));
+	NocsRecord* hr = s->recs.host(t.recs);
 	for (int i = 0; i < n; i++) {
 		memcpy(hr[i].pred, pred + 16 * (size_t)i, sizeof(hr[i].pred));
 		memcpy(hr[i].gt, gt + 16 * (size_t)i, sizeof(hr[i].gt));
@@ -533,11 +535,10 @@ extern "C" int bt_nocs_metrics(bt_ctx* ctx, const double* pred, const double* gt
 		hr[i].sym = symmetric[i] != 0;
 		hr[i].pad = 0;
 	}
-	const size_t bytes = kNocsRot * sizeof(double2) + sizeof(NocsRecord) * (size_t)n;
-	BT_CUDA(cudaMemcpyAsync(s->recs.p, h, bytes, cudaMemcpyHostToDevice, stream));
-	BT_TRY(s->h_recs.in_flight(stream));
-	const double2* d_rot = s->recs.as<double2>();
-	const NocsRecord* d_recs = reinterpret_cast<const NocsRecord*>(s->recs.as<char>() + kNocsRot * sizeof(double2));
+	BT_TRY(s->recs.send(0, t.recs.end(), stream));
+	BT_TRY(s->recs.in_flight(stream));
+	const double2* d_rot = s->recs.dev(t.rot);
+	const NocsRecord* d_recs = s->recs.dev(t.recs);
 	k_nocs_metrics<<<(n + kNocsWarps - 1) / kNocsWarps, 32 * kNocsWarps, 0, stream>>>(d_recs, d_rot, n, theta_deg_out, shift_out, iou_out);
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;

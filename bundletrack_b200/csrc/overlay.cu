@@ -336,15 +336,20 @@ __global__ void k_ovl_stamp(const float* __restrict__ cent, int stride, const in
 struct OverlayState {
 	bool ready = false;
 	int max_pts = 0, max_frames = 0, max_tiles = 0;
-	DevBuf a, b, cent, tiles, grid, hist, scan, cnt, tscan, tbl, nout;
-	UploadBuf h;                                   // tiles, pointer tables and poses of one call
+	DevBuf a, b, cent, grid, hist, scan, cnt, tscan, nout;
+	TableBlock<> tables;                           // tiles, pointer tables and poses of one call
 };
 void StateDeleter::operator()(OverlayState* s) const { delete s; }
 
 namespace {
 
-// the host part of a call: the tile table (and the tables after it) in the pinned block, uploaded behind one copy
-int plan_tiles(const int* n, int n_clouds, Tile* t, int* n_tiles) {
+// the tiles of clouds of n[0 .. n_clouds) points: how many, and the tile table
+int n_tiles_of(const int* n, int n_clouds) {
+	int k = 0;
+	for (int c = 0; c < n_clouds; c++) k += (n[c] + kTile - 1) / kTile;
+	return k;
+}
+void plan_tiles(const int* n, int n_clouds, Tile* t) {
 	int k = 0, start = 0;
 	for (int c = 0; c < n_clouds; c++) {
 		const int nt = (n[c] + kTile - 1) / kTile;
@@ -352,8 +357,21 @@ int plan_tiles(const int* n, int n_clouds, Tile* t, int* n_tiles) {
 		k += nt;
 		start += n[c];
 	}
-	*n_tiles = k;
-	return BT_OK;
+}
+
+// the tables of a bt_voxel_downsample call and of a bt_pose_overlay call
+struct DownsampleTables : TableLayout { Slice<Tile> tiles; Slice<const float*> src; Slice<float*> out; };
+DownsampleTables downsample_tables(size_t n_tiles, size_t n_clouds) {
+	DownsampleTables t;
+	t.tiles = t.add<Tile>(n_tiles); t.src = t.add<const float*>(n_clouds); t.out = t.add<float*>(n_clouds);
+	return t;
+}
+struct OverlayTables : TableLayout { Slice<Tile> tiles; Slice<OverlayFrame> frames; Slice<const uint8_t*> colour, fg; Slice<uint8_t*> viz, raw; };
+OverlayTables overlay_tables(size_t n_tiles, size_t n_frames) {
+	OverlayTables t;
+	t.tiles = t.add<Tile>(n_tiles); t.frames = t.add<OverlayFrame>(n_frames);
+	t.colour = t.add<const uint8_t*>(n_frames); t.fg = t.add<const uint8_t*>(n_frames); t.viz = t.add<uint8_t*>(n_frames); t.raw = t.add<uint8_t*>(n_frames);
+	return t;
 }
 
 // the grid of the clouds already in s->a (after the gather / transform and min / max): keys, sort, centroids
@@ -378,8 +396,6 @@ int grid_and_emit(OverlayState* s, const Tile* d_tiles, int n_tiles, int n_cloud
 	return BT_OK;
 }
 
-size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
-
 }  // namespace
 }  // namespace bt
 
@@ -396,16 +412,13 @@ extern "C" int bt_overlay_reserve(bt_ctx* ctx, int max_pts, int max_frames) {
 	BT_TRY(s->a.alloc(sizeof(float4) * (size_t)total));
 	BT_TRY(s->b.alloc(sizeof(float4) * (size_t)total));
 	BT_TRY(s->cent.alloc(3 * sizeof(float) * (size_t)total));
-	BT_TRY(s->tiles.alloc(sizeof(Tile) * (size_t)tiles));
 	BT_TRY(s->grid.alloc(sizeof(CloudGrid) * (size_t)max_frames));
 	BT_TRY(s->hist.alloc(sizeof(uint32_t) * 256 * (size_t)tiles));
 	BT_TRY(s->scan.alloc(sizeof(uint32_t) * (256 * (size_t)tiles + 1)));
 	BT_TRY(s->cnt.alloc(sizeof(uint32_t) * (size_t)tiles));
 	BT_TRY(s->tscan.alloc(sizeof(uint32_t) * ((size_t)tiles + 1)));
 	BT_TRY(s->nout.alloc(sizeof(int32_t) * (size_t)max_frames));
-	const size_t tbl = align16(sizeof(OverlayFrame) * (size_t)max_frames) + 5 * align16(sizeof(void*) * (size_t)max_frames);
-	BT_TRY(s->tbl.alloc(tbl));
-	BT_TRY(s->h.reserve(align16(sizeof(Tile) * (size_t)tiles) + tbl));
+	BT_TRY(s->tables.reserve(std::max(downsample_tables(tiles, max_frames).total, overlay_tables(tiles, max_frames).total)));
 	s->max_pts = max_pts; s->max_frames = max_frames; s->max_tiles = (int)tiles;
 	s->ready = true;
 	return BT_OK;
@@ -427,20 +440,17 @@ extern "C" int bt_voxel_downsample(bt_ctx* ctx, int n_clouds, const float* const
 	           "bt_voxel_downsample: %d clouds / %lld points exceed the reserved %d clouds / %lld points", n_clouds, total, s->max_frames,
 	           (long long)s->max_pts * s->max_frames);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	char* h;
-	BT_TRY(s->h.acquire(0, &h));
-	int n_tiles = 0;
-	plan_tiles(n_pts, n_clouds, reinterpret_cast<Tile*>(h), &n_tiles);
-	const size_t tb = align16(sizeof(Tile) * (size_t)n_tiles), pb = align16(sizeof(void*) * (size_t)n_clouds);
-	memcpy(h + tb, pts_dev, sizeof(void*) * n_clouds);
-	memcpy(h + tb + pb, out_dev, sizeof(void*) * n_clouds);
-	// tiles to s->tiles, the two pointer tables to s->tbl
-	BT_CUDA(cudaMemcpyAsync(s->tiles.p, h, sizeof(Tile) * (size_t)n_tiles, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaMemcpyAsync(s->tbl.p, h + tb, 2 * pb, cudaMemcpyHostToDevice, stream));
-	BT_TRY(s->h.in_flight(stream));
-	const Tile* d_tiles = s->tiles.as<Tile>();
-	const float* const* d_src = reinterpret_cast<const float* const*>(s->tbl.as<char>());
-	float* const* d_out = reinterpret_cast<float* const*>(s->tbl.as<char>() + pb);
+	const int n_tiles = n_tiles_of(n_pts, n_clouds);
+	const DownsampleTables t = downsample_tables(n_tiles, n_clouds);
+	BT_TRY(s->tables.begin("bt_voxel_downsample", t));
+	plan_tiles(n_pts, n_clouds, s->tables.host(t.tiles));
+	memcpy(s->tables.host(t.src), pts_dev, sizeof(void*) * n_clouds);
+	memcpy(s->tables.host(t.out), out_dev, sizeof(void*) * n_clouds);
+	BT_TRY(s->tables.send(0, t.out.end(), stream));
+	BT_TRY(s->tables.in_flight(stream));
+	const Tile* d_tiles = s->tables.dev(t.tiles);
+	const float* const* d_src = s->tables.dev(t.src);
+	float* const* d_out = s->tables.dev(t.out);
 	k_vox_init<<<(n_clouds + 127) / 128, 128, 0, stream>>>(s->grid.as<CloudGrid>(), n_clouds);
 	k_vox_gather<<<n_tiles, kThreads, 0, stream>>>(d_tiles, d_src, s->a.as<float4>(), s->grid.as<CloudGrid>());
 	return grid_and_emit(s, d_tiles, n_tiles, n_clouds, 1.0f / leaf, d_out, nullptr, n_out_dev, stream);
@@ -459,37 +469,33 @@ extern "C" int bt_pose_overlay(bt_ctx* ctx, int n_frames, const float* model_dev
 	BT_REQUIRE(n_frames <= s->max_frames && n_model <= s->max_pts, BT_ERR_CAPACITY, "bt_pose_overlay: %d frames / %d model points exceed the reserved %d / %d",
 	           n_frames, n_model, s->max_frames, s->max_pts);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	char* h;
-	BT_TRY(s->h.acquire(0, &h));
-	const size_t fb = align16(sizeof(OverlayFrame) * (size_t)n_frames), pb = align16(sizeof(void*) * (size_t)n_frames);
-	OverlayFrame* fr = reinterpret_cast<OverlayFrame*>(h);
+	std::vector<int> n(n_frames, n_model);
+	const OverlayTables t = overlay_tables(n_tiles_of(n.data(), n_frames), n_frames);
+	BT_TRY(s->tables.begin("bt_pose_overlay", t));
+	OverlayFrame* fr = s->tables.host(t.frames);
 	for (int f = 0; f < n_frames; f++) {
 		float ob[16];
 		BT_REQUIRE(inverse4(cur_in_model + 16 * (size_t)f, ob), BT_ERR_INVALID_ARG, "bt_pose_overlay: frame %d's pose is singular", f);
 		memcpy(fr[f].P, ob, sizeof fr[f].P);
 	}
-	const void* const* tabs[4] = { (const void* const*)colour_dev, (const void* const*)fg_dev, (const void* const*)viz_out_dev, (const void* const*)raw_out_dev };
-	for (int k = 0; k < 4; k++)
-		if (tabs[k]) memcpy(h + fb + k * pb, tabs[k], sizeof(void*) * n_frames);
-	const size_t tbl_bytes = fb + 4 * pb;
-	std::vector<int> n(n_frames, n_model);
-	int n_tiles = 0;
-	plan_tiles(n.data(), n_frames, reinterpret_cast<Tile*>(h + tbl_bytes), &n_tiles);
-	BT_CUDA(cudaMemcpyAsync(s->tbl.p, h, tbl_bytes, cudaMemcpyHostToDevice, stream));
-	BT_CUDA(cudaMemcpyAsync(s->tiles.p, h + tbl_bytes, sizeof(Tile) * (size_t)n_tiles, cudaMemcpyHostToDevice, stream));
-	BT_TRY(s->h.in_flight(stream));
-	char* d = s->tbl.as<char>();
-	const OverlayFrame* d_fr = reinterpret_cast<const OverlayFrame*>(d);
-	auto tab = [&](int k) { return reinterpret_cast<uint8_t* const*>(d + fb + k * pb); };
-	const Tile* d_tiles = s->tiles.as<Tile>();
+	memcpy(s->tables.host(t.colour), colour_dev, sizeof(void*) * n_frames);
+	memcpy(s->tables.host(t.fg), fg_dev, sizeof(void*) * n_frames);
+	memcpy(s->tables.host(t.viz), viz_out_dev, sizeof(void*) * n_frames);
+	if (raw_out_dev) memcpy(s->tables.host(t.raw), raw_out_dev, sizeof(void*) * n_frames);
+	plan_tiles(n.data(), n_frames, s->tables.host(t.tiles));
+	BT_TRY(s->tables.send(0, t.raw.end(), stream));
+	BT_TRY(s->tables.in_flight(stream));
+	const int n_tiles = (int)t.tiles.n;
+	const OverlayFrame* d_fr = s->tables.dev(t.frames);
+	const Tile* d_tiles = s->tables.dev(t.tiles);
 	k_vox_init<<<(n_frames + 127) / 128, 128, 0, stream>>>(s->grid.as<CloudGrid>(), n_frames);
 	k_ovl_transform<<<n_tiles, kThreads, 0, stream>>>(d_tiles, model_dev, d_fr, s->a.as<float4>(), s->grid.as<CloudGrid>());
 	int32_t* n_cent = s->nout.as<int32_t>();
 	BT_TRY(grid_and_emit(s, d_tiles, n_tiles, n_frames, 1.0f / 0.01f, nullptr, s->cent.as<float>(), n_cent, stream));
 	const int hw = H * W;
-	k_ovl_pixels<<<dim3((hw + 255) / 256, n_frames), 256, 0, stream>>>((const uint8_t* const*)tab(0), (const uint8_t* const*)tab(1), tab(2),
-	                                                                   raw_out_dev ? tab(3) : nullptr, hw);
-	k_ovl_stamp<<<dim3((n_model + 255) / 256, n_frames), 256, 0, stream>>>(s->cent.as<float>(), n_model, n_cent, tab(2), H, W, fx, fy, cx, cy);
+	k_ovl_pixels<<<dim3((hw + 255) / 256, n_frames), 256, 0, stream>>>(s->tables.dev(t.colour), s->tables.dev(t.fg), s->tables.dev(t.viz),
+	                                                                   raw_out_dev ? s->tables.dev(t.raw) : nullptr, hw);
+	k_ovl_stamp<<<dim3((n_model + 255) / 256, n_frames), 256, 0, stream>>>(s->cent.as<float>(), n_model, n_cent, s->tables.dev(t.viz), H, W, fx, fy, cx, cy);
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;
 }

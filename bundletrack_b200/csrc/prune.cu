@@ -238,11 +238,17 @@ __global__ void __launch_bounds__(256) k_emit_fill(const PrunePair* __restrict__
 struct PruneState {
 	bool ready = false;
 	int max_pairs = 0, max_feats = 0;
-	DevBuf pairs, corr, PA, PB, n_corr, n_nn, rpairs, inl, n_inl, idxAB, distAB, idxBA, distBA, entry_off, total, extra, n_prop;
-	UploadBuf h_pairs, h_extra;
+	DevBuf corr, PA, PB, n_corr, n_nn, rpairs, inl, n_inl, idxAB, distAB, idxBA, distBA, entry_off, total, extra, n_prop;
+	TableBlock<> pairs;                 // the pair table and the host extras of a call (`extra` holds the ones the device table writes)
 	size_t extra_cap = 0;               // propagated matches (float4 each) one call may carry
 };
 void StateDeleter::operator()(PruneState* s) const { delete s; }
+struct PairTables : TableLayout { Slice<PrunePair> pairs; Slice<float4> extra; };
+static PairTables pair_tables(size_t n_pairs, size_t n_extra) {
+	PairTables t;
+	t.pairs = t.add<PrunePair>(n_pairs); t.extra = t.add<float4>(n_extra);
+	return t;
+}
 
 }  // namespace bt
 
@@ -257,7 +263,6 @@ extern "C" int bt_pipeline_reserve(bt_ctx* ctx, int max_pairs, int max_feats, in
 	BT_TRY(bt_ransac_reserve(ctx, max_pairs, 3 * max_feats, max_trials));
 	const size_t cap = (size_t)3 * max_feats * max_pairs;      // nA + nB mutual candidates + up to max_feats propagated map-point matches per pair
 	const size_t extra_cap = (size_t)max_feats * max_pairs;
-	BT_TRY(s->pairs.alloc(sizeof(PrunePair) * max_pairs));
 	BT_TRY(s->corr.alloc(sizeof(bt_correspondence) * cap));
 	BT_TRY(s->PA.alloc(sizeof(float4) * cap)); BT_TRY(s->PB.alloc(sizeof(float4) * cap));
 	BT_TRY(s->n_corr.alloc(sizeof(int32_t) * max_pairs)); BT_TRY(s->n_nn.alloc(sizeof(int32_t) * max_pairs));
@@ -267,8 +272,7 @@ extern "C" int bt_pipeline_reserve(bt_ctx* ctx, int max_pairs, int max_feats, in
 	BT_TRY(s->idxAB.alloc(sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs)); BT_TRY(s->distAB.alloc(sizeof(float) * 8 * (size_t)max_feats * max_pairs));
 	BT_TRY(s->idxBA.alloc(sizeof(int32_t) * 8 * (size_t)max_feats * max_pairs)); BT_TRY(s->distBA.alloc(sizeof(float) * 8 * (size_t)max_feats * max_pairs));
 	BT_TRY(s->entry_off.alloc(sizeof(int32_t) * max_pairs)); BT_TRY(s->total.alloc(16)); BT_TRY(s->n_prop.alloc(sizeof(int32_t) * max_pairs));
-	BT_TRY(s->h_extra.reserve(sizeof(float4) * extra_cap));
-	BT_TRY(s->h_pairs.reserve(sizeof(PrunePair) * max_pairs));
+	BT_TRY(s->pairs.reserve(pair_tables(max_pairs, extra_cap).total));
 	s->max_pairs = max_pairs; s->max_feats = max_feats; s->extra_cap = extra_cap;
 	s->ready = true;
 	return BT_OK;
@@ -292,6 +296,8 @@ struct Chain {
 	int k = 0;
 	bt_correspondence* corr;
 	int32_t* n_corr;
+	const PrunePair *h_pairs = nullptr, *d_pairs = nullptr;    // the pair table on the host and on the device, once pairs() has uploaded it
+	const float4* d_extra = nullptr;                            // the propagated matches on the device
 	Chain(bt_ctx* ctx_, const char* who_, int n_pairs, const bt_match_frame* A_, const bt_match_frame* B_, int H, int W, float fx, float fy, float cx, float cy,
 	      const bt_prune_params* prm_, int trials_, float inlier_dist_, uint64_t seed_, void* stream_)
 	    : ctx(ctx_), s(ctx_->prune.get()), who(who_), n(n_pairs), trials(trials_), A(A_), B(B_), cam{ H, W, 1.0f / fx, 1.0f / fy, -cx / fx, -cy / fy },
@@ -307,10 +313,19 @@ struct Chain {
 	// the pair table, uploaded with the host extras.  prop_room > 0 (bt_find_corres_pairs): no host extras; pair p keeps room for prop_room
 	// propagated matches behind its mutual ones, and its candidates go to extra[p * prop_room, ...) when the device table writes them
 	int pairs(const bt_match_extra* extra, int prop_room) {
-		PrunePair* hp;
-		float4* hx;
-		BT_TRY(s->h_pairs.acquire(0, &hp));
-		BT_TRY(s->h_extra.acquire(0, &hx));
+		// the host extras pairs carry: counted and checked first, so that the table block can be laid out
+		auto n_extra = [&](int p) { return (extra && extra[p].n > 0 && abs(A[p].frame_id - B[p].frame_id) != 1) ? extra[p].n : 0; };
+		size_t n_x = 0;
+		for (int p = 0; p < n; p++) {
+			const int nx = n_extra(p);
+			BT_REQUIRE(nx == 0 || extra[p].uv, BT_ERR_INVALID_ARG, "pair %d: NULL propagated-match array", p);
+			BT_REQUIRE(nx <= s->max_feats && n_x + nx <= s->extra_cap, BT_ERR_CAPACITY, "pair %d: %d propagated matches exceed the reserved room", p, nx);
+			n_x += nx;
+		}
+		const PairTables t = pair_tables(n, n_x);
+		BT_TRY(s->pairs.begin(who, t));
+		PrunePair* hp = s->pairs.host(t.pairs);
+		float4* hx = s->pairs.host(t.extra);
 		int offA = 0, offB = 0, out = 0, xoff = 0;
 		for (int p = 0; p < n; p++) {
 			const bt_match_frame* fr[2] = { &A[p], &B[p] };
@@ -324,42 +339,38 @@ struct Chain {
 			}
 			hp[p].idx_off_A = offA; hp[p].idx_off_B = offB; hp[p].out_off = out;
 			hp[p].win_idx_A = A[p].window_index; hp[p].win_idx_B = B[p].window_index;
-			const int nx = (extra && extra[p].n > 0 && abs(A[p].frame_id - B[p].frame_id) != 1) ? extra[p].n : 0;
-			BT_REQUIRE(nx == 0 || extra[p].uv, BT_ERR_INVALID_ARG, "pair %d: NULL propagated-match array", p);
-			BT_REQUIRE(nx <= s->max_feats && (size_t)(xoff + nx) <= s->extra_cap, BT_ERR_CAPACITY, "pair %d: %d propagated matches exceed the reserved room", p, nx);
+			const int nx = n_extra(p);
 			hp[p].n_extra = nx; hp[p].extra_off = prop_room ? p * prop_room : xoff;
 			if (nx) memcpy(hx + xoff, extra[p].uv, sizeof(float4) * (size_t)nx);
 			xoff += nx;
 			offA += A[p].n; offB += B[p].n; out += A[p].n + B[p].n + nx + prop_room;
 		}
-		if (xoff) {
-			BT_CUDA(cudaMemcpyAsync(s->extra.p, hx, sizeof(float4) * (size_t)xoff, cudaMemcpyHostToDevice, stream));
-			BT_TRY(s->h_extra.in_flight(stream));
-		}
-		BT_CUDA(cudaMemcpyAsync(s->pairs.p, hp, sizeof(PrunePair) * n, cudaMemcpyHostToDevice, stream));
-		return s->h_pairs.in_flight(stream);
+		BT_TRY(s->pairs.send(0, xoff ? t.extra.end() : t.pairs.end(), stream));
+		h_pairs = hp; d_pairs = s->pairs.dev(t.pairs);
+		d_extra = prop_room ? s->extra.as<float4>() : s->pairs.dev(t.extra);
+		return s->pairs.in_flight(stream);
 	}
 	int prune() {
-		k_prune_mutual<<<n, 512, 0, stream>>>(s->pairs.as<PrunePair>(), cam, idxAB, idxBA, k, *prm, corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr);
+		k_prune_mutual<<<n, 512, 0, stream>>>(d_pairs, cam, idxAB, idxBA, k, *prm, corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr);
 		BT_CUDA(cudaGetLastError());
 		return BT_OK;
 	}
 	// findCorresByMapPoints for pairs [p0, p0 + np), with the pair table's counts or, given n_extra_dev, the ones the device table wrote
 	int append(int p0, int np, const int32_t* n_extra_dev) {
-		k_append_propagated<<<np, 256, 0, stream>>>(s->pairs.as<PrunePair>() + p0, cam, s->extra.as<float4>(), corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr + p0,
+		k_append_propagated<<<np, 256, 0, stream>>>(d_pairs + p0, cam, d_extra, corr, s->PA.as<float4>(), s->PB.as<float4>(), n_corr + p0,
 		                                            s->n_nn.as<int32_t>() + p0, n_extra_dev);
 		BT_CUDA(cudaGetLastError());
 		return BT_OK;
 	}
 	int ransac(int p0, int np) {
 		RansacPair* rp = s->rpairs.as<RansacPair>() + p0;
-		k_ransac_table_from_counts<<<(np + 127) / 128, 128, 0, stream>>>(s->pairs.as<PrunePair>() + p0, np, n_corr + p0, s->PA.as<float4>(), s->PB.as<float4>(), rp);
+		k_ransac_table_from_counts<<<(np + 127) / 128, 128, 0, stream>>>(d_pairs + p0, np, n_corr + p0, s->PA.as<float4>(), s->PB.as<float4>(), rp);
 		BT_CUDA(cudaGetLastError());
 		return ransac_run_device(ctx, rp, np, trials, inlier_dist, seed, s->inl.as<int32_t>(), s->n_inl.as<int32_t>() + p0, stream);
 	}
 	int emit(bt_entryj* entry_out, int capacity, int32_t* n_entry_out, int32_t* entry_off_out, int32_t* total_out, int32_t* status_out, float* uv_out) {
-		k_emit_entryj<<<1, 1024, 0, stream>>>(s->pairs.as<PrunePair>(), n, corr, s->inl.as<int32_t>(), s->n_inl.as<int32_t>(), entry_out, n_entry_out, entry_off_out, total_out, capacity, status_out);
-		k_emit_fill<<<n, 256, 0, stream>>>(s->pairs.as<PrunePair>(), corr, s->inl.as<int32_t>(), n_entry_out, entry_off_out, entry_out, capacity, reinterpret_cast<float4*>(uv_out));
+		k_emit_entryj<<<1, 1024, 0, stream>>>(d_pairs, n, corr, s->inl.as<int32_t>(), s->n_inl.as<int32_t>(), entry_out, n_entry_out, entry_off_out, total_out, capacity, status_out);
+		k_emit_fill<<<n, 256, 0, stream>>>(d_pairs, corr, s->inl.as<int32_t>(), n_entry_out, entry_off_out, entry_out, capacity, reinterpret_cast<float4*>(uv_out));
 		BT_CUDA(cudaGetLastError());
 		return BT_OK;
 	}
@@ -455,7 +466,7 @@ extern "C" int bt_find_corres_pairs(bt_ctx* ctx, int n_pairs, const bt_match_fra
 		// updateFramePairMapPoints on the entries the pair emits (none unless its status is OK)
 		BT_TRY(tracks_slot(ctx, A[p].frame_id, true, &sa));
 		BT_TRY(tracks_slot(ctx, B[p].frame_id, true, &sb));
-		const int off = s->h_pairs.buf.as<PrunePair>()[p].out_off;      // (the host copy of the pair table)
+		const int off = c.h_pairs[p].out_off;
 		BT_TRY(tracks_launch_update(ctx, sa, sb, TrkSrc{ reinterpret_cast<const float*>(c.corr + off), (int)(sizeof(bt_correspondence) / sizeof(float)),
 		                                                 s->inl.as<int32_t>() + off, nullptr, 0, s->n_inl.as<int32_t>(), p, entry_capacity }, c.stream));
 	}
@@ -506,29 +517,29 @@ struct MatchCache {
 	bool ready = false;
 	int max_pairs = 0, max_block = 0;  // pairs cached at once; entries per block (the arena size for bt_match_cache_reserve_entries)
 	long long cap = 0, top = 0, live = 0;   // arena entries: size, end of the last block placed, entries in live blocks
-	DevBuf arena, tab;
-	UploadBuf h_tab[2];                 // used in turn: a call waits only for the upload of the call before last
-	int flip = 0;
+	DevBuf arena;
+	TableBlock<2> moves;                // a call waits only for the upload of the call before last
 	struct Rec { long long off; int n, status; };
 	std::map<std::pair<int, int>, Rec> recs;
 };
 void StateDeleter::operator()(MatchCache* c) const { delete c; }
-static int cache_upload(MatchCache* c, const std::vector<CacheMove>& mv, cudaStream_t stream) {
-	UploadBuf& up = c->h_tab[c->flip];
-	c->flip ^= 1;
-	CacheMove* h;
-	BT_TRY(up.acquire(0, &h));
-	memcpy(h, mv.data(), sizeof(CacheMove) * mv.size());
-	BT_CUDA(cudaMemcpyAsync(c->tab.p, h, sizeof(CacheMove) * mv.size(), cudaMemcpyHostToDevice, stream));
-	return up.in_flight(stream);
+struct MoveTable : TableLayout { Slice<CacheMove> moves; };
+static MoveTable move_table(size_t n) { MoveTable t; t.moves = t.add<CacheMove>(n); return t; }
+// the moves of a call on the device
+static int cache_upload(MatchCache* c, const char* who, const std::vector<CacheMove>& mv, cudaStream_t stream, const CacheMove** dev) {
+	const MoveTable t = move_table(mv.size());
+	BT_TRY(c->moves.begin(who, t));
+	memcpy(c->moves.host(t.moves), mv.data(), sizeof(CacheMove) * mv.size());
+	BT_TRY(c->moves.send(0, t.moves.end(), stream));
+	*dev = c->moves.dev(t.moves);
+	return c->moves.in_flight(stream);
 }
 static int cache_reserve(bt_ctx* ctx, int max_pairs_cached, int max_block, long long total) {
 	MatchCache* c;
 	BT_TRY(take_state(ctx, &bt_ctx::mcache, &c));
 	BT_TRY(c->arena.alloc(sizeof(bt_entryj) * (size_t)total));
 	// a put uploads the compaction (every live block) and its own blocks in one table
-	BT_TRY(c->tab.alloc(sizeof(CacheMove) * 2 * (size_t)max_pairs_cached));
-	for (UploadBuf& h : c->h_tab) BT_TRY(h.reserve(sizeof(CacheMove) * 2 * (size_t)max_pairs_cached));
+	BT_TRY(c->moves.reserve(move_table(2 * (size_t)max_pairs_cached).total));
 	c->max_pairs = max_pairs_cached; c->max_block = max_block;
 	c->cap = total; c->top = 0; c->live = 0;
 	c->recs.clear();
@@ -603,10 +614,11 @@ extern "C" int bt_match_cache_put(bt_ctx* ctx, int n_pairs, const int32_t* idA, 
 	}
 	if (mv.empty()) return BT_OK;
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_TRY(cache_upload(c, mv, stream));
-	if (n_compact > 0) k_cache_compact<<<1, kCompactThreads, 0, stream>>>(c->tab.as<CacheMove>(), n_compact, c->arena.as<bt_entryj>());
+	const CacheMove* d_mv;
+	BT_TRY(cache_upload(c, "bt_match_cache_put", mv, stream, &d_mv));
+	if (n_compact > 0) k_cache_compact<<<1, kCompactThreads, 0, stream>>>(d_mv, n_compact, c->arena.as<bt_entryj>());
 	if ((int)mv.size() > n_compact)
-		k_cache_move<<<(unsigned)mv.size() - n_compact, 128, 0, stream>>>(c->tab.as<CacheMove>() + n_compact, entry_dev, c->arena.as<bt_entryj>(), 0);
+		k_cache_move<<<(unsigned)mv.size() - n_compact, 128, 0, stream>>>(d_mv + n_compact, entry_dev, c->arena.as<bt_entryj>(), 0);
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;
 }
@@ -657,8 +669,9 @@ extern "C" int bt_match_cache_gather(bt_ctx* ctx, int n_pairs, const int32_t* id
 	}
 	if (mv.empty()) return BT_OK;
 	cudaStream_t stream = (cudaStream_t)stream_;
-	BT_TRY(cache_upload(c, mv, stream));
-	k_cache_move<<<(unsigned)mv.size(), 128, 0, stream>>>(c->tab.as<CacheMove>(), c->arena.as<bt_entryj>(), dst_dev, 1);
+	const CacheMove* d_mv;
+	BT_TRY(cache_upload(c, "bt_match_cache_gather", mv, stream, &d_mv));
+	k_cache_move<<<(unsigned)mv.size(), 128, 0, stream>>>(d_mv, c->arena.as<bt_entryj>(), dst_dev, 1);
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;
 }

@@ -221,13 +221,15 @@ __global__ void __launch_bounds__(256) k_ransac_inliers(const RansacPair* __rest
 struct RansacState {
 	bool ready = false;
 	int max_pairs = 0, max_pts = 0, max_trials = 0;
-	DevBuf pairs, table, poses, good, best, best_trial;
-	UploadBuf h_pairs;
+	DevBuf table, poses, good, best, best_trial;
+	TableBlock<> pairs;                       // the pair table of a bt_ransac_pairs call
 	unsigned long long table_seed = ~0ull;
 	int table_trials = 0;
 	int last_pairs = 0, last_trials = 0;      // shape of the last run's per-trial poses, flags and keys (bt_ransac_debug_trials)
 };
 void StateDeleter::operator()(RansacState* r) const { delete r; }
+struct PairTable : TableLayout { Slice<RansacPair> pairs; };
+static PairTable pair_table(size_t n_pairs) { PairTable t; t.pairs = t.add<RansacPair>(n_pairs); return t; }
 
 // shared by the host-pointer API below and the fused matcher pipeline (pairs table already on the device)
 int ransac_run_device(bt_ctx* ctx, const RansacPair* d_pairs, int n_pairs, int n_trials, float dist_thresh, uint64_t seed,
@@ -258,13 +260,12 @@ extern "C" int bt_ransac_reserve(bt_ctx* ctx, int max_pairs, int max_pts, int ma
 	BT_REQUIRE(ctx && max_pairs > 0 && max_pts > 0 && max_trials > 0, BT_ERR_INVALID_ARG, "bt_ransac_reserve: bad arguments");
 	RansacState* r;
 	BT_TRY(take_state(ctx, &bt_ctx::ransac, &r));
-	BT_TRY(r->pairs.alloc(sizeof(RansacPair) * max_pairs));
 	BT_TRY(r->table.alloc(sizeof(float) * 3 * max_trials));
 	BT_TRY(r->poses.alloc(sizeof(float) * 12 * (size_t)max_pairs * max_trials));
 	BT_TRY(r->good.alloc(sizeof(int) * (size_t)max_pairs * max_trials));
 	BT_TRY(r->best.alloc(sizeof(unsigned long long) * max_pairs));
 	BT_TRY(r->best_trial.alloc(sizeof(int32_t) * max_pairs));
-	BT_TRY(r->h_pairs.reserve(sizeof(RansacPair) * max_pairs));
+	BT_TRY(r->pairs.reserve(pair_table(max_pairs).total));
 	r->table_seed = ~0ull; r->table_trials = 0; r->last_pairs = r->last_trials = 0;
 	r->max_pairs = max_pairs; r->max_pts = max_pts; r->max_trials = max_trials;
 	r->ready = true;
@@ -278,17 +279,18 @@ extern "C" int bt_ransac_pairs(bt_ctx* ctx, int n_pairs, const float* const* pts
 	BT_REQUIRE(ptsA && ptsB && n_pts && inlier_ids_out && n_inliers_out && n_pairs > 0, BT_ERR_INVALID_ARG, "bt_ransac_pairs: NULL argument");
 	cudaStream_t stream = (cudaStream_t)stream_;
 	BT_REQUIRE(n_pairs <= r->max_pairs, BT_ERR_CAPACITY, "bt_ransac_pairs: %d pairs > reserved %d", n_pairs, r->max_pairs);
-	RansacPair* hp;
-	BT_TRY(r->h_pairs.acquire(0, &hp));
+	const PairTable t = pair_table(n_pairs);
+	BT_TRY(r->pairs.begin("bt_ransac_pairs", t));
+	RansacPair* hp = r->pairs.host(t.pairs);
 	int off = 0;
 	for (int p = 0; p < n_pairs; p++) {
 		BT_REQUIRE(n_pts[p] >= 0 && n_pts[p] <= r->max_pts, BT_ERR_CAPACITY, "bt_ransac_pairs: pair %d has %d points > reserved %d", p, n_pts[p], r->max_pts);
 		hp[p].A = reinterpret_cast<const float4*>(ptsA[p]); hp[p].B = reinterpret_cast<const float4*>(ptsB[p]); hp[p].n = n_pts[p]; hp[p].out_off = off;
 		off += n_pts[p];
 	}
-	BT_CUDA(cudaMemcpyAsync(r->pairs.p, hp, sizeof(RansacPair) * n_pairs, cudaMemcpyHostToDevice, stream));
-	BT_TRY(r->h_pairs.in_flight(stream));
-	return ransac_run_device(ctx, r->pairs.as<RansacPair>(), n_pairs, n_trials, dist_thresh, seed, inlier_ids_out, n_inliers_out, stream);
+	BT_TRY(r->pairs.send(0, t.pairs.end(), stream));
+	BT_TRY(r->pairs.in_flight(stream));
+	return ransac_run_device(ctx, r->pairs.dev(t.pairs), n_pairs, n_trials, dist_thresh, seed, inlier_ids_out, n_inliers_out, stream);
 }
 
 // Debug/parity aid: the 3 uniforms per trial the sampler uses (seed as in bt_ransac_pairs), and the winning trial ids of the last call.

@@ -310,14 +310,19 @@ struct ReconState {
 	bool fused = false;                            // a grid is in sum / cnt
 	Grid grid{};
 	float bounds[6] = {};
-	DevBuf sum, cnt, mask, ntri, voff, foff, blk, tbl, bnd;
+	DevBuf sum, cnt, mask, ntri, voff, foff, blk, bnd;
 	PinnedBuf h_read;                              // the bounds, then the mesh's totals, read back
-	UploadBuf h;                                   // the poses and the depth pointer table of one call
+	TableBlock<> tables;                           // the poses and the depth pointer table of one call
 };
 void StateDeleter::operator()(ReconState* s) const { delete s; }
 
 namespace {
-size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+struct FuseTables : TableLayout { Slice<FramePose> poses; Slice<const float*> depth; };
+FuseTables fuse_tables(size_t n_frames) {
+	FuseTables t;
+	t.poses = t.add<FramePose>(n_frames); t.depth = t.add<const float*>(n_frames);
+	return t;
+}
 long long n_scan_blocks(long long nv) { return (nv + kScanBlock - 1) / kScanBlock; }
 }  // namespace
 
@@ -343,11 +348,9 @@ extern "C" int bt_recon_reserve(bt_ctx* ctx, int max_frames, int H, int W, long 
 	BT_TRY(s->voff.alloc(sizeof(int32_t) * nv));
 	BT_TRY(s->foff.alloc(sizeof(int32_t) * nv));
 	BT_TRY(s->blk.alloc(sizeof(int2) * ((size_t)n_scan_blocks(max_voxels) + 1)));
-	const size_t tbl = align16(sizeof(FramePose) * (size_t)max_frames) + align16(sizeof(void*) * (size_t)max_frames);
-	BT_TRY(s->tbl.alloc(tbl));
+	BT_TRY(s->tables.reserve(fuse_tables(max_frames).total));
 	BT_TRY(s->bnd.alloc(6 * sizeof(int)));
 	BT_TRY(s->h_read.alloc(6 * sizeof(int)));
-	BT_TRY(s->h.reserve(tbl));
 	s->max_frames = max_frames; s->H = H; s->W = W; s->max_voxels = max_voxels; s->max_vertices = max_vertices; s->max_faces = max_faces;
 	s->ready = true;
 	return BT_OK;
@@ -371,10 +374,9 @@ extern "C" int bt_tsdf_fuse(bt_ctx* ctx, int n_frames, const float* const* depth
 	BT_REQUIRE(n_frames <= s->max_frames && H <= s->H && W <= s->W, BT_ERR_CAPACITY, "bt_tsdf_fuse: %d frames of %d x %d exceed the reserved %d frames of %d x %d",
 	           n_frames, W, H, s->max_frames, s->W, s->H);
 	cudaStream_t stream = (cudaStream_t)stream_;
-	char* h;
-	BT_TRY(s->h.acquire(0, &h));
-	const size_t pb = align16(sizeof(FramePose) * (size_t)n_frames);
-	FramePose* fp = reinterpret_cast<FramePose*>(h);
+	const FuseTables t = fuse_tables(n_frames);
+	BT_TRY(s->tables.begin("bt_tsdf_fuse", t));
+	FramePose* fp = s->tables.host(t.poses);
 	for (int f = 0; f < n_frames; f++) {
 		const float* P = cam_in_model + 16 * (size_t)f;
 		for (int r = 0; r < 3; r++) {
@@ -382,11 +384,11 @@ extern "C" int bt_tsdf_fuse(bt_ctx* ctx, int n_frames, const float* const* depth
 			fp[f].t[r] = P[4 * r + 3];
 		}
 	}
-	memcpy(h + pb, depth_dev, sizeof(void*) * n_frames);
-	BT_CUDA(cudaMemcpyAsync(s->tbl.p, h, pb + sizeof(void*) * n_frames, cudaMemcpyHostToDevice, stream));
-	BT_TRY(s->h.in_flight(stream));
-	const FramePose* d_pose = s->tbl.as<FramePose>();
-	const float* const* d_depth = reinterpret_cast<const float* const*>(s->tbl.as<char>() + pb);
+	memcpy(s->tables.host(t.depth), depth_dev, sizeof(void*) * n_frames);
+	BT_TRY(s->tables.send(0, t.depth.end(), stream));
+	BT_TRY(s->tables.in_flight(stream));
+	const FramePose* d_pose = s->tables.dev(t.poses);
+	const float* const* d_depth = s->tables.dev(t.depth);
 	Grid g{};
 	g.voxel = p->voxel; g.trunc = p->trunc;
 	g.fx = fx; g.fy = fy; g.cx = cx; g.cy = cy; g.H = H; g.W = W;

@@ -1575,25 +1575,23 @@ template <int NT, int MINB> __global__ void __launch_bounds__(NT, MINB) k_solve(
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-// Everything bt_solve_stage uploads lives in ONE pinned block mirrored by ONE device block (same offsets), so staging is a
-// single H2D copy: the small tables first (carved for the worst case of this window count), the correspondences last so
-// that the copy length follows the actual number of entries.
-struct StageLayout {
-	size_t wins, dp, np, fw, texp, srcp, nsrcp, pose, pairs, pwin, psrc, late, wsp, gi, gj, gs, mem, corr, total;   // [0,late): needed by k_prep_frames
+// Everything bt_solve_stage uploads lives in ONE pinned block mirrored by the device staging blocks (same offsets): the small tables
+// first (sized for the worst case of this window count), the correspondences last so that the copy length follows the actual number of
+// entries.  [0, wsp.off) is what k_prep_frames needs.
+struct StageLayout : TableLayout {
+	Slice<WinDesc> wins; Slice<const float*> dp; Slice<const float4*> np; Slice<int> fw; Slice<const float4*> texp, srcp; Slice<const int*> nsrcp;
+	Slice<float> pose; Slice<uint2> pairs; Slice<int> pwin, psrc;
+	Slice<WinSparse> wsp; Slice<int> gi, gj, gs, mem; Slice<bt_entryj> corr;
 };
 static StageLayout stage_layout(int n_windows, size_t F, size_t C, int max_frames, size_t maxG, size_t maxP) {
 	StageLayout L;
-	size_t off = 0;
-	auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
 	const size_t nw = (size_t)n_windows;
-	L.wins = carve(sizeof(WinDesc) * nw); L.dp = carve(sizeof(void*) * F); L.np = carve(sizeof(void*) * F); L.fw = carve(sizeof(int) * F);
-	L.texp = carve(sizeof(void*) * F); L.srcp = carve(sizeof(void*) * F); L.nsrcp = carve(sizeof(void*) * F);
-	L.pose = carve(sizeof(float) * 16 * F); L.pairs = carve(sizeof(uint2) * maxP * nw); L.pwin = carve(sizeof(int) * maxP * nw); L.psrc = carve(sizeof(int) * maxP * nw);
-	L.late = off;
-	L.wsp = carve(sizeof(WinSparse) * nw); L.gi = carve(sizeof(int) * maxG * nw); L.gj = carve(sizeof(int) * maxG * nw); L.gs = carve(sizeof(int) * (maxG + 1) * nw);
-	L.mem = carve(sizeof(int) * (2 * ((size_t)max_frames + 1) + 2 * maxG + 2 * maxP) * nw);
-	L.corr = carve(sizeof(bt_entryj) * C + 32);
-	L.total = off;
+	L.wins = L.add<WinDesc>(nw); L.dp = L.add<const float*>(F); L.np = L.add<const float4*>(F); L.fw = L.add<int>(F);
+	L.texp = L.add<const float4*>(F); L.srcp = L.add<const float4*>(F); L.nsrcp = L.add<const int*>(F);
+	L.pose = L.add<float>(16 * F); L.pairs = L.add<uint2>(maxP * nw); L.pwin = L.add<int>(maxP * nw); L.psrc = L.add<int>(maxP * nw);
+	L.wsp = L.add<WinSparse>(nw); L.gi = L.add<int>(maxG * nw); L.gj = L.add<int>(maxG * nw); L.gs = L.add<int>((maxG + 1) * nw);
+	L.mem = L.add<int>((2 * ((size_t)max_frames + 1) + 2 * maxG + 2 * maxP) * nw);
+	L.corr = L.add<bt_entryj>(C + 1);      // (one entry of slack behind the last)
 	return L;
 }
 
@@ -1601,19 +1599,18 @@ struct SolverState {
 	bool ready = false;
 	bt_solver_limits lim{};
 	int npix_max = 0, max_pairs = 0, max_frames_total = 0, max_tiles = 0, max_groups = 0;
-	DevBuf blk_cnt, grp_sums, stage_buf[2], texel, src, nsrc, x, T, pose_out, tiles, scalars, partial, tiles_done, iter_done, pair_tile0, pair_ntile, dbgJ, dbgR, dbgC, dbgS, prof;
+	DevBuf blk_cnt, grp_sums, texel, src, nsrc, x, T, pose_out, tiles, scalars, partial, tiles_done, iter_done, pair_tile0, pair_ntile, dbgJ, dbgR, dbgC, dbgS, prof;
 	StageLayout layout{};
 	// frame cache (bt_frame_cache_*): quarter-res maps of keyframes, built once, referenced by bt_window::cache_slots
 	struct CacheMeta { bool valid = false; int H = 0, W = 0; float fx = 0, fy = 0, cx = 0, cy = 0, dmin = 0, dmax = 0; };
-	DevBuf c_texel, c_src, c_nsrc, c_tables, c_blk;
-	UploadBuf c_htables[2];              // two pinned table blocks, used alternately: a store only waits for the upload of the store before last,
+	DevBuf c_texel, c_src, c_nsrc, c_blk;
+	TableBlock<2> c_tables;              // two pinned table blocks, used alternately: a store only waits for the upload of the store before last,
 	                                     // so back-to-back stores (one new frame per window per step) never stall the host behind the GPU
-	int c_flip = 0;
 	int c_capacity = 0, c_npix = 0;      // (c_capacity 0 until bt_frame_cache_reserve completes)
 	float c_downscale = 0.f;
 	std::vector<CacheMeta> c_meta;
 	int prof_cap = 0;
-	UploadBuf h_stage;                   // read by the uploads on copy_stream
+	TableBlock<1, 2> stage;              // the staging block: read by the uploads on copy_stream into device block stage_cur
 	PinnedBuf h_poses;
 	// streaming form (bt_solve_windows_begin / _end): two batches may be in flight; each has its own pinned pose block and completion event
 	PinnedBuf h_pipe[2];
@@ -1666,7 +1663,7 @@ extern "C" int bt_solver_reserve(bt_ctx* ctx, const bt_solver_limits* lim) {
 	const int max_tiles = lim->max_windows * (lim->max_frames * (lim->max_frames - 1) / 2) * ((npix_max + min_chunk - 1) / min_chunk + 1) + kSparseTiles * lim->max_windows;
 	{   // worst case over every window count <= max_windows (the table offsets grow with the count, so the maximum is at max_windows)
 		const StageLayout L = stage_layout(lim->max_windows, (size_t)F, (size_t)lim->max_corr * lim->max_windows, lim->max_frames, (size_t)max_groups, (size_t)max_pairs);
-		BT_TRY(s->stage_buf[0].alloc(L.total)); BT_TRY(s->stage_buf[1].alloc(L.total));
+		BT_TRY(s->stage.reserve(L.total));
 	}
 	BT_TRY(s->texel.alloc(sizeof(float4) * (size_t)npix_max * F));
 	BT_TRY(s->src.alloc(sizeof(float4) * 2 * (size_t)npix_max * F));
@@ -1760,12 +1757,13 @@ static int validate_windows(const SolverState* s, int n_windows, const bt_window
 // What the frame preparation needs, with no look at the correspondences: window geometry, where each frame slot's maps live (a cache
 // slot or the call's own pointers), poses, the dense pair list with each pair's window and source slot.  *n_pairs = pairs of the batch.
 static int fill_frame_tables(SolverState* s, int n_windows, const bt_window* windows, const bt_solver_params* params, const float* poses_in,
-                             char* hb, const StageLayout& L, size_t* n_pairs) {
-	WinDesc* hw = (WinDesc*)(hb + L.wins);
-	const void** hdp = (const void**)(hb + L.dp); const void** hnp = (const void**)(hb + L.np);
-	const void** htex = (const void**)(hb + L.texp); const void** hsrc = (const void**)(hb + L.srcp); const void** hnsrc = (const void**)(hb + L.nsrcp);
-	int* hfw = (int*)(hb + L.fw); float* hpose = (float*)(hb + L.pose);
-	uint2* hpairs = (uint2*)(hb + L.pairs); int* hpwin = (int*)(hb + L.pwin); int* hpsrc = (int*)(hb + L.psrc);
+                             const StageLayout& L, size_t* n_pairs) {
+	const TableBlock<1, 2>& st = s->stage;
+	WinDesc* hw = st.host(L.wins);
+	const float** hdp = st.host(L.dp); const float4** hnp = st.host(L.np);
+	const float4** htex = st.host(L.texp); const float4** hsrc = st.host(L.srcp); const int** hnsrc = st.host(L.nsrcp);
+	int* hfw = st.host(L.fw); float* hpose = st.host(L.pose);
+	uint2* hpairs = st.host(L.pairs); int* hpwin = st.host(L.pwin); int* hpsrc = st.host(L.psrc);
 	const bool dense = params->w_dense > 0.f;
 	s->frame_off.assign(n_windows, 0); s->n_frames.assign(n_windows, 0);
 	s->any_uncached = false;
@@ -1795,7 +1793,7 @@ static int fill_frame_tables(SolverState* s, int n_windows, const bt_window* win
 				htex[fs] = s->c_texel.as<float4>() + (size_t)cs * s->c_npix; hsrc[fs] = s->c_src.as<float4>() + (size_t)cs * 2 * s->c_npix;
 				hnsrc[fs] = s->c_nsrc.as<int>() + cs;
 			} else {
-				hdp[fs] = dense ? bw.depth_dev[f] : nullptr; hnp[fs] = dense ? bw.normal_dev[f] : nullptr;
+				hdp[fs] = dense ? bw.depth_dev[f] : nullptr; hnp[fs] = dense ? (const float4*)bw.normal_dev[f] : nullptr;
 				htex[fs] = s->texel.as<float4>() + fs * (size_t)s->npix_max; hsrc[fs] = s->src.as<float4>() + fs * 2 * (size_t)s->npix_max;
 				hnsrc[fs] = nullptr;
 				if (dense) s->any_uncached = true;
@@ -1937,7 +1935,7 @@ static size_t window_membership(int N, int ng, int np, const int* gi, const int*
 // entries in page-locked caller memory are read in place, buffers that follow each other in memory as one transfer; blocks on the device are
 // copied device -> device.  The last two leave a hole in the pinned block, so whatever is staged below the hole is flushed first.
 struct CorrUpload {
-	char* dev; const bt_entryj* pinned; cudaStream_t stream;      // entry 0 of the device block and of the pinned block
+	bt_entryj* dev; const bt_entryj* pinned; cudaStream_t stream;      // entry 0 of the device block and of the pinned block
 	size_t sent = 0;                  // entries [0, sent) are uploaded or belong to the pending run
 	const bt_entryj* run_src = nullptr; size_t run_dst = 0, run_n = 0;      // pending in-place transfer
 	int staged(size_t upto) { return (upto - sent) * sizeof(bt_entryj) >= 256 * 1024 ? flush(upto) : BT_OK; }      // host entries now fill the pinned block up to `upto`
@@ -1949,17 +1947,17 @@ struct CorrUpload {
 	}
 	int from_device(const bt_entryj* src, size_t at, size_t n) {
 		BT_TRY(flush(at));
-		BT_CUDA(cudaMemcpyAsync(dev + at * sizeof(bt_entryj), src, n * sizeof(bt_entryj), cudaMemcpyDeviceToDevice, stream));
+		BT_CUDA(cudaMemcpyAsync(dev + at, src, n * sizeof(bt_entryj), cudaMemcpyDeviceToDevice, stream));
 		sent = at + n; return BT_OK;
 	}
 	int finish(size_t upto) { BT_TRY(flush(upto)); return send_run(); }
 private:
 	int flush(size_t upto) {
-		if (upto > sent) BT_CUDA(cudaMemcpyAsync(dev + sent * sizeof(bt_entryj), pinned + sent, (upto - sent) * sizeof(bt_entryj), cudaMemcpyHostToDevice, stream));
+		if (upto > sent) BT_CUDA(cudaMemcpyAsync(dev + sent, pinned + sent, (upto - sent) * sizeof(bt_entryj), cudaMemcpyHostToDevice, stream));
 		sent = upto; return BT_OK;
 	}
 	int send_run() {
-		if (run_n) BT_CUDA(cudaMemcpyAsync(dev + run_dst * sizeof(bt_entryj), run_src, run_n * sizeof(bt_entryj), cudaMemcpyHostToDevice, stream));
+		if (run_n) BT_CUDA(cudaMemcpyAsync(dev + run_dst, run_src, run_n * sizeof(bt_entryj), cudaMemcpyHostToDevice, stream));
 		run_n = 0; return BT_OK;
 	}
 };
@@ -1983,9 +1981,8 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 	BT_TRY(validate_windows(s, n_windows, windows, params, &F, &C));
 	// ---- lay out the pinned block (mirrored by one device block) and fill what the frame preparation needs
 	const StageLayout L = stage_layout(n_windows, F, C, s->lim.max_frames, (size_t)s->max_groups, (size_t)s->max_pairs);
-	BT_REQUIRE(L.total <= s->stage_buf[0].bytes, BT_ERR_CAPACITY, "bt_solve_stage: staging block %zu > reserved %zu bytes", L.total, s->stage_buf[0].bytes);
-	char* hb; BT_TRY(s->h_stage.acquire(L.total, &hb));
-	BT_TRY(fill_frame_tables(s, n_windows, windows, params, poses_in, hb, L, &n_pairs));
+	BT_TRY(s->stage.begin("bt_solve_stage", L));
+	BT_TRY(fill_frame_tables(s, n_windows, windows, params, poses_in, L, &n_pairs));
 	s->n_windows = n_windows; s->frames_total = (int)F; s->prm = *params; s->d2max = sqrt_le_max(params->dense_dist_thresh); s->layout = L;
 	{   // chunk: aim for >= 4 tiles per SM-resident CTA over the batch, between 256 and 2048 source pixels
 		const long long est_px = (long long)n_pairs * (s->npix_max / 8);   // ~12 % valid
@@ -1998,23 +1995,23 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 	BT_TRY(s->copy_stream.create());
 	if (s->run_pending) { BT_TRY(s->ev_stage_free[s->stage_cur].record(s->run_stream)); s->run_pending = false; }     // behind the runs of the block being left
 	s->stage_cur ^= 1;
-	DevBuf& stage_dev = s->stage_buf[s->stage_cur];
 	if (s->ev_stage_free[s->stage_cur]) BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_stage_free[s->stage_cur], 0));
 	// correspondence blocks produced on the device (bt_match_pairs on the caller's stream) are copied device -> device on the copy stream: order them
 	if (std::any_of(windows, windows + n_windows, [](const bt_window& bw) { return bw.corr_dev != nullptr; })) {
 		BT_TRY(s->ev_prev.record(stream)); BT_CUDA(cudaStreamWaitEvent(s->copy_stream, s->ev_prev, 0));
 	}
-	BT_CUDA(cudaMemcpyAsync(stage_dev.p, hb, L.late, cudaMemcpyHostToDevice, s->copy_stream));
+	BT_TRY(s->stage.send(0, L.wsp.off, s->copy_stream, s->stage_cur));
 	BT_TRY(s->ev_early.record(s->copy_stream));
 	BT_CUDA(cudaStreamWaitEvent(stream, s->ev_early, 0));      // the caller's stream (frame prep in the fused call) waits for the early tables only
 	s->host_us[0] = us_since(t_h0);
 	if (early_prep) BT_TRY(launch_prep(ctx, stream));
 	s->host_us[1] = us_since(t_h0) - s->host_us[0];
 	// ---- per window (the GPU is already busy in the fused call): group the correspondences, upload them, membership CSR
-	const WinDesc* hw = (const WinDesc*)(hb + L.wins); WinSparse* hws = (WinSparse*)(hb + L.wsp);
-	int* hgi = (int*)(hb + L.gi); int* hgj = (int*)(hb + L.gj); int* hgs = (int*)(hb + L.gs); int* hmem = (int*)(hb + L.mem);
-	const uint2* hpairs = (const uint2*)(hb + L.pairs); bt_entryj* hcorr = (bt_entryj*)(hb + L.corr);
-	CorrUpload up{stage_dev.as<char>() + L.corr, hcorr, s->copy_stream};
+	const TableBlock<1, 2>& st = s->stage;
+	const WinDesc* hw = st.host(L.wins); WinSparse* hws = st.host(L.wsp);
+	int* hgi = st.host(L.gi); int* hgj = st.host(L.gj); int* hgs = st.host(L.gs); int* hmem = st.host(L.mem);
+	const uint2* hpairs = st.host(L.pairs); bt_entryj* hcorr = st.host(L.corr);
+	CorrUpload up{st.dev(L.corr, s->stage_cur), hcorr, s->copy_stream};
 	size_t c_off = 0, g_off = 0, m_off = 0, p_off = 0, smem_need = 0, smem_lean = 0;
 	std::vector<int> bin; std::vector<char> seen;
 	for (int w = 0; w < n_windows; w++) {
@@ -2037,9 +2034,9 @@ static int stage_impl(bt_ctx* ctx, int n_windows, const bt_window* windows, cons
 	s->grp_in_smem = smem_need <= kTailSmemMax; if (!s->grp_in_smem) smem_need = smem_lean;
 	BT_REQUIRE(smem_need <= kTailSmemMax, BT_ERR_CAPACITY, "bt_solve_stage: window needs %zu bytes of shared memory (> %d KB)", smem_need, (int)(kTailSmemMax / 1024));
 	s->smem_bytes = (int)smem_need;
-	BT_CUDA(cudaMemcpyAsync(stage_dev.as<char>() + L.late, hb + L.late, L.corr - L.late, cudaMemcpyHostToDevice, s->copy_stream));      // ---- late upload: group tables, CSR, WinSparse
-	BT_TRY(s->h_stage.in_flight(s->copy_stream));
-	BT_CUDA(cudaStreamWaitEvent(stream, s->h_stage.ev, 0));     // everything later on the caller's stream sees the correspondences
+	BT_TRY(s->stage.send(L.wsp.off, L.corr.off, s->copy_stream, s->stage_cur));      // ---- late upload: group tables, CSR, WinSparse
+	BT_TRY(s->stage.in_flight(s->copy_stream));
+	BT_CUDA(cudaStreamWaitEvent(stream, s->stage.uploaded(), 0));     // everything later on the caller's stream sees the correspondences
 	if (s->debug) {
 		const int st = 6 * s->lim.max_frames, sp = 6 * (s->lim.max_frames - 1);
 		BT_TRY(s->dbgJ.alloc(sizeof(float) * (size_t)st * st * s->lim.max_windows));
@@ -2089,16 +2086,17 @@ static SolveArgs make_args(bt_ctx* ctx) {
 	SolverState* s = ctx->solver.get();
 	SolveArgs a;
 	memset(&a, 0, sizeof a);
-	char* sd = s->stage_buf[s->stage_cur].as<char>();
+	const TableBlock<1, 2>& sd = s->stage;
+	const int m = s->stage_cur;
 	const StageLayout& L = s->layout;
-	a.wins = (WinDesc*)(sd + L.wins); a.wsp = (const WinSparse*)(sd + L.wsp); a.n_windows = s->n_windows;
-	a.depth_ptr = (const float**)(sd + L.dp); a.normal_ptr = (const float4**)(sd + L.np); a.frame_win = (int*)(sd + L.fw);
+	a.wins = sd.dev(L.wins, m); a.wsp = sd.dev(L.wsp, m); a.n_windows = s->n_windows;
+	a.depth_ptr = sd.dev(L.dp, m); a.normal_ptr = sd.dev(L.np, m); a.frame_win = sd.dev(L.fw, m);
 	a.texel = s->texel.as<float4>(); a.src = s->src.as<float4>(); a.nsrc = s->nsrc.as<int>(); a.grp_sums = s->grp_sums.as<float>();
-	a.texel_tab = (const float4* const*)(sd + L.texp); a.src_tab = (const float4* const*)(sd + L.srcp); a.nsrc_cached = (const int* const*)(sd + L.nsrcp);
-	a.pose_in = (float*)(sd + L.pose); a.x = s->x.as<float>(); a.T = s->T.as<float>(); a.pose_out = s->pose_out.as<float>();
+	a.texel_tab = sd.dev(L.texp, m); a.src_tab = sd.dev(L.srcp, m); a.nsrc_cached = sd.dev(L.nsrcp, m);
+	a.pose_in = sd.dev(L.pose, m); a.x = s->x.as<float>(); a.T = s->T.as<float>(); a.pose_out = s->pose_out.as<float>();
 	a.npix_max = s->npix_max;
-	a.corr = (bt_entryj*)(sd + L.corr); a.grp_i = (int*)(sd + L.gi); a.grp_j = (int*)(sd + L.gj); a.grp_start = (int*)(sd + L.gs);
-	a.pairs = (uint2*)(sd + L.pairs); a.pair_win = (int*)(sd + L.pwin); a.pair_src_slot = (int*)(sd + L.psrc); a.mem = (int*)(sd + L.mem);
+	a.corr = sd.dev(L.corr, m); a.grp_i = sd.dev(L.gi, m); a.grp_j = sd.dev(L.gj, m); a.grp_start = sd.dev(L.gs, m);
+	a.pairs = sd.dev(L.pairs, m); a.pair_win = sd.dev(L.pwin, m); a.pair_src_slot = sd.dev(L.psrc, m); a.mem = sd.dev(L.mem, m);
 	a.tiles = s->tiles.as<Tile>(); a.max_tiles = s->max_tiles; a.partial = s->partial.as<float>();
 	a.pair_tile0 = s->pair_tile0.as<int>(); a.pair_ntile = s->pair_ntile.as<int>();
 	a.n_tiles_total = s->scalars.as<int>(); a.queue = s->scalars.as<int>() + 1; a.n_src_px = (long long*)(s->scalars.as<char>() + 16);
@@ -2261,18 +2259,17 @@ extern "C" int bt_frame_cache_store(bt_ctx* ctx, int n_frames, const int32_t* sl
 	if (n_frames <= kStoreInline) {
 		for (int f = 0; f < n_frames; f++) { c.depth_in[f] = depth_dev[f]; c.normal_in[f] = (const float4*)normal_dev[f]; c.slot_in[f] = slots[f]; }
 	} else {
-		const size_t b_ptr = sizeof(void*) * (size_t)n_frames, bytes = 2 * b_ptr + sizeof(int) * (size_t)n_frames;
-		BT_TRY(s->c_tables.alloc(bytes));
-		UploadBuf& up = s->c_htables[s->c_flip];
-		s->c_flip ^= 1;
-		char* hb;
-		BT_TRY(up.acquire(bytes, &hb));
-		const void** hd = (const void**)hb; const void** hn = (const void**)(hb + b_ptr); int* hs = (int*)(hb + 2 * b_ptr);
-		for (int f = 0; f < n_frames; f++) { hd[f] = depth_dev[f]; hn[f] = normal_dev[f]; hs[f] = slots[f]; }
-		BT_CUDA(cudaMemcpyAsync(s->c_tables.p, hb, bytes, cudaMemcpyHostToDevice, stream));
-		BT_TRY(up.in_flight(stream));
-		char* db = s->c_tables.as<char>();
-		c.depth = (const float* const*)db; c.normal = (const float4* const*)(db + b_ptr); c.slots = (const int*)(db + 2 * b_ptr);
+		TableLayout L;
+		const Slice<const float*> depth = L.add<const float*>(n_frames);
+		const Slice<const float4*> normal = L.add<const float4*>(n_frames);
+		const Slice<int> slot = L.add<int>(n_frames);
+		BT_TRY(s->c_tables.reserve(L.total));
+		BT_TRY(s->c_tables.begin("bt_frame_cache_store", L));
+		const float** hd = s->c_tables.host(depth); const float4** hn = s->c_tables.host(normal); int* hs = s->c_tables.host(slot);
+		for (int f = 0; f < n_frames; f++) { hd[f] = depth_dev[f]; hn[f] = (const float4*)normal_dev[f]; hs[f] = slots[f]; }
+		BT_TRY(s->c_tables.send(0, slot.end(), stream));
+		BT_TRY(s->c_tables.in_flight(stream));
+		c.depth = s->c_tables.dev(depth); c.normal = s->c_tables.dev(normal); c.slots = s->c_tables.dev(slot);
 	}
 	if (n_frames >= 2 * ctx->sm_count) {      // many frames: one CTA per frame fills the machine (faster than count + build there, DESIGN §9.6)
 		k_frame_cache_store<<<n_frames, 1024, 0, stream>>>(c);
