@@ -460,6 +460,11 @@ def write_png(path: str, img: np.ndarray) -> None:
                 + chunk(b"IDAT", zlib.compress(raw, 1)) + chunk(b"IEND", b""))
 
 
+def depth_mm(depth_m: np.ndarray) -> np.ndarray:
+    """Depth in metres as a 16-bit depth PNG holds it: millimetres rounded from the float64 product, clipped to [0, 65535]."""
+    return np.clip(np.round(np.asarray(depth_m, np.float64) * 1000), 0, 65535).astype(np.uint16)
+
+
 def write_ycbineoat_video(seq: Sequence, video_dir: str) -> None:
     """seq as a YCBInEOAT video directory (sequence.YcbineoatVideo reads it): rgb/, depth/ (16-bit millimetres), masks/, cam_K.txt and
     annotated_poses/ (ob_in_cam per frame), frames named %07d.png."""
@@ -467,6 +472,8 @@ def write_ycbineoat_video(seq: Sequence, video_dir: str) -> None:
     for sub in ("rgb", "depth", "masks", "annotated_poses"):
         os.makedirs(os.path.join(video_dir, sub), exist_ok=True)
     for k in range(seq.n_frames):
+        # millimetres from the float32 product, not depth_mm: the two round a few pixels of a sequence 1 mm apart, and the GPU tests'
+        # input videos are written this way
         for sub, img in (("rgb", seq.colour[k]), ("depth", np.round(seq.depth_raw[k] * 1000).astype(np.uint16)), ("masks", seq.mask[k])):
             write_png(os.path.join(video_dir, sub, f"{k:07d}.png"), img)
         G = np.linalg.inv(np.asarray(seq.poses_gt[k], np.float64))
@@ -475,6 +482,45 @@ def write_ycbineoat_video(seq: Sequence, video_dir: str) -> None:
     K = np.array([[seq.K[0], 0, seq.K[2]], [0, seq.K[1], seq.K[3]], [0, 0, 1]])
     with open(os.path.join(video_dir, "cam_K.txt"), "w") as f:
         f.write("".join(" ".join(f"{v:.9g}" for v in row) + "\n" for row in K))
+
+
+def write_nocs_scene(seq: Sequence, root: str, scene: int = 1, model: str = "camera_bench_norm", masks_dir: Optional[str] = None,
+                     obj_points: Optional[np.ndarray] = None) -> tuple:
+    """seq as NOCS-REAL275 scene `scene` of object `model` under root/nocs (sequence.NocsScene reads it): colour and depth PNGs (depth_mm),
+    the first frame's ob_in_cam as the ground truth 0000.txt, the class-3 data list, and with obj_points [n, 3] the object's OBJ model.  The
+    mask PNGs go to masks_dir (default root/masks).  Returns (nocs_dir, masks_dir)."""
+    import os
+    nocs, masks = os.path.join(root, "nocs"), masks_dir or os.path.join(root, "masks")
+    data = f"{nocs}/real_test/scene_{scene}"
+    gt = f"{nocs}/gts/real_test_text/scene_{scene}/model_{model}"
+    lst = f"{nocs}/NOCS-REAL275-additional/data_list/real_val/3/{model}"
+    for d in (data, masks, gt, lst):
+        os.makedirs(d)
+    for k in range(seq.n_frames):
+        write_png(f"{data}/{k:04d}_color.png", seq.colour[k])
+        write_png(f"{data}/{k:04d}_depth.png", depth_mm(seq.depth_raw[k]))
+        write_png(f"{masks}/{k:04d}.png", seq.mask[k])
+    np.savetxt(f"{gt}/0000.txt", np.linalg.inv(seq.poses_gt[0]))
+    with open(f"{lst}/list.txt", "w") as f:
+        f.write("".join(f"real_val/scene_{scene}/{k:04d}\n" for k in range(seq.n_frames)))
+    if obj_points is not None:
+        os.makedirs(f"{nocs}/obj_models/real_test")
+        with open(f"{nocs}/obj_models/real_test/{model}.obj", "w") as f:
+            f.write("".join(f"v {x:.9g} {y:.9g} {z:.9g}\n" for x, y, z in np.asarray(obj_points, np.float64)))
+    return nocs, masks
+
+
+def recorded_features(seq: Sequence):
+    """run_sequence's feature callable that replays seq: frame id_str's keypoints and descriptors, sequence.DetectionFailed for a frame
+    without features."""
+    from .sequence import DetectionFailed
+
+    def features(id_str, request, roi):
+        f = seq.feats[int(id_str)]
+        if f is None:
+            raise DetectionFailed(id_str)
+        return f["kpts"], f["desc"]
+    return features
 
 
 def make_ellipsoid_model(seed: int, n: int, radii=(0.05, 0.04, 0.03)) -> np.ndarray:

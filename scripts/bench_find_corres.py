@@ -13,27 +13,18 @@ import ctypes
 import json
 import os
 import statistics
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from bundletrack_b200 import _lib, synth  # noqa: E402
-from bundletrack_b200.matcher import MatchPipeline, DeviceTracks  # noqa: E402
-from bundletrack_b200.policy import Tracks  # noqa: E402
+import benchkit
+from bundletrack_b200 import _lib, synth
+from bundletrack_b200.matcher import MatchPipeline, DeviceTracks
+from bundletrack_b200.policy import Tracks
 
 NF = 2000
 YML = {"feature_corres": {"max_dist_no_neighbor": 0.02, "max_normal_no_neighbor": 45, "max_dist_neighbor": 10000, "max_normal_neighbor": 180},
        "ransac": {"max_iter": 2000, "inlier_dist": 0.01}}
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
 
 
 class Setup:
@@ -152,7 +143,7 @@ def main():
     import torch
     assert torch.cuda.is_available(), "bench_find_corres needs a GPU"
     dev = torch.device("cuda:0")
-    out = {"card": card(), "rows": [run(w, a.reps, a.warmup, dev) for w in a.windows]}
+    out = {"card": benchkit.card(), "rows": [run(w, a.reps, a.warmup, dev) for w in a.windows]}
     txt = json.dumps(out, indent=1)
     print(txt)
     if a.out:

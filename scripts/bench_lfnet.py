@@ -9,22 +9,13 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
-import sys
 import tempfile
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import benchkit
 
 STAGES = ("trunk", "score_maps", "detection", "keypoints_patches", "descriptor")
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
 
 
 def requests(dev, n):
@@ -48,18 +39,8 @@ def requests(dev, n):
 
 
 def time_detect(net, reqs, iters):
-    import torch
     from bundletrack_b200 import _lib
-    for _ in range(3):
-        net.detect(reqs)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(torch.cuda.current_stream())
-    for _ in range(iters):
-        net.detect(reqs)
-    e1.record(torch.cuda.current_stream())
-    torch.cuda.synchronize()
-    total = e0.elapsed_time(e1) / iters
+    total = benchkit.window_ms(lambda: net.detect(reqs), iters, 3, net.stream)
     _lib.check(net.lib.bt_lfnet_enable_timing(net.ctx, 1))
     ms = (ctypes.c_float * 5)()
     acc = np.zeros(5)
@@ -79,17 +60,7 @@ def sequence_runs(net, dev, n_frames):
     seq = synth.make_sequence(9, n_frames, H=H, W=W)
     tmp = tempfile.mkdtemp()
     video = os.path.join(tmp, "synthvideo")
-    for k in range(n_frames):
-        for sub, img in (("rgb", seq.colour[k]), ("depth", np.round(seq.depth_raw[k] * 1000).astype(np.uint16)), ("masks", seq.mask[k])):
-            os.makedirs(os.path.join(video, sub), exist_ok=True)
-            synth.write_png(os.path.join(video, sub, f"{k:07d}.png"), img)
-    K = np.array([[seq.K[0], 0, seq.K[2]], [0, seq.K[1], seq.K[3]], [0, 0, 1]])
-    with open(os.path.join(video, "cam_K.txt"), "w") as f:
-        f.write("".join(" ".join(f"{v:.9g}" for v in row) + "\n" for row in K))
-    os.makedirs(os.path.join(video, "annotated_poses"))
-    for k in range(n_frames):
-        with open(os.path.join(video, "annotated_poses", f"{k:07d}.txt"), "w") as f:
-            f.write("".join(" ".join(f"{v:.9g}" for v in row) + "\n" for row in np.linalg.inv(seq.poses_gt[k])))
+    synth.write_ycbineoat_video(seq, video)
     loader = sequence.YcbineoatVideo(video)
 
     def host(id_str, request, roi):
@@ -120,7 +91,7 @@ def main():
     hp = dict(lfnet.DEFAULTS)
     net = lfnet.LfnetDevice(lo.random_weights(lfnet.weight_shapes(hp), 11), hp, max_images=8)
     reqs = requests(dev, 8)
-    res = {"card": card(), "torch": torch.__version__,
+    res = {"card": benchkit.card(), "torch": torch.__version__,
            "detect_1": time_detect(net, reqs[:1], a.iters), "detect_8": time_detect(net, reqs, a.iters),
            "run_sequence": sequence_runs(net, dev, a.frames), "tf1_server_on_h100": "not measured"}
     net.close()

@@ -9,16 +9,13 @@ import argparse
 import json
 import os
 import shutil
-import sys
 import tempfile
 import threading
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
+import benchkit
 
 
 def stats(lat_s, wall_s, n):
@@ -101,7 +98,7 @@ def main():
     a = ap.parse_args()
     import torch
     import zmq
-    from bench_lfnet import card, requests
+    from bench_lfnet import requests
     from bundletrack_b200 import lfnet
     from bundletrack_b200.lfnet_server import LfnetServer
     from oracle import lfnet_oracle as lo
@@ -109,7 +106,7 @@ def main():
     hp = dict(lfnet.DEFAULTS)
     w = lo.random_weights(lfnet.weight_shapes(hp), 11)
     images = [r.cpu().numpy() for r in requests(dev, 8)]
-    res = {"card": card(), "torch": torch.__version__}
+    res = {"card": benchkit.card(), "torch": torch.__version__}
     net = lfnet.LfnetDevice(w, hp, max_images=8)
     res["direct_1"] = direct(net, images, a.requests * 2)
     res["direct_batch_8"] = direct_batch(net, images, a.requests)

@@ -19,16 +19,12 @@ import ctypes
 import itertools
 import json
 import os
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-
-from bench_tracker import gpu_info, stats_ms, upload  # noqa: E402
+import benchkit
+from bench_tracker import stats_ms, upload
 
 
 def feed(trk, frames, seq, lo, hi, tb=None, te=None):
@@ -118,7 +114,7 @@ def main():
     H, W = 480, 640
     mode = _lib.BT_MASK_LARGEST_HULL
     y = load_yml(None)
-    res = {"gpu": gpu_info(), "H": H, "W": W, "feats": a.feats, "frames": a.frames, "max_frames_alive": a.alive, "max_keyframes": a.keyframes}
+    res = {"gpu": benchkit.card(), "H": H, "W": W, "feats": a.feats, "frames": a.frames, "max_frames_alive": a.alive, "max_keyframes": a.keyframes}
     t0 = time.perf_counter()
     seq = synth.make_sequence(11, a.frames, H=H, W=W, n_feats=a.feats)
     res["generate_s"] = round(time.perf_counter() - t0, 1)

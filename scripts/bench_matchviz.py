@@ -10,15 +10,11 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import benchkit
 
 
 def main():
@@ -48,20 +44,8 @@ def main():
         jobs.append((colour, ra, colour, rb, torch.from_numpy(uv.astype(np.float32)).to(dev), mv.RNG_DEFAULT))
     outs = [torch.empty((*match_image_shape(j[1], j[3]), 3), dtype=torch.uint8, device=dev) for j in jobs]
     mz = MatchViz(max_images=len(jobs), max_matches=a.matches * len(jobs), stream=torch.cuda.current_stream(dev).cuda_stream)
-    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-
-    def timed(fn):
-        fn()
-        torch.cuda.synchronize()
-        ev0.record()
-        for _ in range(a.reps):
-            fn()
-        ev1.record()
-        torch.cuda.synchronize()
-        return ev0.elapsed_time(ev1) / a.reps
-
-    single = timed(lambda: mz.draw(jobs[:1], outs[:1]))
-    batch = timed(lambda: mz.draw(jobs, outs))
+    single = benchkit.window_ms(lambda: mz.draw(jobs[:1], outs[:1]), a.reps, 1, mz.stream)
+    batch = benchkit.window_ms(lambda: mz.draw(jobs, outs), a.reps, 1, mz.stream)
     import cv2
     host_col = colour.cpu().numpy()
     t0 = time.perf_counter()
@@ -75,11 +59,7 @@ def main():
         cv2.drawMatches(A, ka, B, kb, [cv2.DMatch(i, i, 0) for i in range(len(kp))], None, flags=cv2.DrawMatchesFlags_NOT_DRAW_SINGLE_POINTS)
     host = (time.perf_counter() - t0) * 1e3 / 20
     px = sum(o.numel() // 3 for o in outs) / len(outs)
-    try:
-        card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    except OSError:
-        card = torch.cuda.get_device_name(0)
-    print(json.dumps({"card": card, "matches_per_image": a.matches, "images_per_batch": len(jobs), "mean_pixels_per_image": round(px),
+    print(json.dumps({"card": benchkit.card(), "matches_per_image": a.matches, "images_per_batch": len(jobs), "mean_pixels_per_image": round(px),
                       "device_ms_one_image": round(single, 4), "device_ms_batch": round(batch, 4),
                       "device_ms_per_image_in_batch": round(batch / len(jobs), 4), "host_cv2_ms_per_image": round(host, 3)}))
     mz.close()

@@ -9,21 +9,11 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        return q.stdout.strip().splitlines()[0]
-    except Exception as e:          # the numbers still print; the card is then named by torch alone
-        return f"unknown ({e})"
+import benchkit
 
 
 def main():
@@ -48,7 +38,7 @@ def main():
         gt[f] = synth.se3(Q * np.sign(np.linalg.det(Q)), np.array([0, 0, 0.7]) + rng.normal(0, 0.05, 3))
         pred[f] = synth.se3(synth.so3_exp(rng.normal(size=3) * np.deg2rad(3.0)), rng.normal(0, 0.01, 3)) @ gt[f]
     pm = PoseMetrics(max(sizes), F)
-    res = {"gpu": torch.cuda.get_device_name(0), "nvidia_smi": gpu_info(), "frames": F, "sizes": {}}
+    res = {"gpu": torch.cuda.get_device_name(0), "nvidia_smi": benchkit.card(), "frames": F, "sizes": {}}
     for n in sizes:
         d = rng.normal(size=(n, 3))
         P = d / np.linalg.norm(d, axis=1, keepdims=True) * np.array([0.05, 0.08, 0.03])

@@ -8,14 +8,11 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import benchkit
 
 
 def _records(n: int, seed: int = 0):
@@ -44,11 +41,7 @@ def main():
     import torch
     from bundletrack_b200 import _lib, metrics
     from oracle import nocs_oracle
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        card = q.stdout.strip().splitlines()[0]
-    except Exception:
-        card = torch.cuda.get_device_name(0)
+    card = benchkit.card()
     m = metrics.NocsMetrics(max(a.sizes))
     lib = _lib.load()
     for n in a.sizes:
@@ -59,26 +52,22 @@ def main():
 
         def call():
             _lib.check(lib.bt_nocs_metrics(m.ctx, p(P), p(G), p(Cf), p(S), ctypes.c_int(n), ctypes.c_void_p(out[0].data_ptr()),
-                                           ctypes.c_void_p(out[1].data_ptr()), ctypes.c_void_p(out[2].data_ptr()), None), "bt_nocs_metrics")
-        call()
-        torch.cuda.synchronize()
-        dev_ms = []
+                                           ctypes.c_void_p(out[1].data_ptr()), ctypes.c_void_p(out[2].data_ptr()), m.stream), "bt_nocs_metrics")
+        dev_ms = benchkit.calls_ms(call, 3, 1, m.stream)
+        wall_ms = []
         for _ in range(3):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             h0 = time.perf_counter()
-            e0.record()
             call()
-            e1.record()
             torch.cuda.synchronize()
-            dev_ms.append((e0.elapsed_time(e1), (time.perf_counter() - h0) * 1e3))
+            wall_ms.append((time.perf_counter() - h0) * 1e3)
         nocs_oracle.record_metrics(P[:100], G[:100], C[:100], S[:100])
         host_ms = []
         for _ in range(3):
             h0 = time.perf_counter()
             nocs_oracle.record_metrics(P, G, C, S)
             host_ms.append((time.perf_counter() - h0) * 1e3)
-        print(json.dumps({"records": n, "card": card, "device_call_ms_median": float(np.median([d[0] for d in dev_ms])),
-                          "host_wall_ms_median": float(np.median([d[1] for d in dev_ms])), "oracle_numpy_ms_median": float(np.median(host_ms))}))
+        print(json.dumps({"records": n, "card": card, "device_call_ms_median": float(np.median(dev_ms)),
+                          "host_wall_ms_median": float(np.median(wall_ms)), "oracle_numpy_ms_median": float(np.median(host_ms))}))
     m.close()
 
 

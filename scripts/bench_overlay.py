@@ -18,15 +18,12 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import sys
 import tempfile
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
+import benchkit
 
 
 def main():
@@ -37,7 +34,7 @@ def main():
     ap.add_argument("--out_json", default=None)
     a = ap.parse_args()
     import torch
-    from bench_run_sequence import card, stats
+    from bench_run_sequence import stats
     from bundletrack_b200 import sequence, synth
     from bundletrack_b200.overlay import Overlay
     from oracle import overlay_oracle as oo
@@ -55,22 +52,16 @@ def main():
         ob_in_cam = synth.se3(synth.so3_exp(rng.normal(size=3)), np.array([rng.uniform(-0.1, 0.1), rng.uniform(-0.1, 0.1), rng.uniform(0.5, 0.9)]))
         poses.append(np.linalg.inv(ob_in_cam).astype(np.float32))
     poses = np.stack(poses)
-    out = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "H": H, "W": W, "device": {}, "host": {}}
+    out = {"card": benchkit.card(), "torch_device": torch.cuda.get_device_name(0), "H": H, "W": W, "device": {}, "host": {}}
     stream = torch.cuda.Stream(dev)
     for n in (1000, 10000, 100000):
         model = synth.make_ellipsoid_model(n, n, radii=(0.12, 0.09, 0.07))
         ov = Overlay(model, K, H, W, max_frames=F, stream=stream.cuda_stream, leaf=None)
         try:
             for per_call in (1, F):
-                for _ in range(3):                                  # warm-up
-                    ov.render(poses[:per_call], colour[:per_call], fg[:per_call], viz[:per_call], raw[:per_call])
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(stream)
-                for r in range(a.reps):
-                    ov.render(poses[:per_call], colour[:per_call], fg[:per_call], viz[:per_call], raw[:per_call])
-                e1.record(stream)
-                e1.synchronize()
-                out["device"][f"{n}_pts_{per_call}_per_call_ms_per_frame"] = e0.elapsed_time(e1) / (a.reps * per_call)
+                ms = benchkit.window_ms(lambda: ov.render(poses[:per_call], colour[:per_call], fg[:per_call], viz[:per_call], raw[:per_call]),
+                                        a.reps, 3, stream)
+                out["device"][f"{n}_pts_{per_call}_per_call_ms_per_frame"] = ms / per_call
         finally:
             ov.close()
         try:
@@ -93,31 +84,10 @@ def main():
     # run_sequence with log off and on
     N = a.frames
     seq = synth.make_sequence(7, N, H=H, W=W, n_feats=a.feats)
-
-    def features(id_str, request, roi):
-        f = seq.feats[int(id_str)]
-        if f is None:
-            raise sequence.DetectionFailed(id_str)
-        return f["kpts"], f["desc"]
-
+    features = synth.recorded_features(seq)
     with tempfile.TemporaryDirectory() as tmp:
-        model, scene = "camera_bench_norm", 1
-        nocs = f"{tmp}/nocs"
-        data, masks = f"{nocs}/real_test/scene_{scene}", f"{tmp}/masks"
-        gt = f"{nocs}/gts/real_test_text/scene_{scene}/model_{model}"
-        lst = f"{nocs}/NOCS-REAL275-additional/data_list/real_val/3/{model}"
-        for d in (data, masks, gt, lst, f"{nocs}/obj_models/real_test"):
-            os.makedirs(d)
-        for k in range(N):
-            synth.write_png(f"{data}/{k:04d}_color.png", seq.colour[k])
-            synth.write_png(f"{data}/{k:04d}_depth.png", np.clip(np.round(seq.depth_raw[k].astype(np.float64) * 1000), 0, 65535).astype(np.uint16))
-            synth.write_png(f"{masks}/{k:04d}.png", seq.mask[k])
-        np.savetxt(f"{gt}/0000.txt", np.linalg.inv(seq.poses_gt[0]))
-        with open(f"{lst}/list.txt", "w") as f:
-            f.write("".join(f"real_val/scene_{scene}/{k:04d}\n" for k in range(N)))
-        with open(f"{nocs}/obj_models/real_test/{model}.obj", "w") as f:
-            f.write("".join(f"v {x:.9g} {y:.9g} {z:.9g}\n" for x, y, z in synth.make_ellipsoid_model(1, 20000, radii=seq.radii).astype(np.float64)))
-        loader = sequence.NocsScene(nocs, scene, model, masks)
+        nocs, masks = synth.write_nocs_scene(seq, tmp, obj_points=synth.make_ellipsoid_model(1, 20000, radii=seq.radii))
+        loader = sequence.NocsScene(nocs, 1, "camera_bench_norm", masks)
         sequence.run_sequence(loader, None, features, f"{tmp}/warm", max_feats=a.feats, log=1)
         runs = {0: [], 1: []}
         for rep in range(2):

@@ -17,15 +17,12 @@ import argparse
 import ctypes
 import json
 import os
-import sys
 import tempfile
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
+import benchkit
 
 
 def sphere_views(n: int, dist: float):
@@ -54,13 +51,12 @@ def main():
     ap.add_argument("--out_json", default=None)
     a = ap.parse_args()
     import torch
-    from bench_run_sequence import card
     from bundletrack_b200 import _lib, recon, sequence, synth
     assert torch.cuda.is_available(), "this benchmark needs a GPU"
     dev = torch.device("cuda", 0)
     H, W, K = 480, 640, (590.0, 590.0, 319.5, 239.5)
     radii = (0.12, 0.09, 0.07)
-    out = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "H": H, "W": W, "radii": radii, "device": {}}
+    out = {"card": benchkit.card(), "torch_device": torch.cuda.get_device_name(0), "H": H, "W": W, "radii": radii, "device": {}}
     stream = torch.cuda.Stream(dev)
     T = sphere_views(200, 0.5)
     rng = np.random.default_rng(0)
@@ -74,19 +70,10 @@ def main():
             sel = np.linspace(0, 199, n).round().astype(int)       # spread over the sphere
             d = [depths[k] for k in sel]
             for voxel in (0.002, 0.001):
-                e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
                 nv, nf = ctypes.c_int(0), ctypes.c_int(0)
-                tf, tm = [], []
-                for r in range(a.reps + 2):                        # two warm-up calls
-                    e[0].record(stream)
-                    tsdf.fuse(d, cim[sel], K, voxel, 4 * voxel)
-                    e[1].record(stream)
-                    _lib.check(lib.bt_tsdf_mesh(tsdf.ctx, _lib.ptr(tsdf.verts), _lib.ptr(tsdf.faces), ctypes.byref(nv), ctypes.byref(nf), tsdf.stream))
-                    e[2].record(stream)
-                    e[2].synchronize()
-                    if r >= 2:
-                        tf.append(e[0].elapsed_time(e[1]))
-                        tm.append(e[1].elapsed_time(e[2]))
+                tf = benchkit.calls_ms(lambda: tsdf.fuse(d, cim[sel], K, voxel, 4 * voxel), a.reps, 2, stream)
+                tm = benchkit.calls_ms(lambda: _lib.check(lib.bt_tsdf_mesh(tsdf.ctx, _lib.ptr(tsdf.verts), _lib.ptr(tsdf.faces), ctypes.byref(nv),
+                                                                           ctypes.byref(nf), tsdf.stream)), a.reps, 2, stream)
                 dims = tsdf.grid()["dims"]
                 out["device"][f"{n}_frames_{voxel * 1000:g}mm"] = {"fuse_ms": float(np.median(tf)), "mesh_ms": float(np.median(tm)), "dims": dims,
                                                                    "samples": int(np.prod(dims)), "verts": nv.value, "faces": nf.value}
@@ -95,13 +82,7 @@ def main():
 
     N = a.frames
     seq = synth.make_sequence(9, N, H=H, W=W, n_feats=1000, rot_deg=(3.0, 6.0))
-
-    def features(id_str, request, roi):
-        f = seq.feats[int(id_str)]
-        if f is None:
-            raise sequence.DetectionFailed(id_str)
-        return f["kpts"], f["desc"]
-
+    features = synth.recorded_features(seq)
     with tempfile.TemporaryDirectory() as tmp:
         synth.write_ycbineoat_video(seq, f"{tmp}/video")
         loader = sequence.YcbineoatVideo(f"{tmp}/video")

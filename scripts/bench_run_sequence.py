@@ -16,22 +16,12 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
-import sys
 import tempfile
 import time
 
 import numpy as np
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-
-
-def card():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                              timeout=30).stdout.strip()
-    except Exception as e:        # the numbers stay valid; the card is then named by torch alone
-        return f"nvidia-smi unavailable ({e})"
+import benchkit
 
 
 def stats(t):
@@ -56,30 +46,11 @@ def main():
     seq = synth.make_sequence(7, N, H=H, W=W, n_feats=a.feats)
     print(f"sequence of {N} frames generated in {time.perf_counter() - t0:.1f} s", flush=True)
 
-    def features(id_str, request, roi):
-        f = seq.feats[int(id_str)]
-        if f is None:
-            raise sequence.DetectionFailed(id_str)
-        return f["kpts"], f["desc"]
-
-    mm = [np.clip(np.round(seq.depth_raw[k].astype(np.float64) * 1000), 0, 65535).astype(np.uint16) for k in range(N)]
+    features = synth.recorded_features(seq)
+    mm = [synth.depth_mm(d) for d in seq.depth_raw]
     with tempfile.TemporaryDirectory() as tmp:
-        model, scene = "camera_bench_norm", 1
-        nocs = f"{tmp}/nocs"
-        data = f"{nocs}/real_test/scene_{scene}"
-        masks = f"{tmp}/masks"
-        gt = f"{nocs}/gts/real_test_text/scene_{scene}/model_{model}"
-        lst = f"{nocs}/NOCS-REAL275-additional/data_list/real_val/3/{model}"
-        for d in (data, masks, gt, lst):
-            os.makedirs(d)
-        for k in range(N):
-            synth.write_png(f"{data}/{k:04d}_color.png", seq.colour[k])
-            synth.write_png(f"{data}/{k:04d}_depth.png", mm[k])
-            synth.write_png(f"{masks}/{k:04d}.png", seq.mask[k])
-        np.savetxt(f"{gt}/0000.txt", np.linalg.inv(seq.poses_gt[0]))
-        with open(f"{lst}/list.txt", "w") as f:
-            f.write("".join(f"real_val/scene_{scene}/{k:04d}\n" for k in range(N)))
-        loader = sequence.NocsScene(nocs, scene, model, masks)
+        nocs, masks = synth.write_nocs_scene(seq, tmp)
+        loader = sequence.NocsScene(nocs, 1, "camera_bench_norm", masks)
 
         # host decode per frame
         dec = []
@@ -141,7 +112,7 @@ def main():
         finally:
             fe.close()
 
-    out = {"card": card(), "torch_device": torch.cuda.get_device_name(0), "frames": N, "H": H, "W": W, "feats": a.feats,
+    out = {"card": benchkit.card(), "torch_device": torch.cuda.get_device_name(0), "frames": N, "H": H, "W": W, "feats": a.feats,
            "statuses": {str(s): statuses.count(s) for s in sorted(set(statuses))},
            "prefetch2": stats(runs[2]), "prefetch0": stats(runs[0]), "on_device": stats(on_dev), "decode": stats(dec),
            "frontend_u16_upload": stats(fe_u16), "frontend_host_convert_f32_upload": stats(fe_f32)}

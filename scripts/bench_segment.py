@@ -10,42 +10,12 @@ dilate, invalidate loop, ROI loop, crop and resize) when cv2 is importable, "not
 import argparse
 import json
 import os
-import subprocess
-import sys
+import statistics
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def card():
-    import torch
-    info = {"name": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        info["power_limit_and_max_sm_clock"] = q.stdout.strip().splitlines()[0]
-    except Exception as e:   # the card's name is still reported
-        info["power_limit_and_max_sm_clock"] = f"unavailable ({e})"
-    return info
-
-
-def time_events(fn, iters, warmup=5):
-    import torch
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    ts = []
-    for _ in range(3):
-        a.record()
-        for _ in range(iters):
-            fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) / iters)
-    return sorted(ts)[1]       # median of three windows, ms per call
+import benchkit
 
 
 def cpu_pipeline(cv2, mask, mode, depth, normal, colour):
@@ -89,8 +59,13 @@ def main():
     assert torch.cuda.is_available(), "bench_segment needs a GPU"
     dev = torch.device("cuda:0")
     H, W = args.H, args.W
-    res = {"card": card(), "H": H, "W": W, "rows": {}}
+    res = {"card": benchkit.card(), "H": H, "W": W, "rows": {}}
     fe = FrameFrontEnd()
+
+    def time_events(fn):
+        """ms per call: the median of three windows, the first after five warm-up calls."""
+        return statistics.median(benchkit.window_ms(fn, args.iters, warmup, fe.stream) for warmup in (5, 0, 0))
+
     for B in args.batches:
         raws = [torch.from_numpy(synth.make_raw_depth(s % 8, H, W)[0]).to(dev) for s in range(B)]
         masks = [torch.from_numpy(synth.make_object_mask(s, H, W)).to(dev) for s in range(B)]
@@ -107,9 +82,9 @@ def main():
         }
         row = {}
         for name, fn in fns.items():
-            row[name + "_ms_per_frame"] = time_events(fn, args.iters) / B
+            row[name + "_ms_per_frame"] = time_events(fn) / B
         fe.process_masked(raws, masks, H, W, K, d, nn, fg, mode=_lib.BT_MASK_LARGEST_HULL)
-        row["lfnet_request_ms_per_frame"] = time_events(lambda: fe.lfnet_request(cols, fg, H, W, req), args.iters) / B
+        row["lfnet_request_ms_per_frame"] = time_events(lambda: fe.lfnet_request(cols, fg, H, W, req)) / B
         # kernel times per name, from a profiled run of its own
         from torch.profiler import ProfilerActivity, profile
         torch.cuda.synchronize()

@@ -16,13 +16,11 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import sys
 import tempfile
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import numpy as np
 
-import numpy as np  # noqa: E402
+import benchkit
 
 
 def short(name: str) -> str:
@@ -128,6 +126,7 @@ def main():
     summ["tail"] = tail
     opt.close()
     summ["device"] = torch.cuda.get_device_name(dev)
+    summ["card"] = benchkit.card()
     print(json.dumps(summ, indent=1))
     if args.json:
         with open(args.json, "w") as f:

@@ -15,14 +15,10 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
+import benchkit
 
 
 def ellipsoid(radii, n_lat: int = 200, n_lon: int = 200):
@@ -47,29 +43,18 @@ def main():
     ap.add_argument("--out_json", default=None)
     a = ap.parse_args()
     import torch
-    from bench_run_sequence import card
     from bundletrack_b200.metrics import SurfaceScore
     assert torch.cuda.is_available(), "this benchmark needs a GPU"
     radii = np.array([0.06, 0.045, 0.035])
     mv, mf = ellipsoid(radii)
     rv, rf = ellipsoid(radii + 0.002)
     ss = SurfaceScore(len(mf), max(a.sizes))
-    stream = torch.cuda.ExternalStream(ss.stream.value) if ss.stream.value else torch.cuda.default_stream()
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
 
     def timed(fn):
-        fn()
-        torch.cuda.synchronize()
-        t = []
-        for _ in range(a.reps):
-            ev[0].record(stream)
-            fn()
-            ev[1].record(stream)
-            ev[1].synchronize()
-            t.append(ev[0].elapsed_time(ev[1]) * 1e-3)
+        t = [ms * 1e-3 for ms in benchkit.calls_ms(fn, a.reps, 1, ss.stream)]
         return float(np.median(t)), t
 
-    name = card()
+    name = benchkit.card()
     res = {"card": name, "faces": len(mf), "sizes": {}}
     print(f"card: {name}; meshes of {len(mf)} faces")
     for n in a.sizes:

@@ -10,25 +10,16 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+import benchkit
+
+sys.path.insert(0, os.path.join(benchkit.ROOT, "tests"))
 
 SYNC_CALLS = ("cudaStreamSynchronize", "cudaEventSynchronize", "cudaDeviceSynchronize", "cudaMemcpy")
-
-
-def gpu_info():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True,
-                              timeout=30).stdout.strip()
-    except Exception as e:      # the numbers still stand; the card is then unknown
-        return f"unknown ({e})"
 
 
 def upload(seq, dev):
@@ -89,7 +80,7 @@ def main():
     assert torch.cuda.is_available(), "bench_tracker needs an sm_90 GPU"
     dev = torch.device("cuda", 0)
     H, W, F = 480, 640, 64
-    res = {"gpu": gpu_info(), "H": H, "W": W, "feats": a.feats, "frames": a.frames}
+    res = {"gpu": benchkit.card(), "H": H, "W": W, "feats": a.feats, "frames": a.frames}
     seq = synth.make_sequence(11, a.frames, H=H, W=W, n_feats=a.feats)
     frames = upload(seq, dev)
     warm = synth.make_sequence(12, a.warmup, H=H, W=W, n_feats=a.feats)

@@ -9,12 +9,10 @@ median wall time per frame reading the mask files, and with masks=VosSource prop
 import argparse
 import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import benchkit
 
 
 def backbone_macs(H, W):
@@ -52,11 +50,6 @@ def main():
     assert torch.cuda.is_available(), "bench_vos.py measures on a GPU"
     dev = torch.device("cuda:0")
     name = torch.cuda.get_device_name(0)
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                               text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        power = "unknown"
     H, W, n = a.H, a.W, a.warmup + a.frames
     P = dict(vos.DEFAULTS)
     rng = np.random.default_rng(1)
@@ -87,15 +80,12 @@ def main():
     # per-frame device time with no timing events inside: events around the whole run
     outs = [torch.empty((H, W), dtype=torch.uint8, device=dev) for _ in range(n)]
     v.begin(frames[0], torch.from_numpy(m0).to(dev), out=outs[0], stream=stream)
-    for k in range(1, a.warmup + 1):
+    ks = iter(range(1, n))
+
+    def next_frame():
+        k = next(ks)
         v.next(frames[k], out=outs[k], stream=stream)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(a.warmup + 1, n):
-        v.next(frames[k], out=outs[k], stream=stream)
-    e1.record()
-    torch.cuda.synchronize()
-    per_frame = e0.elapsed_time(e1) / (n - a.warmup - 1)
+    per_frame = benchkit.window_ms(next_frame, n - a.warmup - 1, a.warmup, stream)
     Hd, Wd = -(-H // 8), -(-W // 8)
     HW = Hd * Wd
     bb = backbone_macs(H, W)
@@ -108,11 +98,11 @@ def main():
     comp, d = vo.compress_labels(m0)
     feats = [vo.features(frames[0].cpu().numpy(), sdt, torch.float32, dev).reshape(HW, 256)]
     labels = [torch.from_numpy(vo.init_label(comp, d)).float().to(dev).reshape(HW, d)]
-    ref_masks = [outs[0]]
-    t_ref = []
-    for k in range(1, n):
-        s0, s1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s0.record()
+    ups = []
+    ks = iter(range(1, n))
+
+    def ref_frame():
+        k = next(ks)
         f = vo.features(frames[k].cpu().numpy(), sdt, torch.float32, dev).reshape(HW, 256)
         idx = vo.schedule(k, P["ref_num"], P["range"])
         R = torch.cat([feats[i] for i in idx])
@@ -123,16 +113,13 @@ def main():
             S = S * wd
         pred = torch.cat([labels[i] for i in idx]).T @ S.reshape(-1, HW)
         lab = F.one_hot(pred.argmax(0), d).float()
-        up = F.interpolate(pred.view(1, d, Hd, Wd), size=(H, W), mode="bilinear", align_corners=False)[0].argmax(0)
-        s1.record()
-        torch.cuda.synchronize()
-        if k > a.warmup:
-            t_ref.append(s0.elapsed_time(s1))
+        ups.append(F.interpolate(pred.view(1, d, Hd, Wd), size=(H, W), mode="bilinear", align_corners=False)[0].argmax(0))
         feats.append(f)
         labels.append(lab)
-        ref_masks.append(torch.where(up > 0, 255, 0).to(torch.uint8))
-    disagree = float(np.mean([(ref_masks[k] != outs[k]).float().mean().item() for k in range(1, n)]))
-    res = dict(gpu=name, power_limit=power, H=H, W=W, frames=a.frames, params=P,
+    t_ref = benchkit.calls_ms(ref_frame, n - a.warmup - 1, a.warmup, stream)
+    ref_masks = [torch.where(up > 0, 255, 0).to(torch.uint8) for up in ups]
+    disagree = float(np.mean([(r != o).float().mean().item() for r, o in zip(ref_masks, outs[1:])]))
+    res = dict(gpu=name, power_limit=benchkit.card(), H=H, W=W, frames=a.frames, params=P,
                stage_ms_median=med, per_frame_ms=per_frame,
                backbone_gmac=bb / 1e9, propagation_gmac=prop / 1e9,
                backbone_tflops_3xtf32_counted_once=2 * bb / med["backbone"] / 1e9,
@@ -151,23 +138,10 @@ def run_sequence_times(H, W, n, sd):
     import torch
     from bundletrack_b200 import sequence, synth, vos
     seq = synth.make_sequence(52, n, H=H, W=W, n_feats=400)
+    features = synth.recorded_features(seq)
     with tempfile.TemporaryDirectory() as tmp:
         video = os.path.join(tmp, "synthvideo")
-        for k in range(n):
-            depth_mm = np.clip(np.round(seq.depth_raw[k].astype(np.float64) * 1000), 0, 65535).astype(np.uint16)
-            for sub, img in (("rgb", seq.colour[k]), ("depth", depth_mm), ("masks", seq.mask[k])):
-                os.makedirs(os.path.join(video, sub), exist_ok=True)
-                synth.write_png(os.path.join(video, sub, f"{k:07d}.png"), img)
-        os.makedirs(os.path.join(video, "annotated_poses"))
-        with open(os.path.join(video, "cam_K.txt"), "w") as f:
-            f.write(f"{seq.K[0]} 0 {seq.K[2]}\n0 {seq.K[1]} {seq.K[3]}\n0 0 1\n")
-        np.savetxt(os.path.join(video, "annotated_poses", f"{0:07d}.txt"), np.linalg.inv(np.asarray(seq.poses_gt[0], np.float64)))
-
-        def features(id_str, request, roi):
-            f = seq.feats[int(id_str)]
-            if f is None:
-                raise sequence.DetectionFailed(id_str)
-            return f["kpts"], f["desc"]
+        synth.write_ycbineoat_video(seq, video)
         out = {}
         for name in ("mask_files", "vos_source"):
             masks = None

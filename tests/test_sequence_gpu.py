@@ -27,10 +27,6 @@ def read_depth_image(mm: np.ndarray) -> np.ndarray:
     return d
 
 
-def _to_mm(depth_m: np.ndarray) -> np.ndarray:
-    return np.clip(np.round(depth_m.astype(np.float64) * 1000), 0, 65535).astype(np.uint16)
-
-
 def _dev(a, dev):
     import torch
     a = np.ascontiguousarray(a)
@@ -69,7 +65,7 @@ def test_u16_front_end_equals_float_on_converted_depth(cuda_device, params, mode
     cases = [(every, synth.make_object_mask(1, 256, 256), synth.NOCS_K)]
     for seed, (H, W) in ((2, (240, 320)), (3, (480, 640)), (4, (97, 131))):
         raw, K = synth.make_raw_depth(seed, H, W)
-        cases.append((_to_mm(raw), synth.make_object_mask(seed, H, W), K))
+        cases.append((synth.depth_mm(raw), synth.make_object_mask(seed, H, W), K))
     fe = FrameFrontEnd(yml)
     try:
         for mm, mask, K in cases:
@@ -121,7 +117,7 @@ def test_begin_frame_u16_equals_begin_frame(cuda_device):
     statuses = []
     try:
         for k in range(N):
-            mm = _to_mm(seq.depth_raw[k])
+            mm = synth.depth_mm(seq.depth_raw[k])
             m, c = _dev(seq.mask[k], cuda_device), _dev(seq.colour[k], cuda_device)
             fp = first if k == 0 else np.eye(4, dtype=np.float32)
             ids, poses, _ = a.state()
@@ -164,7 +160,7 @@ def _features(seq):
 
 def _write_frames(seq, colour_path, depth_path, mask_path):
     for k in range(seq.n_frames):
-        for path, img in ((colour_path(k), seq.colour[k]), (depth_path(k), _to_mm(seq.depth_raw[k])), (mask_path(k), seq.mask[k])):
+        for path, img in ((colour_path(k), seq.colour[k]), (depth_path(k), synth.depth_mm(seq.depth_raw[k])), (mask_path(k), seq.mask[k])):
             os.makedirs(os.path.dirname(path), exist_ok=True)
             synth.write_png(path, img)
 
