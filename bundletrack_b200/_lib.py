@@ -286,6 +286,9 @@ PROTOTYPES = {
     "bt_mesh_sample": (_i, (_p, _p, _i, _p, _i, _i, _u64, _p, _p)),
     "bt_surface_distances": (_i, (_p, _p, _i, _p, _i, _p, _p, _p)),
     "bt_surface_score": (_i, (_p, _i, _p, _i, _p, _i, _p)),
+    "bt_mask_reserve": (_i, (_p, _i, _i, _i)),
+    "bt_mask_metrics": (_i, (_p, _p, _p, _i, _i, _i, _d, _p, _p, _p, _p)),
+    "bt_mask_score": (_i, (_p, _p, _i, _p)),
     "bt_voxel_downsample": (_i, (_p, _i, _p, _p, _f, _p, _p, _p)),
     "bt_overlay_reserve": (_i, (_p, _i, _i)),
     "bt_pose_overlay": (_i, (_p, _i, _p, _i, _p, _f, _f, _f, _f, _p, _p, _i, _i, _p, _p, _p)),

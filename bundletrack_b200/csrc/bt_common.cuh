@@ -198,6 +198,7 @@ struct LfnetState;    // lfnet.cu
 struct VosState;      // vos.cu
 struct ReconState;    // recon.cu
 struct SurfaceState;  // metrics.cu
+struct MaskState;     // metrics.cu
 
 // The context owns the module states; each module defines the deleter of its state next to it, so the states stay private to their files.
 struct StateDeleter {
@@ -216,6 +217,7 @@ struct StateDeleter {
 	void operator()(VosState*) const;
 	void operator()(ReconState*) const;
 	void operator()(SurfaceState*) const;
+	void operator()(MaskState*) const;
 };
 template <class T> using StatePtr = std::unique_ptr<T, StateDeleter>;
 
@@ -240,6 +242,7 @@ struct bt_ctx {
 	bt::StatePtr<bt::VosState> vos;
 	bt::StatePtr<bt::ReconState> recon;
 	bt::StatePtr<bt::SurfaceState> surface;
+	bt::StatePtr<bt::MaskState> mask;
 };
 
 namespace bt {

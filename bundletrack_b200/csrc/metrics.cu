@@ -888,3 +888,278 @@ extern "C" int bt_surface_score(const double* d_ab, int n_a, const double* d_ba,
 	}
 	return BT_OK;
 }
+
+// ---- mask accuracy: the DAVIS region similarity J and boundary accuracy F per frame (DESIGN.md §3.16) ----------------------------------
+// J = |P & G| / |P | G| (1 for an empty union).  F: the boundary maps b(P), b(G) with _seg2bmap's edge rules, the tolerance radius
+// r = ceil(bound_th sqrt(H^2 + W^2)), the matches m_P = #{boundary pixels of P with a boundary pixel of G at dx^2 + dy^2 <= r^2} and m_G the
+// same the other way, then precision m_P / n_P, recall m_G / n_G and F = 2 P R / (P + R), with the toolkit's rules for empty boundaries.
+// One CTA per (frame, band of kMaskBand rows) holds both masks as bit rows in shared memory, 64 pixels to a word (bit j of word c is pixel
+// 64 c + j): the band plus r rows above it and r + 1 below, clipped to the image.  The six counts are integers, so summing them per frame
+// in any order is exact, and k_mask_final forms J and F from them in float64.
+namespace bt {
+namespace {
+
+constexpr int kMaskThreads = 256;
+constexpr int kMaskBand = 64;                      // rows per CTA
+constexpr int kMaxMaskRadius = 64;                 // r: a row is dilated from its two neighbouring words at most
+constexpr int kMaskCounts = 6;                     // |P & G|, |P | G|, n_P, n_G, m_P, m_G
+constexpr int kMaxMaskBands = 65535;               // grid.y
+typedef unsigned long long u64;
+
+__host__ __device__ __forceinline__ int mask_words(int w) { return (w + 63) / 64; }
+// shared bit rows of one mask for a band: at most the band, r rows above and r + 1 below
+__host__ __device__ __forceinline__ int mask_rows(int h, int r) { return min(kMaskBand + 2 * r + 1, h); }
+
+// bit j set when byte j of x is not 0: __vcmpne4 gives 0xff per such byte, and the multiply gathers the bytes' low bits into bits 28..31
+__device__ __forceinline__ unsigned nonzero4(unsigned x) { return ((__vcmpne4(x, 0u) & 0x01010101u) * 0x10204080u) >> 28; }
+__device__ __forceinline__ unsigned nonzero16(uint4 v) { return nonzero4(v.x) | nonzero4(v.y) << 4 | nonzero4(v.z) << 8 | nonzero4(v.w) << 12; }
+
+// One warp packs row `src` (w bytes at any alignment) into dst[0, nw): it reads the whole 16-byte blocks that hold a pixel of the row, one
+// per lane, and word c takes the 64 bits that start d = src & 15 bits into blocks 4c .. 4c + 4.  Bits past the row's end are 0.
+__device__ void pack_row(const uint8_t* src, int w, u64* dst, int nw, int lane) {
+	const uint4* blk = reinterpret_cast<const uint4*>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)15);
+	const int d = (int)(reinterpret_cast<uintptr_t>(src) & 15);
+	const int n_blk = (d + w + 15) >> 4;
+	for (int c0 = 0; c0 < nw; c0 += 8) {                // 8 words, 32 blocks (plus the next round's first) per round
+		const int k = 4 * c0 + lane;
+		const unsigned m = k < n_blk ? nonzero16(__ldg(blk + k)) : 0u;
+		const unsigned next = (lane == 31 && k + 1 < n_blk) ? nonzero16(__ldg(blk + k + 1)) : 0u;
+		const int i = lane & 7;
+		const u64 m0 = __shfl_sync(0xffffffffu, m, 4 * i), m1 = __shfl_sync(0xffffffffu, m, 4 * i + 1);
+		const u64 m2 = __shfl_sync(0xffffffffu, m, 4 * i + 2), m3 = __shfl_sync(0xffffffffu, m, 4 * i + 3);
+		const unsigned m4a = __shfl_sync(0xffffffffu, m, (4 * i + 4) & 31), m4b = __shfl_sync(0xffffffffu, next, 31);
+		const u64 m4 = i == 7 ? m4b : m4a;
+		u64 v = m0 | m1 << 16 | m2 << 32 | m3 << 48;
+		if (d) v = (v >> d) | (m4 << (64 - d));
+		const int c = c0 + i, valid = w - 64 * c;
+		if (lane < 8 && c < nw) dst[c] = valid >= 64 ? v : v & ((1ull << valid) - 1);
+	}
+}
+
+// Pixels of word c of bit row R that have a set pixel of R within h columns (0 <= h <= 64): the 192 bits of words c - 1 .. c + 1 are
+// spread h columns one way and then h the other, each by doubling.  Words outside [0, nw) are 0.
+__device__ __forceinline__ u64 dilate_word(const u64* R, int c, int nw, int h) {
+	u64 lo = c > 0 ? R[c - 1] : 0, mid = R[c], hi = c + 1 < nw ? R[c + 1] : 0;
+	if ((lo | mid | hi) == 0) return 0;
+	// every bit takes the OR of itself and the h bits above it (steps of at most 32, so no shift reaches 64)
+	for (int cover = 1; cover <= h;) {
+		const int s = min(cover, h + 1 - cover);
+		lo |= (lo >> s) | (mid << (64 - s));
+		mid |= (mid >> s) | (hi << (64 - s));
+		hi |= hi >> s;
+		cover += s;
+	}
+	// then of itself and the h bits below it
+	for (int cover = 1; cover <= h;) {
+		const int s = min(cover, h + 1 - cover);
+		mid |= (mid << s) | (lo >> (64 - s));
+		lo |= lo << s;
+		cover += s;
+	}
+	return mid;
+}
+
+__device__ __forceinline__ int isqrt(int n) {
+	int v = (int)sqrt((double)n);
+	while (v * v > n) v--;
+	while ((v + 1) * (v + 1) <= n) v++;
+	return v;
+}
+
+// grid (n_frames, n_bands): block (f, band) writes band_counts[f][band][0..5] for rows [y0, y0 + kMaskBand) of frame f
+__global__ void __launch_bounds__(kMaskThreads) k_mask_band(const uint8_t* __restrict__ pred, const uint8_t* __restrict__ gt, int h, int w, int r,
+                                                            unsigned* __restrict__ band_counts) {
+	extern __shared__ u64 s_bits[];                    // [2][n_rows][nw]: the prediction's rows, then the ground truth's
+	__shared__ int s_h[2 * kMaxMaskRadius + 1];        // s_h[dy + r] = isqrt(r^2 - dy^2): the disk's half-width on row dy
+	__shared__ unsigned s_cnt[kMaskCounts];
+	const int f = blockIdx.x, band = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int nw = mask_words(w);
+	const int y0 = band * kMaskBand, y1 = min(y0 + kMaskBand, h);
+	const int ylo = max(0, y0 - r), yhi = min(h, y1 + r + 1);        // the rows held
+	const int n_rows = yhi - ylo, n_brows = min(h, y1 + r) - ylo;      // the first n_brows become boundary rows
+	for (int k = tid; k <= 2 * r; k += kMaskThreads) s_h[k] = isqrt(r * r - (k - r) * (k - r));
+	if (tid < kMaskCounts) s_cnt[tid] = 0;
+
+	for (int t = warp; t < 2 * n_rows; t += kMaskThreads / 32) {
+		const int map = t & 1, row = t >> 1;
+		const uint8_t* src = (map ? gt : pred) + ((size_t)f * h + ylo + row) * (size_t)w;
+		pack_row(src, w, s_bits + ((size_t)map * n_rows + row) * nw, nw, lane);
+	}
+	__syncthreads();
+
+	u64* const P = s_bits;
+	u64* const G = s_bits + (size_t)n_rows * nw;
+	unsigned inter = 0, uni = 0;
+	for (int k = tid; k < (y1 - y0) * nw; k += kMaskThreads) {
+		const int i = (y0 - ylo) * nw + k;
+		inter += __popcll(P[i] & G[i]);
+		uni += __popcll(P[i] | G[i]);
+	}
+
+	// The boundary maps, in place: b at (y, x) reads S at (y, x), (y, x + 1), (y + 1, x) and (y + 1, x + 1), all at or after its own word in
+	// row-major order.  So each round reads its words before the barrier and writes them after it, and no round reads a word an earlier
+	// round has written.
+	const int per_map = n_brows * nw;
+	for (int base = 0; base < 2 * per_map; base += kMaskThreads) {
+		const int k = base + tid;
+		const bool mine = k < 2 * per_map;
+		u64 b = 0;
+		int at = 0;
+		if (mine) {
+			const int map = k >= per_map, rem = k - map * per_map, row = rem / nw, c = rem - row * nw, y = ylo + row;
+			const u64* S = s_bits + (size_t)map * n_rows * nw;
+			at = map * n_rows * nw + rem;
+			const u64 s = S[rem], e = (s >> 1) | ((c + 1 < nw ? S[rem + 1] : 0) << 63);
+			const int n_in = w - 1 - 64 * c;              // pixels of this word left of the last column
+			const u64 inner = n_in >= 64 ? ~0ull : n_in <= 0 ? 0 : (1ull << n_in) - 1;
+			const u64 last = (n_in >= 0 && n_in < 64) ? 1ull << n_in : 0;
+			if (y < h - 1) {
+				const u64 so = S[rem + nw], se = (so >> 1) | ((c + 1 < nw ? S[rem + nw + 1] : 0) << 63);
+				b = (((s ^ e) | (s ^ so) | (s ^ se)) & inner) | ((s ^ so) & last);
+			} else {
+				b = (s ^ e) & inner;                        // the last row; its last pixel is the corner, 0
+			}
+		}
+		__syncthreads();
+		if (mine) s_bits[at] = b;
+		__syncthreads();
+	}
+
+	// matches: a boundary word of one map against the other map's boundary rows y - r .. y + r, each dilated by the disk's half-width
+	unsigned n_p = 0, n_g = 0, m_p = 0, m_g = 0;
+	const int band_words = (y1 - y0) * nw;
+	for (int k = tid; k < 2 * band_words; k += kMaskThreads) {
+		const int map = k >= band_words, rem = k - map * band_words, row = (y0 - ylo) + rem / nw, c = rem % nw;
+		const u64* Q = s_bits + (size_t)map * n_rows * nw;
+		const u64* O = s_bits + (size_t)(1 - map) * n_rows * nw;
+		const u64 q = Q[(size_t)row * nw + c];
+		if (!q) continue;
+		const int dy0 = max(-r, -row), dy1 = min(r, n_brows - 1 - row);
+		u64 hit = 0;
+		for (int dy = dy0; dy <= dy1 && (hit & q) != q; dy++) hit |= dilate_word(O + (size_t)(row + dy) * nw, c, nw, s_h[dy + r]);
+		const unsigned n = __popcll(q), m = __popcll(hit & q);
+		if (map) { n_g += n; m_g += m; }
+		else { n_p += n; m_p += m; }
+	}
+
+	const unsigned v[kMaskCounts] = {inter, uni, n_p, n_g, m_p, m_g};
+#pragma unroll
+	for (int i = 0; i < kMaskCounts; i++) {
+		const unsigned s = __reduce_add_sync(0xffffffffu, v[i]);
+		if (lane == 0 && s) atomicAdd(&s_cnt[i], s);
+	}
+	__syncthreads();
+	if (tid < kMaskCounts) band_counts[((size_t)f * gridDim.y + band) * kMaskCounts + tid] = s_cnt[tid];
+}
+
+// one thread per frame: the bands' counts in band order, then J and F in float64
+__global__ void k_mask_final(const unsigned* __restrict__ band_counts, int n_bands, int n_frames, double* __restrict__ j_out,
+                             double* __restrict__ f_out, long long* __restrict__ counts_out) {
+	const int f = blockIdx.x * blockDim.x + threadIdx.x;
+	if (f >= n_frames) return;
+	long long c[kMaskCounts] = {0, 0, 0, 0, 0, 0};
+	for (int b = 0; b < n_bands; b++)
+		for (int i = 0; i < kMaskCounts; i++) c[i] += band_counts[((size_t)f * n_bands + b) * kMaskCounts + i];
+	const long long inter = c[0], uni = c[1], n_p = c[2], n_g = c[3], m_p = c[4], m_g = c[5];
+	double precision, recall;
+	if (n_p == 0 && n_g > 0) { precision = 1.0; recall = 0.0; }
+	else if (n_p > 0 && n_g == 0) { precision = 0.0; recall = 1.0; }
+	else if (n_p == 0 && n_g == 0) { precision = 1.0; recall = 1.0; }
+	else { precision = __ddiv_rn((double)m_p, (double)n_p); recall = __ddiv_rn((double)m_g, (double)n_g); }
+	const double pr = add(precision, recall);
+	j_out[f] = uni == 0 ? 1.0 : __ddiv_rn((double)inter, (double)uni);
+	f_out[f] = pr == 0.0 ? 0.0 : __ddiv_rn(mul(mul(2.0, precision), recall), pr);
+	if (counts_out)
+		for (int i = 0; i < kMaskCounts; i++) counts_out[(size_t)f * kMaskCounts + i] = c[i];
+}
+
+// bytes of shared bit rows a band needs
+size_t mask_smem(int h, int w, int r) { return 2 * sizeof(u64) * (size_t)mask_rows(h, r) * (size_t)mask_words(w); }
+
+}  // namespace
+
+struct MaskState {
+	bool ready = false;
+	int max_frames = 0, max_h = 0, max_w = 0;
+	DevBuf band;
+};
+void StateDeleter::operator()(MaskState* s) const { delete s; }
+
+}  // namespace bt
+
+extern "C" int bt_mask_reserve(bt_ctx* ctx, int max_frames, int max_h, int max_w) {
+	BT_REQUIRE(ctx, BT_ERR_INVALID_ARG, "bt_mask_reserve: ctx is NULL");
+	BT_REQUIRE(max_frames >= 1 && max_h >= 1 && max_w >= 1, BT_ERR_INVALID_ARG, "bt_mask_reserve: max_frames %d / max_h %d / max_w %d must be >= 1",
+	           max_frames, max_h, max_w);
+	const int max_bands = (max_h + kMaskBand - 1) / kMaskBand;
+	BT_REQUIRE(max_bands <= kMaxMaskBands, BT_ERR_INVALID_ARG, "bt_mask_reserve: max_h %d > %d", max_h, kMaxMaskBands * kMaskBand);
+	BT_CUDA(cudaSetDevice(ctx->device));
+	int optin = 0;
+	cudaFuncAttributes fa;
+	BT_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+	BT_CUDA(cudaFuncGetAttributes(&fa, k_mask_band));
+	const size_t smem = mask_smem(max_h, max_w, kMaxMaskRadius), room = (size_t)optin - fa.sharedSizeBytes;
+	BT_REQUIRE(smem <= room, BT_ERR_INVALID_ARG,
+	           "bt_mask_reserve: a band of %d x %d masks needs %zu bytes of shared memory at r = %d, the device has %zu per block", max_h, max_w, smem,
+	           kMaxMaskRadius, room);
+	MaskState* s;
+	BT_TRY(take_state(ctx, &bt_ctx::mask, &s));
+	// the kernel's limit is the device's, not this reservation's: it is one setting for every context in the process
+	BT_CUDA(cudaFuncSetAttribute(k_mask_band, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)room));
+	BT_TRY(s->band.alloc(sizeof(unsigned) * kMaskCounts * (size_t)max_bands * (size_t)max_frames));
+	s->max_frames = max_frames; s->max_h = max_h; s->max_w = max_w;
+	s->ready = true;
+	return BT_OK;
+}
+
+extern "C" int bt_mask_metrics(bt_ctx* ctx, const uint8_t* pred_dev, const uint8_t* gt_dev, int n_frames, int h, int w, double bound_th,
+                               double* j_dev, double* f_dev, int64_t* counts_dev, void* stream_) {
+	BT_REQUIRE(pred_dev && gt_dev && j_dev && f_dev, BT_ERR_INVALID_ARG, "bt_mask_metrics: NULL argument");
+	BT_REQUIRE(n_frames >= 1 && h >= 1 && w >= 1, BT_ERR_INVALID_ARG, "bt_mask_metrics: n_frames %d / h %d / w %d must be >= 1", n_frames, h, w);
+	BT_REQUIRE(bound_th > 0.0 && bound_th < 1.0, BT_ERR_INVALID_ARG, "bt_mask_metrics: bound_th %g must be in (0, 1)", bound_th);
+	const double rr = ceil(bound_th * sqrt((double)h * h + (double)w * w));
+	BT_REQUIRE(rr <= kMaxMaskRadius, BT_ERR_INVALID_ARG, "bt_mask_metrics: the tolerance radius %.0f of bound_th %g at %d x %d exceeds %d", rr, bound_th, h, w,
+	           kMaxMaskRadius);
+	const int r = (int)rr;
+	MaskState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::mask, "bt_mask_metrics", "bt_mask_reserve", &s));
+	BT_REQUIRE(n_frames <= s->max_frames && h <= s->max_h && w <= s->max_w, BT_ERR_CAPACITY,
+	           "bt_mask_metrics: %d frames of %d x %d exceed the reserved %d of %d x %d", n_frames, h, w, s->max_frames, s->max_h, s->max_w);
+	cudaStream_t stream = (cudaStream_t)stream_;
+	const int n_bands = (h + kMaskBand - 1) / kMaskBand;
+	unsigned* band = s->band.as<unsigned>();
+	k_mask_band<<<dim3(n_frames, n_bands), kMaskThreads, mask_smem(h, w, r), stream>>>(pred_dev, gt_dev, h, w, r, band);
+	k_mask_final<<<(n_frames + 127) / 128, 128, 0, stream>>>(band, n_bands, n_frames, j_dev, f_dev, reinterpret_cast<long long*>(counts_dev));
+	BT_CUDA(cudaGetLastError());
+	return BT_OK;
+}
+
+// db_statistics of one sequence's per-frame values: the mean (numpy's pairwise sum), the recall mean(x > 0.5), and the decay, the mean of
+// the first of four bins minus that of the last, bin i = x[ids[i] .. ids[i + 1]] with ids = round_half_even(linspace(1, n, 5) + 1e-10) - 1.
+static void db_statistics(const double* x, int n, double* mean, double* recall, double* decay) {
+	*mean = np_pairwise_sum(x, n) / (double)n;
+	int above = 0;
+	for (int i = 0; i < n; i++) above += x[i] > 0.5;
+	*recall = (double)above / (double)n;
+	long long ids[5];
+	const double step = (double)(n - 1) / 4.0;
+	for (int i = 0; i < 5; i++) {
+		const double at = i < 4 ? (double)i * step + 1.0 : (double)n;      // numpy's linspace: its last point is exactly `stop`
+		ids[i] = (long long)nearbyint(at + 1e-10) - 1;                     // round half to even, the default rounding mode
+	}
+	const double first = np_pairwise_sum(x + ids[0], (size_t)(ids[1] + 1 - ids[0])) / (double)(ids[1] + 1 - ids[0]);
+	const double last = np_pairwise_sum(x + ids[3], (size_t)(ids[4] + 1 - ids[3])) / (double)(ids[4] + 1 - ids[3]);
+	*decay = first - last;
+}
+
+extern "C" int bt_mask_score(const double* j, const double* f, int n, double* out) {
+	BT_REQUIRE(j && f && out, BT_ERR_INVALID_ARG, "bt_mask_score: NULL argument");
+	BT_REQUIRE(n >= 1, BT_ERR_INVALID_ARG, "bt_mask_score: n %d must be >= 1", n);
+	double jm, jr, jd, fm, fr, fd;
+	db_statistics(j, n, &jm, &jr, &jd);
+	db_statistics(f, n, &fm, &fr, &fd);
+	out[0] = (jm + fm) / 2.0;
+	out[1] = jm; out[2] = jr; out[3] = jd;
+	out[4] = fm; out[5] = fr; out[6] = fd;
+	return BT_OK;
+}

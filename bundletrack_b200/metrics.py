@@ -1,6 +1,7 @@
 """Pose accuracy as BundleTrack is judged: ADD and ADD-S per frame (the reference's scripts/Utils.py add / adi) on the device, and their
 VOCap AUC (scripts/eval_ycbineoat.py) on the host.  A thin ctypes mirror of bt_pose_metrics / bt_vocap (include/bundletrack_b200.h).
-Also the NOCS-REAL275 scores, and an object model's accuracy against a reference mesh (SurfaceScore).
+Also the NOCS-REAL275 scores, an object model's accuracy against a reference mesh (SurfaceScore), and the DAVIS J and F scores of
+object masks against ground-truth masks (MaskScore).
 Poses are ob_in_cam (model -> camera), the matrices poses/<id>.txt holds; `ob_in_cam` turns the tracker's cam -> model poses into them."""
 from __future__ import annotations
 
@@ -209,3 +210,64 @@ class SurfaceScore(_lib.Facade):
         res = surface_score(*self.distances(a, b), taus)
         res["n_samples"] = int(n_samples)
         return res
+
+
+# Mask accuracy (DESIGN.md §3.16): the DAVIS region similarity J and boundary accuracy F per frame on the device, and their per-sequence
+# statistics on the host, in the DAVIS toolkit's CSV order.
+MASK_SCORE_KEYS = ("J&F-Mean", "J-Mean", "J-Recall", "J-Decay", "F-Mean", "F-Recall", "F-Decay")
+MASK_COUNT_KEYS = ("inter", "union", "n_pred", "n_gt", "m_pred", "m_gt")
+
+
+def mask_score(j, f) -> dict:
+    """bt_mask_score (host code) of one sequence's per-frame J and F: the mean, the recall (the fraction of frames above 0.5) and the decay
+    of each, and J&F, the mean of the two means, under MASK_SCORE_KEYS."""
+    a = np.ascontiguousarray(np.asarray(j, np.float64).reshape(-1))
+    b = np.ascontiguousarray(np.asarray(f, np.float64).reshape(-1))
+    if a.size != b.size:
+        raise ValueError(f"mask_score: {a.size} J values and {b.size} F values")
+    out = np.zeros(len(MASK_SCORE_KEYS), np.float64)
+    _lib.check(_lib.load().bt_mask_score(_lib.ptr(a), _lib.ptr(b), a.size, _lib.ptr(out)), "bt_mask_score")
+    return dict(zip(MASK_SCORE_KEYS, out.tolist()))
+
+
+class MaskScore(_lib.Facade):
+    """J and F of predicted masks against ground-truth masks on the device.  Room for calls of up to max_frames frames of h x w is reserved
+    here; longer inputs are scored max_frames at a time."""
+
+    def __init__(self, max_frames: int, h: int, w: int, device: int = 0, stream: int = 0, ctx=None):
+        super().__init__(ctx, device, stream)
+        self.device, self.max_frames = device, int(max_frames)
+        _lib.check(self.lib.bt_mask_reserve(self.ctx, int(max_frames), int(h), int(w)), "bt_mask_reserve")
+
+    @staticmethod
+    def _frames(x, what: str):
+        import torch
+        t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
+        if t.dtype == torch.bool:
+            t = t.view(torch.uint8)
+        if t.dtype != torch.uint8 or t.dim() != 3:
+            raise ValueError(f"{what}: expected uint8 or bool [F, H, W], got {t.dtype} {list(t.shape)}")
+        return t
+
+    def __call__(self, pred, gt, bound_th: float = 0.008, counts: bool = False):
+        """(j, f), float64 numpy [F], of pred against gt (numpy or CUDA, uint8 or bool [F, H, W], foreground = non-zero); with counts=True
+        also the int64 [F, 6] counts |P & G|, |P | G|, n_P, n_G, m_P, m_G (MASK_COUNT_KEYS)."""
+        import torch
+        P, G = self._frames(pred, "pred"), self._frames(gt, "gt")
+        if P.shape != G.shape:
+            raise ValueError(f"pred {list(P.shape)} and gt {list(G.shape)} differ")
+        n, h, w = P.shape
+        dev = torch.device("cuda", self.device)
+        j = torch.empty(n, dtype=torch.float64, device=dev)
+        f = torch.empty(n, dtype=torch.float64, device=dev)
+        c = torch.empty((n, 6), dtype=torch.int64, device=dev) if counts else None
+        held = []                                  # each call's inputs, alive until the stream has read them
+        for s in range(0, n, self.max_frames):
+            e = min(n, s + self.max_frames)
+            p, g = P[s:e].to(dev).contiguous(), G[s:e].to(dev).contiguous()
+            held += [p, g]
+            _lib.check(self.lib.bt_mask_metrics(self.ctx, _lib.ptr(p), _lib.ptr(g), e - s, h, w, float(bound_th), _lib.ptr(j[s:]), _lib.ptr(f[s:]),
+                                                _lib.ptr(c[s:]) if counts else None, self.stream), "bt_mask_metrics")
+        _lib.check(self.lib.bt_stream_sync(self.stream), "bt_stream_sync")
+        out = (j.cpu().numpy(), f.cpu().numpy())
+        return out + (c.cpu().numpy(),) if counts else out

@@ -331,6 +331,30 @@ def make_object_mask(seed: int, H: int = 480, W: int = 640, n_distractors: int =
     return (m * np.uint8(value)).astype(np.uint8)
 
 
+def ragged_ellipse_masks(n_frames: int, H: int = 480, W: int = 640, seed: int = 0):
+    """(pred, gt): uint8 [n_frames, H, W] 0 / 255 masks of an ellipse that moves across the frame and turns, its outline made ragged by a few
+    harmonics of the polar angle.  The prediction is the same ellipse displaced by up to about 2 % of the frame, with harmonics of its own
+    that change from frame to frame, as a segmenter's error would.  For the mask scores' tests and benchmark."""
+    rng = np.random.default_rng(np.uint64(0xDA715) + np.uint64(seed))
+    y, x = np.mgrid[0:H, 0:W].astype(np.float32)
+    k = np.arange(3, 9, dtype=np.float32)
+    amp_g, ph_g = rng.uniform(0.01, 0.04, 6).astype(np.float32), rng.uniform(0, 2 * np.pi, 6).astype(np.float32)
+    out = np.zeros((2, n_frames, H, W), np.uint8)
+    for f in range(n_frames):
+        t = f / max(n_frames - 1, 1)
+        cx, cy = (0.3 + 0.4 * t) * W, (0.4 + 0.2 * np.sin(2 * np.pi * t)) * H
+        ax, ay, th = 0.18 * W, 0.22 * H, np.float32(np.pi * t)
+        d = 0.02 * rng.uniform(-1, 1, 2) * (W, H)
+        amp_p, ph_p = rng.uniform(0.01, 0.04, 6).astype(np.float32), rng.uniform(0, 2 * np.pi, 6).astype(np.float32)
+        for m, (ox, oy, amp, ph) in enumerate(((d[0], d[1], amp_p, ph_p), (0.0, 0.0, amp_g, ph_g))):
+            u, v = x - np.float32(cx + ox), y - np.float32(cy + oy)
+            u, v = u * np.cos(th) + v * np.sin(th), v * np.cos(th) - u * np.sin(th)
+            ang = np.arctan2(v / ay, u / ax)
+            rag = 1 + (amp[:, None, None] * np.cos(k[:, None, None] * ang + ph[:, None, None])).sum(0)
+            out[m, f] = ((u / ax) ** 2 + (v / ay) ** 2 <= rag * rag) * np.uint8(255)
+    return out[0], out[1]
+
+
 def make_ransac_case(seed: int, n: int, inlier_frac: float = 0.7, noise: float = 0.0005):
     """Model-frame point pairs as SiftManager::runRansacMultiPairGPU uploads them (/root/reference/src/FeatureManager.cpp:676-706):
     B = T A + noise for the inliers, the rest displaced by centimetres.  Returns (A [n,4], B [n,4] float32 with w = 1, inlier mask)."""

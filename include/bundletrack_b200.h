@@ -633,6 +633,40 @@ BT_API int bt_surface_distances(bt_ctx* ctx, const double* a_dev, int n_a, const
  * n_taus < 0, a distance that is negative or not finite, or a tau that is not positive and finite. */
 BT_API int bt_surface_score(const double* d_ab, int n_a, const double* d_ba, int n_b, const double* taus, int n_taus, double* out);
 
+/* ---- mask accuracy: the DAVIS region similarity J and boundary accuracy F per frame, and their per-sequence statistics (DESIGN.md §3.16) --
+ * These restate the DAVIS toolkit's metrics (davis2017-evaluation metrics.py / utils.py); oracle/mask_oracle.py restates them in numpy.
+ * P is the prediction and G the ground truth, H x W uint8 each, foreground = value != 0.
+ *   J = |P & G| / |P | G| in float64, 1 when the union is 0.
+ *   b(S), the boundary map (_seg2bmap): with e(y,x) = S(y,x+1), s(y,x) = S(y+1,x), se(y,x) = S(y+1,x+1), each 0 outside the image,
+ *     b = (S ^ e) | (S ^ s) | (S ^ se) for y < H-1 and x < W-1;  b = S ^ e on the last row (x < W-1);  b = S ^ s on the last column
+ *     (y < H-1);  b = 0 at the corner (H-1, W-1).  So a full-frame mask has no boundary, nor does foreground along the top or left edge.
+ *   r = ceil(bound_th sqrt(H^2 + W^2)) in float64 (bound_th 0.008: r = 7 at 480 x 640, 8 at 480 x 854, 12 at 720 x 1280, 18 at 1080 x 1920);
+ *     the disk is every offset with dx^2 + dy^2 <= r^2 (skimage disk(r) under cv2.dilate, nothing dilating in from outside the image).
+ *   m_P = #{pixels of b(P) with a pixel of b(G) within the disk}, m_G the same with P and G swapped, n_P = |b(P)|, n_G = |b(G)|.
+ *   precision, recall = (1, 0) when n_P = 0 < n_G;  (0, 1) when n_G = 0 < n_P;  (1, 1) when both are 0;  else m_P / n_P, m_G / n_G.
+ *   F = 0 when precision + recall = 0, else 2 precision recall / (precision + recall), left to right in float64.
+ * bt_mask_metrics: J and F of n_frames frame pairs.
+ *   pred_dev / gt_dev  DEVICE uint8 [n_frames][h][w], contiguous, any alignment.  The kernel reads the whole 16-byte blocks that hold a pixel
+ *                      of the arrays, so it may read up to 15 bytes before or after them (never across a 16-byte boundary).
+ *   j_dev / f_dev      DEVICE float64 [n_frames].
+ *   counts_dev         DEVICE int64 [n_frames][6] or NULL: |P & G|, |P | G|, n_P, n_G, m_P, m_G of each frame.
+ * Asynchronous on `stream`, with no host synchronisation.  BT_ERR_INVALID_ARG for a NULL input or output, sizes < 1, bound_th outside
+ * (0, 1), r > 64, or a context without a successful bt_mask_reserve; BT_ERR_CAPACITY above the reserved sizes.  A refused call writes nothing.
+ * bt_mask_reserve: room for calls of up to max_frames frames of up to max_h x max_w.  One CTA holds a band of 64 rows of both masks plus
+ * r rows above and r + 1 below as bit rows, 16 B per 64 pixels of a row; the reserve refuses (BT_ERR_INVALID_ARG) sizes whose band at r = 64
+ * does not fit in the device's shared memory per block (on an H100, 227 KB: widths up to 4800, so 4K UHD, r = 36, fits).  24 B per frame
+ * and 64-row band on the device. */
+BT_API int bt_mask_reserve(bt_ctx* ctx, int max_frames, int max_h, int max_w);
+BT_API int bt_mask_metrics(bt_ctx* ctx, const uint8_t* pred_dev, const uint8_t* gt_dev, int n_frames, int h, int w, double bound_th,
+                           double* j_dev, double* f_dev, int64_t* counts_dev, void* stream);
+/* db_statistics of one sequence's per-frame J and F (host code, no GPU).  For X = J and then X = F: the mean, np.mean(X) (numpy's pairwise
+ * sum); the recall, mean(X > 0.5), strictly greater; the decay, mean(bin 0) - mean(bin 3), bin i = X[ids[i] .. ids[i + 1]] inclusive, with
+ * ids = round_half_even(linspace(1, n, 5) + 1e-10) - 1 and linspace's points i ((n - 1) / 4) + 1 for i < 4 and exactly n for i = 4.
+ * out[7] = J&F = (J mean + F mean) / 2, J mean, J recall, J decay, F mean, F recall, F decay (the toolkit's CSV order).  The library scores
+ * the frames it is given: the DAVIS semi-supervised protocol's leaving out of the first and last frames is the caller's.  BT_ERR_INVALID_ARG
+ * for a NULL pointer or n < 1. */
+BT_API int bt_mask_score(const double* j, const double* f, int n, double* out);
+
 /* ---- tracking overlays: the reference's LOG frames (Bundler::saveNewframeResult, Bundler.cpp:379-411) ---------------------------------
  * bt_voxel_downsample: PCL's VoxelGrid (Utils::downsamplePointCloud, Utils.cpp:134-140; pcl::VoxelGrid::applyFilter with every field
  * averaged and no minimum count) of n_clouds clouds in one call, float32 (DESIGN.md §3.10): the voxel bounds from each cloud's finite
