@@ -1,9 +1,10 @@
 """GPU parity tests of the fused frame front end (bt_frames_preprocess through the C-ABI) against the CPU restatement
 (oracle/frame_oracle.py) and the committed golden vectors of the reference's kernels (ref_frame_*.npz, and ref_live_frame.npz:
 the reference's outputs for a whole 640x480 frame, recorded on an H100 by scripts/make_golden_live.py and stored to within a
-small fraction of the tolerances below).  Tolerances: filtered depth 2e-6 m (a few float ulps at ~1 m; the reference build uses
-fast-math exp/division), normals 1e-3 (unit vectors from ~1e-3 m differences amplify depth ulps), both allowing a small
-fraction of pixels where a hard threshold (1 cm filter gate, 2 cm normal gate, 0.1 m validity) flips."""
+small fraction of the tolerances below).  Against the oracle, every pixel outside the float64 statement's taint mask is held to its
+own bound (frame_oracle.device_report, no fraction allowance).  Against the reference's recordings: filtered depth 2e-6 m (a few
+float ulps at ~1 m; the reference build uses fast-math exp/division), normals 1e-3, on every pixel: the pixels beyond those are
+counted and printed, and there are none (measured on an H100: 0 in each of the three recordings)."""
 import glob
 import os
 import zlib
@@ -45,15 +46,28 @@ def _run(fe, raws, K, dev, dp=None, want_xyz=True):
     return [d.cpu().numpy() for d in dout], [n.cpu().numpy() for n in nout], ([x.cpu().numpy() for x in xout] if want_xyz else None)
 
 
-def _check(d, n, x, rd, rn, rx, frac=2e-3):
+def _check64(d, n, x, raw, K, dp=None):
+    """Per pixel against preprocess64 (and, where subnormal filter weights feed a pixel, against the float32 restatement at 2e-6 / 3e-6
+    / 1e-3).  Tainted pixels are exempt, so their number is printed and held below 1 % of the valid pixels."""
+    rep = frame_oracle.device_report(d, x, n, frame_oracle.preprocess64(raw, K, dp), frame_oracle.preprocess(raw, K, dp))
+    print(f"tainted {rep['tainted']}, subnormal-weight {rep['subnormal']}, of {rep['valid']} valid; "
+          f"worst error / bound: depth {rep['depth_frac']:.3f} normal {rep['normal_frac']:.3f}")
+    assert not rep["failures"], "; ".join(rep["failures"])
+    assert rep["tainted"] <= 0.01 * rep["valid"]
+
+
+def _check_recorded(d, n, x, rd, rn, rx, raw, K, dp=None):
+    """Against the reference's recorded maps: no pixel beyond 2e-6 (depth), 3e-6 (points) or 1e-3 (normals).  Differing pixels are
+    printed with whether preprocess64 taints them, i.e. whether a float32 gate decision there may go either way."""
     bad_d = np.abs(d - rd) > 2e-6
-    assert bad_d.mean() <= frac, f"depth: {bad_d.mean():.2e} of the pixels differ by > 2e-6 (max {np.abs(d - rd).max():.2e})"
-    ok = ~bad_d
-    if x is not None:
-        assert np.abs(x[..., :3] - rx[..., :3])[ok].max() <= 3e-6
-        assert np.array_equal(x[..., 3][ok], (rd >= 0.1).astype(np.float32)[ok])
     bad_n = np.abs(n[..., :3] - rn[..., :3]).max(-1) > 1e-3
-    assert bad_n.mean() <= 2 * frac, f"normals: {bad_n.mean():.2e} of the pixels differ by > 1e-3"
+    taint = frame_oracle.preprocess64(raw, K, dp).taint
+    print(f"pixels differing from the reference: depth {int(bad_d.sum())}, normals {int(bad_n.sum())} (tainted in float64: {int(taint.sum())})")
+    bad = bad_d | bad_n
+    assert not bad.any(), [(p, bool(taint[tuple(p)])) for p in np.argwhere(bad)[:10].tolist()]
+    if x is not None:
+        assert np.abs(x[..., :3] - rx[..., :3]).max() <= 3e-6
+        assert np.array_equal(x[..., 3], (rd >= 0.1).astype(np.float32))
     assert np.all(n[..., 3] == 0)
 
 
@@ -61,8 +75,7 @@ def _check(d, n, x, rd, rn, rx, frac=2e-3):
 def test_matches_oracle(fe, cuda_device, seed, H, W):
     raw, K = synth.make_raw_depth(seed, H, W)
     d, n, x = _run(fe, [raw], K, cuda_device)
-    rd, rx, rn = frame_oracle.preprocess(raw, K)
-    _check(d[0], n[0], x[0], rd, rn, rx)
+    _check64(d[0], n[0], x[0], raw, K)
     assert (d[0] > 0).sum() > 0.02 * H * W          # the filter fills small holes and keeps the object
 
 
@@ -74,8 +87,7 @@ def test_other_parameters_and_batch(fe, cuda_device):
         raws.append(r)
     d, n, x = _run(fe, raws, K, cuda_device, dp)
     for i, r in enumerate(raws):
-        rd, rx, rn = frame_oracle.preprocess(r, K, dp)
-        _check(d[i], n[i], x[i], rd, rn, rx)
+        _check64(d[i], n[i], x[i], r, K, dp)
     # a batch equals the same frames one at a time, bit for bit; xyz is optional
     d1, n1, _ = _run(fe, [raws[1]], K, cuda_device, dp, want_xyz=False)
     assert np.array_equal(d1[0], d[1]) and np.array_equal(n1[0], n[1])
@@ -116,7 +128,7 @@ def test_golden_reference_kernels(fe, cuda_device, path):
     d, n, x = _run(fe, [g["raw"]], tuple(g["K"]), cuda_device, dp)
     rn = np.concatenate([g["normal"], np.zeros(g["normal"].shape[:2] + (1,), np.float32)], -1)
     rx = np.concatenate([g["xyz"], (g["depth"] >= 0.1).astype(np.float32)[..., None]], -1)
-    _check(d[0], n[0], x[0], g["depth"], rn, rx)
+    _check_recorded(d[0], n[0], x[0], g["depth"], rn, rx, g["raw"], tuple(g["K"]), dp)
 
 
 # (name, quantisation step): at most half a step from the reference, i.e. <= 6 % of the depth / point tolerance and < 1 % of the normal one
@@ -155,7 +167,7 @@ def test_matches_reference_kernels_live(fe, cuda_device):
     raw, K = synth.make_raw_depth(7, 480, 640)
     rd, rx, rn = frame_decode(raw, K, g)
     d, n, x = _run(fe, [raw], K, cuda_device)
-    _check(d[0], n[0], x[0], rd, rn, rx)
+    _check_recorded(d[0], n[0], x[0], rd, rn, rx, raw, K)
 
 
 def test_feeds_the_solver(fe, cuda_device):
