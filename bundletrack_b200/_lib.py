@@ -288,6 +288,7 @@ PROTOTYPES = {
     "bt_surface_score": (_i, (_p, _i, _p, _i, _p, _i, _p)),
     "bt_mask_reserve": (_i, (_p, _i, _i, _i)),
     "bt_mask_metrics": (_i, (_p, _p, _p, _i, _i, _i, _d, _p, _p, _p, _p)),
+    "bt_mask_metrics_objects": (_i, (_p, _p, _p, _i, _i, _i, _i, _i, _d, _p, _p, _p, _p)),
     "bt_mask_score": (_i, (_p, _p, _i, _p)),
     "bt_voxel_downsample": (_i, (_p, _i, _p, _p, _f, _p, _p, _p)),
     "bt_overlay_reserve": (_i, (_p, _i, _i)),
@@ -314,6 +315,7 @@ PROTOTYPES = {
     "bt_vos_load_weights": (_i, (_p, _p, _sz)),
     "bt_vos_begin": (_i, (_p, _p, _p, _p, _p)),
     "bt_vos_next": (_i, (_p, _p, _p, _p)),
+    "bt_vos_labels": (_i, (_p, _p, _p)),
     "bt_vos_enable_timing": (_i, (_p, _i)),
     "bt_vos_get_timing": (_i, (_p, _p)),
     "bt_vos_debug": (_i, (_p, _i, _p, _p, _p, _p, _p)),

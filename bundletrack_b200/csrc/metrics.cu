@@ -910,20 +910,57 @@ __host__ __device__ __forceinline__ int mask_words(int w) { return (w + 63) / 64
 // shared bit rows of one mask for a band: at most the band, r rows above and r + 1 below
 __host__ __device__ __forceinline__ int mask_rows(int h, int r) { return min(kMaskBand + 2 * r + 1, h); }
 
-// bit j set when byte j of x is not 0: __vcmpne4 gives 0xff per such byte, and the multiply gathers the bytes' low bits into bits 28..31
-__device__ __forceinline__ unsigned nonzero4(unsigned x) { return ((__vcmpne4(x, 0u) & 0x01010101u) * 0x10204080u) >> 28; }
+// bit j set when byte j of x is 0xff (the byte compares of __vcmp*4): the multiply gathers the bytes' low bits into bits 28..31
+__device__ __forceinline__ unsigned bytes4(unsigned m) { return ((m & 0x01010101u) * 0x10204080u) >> 28; }
+__device__ __forceinline__ unsigned nonzero4(unsigned x) { return bytes4(__vcmpne4(x, 0u)); }
 __device__ __forceinline__ unsigned nonzero16(uint4 v) { return nonzero4(v.x) | nonzero4(v.y) << 4 | nonzero4(v.z) << 8 | nonzero4(v.w) << 12; }
+// bit j set when byte j of v equals the byte that k4 holds four times (ne: does not equal it)
+__device__ __forceinline__ unsigned equal16(uint4 v, unsigned k4) {
+	return bytes4(__vcmpeq4(v.x, k4)) | bytes4(__vcmpeq4(v.y, k4)) << 4 | bytes4(__vcmpeq4(v.z, k4)) << 8 | bytes4(__vcmpeq4(v.w, k4)) << 12;
+}
+__device__ __forceinline__ unsigned differ16(uint4 v, unsigned k4) { return ~equal16(v, k4) & 0xffffu; }
+
+// How pack_row turns block b of a row (16 bytes, aligned) into 16 bits, bit j for byte j.
+// The binary masks: the byte is not 0.
+struct NonZeroBits {
+	__device__ __forceinline__ unsigned operator()(const uint4* blk, int b) const { return nonzero16(__ldg(blk + b)); }
+};
+// Object k of a label map: the byte equals k (k4 = k times 0x01010101).  With gt set, also the ground-truth byte of the same pixel is not
+// the void value: byte j of block b is pixel 16 b + j - d of the row, and that pixel is byte s + j of the ground-truth row's blocks gb, gb + 1
+// with gb = b + q, where q (0 or -1) and s (0..15) come from the two rows' offsets in their first blocks.  Only blocks that hold a pixel of
+// the ground-truth row are read; a pixel of the row always lies in one.
+struct ObjectBits {
+	unsigned k4, void4;
+	const uint4* gt;                 // the ground-truth row's first block, or NULL: no void
+	int q, s, n_gt;                  // n_gt: the blocks that hold a pixel of the ground-truth row
+	__device__ __forceinline__ unsigned operator()(const uint4* blk, int b) const {
+		unsigned m = equal16(__ldg(blk + b), k4);
+		if (gt) {
+			const int gb = b + q;
+			const unsigned lo = gb >= 0 && gb < n_gt ? differ16(__ldg(gt + gb), void4) : 0u;
+			const unsigned hi = s && gb + 1 < n_gt ? differ16(__ldg(gt + gb + 1), void4) : 0u;
+			m &= (lo | hi << 16) >> s;
+		}
+		return m;
+	}
+};
+
+__device__ __forceinline__ const uint4* first_block(const uint8_t* src) {
+	return reinterpret_cast<const uint4*>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)15);
+}
 
 // One warp packs row `src` (w bytes at any alignment) into dst[0, nw): it reads the whole 16-byte blocks that hold a pixel of the row, one
-// per lane, and word c takes the 64 bits that start d = src & 15 bits into blocks 4c .. 4c + 4.  Bits past the row's end are 0.
-__device__ void pack_row(const uint8_t* src, int w, u64* dst, int nw, int lane) {
-	const uint4* blk = reinterpret_cast<const uint4*>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)15);
+// per lane, turns each into 16 bits with `bits`, and word c takes the 64 bits that start d = src & 15 bits into blocks 4c .. 4c + 4.  Bits
+// past the row's end are 0.
+template <class Bits>
+__device__ void pack_row(const uint8_t* src, int w, u64* dst, int nw, int lane, const Bits& bits) {
+	const uint4* blk = first_block(src);
 	const int d = (int)(reinterpret_cast<uintptr_t>(src) & 15);
 	const int n_blk = (d + w + 15) >> 4;
 	for (int c0 = 0; c0 < nw; c0 += 8) {                // 8 words, 32 blocks (plus the next round's first) per round
 		const int k = 4 * c0 + lane;
-		const unsigned m = k < n_blk ? nonzero16(__ldg(blk + k)) : 0u;
-		const unsigned next = (lane == 31 && k + 1 < n_blk) ? nonzero16(__ldg(blk + k + 1)) : 0u;
+		const unsigned m = k < n_blk ? bits(blk, k) : 0u;
+		const unsigned next = (lane == 31 && k + 1 < n_blk) ? bits(blk, k + 1) : 0u;
 		const int i = lane & 7;
 		const u64 m0 = __shfl_sync(0xffffffffu, m, 4 * i), m1 = __shfl_sync(0xffffffffu, m, 4 * i + 1);
 		const u64 m2 = __shfl_sync(0xffffffffu, m, 4 * i + 2), m3 = __shfl_sync(0xffffffffu, m, 4 * i + 3);
@@ -966,13 +1003,42 @@ __device__ __forceinline__ int isqrt(int n) {
 	return v;
 }
 
-// grid (n_frames, n_bands): block (f, band) writes band_counts[f][band][0..5] for rows [y0, y0 + kMaskBand) of frame f
+// Which masks a k_mask_band row scores.  frame(x): the frame of grid row x; pack(): one warp packs row y of that frame's prediction
+// (map 0) or ground truth (map 1), given both rows.
+// bt_mask_metrics: row x is frame x, foreground is non-zero.
+struct BinaryMasks {
+	__device__ __forceinline__ int frame(int x) const { return x; }
+	__device__ __forceinline__ void pack(int map, int, const uint8_t* p, const uint8_t* g, int w, u64* dst, int nw, int lane) const {
+		pack_row(map ? g : p, w, dst, nw, lane, NonZeroBits());
+	}
+};
+// bt_mask_metrics_objects: row x is object k = x % n_objects + 1 of frame x / n_objects; P = (pred == k) & ~V, G = (gt == k), which
+// excludes V = (gt == void_value) since void_value is not an object id.
+struct ObjectMasks {
+	int n_objects, void_value;       // -1: no void
+	__device__ __forceinline__ int frame(int x) const { return x / n_objects; }
+	__device__ __forceinline__ void pack(int map, int x, const uint8_t* p, const uint8_t* g, int w, u64* dst, int nw, int lane) const {
+		ObjectBits bits = {(unsigned)(x % n_objects + 1) * 0x01010101u, (unsigned)void_value * 0x01010101u, nullptr, 0, 0, 0};
+		if (map == 0 && void_value >= 0) {
+			const int e = (int)(reinterpret_cast<uintptr_t>(g) & 15) - (int)(reinterpret_cast<uintptr_t>(p) & 15);
+			bits.gt = first_block(g);
+			bits.q = e >> 4;
+			bits.s = e & 15;
+			bits.n_gt = ((int)(reinterpret_cast<uintptr_t>(g) & 15) + w + 15) >> 4;
+		}
+		pack_row(map ? g : p, w, dst, nw, lane, bits);
+	}
+};
+
+// grid (rows, n_bands): block (x, band) writes band_counts[x][band][0..5] for rows [y0, y0 + kMaskBand) of grid row x (Select::frame)
+template <class Select>
 __global__ void __launch_bounds__(kMaskThreads) k_mask_band(const uint8_t* __restrict__ pred, const uint8_t* __restrict__ gt, int h, int w, int r,
-                                                            unsigned* __restrict__ band_counts) {
+                                                            unsigned* __restrict__ band_counts, Select sel) {
 	extern __shared__ u64 s_bits[];                    // [2][n_rows][nw]: the prediction's rows, then the ground truth's
 	__shared__ int s_h[2 * kMaxMaskRadius + 1];        // s_h[dy + r] = isqrt(r^2 - dy^2): the disk's half-width on row dy
 	__shared__ unsigned s_cnt[kMaskCounts];
 	const int f = blockIdx.x, band = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const size_t frame = (size_t)sel.frame(f);
 	const int nw = mask_words(w);
 	const int y0 = band * kMaskBand, y1 = min(y0 + kMaskBand, h);
 	const int ylo = max(0, y0 - r), yhi = min(h, y1 + r + 1);        // the rows held
@@ -982,8 +1048,8 @@ __global__ void __launch_bounds__(kMaskThreads) k_mask_band(const uint8_t* __res
 
 	for (int t = warp; t < 2 * n_rows; t += kMaskThreads / 32) {
 		const int map = t & 1, row = t >> 1;
-		const uint8_t* src = (map ? gt : pred) + ((size_t)f * h + ylo + row) * (size_t)w;
-		pack_row(src, w, s_bits + ((size_t)map * n_rows + row) * nw, nw, lane);
+		const size_t at = (frame * h + ylo + row) * (size_t)w;
+		sel.pack(map, f, pred + at, gt + at, w, s_bits + ((size_t)map * n_rows + row) * nw, nw, lane);
 	}
 	__syncthreads();
 
@@ -1052,7 +1118,7 @@ __global__ void __launch_bounds__(kMaskThreads) k_mask_band(const uint8_t* __res
 	if (tid < kMaskCounts) band_counts[((size_t)f * gridDim.y + band) * kMaskCounts + tid] = s_cnt[tid];
 }
 
-// one thread per frame: the bands' counts in band order, then J and F in float64
+// one thread per grid row of k_mask_band: the bands' counts in band order, then J and F in float64
 __global__ void k_mask_final(const unsigned* __restrict__ band_counts, int n_bands, int n_frames, double* __restrict__ j_out,
                              double* __restrict__ f_out, long long* __restrict__ counts_out) {
 	const int f = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1095,17 +1161,19 @@ extern "C" int bt_mask_reserve(bt_ctx* ctx, int max_frames, int max_h, int max_w
 	BT_REQUIRE(max_bands <= kMaxMaskBands, BT_ERR_INVALID_ARG, "bt_mask_reserve: max_h %d > %d", max_h, kMaxMaskBands * kMaskBand);
 	BT_CUDA(cudaSetDevice(ctx->device));
 	int optin = 0;
-	cudaFuncAttributes fa;
+	cudaFuncAttributes fa, fo;
 	BT_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
-	BT_CUDA(cudaFuncGetAttributes(&fa, k_mask_band));
-	const size_t smem = mask_smem(max_h, max_w, kMaxMaskRadius), room = (size_t)optin - fa.sharedSizeBytes;
+	BT_CUDA(cudaFuncGetAttributes(&fa, k_mask_band<BinaryMasks>));
+	BT_CUDA(cudaFuncGetAttributes(&fo, k_mask_band<ObjectMasks>));
+	const size_t smem = mask_smem(max_h, max_w, kMaxMaskRadius), room = (size_t)optin - std::max(fa.sharedSizeBytes, fo.sharedSizeBytes);
 	BT_REQUIRE(smem <= room, BT_ERR_INVALID_ARG,
 	           "bt_mask_reserve: a band of %d x %d masks needs %zu bytes of shared memory at r = %d, the device has %zu per block", max_h, max_w, smem,
 	           kMaxMaskRadius, room);
 	MaskState* s;
 	BT_TRY(take_state(ctx, &bt_ctx::mask, &s));
 	// the kernel's limit is the device's, not this reservation's: it is one setting for every context in the process
-	BT_CUDA(cudaFuncSetAttribute(k_mask_band, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)room));
+	BT_CUDA(cudaFuncSetAttribute(k_mask_band<BinaryMasks>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)room));
+	BT_CUDA(cudaFuncSetAttribute(k_mask_band<ObjectMasks>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)room));
 	BT_TRY(s->band.alloc(sizeof(unsigned) * kMaskCounts * (size_t)max_bands * (size_t)max_frames));
 	s->max_frames = max_frames; s->max_h = max_h; s->max_w = max_w;
 	s->ready = true;
@@ -1128,8 +1196,37 @@ extern "C" int bt_mask_metrics(bt_ctx* ctx, const uint8_t* pred_dev, const uint8
 	cudaStream_t stream = (cudaStream_t)stream_;
 	const int n_bands = (h + kMaskBand - 1) / kMaskBand;
 	unsigned* band = s->band.as<unsigned>();
-	k_mask_band<<<dim3(n_frames, n_bands), kMaskThreads, mask_smem(h, w, r), stream>>>(pred_dev, gt_dev, h, w, r, band);
+	k_mask_band<<<dim3(n_frames, n_bands), kMaskThreads, mask_smem(h, w, r), stream>>>(pred_dev, gt_dev, h, w, r, band, BinaryMasks());
 	k_mask_final<<<(n_frames + 127) / 128, 128, 0, stream>>>(band, n_bands, n_frames, j_dev, f_dev, reinterpret_cast<long long*>(counts_dev));
+	BT_CUDA(cudaGetLastError());
+	return BT_OK;
+}
+
+extern "C" int bt_mask_metrics_objects(bt_ctx* ctx, const uint8_t* pred_dev, const uint8_t* gt_dev, int n_frames, int h, int w, int n_objects,
+                                       int void_value, double bound_th, double* j_dev, double* f_dev, int64_t* counts_dev, void* stream_) {
+	BT_REQUIRE(pred_dev && gt_dev && j_dev && f_dev, BT_ERR_INVALID_ARG, "bt_mask_metrics_objects: NULL argument");
+	BT_REQUIRE(n_frames >= 1 && h >= 1 && w >= 1, BT_ERR_INVALID_ARG, "bt_mask_metrics_objects: n_frames %d / h %d / w %d must be >= 1", n_frames,
+	           h, w);
+	BT_REQUIRE(n_objects >= 1 && n_objects <= 255, BT_ERR_INVALID_ARG, "bt_mask_metrics_objects: n_objects %d outside [1, 255]", n_objects);
+	BT_REQUIRE(void_value == -1 || (void_value >= 0 && void_value <= 255 && !(void_value >= 1 && void_value <= n_objects)), BT_ERR_INVALID_ARG,
+	           "bt_mask_metrics_objects: void_value %d must be -1 (no void) or in [0, 255] outside the object ids 1..%d", void_value, n_objects);
+	BT_REQUIRE(bound_th > 0.0 && bound_th < 1.0, BT_ERR_INVALID_ARG, "bt_mask_metrics_objects: bound_th %g must be in (0, 1)", bound_th);
+	const double rr = ceil(bound_th * sqrt((double)h * h + (double)w * w));
+	BT_REQUIRE(rr <= kMaxMaskRadius, BT_ERR_INVALID_ARG, "bt_mask_metrics_objects: the tolerance radius %.0f of bound_th %g at %d x %d exceeds %d", rr,
+	           bound_th, h, w, kMaxMaskRadius);
+	const int r = (int)rr;
+	MaskState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::mask, "bt_mask_metrics_objects", "bt_mask_reserve", &s));
+	const long long rows = (long long)n_frames * n_objects;
+	BT_REQUIRE(rows <= s->max_frames && h <= s->max_h && w <= s->max_w, BT_ERR_CAPACITY,
+	           "bt_mask_metrics_objects: %d frames x %d objects = %lld rows of %d x %d exceed the reserved %d of %d x %d", n_frames, n_objects, rows, h, w,
+	           s->max_frames, s->max_h, s->max_w);
+	cudaStream_t stream = (cudaStream_t)stream_;
+	const int n_bands = (h + kMaskBand - 1) / kMaskBand;
+	unsigned* band = s->band.as<unsigned>();
+	k_mask_band<<<dim3((unsigned)rows, n_bands), kMaskThreads, mask_smem(h, w, r), stream>>>(pred_dev, gt_dev, h, w, r, band,
+	                                                                                          ObjectMasks{n_objects, void_value});
+	k_mask_final<<<(unsigned)((rows + 127) / 128), 128, 0, stream>>>(band, n_bands, (int)rows, j_dev, f_dev, reinterpret_cast<long long*>(counts_dev));
 	BT_CUDA(cudaGetLastError());
 	return BT_OK;
 }

@@ -10,7 +10,8 @@
 //                    the unweighted exponential sum and one spatially weighted numerator per label.  S is never stored.
 //   k_vos_merge      combines the per-reference partial softmax states into the low-resolution prediction, and writes the one-hot of its
 //                    argmax into the history ring
-//   k_vos_mask       bilinear upsample of the prediction to full resolution, argmax, uint8 0 / 255
+//   k_vos_mask       bilinear upsample of the prediction to full resolution, argmax, one output byte per channel: 0 / 255 for the mask,
+//                    the initial mask's values for the label map
 //
 // 3xTF32: each FP32 operand x is split into hi = tf32(x) and lo = tf32(x - hi); a product is accumulated as lo.hi + hi.lo + hi.hi in
 // FP32 (the lo.lo term is below FP32's rounding).  The MMA is the warp-level mma.sync.m16n8k8.tf32.
@@ -420,7 +421,11 @@ __device__ __forceinline__ void lin_src(int dst, float scale, int in, int& i0, i
 	l0 = 1.f - l1;
 }
 
-__global__ void k_vos_mask(const float* __restrict__ pred, int Hd, int Wd, int d, uint8_t* __restrict__ mask, int H, int W) {
+// the byte k_vos_mask writes for each label channel
+struct ChanBytes { uint8_t v[MAX_LABELS]; };
+constexpr ChanBytes kMaskBytes = {{0, 255, 255, 255, 255, 255, 255, 255}};
+
+__global__ void k_vos_mask(const float* __restrict__ pred, int Hd, int Wd, int d, ChanBytes out, uint8_t* __restrict__ mask, int H, int W) {
 	const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
 	if (x >= W) return;
 	int y0, y1, x0, x1;
@@ -435,7 +440,7 @@ __global__ void k_vos_mask(const float* __restrict__ pred, int Hd, int Wd, int d
 		const float v = ly0 * (lx0 * p[y0 * Wd + x0] + lx1 * p[y0 * Wd + x1]) + ly1 * (lx0 * p[y1 * Wd + x0] + lx1 * p[y1 * Wd + x1]);
 		if (c == 0 || v > bv) { bv = v; best = c; }
 	}
-	mask[(size_t)y * W + x] = best > 0 ? 255 : 0;
+	mask[(size_t)y * W + x] = out.v[best];
 }
 
 // frame 0: which of the 256 values the initial mask holds
@@ -512,8 +517,9 @@ struct VosState {
 	bool loaded = false;
 	int frame = -1;                 // frames seen since bt_vos_begin; -1 before it
 	int n_labels = 0;
+	ChanBytes values = {};          // label channel -> the initial mask's value
 	Net net = {};
-	DevBuf w, act[5], feat, label, part, pred, chan;
+	DevBuf w, act[5], feat, label, part, pred, chan, init;       // init: the initial mask, bt_vos_labels' output for frame 0
 	PinnedBuf present;
 	bool timing = false;
 	Event ev[N_STAGES + 1];
@@ -615,6 +621,7 @@ extern "C" int bt_vos_reserve(bt_ctx* ctx, const bt_vos_params* p, int H, int W)
 	BT_TRY(s->part.alloc(sizeof(float) * p->ref_num * HW * (2 + MAX_LABELS)));
 	BT_TRY(s->pred.alloc(sizeof(float) * MAX_LABELS * HW));
 	BT_TRY(s->chan.alloc(sizeof(int32_t) * 512));
+	BT_TRY(s->init.alloc((size_t)H * W));
 	BT_TRY(s->present.alloc(sizeof(int32_t) * 256));
 	BT_CUDA(cudaFuncSetAttribute(k_vos_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CB_SMEM));
 	BT_CUDA(cudaFuncSetAttribute(k_vos_propagate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PB_SMEM));
@@ -654,7 +661,11 @@ extern "C" int bt_vos_begin(bt_ctx* ctx, const uint8_t* colour_dev, const uint8_
 	int distinct = 0, d = 1;
 	for (int v = 0; v < 256; v++) distinct += present[v] != 0;
 	int32_t* chan = present;        // rewritten in place as the value -> channel map
-	for (int v = 0; v < 256; v++) chan[v] = v == 0 ? 0 : (present[v] ? d++ : 0);
+	ChanBytes values = {};
+	for (int v = 0; v < 256; v++) {
+		if (v > 0 && present[v] && d < MAX_LABELS) values.v[d] = (uint8_t)v;
+		chan[v] = v == 0 ? 0 : (present[v] ? d++ : 0);
+	}
 	BT_REQUIRE(d <= MAX_LABELS, BT_ERR_INVALID_ARG, "bt_vos_begin: the initial mask has %d distinct values (%d label channels with channel 0); at most %d channels are supported",
 	           distinct, d, MAX_LABELS);
 	BT_CUDA(cudaMemcpyAsync(s->chan.as<int32_t>() + 256, chan, sizeof(int32_t) * 256, cudaMemcpyHostToDevice, st));
@@ -668,9 +679,11 @@ extern "C" int bt_vos_begin(bt_ctx* ctx, const uint8_t* colour_dev, const uint8_
 	k_vos_binarise<<<(n + 255) / 256, 256, 0, st>>>(init_mask_dev, n, mask_out_dev);
 	BT_CUDA(cudaGetLastError());
 	BT_TRY(mark(3));
+	BT_CUDA(cudaMemcpyAsync(s->init.p, init_mask_dev, (size_t)n, cudaMemcpyDeviceToDevice, st));
 	// the chan upload reads the pinned block: wait for it before a later begin rewrites it
 	BT_CUDA(cudaStreamSynchronize(st));
 	s->n_labels = d;
+	s->values = values;
 	s->frame = 0;
 	s->timed = s->timing;
 	return BT_OK;
@@ -708,11 +721,27 @@ extern "C" int bt_vos_next(bt_ctx* ctx, const uint8_t* colour_dev, uint8_t* mask
 	                                               s->label.as<float>() + (size_t)slot * HW * MAX_LABELS);
 	BT_CUDA(cudaGetLastError());
 	BT_TRY(mark(2));
-	k_vos_mask<<<dim3((s->W + 127) / 128, s->H), 128, 0, st>>>(s->pred.as<float>(), s->Hd, s->Wd, s->n_labels, mask_out_dev, s->H, s->W);
+	k_vos_mask<<<dim3((s->W + 127) / 128, s->H), 128, 0, st>>>(s->pred.as<float>(), s->Hd, s->Wd, s->n_labels, kMaskBytes, mask_out_dev, s->H, s->W);
 	BT_CUDA(cudaGetLastError());
 	BT_TRY(mark(3));
 	s->frame = k;
 	s->timed = s->timing;
+	return BT_OK;
+}
+
+extern "C" int bt_vos_labels(bt_ctx* ctx, uint8_t* labels_out_dev, void* stream_) {
+	VosState* s;
+	BT_TRY(state_of(ctx, &bt_ctx::vos, "bt_vos_labels", "bt_vos_reserve", &s));
+	BT_REQUIRE(s->frame >= 0, BT_ERR_INVALID_ARG, "bt_vos_labels: no sequence begun (bt_vos_begin)");
+	BT_REQUIRE(labels_out_dev, BT_ERR_INVALID_ARG, "bt_vos_labels: NULL pointer");
+	cudaStream_t st = (cudaStream_t)stream_;
+	if (s->frame == 0) {
+		BT_CUDA(cudaMemcpyAsync(labels_out_dev, s->init.p, (size_t)s->H * s->W, cudaMemcpyDeviceToDevice, st));
+		return BT_OK;
+	}
+	// the same upsample and argmax as bt_vos_next's mask, with each channel's value in place of 255
+	k_vos_mask<<<dim3((s->W + 127) / 128, s->H), 128, 0, st>>>(s->pred.as<float>(), s->Hd, s->Wd, s->n_labels, s->values, labels_out_dev, s->H, s->W);
+	BT_CUDA(cudaGetLastError());
 	return BT_OK;
 }
 

@@ -271,3 +271,33 @@ class MaskScore(_lib.Facade):
         _lib.check(self.lib.bt_stream_sync(self.stream), "bt_stream_sync")
         out = (j.cpu().numpy(), f.cpu().numpy())
         return out + (c.cpu().numpy(),) if counts else out
+
+    def objects(self, pred, gt, n_objects: int, void_value: int = 255, bound_th: float = 0.008, counts: bool = False):
+        """(j, f), float64 numpy [F, n_objects], of label maps (uint8 [F, H, W] object ids, numpy or CUDA): object k of frame i at [i, k - 1],
+        scored on P = (pred == k) and G = (gt == k) with the pixels where gt == void_value removed from both (void_value -1: none), DAVIS
+        2017's db_eval_iou / f_measure with void_pixels (bt_mask_metrics_objects).  counts=True also gives the int64 [F, n_objects, 6] counts.
+        Each (frame, object) pair takes one of the max_frames reserved rows, so calls hold max_frames // n_objects frames."""
+        import torch
+        P, G = self._frames(pred, "pred"), self._frames(gt, "gt")
+        if P.shape != G.shape:
+            raise ValueError(f"pred {list(P.shape)} and gt {list(G.shape)} differ")
+        n, h, w = P.shape
+        k = int(n_objects)
+        step = self.max_frames // k
+        if step < 1:
+            raise ValueError(f"{k} objects need {k} reserved rows per frame; max_frames is {self.max_frames}")
+        dev = torch.device("cuda", self.device)
+        j = torch.empty((n, k), dtype=torch.float64, device=dev)
+        f = torch.empty((n, k), dtype=torch.float64, device=dev)
+        c = torch.empty((n, k, 6), dtype=torch.int64, device=dev) if counts else None
+        held = []
+        for s in range(0, n, step):
+            e = min(n, s + step)
+            p, g = P[s:e].to(dev).contiguous(), G[s:e].to(dev).contiguous()
+            held += [p, g]
+            _lib.check(self.lib.bt_mask_metrics_objects(self.ctx, _lib.ptr(p), _lib.ptr(g), e - s, h, w, k, int(void_value), float(bound_th),
+                                                        _lib.ptr(j[s:]), _lib.ptr(f[s:]), _lib.ptr(c[s:]) if counts else None, self.stream),
+                       "bt_mask_metrics_objects")
+        _lib.check(self.lib.bt_stream_sync(self.stream), "bt_stream_sync")
+        out = (j.cpu().numpy(), f.cpu().numpy())
+        return out + (c.cpu().numpy(),) if counts else out

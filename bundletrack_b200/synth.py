@@ -355,6 +355,37 @@ def ragged_ellipse_masks(n_frames: int, H: int = 480, W: int = 640, seed: int = 
     return out[0], out[1]
 
 
+def ragged_label_maps(n_frames: int, H: int = 480, W: int = 854, n_objects: int = 3, void_from: int | None = None, seed: int = 0):
+    """(pred, gt): uint8 [n_frames, H, W] DAVIS-style label maps of n_objects ragged ellipses, object k painted with id k over background 0
+    in increasing k, each moving on a path of its own.  The prediction's ellipses are displaced by up to about 2 % of the frame with outlines
+    of their own per frame.  From frame void_from on (None: never) the ground truth also holds the void value 255 on a band about 3 pixels
+    wide along each object's outline, as DAVIS annotations do.  For the per-object mask scores' tests and benchmark."""
+    rng = np.random.default_rng(np.uint64(0x0B1EC7) + np.uint64(seed))
+    y, x = np.mgrid[0:H, 0:W].astype(np.float32)
+    k6 = np.arange(3, 9, dtype=np.float32)
+    out = np.zeros((2, n_frames, H, W), np.uint8)
+    for obj in range(1, n_objects + 1):
+        c0 = rng.uniform(0.2, 0.8, 2) * (W, H)
+        vel = rng.uniform(-0.15, 0.15, 2) * (W, H)
+        ax, ay = rng.uniform(0.06, 0.2) * W, rng.uniform(0.06, 0.2) * H
+        amp_g, ph_g = rng.uniform(0.01, 0.04, 6).astype(np.float32), rng.uniform(0, 2 * np.pi, 6).astype(np.float32)
+        for f in range(n_frames):
+            t = f / max(n_frames - 1, 1)
+            cx, cy = c0 + vel * t
+            th = np.float32(np.pi * t * (0.5 + 0.1 * obj))
+            d = 0.02 * rng.uniform(-1, 1, 2) * (W, H)
+            amp_p, ph_p = rng.uniform(0.01, 0.04, 6).astype(np.float32), rng.uniform(0, 2 * np.pi, 6).astype(np.float32)
+            for m, (ox, oy, amp, ph) in enumerate(((d[0], d[1], amp_p, ph_p), (0.0, 0.0, amp_g, ph_g))):
+                u, v = x - np.float32(cx + ox), y - np.float32(cy + oy)
+                u, v = u * np.cos(th) + v * np.sin(th), v * np.cos(th) - u * np.sin(th)
+                rag = 1 + (amp[:, None, None] * np.cos(k6[:, None, None] * np.arctan2(v / ay, u / ax) + ph[:, None, None])).sum(0)
+                level = np.sqrt((u / ax) ** 2 + (v / ay) ** 2) / rag
+                out[m, f][level <= 1] = obj
+                if m == 1 and void_from is not None and f >= void_from:
+                    out[m, f][np.abs(level - 1) * min(ax, ay) < 1.5] = 255
+    return out[0], out[1]
+
+
 def make_ransac_case(seed: int, n: int, inlier_frac: float = 0.7, noise: float = 0.0005):
     """Model-frame point pairs as SiftManager::runRansacMultiPairGPU uploads them (/root/reference/src/FeatureManager.cpp:676-706):
     B = T A + noise for the inliers, the rest displaced by centimetres.  Returns (A [n,4], B [n,4] float32 with w = 1, inlier mask)."""

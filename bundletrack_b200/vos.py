@@ -1,7 +1,8 @@
 """Object masks on the device: transductive-vos.pytorch's run_video.py (resnet50) as library calls, no PyTorch network.
 
 load_vos(path, params) reads the checkpoint run_video.py --resume takes and returns a VosDevice: begin() takes frame 0 and its mask,
-next() propagates that mask to each later frame, and both write uint8 0 / 255 masks on the device.  DESIGN.md §3.13."""
+next() propagates that mask to each later frame, and both write uint8 0 / 255 masks on the device; labels() gives the last frame's label
+map, the initial mask's values per pixel.  DESIGN.md §3.13, §3.17."""
 from __future__ import annotations
 
 import ctypes
@@ -165,6 +166,15 @@ class VosDevice(_lib.Facade):
         _lib.check(self.lib.bt_vos_next(self.ctx, _lib.ptr(colour), _lib.ptr(out), st), "bt_vos_next")
         return out
 
+    def labels(self, out=None, stream=None):
+        """The label map (CUDA uint8 H x W) of the last frame begin() or next() processed, enqueued on `stream`: the initial mask's value of
+        each pixel's label channel, non-zero exactly where that frame's mask is 255; after begin(), the initial mask itself.  Call it before
+        the next next() in stream order, which overwrites what it reads (bt_vos_labels)."""
+        out = self._out(out)
+        st = self.stream if stream is None else ctypes.c_void_p(stream)
+        _lib.check(self.lib.bt_vos_labels(self.ctx, _lib.ptr(out), st), "bt_vos_labels")
+        return out
+
     def enable_timing(self, on: bool = True) -> None:
         _lib.check(self.lib.bt_vos_enable_timing(self.ctx, int(on)), "bt_vos_enable_timing")
 
@@ -204,6 +214,31 @@ def read_init_mask(path: str) -> np.ndarray:
     if m.dtype != np.uint8:
         raise ValueError(f"{path}: {m.dtype} samples; the initial mask's label values must be 8-bit (uint8)")
     return np.ascontiguousarray(m)
+
+
+def read_palette_mask(path: str) -> tuple:
+    """(indices, palette) of a DAVIS annotation as lib/predict.py's prepare_first_frame reads it: PIL's palette indices (uint8 H x W) and the
+    palette (uint8 [n, 3], None for an 8-bit grey PNG, whose samples are taken as indices).  Any other PNG mode is refused by name."""
+    from PIL import Image
+    with Image.open(path) as im:
+        if im.mode not in ("P", "L"):
+            raise ValueError(f"{path}: a mode {im.mode!r} image; object annotations must be palette (P) or 8-bit grey (L) PNGs")
+        a = np.array(im, dtype=np.uint8)
+        pal = im.getpalette() if im.mode == "P" else None
+    if pal is not None:
+        pal = np.asarray(pal, np.uint8).reshape(-1, 3)
+    return np.ascontiguousarray(a), pal
+
+
+def write_palette_mask(path: str, labels, palette) -> None:
+    """lib/utils.py's save_prediction: labels (uint8 H x W) as a mode P PNG with `palette` (uint8 [n, 3] or a flat list of RGB bytes)."""
+    from PIL import Image
+    a = np.asarray(labels)
+    if a.dtype != np.uint8 or a.ndim != 2:
+        raise ValueError(f"{path}: labels must be uint8 H x W, got {a.dtype} {a.shape}")
+    im = Image.fromarray(np.ascontiguousarray(a)).convert("L")
+    im.putpalette(np.asarray(palette, np.uint8).reshape(-1).tolist())      # an L image with a palette becomes mode P, indices kept
+    im.convert("P").save(path)
 
 
 class MaskWriter:

@@ -659,6 +659,21 @@ BT_API int bt_surface_score(const double* d_ab, int n_a, const double* d_ba, int
 BT_API int bt_mask_reserve(bt_ctx* ctx, int max_frames, int max_h, int max_w);
 BT_API int bt_mask_metrics(bt_ctx* ctx, const uint8_t* pred_dev, const uint8_t* gt_dev, int n_frames, int h, int w, double bound_th,
                            double* j_dev, double* f_dev, int64_t* counts_dev, void* stream);
+/* Per-object mask accuracy of label maps with void pixels (DESIGN.md §3.17), DAVIS 2017's multi-object scoring: the toolkit's db_eval_iou and
+ * f_measure with void_pixels.  pred and gt hold object ids per pixel (0 is background).  For object k in 1..n_objects of a frame pair:
+ *   V = (gt == void_value), the void pixels (none when void_value is -1);
+ *   P = (pred == k) & ~V and G = (gt == k) & ~V, so void is removed from both masks before the counts and before the boundary maps;
+ *   then the six counts, J and F of P and G exactly as bt_mask_metrics defines them above.  An object in neither mask has an empty union
+ *   and no boundary pixels, so J = 1 and F = 1.
+ * bt_mask_metrics_objects: J and F of every object of n_frames frame pairs.
+ *   pred_dev / gt_dev  DEVICE uint8 [n_frames][h][w] object ids, contiguous, any alignment; read as bt_mask_metrics reads its masks.
+ *   n_objects          1 to 255; void_value -1, or 0 to 255 and not in 1..n_objects.
+ *   j_dev / f_dev      DEVICE float64 [n_frames][n_objects], object k of frame i at i * n_objects + k - 1.
+ *   counts_dev         DEVICE int64 [n_frames][n_objects][6] or NULL, the counts of bt_mask_metrics per object.
+ * Each (frame, object) pair is one row of the reservation: n_frames * n_objects above bt_mask_reserve's max_frames is BT_ERR_CAPACITY.
+ * Asynchronous on `stream`; the other refusals are bt_mask_metrics's, and a refused call writes nothing. */
+BT_API int bt_mask_metrics_objects(bt_ctx* ctx, const uint8_t* pred_dev, const uint8_t* gt_dev, int n_frames, int h, int w, int n_objects,
+                                   int void_value, double bound_th, double* j_dev, double* f_dev, int64_t* counts_dev, void* stream);
 /* db_statistics of one sequence's per-frame J and F (host code, no GPU).  For X = J and then X = F: the mean, np.mean(X) (numpy's pairwise
  * sum); the recall, mean(X > 0.5), strictly greater; the decay, mean(bin 0) - mean(bin 3), bin i = X[ids[i] .. ids[i + 1]] inclusive, with
  * ids = round_half_even(linspace(1, n, 5) + 1e-10) - 1 and linspace's points i ((n - 1) / 4) + 1 for i < 4 and exactly n for i = 4.
@@ -854,6 +869,11 @@ BT_API int bt_lfnet_load_file(bt_ctx* ctx, const char* path, int max_images, bt_
  *   synchronises `stream`.
  * bt_vos_next: the next frame, asynchronous on `stream`: mask_out_dev DEVICE H x W uint8, 255 where the label is not channel 0.
  *   BT_ERR_INVALID_ARG before bt_vos_begin.  Both take frames of the reserved size.
+ * bt_vos_labels: the label map of the last frame bt_vos_begin or bt_vos_next processed, asynchronous on `stream`: labels_out_dev DEVICE
+ *   H x W uint8.  After bt_vos_next each pixel holds the initial mask's value of its label channel (the channel bt_vos_next's mask takes,
+ *   the first of equal maxima of the bilinearly upsampled prediction), so a pixel is non-zero exactly where that mask is 255.  After
+ *   bt_vos_begin it is the initial mask as given.  bt_vos_next overwrites the prediction this reads: call it before the next bt_vos_next
+ *   in stream order.  BT_ERR_INVALID_ARG before bt_vos_begin.
  * bt_vos_enable_timing / bt_vos_get_timing: device time of the last call, ms3 = {backbone, propagation, mask}; get_timing waits for it.
  * bt_vos_debug (test aid): ring slot `slot`'s features (Hd x Wd x 256 floats) and label (Hd x Wd x 8 floats), the last bt_vos_next's
  *   low-resolution prediction (8 x Hd x Wd floats, channels past the label count zero) and info5 = {frame index, label channels, ring
@@ -868,6 +888,7 @@ BT_API int bt_vos_reserve(bt_ctx* ctx, const bt_vos_params* params, int H, int W
 BT_API int bt_vos_load_weights(bt_ctx* ctx, const float* blob, size_t n_floats);
 BT_API int bt_vos_begin(bt_ctx* ctx, const uint8_t* colour_dev, const uint8_t* init_mask_dev, uint8_t* mask_out_dev, void* stream);
 BT_API int bt_vos_next(bt_ctx* ctx, const uint8_t* colour_dev, uint8_t* mask_out_dev, void* stream);
+BT_API int bt_vos_labels(bt_ctx* ctx, uint8_t* labels_out_dev, void* stream);
 BT_API int bt_vos_enable_timing(bt_ctx* ctx, int on);
 BT_API int bt_vos_get_timing(bt_ctx* ctx, float* ms3);
 BT_API int bt_vos_debug(bt_ctx* ctx, int slot, float* feat_host, float* label_host, float* pred_host, int32_t* info5, void* stream);

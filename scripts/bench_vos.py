@@ -4,6 +4,9 @@ GPU (cuDNN convolutions with TF32 allowed, an FP32 mm: torch's defaults) with it
 
     python scripts/bench_vos.py [--frames 60] [--warmup 10] [--H 480 --W 640]
 
+The per-frame window is also run with each frame's label map written after it (bt_vos_labels after every bt_vos_next, DESIGN.md §3.17),
+and bt_vos_labels is timed alone; python scripts/bench_vos.py --H 480 --W 854 measures them at DAVIS's 480p size.
+
 It also times run_sequence over a synthetic YCBInEOAT-layout scene (bundletrack_b200.synth, host feature callable) at the same size: the
 median wall time per frame reading the mask files, and with masks=VosSource propagating them on the device.  Weights are seeded (oracle.vos_oracle.random_state_dict, BN statistics calibrated on a frame); speed does not depend on them."""
 import argparse
@@ -86,6 +89,17 @@ def main():
         k = next(ks)
         v.next(frames[k], out=outs[k], stream=stream)
     per_frame = benchkit.window_ms(next_frame, n - a.warmup - 1, a.warmup, stream)
+    # the same window writing each frame's label map too, then bt_vos_labels alone on the last frame
+    lab = torch.empty((H, W), dtype=torch.uint8, device=dev)
+    v.begin(frames[0], torch.from_numpy(m0).to(dev), out=outs[0], stream=stream)
+    ks = iter(range(1, n))
+
+    def next_frame_and_labels():
+        k = next(ks)
+        v.next(frames[k], out=outs[k], stream=stream)
+        v.labels(lab, stream=stream)
+    per_frame_labels = benchkit.window_ms(next_frame_and_labels, n - a.warmup - 1, a.warmup, stream)
+    labels_ms = float(np.median(benchkit.calls_ms(lambda: v.labels(lab, stream=stream), 50, 5, stream)))
     Hd, Wd = -(-H // 8), -(-W // 8)
     HW = Hd * Wd
     bb = backbone_macs(H, W)
@@ -120,7 +134,7 @@ def main():
     ref_masks = [torch.where(up > 0, 255, 0).to(torch.uint8) for up in ups]
     disagree = float(np.mean([(r != o).float().mean().item() for r, o in zip(ref_masks, outs[1:])]))
     res = dict(gpu=name, power_limit=benchkit.card(), H=H, W=W, frames=a.frames, params=P,
-               stage_ms_median=med, per_frame_ms=per_frame,
+               stage_ms_median=med, per_frame_ms=per_frame, per_frame_with_labels_ms=per_frame_labels, labels_ms_median=labels_ms,
                backbone_gmac=bb / 1e9, propagation_gmac=prop / 1e9,
                backbone_tflops_3xtf32_counted_once=2 * bb / med["backbone"] / 1e9,
                propagation_tflops_counted_once=2 * prop / med["propagation"] / 1e9,
